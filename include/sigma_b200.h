@@ -248,6 +248,13 @@ int sigma_split_tf32_fwd(const float *x, float *hi, float *lo, int64_t n, void *
 int sigma_conv3x3_tf32(const float *x, const float *w9, const float *w9_lo, const float *bias, int act, float *y, int batch, int H, int W,
                        int Cin, int Cout, void *stream);
 
+/* Launch plan of the two calls above, host only (no CUDA call, works without a GPU): what sigma_linear_tf32{,x3} (conv_B = 0; M rows,
+ * N outputs, K inputs) or sigma_conv3x3_tf32 (conv_B > 0: input (conv_B, conv_H, conv_W, K), N = Cout; M unused) would launch under
+ * the current environment.  out6_host = {tile width, ring stages, persistent grid, output tiles, dynamic shared memory bytes, CTAs
+ * per SM}.  The environment variable SIGMA_GEMM_BN=<w> forces the tile width of both calls (a multiple of 32 in [32, 256], read
+ * per call; any other value makes the calls and this query return SIGMA_EINVAL).  For tests and tuning.                      */
+int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, int64_t *out6_host);
+
 /* ------------------------------------------------------------------------------------------
  * SURVEY.md §8(f) rank 2, first piece: the evaluator's per-batch metric on the device (eval.py:22-29,
  * utils/metric.py:8-15).  pred = argmax over classes of logits (batch, classes, H, W) — the index numpy.argmax

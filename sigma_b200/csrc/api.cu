@@ -267,6 +267,7 @@ int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw
 size_t ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N);
 int ss2d_pick_segments_hook(long long ctas, int nw, int ntiles, int N);
 int gemm_pick_bn_hook(int N, long long m_tiles);
+int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out);
 size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
 int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                   const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
@@ -416,6 +417,16 @@ int sigma_ss2d_scan_fwd_split(int kind, const float *xc, const float *xdbl, cons
 // test hooks (host logic only, no CUDA call): the launch heuristics, so that CPU tests can hold them to the recorded sweeps
 int sigma_test_pick_segments(long long ctas, int warps_per_cta, int ntiles, int N) { return ss2d_pick_segments_hook(ctas, warps_per_cta, ntiles, N); }
 int sigma_test_pick_bn(int N, long long m_tiles) { return gemm_pick_bn_hook(N, m_tiles); }
+// the launch plan of sigma_linear_tf32{,x3} (conv_B = 0) or of sigma_conv3x3_tf32 (conv_B > 0: input (conv_B, conv_H, conv_W, K),
+// N output channels), SIGMA_GEMM_BN included: out6_host = {tile width, ring stages, grid, tiles, shared-memory bytes, CTAs per SM}
+int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, int64_t *out6_host) {
+  SIGMA_CHECK_ARG(out6_host && N > 0 && K > 0 && (conv_B > 0 ? conv_H > 0 && conv_W > 0 : M > 0), "sigma_test_gemm_plan: bad arguments");
+  long long out[6];
+  const int rc = gemm_plan_hook(M, N, K, x3, conv_B, conv_H, conv_W, out);
+  if (rc) return rc;
+  for (int i = 0; i < 6; ++i) out6_host[i] = out[i];
+  return SIGMA_OK;
+}
 
 // training forward: the forward plus what the fused backward needs (delta' slabs, block-start states)
 size_t sigma_ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N) {

@@ -477,16 +477,70 @@ static int x3_keep_hi() {
   return v;
 }
 
-// Ring depth, shared memory and persistent grid for one call, then the launch of the instance for p.BN.
-template <bool X3, bool CONV>
-static int launch_gemm(GemmParams &p, long long total, cudaStream_t stream) {
-  const int a_bytes = GM_BM * GM_BK * 4, b_bytes = p.BN * GM_BK * 4;
-  const int stage_bytes = (a_bytes + ((b_bytes + 1023) & ~1023)) * (X3 ? 2 : 1);
+// The launch plan of one call: tile width, ring depth, shared memory and persistent grid.  gemm_tf32_launch,
+// conv3x3_tf32_launch and the sigma_test_gemm_plan hook all take it from plan_gemm, so a test that asserts a property of
+// the plan (e.g. "every CTA walks >= 3 tiles") asserts it of the launch.
+struct GemmPlan {
+  int BN, stages, ctas_per_sm;
+  unsigned grid;        // persistent CTAs
+  long long tiles;      // 128 x BN output tiles
+  size_t smem;          // dynamic shared memory per CTA
+};
+
+// SIGMA_GEMM_BN=<w> forces the tile width (a multiple of 32 in [32, 256]; anything else is an error, not clamped), read per
+// call so that a test can run one shape at every width.  Returns 0 when unset, the width, or SIGMA_EINVAL.
+static int forced_bn() {
+  const char *e = getenv("SIGMA_GEMM_BN");
+  if (e == nullptr || e[0] == '\0') return 0;
+  char *end = nullptr;
+  const long v = strtol(e, &end, 10);
+  if (*end != '\0' || v < 32 || v > 256 || v % 32 != 0) {
+    set_error("SIGMA_GEMM_BN=\"%s\": the GEMM tile width must be a multiple of 32 in [32, 256]", e);
+    return SIGMA_EINVAL;
+  }
+  return (int)v;
+}
+
+// conv_B > 0: the implicit-GEMM 3x3 convolution of a (conv_B, conv_H, conv_W, K) input with N output channels (M unused)
+static int plan_gemm(long long M, int N, int K, bool x3, int conv_B, int conv_H, int conv_W, GemmPlan *pl) {
+  (void)K;   // the K loop does not enter the plan
+  const bool conv = conv_B > 0;
+  const long long m_tiles = conv ? (long long)conv_B * ((conv_W + CV_TW - 1) / CV_TW) * ((conv_H + CV_TH - 1) / CV_TH)
+                                 : (M + GM_BM - 1) / GM_BM;
+  int bn = conv ? pick_bn(N) : pick_bn(N, m_tiles);
+  if (!conv) {
+    if (const char *e = getenv("SIGMA_GEMM_BN_RULE")) { if (e[0] == 'o') bn = pick_bn(N); }   // "old": ignore the row-tile count
+  }
+  const int fbn = forced_bn();
+  if (fbn < 0) return fbn;
+  if (fbn > 0) bn = fbn;
+  pl->BN = bn;
+  pl->tiles = m_tiles * ((N + bn - 1) / bn);
+  const int a_bytes = GM_BM * GM_BK * 4, b_bytes = bn * GM_BK * 4;
+  const int stage_bytes = (a_bytes + ((b_bytes + 1023) & ~1023)) * (x3 ? 2 : 1);
   // up to 227 KB per block; tiles of <= 128 columns keep the ring small enough for two CTAs per SM (their register budget)
-  const int regs_ctas = p.BN <= 128 ? 2 : 1;
+  const int regs_ctas = bn <= 128 ? 2 : 1;
   const int budget = (regs_ctas == 2 ? 112 * 1024 : 226 * 1024) - 1024;
-  p.stages = std::max(2, std::min(8, budget / stage_bytes));
-  const size_t smem = (size_t)p.stages * stage_bytes + 1024 /*barriers*/;
+  pl->stages = std::max(2, std::min(8, budget / stage_bytes));
+  pl->smem = (size_t)pl->stages * stage_bytes + 1024 /*barriers*/;
+  pl->ctas_per_sm = std::max(1, std::min(regs_ctas, (int)((228 * 1024) / (pl->smem + 1024))));
+  pl->grid = (unsigned)std::min<long long>(pl->tiles, (long long)kNumSMs * pl->ctas_per_sm);
+  return SIGMA_OK;
+}
+
+// api.cu test hook: out = {BN, stages, grid, tiles, smem bytes, CTAs per SM}
+int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out) {
+  GemmPlan pl;
+  const int rc = plan_gemm(M, N, K, x3 != 0, conv_B, conv_H, conv_W, &pl);
+  if (rc) return rc;
+  out[0] = pl.BN; out[1] = pl.stages; out[2] = pl.grid; out[3] = pl.tiles; out[4] = (long long)pl.smem; out[5] = pl.ctas_per_sm;
+  return SIGMA_OK;
+}
+
+// The launch of the instance for pl.BN.
+template <bool X3, bool CONV>
+static int launch_gemm(GemmParams &p, const GemmPlan &pl, cudaStream_t stream) {
+  p.stages = pl.stages;
   const void *kern = nullptr;
   switch (p.BN) {
 #define SIGMA_GEMM_BN(bn) case bn: kern = (const void *)gemm_tf32_kernel<bn, X3, CONV>; break;
@@ -495,11 +549,9 @@ static int launch_gemm(GemmParams &p, long long total, cudaStream_t stream) {
 #undef SIGMA_GEMM_BN
     default: set_error("gemm: unsupported tile width %d", p.BN); return SIGMA_EINVAL;
   }
-  SIGMA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int ctas_per_sm = std::max(1, std::min(regs_ctas, (int)((228 * 1024) / (smem + 1024))));
-  const unsigned grid = (unsigned)std::min<long long>(total, (long long)kNumSMs * ctas_per_sm);   // persistent CTAs
+  SIGMA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
   void *args[] = {&p};
-  SIGMA_CHECK_CUDA(cudaLaunchKernel(kern, dim3(grid), dim3(GM_THREADS), args, smem, stream));
+  SIGMA_CHECK_CUDA(cudaLaunchKernel(kern, dim3(pl.grid), dim3(GM_THREADS), args, pl.smem, stream));
   count_launch();
   return SIGMA_OK;
 }
@@ -509,19 +561,19 @@ int gemm_tf32_launch(const float *A, long long lda, const float *W, const float 
                      long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream) {
   if (M == 0) return SIGMA_OK;
   const bool x3 = W_lo != nullptr;
+  GemmPlan pl;
+  int rc;
+  if ((rc = plan_gemm(M, N, K, x3, 0, 0, 0, &pl))) return rc;
   GemmParams p;
   memset(&p, 0, sizeof(p));
   p.x3_keep_hi = x3_keep_hi();
   p.bias = bias; p.residual = residual; p.rscale = rscale; p.C = C; p.ldr = ldr; p.ldc = ldc;
   p.M = (int)M; p.N = N; p.K = K;
-  p.BN = pick_bn(N, (M + GM_BM - 1) / GM_BM);
-  if (const char *e = getenv("SIGMA_GEMM_BN_RULE")) { if (e[0] == 'o') p.BN = pick_bn(N); }   // "old": ignore the row-tile count
-  int rc;
+  p.BN = pl.BN;
   if ((rc = make_tmap_2d_sw128(&p.m_a, A, M, K, lda, GM_BM))) return rc;
   if ((rc = make_tmap_2d_sw128(&p.m_w, W, N, K, K, p.BN))) return rc;
   if (x3 && (rc = make_tmap_2d_sw128(&p.m_wlo, W_lo, N, K, K, p.BN))) return rc;
-  const long long total = (long long)((N + p.BN - 1) / p.BN) * ((M + GM_BM - 1) / GM_BM);
-  return x3 ? launch_gemm<true, false>(p, total, stream) : launch_gemm<false, false>(p, total, stream);
+  return x3 ? launch_gemm<true, false>(p, pl, stream) : launch_gemm<false, false>(p, pl, stream);
 }
 
 int make_tmap_generic(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,
@@ -533,6 +585,9 @@ int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, con
                         int Cin, int Cout, cudaStream_t stream) {
   if (B == 0) return SIGMA_OK;
   const bool x3 = W9_lo != nullptr;
+  GemmPlan pl;
+  int rc;
+  if ((rc = plan_gemm(0, Cout, Cin, x3, B, H, W, &pl))) return rc;
   GemmParams p;
   memset(&p, 0, sizeof(p));
   p.x3_keep_hi = x3_keep_hi();
@@ -543,8 +598,7 @@ int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, con
   p.tiles_hw = p.tiles_w * ((H + CV_TH - 1) / CV_TH);
   p.M = B * p.tiles_hw;
   p.kbc = (Cin + GM_BK - 1) / GM_BK;
-  p.BN = pick_bn(Cout);
-  int rc;
+  p.BN = pl.BN;
   {
     uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
     uint64_t str[3] = {(uint64_t)Cin * 4, (uint64_t)W * Cin * 4, (uint64_t)H * W * Cin * 4};
@@ -554,8 +608,7 @@ int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, con
   }
   if ((rc = make_tmap_2d_sw128(&p.m_w, W9, 9LL * Cout, Cin, Cin, p.BN))) return rc;
   if (x3 && (rc = make_tmap_2d_sw128(&p.m_wlo, W9_lo, 9LL * Cout, Cin, Cin, p.BN))) return rc;
-  const long long total = (long long)((Cout + p.BN - 1) / p.BN) * p.M;
-  return x3 ? launch_gemm<true, true>(p, total, stream) : launch_gemm<false, true>(p, total, stream);
+  return x3 ? launch_gemm<true, true>(p, pl, stream) : launch_gemm<false, true>(p, pl, stream);
 }
 
 }  // namespace sigma

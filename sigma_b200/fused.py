@@ -74,7 +74,11 @@ def _split_weight(w):
 def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="dense"):
     """Dense projection out = x·W^T (+bias) (+residual·rscale) through the hand-written wgmma GEMM (csrc/gemm_tf32.cu: TMA-fed,
     register accumulators, fused epilogue), in the precision `precision()` names.  x2d (M, K) with unit column stride, row stride
-    % 4 == 0; weight (N, K).  Shapes the kernel cannot take (K or N not a multiple of 4) go to torch.mm."""
+    % 4 == 0; weight (N, K).  Shapes the kernel cannot take (K or N not a multiple of 4) go to torch.mm.
+
+    Limitation: in tf32x3 mode the weight's hi / lo split is cached per weight and refreshed when `weight._version` changes
+    (optimizer steps, in-place ops under torch.no_grad(), load_state_dict).  A write through `weight.data` does not change
+    `_version`, so the next call still uses the split of the old values (conv3x3's re-ordered weight likewise)."""
     M, K = x2d.shape
     N = weight.shape[0]
     if out is None:

@@ -45,6 +45,17 @@ def record(name, **kv):
             f.write(json.dumps(dict(test=name, **kv)) + "\n")
 
 
+def gemm_plan(M, N, K, x3, conv=None):
+    """The launch plan sigma_linear_tf32{,x3} (conv=None) or sigma_conv3x3_tf32 (conv=(B, H, W): input (B, H, W, K), N output
+    channels) would use under the current environment (SIGMA_GEMM_BN included), from the library's own planner."""
+    import ctypes
+    from sigma_b200 import _lib
+    out = (ctypes.c_int64 * 6)()
+    B, H, W = conv if conv is not None else (0, 0, 0)
+    _lib.check(_lib.lib().sigma_test_gemm_plan(M, N, K, int(bool(x3)), B, H, W, out), "sigma_test_gemm_plan")
+    return dict(zip(("bn", "stages", "grid", "tiles", "smem", "ctas_per_sm"), (int(v) for v in out)))
+
+
 def sample_index(key, numel, k):
     """A fixed, seeded set of min(k, numel) flat indices for `key`: the positions at which a golden file stores a large output."""
     rng = np.random.default_rng(zlib.crc32(key.encode()))

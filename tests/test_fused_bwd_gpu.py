@@ -28,7 +28,7 @@ def _cmp(name, got, ref, bar=1e-3):
 
 
 @pytest.mark.parametrize("B,H,W,D,N,R", [(2, 6, 5, 64, 16, 2), (1, 30, 40, 128, 16, 8), (2, 9, 13, 64, 4, 4), (1, 17, 33, 192, 16, 6),
-                                         (1, 40, 21, 64, 4, 4)])
+                                         (1, 40, 21, 64, 4, 4), (1, 30, 40, 768, 16, 24)])   # last: Sigma stage 2 (CTAS = 4 budget)
 @pytest.mark.parametrize("split", [0, 1, 3])
 @pytest.mark.parametrize("save", [True, False])   # True: forward keeps delta' / block-start states (sigma_ss2d_scan_fwd_save + _bwd_saved)
 def test_fused_core_cross4_matches_composed(B, H, W, D, N, R, split, save, monkeypatch):

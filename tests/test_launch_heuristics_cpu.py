@@ -2,7 +2,9 @@
 * `ss2d_pick_segments` (L-segment count of the fused scan, a cost model of the busiest SM): replayed on every row of
   tests/golden/ss2d_split_sweep_h100.txt (scripts/bench_ss2d_splits.py on an H100 SXM at 400 W: 15 call shapes x {1,2,4,8}
   images x 10 forced counts) its choices must stay within 6 % of the per-row optimum in total and well ahead of the old rule.
-* `pick_bn` (GEMM tile width): the widest divisor in the throughput regime, narrower tiles when few row tiles exist."""
+* `pick_bn` (GEMM tile width): the widest divisor in the throughput regime, narrower tiles when few row tiles exist.
+* `plan_gemm` (the whole launch plan of the GEMM / implicit-GEMM conv, SIGMA_GEMM_BN included, through sigma_test_gemm_plan):
+  every plan is launchable — grid within the tile count, 2-8 ring stages, shared memory within the H100's limits."""
 import os
 import re
 
@@ -78,3 +80,71 @@ def test_gemm_tile_width_is_a_valid_tile(L, N, m_tiles):
         assert bn == wide                               # enough tiles for every persistent CTA: nothing to gain from narrow tiles
     if m_tiles <= 5 and N >= 768:
         assert bn <= 128                                # a handful of row tiles: spread the columns over more CTAs
+
+
+# ---- the launch plan of the wgmma GEMM / implicit-GEMM conv (sigma_test_gemm_plan = the planner the launches use) ----
+SMEM_PER_BLOCK = 227 * 1024      # H100: opt-in dynamic shared memory per block
+SMEM_PER_SM = 228 * 1024
+GEMM_SHAPES = [(1, 16, 32), (77, 160, 192), (1000, 384, 96), (4096, 320, 1536), (38417, 768, 384), (102401, 4, 36),
+               (355200, 768, 192), (355200, 176, 384), (700, 3072, 768), (38401, 260, 100)]
+CONV_SHAPES = [(6, 120, 160, 96, 32), (6, 120, 160, 32, 96), (20, 60, 80, 192, 64), (66, 30, 40, 384, 128), (20, 57, 75, 100, 36),
+               (1, 1, 5, 32, 32), (3, 9, 17, 128, 384)]
+
+
+def _check_plan(pl, x3):
+    assert pl["bn"] % 32 == 0 and 32 <= pl["bn"] <= 256
+    assert 1 <= pl["grid"] <= pl["tiles"]                                   # a persistent CTA never starts without a tile
+    assert 2 <= pl["stages"] <= 8
+    stage = (128 * 32 * 4 + -(-pl["bn"] * 32 * 4 // 1024) * 1024) * (2 if x3 else 1)
+    assert pl["smem"] == pl["stages"] * stage + 1024
+    assert pl["smem"] <= SMEM_PER_BLOCK
+    assert pl["ctas_per_sm"] * (pl["smem"] + 1024) <= SMEM_PER_SM          # the CTAs the grid counts on fit an SM together
+    assert pl["grid"] <= 132 * pl["ctas_per_sm"]
+
+
+@pytest.mark.parametrize("x3", [False, True])
+@pytest.mark.parametrize("M,N,K", GEMM_SHAPES)
+def test_gemm_plan_is_launchable(L, M, N, K, x3, monkeypatch):
+    from helpers import gemm_plan
+    monkeypatch.delenv("SIGMA_GEMM_BN", raising=False)
+    pl = gemm_plan(M, N, K, x3)
+    _check_plan(pl, x3)
+    mt = -(-M // 128)
+    assert pl["bn"] == L.sigma_test_pick_bn(N, mt)                        # the plan's width is the heuristic's
+    assert pl["tiles"] == mt * -(-N // pl["bn"])
+    for bn in range(32, 257, 32):
+        monkeypatch.setenv("SIGMA_GEMM_BN", str(bn))
+        pl = gemm_plan(M, N, K, x3)
+        assert pl["bn"] == bn and pl["tiles"] == mt * -(-N // bn)
+        _check_plan(pl, x3)
+
+
+@pytest.mark.parametrize("x3", [False, True])
+@pytest.mark.parametrize("B,H,W,Cin,Cout", CONV_SHAPES)
+def test_conv_plan_is_launchable(L, B, H, W, Cin, Cout, x3, monkeypatch):
+    from helpers import gemm_plan
+    monkeypatch.delenv("SIGMA_GEMM_BN", raising=False)
+    patches = B * -(-H // 8) * -(-W // 16)                                  # 8 x 16 pixel patches
+    for bn in [None] + list(range(32, 257, 32)):
+        if bn is not None:
+            monkeypatch.setenv("SIGMA_GEMM_BN", str(bn))
+        pl = gemm_plan(0, Cout, Cin, x3, conv=(B, H, W))
+        _check_plan(pl, x3)
+        assert pl["bn"] == (bn or L.sigma_test_pick_bn(Cout, 1 << 30))
+        assert pl["tiles"] == patches * -(-Cout // pl["bn"])
+
+
+@pytest.mark.parametrize("value", ["0", "16", "48", "257", "288", "-32", "64x", "wide"])
+def test_forced_tile_width_rejects_bad_values(L, value, monkeypatch):
+    """SIGMA_GEMM_BN takes a multiple of 32 in [32, 256]; anything else is an error with a message, never a silent clamp."""
+    import ctypes
+    from sigma_b200 import _lib
+    monkeypatch.setenv("SIGMA_GEMM_BN", value)
+    out = (ctypes.c_int64 * 6)()
+    for conv in [(0, 0, 0), (2, 30, 40)]:
+        rc = L.sigma_test_gemm_plan(1000, 768, 192, 1, *conv, out)
+        assert rc == -1                                                     # SIGMA_EINVAL
+        assert "SIGMA_GEMM_BN" in _lib.lib().sigma_last_error().decode()
+    monkeypatch.delenv("SIGMA_GEMM_BN")
+    assert L.sigma_test_gemm_plan(1000, 768, 192, 1, 0, 0, 0, out) == 0
+

@@ -65,6 +65,7 @@ CASES = [  # kind, B(images), H, W, D, N, R
     ("cross4", 1, 30, 40, 80, 16, 12), ("cross4", 1, 7, 9, 768, 4, 24), ("cross4", 1, 9, 13, 128, 8, 5),
     ("seq2", 2, 6, 5, 64, 4, 2), ("seq2", 1, 30, 41, 384, 4, 12), ("cross", 2, 6, 5, 64, 4, 2), ("cross", 1, 31, 40, 192, 4, 6),
     ("cross4", 1, 10, 12, 64, 16, 48), ("cross4", 1, 10, 12, 64, 4, 64),
+    ("cross4", 1, 30, 40, 768, 16, 24), ("cross4", 2, 30, 40, 768, 16, 24),     # Sigma stage 2: the CTAS = 4 register budget
 ]
 
 
@@ -96,6 +97,15 @@ def test_fused_scan_matches_oracle(kind, B, H, W, D, N, R, split):
         fused._FORCE_SPLIT = 0
     scale = float(np.abs(ref).max())
     assert_close(y, ref, 6e-4, 1e-3 * scale, f"{tag} split={split}")
+
+
+@pytest.mark.parametrize("kind,B,H,W,D,N,R", [c for c in CASES if c[5] == 16] + [
+    ("cross4", 1, 10, 12, 64, 16, 16), ("cross4", 1, 10, 12, 64, 16, 32), ("cross4", 1, 10, 12, 64, 16, 64)])
+def test_fused_scan_ctas4_budget_matches_oracle(kind, B, H, W, D, N, R, monkeypatch):
+    """The second register budget of the d_state-16 scan (`CTAS = 4` of ss2d_scan_kernel; ss2d_pick_ctas runs it only at
+    dt_rank 17..24), forced with SIGMA_SCAN_CTAS=4 at every padded dt_rank (4, 8, 12, 16, 24, 32, 48, 64)."""
+    monkeypatch.setenv("SIGMA_SCAN_CTAS", "4")
+    test_fused_scan_matches_oracle(kind, B, H, W, D, N, R, 0)
 
 
 @pytest.mark.parametrize("rows,C", [(7, 32), (100, 96), (33, 192), (5, 768), (9, 3072), (3, 4096)])
