@@ -125,6 +125,12 @@ int sigma_ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const floa
                         int batch, int H, int W, int D, int N, int R, int Cp,
                         void *workspace, size_t workspace_bytes, void *stream);
 
+/* bf16 inference mode: the same scan with xc and y in bf16 (x_dbl, the parameters, the state and the recurrence fp32; y rounded once
+ * on its store).  D % 8 == 0.  Not for training: there is no bf16 counterpart of sigma_ss2d_scan_fwd_save.                      */
+int sigma_ss2d_scan_fwd_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                             const float *Ds, void *y, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                             size_t workspace_bytes, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * f1. Backward of the fused scan (training): replaces the autograd of CrossScan (vmamba.py:80-98) + the dt_proj einsum (:199) +
  * SelectiveScan (selective_scan_bwd_kernel.cuh:68-274) + CrossMerge (:100-121) without materialising the (B,4,D,L) copies.
@@ -164,6 +170,8 @@ int sigma_ss2d_scan_bwd_saved(int kind, const float *xc, const float *xdbl, cons
 /* nn.LayerNorm over the last dim (vmamba.py:1693,724,2173; eps=1e-5): y = (x-mean)/sqrt(var+eps)·w+b */
 int sigma_layernorm_fwd(const float *x, const float *w, const float *b, float *y, int64_t rows,
                         int C, float eps, void *stream);
+/* bf16 inference mode: the same LayerNorm (fp32 statistics) with y stored as bf16 (8-byte aligned), to feed sigma_linear_bf16. */
+int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream);
 
 /* Backward of sigma_layernorm_fwd (training path; the reference's autograd of nn.LayerNorm): dx (rows, C); dw (C) = sum over rows
  * of dy·xhat, db (C) = sum over rows of dy — both zeroed inside, then accumulated.  mean / rstd are recomputed from x.
@@ -177,6 +185,9 @@ int sigma_layernorm_bwd(const float *x, const float *dy, const float *w, float *
  * (every Sigma width is).                                                                    */
 int sigma_patch_merge_norm_fwd(const float *x, const float *w, const float *b, float *y, int batch, int H, int W,
                                int C, float eps, void *stream);
+/* bf16 inference mode: the same gather + LayerNorm with y stored as bf16 (8-byte aligned).                                      */
+int sigma_patch_merge_norm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int batch, int H, int W, int C,
+                                    float eps, void *stream);
 
 /* PatchExpand back half (MambaDecoder.py:24-30): x is the expand Linear's output (batch,H,W,2,2,C) ("b h w (p1 p2 c)"),
  * y[b,2h+p1,2w+p2,:] = LayerNorm(x[b,h,w,p1,p2,:]); y (batch,2H,2W,C).  The pixel shuffle is the store address.   */
@@ -190,6 +201,10 @@ int sigma_pixel_shuffle_norm_fwd(const float *x, const float *w, const float *b,
 int sigma_dwconv3x3_silu_fwd(const float *x, int64_t x_row_stride, int64_t x_batch_stride,
                              const float *w, const float *bias, float *y, int64_t y_batch_stride,
                              int batch, int H, int W, int D, void *stream);
+/* bf16 inference mode: the same depthwise conv + SiLU with x and y bf16 (fp32 weights, bias and accumulation).  x 16-byte aligned,
+ * x strides multiples of 8 elements (TMA); y 8-byte aligned, y_batch_stride % 4 == 0.                                          */
+int sigma_dwconv3x3_silu_fwd_bf16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
+                                  void *y, int64_t y_batch_stride, int batch, int H, int W, int D, void *stream);
 
 /* CrossMerge sum + out_norm LayerNorm + gates (vmamba.py:217-224,1077; ConMB: 423-428,1280-1281):
  *   out[r,:] = (LN(Σ_k y[k][r,:])·gamma+beta) · (z ? SiLU(z[r,:]) : 1) · (gate ? gate[r / rows_per_batch, :] : 1)
@@ -200,6 +215,12 @@ int sigma_merge_norm_gate_fwd(const float *y, int K, int64_t k_stride, int64_t i
                               int64_t z_row_stride, const float *gate, float *out,
                               int64_t out_batch_stride, int64_t out_row_stride, int64_t rows,
                               int64_t rows_per_batch, int D, float eps, void *stream);
+/* bf16 inference mode: the same merge + LayerNorm + gates with y, z and out bf16 (8-byte aligned); gamma, beta, gate and the
+ * statistics fp32.  Strides count elements.                                                                                   */
+int sigma_merge_norm_gate_fwd_bf16(const void *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
+                                   const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *out,
+                                   int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
+                                   int D, float eps, void *stream);
 
 /* UpsampleExpand tail (MambaDecoder.py:47-49): y = LayerNorm(bilinear x2 (align_corners=False) of x); x (batch,H,W,C),
  * y (batch,2H,2W,C).  One pass: the upsampled tensor is never materialised un-normalised.
@@ -240,6 +261,12 @@ int sigma_linear_tf32x3(const float *A, int64_t lda, const float *W_hi, const fl
                         int64_t ldr, const float *rscale, float *C, int64_t ldc, int64_t M, int N, int K, void *stream);
 int sigma_split_tf32_fwd(const float *x, float *hi, float *lo, int64_t n, void *stream);
 
+/* bf16 inference mode: the same GEMM on bf16 operands (`wgmma ... k16.f32.bf16.bf16`, one MMA per 16-wide k-step, fp32 accumulate):
+ * A (M, K) bf16 rows lda elements apart, W (N, K) bf16 contiguous; C rows ldc elements apart, stored as fp32 (c_dtype = SIGMA_F32)
+ * or bf16 (SIGMA_BF16, rounded once); bias / residual / rscale fp32.  K, lda % 8 == 0; N, ldc, ldr % 4 == 0; 16-byte aligned.   */
+int sigma_linear_bf16(const void *A, int64_t lda, const void *W, const float *bias, const float *residual, int64_t ldr,
+                      const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream);
+
 /* Dense 3x3 convolution (pad 1, stride 1) of the ChannelAttentionBlock (vmamba.py:1749-1752), channels-last, as an implicit GEMM on
  * the same wgmma kernel: y (batch, H, W, Cout) = conv(x (batch, H, W, Cin), w9) + bias, act = 1 applies the exact (erf) GELU of
  * nn.GELU() in the epilogue.  w9 = the nn.Conv2d weight (Cout, Cin, 3, 3) re-ordered to (3·3, Cout, Cin); every tap's input patch
@@ -252,7 +279,8 @@ int sigma_conv3x3_tf32(const float *x, const float *w9, const float *w9_lo, cons
  * N outputs, K inputs) or sigma_conv3x3_tf32 (conv_B > 0: input (conv_B, conv_H, conv_W, K), N = Cout; M unused) would launch under
  * the current environment.  out6_host = {tile width, ring stages, persistent grid, output tiles, dynamic shared memory bytes, CTAs
  * per SM}.  The environment variable SIGMA_GEMM_BN=<w> forces the tile width of both calls (a multiple of 32 in [32, 256], read
- * per call; any other value makes the calls and this query return SIGMA_EINVAL).  For tests and tuning.                      */
+ * per call; any other value makes the calls and this query return SIGMA_EINVAL).  For tests and tuning.
+ * x3 selects the instance: 0 = tf32, 1 = tf32x3, 2 = sigma_linear_bf16 (conv_B must be 0); other values are SIGMA_EINVAL.      */
 int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, int64_t *out6_host);
 
 /* ------------------------------------------------------------------------------------------

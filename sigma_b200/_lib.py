@@ -61,6 +61,13 @@ SIGNATURES = {
     "sigma_linear_tf32x3": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p]),
     "sigma_conv3x3_tf32": (c_int, [c_void_p] * 4 + [c_int, c_void_p] + [c_int] * 5 + [c_void_p]),
     "sigma_split_tf32_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "sigma_linear_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int, c_int, c_void_p]),
+    "sigma_layernorm_fwd_bf16": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_float, c_void_p]),
+    "sigma_patch_merge_norm_fwd_bf16": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_float, c_void_p]),
+    "sigma_merge_norm_gate_fwd_bf16": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                               c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_float, c_void_p]),
+    "sigma_dwconv3x3_silu_fwd_bf16": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64] + [c_int] * 4 + [c_void_p]),
+    "sigma_ss2d_scan_fwd_bf16": (c_int, [c_int] + [c_void_p] * 7 + [c_int] * 7 + [c_void_p, c_size_t, c_void_p]),
 }
 
 _lib = None

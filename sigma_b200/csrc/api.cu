@@ -263,7 +263,7 @@ int dwconv3x3_silu_launch(const float *x, long long x_row_stride, long long x_ba
 size_t ss2d_scan_workspace_bytes(int kind, int batch, int D, int N);
 int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                   const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp, void *ws,
-                  size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave = nullptr, float *hsave = nullptr);
+                  size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave = nullptr, float *hsave = nullptr, int xc_bf16 = 0);
 size_t ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N);
 int ss2d_pick_segments_hook(long long ctas, int nw, int ntiles, int N);
 int gemm_pick_bn_hook(int N, long long m_tiles);
@@ -281,6 +281,10 @@ int scale_add_launch(const float *a, const float *sa, const float *b, const floa
 int gemm_tf32_launch(const float *A, long long lda, const float *W, const float *W_lo, const float *bias, const float *residual,
                      long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream);
 int split_tf32_launch(const float *x, float *hi, float *lo, long long n, cudaStream_t stream);
+int gemm_bf16_launch(const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
+                     const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N, int K, cudaStream_t stream);
+int dwconv3x3_silu_bf16_launch(const void *x, long long x_row_stride, long long x_batch_stride, const float *w, const float *bias,
+                               void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream);
 int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, const float *bias, int act, float *y, int B, int H, int W,
                         int Cin, int Cout, cudaStream_t stream);
 struct ImagePreParams {
@@ -297,6 +301,7 @@ int eval_resize_add_launch(const float *acc, int ncls, int AH, int AW, int m_top
 int eval_argmax_hist_launch(const double *score, const unsigned char *labels, unsigned char *pred, unsigned long long *hist,
                             unsigned long long *counts, int ncls, long long HW, cudaStream_t stream);
 static bool al16(const void *p) { return ((uintptr_t)p & 15) == 0; }
+static bool al8(const void *p) { return ((uintptr_t)p & 7) == 0; }
 }  // namespace sigma
 
 extern "C" {
@@ -308,6 +313,15 @@ int sigma_layernorm_fwd(const float *x, const float *w, const float *b, float *y
   SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd: C=%d must be a positive multiple of 4", C);
   SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al16(y), "sigma_layernorm_fwd: pointers must be 16-byte aligned");
   RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
+  return row_norm_launch(p, (cudaStream_t)stream);
+}
+
+int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
+  SIGMA_CHECK_ARG(x && w && b && y, "sigma_layernorm_fwd_bf16: null pointer");
+  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd_bf16: C=%d must be a positive multiple of 4", C);
+  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al8(y), "sigma_layernorm_fwd_bf16: x, w, b must be 16-byte and y 8-byte aligned");
+  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
+  p.io = 1;
   return row_norm_launch(p, (cudaStream_t)stream);
 }
 
@@ -327,6 +341,17 @@ int sigma_patch_merge_norm_fwd(const float *x, const float *w, const float *b, f
   const int64_t rows = (int64_t)batch * ((H + 1) / 2) * ((W + 1) / 2);
   RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, y, rows, rows, 0, 0, 4 * C, 4 * C, eps};
   p.mode = 1; p.gH = H; p.gW = W;
+  return row_norm_launch(p, (cudaStream_t)stream);
+}
+
+int sigma_patch_merge_norm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int batch, int H, int W, int C,
+                                    float eps, void *stream) {
+  SIGMA_CHECK_ARG(x && w && b && y, "sigma_patch_merge_norm_fwd_bf16: null pointer");
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "sigma_patch_merge_norm_fwd_bf16: bad sizes");
+  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al8(y), "sigma_patch_merge_norm_fwd_bf16: x, w, b must be 16-byte and y 8-byte aligned");
+  const int64_t rows = (int64_t)batch * ((H + 1) / 2) * ((W + 1) / 2);
+  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows, 0, 0, 4 * C, 4 * C, eps};
+  p.mode = 1; p.gH = H; p.gW = W; p.io = 1;
   return row_norm_launch(p, (cudaStream_t)stream);
 }
 
@@ -358,6 +383,23 @@ int sigma_merge_norm_gate_fwd(const float *y, int K, int64_t k_stride, int64_t i
   return row_norm_launch(p, (cudaStream_t)stream);
 }
 
+int sigma_merge_norm_gate_fwd_bf16(const void *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
+                                   const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *out,
+                                   int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
+                                   int D, float eps, void *stream) {
+  SIGMA_CHECK_ARG(y && gamma && beta && out, "sigma_merge_norm_gate_fwd_bf16: null pointer");
+  SIGMA_CHECK_ARG(K >= 1 && K <= 8 && D > 0 && D % 4 == 0 && rows >= 0 && rows_per_batch > 0,
+                  "sigma_merge_norm_gate_fwd_bf16: bad sizes K=%d D=%d rows=%lld rows_per_batch=%lld", K, D, (long long)rows,
+                  (long long)rows_per_batch);
+  SIGMA_CHECK_ARG(al8(y) && al16(gamma) && al16(beta) && al8(out) && al8(z) && al16(gate) && k_stride % 4 == 0 &&
+                      in_batch_stride % 4 == 0 && out_batch_stride % 4 == 0 && out_row_stride % 4 == 0 && z_row_stride % 4 == 0,
+                  "sigma_merge_norm_gate_fwd_bf16: y / z / out must be 8-byte and gamma / beta / gate 16-byte aligned, strides multiples of 4");
+  RowNormParams p{(const float *)y, k_stride, K, gamma, beta, (const float *)z, z_row_stride, gate, (float *)out, rows, rows_per_batch,
+                  in_batch_stride, out_batch_stride, out_row_stride, D, eps};
+  p.io = 2;
+  return row_norm_launch(p, (cudaStream_t)stream);
+}
+
 int sigma_dwconv3x3_silu_fwd(const float *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w,
                              const float *bias, float *y, int64_t y_batch_stride, int batch, int H, int W, int D,
                              void *stream) {
@@ -367,6 +409,15 @@ int sigma_dwconv3x3_silu_fwd(const float *x, int64_t x_row_stride, int64_t x_bat
                   "sigma_dwconv3x3_silu_fwd: pointers / strides must be 16-byte aligned");
   return dwconv3x3_silu_launch(x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D,
                                (cudaStream_t)stream);
+}
+
+int sigma_dwconv3x3_silu_fwd_bf16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
+                                  void *y, int64_t y_batch_stride, int batch, int H, int W, int D, void *stream) {
+  SIGMA_CHECK_ARG(x && w && y, "sigma_dwconv3x3_silu_fwd_bf16: null pointer");
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % 4 == 0, "sigma_dwconv3x3_silu_fwd_bf16: bad sizes");
+  SIGMA_CHECK_ARG(al16(x) && al8(y) && x_row_stride % 8 == 0 && x_batch_stride % 8 == 0 && y_batch_stride % 4 == 0,
+                  "sigma_dwconv3x3_silu_fwd_bf16: x must be 16-byte aligned with strides multiples of 8 elements (TMA), y 8-byte aligned");
+  return dwconv3x3_silu_bf16_launch(x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D, (cudaStream_t)stream);
 }
 
 int sigma_ss2d_padded_cp(int N, int R) {
@@ -402,6 +453,16 @@ int sigma_ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const floa
   if (rc) return rc;
   return ss2d_scan_fwd(kind, xc, xdbl, dtw, dtb, A, Ds, y, batch, H, W, D, N, R, Cp, workspace, workspace_bytes, 0,
                        (cudaStream_t)stream);
+}
+
+int sigma_ss2d_scan_fwd_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                             const float *Ds, void *y, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                             size_t workspace_bytes, void *stream) {
+  int rc = ss2d_check(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp);
+  if (rc) return rc;
+  SIGMA_CHECK_ARG(D % 8 == 0, "sigma_ss2d_scan_fwd_bf16: D=%d must be a multiple of 8 (16-byte TMA rows)", D);
+  return ss2d_scan_fwd(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp, workspace, workspace_bytes,
+                       0, (cudaStream_t)stream, nullptr, nullptr, 1);
 }
 
 // test hook: force the number of L-segments
@@ -596,6 +657,19 @@ int sigma_linear_tf32(const float *A, int64_t lda, const float *W, const float *
                   "sigma_linear_tf32: pointers must be 16-byte aligned");
   SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "sigma_linear_tf32: rscale without residual");
   return gemm_tf32_launch(A, lda, W, nullptr, bias, residual, ldr, rscale, C, ldc, M, N, K, (cudaStream_t)stream);
+}
+
+int sigma_linear_bf16(const void *A, int64_t lda, const void *W, const float *bias, const float *residual, int64_t ldr,
+                      const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream) {
+  SIGMA_CHECK_ARG(A && W && C, "sigma_linear_bf16: null pointer");
+  SIGMA_CHECK_ARG(c_dtype == SIGMA_F32 || c_dtype == SIGMA_BF16, "sigma_linear_bf16: c_dtype %d (SIGMA_F32 or SIGMA_BF16)", c_dtype);
+  SIGMA_CHECK_ARG(M >= 0 && M < (1LL << 31) && N > 0 && K > 0, "sigma_linear_bf16: bad sizes M=%lld N=%d K=%d", (long long)M, N, K);
+  SIGMA_CHECK_ARG(K % 8 == 0 && lda % 8 == 0 && N % 4 == 0 && ldc % 4 == 0 && (residual == nullptr || ldr % 4 == 0) && lda >= K && ldc >= N,
+                  "sigma_linear_bf16: K and lda must be multiples of 8 (16-byte bf16 TMA rows); N, ldc, ldr multiples of 4");
+  SIGMA_CHECK_ARG(al16(A) && al16(W) && al16(C) && al16(bias) && al16(residual) && al16(rscale),
+                  "sigma_linear_bf16: pointers must be 16-byte aligned");
+  SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "sigma_linear_bf16: rscale without residual");
+  return gemm_bf16_launch(A, lda, W, bias, residual, ldr, rscale, C, ldc, c_dtype == SIGMA_BF16, M, N, K, (cudaStream_t)stream);
 }
 
 int sigma_linear_tf32x3(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias, const float *residual,

@@ -1,5 +1,6 @@
 // Shared device helpers and host-side error plumbing for libsigma_b200 (sm_90a only).
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -58,7 +59,35 @@ struct RowNormParams {
   // 2 = PatchExpand pixel shuffle (MambaDecoder.py:24-28): input rows are (b, h, w, p1, p2) sub-rows of D channels,
   //     row lands at out (b, 2h+p1, 2w+p2)
   int mode = 0, gH = 0, gW = 0;
+  // element types (the bf16 inference mode): 0 = y, z, out fp32; 1 = y fp32, out bf16 (LayerNorm / patch-merge LN feeding a
+  // bf16 GEMM); 2 = y, z, out bf16 (merge + out_norm + gate of the bf16 scan output).  Pointers and strides count elements.
+  int io = 0;
 };
+
+// ---- 4-element fp32 / bf16 accesses (a float4 or 8 bytes of bf16); bf16 -> fp32 is exact, fp32 -> bf16 rounds to nearest even ----
+__device__ __forceinline__ float4 bf16x4_to_f4(uint2 u) {
+  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
+                     __uint_as_float(u.y & 0xFFFF0000u));
+}
+__device__ __forceinline__ uint32_t f2_to_bf16x2(float a, float b) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<const uint32_t *>(&h);
+}
+__device__ __forceinline__ float4 ld4(const float *p) { return *reinterpret_cast<const float4 *>(p); }
+__device__ __forceinline__ float4 ld4(const __nv_bfloat16 *p) { return bf16x4_to_f4(*reinterpret_cast<const uint2 *>(p)); }
+__device__ __forceinline__ float4 ld4g(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
+__device__ __forceinline__ float4 ld4g(const __nv_bfloat16 *p) { return bf16x4_to_f4(__ldg(reinterpret_cast<const uint2 *>(p))); }
+__device__ __forceinline__ float4 ld4cs(const float *p) { return __ldcs(reinterpret_cast<const float4 *>(p)); }
+__device__ __forceinline__ float4 ld4cs(const __nv_bfloat16 *p) { return bf16x4_to_f4(__ldcs(reinterpret_cast<const uint2 *>(p))); }
+__device__ __forceinline__ void st4(float *p, float4 v) { *reinterpret_cast<float4 *>(p) = v; }
+__device__ __forceinline__ void st4(__nv_bfloat16 *p, float4 v) {
+  *reinterpret_cast<uint2 *>(p) = make_uint2(f2_to_bf16x2(v.x, v.y), f2_to_bf16x2(v.z, v.w));
+}
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <typename T> __device__ __forceinline__ T from_f32(float v);
+template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
 // ---- device math ----
 __device__ __forceinline__ float ex2(float x) {

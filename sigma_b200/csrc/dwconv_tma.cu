@@ -19,20 +19,23 @@ namespace sigma {
 constexpr int DC_CB = 32, DC_TW = 16, DC_TH = 8, DC_NSLOT = 4;
 constexpr int DC_THREADS = 8 * (DC_TW / 4) * (DC_TH / 2);          // 8 channel quads x column groups x row pairs
 constexpr int DC_TILE_FL = DC_CB * (DC_TW + 2) * (DC_TH + 2);
-constexpr int DC_TILE_BYTES = DC_TILE_FL * 4;
 
 struct DwTmaParams {
   CUtensorMap map;
   const float *w, *bias;
-  float *y;
+  void *y;
   long long y_batch_stride;
   int batch, H, W, D, tiles_w, tiles_h;
   long long ntiles;
 };
 
+// T: element type of x and y (float, or __nv_bfloat16 in the bf16 inference mode: same tiles at half the bytes; weights, bias
+// and the accumulation stay fp32)
+template <typename T>
 __global__ void __launch_bounds__(DC_THREADS, 2) dwconv3x3_silu_tma_kernel(const __grid_constant__ DwTmaParams p) {
+  constexpr int DC_TILE_BYTES = DC_TILE_FL * (int)sizeof(T);
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  float *tiles = reinterpret_cast<float *>(smem_raw);
+  T *tiles = reinterpret_cast<T *>(smem_raw);
   uint64_t *full = reinterpret_cast<uint64_t *>(smem_raw + DC_NSLOT * DC_TILE_BYTES);
   __shared__ __align__(16) float sw[9][DC_CB];
   __shared__ __align__(16) float sb[DC_CB];
@@ -81,7 +84,7 @@ __global__ void __launch_bounds__(DC_THREADS, 2) dwconv3x3_silu_tma_kernel(const
     const int b = (int)(t / tiles_per_img);
     const int r = (int)(t - (long long)b * tiles_per_img);
     const int th = r / p.tiles_w, tw = r - th * p.tiles_w;
-    const float *base = tiles + st * DC_TILE_FL + ((2 * hp) * (DC_TW + 2) + 4 * wg) * DC_CB + 4 * cq;
+    const T *base = tiles + st * DC_TILE_FL + ((2 * hp) * (DC_TW + 2) + 4 * wg) * DC_CB + 4 * cq;
     float4 acc[2][4];
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr)
@@ -91,7 +94,7 @@ __global__ void __launch_bounds__(DC_THREADS, 2) dwconv3x3_silu_tma_kernel(const
     for (int wr = 0; wr < 4; ++wr) {       // window row wr feeds output row 0 with tap row wr and output row 1 with tap row wr-1
       float4 win[6];
 #pragma unroll
-      for (int j = 0; j < 6; ++j) win[j] = *reinterpret_cast<const float4 *>(base + (wr * (DC_TW + 2) + j) * DC_CB);
+      for (int j = 0; j < 6; ++j) win[j] = ld4(base + (wr * (DC_TW + 2) + j) * DC_CB);
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         const int tr = wr - rr;
@@ -116,13 +119,13 @@ __global__ void __launch_bounds__(DC_THREADS, 2) dwconv3x3_silu_tma_kernel(const
       for (int rr = 0; rr < 2; ++rr) {
         const int h = h0 + rr;
         if (h >= p.H) continue;
-        float *yb = p.y + (long long)b * p.y_batch_stride + ((long long)h * p.W + w0) * p.D + c;
+        T *yb = reinterpret_cast<T *>(p.y) + (long long)b * p.y_batch_stride + ((long long)h * p.W + w0) * p.D + c;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           if (w0 + j < p.W) {
             float4 o;
             o.x = silu(acc[rr][j].x); o.y = silu(acc[rr][j].y); o.z = silu(acc[rr][j].z); o.w = silu(acc[rr][j].w);
-            *reinterpret_cast<float4 *>(yb + (long long)j * p.D) = o;
+            st4(yb + (long long)j * p.D, o);
           }
         }
       }
@@ -132,16 +135,20 @@ __global__ void __launch_bounds__(DC_THREADS, 2) dwconv3x3_silu_tma_kernel(const
   }
 }
 
-// returns SIGMA_OK, an error, or 1 when the shape cannot use the TMA path (caller falls back to the direct kernel)
-int dwconv3x3_silu_tma_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
-                              const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
-                              cudaStream_t stream) {
-  if ((x_row_stride & 3) || (x_batch_stride & 3) || ((uintptr_t)x & 15) || (D & 3)) return 1;
+int make_tmap_generic(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,
+                      const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo);   // scan_op_tma.cu
+
+template <typename T>
+static int dwconv_tma_launch(const T *x, long long x_row_stride, long long x_batch_stride, const float *w, const float *bias, T *y,
+                             long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream) {
+  constexpr int es = (int)sizeof(T);
   DwTmaParams p;
   const uint64_t dims[4] = {(uint64_t)D, (uint64_t)W, (uint64_t)H, (uint64_t)batch};
-  const uint64_t str[3] = {(uint64_t)x_row_stride * 4, (uint64_t)W * x_row_stride * 4, (uint64_t)x_batch_stride * 4};
+  const uint64_t str[3] = {(uint64_t)x_row_stride * es, (uint64_t)W * x_row_stride * es, (uint64_t)x_batch_stride * es};
   const uint32_t box[4] = {DC_CB, DC_TW + 2, DC_TH + 2, 1};
-  int rc = make_tmap_f32_4d(&p.map, x, dims, str, box);
+  int rc = es == 4 ? make_tmap_f32_4d(&p.map, x, dims, str, box)
+                   : make_tmap_generic(&p.map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                       CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
   if (rc) return rc;
   p.w = w; p.bias = bias; p.y = y; p.y_batch_stride = y_batch_stride;
   p.batch = batch; p.H = H; p.W = W; p.D = D;
@@ -150,17 +157,32 @@ int dwconv3x3_silu_tma_launch(const float *x, long long x_row_stride, long long 
   p.ntiles = (long long)batch * p.tiles_w * p.tiles_h;
   if (p.ntiles == 0) return SIGMA_OK;
   const int cblocks = (D + DC_CB - 1) / DC_CB;
-  const size_t smem = DC_NSLOT * DC_TILE_BYTES + 64;
-  SIGMA_CHECK_CUDA(cudaFuncSetAttribute(dwconv3x3_silu_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const size_t smem = (size_t)DC_NSLOT * DC_TILE_FL * es + 64;
+  SIGMA_CHECK_CUDA(cudaFuncSetAttribute(dwconv3x3_silu_tma_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // persistent over spatial tiles: 2 CTAs per SM in total, channel block fastest so that the CTAs working on one
   // spatial tile (adjacent 128-byte pieces of the same pixel rows) run at the same time
   const long long slots = kNumSMs * 2;
   // (never more CTAs than resident slots: a partial second wave of persistent CTAs would double the kernel time)
   const unsigned ny = (unsigned)std::max<long long>(1, std::min<long long>(p.ntiles, slots / cblocks));
   dim3 grid(cblocks, ny);
-  dwconv3x3_silu_tma_kernel<<<grid, DC_THREADS, smem, stream>>>(p);
+  dwconv3x3_silu_tma_kernel<T><<<grid, DC_THREADS, smem, stream>>>(p);
   SIGMA_CHECK_LAUNCH();
   return SIGMA_OK;
+}
+
+// returns SIGMA_OK, an error, or 1 when the shape cannot use the TMA path (caller falls back to the direct kernel)
+int dwconv3x3_silu_tma_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
+                              const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
+                              cudaStream_t stream) {
+  if ((x_row_stride & 3) || (x_batch_stride & 3) || ((uintptr_t)x & 15) || (D & 3)) return 1;
+  return dwconv_tma_launch<float>(x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D, stream);
+}
+
+// bf16 x and y (the caller checks the 16-byte stride / alignment TMA needs: there is no direct bf16 kernel to fall back to)
+int dwconv3x3_silu_bf16_launch(const void *x, long long x_row_stride, long long x_batch_stride, const float *w, const float *bias,
+                               void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream) {
+  return dwconv_tma_launch<__nv_bfloat16>((const __nv_bfloat16 *)x, x_row_stride, x_batch_stride, w, bias, (__nv_bfloat16 *)y,
+                                          y_batch_stride, batch, H, W, D, stream);
 }
 
 }  // namespace sigma

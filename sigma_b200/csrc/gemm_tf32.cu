@@ -43,6 +43,7 @@ struct alignas(64) GemmParams {
   float *C;
   long long ldr, ldc;
   int M, N, K, BN, stages;   // BN: host-side choice of the template instance
+  int c_bf16;       // BF16: 1 = C is stored as bf16 (bias / residual / rscale stay fp32)
   int x3_keep_hi;   // X3: 1 = the splitter also rewrites the activations' hi part in place (needed unless the tensor core truncates)
   int cH, cW, tiles_w, tiles_hw, kbc, act;   // CONV: image size, 8x16 patches per row / per image, Cin blocks per tap, activation
 };
@@ -247,8 +248,179 @@ template <> __device__ __forceinline__ void wgmma_tf32<256>(float (&d)[128], uin
 }
 
 
-template <int BN, bool X3, bool CONV>
+// D[64 x N] (+)= A[64 x 16] · B[N x 16]^T in bf16 (BF16 instance): a k16 bf16 step is 32 bytes, like a k8 tf32 step, so the
+// swizzled stage layout and the +32 B descriptor advance are shared; both operands K-major (transpose flags 0)
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_bf16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<96>(float (&d)[48], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+      "%48, %49, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<160>(float (&d)[80], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %82, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n160k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
+      "%80, %81, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<192>(float (&d)[96], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %98, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
+      "%96, %97, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<224>(float (&d)[112], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %114, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n224k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111}, "
+      "%112, %113, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<256>(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+
+template <int BN, bool X3, bool CONV, bool BF16 = false>
 __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_tf32_kernel(const __grid_constant__ GemmParams p) {
+  static_assert(!BF16 || (!X3 && !CONV), "the bf16 instance is a plain GEMM");
+  constexpr int KB = BF16 ? 2 * GM_BK : GM_BK;   // elements per k-block: one 128-byte swizzle row either way
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const int S = p.stages;
   constexpr int a_bytes = GM_BM * GM_BK * 4, b_bytes = BN * GM_BK * 4;
@@ -259,7 +431,7 @@ __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_tf32_kerne
   uint64_t *empty = full + S;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nkb = CONV ? 9 * p.kbc : (p.K + GM_BK - 1) / GM_BK;
+  const int nkb = CONV ? 9 * p.kbc : (p.K + KB - 1) / KB;
   const int num_n = (p.N + BN - 1) / BN;
   const int num_m = CONV ? p.M : (p.M + GM_BM - 1) / GM_BM;      // CONV: p.M counts pixel patches
   const long long total = (long long)num_m * num_n;
@@ -293,8 +465,8 @@ __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_tf32_kerne
             tma_load_2d(sa + a_bytes, &p.m_w, &full[st], kc * GM_BK, tap * p.N + n0);
             if (X3) tma_load_2d(sa + half_bytes + a_bytes, &p.m_wlo, &full[st], kc * GM_BK, tap * p.N + n0);
           } else {
-            tma_load_2d(sa, &p.m_a, &full[st], kb * GM_BK, m0);
-            tma_load_2d(sa + a_bytes, &p.m_w, &full[st], kb * GM_BK, n0);
+            tma_load_2d(sa, &p.m_a, &full[st], kb * KB, m0);
+            tma_load_2d(sa + a_bytes, &p.m_w, &full[st], kb * KB, n0);
             if (X3) tma_load_2d(sa + half_bytes + a_bytes, &p.m_wlo, &full[st], kb * GM_BK, n0);
           }
         }
@@ -345,8 +517,10 @@ __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_tf32_kerne
         }
       } else {
 #pragma unroll
-        for (int k = 0; k < GM_BK / GM_UK; ++k)   // +32 B along K inside the swizzle row = +2 in 16-byte units
-          wgmma_tf32<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
+        for (int k = 0; k < GM_BK / GM_UK; ++k) {   // +32 B along K inside the swizzle row = +2 in 16-byte units
+          if (BF16) wgmma_bf16<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
+          else wgmma_tf32<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
+        }
       }
       wgmma_commit();
       acc_fence(acc);
@@ -370,16 +544,16 @@ __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_tf32_kerne
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;   // row inside the 128-row tile
-      float *crow;
+      long long coff;   // element offset of the row in C (fp32 or, BF16 && p.c_bf16, bf16)
       const float *rrow = nullptr;
       if (CONV) {   // row r = pixel (r / 16, r % 16) of the 8 x 16 patch
         const int y = cy0 + r / CV_TW, x = cx0 + (r % CV_TW);
         if (y >= p.cH || x >= p.cW) continue;
-        crow = p.C + (((long long)cb * p.cH + y) * p.cW + x) * p.N;
+        coff = (((long long)cb * p.cH + y) * p.cW + x) * p.N;
       } else {
         const int row = mt * GM_BM + r;
         if (row >= p.M) continue;
-        crow = p.C + (long long)row * p.ldc;
+        coff = (long long)row * p.ldc;
         if (p.residual) rrow = p.residual + (long long)row * p.ldr;
       }
 #pragma unroll
@@ -404,7 +578,10 @@ __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_tf32_kerne
           o.x = 0.5f * o.x * (1.f + erff(o.x * 0.70710678118654752f));
           o.y = 0.5f * o.y * (1.f + erff(o.y * 0.70710678118654752f));
         }
-        *reinterpret_cast<float2 *>(crow + n) = o;
+        if (BF16 && p.c_bf16)
+          *reinterpret_cast<__nv_bfloat162 *>(reinterpret_cast<__nv_bfloat16 *>(p.C) + coff + n) = __floats2bfloat162_rn(o.x, o.y);
+        else
+          *reinterpret_cast<float2 *>(p.C + coff + n) = o;
       }
     }
   }
@@ -416,19 +593,22 @@ typedef CUresult (*EncodeTiledFn2)(CUtensorMap *, CUtensorMapDataType, cuuint32_
                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 void *get_tensor_map_encoder();  // ss2d_scan_host.cu
 
-static int make_tmap_2d_sw128(CUtensorMap *map, const float *base, long long rows, long long cols, long long ld, int box_rows) {
+// bf16 = true: 2-byte elements, a box row of 2·GM_BK elements (still 128 bytes)
+static int make_tmap_2d_sw128(CUtensorMap *map, const void *base, long long rows, long long cols, long long ld, int box_rows,
+                              bool bf16 = false) {
   EncodeTiledFn2 fn = (EncodeTiledFn2)get_tensor_map_encoder();
   if (!fn) return SIGMA_ECUDA;
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstr[1] = {(cuuint64_t)ld * 4};
-  cuuint32_t bdim[2] = {(cuuint32_t)GM_BK, (cuuint32_t)box_rows};
+  cuuint64_t gstr[1] = {(cuuint64_t)ld * (bf16 ? 2 : 4)};
+  cuuint32_t bdim[2] = {(cuuint32_t)(bf16 ? 2 * GM_BK : GM_BK), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(base), gdim, gstr, bdim, estr,
+  CUresult r = fn(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(base), gdim,
+                  gstr, bdim, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled (gemm operand) failed (CUresult %d): rows=%lld cols=%lld ld=%lld box_rows=%d base=%p",
-              (int)r, rows, cols, ld, box_rows, (const void *)base);
+              (int)r, rows, cols, ld, box_rows, base);
     return SIGMA_ECUDA;
   }
   return SIGMA_OK;
@@ -528,22 +708,24 @@ static int plan_gemm(long long M, int N, int K, bool x3, int conv_B, int conv_H,
   return SIGMA_OK;
 }
 
-// api.cu test hook: out = {BN, stages, grid, tiles, smem bytes, CTAs per SM}
+// api.cu test hook: out = {BN, stages, grid, tiles, smem bytes, CTAs per SM}.  x3: 0 = tf32, 1 = tf32x3, 2 = bf16 (the bf16
+// instance stages the same bytes per k-block as tf32 — 128-byte rows — so its plan is the tf32 plan)
 int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out) {
   GemmPlan pl;
-  const int rc = plan_gemm(M, N, K, x3 != 0, conv_B, conv_H, conv_W, &pl);
+  if (x3 < 0 || x3 > 2 || (x3 == 2 && conv_B > 0)) { set_error("gemm plan: mode %d (0 tf32, 1 tf32x3, 2 bf16; bf16 has no conv)", x3); return SIGMA_EINVAL; }
+  const int rc = plan_gemm(M, N, K, x3 == 1, conv_B, conv_H, conv_W, &pl);
   if (rc) return rc;
   out[0] = pl.BN; out[1] = pl.stages; out[2] = pl.grid; out[3] = pl.tiles; out[4] = (long long)pl.smem; out[5] = pl.ctas_per_sm;
   return SIGMA_OK;
 }
 
 // The launch of the instance for pl.BN.
-template <bool X3, bool CONV>
+template <bool X3, bool CONV, bool BF16 = false>
 static int launch_gemm(GemmParams &p, const GemmPlan &pl, cudaStream_t stream) {
   p.stages = pl.stages;
   const void *kern = nullptr;
   switch (p.BN) {
-#define SIGMA_GEMM_BN(bn) case bn: kern = (const void *)gemm_tf32_kernel<bn, X3, CONV>; break;
+#define SIGMA_GEMM_BN(bn) case bn: kern = (const void *)gemm_tf32_kernel<bn, X3, CONV, BF16>; break;
     SIGMA_GEMM_BN(32) SIGMA_GEMM_BN(64) SIGMA_GEMM_BN(96) SIGMA_GEMM_BN(128)
     SIGMA_GEMM_BN(160) SIGMA_GEMM_BN(192) SIGMA_GEMM_BN(224) SIGMA_GEMM_BN(256)
 #undef SIGMA_GEMM_BN
@@ -574,6 +756,23 @@ int gemm_tf32_launch(const float *A, long long lda, const float *W, const float 
   if ((rc = make_tmap_2d_sw128(&p.m_w, W, N, K, K, p.BN))) return rc;
   if (x3 && (rc = make_tmap_2d_sw128(&p.m_wlo, W_lo, N, K, K, p.BN))) return rc;
   return x3 ? launch_gemm<true, false>(p, pl, stream) : launch_gemm<false, false>(p, pl, stream);
+}
+
+// bf16 operands (A (M, K) row stride lda, W (N, K)), fp32 accumulation, C fp32 or (c_bf16) bf16; bias / residual / rscale fp32
+int gemm_bf16_launch(const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
+                     const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N, int K, cudaStream_t stream) {
+  if (M == 0) return SIGMA_OK;
+  GemmPlan pl;
+  int rc;
+  if ((rc = plan_gemm(M, N, K, false, 0, 0, 0, &pl))) return rc;
+  GemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.bias = bias; p.residual = residual; p.rscale = rscale; p.C = (float *)C; p.ldr = ldr; p.ldc = ldc; p.c_bf16 = c_bf16;
+  p.M = (int)M; p.N = N; p.K = K;
+  p.BN = pl.BN;
+  if ((rc = make_tmap_2d_sw128(&p.m_a, A, M, K, lda, GM_BM, true))) return rc;
+  if ((rc = make_tmap_2d_sw128(&p.m_w, W, N, K, K, p.BN, true))) return rc;
+  return launch_gemm<false, false, true>(p, pl, stream);
 }
 
 int make_tmap_generic(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,

@@ -18,13 +18,14 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
-template <int MAXV>
+// TI: element type of y and z, TO: of out (RowNormParams::io); gamma, beta, gate and all arithmetic are fp32
+template <int MAXV, typename TI, typename TO>
 __global__ void __launch_bounds__(256) row_norm_kernel(const RowNormParams p) {
   const int lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= p.rows) return;
   const long long bi = row / p.rows_per_batch, ri = row - bi * p.rows_per_batch;
-  const float *in = p.y + bi * p.in_batch_stride + ri * p.D;
+  const TI *in = reinterpret_cast<const TI *>(p.y) + bi * p.in_batch_stride + ri * p.D;
   const int nvec = p.D >> 2;
   float4 x[MAXV];
   float s = 0.f;
@@ -33,9 +34,9 @@ __global__ void __launch_bounds__(256) row_norm_kernel(const RowNormParams p) {
     const int idx = lane + 32 * v;
     x[v] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (idx < nvec) {
-      float4 a = __ldg(reinterpret_cast<const float4 *>(in) + idx);
+      float4 a = ld4g(in + 4 * idx);
       for (int k = 1; k < p.K; ++k) {
-        const float4 b = __ldg(reinterpret_cast<const float4 *>(in + k * p.k_stride) + idx);
+        const float4 b = ld4g(in + k * p.k_stride + 4 * idx);
         a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
       }
       x[v] = a;
@@ -52,8 +53,8 @@ __global__ void __launch_bounds__(256) row_norm_kernel(const RowNormParams p) {
     }
   }
   const float rstd = rsqrtf(warp_sum(q) / (float)p.D + p.eps);
-  float *out = p.out + bi * p.out_batch_stride + ri * p.out_row_stride;
-  const float *zr = p.z ? p.z + row * p.z_row_stride : nullptr;
+  TO *out = reinterpret_cast<TO *>(p.out) + bi * p.out_batch_stride + ri * p.out_row_stride;
+  const TI *zr = p.z ? reinterpret_cast<const TI *>(p.z) + row * p.z_row_stride : nullptr;
   const float *gr = p.gate ? p.gate + bi * p.D : nullptr;
 #pragma unroll
   for (int v = 0; v < MAXV; ++v) {
@@ -67,14 +68,14 @@ __global__ void __launch_bounds__(256) row_norm_kernel(const RowNormParams p) {
       o.z = fmaf((x[v].z - mean) * rstd, g.z, b.z);
       o.w = fmaf((x[v].w - mean) * rstd, g.w, b.w);
       if (zr) {
-        const float4 zz = __ldg(reinterpret_cast<const float4 *>(zr) + idx);
+        const float4 zz = ld4g(zr + 4 * idx);
         o.x *= silu(zz.x); o.y *= silu(zz.y); o.z *= silu(zz.z); o.w *= silu(zz.w);
       }
       if (gr) {
         const float4 gg = __ldg(reinterpret_cast<const float4 *>(gr) + idx);
         o.x *= gg.x; o.y *= gg.y; o.z *= gg.z; o.w *= gg.w;
       }
-      reinterpret_cast<float4 *>(out)[idx] = o;
+      st4(out + 4 * idx, o);
     }
   }
 }
@@ -83,7 +84,7 @@ __global__ void __launch_bounds__(256) row_norm_kernel(const RowNormParams p) {
 // a warp works on 32/LPR rows at once, every lane issues all its K·V (+V for z) 16-byte loads before the first use
 // (the generic kernel above has one load in flight per lane inside a runtime-K loop: ~45 % of HBM peak under ncu),
 // reductions are LPR-wide shuffles.  y and z are dead after this kernel: streaming loads (evict-first).
-template <int LPR, int V, int K, int MODE>
+template <int LPR, int V, int K, int MODE, typename TI, typename TO>
 __global__ void __launch_bounds__(256) row_norm_fast_kernel(const RowNormParams p) {
   constexpr int RPW = 32 / LPR;
   const int lane = threadIdx.x & 31, sub = lane / LPR, l = lane % LPR;
@@ -92,34 +93,33 @@ __global__ void __launch_bounds__(256) row_norm_fast_kernel(const RowNormParams 
   const long long row = valid ? row_raw : p.rows - 1;     // keep the warp convergent for the shuffles
   long long bi = 0, ri = row;
   if (p.rows_per_batch < p.rows) { bi = row / p.rows_per_batch; ri = row - bi * p.rows_per_batch; }   // 64-bit division only when batched
-  const float4 *in = reinterpret_cast<const float4 *>(p.y + bi * p.in_batch_stride + ri * p.D);
-  const long long ks4 = p.k_stride >> 2;
+  const TI *in = reinterpret_cast<const TI *>(p.y) + bi * p.in_batch_stride + ri * p.D;
   float4 x[V], kk[K > 1 ? (K - 1) * V : 1], zz[V];
   if (MODE == 1) {
     // gather the 2x2 pixel block of output row (b, i, j); quadrant q of the row = pixel (2i + (q&1), 2j + (q>>1))
     const int H2 = (p.gH + 1) >> 1, W2 = (p.gW + 1) >> 1, cq = (p.D >> 2) >> 2;   // float4 per source pixel
     const long long b = row / ((long long)H2 * W2);
     const int rem = (int)(row - b * H2 * W2), i = rem / W2, j = rem - i * W2;
-    const float4 *src = reinterpret_cast<const float4 *>(p.y) + b * p.gH * p.gW * cq;
+    const TI *src = reinterpret_cast<const TI *>(p.y) + b * p.gH * p.gW * 4 * cq;
 #pragma unroll
     for (int v = 0; v < V; ++v) {
       const int idx = l + LPR * v, q = idx / cq, c4 = idx - q * cq;
       const int hh = 2 * i + (q & 1), ww = 2 * j + (q >> 1);
-      x[v] = (hh < p.gH && ww < p.gW) ? __ldg(src + ((long long)hh * p.gW + ww) * cq + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+      x[v] = (hh < p.gH && ww < p.gW) ? ld4g(src + 4 * (((long long)hh * p.gW + ww) * cq + c4)) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   } else {
 #pragma unroll
-    for (int v = 0; v < V; ++v) x[v] = __ldcs(in + l + LPR * v);
+    for (int v = 0; v < V; ++v) x[v] = ld4cs(in + 4 * (l + LPR * v));
   }
 #pragma unroll
   for (int k = 1; k < K; ++k)
 #pragma unroll
-    for (int v = 0; v < V; ++v) kk[(k - 1) * V + v] = __ldcs(in + k * ks4 + l + LPR * v);
+    for (int v = 0; v < V; ++v) kk[(k - 1) * V + v] = ld4cs(in + k * p.k_stride + 4 * (l + LPR * v));
   const bool has_z = p.z != nullptr;
   if (has_z) {
-    const float4 *zr = reinterpret_cast<const float4 *>(p.z + row * p.z_row_stride);
+    const TI *zr = reinterpret_cast<const TI *>(p.z) + row * p.z_row_stride;
 #pragma unroll
-    for (int v = 0; v < V; ++v) zz[v] = __ldcs(zr + l + LPR * v);
+    for (int v = 0; v < V; ++v) zz[v] = ld4cs(zr + 4 * (l + LPR * v));
   }
   float s = 0.f;
 #pragma unroll
@@ -143,12 +143,12 @@ __global__ void __launch_bounds__(256) row_norm_fast_kernel(const RowNormParams 
 #pragma unroll
   for (int o = LPR / 2; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
   const float rstd = rsqrtf(q / (float)p.D + p.eps);
-  float4 *out = reinterpret_cast<float4 *>(p.out + bi * p.out_batch_stride + ri * p.out_row_stride);
+  TO *out = reinterpret_cast<TO *>(p.out) + bi * p.out_batch_stride + ri * p.out_row_stride;
   if (MODE == 2) {
     const int p2 = (int)(row & 1), p1 = (int)((row >> 1) & 1);
     const long long pix = row >> 2, b = pix / ((long long)p.gH * p.gW);
     const int rem = (int)(pix - b * p.gH * p.gW), h = rem / p.gW, w = rem - h * p.gW;
-    out = reinterpret_cast<float4 *>(p.out + (((b * 2 * p.gH + 2 * h + p1) * 2 * p.gW) + 2 * w + p2) * p.D);
+    out = reinterpret_cast<TO *>(p.out) + (((b * 2 * p.gH + 2 * h + p1) * 2 * p.gW) + 2 * w + p2) * p.D;
   }
   const float4 *gr = p.gate ? reinterpret_cast<const float4 *>(p.gate + bi * p.D) : nullptr;
 #pragma unroll
@@ -166,21 +166,37 @@ __global__ void __launch_bounds__(256) row_norm_fast_kernel(const RowNormParams 
       const float4 gg = __ldg(gr + idx);
       o.x *= gg.x; o.y *= gg.y; o.z *= gg.z; o.w *= gg.w;
     }
-    if (valid) out[idx] = o;
+    if (valid) st4(out + 4 * idx, o);
   }
 }
 
 template <int LPR, int V>
 static bool row_norm_fast_k(const RowNormParams &p, cudaStream_t stream) {
+  using bf16 = __nv_bfloat16;
   const int warps = 8, rows_per_cta = warps * (32 / LPR);
   const unsigned grid = (unsigned)((p.rows + rows_per_cta - 1) / rows_per_cta);
-  if (p.mode == 1 && p.K == 1) { row_norm_fast_kernel<LPR, V, 1, 1><<<grid, warps * 32, 0, stream>>>(p); return true; }
-  if (p.mode == 2 && p.K == 1) { row_norm_fast_kernel<LPR, V, 1, 2><<<grid, warps * 32, 0, stream>>>(p); return true; }
+  if (p.io == 1) {   // LayerNorm / patch-merge LayerNorm with bf16 output
+    if (p.K != 1) return false;
+    if (p.mode == 0) { row_norm_fast_kernel<LPR, V, 1, 0, float, bf16><<<grid, warps * 32, 0, stream>>>(p); return true; }
+    if (p.mode == 1) { row_norm_fast_kernel<LPR, V, 1, 1, float, bf16><<<grid, warps * 32, 0, stream>>>(p); return true; }
+    return false;
+  }
+  if (p.io == 2) {   // merge + norm + gate, bf16 in and out
+    if (p.mode != 0) return false;
+    switch (p.K) {
+      case 1: row_norm_fast_kernel<LPR, V, 1, 0, bf16, bf16><<<grid, warps * 32, 0, stream>>>(p); return true;
+      case 2: row_norm_fast_kernel<LPR, V, 2, 0, bf16, bf16><<<grid, warps * 32, 0, stream>>>(p); return true;
+      case 4: row_norm_fast_kernel<LPR, V, 4, 0, bf16, bf16><<<grid, warps * 32, 0, stream>>>(p); return true;
+    }
+    return false;
+  }
+  if (p.mode == 1 && p.K == 1) { row_norm_fast_kernel<LPR, V, 1, 1, float, float><<<grid, warps * 32, 0, stream>>>(p); return true; }
+  if (p.mode == 2 && p.K == 1) { row_norm_fast_kernel<LPR, V, 1, 2, float, float><<<grid, warps * 32, 0, stream>>>(p); return true; }
   if (p.mode != 0) return false;
   switch (p.K) {
-    case 1: row_norm_fast_kernel<LPR, V, 1, 0><<<grid, warps * 32, 0, stream>>>(p); return true;
-    case 2: row_norm_fast_kernel<LPR, V, 2, 0><<<grid, warps * 32, 0, stream>>>(p); return true;
-    case 4: row_norm_fast_kernel<LPR, V, 4, 0><<<grid, warps * 32, 0, stream>>>(p); return true;
+    case 1: row_norm_fast_kernel<LPR, V, 1, 0, float, float><<<grid, warps * 32, 0, stream>>>(p); return true;
+    case 2: row_norm_fast_kernel<LPR, V, 2, 0, float, float><<<grid, warps * 32, 0, stream>>>(p); return true;
+    case 4: row_norm_fast_kernel<LPR, V, 4, 0, float, float><<<grid, warps * 32, 0, stream>>>(p); return true;
   }
   return false;
 }
@@ -209,7 +225,12 @@ int row_norm_launch(const RowNormParams &p, cudaStream_t stream) {
   const int nvec = p.D >> 2;
   const int warps = 8;
   const unsigned grid = (unsigned)((p.rows + warps - 1) / warps);
-#define LAUNCH(MV) row_norm_kernel<MV><<<grid, warps * 32, 0, stream>>>(p)
+#define LAUNCH(MV)                                                                                                     \
+  do {                                                                                                                 \
+    if (p.io == 1) row_norm_kernel<MV, float, __nv_bfloat16><<<grid, warps * 32, 0, stream>>>(p);                      \
+    else if (p.io == 2) row_norm_kernel<MV, __nv_bfloat16, __nv_bfloat16><<<grid, warps * 32, 0, stream>>>(p);         \
+    else row_norm_kernel<MV, float, float><<<grid, warps * 32, 0, stream>>>(p);                                        \
+  } while (0)
   if (nvec <= 32) LAUNCH(1);
   else if (nvec <= 64) LAUNCH(2);
   else if (nvec <= 128) LAUNCH(4);

@@ -59,6 +59,7 @@ struct alignas(64) Ss2dParams {
   int nst;     // TMA ring depth: as many LT-position stages as fit next to CTAS-1 other CTAs in shared memory
   int ablate;  // timing experiments, only in builds with -DSIGMA_SCAN_ABLATION (SIGMA_SCAN_ABLATE env):
                // 1 = no y store, 2 = no per-group prologue, 4 = no TMA reload
+  int xc_bf16; // 1: xc and y are bf16 (the bf16 inference mode, non-SAVE kernels only); x_dbl, the state and the recurrence stay fp32
 };
 
 #ifdef SIGMA_SCAN_ABLATION
@@ -67,9 +68,10 @@ struct alignas(64) Ss2dParams {
 #define SIGMA_ABL(flags, m) false
 #endif
 
-__host__ __device__ inline size_t ss2d_smem_bytes(int LT, int DT, int NST, int Cp, bool cross) {
-  const size_t stage = (size_t)LT * DT + (size_t)LT * Cp * (cross ? 2 : 1);
-  return NST * stage * sizeof(float) + 128 /*barriers + counters*/;
+// xc_bytes: element size of the staged xc tile (4, or 2 for bf16)
+__host__ __device__ inline size_t ss2d_smem_bytes(int LT, int DT, int NST, int Cp, bool cross, int xc_bytes = 4) {
+  const size_t stage = (size_t)LT * DT * xc_bytes + (size_t)LT * Cp * (cross ? 2 : 1) * sizeof(float);
+  return NST * stage + 128 /*barriers + counters*/;
 }
 
 static __device__ float g_ss2d_sink[32];   // y of threads whose channel is >= D goes here (never read)
@@ -98,8 +100,8 @@ __device__ __forceinline__ unsigned long long mul2_raw(unsigned long long a, uns
 // dt_r part of the first row) and whose xc values start at `xrow` (this thread's first channel).  dt_r is read
 // once per position (broadcast LDS.128) and used for all CPT channels; the dot product runs on fma2 pairs
 // (one accumulator chain up to RP = 12, two beyond), softplus is branch-free (common.cuh).
-template <int N, int CPT, int RP, int G>
-__device__ __forceinline__ void group_prologue(const Ss2dThread<N, CPT, RP> &t, const float *xrow, const float *drow, int DT,
+template <int N, int CPT, int RP, int G, typename XT>
+__device__ __forceinline__ void group_prologue(const Ss2dThread<N, CPT, RP> &t, const XT *xrow, const float *drow, int DT,
                                                float (&dl)[CPT][G], float (&u)[CPT][G]) {
   constexpr int Cp = 2 * N + RP;  // x_dbl row length: [B | C | dt_r padded to RP] (sigma_ss2d_padded_cp)
   constexpr bool TWO = RP >= 16;
@@ -130,7 +132,7 @@ __device__ __forceinline__ void group_prologue(const Ss2dThread<N, CPT, RP> &t, 
       float x = s0.x + s0.y;
       if (TWO) { const f2 s1 = unpack2(acc1[c]); x += s1.x + s1.y; }
       dl[c][e] = x;                                   // pre-activation; softplus below, two positions per softplus20x2
-      u[c][e] = xrow[e * DT + c * cstride];
+      u[c][e] = to_f32(xrow[e * DT + c * cstride]);
     }
   }
 #pragma unroll
@@ -150,8 +152,8 @@ __device__ __forceinline__ void group_prologue(const Ss2dThread<N, CPT, RP> &t, 
 // channel lies beyond D walks a one-element sink instead (kernel prologue), so there is no branch around the store.
 // Per position B and C are read ONCE (2·N/4 broadcast LDS.128) and reused by the CPT channels of the thread;
 // per channel and state pair: mul2 (exp arguments), 2 x MUFU.EX2, mul2 (delta·u·B), fma2 (h), fma2 (C·h).
-template <int N, int CPT, int RP, int G, bool WITH_Y, bool REV, bool FULL, bool SAVE = false>
-__device__ __forceinline__ void group_body(Ss2dThread<N, CPT, RP> &t, const float *rb, const float *rc, float *yq,
+template <int N, int CPT, int RP, int G, bool WITH_Y, bool REV, bool FULL, bool SAVE = false, typename XT = float>
+__device__ __forceinline__ void group_body(Ss2dThread<N, CPT, RP> &t, const float *rb, const float *rc, XT *yq,
                                            int ystep, int ycstride, const float (&dl)[CPT][G],
                                            const float (&u)[CPT][G], int cnt, float *dq = nullptr) {
   constexpr int Cp = 2 * N + RP;
@@ -194,7 +196,7 @@ __device__ __forceinline__ void group_body(Ss2dThread<N, CPT, RP> &t, const floa
           float y = yacc[c][0].x + yacc[c][0].y;
           if (NCH == 2) y += yacc[c][1].x + yacc[c][1].y;
           if (SIGMA_ABL(t.ablate, 1)) t.sumdl[c] += y;
-          else yq[c * ycstride] = fmaf(t.Dv[c], u[c][i], y);
+          else yq[c * ycstride] = from_f32<XT>(fmaf(t.Dv[c], u[c][i], y));
           if (SAVE) dq[c * ycstride] = dl[c][i];
         } else {
           t.sumdl[c] += dl[c][i];
@@ -207,19 +209,19 @@ __device__ __forceinline__ void group_body(Ss2dThread<N, CPT, RP> &t, const floa
 }
 
 // Everything a warp needs to walk its CTA's tiles; filled once in the kernel.
-template <int N, int CPT, int RP>
+template <int N, int CPT, int RP, typename XT = float>
 struct Ss2dWalk {
   float *stages;
   uint64_t *full;
   uint32_t *done;
-  float *ybase;
+  XT *ybase;
   long long istride, ostride;
   int ystep;   // y elements from one walked position to the next (sign follows the walk direction; 0 on the sink)
   float *dbase;        // SAVE: this thread's channel in the delta' slab of (k, b) (same addressing as ybase)
   float *hs_base;      // SAVE: hsave + (((k·batch + b)·save_tiles)·D + d)·N; tile tau16 adds tau16·D·N
   long long hs_stride; // D·N (0 on the sink)
   int TPO16, ntiles16; // 16-position blocks per inner walk line / in the whole walk (the backward's tile geometry)
-  int stage_fl, xc_fl, dbl_fl, DT, nwarps, lane, ch;
+  int stage_fl, xc_fl, dbl_fl, DT, nwarps, lane, ch;   // in floats (xc_fl: the xc tile's bytes / 4)
   int t0, t1, TPO, ntiles, I, nst;
   bool cross, rev;
 };
@@ -227,23 +229,23 @@ struct Ss2dWalk {
 // The tile loop of one warp.  The software pipeline over groups of G positions runs ACROSS tiles: while the
 // recurrence of group g runs, delta'/u of group g+1 are computed — from the next tile's ring slot when g is the
 // last group of its tile — so no prologue is exposed at a tile boundary and none is computed twice.
-template <int N, int CPT, int RP, bool WITH_Y, bool REV, bool SAVE, typename Request>
-__device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2dWalk<N, CPT, RP> &w, Request &&request_tile) {
+template <int N, int CPT, int RP, bool WITH_Y, bool REV, bool SAVE, typename XT, typename Request>
+__device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2dWalk<N, CPT, RP, XT> &w, Request &&request_tile) {
   constexpr int G = Ss2dCfg<N>::G, LT = Ss2dCfg<N>::LT;
   constexpr int Cp = 2 * N + RP;
   const int ycs = w.DT / CPT;
 
   // ring slot / phase and (outer index, inner tile) of the tile being opened advance incrementally: no division
   // or modulo per tile.  Tiles are walked in ascending tau; reversed directions map tau -> ntiles-1-tau.
-  struct Tile { const float *sXC, *sDB, *sDC; float *ystart, *dstart; int npos, ng, tm16; };   // ystart: y of the tile's first WALKED group start
+  struct Tile { const XT *sXC; const float *sDB, *sDC; XT *ystart; float *dstart; int npos, ng, tm16; };   // ystart: y of the tile's first WALKED group start
   int ost = 0, oph = 0;                                  // slot and phase parity of the next tile to open
   int tm0 = w.rev ? w.ntiles - 1 - w.t0 : w.t0;          // memory-order tile index of tile t0
   int oo = tm0 / w.TPO, oti = tm0 - oo * w.TPO;          // its (outer index, inner tile)
   auto open_tile = [&]() {   // waits for the next tile's TMA bytes; returns its pointers and advances the cursor
     if (!(SIGMA_ABL(t.ablate, 4) && oph)) mbar_spin(&w.full[ost], (uint32_t)oph);
     Tile T;
-    T.sXC = w.stages + ost * w.stage_fl;
-    T.sDB = T.sXC + w.xc_fl;
+    T.sXC = reinterpret_cast<const XT *>(w.stages + ost * w.stage_fl);
+    T.sDB = w.stages + ost * w.stage_fl + w.xc_fl;
     T.sDC = w.cross ? T.sDB + w.dbl_fl : T.sDB;
     const int i0 = oti * LT;
     T.npos = min(LT, w.I - i0);
@@ -266,7 +268,7 @@ __device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2d
 
   int rst = 0;                    // ring slot of the tile being processed
   const int gstep = G * w.ystep;  // y elements from one group's first walked position to the next group's
-  float *yp = cur.ystart;         // running y pointer: first walked position of the current group
+  XT *yp = cur.ystart;            // running y pointer: first walked position of the current group
   float *dp = cur.dstart;
   for (int tau = w.t0; tau < w.t1; ++tau) {
     Tile nxt = cur;
@@ -274,7 +276,8 @@ __device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2d
 #pragma unroll 1
     for (int g = 0; g < cur.ng; ++g) {
       // next group's delta'/u first, so its loads / dot products / softplus overlap this group's exponentials
-      const float *px, *pd;
+      const XT *px;
+      const float *pd;
       if (g + 1 < cur.ng) {
         jn = REV ? j - 1 : j + 1;
         px = cur.sXC + jn * G * w.DT + w.ch;
@@ -338,9 +341,11 @@ __device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2d
   }
 }
 
-template <int N, int CPT, int RP, int MODE, int CTAS, bool SAVE = false>
+// XT: element type of xc and y (float; __nv_bfloat16 in the bf16 inference mode, not with SAVE)
+template <int N, int CPT, int RP, int MODE, int CTAS, bool SAVE = false, typename XT = float>
 __global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(const __grid_constant__ Ss2dParams p) {
   static_assert(!SAVE || MODE != MODE_SUMMARY, "the summary pass has no final states to save");
+  static_assert(!SAVE || sizeof(XT) == 4, "the training forward stores fp32");
   constexpr int LT = Ss2dCfg<N>::LT;
   constexpr bool WITH_Y = MODE != MODE_SUMMARY;
   const int NST = p.nst;
@@ -353,7 +358,7 @@ __global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(
   const int tid = threadIdx.x;
   const int NTC = blockDim.x;                // every warp computes; there is no producer warp
   const int DT = NTC * CPT;                  // channels per CTA: thread t owns channels t and t + NTC (CPT = 2)
-  const int xc_fl = LT * DT, dbl_fl = LT * Cp;
+  const int xc_fl = LT * DT * (int)sizeof(XT) / 4, dbl_fl = LT * Cp;
   const int stage_fl = xc_fl + dbl_fl * (cross ? 2 : 1);
   uint64_t *full = reinterpret_cast<uint64_t *>(stages + NST * stage_fl);
   uint32_t *done = reinterpret_cast<uint32_t *>(full + NST);   // per-slot count of warps done with the slot
@@ -430,20 +435,20 @@ __global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(
     }
   }
 
-  Ss2dWalk<N, CPT, RP> w;
+  Ss2dWalk<N, CPT, RP, XT> w;
   w.stages = stages; w.full = full; w.done = done;
   static_assert(CPT == 1, "the sink redirection below assumes one channel per thread");
   if (t.ok[0]) {
-    w.ybase = p.y + (((long long)k * p.batch + b) * p.Lseq) * p.D + d0 + tid;
+    w.ybase = reinterpret_cast<XT *>(p.y) + (((long long)k * p.batch + b) * p.Lseq) * p.D + d0 + tid;
     w.istride = p.istride[k]; w.ostride = p.ostride[k];
   } else {                       // channel beyond D (ragged last channel tile): every y address collapses onto the sink
-    w.ybase = &g_ss2d_sink[tid & 31];
+    w.ybase = reinterpret_cast<XT *>(&g_ss2d_sink[tid & 31]);
     w.istride = 0; w.ostride = 0;
   }
   w.ystep = (int)(rev ? -w.istride : w.istride);
   w.dbase = nullptr; w.hs_base = nullptr; w.hs_stride = 0; w.TPO16 = 0; w.ntiles16 = 0;
   if (SAVE) {
-    w.dbase = t.ok[0] ? p.dsave + (w.ybase - p.y) : w.ybase;          // same (K, batch, Lseq, D) addressing as y; sink otherwise
+    w.dbase = t.ok[0] ? p.dsave + (w.ybase - reinterpret_cast<XT *>(p.y)) : reinterpret_cast<float *>(w.ybase);          // same (K, batch, Lseq, D) addressing as y; sink otherwise
     w.TPO16 = (I + 15) >> 4;
     w.ntiles16 = O * w.TPO16;
     w.hs_stride = (long long)p.D * N;

@@ -132,11 +132,17 @@ size_t ss2d_scan_workspace_bytes(int kind, int batch, int D, int N) {
   return (size_t)batch * kind_dirs(kind) * D * kMaxSplit * 2 * N * sizeof(float);
 }
 
+int make_tmap_generic(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,
+                      const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo);   // scan_op_tma.cu
+
+// xc_bf16 = 1: xc and y are bf16 (passed through the float pointers); x_dbl, the parameters and the recurrence stay fp32
 int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                   const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp, void *ws,
-                  size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave, float *hsave) {
+                  size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave, float *hsave, int xc_bf16) {
   Ss2dParams p;
   memset(&p, 0, sizeof(p));
+  p.xc_bf16 = xc_bf16;
+  const int xes = xc_bf16 ? 2 : 4;   // bytes per xc / y element
   p.dtw = dtw; p.dtb = dtb; p.A = A; p.Ds = Ds; p.y = y; p.carry = (float *)ws;
   p.D = D; p.N = N; p.R = R; p.Cp = Cp; p.kind = kind; p.batch = batch;
   p.dsave = dsave; p.hsave = hsave; p.save_tiles = hsave ? ss2d_save_tiles(kind, H, W) : 0;
@@ -163,14 +169,16 @@ int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw
       p.I[k] = (int)Lseq; p.O[k] = 1;
       p.istride[k] = D; p.ostride[k] = 0;
       dims[0] = D; dims[1] = Lseq; dims[2] = 1; dims[3] = batch;
-      str[0] = (uint64_t)D * 4; str[1] = (uint64_t)Lseq * D * 4; str[2] = (uint64_t)Lseq * D * 4;
+      str[0] = (uint64_t)D * xes; str[1] = (uint64_t)Lseq * D * xes; str[2] = (uint64_t)Lseq * D * xes;
     } else {  // walk h (inner) at fixed w (outer): l1 = w·H + h  <->  position h·W + w   (vmamba.py:87)
       p.I[k] = H; p.O[k] = W;
       p.istride[k] = (long long)W * D; p.ostride[k] = D;
       dims[0] = D; dims[1] = H; dims[2] = W; dims[3] = batch;
-      str[0] = (uint64_t)W * D * 4; str[1] = (uint64_t)D * 4; str[2] = (uint64_t)Lseq * D * 4;
+      str[0] = (uint64_t)W * D * xes; str[1] = (uint64_t)D * xes; str[2] = (uint64_t)Lseq * D * xes;
     }
-    if ((rc = make_tmap_f32_4d(&p.m_xc[k], xc, dims, str, box))) return rc;
+    if ((rc = xc_bf16 ? make_tmap_generic(&p.m_xc[k], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, xc, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B)
+                      : make_tmap_f32_4d(&p.m_xc[k], xc, dims, str, box))) return rc;
     // x_dbl (batch, Lseq, K, Cp): direction k's row starts at column k·Cp
     uint32_t boxd[4] = {(uint32_t)Cp, (uint32_t)LT, 1, 1};
     dims[0] = Cp;
@@ -211,14 +219,14 @@ int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw
   // register budget (ss2d_scan.cuh): which `__launch_bounds__(128, CTAS)` build runs.  SIGMA_SCAN_CTAS overrides.
   int rbud = ss2d_pick_ctas(N, pad_rp(R));
   if (const char *e = getenv("SIGMA_SCAN_CTAS")) rbud = std::max(3, std::min(5, atoi(e)));
-  if (N != 16) rbud = 3;
+  if (N != 16 || xc_bf16) rbud = 3;   // bf16: only the 3-CTA budget is built (ss2d_scan_inst.inc)
   rbud = std::min(rbud, 4);
   {
     // TMA ring depth: as many stages as fit without lowering the register-limited occupancy (227 KB per SM, 1 KB
     // reserved per CTA).
     // Deep rings matter: a tile is requested when the LAST warp releases its slot and needed by the FIRST warp
     // nst-1 tiles later; with 3-4 stages the warps spun on the full barrier ~80 times per tile (ncu, round 1).
-    const size_t stage = ((size_t)LT * DT + (size_t)LT * Cp * (kind == SIGMA_DIRS_CROSS ? 2 : 1)) * sizeof(float);
+    const size_t stage = (size_t)LT * DT * xes + (size_t)LT * Cp * (kind == SIGMA_DIRS_CROSS ? 2 : 1) * sizeof(float);
     // resident CTAs per SM by registers (e.g. 168 per thread under __launch_bounds__(128, 3): 3 / 4 / 6 / 12 for 4 / 3 / 2 / 1 warps)
     const int ctas_sm = std::max(rbud, std::min(16, 65536 / (32 * NW * ss2d_reg_cap(rbud))));
     const size_t budget = (227 * 1024) / ctas_sm - 1024 - 128;

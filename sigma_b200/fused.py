@@ -6,6 +6,15 @@ Per SS2D block (vmamba.py:1067-1089 + cross_selective_scan :165-226) the kernels
     merge(4) + out_norm + ·SiLU(z) -> out_proj GEMM (+ residual)
 so neither CrossScan's (B,4,D,L) copy, nor delta (B,4D,L), nor CrossMerge's transposes ever exist.
 Dense projections go through `linear()` (see there).  Everything here assumes no autograd.
+
+Storage in the bf16 mode (`precision() == "bf16"`, selected by torch.autocast("cuda", dtype=torch.bfloat16) with autograd off):
+the residual stream between blocks stays fp32, as do the LayerNorm statistics, the scan state and every accumulator.  Inside
+SS2D, ConMB_SS2D, CrossMambaFusion_SS2D_SSM and PatchMerging2D, the LayerNorm output that feeds a GEMM, xz / tr / te,
+xc / seq, the scan output y and the gated yg / ycat / yn are stored in bf16 (each value rounded once, to nearest even).
+x_dbl stays fp32 (it carries dt, B and C into softplus and exp, and it is small), the SE gates of ConMB average in fp32, and
+out_proj, the PatchMerging reduction and x_proj write fp32, so their residual and rscale epilogues read fp32.  Everything
+else (the decoder's CAB convs, patch embed, PatchExpand, UpsampleExpand, the final head, the pools) runs in the dense mode
+torch's matmul switch selects, with autocast switched off around the torch ops the fused path calls.
 """
 import ctypes
 
@@ -27,12 +36,12 @@ def _stream():
 
 
 # ---------------------------------------------------------------- primitive wrappers
-def layernorm(x2d, ln):
-    """nn.LayerNorm over the last dim of a contiguous (rows, C) tensor."""
+def layernorm(x2d, ln, dtype=torch.float32):
+    """nn.LayerNorm over the last dim of a contiguous (rows, C) fp32 tensor; dtype=torch.bfloat16 stores the output as bf16."""
     rows, C = x2d.shape
-    y = torch.empty_like(x2d)
-    _lib.check(_lib.lib().sigma_layernorm_fwd(_p(x2d), _p(ln.weight), _p(ln.bias), _p(y), rows, C, float(ln.eps), _stream()),
-               "sigma_layernorm_fwd")
+    y = torch.empty((rows, C), dtype=dtype, device=x2d.device)
+    fn = "sigma_layernorm_fwd_bf16" if dtype == torch.bfloat16 else "sigma_layernorm_fwd"
+    _lib.check(getattr(_lib.lib(), fn)(_p(x2d), _p(ln.weight), _p(ln.bias), _p(y), rows, C, float(ln.eps), _stream()), fn)
     return y
 
 
@@ -40,23 +49,54 @@ USE_OWN_GEMM = True  # False: cuBLAS through torch (library GEMM, precision by t
 
 
 def precision():
-    """Dense-projection precision of the fused path (the scan, LayerNorms and the convolutions' accumulation are fp32 regardless).
-    It follows torch's own switch, exactly like the reference's nn.Linear layers do:
+    """Precision of the fused path.  With autograd off and torch.autocast("cuda", dtype=torch.bfloat16) active it is "bf16": the
+    SS2D / ConMB / CroMB / PatchMerging interiors store bf16 and their GEMMs run bf16 wgmma (module docstring); logits within
+    2x the error of the reference's own layers under the same autocast.  Autocast with fp16 is not a mode of the fused path: it
+    keeps the fp32 modes below.  With autograd on (training) autocast does not change the fused core either.
+    Otherwise the dense-projection precision (the scan, LayerNorms and the convolutions' accumulation are fp32 regardless)
+    follows torch's own switch, exactly like the reference's nn.Linear layers do:
       torch.backends.cuda.matmul.allow_tf32 = False (torch's default) -> "tf32x3": fp32-GRADE products on the tensor cores — the
           hand-written wgmma GEMM with the error-compensated operand split (3 MMAs per k-step, sigma_linear_tf32x3); logits agree
           with the reference's fp32 results to ~1e-6 of their scale (1e-3 bar);
       torch.backends.cuda.matmul.allow_tf32 = True -> "tf32": the same kernel, one TF32 MMA per k-step (10-bit mantissa
           operands, fp32 accumulate in registers); logits within ~3e-3 of the reference's (1e-2 bar)."""
+    if not torch.is_grad_enabled() and torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16:
+        return "bf16"
+    return _dense_precision()
+
+
+def _dense_precision():
     return "tf32" if torch.backends.cuda.matmul.allow_tf32 else "tf32x3"
 
 
-def logits_bar():
-    """Parity bar for end-to-end logits of the fused path, as a fraction of the logit scale (tests state it through this)."""
-    return 1e-2 if precision() == "tf32" else 1e-3
+BF16_FLOOR = 1e-3   # fraction of the logit scale added to the bf16 bar
+
+
+def logits_bar(composed_err=None):
+    """Parity bar for end-to-end logits of the fused path, as a fraction of the logit scale (tests state it through this).
+    bf16 has no fixed bar: it is 2 x `composed_err` + BF16_FLOOR, where `composed_err` is the error (same fraction of the
+    scale) of the reference's op composition (modules.composed_path()) on the same inputs under the same autocast — so the
+    caller measures it first (tests/test_bf16_gpu.py)."""
+    mode = precision()
+    if mode == "bf16":
+        if composed_err is None:
+            raise ValueError("logits_bar(): the bf16 bar is relative; pass the composed path's error under the same autocast")
+        return 2.0 * composed_err + BF16_FLOOR
+    return 1e-2 if mode == "tf32" else 1e-3
+
+
+def _bf16_mode():
+    return precision() == "bf16"
+
+
+def _no_autocast():
+    """Context for the torch ops the fused path calls itself (SE / channel-attention gates, cuDNN fallbacks): they stay fp32."""
+    return torch.autocast("cuda", enabled=False)
 
 
 _FP32_KINDS = set()   # experiment hook (scripts/tf32_error_budget.py): kinds of projections forced to full precision in tf32 mode
 _SPLIT = {}           # id(weight) -> (weakref, version, W_hi, W_lo): the tf32x3 operand split of a weight, made once per version
+_BF16 = {}            # id(weight) -> (weakref, version, W_bf16): the bf16 copy of a weight, made once per version
 
 
 def _split_weight(w):
@@ -71,20 +111,38 @@ def _split_weight(w):
     return hi, lo
 
 
-def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="dense"):
+def _bf16_weight(w):
+    import weakref
+    ent = _BF16.get(id(w))
+    if ent is not None and ent[0]() is w and ent[1] == w._version:
+        return ent[2]
+    wb = w.detach().to(torch.bfloat16).contiguous()
+    key = id(w)
+    _BF16[key] = (weakref.ref(w, lambda _r, k=key: _BF16.pop(k, None)), w._version, wb)
+    return wb
+
+
+def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="dense", out_dtype=torch.float32):
     """Dense projection out = x·W^T (+bias) (+residual·rscale) through the hand-written wgmma GEMM (csrc/gemm_tf32.cu: TMA-fed,
     register accumulators, fused epilogue), in the precision `precision()` names.  x2d (M, K) with unit column stride, row stride
     % 4 == 0; weight (N, K).  Shapes the kernel cannot take (K or N not a multiple of 4) go to torch.mm.
 
     Limitation: in tf32x3 mode the weight's hi / lo split is cached per weight and refreshed when `weight._version` changes
     (optimizer steps, in-place ops under torch.no_grad(), load_state_dict).  A write through `weight.data` does not change
-    `_version`, so the next call still uses the split of the old values (conv3x3's re-ordered weight likewise)."""
+    `_version`, so the next call still uses the split of the old values (conv3x3's re-ordered weight likewise).
+
+    A bf16 x2d runs the bf16 instance (sigma_linear_bf16: bf16 operands, fp32 accumulation) whatever `precision()` says, with a
+    bf16 copy of the weight cached on `_version` exactly like the tf32x3 split (same `.data` limitation); the output is fp32 or
+    (out_dtype=torch.bfloat16) bf16.  Rows whose byte stride is not a multiple of 16 go to torch.mm."""
     M, K = x2d.shape
     N = weight.shape[0]
+    if x2d.dtype == torch.bfloat16:
+        return _linear_bf16(x2d, weight, bias, out, residual, rscale, out_dtype)
     if out is None:
         out = torch.empty((M, N), dtype=torch.float32, device=x2d.device)
     if not USE_OWN_GEMM or K % 4 or x2d.stride(1) != 1 or x2d.stride(0) % 4 or N % 4:
-        torch.mm(x2d, weight.t(), out=out)
+        with _no_autocast():
+            torch.mm(x2d, weight.t(), out=out)
         if bias is not None:
             out += bias
         if residual is not None:
@@ -92,7 +150,7 @@ def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="d
         return out
     w = weight if weight.is_contiguous() else weight.contiguous()
     ldr = residual.stride(0) if residual is not None else 0
-    if precision() == "tf32" and kind not in _FP32_KINDS:
+    if _dense_precision() == "tf32" and kind not in _FP32_KINDS:
         rc = _lib.lib().sigma_linear_tf32(_p(x2d), x2d.stride(0), _p(w), _p(bias), _p(residual), ldr, _p(rscale), _p(out),
                                           out.stride(0), M, N, K, _stream())
         _lib.check(rc, "sigma_linear_tf32")
@@ -101,6 +159,29 @@ def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="d
         rc = _lib.lib().sigma_linear_tf32x3(_p(x2d), x2d.stride(0), _p(hi), _p(lo), _p(bias), _p(residual), ldr, _p(rscale), _p(out),
                                             out.stride(0), M, N, K, _stream())
         _lib.check(rc, "sigma_linear_tf32x3")
+    return out
+
+
+def _linear_bf16(x2d, weight, bias, out, residual, rscale, out_dtype):
+    M, K = x2d.shape
+    N = weight.shape[0]
+    if out is None:
+        out = torch.empty((M, N), dtype=out_dtype, device=x2d.device)
+    w = _bf16_weight(weight)
+    if not USE_OWN_GEMM or K % 8 or x2d.stride(1) != 1 or x2d.stride(0) % 8 or N % 4 or out.stride(0) % 4:
+        with _no_autocast():
+            t = torch.mm(x2d.float(), w.float().t())              # bf16 values are exact in fp32 (and in TF32)
+            if bias is not None:
+                t += bias
+            if residual is not None:
+                t += residual * rscale if rscale is not None else residual
+            out.copy_(t)
+        return out
+    ldr = residual.stride(0) if residual is not None else 0
+    c_dtype = _lib.BF16 if out.dtype == torch.bfloat16 else _lib.F32
+    rc = _lib.lib().sigma_linear_bf16(_p(x2d), x2d.stride(0), _p(w), _p(bias), _p(residual), ldr, _p(rscale), _p(out), out.stride(0),
+                                      c_dtype, M, N, K, _stream())
+    _lib.check(rc, "sigma_linear_bf16")
     return out
 
 
@@ -150,9 +231,10 @@ def conv3x3(x, conv, gelu=False):
 
 
 def dwconv3x3_silu(x, x_row_stride, x_batch_stride, conv, out, out_batch_stride, batch, H, W, D):
-    _lib.check(_lib.lib().sigma_dwconv3x3_silu_fwd(_p(x), x_row_stride, x_batch_stride, _p(conv.weight), _p(conv.bias),
-                                                   _p(out), out_batch_stride, batch, H, W, D, _stream()),
-               "sigma_dwconv3x3_silu_fwd")
+    """x and out both fp32, or both bf16 (sigma_dwconv3x3_silu_fwd_bf16)."""
+    fn = "sigma_dwconv3x3_silu_fwd_bf16" if x.dtype == torch.bfloat16 else "sigma_dwconv3x3_silu_fwd"
+    _lib.check(getattr(_lib.lib(), fn)(_p(x), x_row_stride, x_batch_stride, _p(conv.weight), _p(conv.bias),
+                                       _p(out), out_batch_stride, batch, H, W, D, _stream()), fn)
     return out
 
 
@@ -160,9 +242,14 @@ def ss2d_scan(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
     L_ = _lib.lib()
     ndir = {_lib.DIRS_CROSS4: 4, _lib.DIRS_SEQ2: 2, _lib.DIRS_CROSS: 1}[kind]
     Lseq = 2 * H * W if kind == _lib.DIRS_SEQ2 else H * W
-    y = torch.empty((ndir, batch, Lseq, D), dtype=torch.float32, device=xc.device)
+    y = torch.empty((ndir, batch, Lseq, D), dtype=xc.dtype, device=xc.device)      # bf16 xc -> bf16 y
     wsb = L_.sigma_ss2d_scan_workspace_bytes(kind, batch, H, W, D, N)
     ws = torch.empty(wsb, dtype=torch.uint8, device=xc.device)
+    if xc.dtype == torch.bfloat16:
+        rc = L_.sigma_ss2d_scan_fwd_bf16(kind, _p(xc), _p(xdbl), _p(dtw), _p(dtb), _p(A), _p(Ds), _p(y), batch, H, W, D, N, R, Cp,
+                                         _p(ws), wsb, _stream())
+        _lib.check(rc, "sigma_ss2d_scan_fwd_bf16")
+        return y
     if _FORCE_SPLIT:
         rc = L_.sigma_ss2d_scan_fwd_split(kind, _p(xc), _p(xdbl), _p(dtw), _p(dtb), _p(A), _p(Ds), _p(y), batch, H, W, D, N,
                                           R, Cp, _p(ws), wsb, _FORCE_SPLIT, _stream())
@@ -192,12 +279,13 @@ def ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
 
 def merge_norm_gate(y, K, k_stride, in_batch_stride, ln, z, z_row_stride, gate, out, out_batch_stride, out_row_stride,
                     rows, rows_per_batch, D, y_offset=0, out_offset=0):
-    yp = ctypes.c_void_p(y.data_ptr() + 4 * y_offset)
-    op = ctypes.c_void_p(out.data_ptr() + 4 * out_offset)
-    rc = _lib.lib().sigma_merge_norm_gate_fwd(yp, K, k_stride, in_batch_stride, _p(ln.weight), _p(ln.bias), z, z_row_stride,
-                                              _p(gate), op, out_batch_stride, out_row_stride, rows, rows_per_batch, D,
-                                              float(ln.eps), _stream())
-    _lib.check(rc, "sigma_merge_norm_gate_fwd")
+    """y, z and out all fp32, or all bf16 (sigma_merge_norm_gate_fwd_bf16); offsets and strides count elements."""
+    fn = "sigma_merge_norm_gate_fwd_bf16" if y.dtype == torch.bfloat16 else "sigma_merge_norm_gate_fwd"
+    yp = ctypes.c_void_p(y.data_ptr() + y.element_size() * y_offset)
+    op = ctypes.c_void_p(out.data_ptr() + out.element_size() * out_offset)
+    rc = getattr(_lib.lib(), fn)(yp, K, k_stride, in_batch_stride, _p(ln.weight), _p(ln.bias), z, z_row_stride,
+                                 _p(gate), op, out_batch_stride, out_row_stride, rows, rows_per_batch, D, float(ln.eps), _stream())
+    _lib.check(rc, fn)
     return out
 
 
@@ -255,27 +343,32 @@ def _cma_params(cm):
 def ss2d(m, x, residual=None, rscale=None):
     """SS2D.forward (vmamba.py:1067-1089); x (B,H,W,C) contiguous.  Returns (B,H,W,C) [+ residual (· rscale)], the
     residual being added in the out_proj GEMM epilogue."""
-    x = x.contiguous()
+    dt = torch.bfloat16 if _bf16_mode() else torch.float32     # storage of the block's interior (module docstring)
+    x = x.to(dt).contiguous()
     B, H, W, C = x.shape
     D, N, R, L = m.d_inner, m.d_state, m.dt_rank, H * W
     c = _ssm_params(m)
-    xz = linear(x.view(B * L, C), m.in_proj.weight, m.in_proj.bias, kind="in_proj")                    # (BL, 2D): [x | z]
-    xc = torch.empty((B, L, D), dtype=torch.float32, device=x.device)
+    xz = linear(x.view(B * L, C), m.in_proj.weight, m.in_proj.bias, kind="in_proj", out_dtype=dt)      # (BL, 2D): [x | z]
+    xc = torch.empty((B, L, D), dtype=dt, device=x.device)
     dwconv3x3_silu(xz, 2 * D, L * 2 * D, m.conv2d, xc, L * D, B, H, W, D)
-    xdbl = linear(xc.view(B * L, D), c["xproj"], kind="x_proj")                                        # (BL, 4·Cp)
+    xdbl = linear(xc.view(B * L, D), c["xproj"], kind="x_proj")                                        # (BL, 4·Cp) fp32
     y = ss2d_scan(_lib.DIRS_CROSS4, xc, xdbl, c["dtw"], c["dtb"], c["A"], c["Ds"], B, H, W, D, N, R, c["Cp"])
-    yg = torch.empty((B * L, D), dtype=torch.float32, device=x.device)
-    z = ctypes.c_void_p(xz.data_ptr() + 4 * D)
+    yg = torch.empty((B * L, D), dtype=dt, device=x.device)
+    z = ctypes.c_void_p(xz.data_ptr() + xz.element_size() * D)
     merge_norm_gate(y, 4, B * L * D, 0, m.out_norm, z, 2 * D, None, yg, 0, D, B * L, B * L, D)
     res2d = residual.reshape(B * L, C) if residual is not None else None
     return linear(yg, m.out_proj.weight, m.out_proj.bias, residual=res2d, rscale=rscale, kind="out_proj").view(B, H, W, C)
+
+
+def _interior_dtype():
+    return torch.bfloat16 if _bf16_mode() else torch.float32
 
 
 def vss_block(blk, x):
     """VSSBlock._forward (vmamba.py:1712-1716), mlp_ratio = 0."""
     x = x.contiguous()
     B, H, W, C = x.shape
-    xn = layernorm(x.view(-1, C), blk.norm).view(B, H, W, C)
+    xn = layernorm(x.view(-1, C), blk.norm, _interior_dtype()).view(B, H, W, C)
     return ss2d(blk.op, xn, residual=x)
 
 
@@ -284,10 +377,11 @@ def patch_merging(m, x):
     x = x.contiguous()
     B, H, W, C = x.shape
     H2, W2 = (H + 1) // 2, (W + 1) // 2
-    xn = torch.empty((B * H2 * W2, 4 * C), dtype=torch.float32, device=x.device)
+    bf16 = _bf16_mode()
+    xn = torch.empty((B * H2 * W2, 4 * C), dtype=torch.bfloat16 if bf16 else torch.float32, device=x.device)
     # 2x2 gather (+ zero padding of odd sizes) + LayerNorm(4C) in one kernel: no concatenated tensor
-    _lib.check(_lib.lib().sigma_patch_merge_norm_fwd(_p(x), _p(m.norm.weight), _p(m.norm.bias), _p(xn), B, H, W, C,
-                                                      float(m.norm.eps), _stream()), "sigma_patch_merge_norm_fwd")
+    fn = "sigma_patch_merge_norm_fwd_bf16" if bf16 else "sigma_patch_merge_norm_fwd"
+    _lib.check(getattr(_lib.lib(), fn)(_p(x), _p(m.norm.weight), _p(m.norm.bias), _p(xn), B, H, W, C, float(m.norm.eps), _stream()), fn)
     return linear(xn, m.reduction.weight).view(B, H2, W2, -1)
 
 
@@ -300,16 +394,18 @@ def cromb_ss2d(m, x_rgb, x_e, residual=False):
     N, R = cm.d_state, cm.dt_rank
     c = _cma_params(cm)
     dev = x_rgb.device
-    xp = torch.empty((2, B * L, D), dtype=torch.float32, device=dev)          # modality-major
-    linear(x_rgb.view(B * L, C), m.in_proj.weight, m.in_proj.bias, out=xp[0])
-    linear(x_e.view(B * L, C), m.in_proj_modalx.weight, m.in_proj_modalx.bias, out=xp[1])
-    xc = torch.empty((2 * B, L, D), dtype=torch.float32, device=dev)
+    dt = _interior_dtype()
+    a_r, a_e = x_rgb.to(dt), x_e.to(dt)                                        # GEMM operands (the residuals below stay fp32)
+    xp = torch.empty((2, B * L, D), dtype=dt, device=dev)                     # modality-major
+    linear(a_r.view(B * L, C), m.in_proj.weight, m.in_proj.bias, out=xp[0])
+    linear(a_e.view(B * L, C), m.in_proj_modalx.weight, m.in_proj_modalx.bias, out=xp[1])
+    xc = torch.empty((2 * B, L, D), dtype=dt, device=dev)
     dwconv3x3_silu(xp, D, L * D, m.conv2d, xc, L * D, 2 * B, H, W, D)         # ONE conv for both modalities (:1629-1630)
     xdbl = torch.empty((2, B * L, c["Cp"]), dtype=torch.float32, device=dev)
     linear(xc[:B].view(B * L, D), c["xproj1"], out=xdbl[0], kind="x_proj")
     linear(xc[B:].view(B * L, D), c["xproj2"], out=xdbl[1], kind="x_proj")
     y = ss2d_scan(_lib.DIRS_CROSS, xc, xdbl, c["dtw"], c["dtb"], c["A"], c["Ds"], 2 * B, H, W, D, N, R, c["Cp"])  # (1,2B,L,D)
-    yn = torch.empty((2, B * L, D), dtype=torch.float32, device=dev)
+    yn = torch.empty((2, B * L, D), dtype=dt, device=dev)
     merge_norm_gate(y, 1, 0, 0, cm.out_norm_1, None, 0, None, yn, 0, D, B * L, B * L, D)
     merge_norm_gate(y, 1, 0, 0, cm.out_norm_2, None, 0, None, yn, 0, D, B * L, B * L, D, y_offset=B * L * D, out_offset=B * L * D)
     r_r = x_rgb.view(B * L, C) if residual else None
@@ -326,17 +422,19 @@ def conmb_ss2d(m, x_rgb, x_e, residual=None):
     D, N, R, L = m.d_inner, m.d_state, m.dt_rank, H * W
     c = _ssm_params(m)
     dev = x_rgb.device
-    tr = linear(x_rgb.view(B * L, C), m.in_proj.weight, m.in_proj.bias)
-    te = linear(x_e.view(B * L, C), m.in_proj_modalx.weight, m.in_proj_modalx.bias)
-    seq = torch.empty((B, 2 * L, D), dtype=torch.float32, device=dev)         # [rgb ‖ x] along L (vmamba.py:130)
+    dt = _interior_dtype()
+    tr = linear(x_rgb.to(dt).view(B * L, C), m.in_proj.weight, m.in_proj.bias, out_dtype=dt)
+    te = linear(x_e.to(dt).view(B * L, C), m.in_proj_modalx.weight, m.in_proj_modalx.bias, out_dtype=dt)
+    seq = torch.empty((B, 2 * L, D), dtype=dt, device=dev)                    # [rgb ‖ x] along L (vmamba.py:130)
     dwconv3x3_silu(tr, D, L * D, m.conv2d, seq, 2 * L * D, B, H, W, D)
     dwconv3x3_silu(te, D, L * D, m.conv2d_modalx, seq[:, L:], 2 * L * D, B, H, W, D)
     xdbl = linear(seq.view(B * 2 * L, D), c["xproj"], kind="x_proj")          # (B·2L, 2·Cp)
     y = ss2d_scan(_lib.DIRS_SEQ2, seq, xdbl, c["dtw"], c["dtb"], c["A"], c["Ds"], B, H, W, D, N, R, c["Cp"])  # (2,B,2L,D)
     # SE gates from the PRE-conv projections, applied crosswise (vmamba.py:1276-1281)
-    g_r = m.fc1(tr.view(B, L, D).mean(dim=1))
-    g_e = m.fc2(te.view(B, L, D).mean(dim=1))
-    ycat = torch.empty((B * L, 2 * D), dtype=torch.float32, device=dev)
+    with _no_autocast():                                                      # the gates average and run in fp32
+        g_r = m.fc1(tr.view(B, L, D).mean(dim=1, dtype=torch.float32))
+        g_e = m.fc2(te.view(B, L, D).mean(dim=1, dtype=torch.float32))
+    ycat = torch.empty((B * L, 2 * D), dtype=dt, device=dev)
     ks = B * 2 * L * D
     merge_norm_gate(y, 2, ks, 2 * L * D, m.out_norm1, None, 0, g_e, ycat, L * 2 * D, 2 * D, B * L, L, D)
     merge_norm_gate(y, 2, ks, 2 * L * D, m.out_norm2, None, 0, g_r, ycat, L * 2 * D, 2 * D, B * L, L, D,
@@ -401,7 +499,7 @@ def cvss_decoder_block(blk, x):
     """CVSSDecoderBlock._forward (vmamba.py:1800-1805) with ChannelAttentionBlock (vmamba.py:1725-1757)."""
     x = x.contiguous()
     B, H, W, C = x.shape
-    xn = layernorm(x.view(-1, C), blk.norm1).view(B, H, W, C)
+    xn = layernorm(x.view(-1, C), blk.norm1, _interior_dtype()).view(B, H, W, C)
     x1 = ss2d(blk.op, xn, residual=x, rscale=blk.scale1)            # x·scale1 + SS2D(LN(x)) in the GEMM epilogue
     xn2 = layernorm(x1.view(-1, C), blk.norm2).view(B, H, W, C)
     cab = blk.conv_blk.cab
@@ -409,11 +507,12 @@ def cvss_decoder_block(blk, x):
     if isinstance(cab[1], torch.nn.GELU) and getattr(cab[1], "approximate", "none") == "none":
         h1 = conv3x3(xn2, cab[0], gelu=True)                         # conv3x3 + bias + GELU: implicit GEMM on the wgmma kernel
         t = conv3x3(h1, cab[2]) if h1 is not None else None
-    if t is None:                                                    # other conv forms: cuDNN on a channels_last view
-        t = cab[2](cab[1](cab[0](xn2.permute(0, 3, 1, 2)))).permute(0, 2, 3, 1).contiguous()
-    avg, mx = pool_avgmax(t)
-    fc = cab[3].fc
-    attn = torch.sigmoid(fc(avg.view(B, C, 1, 1)) + fc(mx.view(B, C, 1, 1))).view(B, C).contiguous()
+    with _no_autocast():                                             # CAB stays in the dense mode under autocast
+        if t is None:                                                # other conv forms: cuDNN on a channels_last view
+            t = cab[2](cab[1](cab[0](xn2.permute(0, 3, 1, 2)))).permute(0, 2, 3, 1).contiguous()
+        avg, mx = pool_avgmax(t)
+        fc = cab[3].fc
+        attn = torch.sigmoid(fc(avg.view(B, C, 1, 1)) + fc(mx.view(B, C, 1, 1))).view(B, C).contiguous()
     return scale_add(t, attn, x1, blk.scale2, H * W)               # CAB(x)·attn + x·scale2
 
 

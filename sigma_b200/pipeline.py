@@ -13,6 +13,8 @@ stages of neighbouring batches on three streams:
 The forward is one CUDA graph (captured once); the graph's static input / output tensors are decoupled from the
 transfers by device-side staging buffers (two of each), so a transfer never touches a tensor the graph is using.
 """
+import contextlib
+
 import torch
 
 
@@ -26,10 +28,14 @@ class InferencePipeline:
     The model must be in eval mode.  The captured graph holds the device pointers of the model's parameters AND of the
     packed SSM tensors the fused path derives from them (x_proj / dt / A = -exp(A_logs) / D copies, fused._cache): when
     any parameter is modified in place afterwards (load_state_dict, an optimizer step) `submit` notices the changed
-    version counters and re-captures the graph, so stale packed copies are never replayed."""
+    version counters and re-captures the graph, so stale packed copies are never replayed.
 
-    def __init__(self, model, batch, height, width, use_graph=True):
+    amp_dtype=torch.bfloat16 runs the forward (warm-up, capture and any re-capture) under torch.autocast("cuda", dtype=amp_dtype),
+    so the captured graph is the one of the fused path's bf16 mode (sigma_b200.fused.precision); None runs it as called."""
+
+    def __init__(self, model, batch, height, width, use_graph=True, amp_dtype=None):
         self.model = model
+        self.amp_dtype = amp_dtype
         p = next(model.parameters())
         if p.device.type != "cuda":
             raise RuntimeError("sigma_b200.InferencePipeline needs the model on a CUDA device (there is no CPU path)")
@@ -57,14 +63,17 @@ class InferencePipeline:
     def _versions(self):
         return sum(p._version for p in self.model.parameters())
 
+    def _autocast(self):
+        return torch.autocast("cuda", dtype=self.amp_dtype) if self.amp_dtype is not None else contextlib.nullcontext()
+
     def _capture(self):
-        with torch.cuda.stream(self.compute), torch.no_grad():
+        with torch.cuda.stream(self.compute), torch.no_grad(), self._autocast():
             for _ in range(2):                       # warm-up: allocator, kernel attributes, cuDNN algorithm choice, packed-parameter cache
                 out = self.model(self.rgb, self.x)
         self.compute.synchronize()
         if self.use_graph:
             self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph, stream=self.compute), torch.no_grad():
+            with torch.cuda.graph(self.graph, stream=self.compute), torch.no_grad(), self._autocast():
                 out = self.model(self.rgb, self.x)
             self.compute.synchronize()
         self.out = out                               # the graph's static output tensor
@@ -94,7 +103,8 @@ class InferencePipeline:
             if self.graph is not None:
                 self.graph.replay()
             else:
-                self.out = self.model(self.rgb, self.x)
+                with self._autocast():
+                    self.out = self.model(self.rgb, self.x)
             if not first_use:
                 self.compute.wait_event(self.ev_out_free[s])
             self.stage_out[s].copy_(self.out, non_blocking=True)
