@@ -283,6 +283,12 @@ int sigma_conv3x3_tf32(const float *x, const float *w9, const float *w9_lo, cons
  * x3 selects the instance: 0 = tf32, 1 = tf32x3, 2 = sigma_linear_bf16 (conv_B must be 0); other values are SIGMA_EINVAL.      */
 int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, int64_t *out6_host);
 
+/* L-segment plan of the fused scan backward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_bwd (nsplit = 0)
+ * or sigma_ss2d_scan_bwd_split / sigma_ss2d_scan_bwd_saved with that nsplit would launch for kind CROSS4 / SEQ2 at (batch, H, W, D,
+ * N).  out4_host = {segments, 16-position tiles per segment, tiles of the longest direction's walk, tiles of the shortest}.  The
+ * directions share the tiles per segment, so a walk shorter than the longest can end in empty segments.  For tests and tuning. */
+int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, int nsplit, int64_t *out4_host);
+
 /* ------------------------------------------------------------------------------------------
  * SURVEY.md §8(f) rank 2, first piece: the evaluator's per-batch metric on the device (eval.py:22-29,
  * utils/metric.py:8-15).  pred = argmax over classes of logits (batch, classes, H, W) — the index numpy.argmax

@@ -269,6 +269,7 @@ int ss2d_pick_segments_hook(long long ctas, int nw, int ntiles, int N);
 int gemm_pick_bn_hook(int N, long long m_tiles);
 int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out);
 size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
+int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int force_split, long long *out4);
 int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                   const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
                   int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream,
@@ -486,6 +487,19 @@ int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H
   const int rc = gemm_plan_hook(M, N, K, x3, conv_B, conv_H, conv_W, out);
   if (rc) return rc;
   for (int i = 0; i < 6; ++i) out6_host[i] = out[i];
+  return SIGMA_OK;
+}
+
+// the L-segment plan of sigma_ss2d_scan_bwd{,_split,_saved} (nsplit = 0: the library's choice):
+// out4_host = {segments, tiles per segment, tiles of the longest walk, tiles of the shortest walk}
+int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, int nsplit, int64_t *out4_host) {
+  SIGMA_CHECK_ARG(out4_host && (kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2) && batch > 0 && H > 0 && W > 0 && D > 0 &&
+                      D % 64 == 0 && (N == 4 || N == 16) && nsplit >= 0,
+                  "sigma_test_ss2d_bwd_plan: bad arguments");
+  long long out[4];
+  const int rc = ss2d_bwd_plan_hook(kind, batch, H, W, D, N, nsplit, out);
+  if (rc) return rc;
+  for (int i = 0; i < 4; ++i) out4_host[i] = out[i];
   return SIGMA_OK;
 }
 

@@ -461,6 +461,32 @@ size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, i
   return fb_al((size_t)K * batch * fb_max_tiles(kind, H, W) * D * N * sizeof(float)) + 2 * fb_al(carry);
 }
 
+// The L-segment plan of the three sweeps.  All directions share tiles_per_split, so a direction with fewer tiles than the
+// longest walk (min_tiles < max_tiles) can get empty trailing segments.  force_split > 0 overrides the count (capped at 64).
+struct FbPlan { int nsplit, tiles_per_split, max_tiles, min_tiles; };
+
+static FbPlan fb_plan(int kind, int batch, int H, int W, int D, int N, int force_split) {
+  const int K = kind == SIGMA_DIRS_CROSS4 ? 4 : 2;
+  const long long Lseq = kind == SIGMA_DIRS_SEQ2 ? 2LL * H * W : (long long)H * W;
+  const int row_tiles = (int)((Lseq + FB_LT - 1) / FB_LT), col_tiles = W * ((H + FB_LT - 1) / FB_LT);
+  FbPlan pl;
+  pl.max_tiles = kind == SIGMA_DIRS_CROSS4 ? std::max(row_tiles, col_tiles) : row_tiles;
+  pl.min_tiles = kind == SIGMA_DIRS_CROSS4 ? std::min(row_tiles, col_tiles) : row_tiles;
+  const int lpc = N >= 16 ? 2 : 1;
+  int nsplit = pick_segments((long long)(D / FB_DT) * K * batch, pl.max_tiles, kNumSMs * (lpc == 2 ? 2 : 4), 1.3, kFbMaxSplit);
+  if (force_split > 0) nsplit = std::min(force_split, kFbMaxSplit);
+  nsplit = std::max(1, std::min(nsplit, pl.max_tiles));
+  pl.tiles_per_split = (pl.max_tiles + nsplit - 1) / nsplit;
+  pl.nsplit = (pl.max_tiles + pl.tiles_per_split - 1) / pl.tiles_per_split;
+  return pl;
+}
+
+int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int force_split, long long *out4) {
+  const FbPlan pl = fb_plan(kind, batch, H, W, D, N, force_split);
+  out4[0] = pl.nsplit; out4[1] = pl.tiles_per_split; out4[2] = pl.max_tiles; out4[3] = pl.min_tiles;
+  return SIGMA_OK;
+}
+
 // delta / ddelta: (K, batch, Lseq, D) slabs stored at the position a value belongs to; dxc (batch, Lseq, D) and dxdbl
 // (batch, Lseq, K, Cp) are ACCUMULATED INTO after being zeroed here; dA (K·D, N), dDs (K·D), ddtb (K, D) overwritten.
 int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
@@ -485,7 +511,7 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
   p.hs_in = hs_saved ? hs_saved : p.hs;   // hs_saved: the training forward already wrote delta' and the block-start states
   float *fcarry = (float *)((char *)ws + hs_b), *rcarry = (float *)((char *)ws + hs_b + carry_b);
   const int CPW = N >= 16 ? 16 : 32;
-  int rc, max_tiles = 0;
+  int rc;
   for (int k = 0; k < K; ++k) {
     const bool colmajor = kind == SIGMA_DIRS_CROSS4 && (k & 1);
     p.rev[k] = kind == SIGMA_DIRS_CROSS4 ? (k >= 2) : (k == 1);
@@ -512,15 +538,10 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
     if (!colmajor) { str[0] = pos; str[1] = Lseq * pos; str[2] = Lseq * pos; }
     else { str[0] = W * pos; str[1] = pos; str[2] = Lseq * pos; }
     if ((rc = make_tmap_f32_4d(&p.m_dbl[k], xdbl + (long long)k * Cp, dims, str, boxd))) return rc;
-    max_tiles = std::max(max_tiles, p.O[k] * ((p.I[k] + FB_LT - 1) / FB_LT));
   }
-  // L-segments: all directions share tiles_per_split (directions with fewer tiles get empty trailing segments)
-  const int lpc = N >= 16 ? 2 : 1;
-  int nsplit = pick_segments((long long)(D / FB_DT) * K * batch, max_tiles, kNumSMs * (lpc == 2 ? 2 : 4), 1.3, kFbMaxSplit);
-  if (force_split > 0) nsplit = std::min(force_split, kFbMaxSplit);
-  nsplit = std::max(1, std::min(nsplit, max_tiles));
-  p.tiles_per_split = (max_tiles + nsplit - 1) / nsplit;
-  p.nsplit = (max_tiles + p.tiles_per_split - 1) / p.tiles_per_split;
+  const FbPlan pl = fb_plan(kind, batch, H, W, D, N, force_split);
+  p.tiles_per_split = pl.tiles_per_split;
+  p.nsplit = pl.nsplit;
   p.nst = 2;
 
   SIGMA_CHECK_CUDA(cudaMemsetAsync(dxc, 0, (size_t)batch * Lseq * D * sizeof(float), stream));

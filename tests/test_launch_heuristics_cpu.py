@@ -148,3 +148,45 @@ def test_forced_tile_width_rejects_bad_values(L, value, monkeypatch):
     monkeypatch.delenv("SIGMA_GEMM_BN")
     assert L.sigma_test_gemm_plan(1000, 768, 192, 1, 0, 0, 0, out) == 0
 
+
+
+# ---- the L-segment plan of the fused scan backward (sigma_test_ss2d_bwd_plan = the planner sigma_ss2d_scan_bwd* launch with) ----
+# Sigma's training shapes: (kind, H, W, D, d_state) — encoder SS2D stages of tiny / small (D 192..1536) and base (45 x 60, 23 x 30),
+# ConMB (SEQ2, d_state 4) and the decoder's SS2D (d_state 4)
+BWD_SHAPES = [("cross4", 120, 160, 192, 16), ("cross4", 60, 80, 384, 16), ("cross4", 30, 40, 768, 16), ("cross4", 15, 20, 1536, 16),
+              ("cross4", 45, 60, 1024, 16), ("cross4", 23, 30, 2048, 16), ("seq2", 120, 160, 192, 4), ("seq2", 60, 80, 384, 4),
+              ("seq2", 30, 40, 768, 4), ("seq2", 15, 20, 1536, 4), ("seq2", 23, 30, 2048, 4), ("cross4", 120, 160, 192, 4),
+              ("cross4", 60, 80, 384, 4), ("cross4", 30, 40, 768, 4)]
+
+
+def ss2d_bwd_plan(kind, B, H, W, D, N, nsplit=0):
+    import ctypes
+    from sigma_b200 import _lib
+    out = (ctypes.c_int64 * 4)()
+    k = _lib.DIRS_CROSS4 if kind == "cross4" else _lib.DIRS_SEQ2
+    _lib.check(_lib.lib().sigma_test_ss2d_bwd_plan(k, B, H, W, D, N, nsplit, out), "sigma_test_ss2d_bwd_plan")
+    return dict(zip(("nsplit", "tiles_per_split", "max_tiles", "min_tiles"), (int(v) for v in out)))
+
+
+@pytest.mark.parametrize("kind,H,W,D,N", BWD_SHAPES)
+@pytest.mark.parametrize("B", [1, 2, 3, 8])
+def test_ss2d_bwd_plan_invariants(L, kind, H, W, D, N, B):
+    rows = -(-H * W * (2 if kind == "seq2" else 1) // 16)
+    for force in [0, 1, 2, 7, 20, 64, 100]:
+        pl = ss2d_bwd_plan(kind, B, H, W, D, N, force)
+        assert pl["max_tiles"] == (max(rows, W * -(-H // 16)) if kind == "cross4" else rows)
+        assert pl["min_tiles"] == (min(rows, W * -(-H // 16)) if kind == "cross4" else rows)
+        assert 1 <= pl["nsplit"] <= 64
+        assert pl["tiles_per_split"] * pl["nsplit"] >= pl["max_tiles"]                 # every tile of the longest walk is covered
+        assert (pl["nsplit"] - 1) * pl["tiles_per_split"] < pl["max_tiles"]             # and none of its segments is empty
+        if force:
+            assert pl["nsplit"] <= min(force, 64)
+
+
+def test_ss2d_bwd_plan_rejects_bad_arguments(L):
+    import ctypes
+    out = (ctypes.c_int64 * 4)()
+    assert L.sigma_test_ss2d_bwd_plan(2, 1, 15, 20, 1536, 4, 0, out) != 0            # CROSS has no fused backward
+    assert L.sigma_test_ss2d_bwd_plan(0, 1, 15, 20, 96, 16, 0, out) != 0              # D % 64
+    assert L.sigma_test_ss2d_bwd_plan(0, 1, 15, 20, 1536, 8, 0, out) != 0             # d_state
+    assert L.sigma_test_ss2d_bwd_plan(0, 1, 15, 20, 1536, 16, -1, out) != 0

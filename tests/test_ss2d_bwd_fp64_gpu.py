@@ -1,0 +1,283 @@
+"""GPU: the fused SS2D scan backward (sigma_ss2d_scan_bwd / _bwd_split with its state sweep, and the training pair
+sigma_ss2d_scan_fwd_save + sigma_ss2d_scan_bwd_saved) against the fp64 reference of oracle/ss2d_ref64.py, element by element inside
+that module's per-element error bounds, at Sigma's training shapes:
+* every padded dt_rank Sigma trains with (6 .. 64), so every x_dbl tile size and state-sweep shared-memory layout runs;
+* ragged maps (15 x 20: every column tile has 15 rows; 23 x 30 odd in both), batch 1, 2 and 3;
+* L-segments 1, 2, 7, the library's choice and the 64 cap, a count that leaves the shorter walks an empty trailing segment, and a
+  training forward cut differently from its backward.  The premises (more than one segment at stage 0 by default, the empty
+  segment) are asserted through the backward's planner (sigma_test_ss2d_bwd_plan);
+* every output inside NaN-filled memory whose guard elements must stay bit-identical, the dt_r and padding columns of dxdbl 0;
+* y, delta' and the tile-start states hs of the training forward too, and of the state sweep (its workspace).
+At the autograd level FusedSS2DCore.apply is checked through all six gradients against the reference chained with the fp64
+x_proj / dt_proj algebra of its backward.  Parameters: dt log-uniform in [1e-3, 0.1] through the inverse softplus, A = -exp(A_log)
+around the S4D-real init, Ds near 1; one widened set (dt up to 0.5, |A| up to 4x).  Worst bound fractions go to helpers.record."""
+import ctypes
+import math
+
+import pytest
+import torch
+
+import procedural as P
+from helpers import record
+from oracle import ss2d_ref64 as R64
+
+pytestmark = pytest.mark.gpu
+S = 97
+G = 64                                   # guard floats on each side of every output (keeps 16-byte alignment)
+NAN32 = 0x7FC00000
+OUTS = ("y", "delta", "hs", "dxc", "ddelta", "dA", "dDs", "ddtb")
+# d dt_bias sums the per-element bounds of ddelta over all B·L positions; at dt_rank 48 / 64 that leaves its bound at the largest
+# element up to ~6x looser than 1e-3 of scale, so it must also meet that max-norm bar
+MAXNORM_TOO = ("ddtb",)
+
+
+def _p(t):
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def _stream():
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def _guarded(shape):
+    n = math.prod(shape)
+    buf = torch.full((n + 2 * G,), float("nan"), device="cuda")
+    return buf, buf[G:G + n].view(shape)
+
+
+def _guard_ok(buf, what):
+    n = buf.numel() - 2 * G
+    bits = torch.cat([buf[:G], buf[G + n:]]).view(torch.int32)
+    bad = int((bits != NAN32).sum())
+    assert bad == 0, f"{what}: {bad} guard elements were written"
+
+
+def _plan(kind, B, H, W, D, N, nsplit):
+    from sigma_b200 import _lib
+    out = (ctypes.c_int64 * 4)()
+    _lib.check(_lib.lib().sigma_test_ss2d_bwd_plan(_kid(kind), B, H, W, D, N, nsplit, out), "sigma_test_ss2d_bwd_plan")
+    return dict(zip(("nsplit", "tiles_per_split", "max_tiles", "min_tiles"), (int(v) for v in out)))
+
+
+def _kid(kind):
+    from sigma_b200 import _lib
+    return _lib.DIRS_CROSS4 if kind == "cross4" else _lib.DIRS_SEQ2
+
+
+def _params(kind, B, H, W, D, N, R, tag, wide=False):
+    from sigma_b200 import _lib
+    K = 4 if kind == "cross4" else 2
+    Lseq = H * W * (2 if kind == "seq2" else 1)
+    Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
+    xc = P.randn(S, tag + "/xc", (B, Lseq, D))
+    xdbl = P.randn(S, tag + "/xdbl", (B, Lseq, K, Cp))
+    xdbl[..., 2 * N:2 * N + R] *= 2.0
+    xdbl[..., 2 * N + R:] = 0.0                                          # padding columns, as the packed x_proj leaves them
+    dtw = P.rand(S, tag + "/dtw", (K, D, R), -R ** -0.5, R ** -0.5)
+    dt = torch.exp(P.rand(S, tag + "/dt", (K, D), math.log(1e-3), math.log(0.5 if wide else 0.1)))
+    dtb = dt + torch.log(-torch.expm1(-dt))                              # inverse softplus
+    A_log = torch.log(torch.arange(1, N + 1, dtype=torch.float32)).repeat(K * D, 1) + P.rand(S, tag + "/A", (K * D, N), -0.2,
+                                                                                                  1.4 if wide else 0.2)
+    A = -torch.exp(A_log)
+    Ds = P.randn(S, tag + "/Ds", (K * D,), 0.1, 1.0)
+    dy = P.randn(S, tag + "/dy", (B, Lseq, D))
+    return [t.cuda() for t in (xc, xdbl, dtw, dtb, A, Ds, dy)], Cp
+
+
+def _check(tag, name, got, ref, bnd, worst):
+    ok = ~ref.isnan()
+    assert bool(torch.equal(got.isnan(), ~ok)), f"{tag} {name}: written where the kernel has nothing to write, or NaN"
+    frac = R64.bound_fraction(got[ok], ref[ok], bnd[ok])
+    worst[name] = max(worst.get(name, 0.0), frac)
+    assert frac <= 1.0, f"{tag} {name}: {frac:.3f} of the per-element bound"
+    # per element, yet at the largest element no looser than 1e-3 of the tensor's scale (checked once the fractions are logged)
+    if name in MAXNORM_TOO:
+        err = float((got[ok].double() - ref[ok]).abs().max()) / float(ref[ok].abs().max())
+        assert err <= 1e-3, f"{tag} {name}: {err:.2e} of its scale"
+    i = int(ref[ok].abs().argmax())
+    worst["at_max/" + name] = max(worst.get("at_max/" + name, 0.0), float(bnd[ok][i]) / (1e-3 * float(ref[ok].abs().max())))
+
+
+def _finish(tag, worst, tight=True):
+    record(tag, **worst)
+    loose = {k: v for k, v in worst.items() if k.startswith("at_max/") and k[7:] not in MAXNORM_TOO and v > 1.0}
+    assert not (tight and loose), f"{tag}: bound at the largest element looser than 1e-3 of scale: {loose}"
+
+
+def _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, tag, worst, split=None, saved=None):
+    """split: the state-sweep backward with that L-segment count (0: the library's choice).  saved = (fwd_split, bwd_split): the
+    training forward followed by the backward that consumes its delta' and states."""
+    from sigma_b200 import _lib
+    L_ = _lib.lib()
+    xc, xdbl, dtw, dtb, A, Ds, dy = args
+    K = xdbl.shape[2]
+    Lseq = xc.shape[1]
+    T = L_.sigma_ss2d_scan_hs_bytes(_kid(kind), B, H, W, D, N) // (4 * K * B * D * N)
+    bufs, outs = {}, {}
+    for name, shape in [("delta", (K, B, Lseq, D)), ("dxc", (B, Lseq, D)), ("ddelta", (K, B, Lseq, D)), ("dxdbl", (B, Lseq, K, Cp)),
+                        ("dA", (K * D, N)), ("dDs", (K * D,)), ("ddtb", (K, D)), ("y", (K, B, Lseq, D)), ("hs", (K, B, T, D, N))]:
+        bufs[name], outs[name] = _guarded(shape)
+    wsb = L_.sigma_ss2d_scan_bwd_workspace_bytes(_kid(kind), B, H, W, D, N)
+    ws = torch.full((wsb // 4,), float("nan"), device="cuda")
+    tail = (_p(outs["dxc"]), _p(outs["ddelta"]), _p(outs["dxdbl"]), _p(outs["dA"]), _p(outs["dDs"]), _p(outs["ddtb"]), B, H, W, D, N, R, Cp,
+            _p(ws), wsb)
+    head = (_kid(kind), _p(xc), _p(xdbl), _p(dtw), _p(dtb), _p(A), _p(Ds))
+    if saved is None:
+        if split:
+            rc = L_.sigma_ss2d_scan_bwd_split(*head, _p(dy), _p(outs["delta"]), *tail, split, _stream())
+        else:
+            rc = L_.sigma_ss2d_scan_bwd(*head, _p(dy), _p(outs["delta"]), *tail, _stream())
+        _lib.check(rc, "sigma_ss2d_scan_bwd")
+        hs = ws[:K * B * T * D * N].view(K, B, T, D, N)
+        names = ("delta", "hs", "dxc", "ddelta", "dA", "dDs", "ddtb")
+    else:
+        fwb = L_.sigma_ss2d_scan_workspace_bytes(_kid(kind), B, H, W, D, N)
+        fws = torch.zeros(max(fwb, 4), dtype=torch.uint8, device="cuda")
+        _lib.check(L_.sigma_ss2d_scan_fwd_save(*head, _p(outs["y"]), _p(outs["delta"]), _p(outs["hs"]), B, H, W, D, N, R, Cp, _p(fws), fwb,
+                                               saved[0], _stream()), "sigma_ss2d_scan_fwd_save")
+        _lib.check(L_.sigma_ss2d_scan_bwd_saved(*head, _p(dy), _p(outs["delta"]), _p(outs["hs"]), *tail, saved[1], _stream()),
+                   "sigma_ss2d_scan_bwd_saved")
+        hs = outs["hs"]
+        names = OUTS
+    torch.cuda.synchronize()
+    for name in names:
+        _check(tag, name, hs if name == "hs" else outs[name], ref[name], bnd[name], worst)
+    dx = outs["dxdbl"]
+    _check(tag, "dB", dx[..., :N], ref["dB"], bnd["dB"], worst)
+    _check(tag, "dC", dx[..., N:2 * N], ref["dC"], bnd["dC"], worst)
+    assert bool((dx[..., 2 * N:] == 0).all()), f"{tag}: the dt_r / padding columns of dxdbl must stay 0"
+    for name, buf in bufs.items():
+        _guard_ok(buf, f"{tag} {name}")
+
+
+# kind, B, H, W, D, N, R
+CASES = [
+    ("cross4", 2, 120, 160, 192, 16, 6), ("cross4", 2, 60, 80, 384, 16, 12), ("cross4", 2, 30, 40, 768, 16, 24),
+    ("cross4", 2, 15, 20, 1536, 16, 48), ("cross4", 2, 45, 60, 1024, 16, 32), ("cross4", 2, 23, 30, 2048, 16, 64),   # SS2D
+    ("seq2", 2, 120, 160, 192, 4, 6), ("seq2", 2, 15, 20, 1536, 4, 48), ("seq2", 2, 23, 30, 2048, 4, 64),              # ConMB
+    ("cross4", 2, 120, 160, 192, 4, 6), ("cross4", 2, 60, 80, 384, 4, 12), ("cross4", 2, 30, 40, 768, 4, 24),          # decoder SS2D
+    ("cross4", 1, 30, 40, 768, 16, 24), ("cross4", 3, 30, 40, 768, 16, 24),
+]
+
+
+@pytest.mark.parametrize("kind,B,H,W,D,N,R", CASES)
+def test_fused_bwd_matches_fp64(kind, B, H, W, D, N, R):
+    tag = f"{kind}/{B}/{H}x{W}/D{D}/N{N}/R{R}"
+    args, Cp = _params(kind, B, H, W, D, N, R, tag)
+    ref, bnd = R64.ss2d_ref64(kind, *args, H, W)
+    worst = {}
+    auto = _plan(kind, B, H, W, D, N, 0)
+    if (H, W) == (120, 160):
+        assert auto["nsplit"] > 1, auto                                  # stage 0 runs L-segments by default
+    splits = [1, 2, 7, 0, 100]
+    cap = _plan(kind, B, H, W, D, N, 100)
+    assert cap["tiles_per_split"] == -(-cap["max_tiles"] // 64) and cap["nsplit"] <= 64     # 100 is capped at 64 segments
+    if (H, W) == (15, 20):
+        pl = _plan(kind, B, H, W, D, N, 20)
+        if pl["min_tiles"] < pl["max_tiles"]:
+            assert (pl["nsplit"] - 1) * pl["tiles_per_split"] >= pl["min_tiles"]   # the shorter walks end in an empty segment
+            splits.append(20)
+    for sp in splits:
+        _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, f"{tag} split={sp}", worst, split=sp)
+    for fs, bs in [(0, 0), (3, 7), (1, 2)]:
+        _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, f"{tag} saved fwd={fs} bwd={bs}", worst, saved=(fs, bs))
+    _finish(f"ss2d bwd fp64 {tag}", worst)
+
+
+@pytest.mark.parametrize("kind,B,H,W,D,N,R", [("cross4", 2, 15, 20, 1536, 16, 48), ("seq2", 2, 60, 80, 384, 4, 12),
+                                               ("cross4", 1, 120, 160, 192, 16, 6)])
+def test_fused_bwd_matches_fp64_widened(kind, B, H, W, D, N, R):
+    """larger steps and decays: dt up to 0.5, |A| up to 4x the S4D-real init"""
+    tag = f"wide/{kind}/{B}/{H}x{W}/D{D}/N{N}/R{R}"
+    args, Cp = _params(kind, B, H, W, D, N, R, tag, wide=True)
+    ref, bnd = R64.ss2d_ref64(kind, *args, H, W)
+    worst = {}
+    for sp in [1, 0, 7]:
+        _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, f"{tag} split={sp}", worst, split=sp)
+    _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, f"{tag} saved", worst, saved=(0, 0))
+    _finish(f"ss2d bwd fp64 {tag}", worst)
+
+
+def _mm_bound(a, ea, b, n):
+    """bound of the fp32 product a @ b (b exact) given a's element bound: propagated error plus accumulation"""
+    return ea @ b.abs() + R64._gt(n) * (a.abs() @ b.abs())
+
+
+def _mm_bound_positions(aT, eaT, b):
+    """the same for a contraction over the B·L positions (aT (M, B·L), b (B·L, P)): the propagated first-order errors of
+    16-position chunks are combined as independent (oracle.ss2d_ref64.tile_rss); the fp32 accumulation's partial sums are bounded
+    by |result| + sqrt(sum of squared terms) (a drift plus a random walk), n roundings of them by LAMBDA·sqrt(n)·u of that"""
+    M, n = aT.shape
+    pad = (-n) % 16
+    ea = torch.nn.functional.pad(eaT, (0, pad)).view(M, -1, 16).transpose(0, 1)          # (chunks, M, 16)
+    bb = torch.nn.functional.pad(b.abs(), (0, 0, 0, pad)).view(-1, 16, b.shape[1])        # (chunks, 16, P)
+    part = torch.bmm(ea, bb)                                                              # (chunks, M, P)
+    rss = R64.LAMBDA * (part * part).sum(0).sqrt()
+    return rss + R64.LAMBDA * R64.U * math.sqrt(n) * ((aT @ b).abs() + ((aT * aT) @ (b * b)).sqrt())
+
+
+@pytest.mark.parametrize("kind,B,H,W,D,N,R", [("cross4", 2, 120, 160, 192, 16, 6), ("seq2", 2, 15, 20, 1536, 4, 48),
+                                               ("cross4", 2, 15, 20, 1536, 16, 48)])
+@pytest.mark.parametrize("save", [True, False])
+def test_fused_core_autograd_matches_fp64(kind, B, H, W, D, N, R, save, monkeypatch):
+    """FusedSS2DCore.apply: y and all six gradients against the reference chained with the fp64 x_proj / dt_proj algebra.  The
+    reference takes the very x_dbl the forward computed (the same deterministic GEMM call), so only the scan and the backward's
+    own fp32 GEMMs are under test; this pins the [dt | B | C] row order and the dA·A step at a real shape."""
+    from sigma_b200 import _lib, fused, ops
+    monkeypatch.setattr(ops, "FUSED_SAVE_STATES", save)
+    monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
+    K = 4 if kind == "cross4" else 2
+    Lseq = H * W * (2 if kind == "seq2" else 1)
+    Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
+    tag = f"ag/{kind}/{B}/{H}x{W}/D{D}/N{N}/R{R}"
+    xc0 = P.randn(S, tag + "/xc", (B, Lseq, D)).cuda()
+    wgt = P.randn(S, tag + "/w", (B, Lseq, D)).cuda()
+    xpw = P.randn(S, tag + "/xpw", (K, R + 2 * N, D), D ** -0.5).cuda()
+    dtw = P.rand(S, tag + "/dtw", (K, D, R), -R ** -0.5, R ** -0.5).cuda()
+    dt = torch.exp(P.rand(S, tag + "/dt", (K, D), math.log(1e-3), math.log(0.1)))
+    dtb = (dt + torch.log(-torch.expm1(-dt))).cuda()
+    Al = (torch.log(torch.arange(1, N + 1, dtype=torch.float32)).repeat(K * D, 1) + P.rand(S, tag + "/A", (K * D, N), -0.2, 0.2)).cuda()
+    Ds = P.randn(S, tag + "/Ds", (K * D,), 0.1, 1.0).cuda()
+    leaves = [t.clone().requires_grad_(True) for t in (xc0, xpw, dtw, dtb, Al, Ds)]
+    y = ops.FusedSS2DCore.apply(*leaves, _kid(kind), H, W)
+    (y * wgt).sum().backward()
+    got = [t.grad for t in leaves]
+    with torch.no_grad():
+        xw = torch.cat([fused._pack_xproj(xpw[k], N, R, Cp) for k in range(K)], dim=0).contiguous()
+        xdbl = fused.linear(xc0.view(B * Lseq, D), xw, kind="x_proj").view(B, Lseq, K, Cp)
+        A = -torch.exp(Al)
+        ref, bnd = R64.ss2d_ref64(kind, xc0, xdbl, dtw, dtb, A, Ds, wgt, H, W)
+        d = lambda t: t.double()
+        BL = B * Lseq
+        worst = {}
+        yr = ref["y"].sum(0)
+        yb = bnd["y"].sum(0) + K * R64.U * ref["y"].abs().sum(0)
+        _check(tag, "y", y.detach(), yr, yb, worst)
+        # dxdbl = [dB | dC | ddelta_k · W_dt[k] | 0] (fp32 GEMM per direction), then dxc += dxdbl · xw, d xw = dxdbl^T · xc
+        dxd, edxd = torch.zeros(B, Lseq, K, Cp, dtype=torch.float64, device="cuda"), torch.zeros(B, Lseq, K, Cp, dtype=torch.float64, device="cuda")
+        dxd[..., :N], dxd[..., N:2 * N] = ref["dB"], ref["dC"]
+        edxd[..., :N], edxd[..., N:2 * N] = bnd["dB"], bnd["dC"]
+        dW, edW = [], []
+        for k in range(K):
+            dd, edd = ref["ddelta"][k].reshape(BL, D), bnd["ddelta"][k].reshape(BL, D)
+            dxd[:, :, k, 2 * N:2 * N + R] = (dd @ d(dtw[k])).view(B, Lseq, R)
+            edxd[:, :, k, 2 * N:2 * N + R] = _mm_bound(dd, edd, d(dtw[k]), D).view(B, Lseq, R)
+            dtr = d(xdbl[:, :, k, 2 * N:2 * N + R]).reshape(BL, R)
+            dW.append(dd.t() @ dtr)
+            edW.append(_mm_bound_positions(dd.t(), edd.t(), dtr))
+        d2, e2 = dxd.view(BL, K * Cp), edxd.view(BL, K * Cp)
+        dxc = ref["dxc"] + (d2 @ d(xw)).view(B, Lseq, D)
+        edxc = bnd["dxc"] + _mm_bound(d2, e2, d(xw), K * Cp).view(B, Lseq, D) + R64.U * dxc.abs()
+        dxw = (d2.t() @ d(xc0).view(BL, D)).view(K, Cp, D)
+        edxw = _mm_bound_positions(d2.t(), e2.t(), d(xc0).view(BL, D)).view(K, Cp, D)
+        order = lambda t: torch.cat([t[:, 2 * N:2 * N + R], t[:, 0:N], t[:, N:2 * N]], dim=1)
+        A64 = d(A)
+        want = [(dxc, edxc), (order(dxw), order(edxw)), (torch.stack(dW), torch.stack(edW)), (ref["ddtb"], bnd["ddtb"]),
+                (ref["dA"] * A64, bnd["dA"] * A64.abs() + 2 * R64.U * (ref["dA"] * A64).abs()), (ref["dDs"], bnd["dDs"])]
+        for name, g, (r, b) in zip(["dxc", "dx_proj_weight", "ddt_projs_weight", "ddt_projs_bias", "dA_logs", "dDs"], got, want):
+            _check(f"{tag} save={save}", name, g, r, b, worst)
+            # the weight gradients contract the scan's per-element bounds over all B·L positions, which leaves their propagated
+            # bound looser than 1e-3 of scale at the largest element: there the max-norm bar holds as well
+            err = float((g.double() - r).abs().max()) / float(r.abs().max())
+            assert err <= 1e-3, f"{tag} save={save} {name}: {err:.2e} of its scale"
+    _finish(f"ss2d autograd fp64 {tag} save={save}", worst, tight=False)
