@@ -1,5 +1,7 @@
-"""Dense-projection GEMMs of Sigma-tiny at `--images` per GPU: our wgmma TF32 kernel vs cuBLAS TF32 (torch.mm).
-Reports ms and effective GB/s over (A read once + C written once [+ residual read])."""
+"""Dense-projection GEMMs of Sigma-tiny at `--images` per GPU: our wgmma kernel vs cuBLAS (torch.mm), in the precision of
+`--precision` (tf32: one TF32 MMA per k-step, cuBLAS TF32; tf32x3: three TF32 MMAs per k-step, cuBLAS fp32).
+Reports ms, effective GB/s over (A read once + C written once [+ residual read]) and TFLOP/s over 2·M·N·K; for our tf32x3
+kernel also the TF32 tensor-core rate, 3 x 2·M·N·K (A_lo·W_hi + A_hi·W_lo + A_hi·W_hi)."""
 import argparse
 import os
 import sys
@@ -12,8 +14,9 @@ from sigma_b200 import fused  # noqa: E402
 ap = argparse.ArgumentParser()
 ap.add_argument("--images", type=int, default=16)
 ap.add_argument("--only", nargs="*", default=None)
+ap.add_argument("--precision", default="tf32", choices=["tf32", "tf32x3"])
 a = ap.parse_args()
-torch.backends.cuda.matmul.allow_tf32 = True
+torch.backends.cuda.matmul.allow_tf32 = a.precision == "tf32"
 S = 2 * a.images
 # name, M, N, K, residual
 SHAPES = [
@@ -23,6 +26,7 @@ SHAPES = [
     ("in_proj3", S * 300, 3072, 768, False), ("x_proj3", S * 300, 320, 1536, False), ("out_proj3", S * 300, 768, 1536, True),
     ("merge0", S * 4800, 192, 384, False), ("dec_x_proj", a.images * 19200, 64, 192, False),
 ]
+print(f"precision {fused.precision()}, {torch.cuda.get_device_name()}", flush=True)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 for name, M, N, K, res in SHAPES:
     if a.only and name not in a.only:
@@ -32,6 +36,7 @@ for name, M, N, K, res in SHAPES:
     R = torch.randn(M, N, device="cuda") if res else None
     out = torch.empty(M, N, device="cuda")
     byt = 4 * (M * K + M * N * (2 if res else 1) + N * K)
+    flop = 2 * M * N * K
     line = f"{name:11s} M={M:7d} N={N:5d} K={K:5d}: "
     for mode in ("wgmma", "cublas"):
         fused.USE_OWN_GEMM = mode == "wgmma"
@@ -45,5 +50,8 @@ for name, M, N, K, res in SHAPES:
             torch.cuda.synchronize()
             ts.append(e0.elapsed_time(e1))
         ms = sorted(ts[1:])[2]
-        line += f"{mode} {ms:7.3f} ms {byt / ms / 1e6:7.1f} GB/s   "
+        line += f"{mode} {ms:7.3f} ms {byt / ms / 1e6:7.1f} GB/s {flop / ms / 1e9:6.1f} TFLOP/s"
+        if mode == "wgmma" and a.precision == "tf32x3":
+            line += f" ({3 * flop / ms / 1e9:6.1f} tensor)"
+        line += "   "
     print(line, flush=True)
