@@ -95,6 +95,16 @@ int sigma_scan_bwd(const void *u, const void *delta, const float *A, const void 
                    int batch, int dim, int seqlen, int dstate, int ngroups, int dtype,
                    int delta_softplus, void *workspace, size_t workspace_bytes, void *stream);
 
+/* Deterministic build of sigma_scan_bwd (torch.use_deterministic_algorithms): the same outputs, bitwise reproducible for the
+ * same inputs, GPU model and L-segment plan.  dB / dC are kept per channel tile of a group and dA / dD / ddelta_bias per
+ * (batch, L-segment) in the workspace, then summed in a fixed order; no float atomics.  nsplit = 0 lets the library choose
+ * the L-segments, as sigma_scan_bwd does. */
+size_t sigma_scan_bwd_det_workspace_bytes(int batch, int dim, int seqlen, int dstate, int ngroups, int dtype);
+int sigma_scan_bwd_det(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
+                       const float *delta_bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC,
+                       float *dD, float *ddelta_bias, int batch, int dim, int seqlen, int dstate, int ngroups, int dtype,
+                       int delta_softplus, void *workspace, size_t workspace_bytes, int nsplit, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * a4+a5 (+a8/a9 cores). Fused multi-direction SS2D scan, channels-last.
  * Replaces, in one launch, CrossScan (vmamba.py:80-98) + the dt_proj einsum (vmamba.py:199) +
@@ -164,6 +174,20 @@ int sigma_ss2d_scan_bwd_saved(int kind, const float *xc, const float *xdbl, cons
                               float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                               size_t workspace_bytes, int nsplit, void *stream);
 
+/* Deterministic builds of the fused backward (state sweep / after sigma_ss2d_scan_fwd_save): the same outputs, bitwise
+ * reproducible for the same inputs, GPU model and L-segment plan.  Each direction's du goes to a slab summed over k into dxc,
+ * dB / dC are kept per warp channel tile and dA / dDs / ddtb per (image, L-segment), all in the workspace, then summed in a
+ * fixed order; no float atomics and no bulk reduce.  nsplit = 0 lets the library choose the L-segments. */
+size_t sigma_ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
+int sigma_ss2d_scan_bwd_det(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
+                            const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb,
+                            int batch, int H, int W, int D, int N, int R, int Cp, void *workspace, size_t workspace_bytes, int nsplit,
+                            void *stream);
+int sigma_ss2d_scan_bwd_saved_det(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                  const float *Ds, const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl,
+                                  float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                                  size_t workspace_bytes, int nsplit, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * Row-wise / stencil pieces of a5-a11 (channels-last, fp32; D % 4 == 0, 16-byte aligned rows).
  * ------------------------------------------------------------------------------------------ */
@@ -178,6 +202,17 @@ int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, voi
  * C/4 must be one of {8, 16, 24, 32, 48, 64, 96, 128, 192, 256, 384} (every Sigma width up to 1536); else SIGMA_EUNSUPPORTED. */
 int sigma_layernorm_bwd(const float *x, const float *dy, const float *w, float *dx, float *dw, float *db, int64_t rows, int C,
                         float eps, void *stream);
+/* Deterministic build: dw / db kept per warp in the (16-byte aligned) workspace and summed in warp order; no float atomics. */
+size_t sigma_layernorm_bwd_det_workspace_bytes(int64_t rows, int C);
+int sigma_layernorm_bwd_det(const float *x, const float *dy, const float *w, float *dx, float *dw, float *db, int64_t rows, int C,
+                            float eps, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Backward of F.interpolate(mode="bilinear", align_corners=False), fp32, gather form (deterministic: every input element sums
+ * the output elements that tap it in a fixed order).  dy (batch, C, Hout, Wout) -> dx (batch, C, Hin, Win), NCHW, or with
+ * channels_last = 1 (batch, Hout, Wout, C) -> (batch, Hin, Win, C).  ratio_h / ratio_w are torch's source-index scales rounded
+ * to fp32: 1/scale_factor when the forward was given one, Hin/Hout (Win/Wout) when it was given a size. */
+int sigma_upsample_bilinear_bwd(const float *dy, float *dx, int batch, int C, int Hin, int Win, int Hout, int Wout, float ratio_h,
+                                float ratio_w, int channels_last, void *stream);
 
 /* PatchMerging2D front half (vmamba.py:619-633): y[b,i,j,:] = LayerNorm(cat(x[b,2i,2j], x[b,2i+1,2j], x[b,2i,2j+1],
  * x[b,2i+1,2j+1])) over 4C channels, zero rows beyond an odd H / W (F.pad).  x (batch,H,W,C) -> y (batch,⌈H/2⌉,⌈W/2⌉,4C);

@@ -69,6 +69,14 @@ SIGNATURES = {
                                                c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_float, c_void_p]),
     "sigma_dwconv3x3_silu_fwd_bf16": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64] + [c_int] * 4 + [c_void_p]),
     "sigma_ss2d_scan_fwd_bf16": (c_int, [c_int] + [c_void_p] * 7 + [c_int] * 7 + [c_void_p, c_size_t, c_void_p]),
+    "sigma_scan_bwd_det_workspace_bytes": (c_size_t, [c_int] * 6),
+    "sigma_scan_bwd_det": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
+    "sigma_ss2d_scan_bwd_det_workspace_bytes": (c_size_t, [c_int] * 6),
+    "sigma_ss2d_scan_bwd_det": (c_int, [c_int] + [c_void_p] * 14 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
+    "sigma_ss2d_scan_bwd_saved_det": (c_int, [c_int] + [c_void_p] * 15 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
+    "sigma_layernorm_bwd_det_workspace_bytes": (c_size_t, [c_int64, c_int]),
+    "sigma_layernorm_bwd_det": (c_int, [c_void_p] * 6 + [c_int64, c_int, c_float, c_void_p, c_size_t, c_void_p]),
+    "sigma_upsample_bilinear_bwd": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_float, c_float, c_int, c_void_p]),
 }
 
 _lib = None

@@ -46,12 +46,15 @@ template <typename T>
 int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
                     const float *bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC, float *dD,
                     float *dbias, int batch, int dim, int L, int N, int G, int softplus, void *ws, size_t ws_bytes,
-                    int force_split, cudaStream_t stream);
+                    int force_split, cudaStream_t stream, void *det_ws);
 template <typename T>
 int scan_op_bwd_generic(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
                         const float *bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC,
                         float *dD, float *dbias, int batch, int dim, int L, int N, int G, int softplus, void *ws,
-                        size_t ws_bytes, cudaStream_t stream);
+                        size_t ws_bytes, cudaStream_t stream, void *det_ws);
+// scratch of the deterministic backward builds (det_ws != nullptr above)
+size_t scan_op_bwd_tma_det_bytes(int batch, int dim, int L, int N, int G);
+size_t scan_op_bwd_det_bytes(int batch, int dim, int L, int N, int G);
 
 // SIGMA_OP_GENERIC=1 forces the generic kernels (A/B timing, tests of the fallback on TMA-eligible shapes)
 static bool force_generic() {
@@ -162,12 +165,12 @@ template <typename T>
 static int scan_bwd_dispatch(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
                              const float *bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC,
                              float *dD, float *dbias, int batch, int dim, int L, int N, int G, int softplus, void *ws,
-                             size_t ws_bytes, int force_split, cudaStream_t stream) {
+                             size_t ws_bytes, int force_split, cudaStream_t stream, void *det_ws) {
   const sigma_scan_strides st = contiguous_strides(dim, L, N, G);
   const bool al = (((uintptr_t)dout | (uintptr_t)du | (uintptr_t)ddelta | (uintptr_t)dB | (uintptr_t)dC) & 15) == 0;
   if (!force_generic() && al && scan_op_tma_eligible<T>(u, delta, B, C, du, dim, L, N, G, st))
     return scan_op_bwd_tma<T>(u, delta, A, B, C, D, bias, dout, du, ddelta, dA, dB, dC, dD, dbias, batch, dim, L, N, G, softplus,
-                              ws, ws_bytes, force_split, stream);
+                              ws, ws_bytes, force_split, stream, det_ws);
   if constexpr (sizeof(T) == 2) {
     const size_t core = align256(scan_op_bwd_tma_workspace_bytes(batch, dim, L, N, 4));
     if (!force_generic() && widen_shape_ok(dim, L, N, G, 2) && ws_bytes >= core + widen_bwd_bytes(batch, dim, L, N, G)) {
@@ -182,13 +185,13 @@ static int scan_bwd_dispatch(const void *u, const void *delta, const float *A, c
       if ((rc = widen<T>(B, B32, batch, G, N, L, st.B_batch, st.B_group, st.B_dstate, stream))) return rc;
       if ((rc = widen<T>(C, C32, batch, G, N, L, st.C_batch, st.C_group, st.C_dstate, stream))) return rc;
       if ((rc = scan_op_bwd_tma<float>(u32, d32, A, B32, C32, D, bias, g32, du32, dd32, dA, dB, dC, dD, dbias, batch, dim, L, N, G, softplus, ws,
-                                       core, force_split, stream))) return rc;
+                                       core, force_split, stream, det_ws))) return rc;
       if ((rc = narrow_to<T>(du32, du, batch, dim, L, st.u_batch, st.u_dim, stream))) return rc;
       return narrow_to<T>(dd32, ddelta, batch, dim, L, st.u_batch, st.u_dim, stream);
     }
   }
   return scan_op_bwd_generic<T>(u, delta, A, B, C, D, bias, dout, du, ddelta, dA, dB, dC, dD, dbias, batch, dim, L, N, G,
-                                softplus, ws, ws_bytes, stream);
+                                softplus, ws, ws_bytes, stream, det_ws);
 }
 
 }  // namespace sigma
@@ -254,7 +257,10 @@ int sigma_scan_fwd_f32_split(const float *u, const float *delta, const float *A,
 namespace sigma {
 int row_norm_launch(const RowNormParams &p, cudaStream_t stream);
 int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                         int D, float eps, cudaStream_t stream);
+                         int D, float eps, cudaStream_t stream, float *part = nullptr);
+size_t layernorm_bwd_det_workspace_bytes(long long rows, int D);
+int upsample_bilinear_bwd_launch(const float *dy, float *dx, int batch, int C, int Hin, int Win, int Hout, int Wout, float rh, float rw,
+                                 int channels_last, cudaStream_t stream);
 int argmax_hist_launch(const float *logits, const void *labels, int label_bytes, unsigned long long *hist,
                        unsigned long long *counts, unsigned char *pred_out, int batch, int ncls, long long HW, cudaStream_t stream);
 int dwconv3x3_silu_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
@@ -269,11 +275,12 @@ int ss2d_pick_segments_hook(long long ctas, int nw, int ntiles, int N);
 int gemm_pick_bn_hook(int N, long long m_tiles);
 int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out);
 size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
+size_t ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
 int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int force_split, long long *out4);
 int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                   const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
                   int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream,
-                  const float *hs_saved = nullptr);
+                  const float *hs_saved = nullptr, int det = 0);
 int upsample2x_norm_launch(const float *in, const float *gamma, const float *beta, const float *wcls, int ncls, float *out,
                            int B, int Hin, int Win, int C, float eps, cudaStream_t stream);
 int pool_avgmax_partial_launch(const float *x, float *partial, int B, long long L, int C, int nslice, cudaStream_t stream);
@@ -332,6 +339,30 @@ int sigma_layernorm_bwd(const float *x, const float *dy, const float *w, float *
   SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_bwd: C=%d must be a positive multiple of 4", C);
   SIGMA_CHECK_ARG(al16(x) && al16(dy) && al16(w) && al16(dx), "sigma_layernorm_bwd: pointers must be 16-byte aligned");
   return layernorm_bwd_launch(x, dy, w, dx, dw, db, rows, C, eps, (cudaStream_t)stream);
+}
+
+size_t sigma_layernorm_bwd_det_workspace_bytes(int64_t rows, int C) {
+  if (rows < 0 || C <= 0 || C % 4) return 0;
+  return layernorm_bwd_det_workspace_bytes(rows, C);
+}
+
+int sigma_layernorm_bwd_det(const float *x, const float *dy, const float *w, float *dx, float *dw, float *db, int64_t rows, int C, float eps,
+                            void *workspace, size_t workspace_bytes, void *stream) {
+  SIGMA_CHECK_ARG(x && dy && w && dx && dw && db, "sigma_layernorm_bwd_det: null pointer");
+  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_bwd_det: C=%d must be a positive multiple of 4", C);
+  SIGMA_CHECK_ARG(al16(x) && al16(dy) && al16(w) && al16(dx), "sigma_layernorm_bwd_det: pointers must be 16-byte aligned");
+  const size_t need = layernorm_bwd_det_workspace_bytes(rows, C);
+  SIGMA_CHECK_ARG(workspace != nullptr && al16(workspace) && workspace_bytes >= need,
+                  "sigma_layernorm_bwd_det: needs %zu 16-byte aligned workspace bytes, got %zu", need, workspace_bytes);
+  return layernorm_bwd_launch(x, dy, w, dx, dw, db, rows, C, eps, (cudaStream_t)stream, (float *)workspace);
+}
+
+int sigma_upsample_bilinear_bwd(const float *dy, float *dx, int batch, int C, int Hin, int Win, int Hout, int Wout, float ratio_h,
+                                float ratio_w, int channels_last, void *stream) {
+  SIGMA_CHECK_ARG(dy && dx, "sigma_upsample_bilinear_bwd: null pointer");
+  SIGMA_CHECK_ARG(batch > 0 && C > 0 && Hin > 0 && Win > 0 && Hout > 0 && Wout > 0, "sigma_upsample_bilinear_bwd: bad sizes");
+  SIGMA_CHECK_ARG(ratio_h > 0.f && ratio_w > 0.f, "sigma_upsample_bilinear_bwd: ratios must be positive");
+  return upsample_bilinear_bwd_launch(dy, dx, batch, C, Hin, Win, Hout, Wout, ratio_h, ratio_w, channels_last, (cudaStream_t)stream);
 }
 
 int sigma_patch_merge_norm_fwd(const float *x, const float *w, const float *b, float *y, int batch, int H, int W, int C,
@@ -526,10 +557,15 @@ size_t sigma_ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, in
   return ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N);
 }
 
+size_t sigma_ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
+  if ((kind != SIGMA_DIRS_CROSS4 && kind != SIGMA_DIRS_SEQ2) || (N != 4 && N != 16) || D % 64) return 0;
+  return ss2d_scan_bwd_det_workspace_bytes(kind, batch, H, W, D, N);
+}
+
 static int ss2d_bwd_entry(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                           const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb,
                           int batch, int H, int W, int D, int N, int R, int Cp, void *ws, size_t wsb, int nsplit, void *stream,
-                          const float *hs_saved = nullptr) {
+                          const float *hs_saved = nullptr, int det = 0) {
   SIGMA_CHECK_ARG(xc && xdbl && dtw && dtb && A && Ds && dy && delta && dxc && ddelta && dxdbl && dA && dDs && ddtb, "sigma_ss2d_scan_bwd: null pointer");
   SIGMA_CHECK_ARG(kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2, "sigma_ss2d_scan_bwd: kind %d unsupported (CROSS4, SEQ2)", kind);
   SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % 64 == 0 && R > 0, "sigma_ss2d_scan_bwd: bad sizes (D=%d must be a multiple of 64)", D);
@@ -538,7 +574,7 @@ static int ss2d_bwd_entry(int kind, const float *xc, const float *xdbl, const fl
   SIGMA_CHECK_ARG(al16(xc) && al16(xdbl) && al16(dy) && al16(delta) && al16(dxc) && al16(ddelta) && al16(dxdbl), "sigma_ss2d_scan_bwd: pointers must be 16-byte aligned");
   SIGMA_CHECK_ARG(hs_saved == nullptr || al16(hs_saved), "sigma_ss2d_scan_bwd_saved: hs must be 16-byte aligned");
   return ss2d_scan_bwd(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, ws, wsb, nsplit,
-                       (cudaStream_t)stream, hs_saved);
+                       (cudaStream_t)stream, hs_saved, det);
 }
 
 // backward after sigma_ss2d_scan_fwd_save: `delta` and `hs` are INPUTS (what that call wrote); no state sweep runs
@@ -565,6 +601,26 @@ int sigma_ss2d_scan_bwd_split(int kind, const float *xc, const float *xdbl, cons
                               void *stream) {
   return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace,
                         workspace_bytes, nsplit, stream);
+}
+
+// deterministic builds of sigma_ss2d_scan_bwd_split / sigma_ss2d_scan_bwd_saved (nsplit = 0: the library's choice)
+int sigma_ss2d_scan_bwd_det(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
+                            const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb,
+                            int batch, int H, int W, int D, int N, int R, int Cp, void *workspace, size_t workspace_bytes, int nsplit,
+                            void *stream) {
+  SIGMA_CHECK_ARG(nsplit >= 0, "sigma_ss2d_scan_bwd_det: nsplit=%d < 0", nsplit);
+  return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace,
+                        workspace_bytes, nsplit, stream, nullptr, 1);
+}
+
+int sigma_ss2d_scan_bwd_saved_det(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                  const float *Ds, const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl,
+                                  float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                                  size_t workspace_bytes, int nsplit, void *stream) {
+  SIGMA_CHECK_ARG(hs != nullptr, "sigma_ss2d_scan_bwd_saved_det: null hs");
+  SIGMA_CHECK_ARG(nsplit >= 0, "sigma_ss2d_scan_bwd_saved_det: nsplit=%d < 0", nsplit);
+  return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, const_cast<float *>(delta), dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R,
+                        Cp, workspace, workspace_bytes, nsplit, stream, hs, 1);
 }
 
 int sigma_upsample2x_norm_fwd(const float *x, const float *w, const float *b, float *y, int batch, int H, int W, int C,
@@ -616,10 +672,18 @@ size_t sigma_scan_bwd_workspace_bytes(int batch, int dim, int seqlen, int dstate
   return w;
 }
 
+// the deterministic build appends the partials of whichever kernel runs (TMA-staged or generic) to the workspace
+size_t sigma_scan_bwd_det_workspace_bytes(int batch, int dim, int seqlen, int dstate, int ngroups, int dtype) {
+  if (batch <= 0 || dim <= 0 || seqlen <= 0 || dstate <= 0 || dstate > 16 || ngroups <= 0 || dim % ngroups) return 0;
+  return align256(sigma_scan_bwd_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype)) +
+         std::max(scan_op_bwd_tma_det_bytes(batch, dim, seqlen, dstate, ngroups), scan_op_bwd_det_bytes(batch, dim, seqlen, dstate, ngroups));
+}
+
 static int scan_bwd_entry(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
                           const float *delta_bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC,
                           float *dD, float *ddelta_bias, int batch, int dim, int seqlen, int dstate, int ngroups, int dtype,
-                          int delta_softplus, void *workspace, size_t workspace_bytes, int force_split, cudaStream_t stream) {
+                          int delta_softplus, void *workspace, size_t workspace_bytes, int force_split, cudaStream_t stream,
+                          int det = 0) {
   SIGMA_CHECK_ARG(u && delta && A && B && C && dout && du && ddelta && dA && dB && dC, "sigma_scan_bwd: null pointer argument");
   SIGMA_CHECK_ARG((D == nullptr || dD != nullptr) && (delta_bias == nullptr || ddelta_bias != nullptr),
                   "sigma_scan_bwd: dD / ddelta_bias required when D / delta_bias are given");
@@ -627,20 +691,27 @@ static int scan_bwd_entry(const void *u, const void *delta, const float *A, cons
                   "sigma_scan_bwd: bad sizes (batch=%d dim=%d seqlen=%d dstate=%d ngroups=%d)", batch, dim, seqlen, dstate, ngroups);
   SIGMA_CHECK_ARG(dtype == SIGMA_F32 || dtype == SIGMA_F16 || dtype == SIGMA_BF16, "sigma_scan_bwd: unknown dtype %d", dtype);
   if (dstate > 16) { set_error("sigma_scan_bwd: d_state=%d > 16 is not supported by the backward kernels", dstate); return SIGMA_EUNSUPPORTED; }
-  const size_t need = sigma_scan_bwd_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype);
+  const size_t need = det ? sigma_scan_bwd_det_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype)
+                          : sigma_scan_bwd_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype);
   if (workspace == nullptr || workspace_bytes < need) {
     set_error("sigma_scan_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
     return SIGMA_EWORKSPACE;
   }
+  void *det_ws = nullptr;
+  if (det) {   // the kernels see only the plain workspace; the partials follow it
+    const size_t base = align256(sigma_scan_bwd_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype));
+    det_ws = (char *)workspace + base;
+    workspace_bytes = base;
+  }
   if (dtype == SIGMA_F32)
     return scan_bwd_dispatch<float>(u, delta, A, B, C, D, delta_bias, dout, du, ddelta, dA, dB, dC, dD, ddelta_bias, batch, dim,
-                                    seqlen, dstate, ngroups, delta_softplus, workspace, workspace_bytes, force_split, stream);
+                                    seqlen, dstate, ngroups, delta_softplus, workspace, workspace_bytes, force_split, stream, det_ws);
   if (dtype == SIGMA_F16)
     return scan_bwd_dispatch<__half>(u, delta, A, B, C, D, delta_bias, dout, du, ddelta, dA, dB, dC, dD, ddelta_bias, batch, dim,
-                                     seqlen, dstate, ngroups, delta_softplus, workspace, workspace_bytes, force_split, stream);
+                                     seqlen, dstate, ngroups, delta_softplus, workspace, workspace_bytes, force_split, stream, det_ws);
   return scan_bwd_dispatch<__nv_bfloat16>(u, delta, A, B, C, D, delta_bias, dout, du, ddelta, dA, dB, dC, dD, ddelta_bias, batch,
                                           dim, seqlen, dstate, ngroups, delta_softplus, workspace, workspace_bytes, force_split,
-                                          stream);
+                                          stream, det_ws);
 }
 
 int sigma_scan_bwd(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
@@ -658,6 +729,15 @@ int sigma_scan_bwd_split(const void *u, const void *delta, const float *A, const
                          int delta_softplus, void *workspace, size_t workspace_bytes, int nsplit, void *stream_) {
   return scan_bwd_entry(u, delta, A, B, C, D, delta_bias, dout, du, ddelta, dA, dB, dC, dD, ddelta_bias, batch, dim, seqlen,
                         dstate, ngroups, dtype, delta_softplus, workspace, workspace_bytes, nsplit, (cudaStream_t)stream_);
+}
+
+int sigma_scan_bwd_det(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
+                       const float *delta_bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC,
+                       float *dD, float *ddelta_bias, int batch, int dim, int seqlen, int dstate, int ngroups, int dtype,
+                       int delta_softplus, void *workspace, size_t workspace_bytes, int nsplit, void *stream_) {
+  SIGMA_CHECK_ARG(nsplit >= 0, "sigma_scan_bwd_det: nsplit=%d < 0", nsplit);
+  return scan_bwd_entry(u, delta, A, B, C, D, delta_bias, dout, du, ddelta, dA, dB, dC, dD, ddelta_bias, batch, dim, seqlen,
+                        dstate, ngroups, dtype, delta_softplus, workspace, workspace_bytes, nsplit, (cudaStream_t)stream_, 1);
 }
 
 int sigma_linear_tf32(const float *A, int64_t lda, const float *W, const float *bias, const float *residual, int64_t ldr,

@@ -248,11 +248,12 @@ int row_norm_launch(const RowNormParams &p, cudaStream_t stream) {
 // recomputed from x (x is read anyway), so the forward saves nothing.  A warp walks rows with a grid stride and keeps its lanes'
 // dgamma / dbeta columns in registers; they are reduced over the warp's sub-rows by shuffles and leave the warp as one
 // atomicAdd per column (torch's GammaBetaBackwardCUDAKernel spent 5.9 ms per Sigma-tiny training step on this reduction).
-template <int LPR, int V>
-__global__ void __launch_bounds__(256) layernorm_bwd_kernel(const float *__restrict__ x, const float *__restrict__ dy,
-                                                             const float *__restrict__ gamma, float *__restrict__ dx,
-                                                             float *__restrict__ dgamma, float *__restrict__ dbeta, long long rows,
-                                                             int D, float eps) {
+// DET: instead of the atomics, warp w of the grid writes its column sums to part[w·D ...] (dgamma) and
+// part[(nwarps + w)·D ...] (dbeta); sum_parts_det_kernel adds them in warp order.
+template <int LPR, int V, bool DET>
+__device__ __forceinline__ void layernorm_bwd_body(const float *__restrict__ x, const float *__restrict__ dy, const float *__restrict__ gamma,
+                                                   float *__restrict__ dx, float *__restrict__ dgamma, float *__restrict__ dbeta,
+                                                   long long rows, int D, float eps, float *__restrict__ part) {
   constexpr int RPW = 32 / LPR;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane / LPR, l = lane % LPR;
   const long long wstride = (long long)gridDim.x * (blockDim.x >> 5);
@@ -333,7 +334,17 @@ __global__ void __launch_bounds__(256) layernorm_bwd_kernel(const float *__restr
       db[v].z += __shfl_xor_sync(0xffffffffu, db[v].z, o); db[v].w += __shfl_xor_sync(0xffffffffu, db[v].w, o);
     }
   }
-  if (sub == 0) {                     // one red.global.add per column and warp (<= ~1M per call: the grid is sized for it)
+  if (DET) {
+    if (sub == 0) {
+      const long long gw = (long long)blockIdx.x * (blockDim.x >> 5) + warp, nw = (long long)gridDim.x * (blockDim.x >> 5);
+#pragma unroll
+      for (int v = 0; v < V; ++v) {
+        const int c = 4 * (l + LPR * v);
+        *reinterpret_cast<float4 *>(part + gw * D + c) = dg[v];
+        *reinterpret_cast<float4 *>(part + (nw + gw) * D + c) = db[v];
+      }
+    }
+  } else if (sub == 0) {              // one red.global.add per column and warp (<= ~1M per call: the grid is sized for it)
 #pragma unroll
     for (int v = 0; v < V; ++v) {
       const int c = 4 * (l + LPR * v);
@@ -344,30 +355,75 @@ __global__ void __launch_bounds__(256) layernorm_bwd_kernel(const float *__restr
 }
 
 template <int LPR, int V>
-static void layernorm_bwd_k(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                            int D, float eps, cudaStream_t stream) {
-  const int warps = 8, rpw = 32 / LPR;
-  const long long nsteps = (rows + rpw - 1) / rpw;
-  // enough CTAs to fill the machine, few enough that the 2·D atomics per warp stay negligible (a warp walks >= 4 steps)
-  const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>(kNumSMs * 8, (nsteps + warps * 4 - 1) / (warps * 4)));
-  layernorm_bwd_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps);
+__global__ void __launch_bounds__(256) layernorm_bwd_kernel(const float *__restrict__ x, const float *__restrict__ dy,
+                                                             const float *__restrict__ gamma, float *__restrict__ dx,
+                                                             float *__restrict__ dgamma, float *__restrict__ dbeta, long long rows,
+                                                             int D, float eps) {
+  layernorm_bwd_body<LPR, V, false>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, nullptr);
 }
 
-// dgamma / dbeta are zeroed here and accumulated into; false if D has no instantiation (the fast forward's D set)
+template <int LPR, int V>
+__global__ void __launch_bounds__(256) layernorm_bwd_det_kernel(const float *__restrict__ x, const float *__restrict__ dy,
+                                                                 const float *__restrict__ gamma, float *__restrict__ dx, long long rows,
+                                                                 int D, float eps, float *__restrict__ part) {
+  layernorm_bwd_body<LPR, V, true>(x, dy, gamma, dx, nullptr, nullptr, rows, D, eps, part);
+}
+
+// enough CTAs to fill the machine, few enough that the 2·D atomics per warp stay negligible (a warp walks >= 4 steps);
+// lanes per row as in the instantiation table of layernorm_bwd_launch
+static unsigned layernorm_bwd_grid(long long rows, int D) {
+  const int warps = 8, nvec = D >> 2, lpr = nvec % 32 == 0 && nvec >= 96 ? 32 : nvec % 16 == 0 && nvec >= 48 ? 16 : 8;
+  const long long nsteps = (rows + 32 / lpr - 1) / (32 / lpr);
+  return (unsigned)std::max<long long>(1, std::min<long long>(kNumSMs * 8, (nsteps + warps * 4 - 1) / (warps * 4)));
+}
+
+template <int LPR, int V>
+static void layernorm_bwd_k(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
+                            int D, float eps, float *part, cudaStream_t stream) {
+  const int warps = 8;
+  const unsigned grid = layernorm_bwd_grid(rows, D);
+  if (part) layernorm_bwd_det_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>(x, dy, gamma, dx, rows, D, eps, part);
+  else layernorm_bwd_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps);
+}
+
+// deterministic build: one dgamma and one dbeta row of D floats per warp of the grid
+size_t layernorm_bwd_det_workspace_bytes(long long rows, int D) {
+  return (size_t)2 * layernorm_bwd_grid(rows, D) * 8 * D * sizeof(float);
+}
+
+int sum_parts_det_launch(const float *part, int nparts, long long ncols, long long inner, long long ostride, float *out, cudaStream_t stream);
+
+// dgamma / dbeta are zeroed here and accumulated into; false if D has no instantiation (the fast forward's D set).
+// part != nullptr: the deterministic build (layernorm_bwd_det_workspace_bytes of scratch), dgamma / dbeta written by the
+// fixed-order sum over the grid's warps
 int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                         int D, float eps, cudaStream_t stream) {
-  if (rows == 0) return SIGMA_OK;
+                         int D, float eps, cudaStream_t stream, float *part) {
   if (D & 3) { set_error("layernorm_bwd: D=%d must be a multiple of 4", D); return SIGMA_EUNSUPPORTED; }
-  SIGMA_CHECK_CUDA(cudaMemsetAsync(dgamma, 0, (size_t)D * sizeof(float), stream));
-  SIGMA_CHECK_CUDA(cudaMemsetAsync(dbeta, 0, (size_t)D * sizeof(float), stream));
+  if (rows == 0 && !part) return SIGMA_OK;
+  if (rows == 0) {
+    SIGMA_CHECK_CUDA(cudaMemsetAsync(dgamma, 0, (size_t)D * sizeof(float), stream));
+    SIGMA_CHECK_CUDA(cudaMemsetAsync(dbeta, 0, (size_t)D * sizeof(float), stream));
+    return SIGMA_OK;
+  }
+  if (!part) {
+    SIGMA_CHECK_CUDA(cudaMemsetAsync(dgamma, 0, (size_t)D * sizeof(float), stream));
+    SIGMA_CHECK_CUDA(cudaMemsetAsync(dbeta, 0, (size_t)D * sizeof(float), stream));
+  }
   const int nvec = D >> 2;
-#define TRY(LPR, V) if (nvec == (LPR) * (V)) { layernorm_bwd_k<LPR, V>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, stream); SIGMA_CHECK_LAUNCH(); return SIGMA_OK; }
+  bool ok = false;
+#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) { layernorm_bwd_k<LPR, V>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, part, stream); SIGMA_CHECK_LAUNCH(); ok = true; }
   TRY(8, 1) TRY(8, 2) TRY(8, 3) TRY(8, 4)
   TRY(16, 3) TRY(16, 4)
   TRY(32, 3) TRY(32, 4) TRY(32, 6) TRY(32, 8) TRY(32, 12)
 #undef TRY
-  set_error("layernorm_bwd: D=%d has no instantiation (D/4 = lanes-per-row x vectors in {8x1..4, 16x3..4, 32x3,4,6,8,12})", D);
-  return SIGMA_EUNSUPPORTED;
+  if (!ok) {
+    set_error("layernorm_bwd: D=%d has no instantiation (D/4 = lanes-per-row x vectors in {8x1..4, 16x3..4, 32x3,4,6,8,12})", D);
+    return SIGMA_EUNSUPPORTED;
+  }
+  if (!part) return SIGMA_OK;
+  const int nw = (int)layernorm_bwd_grid(rows, D) * 8;
+  const int rc = sum_parts_det_launch(part, nw, D, D, 0, dgamma, stream);
+  return rc ? rc : sum_parts_det_launch(part + (size_t)nw * D, nw, D, D, 0, dbeta, stream);
 }
 
 // ---- depthwise 3x3 + bias + SiLU, NHWC ----

@@ -38,6 +38,9 @@ struct ScanBwdParams {
   void *du, *ddelta;                      // element type T
   float *dA, *dB, *dC, *dD, *dbias;
   int batch, dim, L, N, G, dpg, tiles_per_group, ntiles, softplus;
+  // deterministic build (scan_op_bwd_det_kernel): dB / dC partials per CTA channel tile of a group (tiles_per_group, batch,
+  // G, N, L); dA (batch, dim, N), dD and ddelta_bias (batch, dim) per batch
+  float *part_B, *part_C, *part_dA, *part_dD, *part_db;
 };
 
 template <int SPT, int LPC>
@@ -47,8 +50,10 @@ __host__ __device__ constexpr int bwd_smem_floats() {
   return (3 * BW_DT + 2 * SPT * LPC) * BW_LTP + (2 * BW_DT + 2 * SPT * LPC) * BW_LTP + BW_LT * 32 * LPC * SPT;
 }
 
-template <typename T, int SPT, int LPC>
-__global__ void __launch_bounds__(32 * LPC) scan_op_bwd_kernel(const ScanBwdParams p) {
+// DET: the warps' dB / dC rows go to per-warp shared-memory slots summed in warp order (after the h rows), the CTA's sums
+// and the per-thread dA / dD / ddelta_bias to the partials of the deterministic build (see ScanBwdParams)
+template <typename T, int SPT, int LPC, bool DET>
+__device__ __forceinline__ void scan_op_bwd_body(const ScanBwdParams &p) {
   const T *pu = (const T *)p.u, *pdl = (const T *)p.delta, *pdo = (const T *)p.dout, *pB = (const T *)p.B, *pC = (const T *)p.C;
   constexpr int NP = SPT * LPC, CPW = 32 / LPC, NTH = 32 * LPC;
   extern __shared__ __align__(16) float smem[];
@@ -57,6 +62,7 @@ __global__ void __launch_bounds__(32 * LPC) scan_op_bwd_kernel(const ScanBwdPara
   float *sDu = sC + NP * BW_LTP, *sDd = sDu + BW_DT * BW_LTP;
   float *sDB = sDd + BW_DT * BW_LTP, *sDC = sDB + NP * BW_LTP;
   float *sH = sDC + NP * BW_LTP;  // [position][thread][SPT]
+  float *sBCw = sH + BW_LT * NTH * SPT;   // DET: [warp][dB rows | dC rows]
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int q = lane % LPC, c_local = warp * CPW + lane / LPC;
@@ -157,8 +163,13 @@ __global__ void __launch_bounds__(32 * LPC) scan_op_bwd_kernel(const ScanBwdPara
       if (lane < LPC) {
 #pragma unroll
         for (int s = 0; s < SPT; ++s) {
-          atomicAdd(&sDB[(q * SPT + s) * BW_LTP + i], cB[s]);
-          atomicAdd(&sDC[(q * SPT + s) * BW_LTP + i], cC[s]);
+          if (DET) {
+            sBCw[(warp * 2 * NP + q * SPT + s) * BW_LTP + i] = cB[s];
+            sBCw[(warp * 2 * NP + NP + q * SPT + s) * BW_LTP + i] = cC[s];
+          } else {
+            atomicAdd(&sDB[(q * SPT + s) * BW_LTP + i], cB[s]);
+            atomicAdd(&sDC[(q * SPT + s) * BW_LTP + i], cC[s]);
+          }
         }
       }
       ddl = channel_reduce<LPC>(ddl);
@@ -185,12 +196,32 @@ __global__ void __launch_bounds__(32 * LPC) scan_op_bwd_kernel(const ScanBwdPara
     }
     for (int i = tid; i < 2 * NP * BW_LT; i += NTH) {
       const int which = i / (NP * BW_LT), n = (i >> 5) % NP, e = i & 31;
-      if (n < p.N && e < npos)
-        atomicAdd((which ? p.dC : p.dB) + bc0 + (long long)n * p.L + l0 + e, (which ? sDC : sDB)[n * BW_LTP + e]);
+      if (n < p.N && e < npos) {
+        if (DET) {
+          float v = 0.f;
+#pragma unroll
+          for (int wp = 0; wp < NTH / 32; ++wp) v += sBCw[(wp * 2 * NP + which * NP + n) * BW_LTP + e];
+          const long long po = (long long)tg * p.batch * p.G * p.N * p.L + bc0 + (long long)n * p.L + l0 + e;
+          (which ? p.part_C : p.part_B)[po] = v;
+        } else {
+          atomicAdd((which ? p.dC : p.dB) + bc0 + (long long)n * p.L + l0 + e, (which ? sDC : sDB)[n * BW_LTP + e]);
+        }
+      }
     }
     __syncthreads();
   }
-  if (ch_ok) {
+  if (DET && ch_ok) {
+    const long long bd = (long long)b * p.dim + d;
+#pragma unroll
+    for (int s = 0; s < SPT; ++s) {
+      const int n = q * SPT + s;
+      if (n < p.N) p.part_dA[bd * p.N + n] = dAacc[s];
+    }
+    if (q == 0) {
+      if (p.dD) p.part_dD[bd] = dDacc;
+      if (p.dbias) p.part_db[bd] = dbacc;
+    }
+  } else if (ch_ok) {
 #pragma unroll
     for (int s = 0; s < SPT; ++s) {
       const int n = q * SPT + s;
@@ -203,6 +234,12 @@ __global__ void __launch_bounds__(32 * LPC) scan_op_bwd_kernel(const ScanBwdPara
   }
 }
 
+template <typename T, int SPT, int LPC>
+__global__ void __launch_bounds__(32 * LPC) scan_op_bwd_kernel(const ScanBwdParams p) { scan_op_bwd_body<T, SPT, LPC, false>(p); }
+
+template <typename T, int SPT, int LPC>
+__global__ void __launch_bounds__(32 * LPC) scan_op_bwd_det_kernel(const ScanBwdParams p) { scan_op_bwd_body<T, SPT, LPC, true>(p); }
+
 int scan_op_npad(int N);
 template <typename T>
 int scan_op_fwd_generic(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
@@ -210,15 +247,37 @@ int scan_op_fwd_generic(const void *u, const void *delta, const float *A, const 
                         int softplus, const sigma_scan_strides &s, void *ws, size_t ws_bytes, int force_split,
                         cudaStream_t stream);
 
+int sum_parts_det_launch(const float *part, int nparts, long long ncols, long long inner, long long ostride, float *out, cudaStream_t stream);
+
 template <typename T, int SPT, int LPC>
 static int launch_bwd(const ScanBwdParams &p, cudaStream_t stream) {
-  const size_t smem = (size_t)bwd_smem_floats<SPT, LPC>() * sizeof(float);
-  auto kern = scan_op_bwd_kernel<T, SPT, LPC>;
+  const bool det = p.part_B != nullptr;
+  const size_t smem = (size_t)(bwd_smem_floats<SPT, LPC>() + (det ? LPC * 2 * SPT * LPC * BW_LTP : 0)) * sizeof(float);
+  auto kern = det ? scan_op_bwd_det_kernel<T, SPT, LPC> : scan_op_bwd_kernel<T, SPT, LPC>;
   SIGMA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   dim3 grid(p.G * p.tiles_per_group, p.batch);
   kern<<<grid, 32 * LPC, smem, stream>>>(p);
   SIGMA_CHECK_LAUNCH();
+  if (!det) return SIGMA_OK;
+  // fixed-order sums: dB / dC over the channel tiles of a group, dA / dD / ddelta_bias over the batch
+  const long long bgnl = (long long)p.batch * p.G * p.N * p.L, dn = (long long)p.dim * p.N;
+  int rc;
+  if ((rc = sum_parts_det_launch(p.part_B, p.tiles_per_group, bgnl, bgnl, 0, p.dB, stream))) return rc;
+  if ((rc = sum_parts_det_launch(p.part_C, p.tiles_per_group, bgnl, bgnl, 0, p.dC, stream))) return rc;
+  if ((rc = sum_parts_det_launch(p.part_dA, p.batch, dn, dn, 0, p.dA, stream))) return rc;
+  if (p.dD && (rc = sum_parts_det_launch(p.part_dD, p.batch, p.dim, p.dim, 0, p.dD, stream))) return rc;
+  if (p.dbias && (rc = sum_parts_det_launch(p.part_db, p.batch, p.dim, p.dim, 0, p.dbias, stream))) return rc;
   return SIGMA_OK;
+}
+
+static size_t al256g(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// scratch of the deterministic build: [dB partials] [dC partials] (tiles_per_group, batch, G, N, L) [dA partials (batch, dim, N)]
+// [dD partials] [ddelta_bias partials] (batch, dim)
+size_t scan_op_bwd_det_bytes(int batch, int dim, int L, int N, int G) {
+  const size_t tpg = (size_t)(dim / G + BW_DT - 1) / BW_DT;
+  return 2 * al256g(tpg * batch * G * N * L * sizeof(float)) + al256g((size_t)batch * dim * N * sizeof(float)) +
+         2 * al256g((size_t)batch * dim * sizeof(float));
 }
 
 size_t scan_op_bwd_workspace_bytes(int batch, int dim, int L, int N, int elem_bytes) {
@@ -233,7 +292,7 @@ template <typename T>
 int scan_op_bwd_generic(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
                         const float *bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC,
                         float *dD, float *dbias, int batch, int dim, int L, int N, int G, int softplus, void *ws,
-                        size_t ws_bytes, cudaStream_t stream) {
+                        size_t ws_bytes, cudaStream_t stream, void *det_ws) {
   if (N > 16) { set_error("sigma_scan_bwd: d_state=%d > 16 is not supported by the backward kernels", N); return SIGMA_EUNSUPPORTED; }
   if (ws == nullptr || ws_bytes < scan_op_bwd_workspace_bytes(batch, dim, L, N, (int)sizeof(T))) {
     set_error("sigma_scan_bwd: workspace too small (%zu < %zu)", ws_bytes, scan_op_bwd_workspace_bytes(batch, dim, L, N, (int)sizeof(T)));
@@ -265,6 +324,14 @@ int scan_op_bwd_generic(const void *u, const void *delta, const float *A, const 
   p.batch = batch; p.dim = dim; p.L = L; p.N = N; p.G = G; p.dpg = dim / G;
   p.tiles_per_group = (p.dpg + BW_DT - 1) / BW_DT;
   p.ntiles = ntiles; p.softplus = softplus;
+  p.part_B = p.part_C = p.part_dA = p.part_dD = p.part_db = nullptr;
+  if (det_ws) {   // layout of scan_op_bwd_det_bytes
+    const size_t bc = al256g((size_t)p.tiles_per_group * batch * G * N * L * sizeof(float));
+    const size_t da = al256g((size_t)batch * dim * N * sizeof(float)), dd = al256g((size_t)batch * dim * sizeof(float));
+    char *w = (char *)det_ws;
+    p.part_B = (float *)w; p.part_C = (float *)(w + bc); p.part_dA = (float *)(w + 2 * bc);
+    p.part_dD = (float *)(w + 2 * bc + da); p.part_db = (float *)(w + 2 * bc + da + dd);
+  }
   switch (NP) {
     case 4: return launch_bwd<T, 4, 1>(p, stream);
     case 8: return launch_bwd<T, 4, 2>(p, stream);
@@ -275,7 +342,7 @@ int scan_op_bwd_generic(const void *u, const void *delta, const float *A, const 
 #define SIGMA_INST(T)                                                                                                       \
   template int scan_op_bwd_generic<T>(const void *, const void *, const float *, const void *, const void *, const float *, \
                                       const float *, const void *, void *, void *, float *, float *, float *, float *,     \
-                                      float *, int, int, int, int, int, int, void *, size_t, cudaStream_t);
+                                      float *, int, int, int, int, int, int, void *, size_t, cudaStream_t, void *);
 SIGMA_INST(float)
 SIGMA_INST(__half)
 SIGMA_INST(__nv_bfloat16)

@@ -31,6 +31,9 @@ struct alignas(64) ScanBwdTmaParams {
   float *dA, *dB, *dC, *dD, *dbias, *carry;
   int batch, dim, L, N, G, dpg, ctiles_per_group, DT, softplus;
   int nsplit, tiles_per_split, ntiles, nst, nhs;
+  // deterministic build (scan_op_bwd_tma_det_kernel): dB / dC partials per warp channel tile of a group (dpg / CPW, batch, G,
+  // N, L); dA (batch·nsplit, dim, N), dD and ddelta_bias (batch·nsplit, dim) per (batch, L-segment)
+  float *part_B, *part_C, *part_dA, *part_dD, *part_db;
 };
 
 template <int NP> struct BwdCfg {
@@ -78,8 +81,9 @@ __device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float 
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
-template <typename T, int NP, int MODE>
-__global__ void __launch_bounds__(128, 2) scan_op_bwd_tma_kernel(const __grid_constant__ ScanBwdTmaParams p) {
+// DET: the sums across warps and CTAs go to the partials of the deterministic build (see ScanBwdTmaParams), not to atomics
+template <typename T, int NP, int MODE, bool DET>
+__device__ __forceinline__ void scan_op_bwd_tma_body(const ScanBwdTmaParams &p) {
   constexpr int LT = OpT<T>::LT, PITCH = 2 * NP + 4, G = 4, SUB = OPT_HS_POS, GPS = SUB / G;   // 4 groups per sub-tile
   constexpr int LPC = BwdCfg<NP>::LPC, NS = BwdCfg<NP>::NS, CPW = BwdCfg<NP>::CPW;
   constexpr float kLn2 = 0.6931471805599453f;
@@ -107,7 +111,18 @@ __global__ void __launch_bounds__(128, 2) scan_op_bwd_tma_kernel(const __grid_co
     fence_mbar_init();
   }
   __syncthreads();
-  if (t0 >= t1) return;
+  if (t0 >= t1) {
+    if (DET) {   // an empty segment's partials are zero
+      const long long seg = (long long)b * p.nsplit + split;
+#pragma unroll
+      for (int s = 0; s < NS; ++s) p.part_dA[(seg * p.dim + d) * p.N + n0 + s] = 0.f;
+      if (half == 0) {
+        if (p.dD) p.part_dD[seg * p.dim + d] = 0.f;
+        if (p.dbias) p.part_db[seg * p.dim + d] = 0.f;
+      }
+    }
+    return;
+  }
 
   // tiles are walked from t1-1 down to t0; k = t1-1-tau is the ring order
   auto request_tile = [&](int k, int st) {
@@ -269,8 +284,15 @@ __global__ void __launch_bounds__(128, 2) scan_op_bwd_tma_kernel(const __grid_co
       constexpr int DUP = CPW / NS;
       if ((cl & (DUP - 1)) == 0) {
         const long long off = (long long)(n0 + which) * p.L + (long long)tau * LT + (gbase + gi) * G;
-        red_add_v4(dBg + off, rB[0], rB[1], rB[2], rB[3]);
-        red_add_v4(dCg + off, rC[0], rC[1], rC[2], rC[3]);
+        if (DET) {
+          const long long tile = (long long)ct * nwarps + warp;
+          const long long po = (tile * p.batch * p.G + (long long)b * p.G + g) * p.N * (long long)p.L + off;
+          *reinterpret_cast<float4 *>(p.part_B + po) = make_float4(rB[0], rB[1], rB[2], rB[3]);
+          *reinterpret_cast<float4 *>(p.part_C + po) = make_float4(rC[0], rC[1], rC[2], rC[3]);
+        } else {
+          red_add_v4(dBg + off, rB[0], rB[1], rB[2], rB[3]);
+          red_add_v4(dCg + off, rC[0], rC[1], rC[2], rC[3]);
+        }
       }
     }
 #pragma unroll
@@ -296,12 +318,32 @@ __global__ void __launch_bounds__(128, 2) scan_op_bwd_tma_kernel(const __grid_co
   }
   if (lane == 0) tma_store_wait_all<0>();
 
+  if (DET) {
+    const long long seg = (long long)b * p.nsplit + split;
+#pragma unroll
+    for (int s = 0; s < NS; ++s) p.part_dA[(seg * p.dim + d) * p.N + n0 + s] = dAacc[s];
+    if (half == 0) {
+      if (p.dD) p.part_dD[seg * p.dim + d] = dDacc;
+      if (p.dbias) p.part_db[seg * p.dim + d] = dbacc;
+    }
+    return;
+  }
 #pragma unroll
   for (int s = 0; s < NS; ++s) atomicAdd(&p.dA[(long long)d * p.N + n0 + s], dAacc[s]);   // over batch and segments (:262-273)
   if (half == 0) {
     if (p.dD) atomicAdd(&p.dD[d], dDacc);
     if (p.dbias) atomicAdd(&p.dbias[d], dbacc);
   }
+}
+
+template <typename T, int NP, int MODE>
+__global__ void __launch_bounds__(128, 2) scan_op_bwd_tma_kernel(const __grid_constant__ ScanBwdTmaParams p) {
+  scan_op_bwd_tma_body<T, NP, MODE, false>(p);
+}
+
+template <typename T, int NP, int MODE>
+__global__ void __launch_bounds__(128, 2) scan_op_bwd_tma_det_kernel(const __grid_constant__ ScanBwdTmaParams p) {
+  scan_op_bwd_tma_body<T, NP, MODE, true>(p);
 }
 
 // Reverse summary of one L-segment: P[n] = prod a over the segment, g[n] = value the reverse recurrence
@@ -431,6 +473,15 @@ size_t scan_op_tma_workspace_bytes(int batch, int dim, int dstate);
 
 static size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
 
+int sum_parts_det_launch(const float *part, int nparts, long long ncols, long long inner, long long ostride, float *out, cudaStream_t stream);
+
+// scratch of the deterministic build: [dB partials] [dC partials] (dpg / CPW, batch, G, N, L) [dA partials (batch·64, dim, N)]
+// [dD partials] [ddelta_bias partials] (batch·64, dim)
+size_t scan_op_bwd_tma_det_bytes(int batch, int dim, int L, int N, int G) {
+  const size_t cpw = N >= 16 ? 16 : 32, ntile = (size_t)(dim / G) / cpw, segs = (size_t)batch * kBwdMaxSplit;
+  return 2 * al256(ntile * batch * G * N * L * sizeof(float)) + al256(segs * dim * N * sizeof(float)) + 2 * al256(segs * dim * sizeof(float));
+}
+
 // workspace = [hs (batch, dim, ntiles, N)] [forward-split carry] [reverse-split carry]
 size_t scan_op_bwd_tma_workspace_bytes(int batch, int dim, int L, int N, int elem_bytes) {
   (void)elem_bytes;
@@ -456,16 +507,22 @@ static int launch_bwd_tma(ScanBwdTmaParams &p, cudaStream_t stream) {
     SIGMA_CHECK_LAUNCH();
   }
   const size_t smem = bwd_tma_smem_bytes<T, NP>(p.DT, p.nst);
-  if (p.nsplit == 1) {
-    auto k = scan_op_bwd_tma_kernel<T, NP, MODE_SERIAL>;
-    SIGMA_CHECK_CUDA(prep((const void *)k, smem));
-    k<<<grid, p.DT * LPC, smem, stream>>>(p);
-  } else {
-    auto k = scan_op_bwd_tma_kernel<T, NP, MODE_APPLY>;
-    SIGMA_CHECK_CUDA(prep((const void *)k, smem));
-    k<<<grid, p.DT * LPC, smem, stream>>>(p);
-  }
+  const bool det = p.part_B != nullptr;
+  auto k = p.nsplit == 1 ? (det ? scan_op_bwd_tma_det_kernel<T, NP, MODE_SERIAL> : scan_op_bwd_tma_kernel<T, NP, MODE_SERIAL>)
+                         : (det ? scan_op_bwd_tma_det_kernel<T, NP, MODE_APPLY> : scan_op_bwd_tma_kernel<T, NP, MODE_APPLY>);
+  SIGMA_CHECK_CUDA(prep((const void *)k, smem));
+  k<<<grid, p.DT * LPC, smem, stream>>>(p);
   SIGMA_CHECK_LAUNCH();
+  if (!det) return SIGMA_OK;
+  // fixed-order sums: dB / dC over the warp channel tiles of a group, dA / dD / ddelta_bias over (batch, segment)
+  const int ntile = p.dpg / BwdCfg<NP>::CPW, segs = p.batch * p.nsplit;
+  const long long bgnl = (long long)p.batch * p.G * p.N * p.L, dn = (long long)p.dim * p.N;
+  int rc;
+  if ((rc = sum_parts_det_launch(p.part_B, ntile, bgnl, bgnl, 0, p.dB, stream))) return rc;
+  if ((rc = sum_parts_det_launch(p.part_C, ntile, bgnl, bgnl, 0, p.dC, stream))) return rc;
+  if ((rc = sum_parts_det_launch(p.part_dA, segs, dn, dn, 0, p.dA, stream))) return rc;
+  if (p.dD && (rc = sum_parts_det_launch(p.part_dD, segs, p.dim, p.dim, 0, p.dD, stream))) return rc;
+  if (p.dbias && (rc = sum_parts_det_launch(p.part_db, segs, p.dim, p.dim, 0, p.dbias, stream))) return rc;
   return SIGMA_OK;
 }
 
@@ -475,7 +532,7 @@ template <typename T>
 int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
                     const float *bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC, float *dD,
                     float *dbias, int batch, int dim, int L, int N, int G, int softplus, void *ws, size_t ws_bytes,
-                    int force_split, cudaStream_t stream) {
+                    int force_split, cudaStream_t stream, void *det_ws) {
   constexpr int LT = OpT<T>::LT;
   const int NP = N;
   if (ws == nullptr || ws_bytes < scan_op_bwd_tma_workspace_bytes(batch, dim, L, N, (int)sizeof(T))) {
@@ -512,6 +569,14 @@ int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void
   p.A = A; p.D = D; p.bias = bias; p.hs = hs;
   p.dA = dA; p.dB = dB; p.dC = dC; p.dD = dD; p.dbias = dbias; p.carry = rcarry;
   p.batch = batch; p.dim = dim; p.L = L; p.N = N; p.G = G; p.dpg = dim / G; p.softplus = softplus;
+  if (det_ws) {   // layout of scan_op_bwd_tma_det_bytes
+    const size_t cpw = N >= 16 ? 16 : 32, ntile = (size_t)p.dpg / cpw, segs = (size_t)batch * kBwdMaxSplit;
+    const size_t bc = al256(ntile * batch * G * N * L * sizeof(float)), da = al256(segs * dim * N * sizeof(float));
+    const size_t dd = al256(segs * dim * sizeof(float));
+    char *w = (char *)det_ws;
+    p.part_B = (float *)w; p.part_C = (float *)(w + bc); p.part_dA = (float *)(w + 2 * bc);
+    p.part_dD = (float *)(w + 2 * bc + da); p.part_db = (float *)(w + 2 * bc + da + dd);
+  }
   p.DT = (p.dpg % 64 == 0) ? 64 : 32;
   p.ctiles_per_group = p.dpg / p.DT;
   p.ntiles = ntiles;
@@ -564,7 +629,7 @@ int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void
 #define SIGMA_INST(T)                                                                                                         \
   template int scan_op_bwd_tma<T>(const void *, const void *, const float *, const void *, const void *, const float *,       \
                                   const float *, const void *, void *, void *, float *, float *, float *, float *, float *,   \
-                                  int, int, int, int, int, int, void *, size_t, int, cudaStream_t);
+                                  int, int, int, int, int, int, void *, size_t, int, cudaStream_t, void *);
 SIGMA_INST(float)
 SIGMA_INST(__half)
 SIGMA_INST(__nv_bfloat16)

@@ -48,6 +48,10 @@ struct alignas(64) Ss2dBwdParams {
   int I[4], O[4], rev[4];
   long long psi[4], pso[4];     // position = o·pso + i·psi
   int nsplit, tiles_per_split, max_tiles, nst;
+  // deterministic build (ss2d_bwd_det_kernel): m_dxc points at the du slabs (K, batch, Lseq, D); dB / dC partials per warp
+  // channel tile (D / CPW, batch, Lseq, K, 2N); dA (batch·nsplit, K·D, N), dDs and d dt_bias (batch·nsplit, K·D) per
+  // (image, L-segment)
+  float *part_bc, *part_dA, *part_dD, *part_db;
 };
 
 template <int N> struct FbCfg {
@@ -239,8 +243,9 @@ __global__ void __launch_bounds__(128, 3) ss2d_state_kernel(const __grid_constan
 // ---------------------------------------------------------------------------------------------------------------------
 // 2 + 3. reverse summaries (MODE_SUMMARY) and the main backward sweep (MODE_SERIAL / MODE_APPLY)
 // ---------------------------------------------------------------------------------------------------------------------
-template <int N, int MODE>
-__global__ void __launch_bounds__(128, 2) ss2d_bwd_kernel(const __grid_constant__ Ss2dBwdParams p) {
+// DET: every sum across CTAs goes to the partials of the deterministic build (see Ss2dBwdParams) instead of an atomic
+template <int N, int MODE, bool DET>
+__device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
   constexpr int LPC = FbCfg<N>::LPC, NS = FbCfg<N>::NS, CPW = FbCfg<N>::CPW, NT = FB_DT * LPC;
   constexpr bool MAIN = MODE != MODE_SUMMARY;
   constexpr float kLn2 = 0.6931471805599453f;
@@ -268,6 +273,11 @@ __global__ void __launch_bounds__(128, 2) ss2d_bwd_kernel(const __grid_constant_
       float *cr = p.carry + ((((long long)w.b * p.K + w.k) * p.D + d) * p.nsplit + w.split) * 2 * N;
 #pragma unroll
       for (int s = 0; s < NS; ++s) { cr[n0 + s] = 1.f; cr[N + n0 + s] = 0.f; }
+    } else if (DET) {              // an empty segment's partials are zero
+      const long long seg = (long long)w.b * p.nsplit + w.split, wd = (long long)w.k * p.D + d;
+#pragma unroll
+      for (int s = 0; s < NS; ++s) p.part_dA[(seg * p.K * p.D + wd) * N + n0 + s] = 0.f;
+      if (half == 0) { p.part_dD[seg * p.K * p.D + wd] = 0.f; p.part_db[seg * p.K * p.D + wd] = 0.f; }
     }
     return;
   }
@@ -388,9 +398,17 @@ __global__ void __launch_bounds__(128, 2) ss2d_bwd_kernel(const __grid_constant_
       const float rC = fb_transpose_reduce<NS, CPW / 2>(cC, lane, wc);
       constexpr int DUP = CPW / NS;
       if ((cl & (DUP - 1)) == 0) {
-        float *dst = dxrow0 + ((long long)o * p.pso[w.k] + (long long)(i0 + r) * p.psi[w.k]) * p.K * Cp;
-        atomicAdd(dst + n0 + wb, rB);
-        atomicAdd(dst + N + n0 + wb, rC);
+        const long long pos = (long long)o * p.pso[w.k] + (long long)(i0 + r) * p.psi[w.k];
+        if (DET) {
+          const long long tile = (long long)blockIdx.x * (NT / 32) + warp;
+          float *dst = p.part_bc + (((tile * p.batch + w.b) * p.Lseq + pos) * p.K + w.k) * 2 * N;
+          dst[n0 + wb] = rB;
+          dst[N + n0 + wb] = rC;
+        } else {
+          float *dst = dxrow0 + pos * p.K * Cp;
+          atomicAdd(dst + n0 + wb, rB);
+          atomicAdd(dst + N + n0 + wb, rC);
+        }
       }
       if (LPC == 2) {
         s1 += __shfl_xor_sync(0xffffffffu, s1, 16);
@@ -409,7 +427,8 @@ __global__ void __launch_bounds__(128, 2) ss2d_bwd_kernel(const __grid_constant_
       fence_proxy_async();
       __syncwarp();
       if (lane == 0) {
-        tma_reduce_add_4d(&p.m_dxc[w.k], sdu, w.d0 + warp * CPW, i0, o, w.b);
+        if (DET) tma_store_4d(&p.m_dxc[w.k], sdu, w.d0 + warp * CPW, i0, o, w.k * p.batch + w.b);   // this direction's du slab
+        else tma_reduce_add_4d(&p.m_dxc[w.k], sdu, w.d0 + warp * CPW, i0, o, w.b);
         tma_store_4d(&p.m_dd[w.k], sdd, w.d0 + warp * CPW, i0, o, w.k * p.batch + w.b);
         tma_store_commit();
         tma_store_wait_read<0>();
@@ -424,17 +443,30 @@ __global__ void __launch_bounds__(128, 2) ss2d_bwd_kernel(const __grid_constant_
   }
   if (MAIN) {
     if (lane == 0) tma_store_wait_all<0>();
+    if (DET) {
+      const long long seg = (long long)w.b * p.nsplit + w.split;
 #pragma unroll
-    for (int s = 0; s < NS; ++s) atomicAdd(&p.dA[wd * N + n0 + s], dAacc[s]);
-    if (half == 0) {
-      atomicAdd(&p.dDs[wd], dDacc);
-      atomicAdd(&p.ddtb[wd], dbacc);
+      for (int s = 0; s < NS; ++s) p.part_dA[(seg * p.K * p.D + wd) * N + n0 + s] = dAacc[s];
+      if (half == 0) { p.part_dD[seg * p.K * p.D + wd] = dDacc; p.part_db[seg * p.K * p.D + wd] = dbacc; }
+    } else {
+#pragma unroll
+      for (int s = 0; s < NS; ++s) atomicAdd(&p.dA[wd * N + n0 + s], dAacc[s]);
+      if (half == 0) {
+        atomicAdd(&p.dDs[wd], dDacc);
+        atomicAdd(&p.ddtb[wd], dbacc);
+      }
     }
   } else {
 #pragma unroll
     for (int s = 0; s < NS; ++s) { carry_row[n0 + s] = ex2(a2[s] * sumdl); carry_row[N + n0 + s] = dh[s]; }
   }
 }
+
+template <int N, int MODE>
+__global__ void __launch_bounds__(128, 2) ss2d_bwd_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, false>(p); }
+
+template <int N, int MODE>
+__global__ void __launch_bounds__(128, 2) ss2d_bwd_det_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, true>(p); }
 
 // ---- host ----
 constexpr int kFbMaxSplit = 64;
@@ -459,6 +491,27 @@ size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, i
   const int K = kind == SIGMA_DIRS_CROSS4 ? 4 : 2;
   const size_t carry = (size_t)batch * K * D * kFbMaxSplit * 2 * N * sizeof(float);
   return fb_al((size_t)K * batch * fb_max_tiles(kind, H, W) * D * N * sizeof(float)) + 2 * fb_al(carry);
+}
+
+// the deterministic build appends [du slabs (K, batch, Lseq, D)] [dB / dC partials (D / CPW, batch, Lseq, K, 2N)]
+// [dA partials (batch·64, K·D, N)] [dDs partials (batch·64, K·D)] [d dt_bias partials (batch·64, K·D)]
+struct FbDetLayout { size_t du, bc, dA, dD, total; };
+
+static FbDetLayout fb_det_layout(int kind, int batch, int H, int W, int D, int N) {
+  const int K = kind == SIGMA_DIRS_CROSS4 ? 4 : 2, CPW = N >= 16 ? 16 : 32;
+  const size_t Lseq = kind == SIGMA_DIRS_SEQ2 ? 2ull * H * W : (size_t)H * W;
+  const size_t segs = (size_t)batch * kFbMaxSplit;
+  FbDetLayout l;
+  l.du = ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N);
+  l.bc = l.du + fb_al((size_t)K * batch * Lseq * D * sizeof(float));
+  l.dA = l.bc + fb_al((size_t)(D / CPW) * batch * Lseq * K * 2 * N * sizeof(float));
+  l.dD = l.dA + fb_al(segs * K * D * N * sizeof(float));
+  l.total = l.dD + 2 * fb_al(segs * K * D * sizeof(float));
+  return l;
+}
+
+size_t ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
+  return fb_det_layout(kind, batch, H, W, D, N).total;
 }
 
 // The L-segment plan of the three sweeps.  All directions share tiles_per_split, so a direction with fewer tiles than the
@@ -487,14 +540,18 @@ int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int forc
   return SIGMA_OK;
 }
 
+int sum_parts_det_launch(const float *part, int nparts, long long ncols, long long inner, long long ostride, float *out, cudaStream_t stream);
+
 // delta / ddelta: (K, batch, Lseq, D) slabs stored at the position a value belongs to; dxc (batch, Lseq, D) and dxdbl
 // (batch, Lseq, K, Cp) are ACCUMULATED INTO after being zeroed here; dA (K·D, N), dDs (K·D), ddtb (K, D) overwritten.
+// det: the main sweep writes partials (see fb_det_layout) that sum_parts_det_kernel adds in a fixed order.
 int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                   const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
                   int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream,
-                  const float *hs_saved) {
-  if (ws == nullptr || ws_bytes < ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N)) {
-    set_error("sigma_ss2d_scan_bwd: workspace too small (%zu < %zu)", ws_bytes, ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N));
+                  const float *hs_saved, int det) {
+  const size_t need = det ? ss2d_scan_bwd_det_workspace_bytes(kind, batch, H, W, D, N) : ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N);
+  if (ws == nullptr || ws_bytes < need) {
+    set_error("sigma_ss2d_scan_bwd: workspace too small (%zu < %zu)", ws_bytes, need);
     return SIGMA_EWORKSPACE;
   }
   Ss2dBwdParams p;
@@ -551,7 +608,7 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
   SIGMA_CHECK_CUDA(cudaMemsetAsync(ddtb, 0, (size_t)K * D * sizeof(float), stream));
 
   // the state sweep stores delta' through m_dd (per-warp boxes over the delta slabs); the main sweep re-points it at ddelta
-  auto make_dd = [&](float *slab) -> int {
+  auto make_dd = [&](float *slab, CUtensorMap *maps = nullptr) -> int {
     for (int k = 0; k < K; ++k) {
       const bool colmajor = kind == SIGMA_DIRS_CROSS4 && (k & 1);
       uint64_t dims[4], str[3];
@@ -563,7 +620,7 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
         dims[0] = D; dims[1] = H; dims[2] = W; dims[3] = (uint64_t)K * batch;
         str[0] = (uint64_t)W * D * 4; str[1] = (uint64_t)D * 4; str[2] = (uint64_t)Lseq * D * 4;
       }
-      int r = make_tmap_f32_4d(&p.m_dd[k], slab, dims, str, boxw);
+      int r = make_tmap_f32_4d(maps ? &maps[k] : &p.m_dd[k], slab, dims, str, boxw);
       if (r) return r;
     }
     return SIGMA_OK;
@@ -571,6 +628,15 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
   if ((rc = make_dd(delta))) return rc;
   Ss2dBwdParams ps = p;
   if ((rc = make_dd(ddelta))) return rc;
+  const FbDetLayout dl = fb_det_layout(kind, batch, H, W, D, N);
+  float *du_slabs = (float *)((char *)ws + dl.du);
+  if (det) {   // du goes to per-direction slabs (plain TMA stores with the slab maps), the partials to the workspace
+    if ((rc = make_dd(du_slabs, p.m_dxc))) return rc;
+    p.part_bc = (float *)((char *)ws + dl.bc);
+    p.part_dA = (float *)((char *)ws + dl.dA);
+    p.part_dD = (float *)((char *)ws + dl.dD);
+    p.part_db = p.part_dD + (size_t)batch * kFbMaxSplit * K * D;
+  }
   Ss2dBwdParams pm = p;
   // ps holds m_dd -> delta (state sweep), pm holds m_dd -> ddelta (main sweep)
   auto go = [&](auto tag) -> int {
@@ -600,11 +666,29 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
       if ((r = run(ss2d_state_kernel<NN, MODE_APPLY>, ps, st_smem))) return r;
     }
     pm.carry = rcarry;
-    if (pm.nsplit == 1) return run(ss2d_bwd_kernel<NN, MODE_SERIAL>, pm, mn_smem);
-    if ((r = run(ss2d_bwd_kernel<NN, MODE_SUMMARY>, pm, sm_smem))) return r;
-    scan_combine_rev_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(rcarry, nrows, pm.nsplit, NN);
-    SIGMA_CHECK_LAUNCH();
-    return run(ss2d_bwd_kernel<NN, MODE_APPLY>, pm, mn_smem);
+    if (!det) {
+      if (pm.nsplit == 1) return run(ss2d_bwd_kernel<NN, MODE_SERIAL>, pm, mn_smem);
+      if ((r = run(ss2d_bwd_kernel<NN, MODE_SUMMARY>, pm, sm_smem))) return r;
+      scan_combine_rev_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(rcarry, nrows, pm.nsplit, NN);
+      SIGMA_CHECK_LAUNCH();
+      return run(ss2d_bwd_kernel<NN, MODE_APPLY>, pm, mn_smem);
+    }
+    if (pm.nsplit == 1) {
+      if ((r = run(ss2d_bwd_det_kernel<NN, MODE_SERIAL>, pm, mn_smem))) return r;
+    } else {
+      if ((r = run(ss2d_bwd_kernel<NN, MODE_SUMMARY>, pm, sm_smem))) return r;
+      scan_combine_rev_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(rcarry, nrows, pm.nsplit, NN);
+      SIGMA_CHECK_LAUNCH();
+      if ((r = run(ss2d_bwd_det_kernel<NN, MODE_APPLY>, pm, mn_smem))) return r;
+    }
+    // fixed-order sums: du over directions k, dB / dC over warp channel tiles, dA / dDs / d dt_bias over (image, segment)
+    const int segs = batch * pm.nsplit;
+    const long long KD = (long long)K * D;
+    if ((r = sum_parts_det_launch(du_slabs, K, (long long)batch * Lseq * D, (long long)batch * Lseq * D, 0, dxc, stream))) return r;
+    if ((r = sum_parts_det_launch(pm.part_bc, D / CPWc, (long long)batch * Lseq * K * 2 * NN, 2 * NN, Cp, dxdbl, stream))) return r;
+    if ((r = sum_parts_det_launch(pm.part_dA, segs, KD * NN, KD * NN, 0, dA, stream))) return r;
+    if ((r = sum_parts_det_launch(pm.part_dD, segs, KD, KD, 0, dDs, stream))) return r;
+    return sum_parts_det_launch(pm.part_db, segs, KD, KD, 0, ddtb, stream);
   };
   if (N == 16) return go(std::integral_constant<int, 16>{});
   return go(std::integral_constant<int, 4>{});

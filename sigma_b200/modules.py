@@ -749,7 +749,7 @@ class vssm_base(RGBXTransformer):
 def _bilinear_nhwc(x, size=None, scale_factor=None):
     """F.interpolate(bilinear, align_corners=False) on a channels-last tensor, staying channels-last."""
     t = x.permute(0, 3, 1, 2)  # NCHW view with channels_last strides: no copy
-    t = F.interpolate(t, size=size, scale_factor=scale_factor, mode="bilinear", align_corners=False)
+    t = ops.upsample_bilinear(t, size=size, scale_factor=scale_factor)
     return t.permute(0, 2, 3, 1).contiguous()
 
 
@@ -894,7 +894,7 @@ class MambaDecoder(nn.Module):
         x, ups = self.forward_up_features(inputs)
         outs = [self.up_x4(x, self.patch_size).contiguous()]
         for i, s in enumerate((16, 8, 4)):
-            t = F.interpolate(ups[i].permute(0, 3, 1, 2).contiguous(), scale_factor=s, mode="bilinear", align_corners=False)
+            t = ops.upsample_bilinear(ups[i].permute(0, 3, 1, 2).contiguous(), scale_factor=s)
             outs.append(self.output_ds[i](t))
         return tuple(outs)
 
@@ -943,7 +943,7 @@ class EncoderDecoder(nn.Module):
     def encode_decode(self, rgb, modal_x):
         out = self.decode_head(self.backbone(rgb, modal_x))
         if out.shape[2:] != rgb.shape[2:]:
-            out = F.interpolate(out, size=rgb.shape[2:], mode="bilinear", align_corners=False)
+            out = ops.upsample_bilinear(out, size=rgb.shape[2:])
         return out
 
     def forward(self, rgb, modal_x, label=None):
@@ -951,5 +951,8 @@ class EncoderDecoder(nn.Module):
             raise RuntimeError("sigma_b200.EncoderDecoder runs on CUDA only (no CPU path)")
         out = self.encode_decode(rgb, modal_x)
         if label is not None:
+            ignore = ops.plain_cross_entropy(self.criterion) if ops.deterministic() else None
+            if ignore is not None:   # nll_loss's CUDA backward raises under torch.use_deterministic_algorithms(True)
+                return ops.deterministic_cross_entropy(out, label.long(), ignore)
             return self.criterion(out, label.long())
         return out

@@ -6,7 +6,9 @@ re-exports them under the reference's module name.
 """
 import ctypes
 
+import numpy as np
 import torch
+import torch.nn.functional as F
 
 from . import _lib
 
@@ -19,6 +21,13 @@ def _ptr(t):
 
 def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def deterministic():
+    """True when torch.use_deterministic_algorithms(True) is in effect: the backward kernels then run their `_det` builds, which
+    keep every cross-CTA sum as partials and add them in a fixed order (bitwise reproducible for the same inputs, GPU model and
+    launch plan)."""
+    return torch.are_deterministic_algorithms_enabled()
 
 
 def _require_cuda(*ts):
@@ -99,6 +108,14 @@ def selective_scan_cuda_core_bwd(u, delta, A, B, C, D, delta_bias, dout, x, delt
     dbias = torch.empty(dim, dtype=torch.float32, device=u.device) if delta_bias is not None else None
     L_ = _lib.lib()
     dt = _DTYPE[u.dtype]
+    if deterministic():
+        wsb = L_.sigma_scan_bwd_det_workspace_bytes(batch, dim, L, N, G, dt)
+        ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=u.device)
+        rc = L_.sigma_scan_bwd_det(_ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C), _ptr(D), _ptr(delta_bias), _ptr(dout),
+                                   _ptr(du), _ptr(ddelta), _ptr(dA), _ptr(dB), _ptr(dC), _ptr(dD), _ptr(dbias),
+                                   batch, dim, L, N, G, dt, int(bool(delta_softplus)), _ptr(ws), wsb, int(_force_split), _stream())
+        _lib.check(rc, "sigma_scan_bwd_det")
+        return [du, ddelta, dA, dB.to(u.dtype), dC.to(u.dtype), dD, dbias]
     wsb = L_.sigma_scan_bwd_workspace_bytes(batch, dim, L, N, G, dt)
     ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=u.device)
     if _force_split:
@@ -360,6 +377,13 @@ class LayerNormFn(torch.autograd.Function):
         dy2 = dy.contiguous().float().view(-1, x2.shape[1])
         dx = torch.empty_like(x2)
         dw, db = torch.empty_like(w), torch.empty_like(w)
+        if deterministic():
+            L_ = _lib.lib()
+            wsb = L_.sigma_layernorm_bwd_det_workspace_bytes(x2.shape[0], x2.shape[1])
+            ws = torch.empty(max(wsb, 16), dtype=torch.uint8, device=x2.device)
+            _lib.check(L_.sigma_layernorm_bwd_det(_ptr(x2), _ptr(dy2), _ptr(w), _ptr(dx), _ptr(dw), _ptr(db), x2.shape[0], x2.shape[1],
+                                                  ctx.eps, _ptr(ws), wsb, _stream()), "sigma_layernorm_bwd_det")
+            return dx.view(dy.shape), dw, db, None
         _lib.check(_lib.lib().sigma_layernorm_bwd(_ptr(x2), _ptr(dy2), _ptr(w), _ptr(dx), _ptr(dw), _ptr(db), x2.shape[0], x2.shape[1], ctx.eps,
                                                  _stream()), "sigma_layernorm_bwd")
         return dx.view(dy.shape), dw, db, None
@@ -378,10 +402,14 @@ def layer_norm(norm, x):
 FUSED_SAVE_STATES = True      # training forward keeps delta' and the block-start states, so the backward runs no state sweep
 
 
-def _call_ss2d_bwd(args, saved=False):
+def _call_ss2d_bwd(args, saved=False, det=False):
     """The native call of the fused backward (a module-level function so that bench.py can bracket it with events)."""
     from . import fused
     L_ = _lib.lib()
+    if det:
+        fn = L_.sigma_ss2d_scan_bwd_saved_det if saved else L_.sigma_ss2d_scan_bwd_det
+        _lib.check(fn(*args, int(fused._FORCE_SPLIT or 0), _stream()), "sigma_ss2d_scan_bwd_det")
+        return
     if saved:
         _lib.check(L_.sigma_ss2d_scan_bwd_saved(*args, int(fused._FORCE_SPLIT or 0), _stream()), "sigma_ss2d_scan_bwd_saved")
         return
@@ -445,11 +473,12 @@ class FusedSS2DCore(torch.autograd.Function):
         dDs = torch.empty(K * D, dtype=torch.float32, device=dev)
         ddtb = torch.empty((K, D), dtype=torch.float32, device=dev)
         L_ = _lib.lib()
-        wsb = L_.sigma_ss2d_scan_bwd_workspace_bytes(kind, B, H, W, D, N)
+        det = deterministic()
+        wsb = (L_.sigma_ss2d_scan_bwd_det_workspace_bytes if det else L_.sigma_ss2d_scan_bwd_workspace_bytes)(kind, B, H, W, D, N)
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
         head = (kind, _ptr(xc), _ptr(xdbl), _ptr(dtw), _ptr(dtb), _ptr(A), _ptr(Ds), _ptr(dy), _ptr(delta))
         tail = (_ptr(dxc), _ptr(ddelta), _ptr(dxdbl), _ptr(dA), _ptr(dDs), _ptr(ddtb), B, H, W, D, N, R, Cp, _ptr(ws), wsb)
-        _call_ss2d_bwd(head + ((_ptr(hs),) if saved else ()) + tail, saved)
+        _call_ss2d_bwd(head + ((_ptr(hs),) if saved else ()) + tail, saved, det)
         # dt_proj: d dt_r = ddelta_k · W_dt[k]  (into the dt_r columns of dxdbl),  dW_dt[k] = ddelta_k^T · dt_r_k
         xd3 = xdbl.view(B * Lseq, K, Cp)
         dW = torch.empty_like(dtw)
@@ -464,3 +493,69 @@ class FusedSS2DCore(torch.autograd.Function):
         dxw = (d2.t() @ xc.view(B * Lseq, D)).view(K, Cp, D)
         dxpw = torch.cat([dxw[:, 2 * N:2 * N + R], dxw[:, 0:N], dxw[:, N:2 * N]], dim=1)          # back to [dt | B | C] rows
         return dxc, dxpw, dW, ddtb, dA * A, dDs, None, None, None
+
+
+# ---- deterministic training: bilinear upsampling and cross-entropy ----
+def _pair(v):
+    return (v, v) if not isinstance(v, (tuple, list)) else tuple(v)
+
+
+class UpsampleBilinearFn(torch.autograd.Function):
+    """F.interpolate(mode="bilinear", align_corners=False) of a CUDA tensor with a deterministic backward: forward is the kernel
+    F.interpolate runs without the switch (same bits); backward is sigma_upsample_bilinear_bwd, a gather in which every input
+    pixel sums the output pixels that tap it in a fixed order (torch's own backward adds them with atomics; under
+    use_deterministic_algorithms torch falls back to a slower index_put decomposition with other forward bits).
+    NCHW and channels-last inputs; `size=` or `scale_factor=` with torch's source-index rule for each."""
+
+    @staticmethod
+    def forward(ctx, x, size, scale_factor):
+        # the native kernel F.interpolate calls (under the switch F.interpolate itself would route to a decomposition with other bits)
+        y = torch._C._nn.upsample_bilinear2d(x, list(_pair(size)) if size is not None else None, False,
+                                             [float(s) for s in _pair(scale_factor)] if scale_factor is not None else None)
+        Hin, Win = x.shape[2:]
+        Hout, Wout = y.shape[2:]
+        if scale_factor is not None:   # torch passes the scale to the kernel: ratio = (float) (1.0 / scale)
+            rh, rw = (float(np.float32(1.0 / float(s))) for s in _pair(scale_factor))
+        else:                          # ratio = (float) in / out, in fp32
+            rh, rw = float(np.float32(Hin) / np.float32(Hout)), float(np.float32(Win) / np.float32(Wout))
+        ctx.meta = (tuple(x.shape), x.dtype, rh, rw, x.is_contiguous(memory_format=torch.channels_last) and not x.is_contiguous())
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (B, C, Hin, Win), dtype, rh, rw, cl = ctx.meta
+        Hout, Wout = dy.shape[2:]
+        fmt = torch.channels_last if cl else torch.contiguous_format
+        dy = dy.float().contiguous(memory_format=fmt)
+        dx = torch.empty((B, C, Hin, Win), dtype=torch.float32, device=dy.device, memory_format=fmt)
+        _lib.check(_lib.lib().sigma_upsample_bilinear_bwd(_ptr(dy), _ptr(dx), B, C, Hin, Win, Hout, Wout, rh, rw, int(cl), _stream()),
+                   "sigma_upsample_bilinear_bwd")
+        return dx.to(dtype), None, None
+
+
+def upsample_bilinear(x, size=None, scale_factor=None):
+    """F.interpolate(x, size, scale_factor, mode="bilinear", align_corners=False); under autograd with
+    torch.use_deterministic_algorithms(True), through UpsampleBilinearFn (same forward, deterministic backward)."""
+    if deterministic() and torch.is_grad_enabled() and x.requires_grad and x.is_cuda:
+        return UpsampleBilinearFn.apply(x, size, scale_factor)
+    return F.interpolate(x, size=size, scale_factor=scale_factor, mode="bilinear", align_corners=False)
+
+
+def plain_cross_entropy(criterion):
+    """The ignore_index of an nn.CrossEntropyLoss that deterministic_cross_entropy computes exactly (no class weights, no label
+    smoothing, reduction "mean"), else None."""
+    if (type(criterion) is torch.nn.CrossEntropyLoss and criterion.weight is None and criterion.label_smoothing == 0.0
+            and criterion.reduction == "mean"):
+        return criterion.ignore_index
+    return None
+
+
+def deterministic_cross_entropy(logits, target, ignore_index):
+    """nn.CrossEntropyLoss(ignore_index=ignore_index)(logits, target) for (B, K, ...) logits without nll_loss, whose CUDA
+    backward raises under use_deterministic_algorithms: log-softmax over K, gather of the target class (torch makes gather's
+    backward deterministic under the switch), then the mean over the pixels whose target is not ignore_index."""
+    keep = target != ignore_index
+    t = torch.where(keep, target, torch.zeros_like(target)).unsqueeze(1)
+    nll = -torch.gather(F.log_softmax(logits, dim=1), 1, t).squeeze(1)
+    nll = torch.where(keep, nll, torch.zeros_like(nll))
+    return nll.sum() / keep.sum().to(nll.dtype)
