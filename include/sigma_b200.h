@@ -324,6 +324,16 @@ int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H
  * directions share the tiles per segment, so a walk shorter than the longest can end in empty segments.  For tests and tuning. */
 int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, int nsplit, int64_t *out4_host);
 
+/* Launch plan of the fused scan forward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_fwd (force_split = 0),
+ * sigma_ss2d_scan_fwd_split (force_split > 0) or, with bf16 = 1, sigma_ss2d_scan_fwd_bf16 would launch for any kind at (batch, H,
+ * W, D, N, R) given a workspace of workspace_bytes (0: none), under the current environment (SIGMA_SCAN_WARPS, SIGMA_SCAN_NST,
+ * SIGMA_SCAN_CTAS, SIGMA_SCAN_SPLIT_RULE).  out8_host = {segments, LT-position tiles per segment, tiles of the longest direction's
+ * walk, tiles of the shortest, warps per CTA, TMA ring depth, register budget (the CTAs per SM the kernel build assumes: 3 or 4),
+ * dynamic shared-memory bytes per CTA}.  Returns what the launch would: SIGMA_EWORKSPACE for force_split > 1 without a large
+ * enough workspace.  For tests and tuning.                                                                                     */
+int sigma_test_ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R, int bf16, int force_split, size_t workspace_bytes,
+                             int64_t *out8_host);
+
 /* ------------------------------------------------------------------------------------------
  * SURVEY.md §8(f) rank 2, first piece: the evaluator's per-batch metric on the device (eval.py:22-29,
  * utils/metric.py:8-15).  pred = argmax over classes of logits (batch, classes, H, W) — the index numpy.argmax

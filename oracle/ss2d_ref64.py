@@ -1,7 +1,12 @@
-"""fp64 reference of the fused SS2D scan core (sigma_ss2d_scan_fwd_save, sigma_ss2d_scan_bwd{,_saved}) with a per-element error
-bound for each output of the fp32 kernels.  ORACLE — test infrastructure only.  Plain torch float64, device-agnostic.
+"""fp64 reference of the fused SS2D scan core (sigma_ss2d_scan_fwd{,_split,_bf16,_save}, sigma_ss2d_scan_bwd{,_saved}) with a
+per-element error bound for each output of the fp32 kernels.  ORACLE — test infrastructure only.  Plain torch float64,
+device-agnostic.  ss2d_fwd_ref64 is the forward alone (y and its bound, every kind, fp32 or bf16 xc); ss2d_ref64 runs it and
+adds the backward (kinds "cross4" and "seq2").
 
-Operation (kind "cross4": four directions over an H x W map; "seq2": forward and reversed walks over [rgb ‖ x], Lseq = 2·H·W).
+Operation (kind "cross4": four directions over an H x W map; "seq2": forward and reversed walks over [rgb ‖ x], Lseq = 2·H·W;
+"cross": the cross-modality scan, one row-major walk over the batch Bt = 2·images, images [0, Bt/2) of modality 0 and
+[Bt/2, Bt) of modality 1: image b runs with weight set w = [b >= Bt/2] (its rows of A, Ds, dt_proj and bias, A (2·D, N)) and its
+own B and dt_r, but takes C from the other modality's image (b + Bt/2) mod Bt (vmamba.py:1530,1536)).
 For direction k, walk step l visits position p = idx_k[l] (row-major, column-major l = w·H + h, and their reverses):
     delta'_l = softplus(dt_r[p] · W_dt[k]^T + bias[k])                  (K, B, Lseq, D) slabs, stored at position p
     h_l = exp(delta'_l · A) ⊙ h_{l-1} + delta'_l · u_l · B_l,  y_l = C_l · h_l + Ds · u_l
@@ -11,10 +16,11 @@ indexed as FbWalk::tile / ss2d_save_tiles define it: tile tau of a reversed walk
 holds min(16, H - i0) positions of one column.  Blocks a direction's walk does not reach are NaN.
 
 Memory and time.  Each walk is cut into its 16-position tiles (ragged tiles padded with identity steps: delta' = 0, u = B = C =
-dy = 0).  A scan runs in three levels: (1) every tile from a zero state, 16 steps vectorised over the tiles, keeping its end state
-and decay product; (2) the tile-start states, sequentially over the tiles; (3) the 16 steps again from those states.  Only one
-direction's states (h in fp64 and its error bound in fp32, (B, tiles, 16, D, N) each) are held at a time.  The largest case,
-Sigma-tiny stage 0 (B 2, 120 x 160, D 192, N 16), takes about 2 s and under 8 GB on an H100.
+dy = 0).  The reference's tiling is its own: the kernels' tiles are 32 positions at d_state 4 and 8.  A scan runs in three levels:
+(1) every tile from a zero state, 16 steps vectorised over the tiles, keeping its end state and decay product; (2) the tile-start
+states, sequentially over the tiles; (3) the 16 steps again from those states.  Only one direction's states (h in fp64 and its
+error bound in fp32, (B, tiles, 16, D, N) each) are held at a time, and the forward alone keeps none of them.  The largest
+backward case, Sigma-tiny stage 0 (B 2, 120 x 160, D 192, N 16), takes about 2 s and under 8 GB on an H100.
 
 Error bound.  A first-order running error analysis in fp64, carried through both recurrences alongside the values, in units of
 u = 2^-24 (fp32 rounding) and E2 = 2^-22 (the relative error bound the PTX ISA documents for ex2.approx.f32):
@@ -26,6 +32,16 @@ u = 2^-24 (fp32 rounding) and E2 = 2^-22 (the relative error bound the PTX ISA d
     products): to first order the error of h_l is exactly the decayed sum of these local perturbations.
     In the long-memory regime (delta' near dt_min = 1e-3, A = -1) e_l sums about 1/(delta'|A|) = 1000 decay errors before they
     fade, and so does the bound.
+  * y = C·h + Ds·u:  sum_n |C| e_l + (N+2)·u·(sum_n |C h| + |Ds u|)  (the N-term dot product and the skip's fma).  With bf16 xc
+    the reference takes xc's exact bf16 values (the kernel widens them exactly), and the bf16 store's round-to-nearest adds
+    2^-8·|y| relative, on the fp32 value: 2^-8·(|y| + its fp32 bound), after SAFETY.
+  * L-segments (the forward's summary / combine / apply passes): a segment's carried decay is ex2(a2·S), S the fp32 sum of the
+    segment's delta' (up to 32·tiles_per_split terms), in place of the product of the per-step decays.  Its relative error is one
+    E2, two roundings of the argument, |A|·(the sum's rounding, at most n·u·S for n terms) and |A|·(sum of the delta' errors).
+    The last is the per-step |A|·err(delta') summed; the rest replaces n per-step E2 terms, n·E2 = 4n·u, applied to the same
+    carried state.  |A|·S·n·u exceeds 4n·u only when |A|·S > 4, where the carried state has decayed below e^-4 of its value and
+    the per-step terms of the positions after it dominate, so the itemised per-step bound covers the segmented walk (checked by
+    an fp32 emulation that forms 32-segment carries the way the summary pass does, tests/test_ss2d_ref64_cpu.py).
   * backward: g_l = dy_l C_l + a_{l+1} g_{l+1} (the gradient reaching h_l) with error
     e^g_l = a_{l+1} e^g_{l+1} + a_{l+1} rho_{l+1} |g_{l+1}| + 2u |g_l|.  Every output is then a short expression in h, g, delta', u,
     B, C; its bound is the first-order sum of |partial| x error of each operand plus u per rounding on the magnitudes.
@@ -39,21 +55,24 @@ u = 2^-24 (fp32 rounding) and E2 = 2^-22 (the relative error bound the PTX ISA d
     squares (chan), since every channel runs its own recurrence.
   * the first-order errors of the B·L terms of dA and ddtb: added in absolute value within a 16-position tile, and as independent
     across tiles (tile_rss).  Summed in absolute value over all 38400 terms they would again exceed the 1e-3-of-scale bar.
-All first-order terms are multiplied by SAFETY = 1.5 to cover second-order terms and the few roundings not itemised above (the L-segment
-summaries' sum of delta' and the combine kernels, whose carry is a product of decays applied to a segment's start state rather than
-to each step's state).  Every bound is per element; none is a fraction of the tensor's maximum.
+All first-order terms are multiplied by SAFETY = 1.5 to cover second-order terms and the few roundings not itemised above (the
+combine kernels, whose carry is a product of decays applied to a segment's start state rather than to each step's state).  Every
+bound is per element; none is a fraction of the tensor's maximum.
 """
 import math
+import types
 
 import numpy as np
 import torch
 
 U = 2.0 ** -24
 E2 = 2.0 ** -22
+BF16_RN = 2.0 ** -8          # relative error of rounding to bf16 (8 significand bits) to nearest
 SP = 6e-7
 SAFETY = 1.5
 LAMBDA = 6.0
 LT = 16
+KINDS = {"cross4": 4, "seq2": 2, "cross": 1}     # directions (x_dbl rows per position)
 
 
 def dir_index(kind, H, W):
@@ -63,29 +82,41 @@ def dir_index(kind, H, W):
         row = np.arange(L)
         col = (np.arange(H)[None, :] * W + np.arange(W)[:, None]).reshape(-1)      # l = w·H + h -> position h·W + w
         return [row, col, row[::-1].copy(), col[::-1].copy()]
+    if kind == "cross":
+        return [np.arange(L)]
     a = np.arange(2 * L)
     return [a, a[::-1].copy()]
 
 
-def walk_tiles(kind, H, W):
-    """per direction: (ntiles, 16) positions of each walk-order tile in walk order, -1 past a ragged tile's end"""
+def walk_tiles(kind, H, W, lt=LT):
+    """per direction: (ntiles, lt) positions of each walk-order tile in walk order, -1 past a ragged tile's end"""
     out = []
     Lseq = H * W * (2 if kind == "seq2" else 1)
     for k, idx in enumerate(dir_index(kind, H, W)):
         colmajor = kind == "cross4" and k % 2 == 1
-        rev = k >= 2 if kind == "cross4" else k == 1
+        rev = (k >= 2) if kind == "cross4" else (k == 1 and kind == "seq2")
         I, O = (H, W) if colmajor else (Lseq, 1)
-        tpo = -(-I // LT)
+        tpo = -(-I // lt)
         ntiles = O * tpo
         o, i = (idx % W, idx // W) if colmajor else (np.zeros_like(idx), idx)
-        tm = o * tpo + i // LT
+        tm = o * tpo + i // lt
         tau = ntiles - 1 - tm if rev else tm
         assert np.all(np.diff(tau) >= 0)
         start = np.searchsorted(tau, np.arange(ntiles))
-        blk = np.full((ntiles, LT), -1, np.int64)
+        blk = np.full((ntiles, lt), -1, np.int64)
         blk[tau, np.arange(len(idx)) - start[tau]] = idx
         out.append(blk)
     return out
+
+
+def walk_groups(kind, Bt):
+    """(direction k, images, weight set, images C is read from) of every walk the kernels run: each direction over the whole
+    batch, or for "cross" each modality's half with its own weights and the other half's C"""
+    if kind != "cross":
+        return [(k, slice(0, Bt), k, slice(0, Bt)) for k in range(KINDS[kind])]
+    assert Bt % 2 == 0, "cross: the batch holds 2·images"
+    h = Bt // 2
+    return [(0, slice(0, h), 0, slice(h, Bt)), (0, slice(h, Bt), 1, slice(0, h))]
 
 
 def bound_fraction(got, ref, bound):
@@ -134,45 +165,47 @@ def _chain(P, loc, rev=False):
     return starts
 
 
-def ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None):
-    """kind "cross4" / "seq2"; xc, dy (B, Lseq, D), xdbl (B, Lseq, K, Cp) = [B | C | dt_r | padding], dtw (K, D, R), dtb (K, D),
-    A (K·D, N), Ds (K·D).  Returns (ref, bound): two dicts of float64 tensors with keys y, delta, hs, dxc, ddelta, dB, dC, dA, dDs,
-    ddtb.  y / delta / ddelta (K, B, Lseq, D), hs (K, B, max_tiles, D, N), dB / dC (B, Lseq, K, N)."""
+def _pad(t):
+    return torch.cat([t, torch.zeros_like(t[:, :1])], 1)          # position Lseq = the padding's zero row
+
+
+def ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, device=None, on_walk=None):
+    """The forward alone.  kind "cross4" / "seq2" / "cross"; xc (B, Lseq, D) fp32 or bf16, xdbl (B, Lseq, K, Cp) = [B | C | dt_r |
+    padding], dtw (Kw, D, R), dtb (Kw, D), A (Kw·D, N), Ds (Kw·D), Kw = K or 2 (modalities) for "cross".  Returns (y, bound), float64
+    (K, B, Lseq, D): direction k's output at the position it belongs to, and its per-element bound (SAFETY applied; with bf16 xc it
+    includes the final rounding to bf16).
+    on_walk(g): called after each walk with its tensors (tiles, inputs, delta', the states at every step and their bounds); the
+    states are only kept when it is given.  ss2d_ref64 runs its backward from there."""
+    bf16 = xc.dtype == torch.bfloat16
     dev = torch.device(device) if device is not None else xc.device
     f = lambda t: t.detach().to(dev, torch.float64)
-    xc, xdbl, dtw, dtb, A, Ds, dy = map(f, (xc, xdbl, dtw, dtb, A, Ds, dy))
+    xc, xdbl, dtw, dtb, A, Ds = map(f, (xc, xdbl, dtw, dtb, A, Ds))
     Bt, Lseq, D = xc.shape
     K, N, R = xdbl.shape[2], A.shape[1], dtw.shape[2]
+    assert K == KINDS[kind]
     tiles = walk_tiles(kind, H, W)
-    assert len(tiles) == K
-    T = max(t.shape[0] for t in tiles)
     z = lambda *s: torch.zeros(s, dtype=torch.float64, device=dev)
-    ref = dict(y=z(K, Bt, Lseq + 1, D), delta=z(K, Bt, Lseq + 1, D), hs=torch.full((K, Bt, T, D, N), math.nan, dtype=torch.float64, device=dev),
-               dxc=z(Bt, Lseq + 1, D), ddelta=z(K, Bt, Lseq + 1, D), dB=z(Bt, Lseq + 1, K, N), dC=z(Bt, Lseq + 1, K, N), dA=z(K * D, N),
-               dDs=z(K * D), ddtb=z(K, D))
-    bnd = {k: torch.zeros_like(v) for k, v in ref.items()}
-    bnd["hs"].fill_(math.nan)
-    dxc_mag = z(Bt, Lseq + 1, D)
-    pad = lambda t: torch.cat([t, torch.zeros_like(t[:, :1])], 1)          # position Lseq = the padding's zero row
-    xcp, dyp, xdp = pad(xc), pad(dy), pad(xdbl)
-    for k in range(K):
+    y, ey = z(K, Bt, Lseq + 1, D), z(K, Bt, Lseq + 1, D)
+    xcp, xdp = _pad(xc), _pad(xdbl)
+    for k, bs, kw, cs in walk_groups(kind, Bt):
         blk = torch.from_numpy(tiles[k]).to(dev)
         nb = blk.shape[0]
         m = (blk >= 0).double()[None, :, :, None]                               # (1, nb, 16, 1)
         p = torch.where(blk >= 0, blk, torch.full_like(blk, Lseq))
-        u = xcp[:, p]                                                           # (B, nb, 16, D)
-        xk = xdp[:, p, k]
-        Bm, Cm, dtr = xk[..., :N], xk[..., N:2 * N], xk[..., 2 * N:2 * N + R]
-        pre = dtr @ dtw[k].t() + dtb[k]
-        Tm = dtr.abs() @ dtw[k].abs().t() + dtb[k].abs()
+        u = xcp[bs][:, p]                                                       # (b, nb, 16, D)
+        xk = xdp[bs][:, p, k]
+        Bm, dtr = xk[..., :N], xk[..., 2 * N:2 * N + R]
+        Cm = xdp[cs][:, p, k, N:2 * N]
+        pre = dtr @ dtw[kw].t() + dtb[kw]
+        Tm = dtr.abs() @ dtw[kw].abs().t() + dtb[kw].abs()
         dl = torch.nn.functional.softplus(pre) * m
         sig = torch.sigmoid(pre)
         edl = (sig * (R + 2) * U * Tm + SP * dl) * m
         del Tm, dtr, xk
-        dyk = dyp[:, p]
-        Ak, Dk = A[k * D:(k + 1) * D], Ds[k * D:(k + 1) * D]
+        Ak, Dk = A[kw * D:(kw + 1) * D], Ds[kw * D:(kw + 1) * D]
         dlu = dl * u
         absA = Ak.abs()
+        b = u.shape[0]
 
         def slot(s):
             d_, e_ = dl[:, :, s, :, None], edl[:, :, s, :, None]
@@ -182,8 +215,8 @@ def ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None):
             ein = u[:, :, s, :, None].abs() * Bm[:, :, s, None, :].abs() * e_ + 3 * U * v.abs()
             return a, rho, v, ein
 
-        # ---- forward: h (levels 1 + 2), its error e (levels 1 + 2), then both at every step (level 3) ----
-        sh = (Bt, nb, D, N)
+        # ---- h (levels 1 + 2), its error e (levels 1 + 2), then both at every step (level 3) ----
+        sh = (b, nb, D, N)
         hl, P = z(*sh), torch.ones(sh, dtype=torch.float64, device=dev)
         for s in range(LT):
             a, _, v, _ = slot(s)
@@ -197,27 +230,63 @@ def ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None):
             h = hn
         e0 = _chain(P, el)
         del hl, el
-        h_all = torch.empty((Bt, nb, LT, D, N), dtype=torch.float64, device=dev)
-        e_all = torch.empty(h_all.shape, dtype=torch.float32, device=dev)      # a bound: 24 bits are plenty
+        keep = on_walk is not None
+        if keep:
+            h_all = torch.empty((b, nb, LT, D, N), dtype=torch.float64, device=dev)
+            e_all = torch.empty(h_all.shape, dtype=torch.float32, device=dev)  # a bound: 24 bits are plenty
         h, e = h0, e0
-        yk, ey = torch.empty_like(u), torch.empty_like(u)
+        yk, eyk = torch.empty_like(u), torch.empty_like(u)
         for s in range(LT):
             a, rho, v, ein = slot(s)
             hn = a * h + v
             e = a * e + a * rho * h.abs() + ein + U * hn.abs()
             h = hn
-            h_all[:, :, s], e_all[:, :, s] = h, e
+            if keep:
+                h_all[:, :, s], e_all[:, :, s] = h, e
             C = Cm[:, :, s, None, :]
             du_ = Dk * u[:, :, s]
             yk[:, :, s] = (C * h).sum(-1) + du_
-            ey[:, :, s] = (C.abs() * e).sum(-1) + (N + 2) * U * ((C * h).abs().sum(-1) + du_.abs())
-        ntk = nb
-        ref["hs"][k, :, :ntk], bnd["hs"][k, :, :ntk] = h0, e0
+            eyk[:, :, s] = (C.abs() * e).sum(-1) + (N + 2) * U * ((C * h).abs().sum(-1) + du_.abs())
         pf = p.reshape(-1)
+        y[k, bs].index_copy_(1, pf, yk.reshape(b, nb * LT, D))
+        ey[k, bs].index_copy_(1, pf, eyk.reshape(b, nb * LT, D))
+        del yk, eyk
+        if keep:
+            on_walk(types.SimpleNamespace(k=k, nb=nb, m=m, p=p, pf=pf, u=u, Bm=Bm, Cm=Cm, dl=dl, edl=edl, sig=sig, Ak=Ak, Dk=Dk,
+                                          absA=absA, slot=slot, P=P, h0=h0, e0=e0, h_all=h_all, e_all=e_all))
+            del h_all, e_all
+    y, ey = y[:, :, :Lseq].contiguous(), ey[:, :, :Lseq] * SAFETY
+    if bf16:
+        ey = ey + BF16_RN * (y.abs() + ey)
+    return y, ey.contiguous()
+
+
+def ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None):
+    """kind "cross4" / "seq2"; the inputs of ss2d_fwd_ref64 (fp32) and dy (B, Lseq, D).  Returns (ref, bound): two dicts of float64
+    tensors with keys y, delta, hs, dxc, ddelta, dB, dC, dA, dDs, ddtb.  y / delta / ddelta (K, B, Lseq, D), hs (K, B, max_tiles, D,
+    N), dB / dC (B, Lseq, K, N).  y and its bound are ss2d_fwd_ref64's, bit for bit."""
+    assert kind in ("cross4", "seq2"), "the fused backward covers CROSS4 and SEQ2"
+    dev = torch.device(device) if device is not None else xc.device
+    Bt, Lseq, D = xc.shape
+    K, N = xdbl.shape[2], A.shape[1]
+    T = max(t.shape[0] for t in walk_tiles(kind, H, W))
+    z = lambda *s: torch.zeros(s, dtype=torch.float64, device=dev)
+    ref = dict(delta=z(K, Bt, Lseq + 1, D), hs=torch.full((K, Bt, T, D, N), math.nan, dtype=torch.float64, device=dev),
+               dxc=z(Bt, Lseq + 1, D), ddelta=z(K, Bt, Lseq + 1, D), dB=z(Bt, Lseq + 1, K, N), dC=z(Bt, Lseq + 1, K, N), dA=z(K * D, N),
+               dDs=z(K * D), ddtb=z(K, D))
+    bnd = {k: torch.zeros_like(v) for k, v in ref.items()}
+    bnd["hs"].fill_(math.nan)
+    dxc_mag = z(Bt, Lseq + 1, D)
+    dyp = _pad(dy.detach().to(dev, torch.float64))
+
+    def backward(g):
+        k, nb, m, p, pf, u, Bm, Cm, dl, edl, sig = g.k, g.nb, g.m, g.p, g.pf, g.u, g.Bm, g.Cm, g.dl, g.edl, g.sig
+        Ak, Dk, absA, slot, P, h0, h_all, e_all = g.Ak, g.Dk, g.absA, g.slot, g.P, g.h0, g.h_all, g.e_all
+        sh = (Bt, nb, D, N)
         put = lambda dst, src: dst.index_copy_(1, pf, src.reshape(Bt, nb * LT, *src.shape[3:]))
-        put(ref["y"][k], yk); put(bnd["y"][k], ey)
+        ref["hs"][k, :, :nb], bnd["hs"][k, :, :nb] = h0, g.e0
         put(ref["delta"][k], dl); put(bnd["delta"][k], edl)
-        del yk, ey
+        dyk = dyp[:, p]
 
         # ---- backward: q = a·g entering each step from the right, and its error, tile by tile from the right ----
         def wslot(s):
@@ -303,11 +372,13 @@ def ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None):
         dd_k *= m
         ref["ddtb"][k] = dd_k.sum((0, 1, 2))
         bnd["ddtb"][k] = tile_rss(edd_k.sum(2)) + _acc(dd_k.sum(2), (dd_k.abs() + edd_k).sum(2), Lseq)
-        del h_all, e_all
+
+    y, ey = ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, device=dev, on_walk=backward)
     bnd["dxc"] += K * U * dxc_mag
-    for key in ("y", "delta", "dxc", "ddelta", "dB", "dC"):
+    for key in ("delta", "dxc", "ddelta", "dB", "dC"):
         sl = (slice(None), slice(0, Lseq)) if key in ("dxc", "dB", "dC") else (slice(None), slice(None), slice(0, Lseq))
         ref[key], bnd[key] = ref[key][sl].contiguous(), bnd[key][sl].contiguous()
     for key in bnd:
         bnd[key] = bnd[key] * SAFETY
+    ref["y"], bnd["y"] = y, ey
     return ref, bnd

@@ -38,6 +38,7 @@ SIGNATURES = {
     "sigma_test_pick_bn": (c_int, [c_int, c_int64]),
     "sigma_test_gemm_plan": (c_int, [c_int64, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int64)]),
     "sigma_test_ss2d_bwd_plan": (c_int, [c_int] * 7 + [ctypes.POINTER(c_int64)]),
+    "sigma_test_ss2d_fwd_plan": (c_int, [c_int] * 9 + [c_size_t, ctypes.POINTER(c_int64)]),
     "sigma_ss2d_scan_fwd_save": (c_int, [c_int] + [c_void_p] * 9 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
     "sigma_ss2d_scan_bwd_saved": (c_int, [c_int] + [c_void_p] * 15 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
     "sigma_ss2d_scan_bwd": (c_int, [c_int] + [c_void_p] * 14 + [c_int] * 7 + [c_void_p, c_size_t, c_void_p]),

@@ -272,6 +272,8 @@ int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw
                   size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave = nullptr, float *hsave = nullptr, int xc_bf16 = 0);
 size_t ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N);
 int ss2d_pick_segments_hook(long long ctas, int nw, int ntiles, int N);
+int ss2d_fwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int R, int xc_bf16, int force_split, size_t ws_bytes,
+                       long long *out8);
 int gemm_pick_bn_hook(int N, long long m_tiles);
 int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out);
 size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
@@ -531,6 +533,22 @@ int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, in
   const int rc = ss2d_bwd_plan_hook(kind, batch, H, W, D, N, nsplit, out);
   if (rc) return rc;
   for (int i = 0; i < 4; ++i) out4_host[i] = out[i];
+  return SIGMA_OK;
+}
+
+// the launch plan of sigma_ss2d_scan_fwd{,_split,_bf16} (force_split = 0: the library's choice), environment overrides included:
+// out8_host = {segments, tiles per segment, tiles of the longest walk, of the shortest, warps per CTA, ring depth, register
+// budget (CTAs per SM the kernel build assumes), dynamic shared-memory bytes}
+int sigma_test_ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R, int bf16, int force_split, size_t workspace_bytes,
+                             int64_t *out8_host) {
+  SIGMA_CHECK_ARG(out8_host && (kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2 || kind == SIGMA_DIRS_CROSS) && batch > 0 &&
+                      H > 0 && W > 0 && D > 0 && D % (bf16 ? 8 : 4) == 0 && R > 0 && force_split >= 0 &&
+                      (kind != SIGMA_DIRS_CROSS || batch % 2 == 0),
+                  "sigma_test_ss2d_fwd_plan: bad arguments");
+  long long out[8];
+  const int rc = ss2d_fwd_plan_hook(kind, batch, H, W, D, N, R, bf16 ? 1 : 0, force_split, workspace_bytes, out);
+  if (rc) return rc;
+  for (int i = 0; i < 8; ++i) out8_host[i] = out[i];
   return SIGMA_OK;
 }
 

@@ -135,10 +135,116 @@ size_t ss2d_scan_workspace_bytes(int kind, int batch, int D, int N) {
 int make_tmap_generic(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,
                       const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo);   // scan_op_tma.cu
 
+// The launch plan of the forward: everything ss2d_scan_fwd decides before it builds the tensor maps.  One function, so that the
+// launch and its host-only query (sigma_test_ss2d_fwd_plan) cannot disagree.
+struct Ss2dFwdPlan {
+  int nw;                        // warps per CTA (the CTA covers 32·nw channels)
+  int nsplit, tiles_per_split;   // L-segments and LT-position tiles per segment, shared by all directions
+  int max_tiles, min_tiles;      // LT-position tiles of the longest / shortest direction's walk
+  int nst;                       // TMA ring depth
+  int rbud;                      // register budget: the `CTAS` of the ss2d_scan_kernel build that runs
+  size_t smem;                   // dynamic shared memory per CTA
+};
+
+// have_ws: the caller passed a workspace of at least ss2d_scan_workspace_bytes
+static int ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R, int xc_bf16, int force_split, bool have_ws,
+                         Ss2dFwdPlan &pl) {
+  if (N != 4 && N != 8 && N != 16) {
+    set_error("sigma_ss2d_scan_fwd: d_state=%d unsupported by the fused kernel (4, 8, 16)", N);
+    return SIGMA_EUNSUPPORTED;
+  }
+  if (pad_rp(R) < 0) {
+    set_error("sigma_ss2d_scan_fwd: dt_rank %d > 64 unsupported", R);
+    return SIGMA_EUNSUPPORTED;
+  }
+  const int Cp = 2 * N + pad_rp(R);
+  const int xes = xc_bf16 ? 2 : 4;   // bytes per xc / y element
+  const int ndir = kind_dirs(kind);
+  const long long Lseq = kind == SIGMA_DIRS_SEQ2 ? 2LL * H * W : (long long)H * W;
+  const int LT = lt_for(N);
+  const int cpt = 1;   // channels per thread; CPT = 2 (shared B/C reads) lost at every Sigma shape (profiles/r01_scan_variants.txt)
+  int maxw = 4;  // warps per CTA (Ss2dCfg::MAXW; the kernels' register budget assumes 128 threads)
+  if (const char *e = getenv("SIGMA_SCAN_WARPS")) maxw = std::max(1, std::min(4, atoi(e)));
+  const int NW = pick_warps(D, cpt, maxw), DT = 32 * cpt * NW;
+  int max_tiles = 0, min_tiles = 0;
+  for (int k = 0; k < ndir; ++k) {
+    const bool colmajor = kind == SIGMA_DIRS_CROSS4 && (k & 1);
+    const long long I = colmajor ? H : Lseq, O = colmajor ? W : 1;
+    const int nt = (int)(O * ((I + LT - 1) / LT));
+    max_tiles = std::max(max_tiles, nt);
+    min_tiles = k == 0 ? nt : std::min(min_tiles, nt);
+  }
+  // L-segments (MODE_SUMMARY -> combine -> MODE_APPLY): a second pass over the data, so only when the unsplit grid leaves SM
+  // sub-partitions without a warp.  ss2d_pick_segments models the busiest SM (the old rule, "fill 592 warp slots", ignored
+  // wave quantisation: 312 CTAs of 2 warps put 6 warps on some SMs where 288 put 4 on every SM).  SIGMA_SCAN_SPLIT_RULE=old
+  // restores the round-1 rule for comparison.
+  const long long ctas = (long long)((D + DT - 1) / DT) * ndir * batch;
+  const long long warps = ctas * NW;
+  const long long full = kNumSMs * 4;
+  int nsplit = 1;
+  const char *rule = getenv("SIGMA_SCAN_SPLIT_RULE");
+  if (rule && rule[0] == 'o') {
+    if (warps < full) {
+      const long long want = N >= 16 ? full : 2 * full;
+      nsplit = (int)std::min<long long>((want + warps - 1) / warps, kMaxSplit);
+    }
+  } else if (warps < 3 * full) {
+    nsplit = ss2d_pick_segments(ctas, NW, max_tiles, N);
+  }
+  if (force_split > 0) nsplit = std::min(force_split, kMaxSplit);
+  if (!have_ws) {
+    if (force_split > 1) { set_error("sigma_ss2d_scan_fwd: workspace too small for %d segments", force_split); return SIGMA_EWORKSPACE; }
+    nsplit = 1;
+  }
+  nsplit = std::max(1, std::min(nsplit, max_tiles));
+  // all directions share tiles_per_split; directions with fewer tiles simply get empty trailing segments
+  pl.tiles_per_split = (max_tiles + nsplit - 1) / nsplit;
+  pl.nsplit = nsplit;
+  pl.max_tiles = max_tiles;
+  pl.min_tiles = min_tiles;
+  pl.nw = NW;
+
+  // register budget (ss2d_scan.cuh): which `__launch_bounds__(128, CTAS)` build runs.  SIGMA_SCAN_CTAS overrides.
+  int rbud = ss2d_pick_ctas(N, pad_rp(R));
+  if (const char *e = getenv("SIGMA_SCAN_CTAS")) rbud = std::max(3, std::min(5, atoi(e)));
+  if (N != 16 || xc_bf16) rbud = 3;   // bf16: only the 3-CTA budget is built (ss2d_scan_inst.inc)
+  rbud = std::min(rbud, 4);
+  pl.rbud = rbud;
+  {
+    // TMA ring depth: as many stages as fit without lowering the register-limited occupancy (227 KB per SM, 1 KB
+    // reserved per CTA).
+    // Deep rings matter: a tile is requested when the LAST warp releases its slot and needed by the FIRST warp
+    // nst-1 tiles later; with 3-4 stages the warps spun on the full barrier ~80 times per tile (ncu, round 1).
+    const size_t stage = (size_t)LT * DT * xes + (size_t)LT * Cp * (kind == SIGMA_DIRS_CROSS ? 2 : 1) * sizeof(float);
+    // resident CTAs per SM by registers (e.g. 168 per thread under __launch_bounds__(128, 3): 3 / 4 / 6 / 12 for 4 / 3 / 2 / 1 warps)
+    const int ctas_sm = std::max(rbud, std::min(16, 65536 / (32 * NW * ss2d_reg_cap(rbud))));
+    const size_t budget = (227 * 1024) / ctas_sm - 1024 - 128;
+    pl.nst = (int)std::max<size_t>(2, std::min<size_t>(Ss2dCfg<16>::MAX_NST, budget / stage));
+    if (const char *e = getenv("SIGMA_SCAN_NST")) pl.nst = std::max(2, std::min(Ss2dCfg<16>::MAX_NST, atoi(e)));
+  }
+  pl.smem = ss2d_smem_bytes(LT, DT, pl.nst, Cp, kind == SIGMA_DIRS_CROSS, xes);
+  return SIGMA_OK;
+}
+
+int ss2d_fwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int R, int xc_bf16, int force_split, size_t ws_bytes,
+                       long long *out8) {   // api.cu: sigma_test_ss2d_fwd_plan
+  Ss2dFwdPlan pl;
+  const bool have_ws = ws_bytes > 0 && ws_bytes >= ss2d_scan_workspace_bytes(kind, batch, D, N);
+  const int rc = ss2d_fwd_plan(kind, batch, H, W, D, N, R, xc_bf16, force_split, have_ws, pl);
+  if (rc) return rc;
+  const long long v[8] = {pl.nsplit, pl.tiles_per_split, pl.max_tiles, pl.min_tiles, pl.nw, pl.nst, pl.rbud, (long long)pl.smem};
+  for (int i = 0; i < 8; ++i) out8[i] = v[i];
+  return SIGMA_OK;
+}
+
 // xc_bf16 = 1: xc and y are bf16 (passed through the float pointers); x_dbl, the parameters and the recurrence stay fp32
 int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                   const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp, void *ws,
                   size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave, float *hsave, int xc_bf16) {
+  Ss2dFwdPlan pl;
+  int rc = ss2d_fwd_plan(kind, batch, H, W, D, N, R, xc_bf16, force_split,
+                         ws != nullptr && ws_bytes >= ss2d_scan_workspace_bytes(kind, batch, D, N), pl);
+  if (rc) return rc;
   Ss2dParams p;
   memset(&p, 0, sizeof(p));
   p.xc_bf16 = xc_bf16;
@@ -153,12 +259,7 @@ int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw
   const long long Lseq = kind == SIGMA_DIRS_SEQ2 ? 2LL * H * W : (long long)H * W;
   p.Lseq = Lseq;
   const int LT = lt_for(N);
-  const int cpt = 1;   // channels per thread; CPT = 2 (shared B/C reads) lost at every Sigma shape (profiles/r01_scan_variants.txt)
-  int maxw = 4;  // warps per CTA (Ss2dCfg::MAXW; the kernels' register budget assumes 128 threads)
-  if (const char *e = getenv("SIGMA_SCAN_WARPS")) maxw = std::max(1, std::min(4, atoi(e)));
-  const int NW = pick_warps(D, cpt, maxw), DT = 32 * cpt * NW;
-  int rc;
-  int max_tiles = 0;
+  const int NW = pl.nw, DT = 32 * NW;
   for (int k = 0; k < ndir; ++k) {
     const bool colmajor = kind == SIGMA_DIRS_CROSS4 && (k & 1);
     p.rev[k] = (kind == SIGMA_DIRS_CROSS4) ? (k >= 2) : (kind == SIGMA_DIRS_SEQ2 ? (k == 1) : 0);
@@ -187,57 +288,15 @@ int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw
     else { str[0] = W * pos; str[1] = pos; str[2] = Lseq * pos; }
     if ((rc = make_tmap_f32_4d(&p.m_dbl[k], xdbl + (long long)(kind == SIGMA_DIRS_CROSS ? 0 : k) * Cp, dims, str, boxd)))
       return rc;
-    max_tiles = std::max(max_tiles, p.O[k] * ((p.I[k] + LT - 1) / LT));
   }
-  // L-segments (MODE_SUMMARY -> combine -> MODE_APPLY): a second pass over the data, so only when the unsplit grid leaves SM
-  // sub-partitions without a warp.  ss2d_pick_segments models the busiest SM (the old rule, "fill 592 warp slots", ignored
-  // wave quantisation: 312 CTAs of 2 warps put 6 warps on some SMs where 288 put 4 on every SM).  SIGMA_SCAN_SPLIT_RULE=old
-  // restores the round-1 rule for comparison.
-  const long long ctas = (long long)((D + DT - 1) / DT) * ndir * batch;
-  const long long warps = ctas * NW;
-  const long long full = kNumSMs * 4;
-  int nsplit = 1;
-  const char *rule = getenv("SIGMA_SCAN_SPLIT_RULE");
-  if (rule && rule[0] == 'o') {
-    if (warps < full) {
-      const long long want = N >= 16 ? full : 2 * full;
-      nsplit = (int)std::min<long long>((want + warps - 1) / warps, kMaxSplit);
-    }
-  } else if (warps < 3 * full) {
-    nsplit = ss2d_pick_segments(ctas, NW, max_tiles, N);
-  }
-  if (force_split > 0) nsplit = std::min(force_split, kMaxSplit);
-  if (ws == nullptr || ws_bytes < ss2d_scan_workspace_bytes(kind, batch, D, N)) {
-    if (force_split > 1) { set_error("sigma_ss2d_scan_fwd: workspace too small for %d segments", force_split); return SIGMA_EWORKSPACE; }
-    nsplit = 1;
-  }
-  nsplit = std::max(1, std::min(nsplit, max_tiles));
-  // all directions share tiles_per_split; directions with fewer tiles simply get empty trailing segments
-  p.tiles_per_split = (max_tiles + nsplit - 1) / nsplit;
-  p.nsplit = nsplit;
-
-  // register budget (ss2d_scan.cuh): which `__launch_bounds__(128, CTAS)` build runs.  SIGMA_SCAN_CTAS overrides.
-  int rbud = ss2d_pick_ctas(N, pad_rp(R));
-  if (const char *e = getenv("SIGMA_SCAN_CTAS")) rbud = std::max(3, std::min(5, atoi(e)));
-  if (N != 16 || xc_bf16) rbud = 3;   // bf16: only the 3-CTA budget is built (ss2d_scan_inst.inc)
-  rbud = std::min(rbud, 4);
-  {
-    // TMA ring depth: as many stages as fit without lowering the register-limited occupancy (227 KB per SM, 1 KB
-    // reserved per CTA).
-    // Deep rings matter: a tile is requested when the LAST warp releases its slot and needed by the FIRST warp
-    // nst-1 tiles later; with 3-4 stages the warps spun on the full barrier ~80 times per tile (ncu, round 1).
-    const size_t stage = (size_t)LT * DT * xes + (size_t)LT * Cp * (kind == SIGMA_DIRS_CROSS ? 2 : 1) * sizeof(float);
-    // resident CTAs per SM by registers (e.g. 168 per thread under __launch_bounds__(128, 3): 3 / 4 / 6 / 12 for 4 / 3 / 2 / 1 warps)
-    const int ctas_sm = std::max(rbud, std::min(16, 65536 / (32 * NW * ss2d_reg_cap(rbud))));
-    const size_t budget = (227 * 1024) / ctas_sm - 1024 - 128;
-    p.nst = (int)std::max<size_t>(2, std::min<size_t>(Ss2dCfg<16>::MAX_NST, budget / stage));
-    if (const char *e = getenv("SIGMA_SCAN_NST")) p.nst = std::max(2, std::min(Ss2dCfg<16>::MAX_NST, atoi(e)));
-  }
+  p.tiles_per_split = pl.tiles_per_split;
+  p.nsplit = pl.nsplit;
+  p.nst = pl.nst;
   const int nthreads = 32 * NW;
   switch (N) {
-    case 4: return dispatch_rp<4, 1>(p, nthreads, rbud, stream);
-    case 8: return dispatch_rp<8, 1>(p, nthreads, rbud, stream);
-    case 16: return dispatch_rp<16, 1>(p, nthreads, rbud, stream);
+    case 4: return dispatch_rp<4, 1>(p, nthreads, pl.rbud, stream);
+    case 8: return dispatch_rp<8, 1>(p, nthreads, pl.rbud, stream);
+    case 16: return dispatch_rp<16, 1>(p, nthreads, pl.rbud, stream);
   }
   set_error("sigma_ss2d_scan_fwd: d_state=%d unsupported by the fused kernel (4, 8, 16)", N);
   return SIGMA_EUNSUPPORTED;

@@ -60,3 +60,83 @@ def sample_index(key, numel, k):
     """A fixed, seeded set of min(k, numel) flat indices for `key`: the positions at which a golden file stores a large output."""
     rng = np.random.default_rng(zlib.crc32(key.encode()))
     return np.sort(rng.choice(numel, size=min(k, numel), replace=False))
+
+
+# ---- the fused SS2D scan through its C-ABI (the fp64 tests of its forward and backward) ----
+SS2D_GUARD = 64                          # guard elements on each side of every output (keeps 16-byte alignment)
+_NAN_BITS = {torch.float32: (torch.int32, 0x7FC00000), torch.bfloat16: (torch.int16, 0x7FC0)}
+
+
+def ptr(t):
+    import ctypes
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def stream():
+    import ctypes
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def ss2d_kind(kind):
+    from sigma_b200 import _lib
+    return {"cross4": _lib.DIRS_CROSS4, "seq2": _lib.DIRS_SEQ2, "cross": _lib.DIRS_CROSS}[kind]
+
+
+def guarded(shape, dtype=torch.float32):
+    """(buffer, interior view): NaN-filled device memory with SS2D_GUARD elements on each side of `shape`"""
+    import math
+    n = math.prod(shape)
+    buf = torch.full((n + 2 * SS2D_GUARD,), float("nan"), dtype=dtype, device="cuda")
+    return buf, buf[SS2D_GUARD:SS2D_GUARD + n].view(shape)
+
+
+def guard_ok(buf, what):
+    """no guard element of a `guarded` buffer was written: every one still has the bits of the NaN it was filled with"""
+    n = buf.numel() - 2 * SS2D_GUARD
+    ity, nan = _NAN_BITS[buf.dtype]
+    bits = torch.cat([buf[:SS2D_GUARD], buf[SS2D_GUARD + n:]]).view(ity)
+    bad = int((bits != nan).sum())
+    assert bad == 0, f"{what}: {bad} guard elements were written"
+
+
+def ss2d_params(seed, kind, B, H, W, D, N, R, tag, wide=False):
+    """inputs of the fused scan at Sigma's scales: dt log-uniform in [1e-3, 0.1] (0.5 when wide) through the inverse softplus,
+    A = -exp(A_log) around the S4D-real init (|A| up to 4x when wide), Ds near 1, x_dbl's padding columns 0.  B is the batch
+    (2·images for "cross", which has two weight sets).  Returns ([xc, xdbl, dtw, dtb, A, Ds, dy] on the GPU, Cp)."""
+    import math
+    import procedural as P
+    from sigma_b200 import _lib
+    K = {"cross4": 4, "seq2": 2, "cross": 1}[kind]
+    Kw = 2 if kind == "cross" else K
+    Lseq = H * W * (2 if kind == "seq2" else 1)
+    Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
+    xc = P.randn(seed, tag + "/xc", (B, Lseq, D))
+    xdbl = P.randn(seed, tag + "/xdbl", (B, Lseq, K, Cp))
+    xdbl[..., 2 * N:2 * N + R] *= 2.0
+    xdbl[..., 2 * N + R:] = 0.0                                          # padding columns, as the packed x_proj leaves them
+    dtw = P.rand(seed, tag + "/dtw", (Kw, D, R), -R ** -0.5, R ** -0.5)
+    dt = torch.exp(P.rand(seed, tag + "/dt", (Kw, D), math.log(1e-3), math.log(0.5 if wide else 0.1)))
+    dtb = dt + torch.log(-torch.expm1(-dt))                              # inverse softplus
+    A_log = torch.log(torch.arange(1, N + 1, dtype=torch.float32)).repeat(Kw * D, 1) + P.rand(seed, tag + "/A", (Kw * D, N), -0.2,
+                                                                                                   1.4 if wide else 0.2)
+    A = -torch.exp(A_log)
+    Ds = P.randn(seed, tag + "/Ds", (Kw * D,), 0.1, 1.0)
+    dy = P.randn(seed, tag + "/dy", (B, Lseq, D))
+    return [t.cuda() for t in (xc, xdbl, dtw, dtb, A, Ds, dy)], Cp
+
+
+SS2D_FWD_PLAN = ("nsplit", "tiles_per_split", "max_tiles", "min_tiles", "warps", "nst", "ctas", "smem")
+
+
+def ss2d_fwd_plan(kind, B, H, W, D, N, R, bf16=False, force=0, ws_bytes=None):
+    """The launch plan sigma_ss2d_scan_fwd{,_split,_bf16} would use under the current environment (SIGMA_SCAN_* included), from the
+    library's own planner.  ws_bytes: the workspace the call gets (None: sigma_ss2d_scan_workspace_bytes, 0: none)."""
+    import ctypes
+    from sigma_b200 import _lib
+    L = _lib.lib()
+    if ws_bytes is None:
+        ws_bytes = L.sigma_ss2d_scan_workspace_bytes(ss2d_kind(kind), B, H, W, D, N)
+    out = (ctypes.c_int64 * 8)()
+    _lib.check(L.sigma_test_ss2d_fwd_plan(ss2d_kind(kind), B, H, W, D, N, R, int(bool(bf16)), force, ws_bytes, out),
+               "sigma_test_ss2d_fwd_plan")
+    return dict(zip(SS2D_FWD_PLAN, (int(v) for v in out)))

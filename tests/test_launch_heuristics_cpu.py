@@ -4,7 +4,10 @@
   images x 10 forced counts) its choices must stay within 6 % of the per-row optimum in total and well ahead of the old rule.
 * `pick_bn` (GEMM tile width): the widest divisor in the throughput regime, narrower tiles when few row tiles exist.
 * `plan_gemm` (the whole launch plan of the GEMM / implicit-GEMM conv, SIGMA_GEMM_BN included, through sigma_test_gemm_plan):
-  every plan is launchable — grid within the tile count, 2-8 ring stages, shared memory within the H100's limits."""
+  every plan is launchable — grid within the tile count, 2-8 ring stages, shared memory within the H100's limits.
+* the fused scan forward's whole launch plan (through sigma_test_ss2d_fwd_plan) at every Sigma inference shape and 1, 2, 8 and 74
+  images: segments capped at 32 and never empty for the longest walk by choice, one segment without a workspace, the 4-CTA register
+  budget only where it is built and chosen, a ring of 2-8 stages whose shared memory fits the CTAs the budget puts on an SM."""
 import os
 import re
 
@@ -190,3 +193,121 @@ def test_ss2d_bwd_plan_rejects_bad_arguments(L):
     assert L.sigma_test_ss2d_bwd_plan(0, 1, 15, 20, 96, 16, 0, out) != 0              # D % 64
     assert L.sigma_test_ss2d_bwd_plan(0, 1, 15, 20, 1536, 8, 0, out) != 0             # d_state
     assert L.sigma_test_ss2d_bwd_plan(0, 1, 15, 20, 1536, 16, -1, out) != 0
+
+
+# ---- the launch plan of the fused scan forward (sigma_test_ss2d_fwd_plan = the planner sigma_ss2d_scan_fwd* launch with) ----
+# Sigma's inference shapes: (kind, H, W, D, d_state, dt_rank) — the SS2D blocks of tiny / small (D 192..1536) and base (45 x 60,
+# 23 x 30), CroMB (CROSS) and ConMB (SEQ2) at d_state 4, and the decoder's SS2D (d_state 4)
+FWD_SHAPES = ([("cross4", 120, 160, 192, 16, 6), ("cross4", 60, 80, 384, 16, 12), ("cross4", 30, 40, 768, 16, 24),
+               ("cross4", 15, 20, 1536, 16, 48), ("cross4", 45, 60, 1024, 16, 32), ("cross4", 23, 30, 2048, 16, 64)]
+              + [(k, H, W, D, 4, R) for k in ("cross", "seq2")
+                 for H, W, D, R in [(120, 160, 192, 6), (60, 80, 384, 12), (30, 40, 768, 24), (15, 20, 1536, 48), (23, 30, 2048, 64)]]
+              + [("cross4", 120, 160, 192, 4, 6), ("cross4", 60, 80, 384, 4, 12), ("cross4", 30, 40, 768, 4, 24)])
+SCAN_ENV = ("SIGMA_SCAN_WARPS", "SIGMA_SCAN_NST", "SIGMA_SCAN_CTAS", "SIGMA_SCAN_SPLIT_RULE")
+
+
+def _reg_cap(ctas):
+    return (65536 // (ctas * 128)) // 8 * 8                                  # ss2d_reg_cap (ss2d_scan.cuh)
+
+
+def _walk_tiles(kind, H, W, N):
+    lt = 16 if N >= 16 else 32
+    rows = -(-H * W * (2 if kind == "seq2" else 1) // lt)
+    return (max(rows, W * -(-H // lt)), min(rows, W * -(-H // lt))) if kind == "cross4" else (rows, rows)
+
+
+def _check_fwd_plan(pl, kind, H, W, D, N, R, bf16):
+    from sigma_b200 import _lib
+    assert (pl["max_tiles"], pl["min_tiles"]) == _walk_tiles(kind, H, W, N)
+    assert 1 <= pl["nsplit"] <= min(32, pl["max_tiles"])
+    assert pl["tiles_per_split"] == -(-pl["max_tiles"] // pl["nsplit"])
+    assert 1 <= pl["warps"] <= 4 and 2 <= pl["nst"] <= 8
+    assert pl["ctas"] in (3, 4)
+    lt = 16 if N >= 16 else 32
+    stage = lt * 32 * pl["warps"] * (2 if bf16 else 4) + lt * _lib.lib().sigma_ss2d_padded_cp(N, R) * 4 * (2 if kind == "cross" else 1)
+    assert pl["smem"] == pl["nst"] * stage + 128
+    assert pl["smem"] <= SMEM_PER_BLOCK
+    return stage
+
+
+@pytest.mark.parametrize("bf16", [False, True])
+@pytest.mark.parametrize("kind,H,W,D,N,R", FWD_SHAPES)
+@pytest.mark.parametrize("images", [1, 2, 8, 74])
+def test_ss2d_fwd_plan_invariants(L, kind, H, W, D, N, R, images, bf16, monkeypatch):
+    from helpers import ss2d_fwd_plan
+    for e in SCAN_ENV:
+        monkeypatch.delenv(e, raising=False)
+    B = 2 * images if kind == "cross" else images
+    auto = ss2d_fwd_plan(kind, B, H, W, D, N, R, bf16)
+    _check_fwd_plan(auto, kind, H, W, D, N, R, bf16)
+    assert (auto["nsplit"] - 1) * auto["tiles_per_split"] < auto["max_tiles"]      # no segment of the longest walk is empty
+    # the register budget: 4 CTAs (128 registers) only for d_state 16 at padded dt_rank 24, and only in fp32
+    assert auto["ctas"] == (4 if N == 16 and L.sigma_ss2d_padded_cp(N, R) == 2 * N + 24 and not bf16 else 3)
+    # the ring fits the shared memory of the CTAs the register budget puts on an SM together
+    ctas_sm = max(auto["ctas"], min(16, 65536 // (32 * auto["warps"] * _reg_cap(auto["ctas"]))))
+    assert ctas_sm * (auto["smem"] + 1024) <= SMEM_PER_SM
+    capped = ss2d_fwd_plan(kind, B, H, W, D, N, R, bf16, force=100)
+    _check_fwd_plan(capped, kind, H, W, D, N, R, bf16)
+    assert capped["nsplit"] == min(32, capped["max_tiles"])                        # 100 is capped at 32 segments
+    for force in (1, 2, 7, 8, 20):
+        pl = ss2d_fwd_plan(kind, B, H, W, D, N, R, bf16, force=force)
+        _check_fwd_plan(pl, kind, H, W, D, N, R, bf16)
+        assert pl["nsplit"] == min(force, pl["max_tiles"])                         # a forced count is kept, even if segments end empty
+        assert {k: pl[k] for k in ("warps", "nst", "ctas", "smem")} == {k: auto[k] for k in ("warps", "nst", "ctas", "smem")}
+    # without a workspace: one segment, and a forced count above 1 is an error
+    assert ss2d_fwd_plan(kind, B, H, W, D, N, R, bf16, ws_bytes=0)["nsplit"] == 1
+    assert ss2d_fwd_plan(kind, B, H, W, D, N, R, bf16, force=1, ws_bytes=0)["nsplit"] == 1
+    import ctypes
+    from helpers import ss2d_kind
+    out = (ctypes.c_int64 * 8)()
+    assert L.sigma_test_ss2d_fwd_plan(ss2d_kind(kind), B, H, W, D, N, R, int(bf16), 2, 0, out) == -3   # SIGMA_EWORKSPACE
+
+
+@pytest.mark.parametrize("kind", ["cross4", "seq2", "cross"])
+def test_ss2d_fwd_split_without_workspace_is_an_error(L, kind):
+    """sigma_ss2d_scan_fwd_split with more than one forced segment and no workspace returns SIGMA_EWORKSPACE before it touches the
+    device (the plan comes first), so the pointers here are never dereferenced"""
+    import ctypes
+    from sigma_b200 import _lib
+    from helpers import ss2d_kind
+    fake = ctypes.c_void_p(1 << 20)                                                # non-null and 16-byte aligned, never read
+    rc = L.sigma_ss2d_scan_fwd_split(ss2d_kind(kind), *[fake] * 7, 2, 30, 40, 384, 4, 12, L.sigma_ss2d_padded_cp(4, 12), None, 0, 3,
+                                     None)
+    assert rc == -3, rc                                                            # SIGMA_EWORKSPACE
+    assert "workspace" in _lib.lib().sigma_last_error().decode()
+
+
+def test_ss2d_fwd_plan_honours_the_environment(L, monkeypatch):
+    from helpers import ss2d_fwd_plan
+    for e in SCAN_ENV:
+        monkeypatch.delenv(e, raising=False)
+    shape = ("cross4", 1, 30, 40, 768, 16, 24)
+    assert ss2d_fwd_plan(*shape)["warps"] == 4 and ss2d_fwd_plan(*shape)["ctas"] == 4
+    for w in (1, 2, 3, 4):
+        monkeypatch.setenv("SIGMA_SCAN_WARPS", str(w))
+        # SIGMA_SCAN_WARPS caps the width; pick_warps tries 4, 2, 3, 1 warps for one that divides D
+        assert ss2d_fwd_plan(*shape)["warps"] == next(x for x in (4, 2, 3, 1) if x <= w and 768 % (32 * x) == 0)
+    monkeypatch.delenv("SIGMA_SCAN_WARPS")
+    for n in (2, 8):
+        monkeypatch.setenv("SIGMA_SCAN_NST", str(n))
+        assert ss2d_fwd_plan(*shape)["nst"] == n
+    monkeypatch.delenv("SIGMA_SCAN_NST")
+    for c in (3, 4):
+        monkeypatch.setenv("SIGMA_SCAN_CTAS", str(c))
+        assert ss2d_fwd_plan(*shape)["ctas"] == c
+        assert ss2d_fwd_plan("cross4", 1, 30, 40, 768, 16, 24, bf16=True)["ctas"] == 3        # bf16 builds one budget
+        assert ss2d_fwd_plan("cross4", 1, 30, 40, 768, 4, 24)["ctas"] == 3                    # d_state 4 builds one budget
+    # ragged D: enough warps to cover it, the last CTA partly filled
+    monkeypatch.delenv("SIGMA_SCAN_CTAS")
+    assert ss2d_fwd_plan("cross4", 1, 30, 40, 100, 16, 6)["warps"] == 4
+    assert ss2d_fwd_plan("cross4", 1, 30, 40, 132, 16, 6)["warps"] == 4
+
+
+def test_ss2d_fwd_plan_rejects_bad_arguments(L):
+    import ctypes
+    out = (ctypes.c_int64 * 8)()
+    assert L.sigma_test_ss2d_fwd_plan(2, 3, 15, 20, 1536, 4, 48, 0, 0, 1 << 30, out) != 0      # CROSS: batch = 2·images
+    assert L.sigma_test_ss2d_fwd_plan(0, 1, 15, 20, 100, 4, 48, 1, 0, 1 << 30, out) != 0       # bf16: D % 8
+    assert L.sigma_test_ss2d_fwd_plan(0, 1, 15, 20, 1536, 12, 48, 0, 0, 1 << 30, out) != 0     # d_state
+    assert L.sigma_test_ss2d_fwd_plan(0, 1, 15, 20, 1536, 16, 65, 0, 0, 1 << 30, out) != 0     # dt_rank
+    assert L.sigma_test_ss2d_fwd_plan(0, 1, 15, 20, 1536, 16, 48, 0, -1, 1 << 30, out) != 0

@@ -18,38 +18,16 @@ import pytest
 import torch
 
 import procedural as P
-from helpers import record
+from helpers import guard_ok as _guard_ok, guarded as _guarded, ptr as _p, record, ss2d_kind as _kid, ss2d_params, \
+    stream as _stream
 from oracle import ss2d_ref64 as R64
 
 pytestmark = pytest.mark.gpu
 S = 97
-G = 64                                   # guard floats on each side of every output (keeps 16-byte alignment)
-NAN32 = 0x7FC00000
 OUTS = ("y", "delta", "hs", "dxc", "ddelta", "dA", "dDs", "ddtb")
 # d dt_bias sums the per-element bounds of ddelta over all B·L positions; at dt_rank 48 / 64 that leaves its bound at the largest
 # element up to ~6x looser than 1e-3 of scale, so it must also meet that max-norm bar
 MAXNORM_TOO = ("ddtb",)
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _guarded(shape):
-    n = math.prod(shape)
-    buf = torch.full((n + 2 * G,), float("nan"), device="cuda")
-    return buf, buf[G:G + n].view(shape)
-
-
-def _guard_ok(buf, what):
-    n = buf.numel() - 2 * G
-    bits = torch.cat([buf[:G], buf[G + n:]]).view(torch.int32)
-    bad = int((bits != NAN32).sum())
-    assert bad == 0, f"{what}: {bad} guard elements were written"
 
 
 def _plan(kind, B, H, W, D, N, nsplit):
@@ -59,29 +37,8 @@ def _plan(kind, B, H, W, D, N, nsplit):
     return dict(zip(("nsplit", "tiles_per_split", "max_tiles", "min_tiles"), (int(v) for v in out)))
 
 
-def _kid(kind):
-    from sigma_b200 import _lib
-    return _lib.DIRS_CROSS4 if kind == "cross4" else _lib.DIRS_SEQ2
-
-
 def _params(kind, B, H, W, D, N, R, tag, wide=False):
-    from sigma_b200 import _lib
-    K = 4 if kind == "cross4" else 2
-    Lseq = H * W * (2 if kind == "seq2" else 1)
-    Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
-    xc = P.randn(S, tag + "/xc", (B, Lseq, D))
-    xdbl = P.randn(S, tag + "/xdbl", (B, Lseq, K, Cp))
-    xdbl[..., 2 * N:2 * N + R] *= 2.0
-    xdbl[..., 2 * N + R:] = 0.0                                          # padding columns, as the packed x_proj leaves them
-    dtw = P.rand(S, tag + "/dtw", (K, D, R), -R ** -0.5, R ** -0.5)
-    dt = torch.exp(P.rand(S, tag + "/dt", (K, D), math.log(1e-3), math.log(0.5 if wide else 0.1)))
-    dtb = dt + torch.log(-torch.expm1(-dt))                              # inverse softplus
-    A_log = torch.log(torch.arange(1, N + 1, dtype=torch.float32)).repeat(K * D, 1) + P.rand(S, tag + "/A", (K * D, N), -0.2,
-                                                                                                  1.4 if wide else 0.2)
-    A = -torch.exp(A_log)
-    Ds = P.randn(S, tag + "/Ds", (K * D,), 0.1, 1.0)
-    dy = P.randn(S, tag + "/dy", (B, Lseq, D))
-    return [t.cuda() for t in (xc, xdbl, dtw, dtb, A, Ds, dy)], Cp
+    return ss2d_params(S, kind, B, H, W, D, N, R, tag, wide)
 
 
 def _check(tag, name, got, ref, bnd, worst):
