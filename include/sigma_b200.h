@@ -334,6 +334,24 @@ int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, in
 int sigma_test_ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R, int bf16, int force_split, size_t workspace_bytes,
                              int64_t *out8_host);
 
+/* sigma_scan_fwd with a forced number of L-segments (nsplit = 0: the library's choice; more than 64 is capped at 64), any dtype
+ * and route.  Without a workspace large enough for the carries the scan runs unsplit.  For tests and tuning.                    */
+int sigma_scan_fwd_split(const void *u, const void *delta, const float *A, const void *B, const void *C,
+                         const float *D, const float *delta_bias, void *out, float *x,
+                         int batch, int dim, int seqlen, int dstate, int ngroups, int dtype,
+                         int delta_softplus, const sigma_scan_strides *strides,
+                         void *workspace, size_t workspace_bytes, int nsplit, void *stream);
+
+/* Launch plan of the op-level selective scan, host only (no CUDA call, works without a GPU): what sweep 0 = sigma_scan_fwd{,_split},
+ * 1 = sigma_scan_bwd{,_split}, 2 = sigma_scan_bwd_det would launch at (batch, dim, seqlen, dstate, ngroups, dtype) with nsplit
+ * forced L-segments (0: the library's choice) and workspace_bytes of workspace, for contiguous 16-byte aligned operands, under
+ * the current environment (SIGMA_OP_GENERIC, SIGMA_OP_NST).  out8_host = {route (0 TMA-staged, 1 TMA-staged on fp32 copies of
+ * 16-bit operands, 2 generic), segments, position tiles per segment, position tiles, channels per CTA, ring stages, and for the
+ * backward the segments and tiles per segment of its state sweep (0 for the forward)}.  The generic backward runs one segment.
+ * Returns what the launch would: SIGMA_EWORKSPACE for a backward without its workspace.  For tests and tuning.                  */
+int sigma_test_scan_plan(int sweep, int batch, int dim, int seqlen, int dstate, int ngroups, int dtype, int nsplit,
+                         size_t workspace_bytes, int64_t *out8_host);
+
 /* ------------------------------------------------------------------------------------------
  * SURVEY.md §8(f) rank 2, first piece: the evaluator's per-batch metric on the device (eval.py:22-29,
  * utils/metric.py:8-15).  pred = argmax over classes of logits (batch, classes, H, W) — the index numpy.argmax

@@ -24,7 +24,8 @@ SIGNATURES = {
     "sigma_launch_count": (c_uint64, []),
     "sigma_scan_fwd_workspace_bytes": (c_size_t, [c_int] * 6),
     "sigma_scan_fwd": (c_int, [c_void_p] * 9 + [c_int] * 7 + [ctypes.POINTER(ScanStrides), c_void_p, c_size_t, c_void_p]),
-    "sigma_scan_fwd_f32_split": (c_int, [c_void_p] * 9 + [c_int] * 6 + [ctypes.POINTER(ScanStrides), c_void_p, c_size_t, c_int, c_void_p]),
+    "sigma_scan_fwd_split": (c_int, [c_void_p] * 9 + [c_int] * 7 + [ctypes.POINTER(ScanStrides), c_void_p, c_size_t, c_int, c_void_p]),
+    "sigma_test_scan_plan": (c_int, [c_int] * 8 + [c_size_t, ctypes.POINTER(c_int64)]),
     "sigma_scan_bwd_workspace_bytes": (c_size_t, [c_int] * 6),
     "sigma_scan_bwd": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_void_p, c_size_t, c_void_p]),
     "sigma_scan_bwd_split": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),

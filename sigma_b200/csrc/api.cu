@@ -55,6 +55,10 @@ int scan_op_bwd_generic(const void *u, const void *delta, const float *A, const 
 // scratch of the deterministic backward builds (det_ws != nullptr above)
 size_t scan_op_bwd_tma_det_bytes(int batch, int dim, int L, int N, int G);
 size_t scan_op_bwd_det_bytes(int batch, int dim, int L, int N, int G);
+// launch plans, host only: the launchers above plan through these very functions
+ScanOpPlan scan_op_fwd_generic_plan(int batch, int dim, int L, int N, int G, bool have_ws, int force_split);
+ScanOpPlan scan_op_fwd_tma_plan(int elem_bytes, int batch, int dim, int L, int N, int G, bool have_ws, int force_split);
+ScanOpPlan scan_op_bwd_tma_plan(int elem_bytes, int batch, int dim, int L, int N, int G, int force_split);
 
 // SIGMA_OP_GENERIC=1 forces the generic kernels (A/B timing, tests of the fallback on TMA-eligible shapes)
 static bool force_generic() {
@@ -131,17 +135,42 @@ static sigma_scan_strides contiguous_strides(int dim, int L, int N, int G) {
   return st;
 }
 
+// which kernels a call runs: TMA-staged, TMA-staged on widened fp32 copies of 16-bit operands, or generic
+enum { ROUTE_TMA = 0, ROUTE_WIDENED = 1, ROUTE_GENERIC = 2 };
+
+template <typename T>
+static int fwd_route(const void *u, const void *delta, const void *B, const void *C, const void *out, int batch, int dim, int L, int N,
+                     int G, const sigma_scan_strides &s, const void *ws, size_t ws_bytes) {
+  if (!force_generic() && scan_op_tma_eligible<T>(u, delta, B, C, out, dim, L, N, G, s)) return ROUTE_TMA;
+  if (sizeof(T) == 2 && !force_generic() && widen_shape_ok(dim, L, N, G, 2) && ws != nullptr &&
+      ws_bytes >= align256(scan_op_tma_workspace_bytes(batch, dim, N)) + widen_fwd_bytes(batch, dim, L, N, G) && s.A_dstate >= 0)
+    return ROUTE_WIDENED;
+  return ROUTE_GENERIC;
+}
+
+// `aligned`: dout / du / ddelta / dB / dC are 16-byte aligned (the other operands are checked by the eligibility test)
+template <typename T>
+static int bwd_route(bool aligned, const void *u, const void *delta, const void *B, const void *C, const void *du, int batch, int dim,
+                     int L, int N, int G, size_t ws_bytes) {
+  if (!force_generic() && aligned && scan_op_tma_eligible<T>(u, delta, B, C, du, dim, L, N, G, contiguous_strides(dim, L, N, G)))
+    return ROUTE_TMA;
+  if (sizeof(T) == 2 && !force_generic() && widen_shape_ok(dim, L, N, G, 2) &&
+      ws_bytes >= align256(scan_op_bwd_tma_workspace_bytes(batch, dim, L, N, 4)) + widen_bwd_bytes(batch, dim, L, N, G))
+    return ROUTE_WIDENED;
+  return ROUTE_GENERIC;
+}
+
 template <typename T>
 static int scan_fwd_dispatch(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
                              const float *bias, void *out, float *x, int batch, int dim, int L, int N, int G, int softplus,
                              const sigma_scan_strides &s, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream) {
-  if (!force_generic() && scan_op_tma_eligible<T>(u, delta, B, C, out, dim, L, N, G, s))
+  const int route = fwd_route<T>(u, delta, B, C, out, batch, dim, L, N, G, s, ws, ws_bytes);
+  if (route == ROUTE_TMA)
     return scan_op_fwd_tma<T>(u, delta, A, B, C, D, bias, out, x, nullptr, batch, dim, L, N, G, softplus, s, ws, ws_bytes,
                               force_split, stream);
   if constexpr (sizeof(T) == 2) {
     const size_t core = align256(scan_op_tma_workspace_bytes(batch, dim, N));
-    if (!force_generic() && widen_shape_ok(dim, L, N, G, 2) && ws != nullptr && ws_bytes >= core + widen_fwd_bytes(batch, dim, L, N, G) &&
-        s.A_dstate >= 0) {
+    if (route == ROUTE_WIDENED) {
       char *w = (char *)ws + core;
       const size_t bdl = align256((size_t)batch * dim * L * 4), bgn = align256((size_t)batch * G * N * L * 4);
       float *u32 = (float *)w, *d32 = (float *)(w + bdl), *o32 = (float *)(w + 2 * bdl), *B32 = (float *)(w + 3 * bdl), *C32 = (float *)(w + 3 * bdl + bgn);
@@ -168,12 +197,13 @@ static int scan_bwd_dispatch(const void *u, const void *delta, const float *A, c
                              size_t ws_bytes, int force_split, cudaStream_t stream, void *det_ws) {
   const sigma_scan_strides st = contiguous_strides(dim, L, N, G);
   const bool al = (((uintptr_t)dout | (uintptr_t)du | (uintptr_t)ddelta | (uintptr_t)dB | (uintptr_t)dC) & 15) == 0;
-  if (!force_generic() && al && scan_op_tma_eligible<T>(u, delta, B, C, du, dim, L, N, G, st))
+  const int route = bwd_route<T>(al, u, delta, B, C, du, batch, dim, L, N, G, ws_bytes);
+  if (route == ROUTE_TMA)
     return scan_op_bwd_tma<T>(u, delta, A, B, C, D, bias, dout, du, ddelta, dA, dB, dC, dD, dbias, batch, dim, L, N, G, softplus,
                               ws, ws_bytes, force_split, stream, det_ws);
   if constexpr (sizeof(T) == 2) {
     const size_t core = align256(scan_op_bwd_tma_workspace_bytes(batch, dim, L, N, 4));
-    if (!force_generic() && widen_shape_ok(dim, L, N, G, 2) && ws_bytes >= core + widen_bwd_bytes(batch, dim, L, N, G)) {
+    if (route == ROUTE_WIDENED) {
       char *w = (char *)ws + core;
       const size_t bdl = align256((size_t)batch * dim * L * 4), bgn = align256((size_t)batch * G * N * L * 4);
       float *u32 = (float *)w, *d32 = (float *)(w + bdl), *g32 = (float *)(w + 2 * bdl), *du32 = (float *)(w + 3 * bdl), *dd32 = (float *)(w + 4 * bdl);
@@ -192,6 +222,38 @@ static int scan_bwd_dispatch(const void *u, const void *delta, const float *A, c
   }
   return scan_op_bwd_generic<T>(u, delta, A, B, C, D, bias, dout, du, ddelta, dA, dB, dC, dD, dbias, batch, dim, L, N, G,
                                 softplus, ws, ws_bytes, stream, det_ws);
+}
+
+// sigma_test_scan_plan for element type T: the route and plans the dispatchers above would pick for contiguous, 16-byte aligned
+// operands and a workspace of ws_bytes.  sweep 0 = forward; 1 / 2 = backward / its deterministic build, whose kernels see
+// ws_bytes (the partials of the deterministic build follow it).  out = {route, segments, tiles per segment, tiles, channels per
+// CTA, ring stages, state-sweep segments, state-sweep tiles per segment}.
+template <typename T>
+static void scan_plan(int sweep, int batch, int dim, int L, int N, int G, int force_split, size_t ws_bytes, long long *out) {
+  const void *al = (const void *)(uintptr_t)256;   // stands for any 16-byte aligned pointer
+  const sigma_scan_strides st = contiguous_strides(dim, L, N, G);
+  const int eb = (int)sizeof(T);
+  ScanOpPlan main, state;
+  int route;
+  if (sweep == 0) {
+    route = fwd_route<T>(al, al, al, al, al, batch, dim, L, N, G, st, ws_bytes ? al : nullptr, ws_bytes);
+    if (route == ROUTE_GENERIC) main = scan_op_fwd_generic_plan(batch, dim, L, N, G, ws_bytes >= scan_op_workspace_bytes(batch, dim, N), force_split);
+    else main = scan_op_fwd_tma_plan(route == ROUTE_TMA ? eb : 4, batch, dim, L, N, G, ws_bytes >= scan_op_tma_workspace_bytes(batch, dim, N), force_split);
+    state.nsplit = state.tiles_per_split = 0;
+  } else {
+    route = bwd_route<T>(true, al, al, al, al, al, batch, dim, L, N, G, ws_bytes);
+    if (route == ROUTE_GENERIC) {
+      // one reverse walk per CTA after a serial state sweep (scan_op_bwd.cu): 32-position tiles, plain loads
+      main.ntiles = (L + 31) / 32; main.nsplit = 1; main.tiles_per_split = main.ntiles; main.DT = 32; main.nst = 1;
+      state = scan_op_fwd_generic_plan(batch, dim, L, N, G, false, 1);
+    } else {
+      const int e = route == ROUTE_TMA ? eb : 4;
+      main = scan_op_bwd_tma_plan(e, batch, dim, L, N, G, force_split);
+      state = scan_op_fwd_tma_plan(e, batch, dim, L, N, G, true, force_split);   // the workspace always holds its carries
+    }
+  }
+  const long long v[8] = {route, main.nsplit, main.tiles_per_split, main.ntiles, main.DT, main.nst, state.nsplit, state.tiles_per_split};
+  for (int i = 0; i < 8; ++i) out[i] = v[i];
 }
 
 }  // namespace sigma
@@ -213,11 +275,10 @@ size_t sigma_scan_fwd_workspace_bytes(int batch, int dim, int seqlen, int dstate
   return w;
 }
 
-int sigma_scan_fwd(const void *u, const void *delta, const float *A, const void *B, const void *C,
-                   const float *D, const float *delta_bias, void *out, float *x, int batch, int dim,
-                   int seqlen, int dstate, int ngroups, int dtype, int delta_softplus,
-                   const sigma_scan_strides *st, void *workspace, size_t workspace_bytes, void *stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
+static int scan_fwd_entry(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
+                          const float *delta_bias, void *out, float *x, int batch, int dim, int seqlen, int dstate, int ngroups,
+                          int dtype, int delta_softplus, const sigma_scan_strides *st, void *workspace, size_t workspace_bytes,
+                          int force_split, cudaStream_t stream) {
   SIGMA_CHECK_ARG(u && delta && A && B && C && out && st, "sigma_scan_fwd: null pointer argument");
   SIGMA_CHECK_ARG(batch > 0 && dim > 0 && seqlen > 0 && dstate > 0 && ngroups > 0,
                   "sigma_scan_fwd: non-positive size (batch=%d dim=%d seqlen=%d dstate=%d ngroups=%d)",
@@ -226,26 +287,57 @@ int sigma_scan_fwd(const void *u, const void *delta, const float *A, const void 
   SIGMA_CHECK_ARG(dim % ngroups == 0, "sigma_scan_fwd: dim=%d not divisible by ngroups=%d", dim, ngroups);
   SIGMA_CHECK_ARG(dtype == SIGMA_F32 || dtype == SIGMA_F16 || dtype == SIGMA_BF16,
                   "sigma_scan_fwd: unknown dtype %d", dtype);
+  SIGMA_CHECK_ARG(force_split >= 0, "sigma_scan_fwd_split: nsplit=%d < 0", force_split);
   if (dtype == SIGMA_F32)
     return scan_fwd_dispatch<float>(u, delta, A, B, C, D, delta_bias, out, x, batch, dim, seqlen, dstate, ngroups, delta_softplus,
-                                    *st, workspace, workspace_bytes, 0, stream);
+                                    *st, workspace, workspace_bytes, force_split, stream);
   if (dtype == SIGMA_F16)
     return scan_fwd_dispatch<__half>(u, delta, A, B, C, D, delta_bias, out, x, batch, dim, seqlen, dstate, ngroups, delta_softplus,
-                                     *st, workspace, workspace_bytes, 0, stream);
+                                     *st, workspace, workspace_bytes, force_split, stream);
   return scan_fwd_dispatch<__nv_bfloat16>(u, delta, A, B, C, D, delta_bias, out, x, batch, dim, seqlen, dstate, ngroups,
-                                          delta_softplus, *st, workspace, workspace_bytes, 0, stream);
+                                          delta_softplus, *st, workspace, workspace_bytes, force_split, stream);
 }
 
-// test hook (not part of the drop-in surface): force the number of L-segments of the fp32 op kernel
-int sigma_scan_fwd_f32_split(const float *u, const float *delta, const float *A, const float *B, const float *C,
-                             const float *D, const float *delta_bias, float *out, float *x, int batch, int dim,
-                             int seqlen, int dstate, int ngroups, int delta_softplus,
-                             const sigma_scan_strides *st, void *workspace, size_t workspace_bytes,
-                             int nsplit, void *stream) {
-  SIGMA_CHECK_ARG(u && delta && A && B && C && out && st, "sigma_scan_fwd_f32_split: null pointer argument");
-  SIGMA_CHECK_ARG(dim % ngroups == 0 && dstate <= 256, "sigma_scan_fwd_f32_split: bad dim/ngroups/dstate");
-  return scan_fwd_dispatch<float>(u, delta, A, B, C, D, delta_bias, out, x, batch, dim, seqlen, dstate, ngroups,
-                                  delta_softplus, *st, workspace, workspace_bytes, nsplit, (cudaStream_t)stream);
+int sigma_scan_fwd(const void *u, const void *delta, const float *A, const void *B, const void *C,
+                   const float *D, const float *delta_bias, void *out, float *x, int batch, int dim,
+                   int seqlen, int dstate, int ngroups, int dtype, int delta_softplus,
+                   const sigma_scan_strides *st, void *workspace, size_t workspace_bytes, void *stream_) {
+  return scan_fwd_entry(u, delta, A, B, C, D, delta_bias, out, x, batch, dim, seqlen, dstate, ngroups, dtype, delta_softplus, st,
+                        workspace, workspace_bytes, 0, (cudaStream_t)stream_);
+}
+
+// test hook: force the number of L-segments of the forward, any dtype and route (nsplit = 0: the library's choice)
+int sigma_scan_fwd_split(const void *u, const void *delta, const float *A, const void *B, const void *C,
+                         const float *D, const float *delta_bias, void *out, float *x, int batch, int dim,
+                         int seqlen, int dstate, int ngroups, int dtype, int delta_softplus,
+                         const sigma_scan_strides *st, void *workspace, size_t workspace_bytes, int nsplit, void *stream_) {
+  return scan_fwd_entry(u, delta, A, B, C, D, delta_bias, out, x, batch, dim, seqlen, dstate, ngroups, dtype, delta_softplus, st,
+                        workspace, workspace_bytes, nsplit, (cudaStream_t)stream_);
+}
+
+// the launch plan of the op-level scan, host only (see include/sigma_b200.h)
+int sigma_test_scan_plan(int sweep, int batch, int dim, int seqlen, int dstate, int ngroups, int dtype, int nsplit,
+                         size_t workspace_bytes, int64_t *out8_host) {
+  SIGMA_CHECK_ARG(out8_host && sweep >= 0 && sweep <= 2 && batch > 0 && dim > 0 && seqlen > 0 && dstate > 0 && dstate <= 256 &&
+                      ngroups > 0 && dim % ngroups == 0 && nsplit >= 0 &&
+                      (dtype == SIGMA_F32 || dtype == SIGMA_F16 || dtype == SIGMA_BF16),
+                  "sigma_test_scan_plan: bad arguments");
+  if (sweep > 0) {   // what scan_bwd_entry checks before it dispatches
+    if (dstate > 16) { set_error("sigma_scan_bwd: d_state=%d > 16 is not supported by the backward kernels", dstate); return SIGMA_EUNSUPPORTED; }
+    const size_t base = sigma_scan_bwd_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype);
+    const size_t need = sweep == 2 ? sigma_scan_bwd_det_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype) : base;
+    if (workspace_bytes < need) {
+      set_error("sigma_scan_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+      return SIGMA_EWORKSPACE;
+    }
+    if (sweep == 2) workspace_bytes = align256(base);
+  }
+  long long out[8];
+  if (dtype == SIGMA_F32) scan_plan<float>(sweep, batch, dim, seqlen, dstate, ngroups, nsplit, workspace_bytes, out);
+  else if (dtype == SIGMA_F16) scan_plan<__half>(sweep, batch, dim, seqlen, dstate, ngroups, nsplit, workspace_bytes, out);
+  else scan_plan<__nv_bfloat16>(sweep, batch, dim, seqlen, dstate, ngroups, nsplit, workspace_bytes, out);
+  for (int i = 0; i < 8; ++i) out8_host[i] = out[i];
+  return SIGMA_OK;
 }
 
 #pragma GCC visibility pop

@@ -41,6 +41,15 @@ void count_launch(int n = 1);
   } while (0)
 
 // ---- shared host-side parameter blocks ----
+// Launch plan of one op-level scan sweep (scan_op*.cu): what the launcher runs and what sigma_test_scan_plan reports.
+struct ScanOpPlan {
+  int nsplit;            // L-segments
+  int tiles_per_split;   // position tiles per segment
+  int ntiles;            // position tiles of the sequence
+  int DT;                // channels per CTA
+  int nst;               // ring / pipeline stages
+};
+
 struct RowNormParams {
   const float *y;          // K slabs
   long long k_stride;      // floats between slabs

@@ -338,31 +338,39 @@ static int launch_scan_op(ScanOpParams &p, cudaStream_t stream) {
   return SIGMA_OK;
 }
 
+constexpr int kGenMaxSplit = 64;   // the carry workspace holds this many segments per row (scan_op_workspace_bytes)
+
+// lanes per channel: d_state > 16 runs with up to 16 lanes per channel (8-16 states per lane) so that no instantiation spills
+static int pick_lpc(int NP) { return NP <= 4 ? 1 : (NP <= 8 ? 2 : (NP <= 32 ? 4 : (NP <= 128 ? NP / 8 : 16))); }
+
 // Decide how many L-segments to use.  Splitting doubles the exp work, so only do it when the
-// unsplit grid leaves most of the SMs idle.
-static void plan_split(ScanOpParams &p, int lpc, bool have_ws, int force_split) {
-  p.ntiles = (p.L + OP_LT - 1) / OP_LT;
-  const long long warps = (long long)p.batch * p.G * p.tiles_per_group * lpc;
+// unsplit grid leaves most of the SMs idle.  A forced count is capped like the automatic one.
+ScanOpPlan scan_op_fwd_generic_plan(int batch, int dim, int L, int N, int G, bool have_ws, int force_split) {
+  ScanOpPlan pl;
+  pl.ntiles = (L + OP_LT - 1) / OP_LT;
+  pl.DT = OP_DT;
+  pl.nst = OP_NST;
+  const long long warps = (long long)batch * G * ((dim / G + OP_DT - 1) / OP_DT) * pick_lpc(pick_npad(N));
   int nsplit = 1;
   const long long target = kNumSMs * 8;  // warps for a reasonably busy machine
-  if (warps * 3 < target) nsplit = (int)std::min<long long>((target + warps - 1) / warps, 64);
-  if (force_split > 0) nsplit = force_split;
+  if (warps * 3 < target) nsplit = (int)std::min<long long>((target + warps - 1) / warps, kGenMaxSplit);
+  if (force_split > 0) nsplit = std::min(force_split, kGenMaxSplit);
   if (!have_ws) nsplit = 1;
-  int tps = (p.ntiles + nsplit - 1) / nsplit;
+  int tps = (pl.ntiles + nsplit - 1) / nsplit;
   tps = std::max(tps, 1);
-  nsplit = (p.ntiles + tps - 1) / tps;
-  p.tiles_per_split = tps;
-  p.nsplit = std::max(nsplit, 1);
+  nsplit = (pl.ntiles + tps - 1) / tps;
+  pl.tiles_per_split = tps;
+  pl.nsplit = std::max(nsplit, 1);
+  return pl;
 }
 
 size_t scan_op_workspace_bytes(int batch, int dim, int dstate) {
-  return (size_t)batch * dim * 64 * 2 * pick_npad(dstate) * sizeof(float);
+  return (size_t)batch * dim * kGenMaxSplit * 2 * pick_npad(dstate) * sizeof(float);
 }
 
 int scan_op_npad(int N) { return pick_npad(N); }
 
 // `hs` (nullable): state at the start of every 32-position tile, (batch, dim, ntiles, NP) — forces a single pass.
-// d_state > 16 runs with up to 16 lanes per channel (8-16 states per lane) so that no instantiation spills.
 template <typename T>
 int scan_op_fwd_generic(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
                         const float *bias, void *out, float *x, float *hs, int batch, int dim, int L, int N, int G,
@@ -389,9 +397,11 @@ int scan_op_fwd_generic(const void *u, const void *delta, const float *A, const 
   p.vec_out = sizeof(T) == 4 && al16(out) && m4(p.o_b) && m4(p.o_d);
 
   const int NP = pick_npad(N);
-  const int lpc = NP <= 4 ? 1 : (NP <= 8 ? 2 : (NP <= 32 ? 4 : (NP <= 128 ? NP / 8 : 16)));
   const bool have_ws = ws != nullptr && ws_bytes >= scan_op_workspace_bytes(batch, dim, N);
-  plan_split(p, lpc, have_ws, force_split);
+  const ScanOpPlan pl = scan_op_fwd_generic_plan(batch, dim, L, N, G, have_ws, force_split);
+  p.ntiles = pl.ntiles;
+  p.nsplit = pl.nsplit;
+  p.tiles_per_split = pl.tiles_per_split;
 
   switch (NP) {
     case 4: return launch_scan_op<T, 4, 1>(p, stream);

@@ -490,6 +490,42 @@ size_t scan_op_bwd_tma_workspace_bytes(int batch, int dim, int L, int N, int ele
          al256((size_t)batch * dim * kBwdMaxSplit * 2 * N * sizeof(float));
 }
 
+template <typename T>
+static ScanOpPlan bwd_tma_plan(int batch, int dim, int L, int N, int G, int force_split) {
+  constexpr int LT = OpT<T>::LT;
+  const int NP = N, dpg = dim / G;
+  ScanOpPlan pl;
+  pl.DT = (dpg % 64 == 0) ? 64 : 32;
+  pl.ntiles = (L + LT - 1) / LT;
+  // L-segments: the reverse summaries are a cheap extra sweep (no h, no reductions: ~0.3 of the main sweep), so fill whole
+  // waves of the resident CTA slots (2 x 128-thread CTAs per SM at d_state 16, ~5 x 64-thread CTAs below)
+  const int lpc = NP >= 16 ? 2 : 1;
+  int nsplit = pick_segments((long long)batch * G * (dpg / pl.DT), pl.ntiles, kNumSMs * (lpc == 2 ? 2 : 5), 1.3, kBwdMaxSplit);
+  if (force_split > 0) nsplit = std::min(force_split, kBwdMaxSplit);
+  int tps = std::max(1, (pl.ntiles + nsplit - 1) / nsplit);
+  pl.tiles_per_split = tps;
+  pl.nsplit = std::max(1, (pl.ntiles + tps - 1) / tps);
+  {
+    const size_t stage = (size_t)3 * pl.DT * OPT_ROW_BYTES + (size_t)2 * NP * OPT_ROW_BYTES;
+    const size_t budget = (size_t)(227 * 1024) / (lpc == 2 ? 2 : 4) - 1024;   // 2 x 128-thread / 4 x 64-thread CTAs per SM
+    size_t base;
+    switch (NP) {
+      case 4: base = bwd_tma_smem_bytes<T, 4>(pl.DT, 0); break;
+      case 8: base = bwd_tma_smem_bytes<T, 8>(pl.DT, 0); break;
+      default: base = bwd_tma_smem_bytes<T, 16>(pl.DT, 0); break;
+    }
+    int nst = budget > base ? (int)((budget - base) / stage) : 2;
+    pl.nst = std::max(2, std::min(4, nst));
+  }
+  return pl;
+}
+
+// Launch plan of the main (reverse) sweep of scan_op_bwd_tma (host only; eligibility guarantees N in {4, 8, 16}).  Its state
+// sweep is scan_op_fwd_tma with the same force_split and the forward-carry part of the workspace (scan_op_fwd_tma_plan).
+ScanOpPlan scan_op_bwd_tma_plan(int elem_bytes, int batch, int dim, int L, int N, int G, int force_split) {
+  return elem_bytes == 4 ? bwd_tma_plan<float>(batch, dim, L, N, G, force_split) : bwd_tma_plan<__half>(batch, dim, L, N, G, force_split);
+}
+
 template <typename T, int NP>
 static int launch_bwd_tma(ScanBwdTmaParams &p, cudaStream_t stream) {
   constexpr int LPC = BwdCfg<NP>::LPC;
@@ -577,30 +613,15 @@ int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void
     p.part_B = (float *)w; p.part_C = (float *)(w + bc); p.part_dA = (float *)(w + 2 * bc);
     p.part_dD = (float *)(w + 2 * bc + da); p.part_db = (float *)(w + 2 * bc + da + dd);
   }
-  p.DT = (p.dpg % 64 == 0) ? 64 : 32;
+  const ScanOpPlan pl = scan_op_bwd_tma_plan((int)sizeof(T), batch, dim, L, N, G, force_split);
+  p.DT = pl.DT;
   p.ctiles_per_group = p.dpg / p.DT;
   p.ntiles = ntiles;
   p.nhs = (L + OPT_HS_POS - 1) / OPT_HS_POS;
-  // L-segments: the reverse summaries are a cheap extra sweep (no h, no reductions: ~0.3 of the main sweep), so fill whole
-  // waves of the resident CTA slots (2 x 128-thread CTAs per SM at d_state 16, ~5 x 64-thread CTAs below)
-  const int lpc = NP >= 16 ? 2 : 1;
-  int nsplit = pick_segments((long long)batch * G * p.ctiles_per_group, ntiles, kNumSMs * (lpc == 2 ? 2 : 5), 1.3, kBwdMaxSplit);
-  if (force_split > 0) nsplit = std::min(force_split, kBwdMaxSplit);
-  int tps = std::max(1, (ntiles + nsplit - 1) / nsplit);
-  p.tiles_per_split = tps;
-  p.nsplit = std::max(1, (ntiles + tps - 1) / tps);
-  {
-    const size_t stage = (size_t)3 * p.DT * OPT_ROW_BYTES + (size_t)2 * NP * OPT_ROW_BYTES;
-    const size_t budget = (size_t)(227 * 1024) / (lpc == 2 ? 2 : 4) - 1024;   // 2 x 128-thread / 4 x 64-thread CTAs per SM
-    size_t base;
-    switch (NP) {
-      case 4: base = bwd_tma_smem_bytes<T, 4>(p.DT, 0); break;
-      case 8: base = bwd_tma_smem_bytes<T, 8>(p.DT, 0); break;
-      default: base = bwd_tma_smem_bytes<T, 16>(p.DT, 0); break;
-    }
-    int nst = budget > base ? (int)((budget - base) / stage) : 2;
-    p.nst = std::max(2, std::min(4, nst));
-  }
+  p.tiles_per_split = pl.tiles_per_split;
+  p.nsplit = pl.nsplit;
+  p.nst = pl.nst;
+  const int lpc = NP >= 16 ? 2 : 1;   // lanes per channel (BwdCfg)
   const uint64_t sz = sizeof(T);
   {
     uint64_t dims[3] = {(uint64_t)L, (uint64_t)dim, (uint64_t)batch};

@@ -361,6 +361,44 @@ static int launch_tma(ScanTmaParams &p, bool yout, cudaStream_t stream) {
   return yout ? run(scan_op_tma_kernel<T, NP, MODE_APPLY, true>) : run(scan_op_tma_kernel<T, NP, MODE_APPLY, false>);
 }
 
+// Launch plan of scan_op_fwd_tma (host only; eligibility guarantees N in {4, 8, 16} and dim / G a multiple of 32).  16-bit
+// elements have 32-position tiles, fp32 16-position ones.
+ScanOpPlan scan_op_fwd_tma_plan(int elem_bytes, int batch, int dim, int L, int N, int G, bool have_ws, int force_split) {
+  const int LT = elem_bytes == 4 ? OpT<float>::LT : OpT<__half>::LT, NP = N, dpg = dim / G;
+  ScanOpPlan pl;
+  // channels per CTA: the largest of 128 / 96 / 64 / 32 that divides the group
+  pl.DT = 32;
+  for (int w = 4; w >= 1; --w)
+    if (dpg % (32 * w) == 0) { pl.DT = 32 * w; break; }
+  pl.ntiles = (L + LT - 1) / LT;
+
+  // L-segments (MODE_SUMMARY -> combine -> MODE_APPLY).  Model: a
+  // tile costs about the same 3-5 us whether 1 or 3 warps share an SM sub-partition (latency-bound alone, MUFU-bound together),
+  // so time ~ waves x tiles-per-segment x passes: pick the segment count that minimises that, i.e. fills whole waves of the
+  // resident CTA slots.  Segments need not end on the 2048-position chunk boundaries of `x`: a segment that crosses one writes
+  // that chunk's state itself (true h, prefix product = carry-in x local).
+  const long long ctas_base = (long long)batch * G * (dpg / pl.DT);
+  int nsplit = pick_segments(ctas_base, pl.ntiles, kNumSMs * (N >= 16 ? 3 : 4) * 4 / (pl.DT / 32), 2.2, kOpMaxSplit);
+  if (force_split > 0) nsplit = std::min(force_split, kOpMaxSplit);
+  if (!have_ws) nsplit = 1;
+  const int tps = std::max(1, (pl.ntiles + nsplit - 1) / nsplit);
+  pl.tiles_per_split = tps;
+  pl.nsplit = std::max(1, (pl.ntiles + tps - 1) / tps);
+
+  // ring depth: what fits next to the other resident CTAs
+  {
+    const int nw = pl.DT / 32;
+    const int regs_ctas = std::min(NP >= 16 ? 12 / nw : 16 / nw, 16);          // 12 / 16 resident warps per SM by registers
+    const size_t budget = (size_t)(227 * 1024) / std::max(1, regs_ctas) - 1024;
+    const size_t stage = (size_t)2 * pl.DT * OPT_ROW_BYTES + (size_t)2 * NP * OPT_ROW_BYTES;
+    const size_t fixed = 1024 + 256 + (size_t)nw * LT * (2 * NP + 4) * sizeof(float);
+    int nst = budget > fixed ? (int)((budget - fixed) / stage) : 2;
+    pl.nst = std::max(3, std::min(8, nst));   // >= 3: a slot is released one tile after its last use
+    if (const char *e = getenv("SIGMA_OP_NST")) pl.nst = std::max(3, std::min(8, atoi(e)));
+  }
+  return pl;
+}
+
 // `hs` (nullable): state at the start of every OPT_HS_POS positions, (batch, dim, ceil(L / OPT_HS_POS), NP) fp32.  out == nullptr: state-only
 // sweep (no y), the first half of the backward.
 template <typename T>
@@ -374,39 +412,16 @@ int scan_op_fwd_tma(const void *u, const void *delta, const float *A, const void
   p.A = A; p.D = D; p.bias = bias; p.x = x; p.hs = hs; p.carry = (float *)ws;
   p.A_d = s.A_dim; p.A_n = s.A_dstate;
   p.batch = batch; p.dim = dim; p.L = L; p.N = N; p.G = G; p.dpg = dim / G; p.softplus = softplus;
-  // channels per CTA: the largest of 128 / 96 / 64 / 32 that divides the group
-  p.DT = 32;
-  for (int w = 4; w >= 1; --w)
-    if (p.dpg % (32 * w) == 0) { p.DT = 32 * w; break; }
+  const bool have_ws = ws != nullptr && ws_bytes >= scan_op_tma_workspace_bytes(batch, dim, N);
+  const ScanOpPlan pl = scan_op_fwd_tma_plan((int)sizeof(T), batch, dim, L, N, G, have_ws, force_split);
+  p.DT = pl.DT;
   p.ctiles_per_group = p.dpg / p.DT;
-  p.ntiles = (L + LT - 1) / LT;
+  p.ntiles = pl.ntiles;
   p.nchunks = (L + 2047) / 2048;
   p.nhs = (L + OPT_HS_POS - 1) / OPT_HS_POS;
-
-  // L-segments (MODE_SUMMARY -> combine -> MODE_APPLY).  Model: a
-  // tile costs about the same 3-5 us whether 1 or 3 warps share an SM sub-partition (latency-bound alone, MUFU-bound together),
-  // so time ~ waves x tiles-per-segment x passes: pick the segment count that minimises that, i.e. fills whole waves of the
-  // resident CTA slots.  Segments need not end on the 2048-position chunk boundaries of `x`: a segment that crosses one writes
-  // that chunk's state itself (true h, prefix product = carry-in x local).
-  const long long ctas_base = (long long)batch * G * p.ctiles_per_group;
-  int nsplit = pick_segments(ctas_base, p.ntiles, kNumSMs * (N >= 16 ? 3 : 4) * 4 / (p.DT / 32), 2.2, kOpMaxSplit);
-  if (force_split > 0) nsplit = std::min(force_split, kOpMaxSplit);
-  if (ws == nullptr || ws_bytes < scan_op_tma_workspace_bytes(batch, dim, N)) nsplit = 1;
-  const int tps = std::max(1, (p.ntiles + nsplit - 1) / nsplit);
-  p.tiles_per_split = tps;
-  p.nsplit = std::max(1, (p.ntiles + tps - 1) / tps);
-
-  // ring depth: what fits next to the other resident CTAs
-  {
-    const int nw = p.DT / 32;
-    const int regs_ctas = std::min(NP >= 16 ? 12 / nw : 16 / nw, 16);          // 12 / 16 resident warps per SM by registers
-    const size_t budget = (size_t)(227 * 1024) / std::max(1, regs_ctas) - 1024;
-    const size_t stage = (size_t)2 * p.DT * OPT_ROW_BYTES + (size_t)2 * NP * OPT_ROW_BYTES;
-    const size_t fixed = 1024 + 256 + (size_t)nw * LT * (2 * NP + 4) * sizeof(float);
-    int nst = budget > fixed ? (int)((budget - fixed) / stage) : 2;
-    p.nst = std::max(3, std::min(8, nst));   // >= 3: a slot is released one tile after its last use
-    if (const char *e = getenv("SIGMA_OP_NST")) p.nst = std::max(3, std::min(8, atoi(e)));
-  }
+  p.tiles_per_split = pl.tiles_per_split;
+  p.nsplit = pl.nsplit;
+  p.nst = pl.nst;
 
   const uint64_t sz = sizeof(T);
   int rc;

@@ -76,10 +76,10 @@ def selective_scan_cuda_core_fwd(u, delta, A, B, C, D=None, delta_bias=None, del
     dt = _DTYPE[u.dtype]
     wsb = L_.sigma_scan_fwd_workspace_bytes(batch, dim, L, N, G, dt)
     ws = torch.empty(wsb, dtype=torch.uint8, device=u.device)
-    if _force_split and dt == _lib.F32:  # the split hook is fp32-only
-        rc = L_.sigma_scan_fwd_f32_split(_ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C), _ptr(D), _ptr(delta_bias),
-                                         _ptr(out), _ptr(x), batch, dim, L, N, G, int(bool(delta_softplus)),
-                                         ctypes.byref(st), _ptr(ws), wsb, int(_force_split), _stream())
+    if _force_split:
+        rc = L_.sigma_scan_fwd_split(_ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C), _ptr(D), _ptr(delta_bias),
+                                     _ptr(out), _ptr(x), batch, dim, L, N, G, dt, int(bool(delta_softplus)),
+                                     ctypes.byref(st), _ptr(ws), wsb, int(_force_split), _stream())
     else:
         rc = L_.sigma_scan_fwd(_ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C), _ptr(D), _ptr(delta_bias),
                                _ptr(out), _ptr(x), batch, dim, L, N, G, dt, int(bool(delta_softplus)),

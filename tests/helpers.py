@@ -64,7 +64,7 @@ def sample_index(key, numel, k):
 
 # ---- the fused SS2D scan through its C-ABI (the fp64 tests of its forward and backward) ----
 SS2D_GUARD = 64                          # guard elements on each side of every output (keeps 16-byte alignment)
-_NAN_BITS = {torch.float32: (torch.int32, 0x7FC00000), torch.bfloat16: (torch.int16, 0x7FC0)}
+_NAN_BITS = {torch.float32: (torch.int32, 0x7FC00000), torch.bfloat16: (torch.int16, 0x7FC0), torch.float16: (torch.int16, 0x7E00)}
 
 
 def ptr(t):
@@ -123,6 +123,60 @@ def ss2d_params(seed, kind, B, H, W, D, N, R, tag, wide=False):
     Ds = P.randn(seed, tag + "/Ds", (Kw * D,), 0.1, 1.0)
     dy = P.randn(seed, tag + "/dy", (B, Lseq, D))
     return [t.cuda() for t in (xc, xdbl, dtw, dtb, A, Ds, dy)], Cp
+
+
+def op_scan_params(seed, batch, dim, L, N, G, tag, dist="sigma", dtype=torch.float32, has_D=True, has_bias=True, softplus=True):
+    """inputs of the op-level scan, on the CPU: [u, delta, A, B, C, D, delta_bias, dout]; u / delta / B / C / dout in `dtype`.
+    dist "sigma": delta = a small dt_proj-like term (0.5·randn) + delta_bias, delta_bias = the inverse softplus of dt log-uniform
+    in [1e-3, 0.1] per channel (folded into delta when has_bias is False); A = -exp(A_log) around the S4D-real init; D near 1.
+    "wide": dt up to 0.5, |A| up to 4x.  Without softplus, delta' = delta (+ bias) must be a step itself: dt · exp(0.3·randn).
+    "ref": the reference test's distribution (procedural.scan_inputs: delta, bias in [0, 0.5), A in [-0.5, 0])."""
+    import math
+    import procedural as P
+    if dist == "ref":
+        u, delta, A, B, C, D, bias = P.scan_inputs(seed, batch, dim, N, L, G, dtype, has_D, has_bias)
+        dout = P.randn(seed, tag + "/dout", (batch, dim, L)).to(dtype)
+        return [u, delta, A, B, C, D, bias, dout]
+    wide = dist == "wide"
+    dt = torch.exp(P.rand(seed, tag + "/dt", (dim,), math.log(1e-3), math.log(0.5 if wide else 0.1)))
+    if softplus:
+        isp = dt + torch.log(-torch.expm1(-dt))                          # inverse softplus
+        delta = 0.5 * P.randn(seed, tag + "/delta", (batch, dim, L)) + (0.0 if has_bias else isp[:, None])
+        bias = isp if has_bias else None
+    else:
+        delta = dt[:, None] * torch.exp(0.3 * P.randn(seed, tag + "/delta", (batch, dim, L)))
+        bias = 0.1 * dt if has_bias else None
+    A_log = torch.log(torch.arange(1, N + 1, dtype=torch.float32)).repeat(dim, 1) + P.rand(seed, tag + "/A", (dim, N), -0.2,
+                                                                                            1.4 if wide else 0.2)
+    A = -torch.exp(A_log)
+    D = P.randn(seed, tag + "/D", (dim,), 0.1, 1.0) if has_D else None
+    u = P.randn(seed, tag + "/u", (batch, dim, L))
+    B = P.randn(seed, tag + "/B", (batch, G, N, L))
+    C = P.randn(seed, tag + "/C", (batch, G, N, L))
+    dout = P.randn(seed, tag + "/dout", (batch, dim, L))
+    return [t.to(dtype) if i in (0, 1, 3, 4, 7) else t for i, t in enumerate((u, delta, A, B, C, D, bias, dout))]
+
+
+SCAN_PLAN = ("route", "nsplit", "tiles_per_split", "ntiles", "channels", "stages", "state_nsplit", "state_tiles_per_split")
+SCAN_ROUTES = ("tma", "widened", "generic")
+_SCAN_SWEEPS = {"fwd": 0, "bwd": 1, "bwd_det": 2}
+
+
+def scan_plan(sweep, batch, dim, L, N, G, dtype=torch.float32, nsplit=0, ws_bytes=None):
+    """The launch plan the op-level scan would use (sigma_test_scan_plan), route as a name.  sweep "fwd" / "bwd" / "bwd_det";
+    ws_bytes: the workspace the call gets (None: what sigma_b200.ops allocates, 0: none)."""
+    import ctypes
+    from sigma_b200 import _lib
+    L_ = _lib.lib()
+    dt = {torch.float32: _lib.F32, torch.float16: _lib.F16, torch.bfloat16: _lib.BF16}[dtype]
+    if ws_bytes is None:
+        ws_bytes = {"fwd": L_.sigma_scan_fwd_workspace_bytes, "bwd": L_.sigma_scan_bwd_workspace_bytes,
+                    "bwd_det": L_.sigma_scan_bwd_det_workspace_bytes}[sweep](batch, dim, L, N, G, dt)
+    out = (ctypes.c_int64 * 8)()
+    _lib.check(L_.sigma_test_scan_plan(_SCAN_SWEEPS[sweep], batch, dim, L, N, G, dt, nsplit, ws_bytes, out), "sigma_test_scan_plan")
+    plan = dict(zip(SCAN_PLAN, (int(v) for v in out)))
+    plan["route"] = SCAN_ROUTES[plan["route"]]
+    return plan
 
 
 SS2D_FWD_PLAN = ("nsplit", "tiles_per_split", "max_tiles", "min_tiles", "warps", "nst", "ctas", "smem")

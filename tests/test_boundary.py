@@ -30,7 +30,7 @@ def test_library_exports_every_declared_symbol(lib_path):
     assert declared, "no declarations parsed"
     assert declared <= exported, f"declared but not exported: {sorted(declared - exported)}"
     extra = {s for s in exported - declared if s.startswith("sigma_")}
-    assert extra <= {"sigma_scan_fwd_f32_split", "sigma_scan_bwd_split", "sigma_ss2d_scan_fwd_split", "sigma_ss2d_scan_bwd_split",
+    assert extra <= {"sigma_scan_bwd_split", "sigma_ss2d_scan_fwd_split", "sigma_ss2d_scan_bwd_split",
                      "sigma_test_pick_segments", "sigma_test_pick_bn"}, f"undeclared exports: {sorted(extra)}"
 
 

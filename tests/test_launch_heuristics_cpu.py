@@ -311,3 +311,69 @@ def test_ss2d_fwd_plan_rejects_bad_arguments(L):
     assert L.sigma_test_ss2d_fwd_plan(0, 1, 15, 20, 1536, 12, 48, 0, 0, 1 << 30, out) != 0     # d_state
     assert L.sigma_test_ss2d_fwd_plan(0, 1, 15, 20, 1536, 16, 65, 0, 0, 1 << 30, out) != 0     # dt_rank
     assert L.sigma_test_ss2d_fwd_plan(0, 1, 15, 20, 1536, 16, 48, 0, -1, 1 << 30, out) != 0
+
+
+# ---- the op-level selective scan's launch plan (sigma_test_scan_plan): the routes, the 64-segment cap on every route, the
+# segments covering the tiles, and the backward's two sweeps.  (batch, dim, L, N, G) of Sigma's calls and a few ragged ones.
+OP_SHAPES = [(2, 192, 19200, 4, 1), (2, 384, 4800, 4, 1), (2, 768, 1200, 4, 1), (2, 1536, 300, 4, 1), (1, 256, 43200, 4, 1),
+             (1, 2048, 690, 4, 1), (2, 768, 19200, 16, 4), (2, 6144, 300, 16, 4), (2, 384, 38400, 4, 2), (3, 64, 1001, 8, 2),
+             (1, 96, 77, 16, 1), (2, 40, 500, 4, 1)]
+
+
+def test_op_scan_plan_routes(monkeypatch):
+    import torch
+    from helpers import scan_plan
+    monkeypatch.delenv("SIGMA_OP_GENERIC", raising=False)
+    for sweep in ("fwd", "bwd", "bwd_det"):
+        assert scan_plan(sweep, 1, 2048, 690, 4, 1)["route"] == "generic"                  # fp32 rows of 690 are not 16-byte aligned
+        for dt in (torch.float16, torch.bfloat16):
+            assert scan_plan(sweep, 2, 1536, 300, 4, 1, dt)["route"] == "widened"            # 16-bit rows of 300: fp32 copies are
+            assert scan_plan(sweep, 2, 192, 19200, 4, 1, dt)["route"] == "tma"
+            assert scan_plan(sweep, 1, 2048, 690, 4, 1, dt)["route"] == "generic"
+        assert scan_plan(sweep, 2, 768, 19200, 16, 4)["route"] == "tma"
+        assert scan_plan(sweep, 2, 40, 500, 4, 1)["route"] == "generic"                     # channel groups not a multiple of 32
+    assert scan_plan("fwd", 2, 1536, 300, 4, 1, torch.bfloat16, ws_bytes=0)["route"] == "generic"   # widening needs scratch
+    monkeypatch.setenv("SIGMA_OP_GENERIC", "1")
+    for sweep in ("fwd", "bwd"):
+        assert scan_plan(sweep, 2, 192, 19200, 4, 1)["route"] == "generic"
+    p = scan_plan("fwd", 2, 192, 19200, 4, 1, nsplit=100)                                     # the generic forward's cap
+    assert p["nsplit"] <= 64 and p["tiles_per_split"] == -(-p["ntiles"] // 64) == 10, p
+
+
+def test_op_scan_plan_segments(monkeypatch):
+    import torch
+    from helpers import scan_plan
+    for generic in ("0", "1"):
+        monkeypatch.setenv("SIGMA_OP_GENERIC", generic)
+        for shape in OP_SHAPES:
+            for dt in (torch.float32, torch.bfloat16):
+                for sweep in ("fwd", "bwd", "bwd_det"):
+                    if sweep != "fwd" and shape[3] > 16:
+                        continue
+                    for ns in (0, 1, 2, 7, 64, 100):
+                        p = scan_plan(sweep, *shape, dt, nsplit=ns)
+                        what = (generic, shape, dt, sweep, ns, p)
+                        assert 1 <= p["nsplit"] <= 64, what
+                        assert p["nsplit"] * p["tiles_per_split"] >= p["ntiles"] > (p["nsplit"] - 1) * p["tiles_per_split"], what
+                        seg = not (sweep != "fwd" and p["route"] == "generic")
+                        if ns == 1 or not seg:
+                            assert p["nsplit"] == 1, what                                    # the generic backward has no segments
+                        if ns == 100 and seg:
+                            assert p["tiles_per_split"] == -(-p["ntiles"] // 64), what
+                        if sweep == "fwd":
+                            assert p["state_nsplit"] == 0, what
+                            continue
+                        # the state sweep: the forward planner with the same forced count (its own choice at nsplit = 0)
+                        assert 1 <= p["state_nsplit"] <= 64, what
+                        if not seg:
+                            assert p["state_nsplit"] == 1, what
+                        elif ns:
+                            f = scan_plan("fwd", *shape, dt if p["route"] == "tma" else torch.float32, nsplit=ns, ws_bytes=1 << 40)
+                            assert (p["state_nsplit"], p["state_tiles_per_split"]) == (f["nsplit"], f["tiles_per_split"]), what
+    monkeypatch.delenv("SIGMA_OP_GENERIC")
+    # no workspace: one segment whatever is asked; a backward without its workspace is refused as the launch would be
+    assert scan_plan("fwd", 2, 192, 19200, 4, 1, nsplit=7, ws_bytes=0)["nsplit"] == 1
+    with pytest.raises(RuntimeError):
+        scan_plan("bwd", 2, 192, 19200, 4, 1, ws_bytes=0)
+    # the drop-in CroMB stage-0 call runs L-segments by default, forward and backward
+    assert scan_plan("fwd", 2, 192, 19200, 4, 1)["nsplit"] > 1 and scan_plan("bwd", 2, 192, 19200, 4, 1)["nsplit"] > 1
