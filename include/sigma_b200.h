@@ -289,7 +289,7 @@ int sigma_linear_tf32(const float *A, int64_t lda, const float *W, const float *
                       const float *rscale, float *C, int64_t ldc, int64_t M, int N, int K, void *stream);
 
 /* The same GEMM with fp32-GRADE products on the TF32 tensor pipe ("tf32x3": A·W = A_hi·W_hi + A_lo·W_hi + A_hi·W_lo, x_hi = x with
- * the low 13 mantissa bits cleared; three wgmma MMAs per k-step, activations split in shared memory inside the kernel): what
+ * the low 13 mantissa bits cleared; three wgmma MMAs per k-step, activations split in registers inside the kernel): what
  * torch's nn.Linear computes with torch.backends.cuda.matmul.allow_tf32 = False, to ~1e-6 relative.  The weights arrive
  * pre-split (W_hi, W_lo each (N, K) contiguous): split them once with sigma_split_tf32_fwd.                                  */
 int sigma_linear_tf32x3(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias, const float *residual,
@@ -351,6 +351,31 @@ int sigma_scan_fwd_split(const void *u, const void *delta, const float *A, const
  * Returns what the launch would: SIGMA_EWORKSPACE for a backward without its workspace.  For tests and tuning.                  */
 int sigma_test_scan_plan(int sweep, int batch, int dim, int seqlen, int dstate, int ngroups, int dtype, int nsplit,
                          size_t workspace_bytes, int64_t *out8_host);
+
+/* ------------------------------------------------------------------------------------------
+ * Test hooks: the scans with a forced number of L-segments, and the launch heuristics alone.  For tests and tuning.
+ * ------------------------------------------------------------------------------------------ */
+/* sigma_scan_bwd with a forced number of L-segments (nsplit = 0: the library's choice; more than 64 is capped at 64).  The generic
+ * backward runs one segment.                                                                                                   */
+int sigma_scan_bwd_split(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
+                         const float *delta_bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC,
+                         float *dD, float *ddelta_bias, int batch, int dim, int seqlen, int dstate, int ngroups, int dtype,
+                         int delta_softplus, void *workspace, size_t workspace_bytes, int nsplit, void *stream);
+/* sigma_ss2d_scan_fwd with a forced number of L-segments (nsplit = 0: the library's choice; capped at 32 and at the tile count of
+ * the longest walk).  nsplit > 1 without a large enough workspace is SIGMA_EWORKSPACE.                                         */
+int sigma_ss2d_scan_fwd_split(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                              const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                              size_t workspace_bytes, int nsplit, void *stream);
+/* sigma_ss2d_scan_bwd with a forced number of L-segments (nsplit = 0: the library's choice; capped at 64 and at the tile count of
+ * the longest walk).                                                                                                           */
+int sigma_ss2d_scan_bwd_split(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                              const float *Ds, const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA,
+                              float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                              size_t workspace_bytes, int nsplit, void *stream);
+/* Host only (no CUDA call, works without a GPU): the L-segment count the fused scan forward picks for a grid of `ctas` CTAs of
+ * warps_per_cta warps walking ntiles tiles at d_state N, and the GEMM tile width for N output columns and m_tiles 128-row tiles. */
+int sigma_test_pick_segments(int64_t ctas, int warps_per_cta, int ntiles, int N);
+int sigma_test_pick_bn(int N, int64_t m_tiles);
 
 /* ------------------------------------------------------------------------------------------
  * SURVEY.md §8(f) rank 2, first piece: the evaluator's per-batch metric on the device (eval.py:22-29,

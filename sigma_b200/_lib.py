@@ -2,7 +2,10 @@
 library is missing or a call fails, a RuntimeError carrying sigma_last_error() is raised."""
 import ctypes
 import os
+import re
 from ctypes import c_char_p, c_double, c_float, c_int, c_int64, c_size_t, c_uint64, c_void_p
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsigma_b200.so")
@@ -17,69 +20,36 @@ class ScanStrides(ctypes.Structure):
         "B_batch", "B_group", "B_dstate", "C_batch", "C_group", "C_dstate", "out_batch", "out_dim")]
 
 
-# name -> (restype, argtypes); mirrors include/sigma_b200.h declaration by declaration
-SIGNATURES = {
-    "sigma_abi_version": (c_int, []),
-    "sigma_last_error": (c_char_p, []),
-    "sigma_launch_count": (c_uint64, []),
-    "sigma_scan_fwd_workspace_bytes": (c_size_t, [c_int] * 6),
-    "sigma_scan_fwd": (c_int, [c_void_p] * 9 + [c_int] * 7 + [ctypes.POINTER(ScanStrides), c_void_p, c_size_t, c_void_p]),
-    "sigma_scan_fwd_split": (c_int, [c_void_p] * 9 + [c_int] * 7 + [ctypes.POINTER(ScanStrides), c_void_p, c_size_t, c_int, c_void_p]),
-    "sigma_test_scan_plan": (c_int, [c_int] * 8 + [c_size_t, ctypes.POINTER(c_int64)]),
-    "sigma_scan_bwd_workspace_bytes": (c_size_t, [c_int] * 6),
-    "sigma_scan_bwd": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_void_p, c_size_t, c_void_p]),
-    "sigma_scan_bwd_split": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
-    "sigma_ss2d_padded_cp": (c_int, [c_int, c_int]),
-    "sigma_ss2d_scan_workspace_bytes": (c_size_t, [c_int] * 6),
-    "sigma_ss2d_scan_fwd": (c_int, [c_int] + [c_void_p] * 7 + [c_int] * 7 + [c_void_p, c_size_t, c_void_p]),
-    "sigma_ss2d_scan_fwd_split": (c_int, [c_int] + [c_void_p] * 7 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
-    "sigma_ss2d_scan_bwd_workspace_bytes": (c_size_t, [c_int] * 6),
-    "sigma_ss2d_scan_hs_bytes": (c_size_t, [c_int] * 6),
-    "sigma_test_pick_segments": (c_int, [c_int64, c_int, c_int, c_int]),
-    "sigma_test_pick_bn": (c_int, [c_int, c_int64]),
-    "sigma_test_gemm_plan": (c_int, [c_int64, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int64)]),
-    "sigma_test_ss2d_bwd_plan": (c_int, [c_int] * 7 + [ctypes.POINTER(c_int64)]),
-    "sigma_test_ss2d_fwd_plan": (c_int, [c_int] * 9 + [c_size_t, ctypes.POINTER(c_int64)]),
-    "sigma_ss2d_scan_fwd_save": (c_int, [c_int] + [c_void_p] * 9 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
-    "sigma_ss2d_scan_bwd_saved": (c_int, [c_int] + [c_void_p] * 15 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
-    "sigma_ss2d_scan_bwd": (c_int, [c_int] + [c_void_p] * 14 + [c_int] * 7 + [c_void_p, c_size_t, c_void_p]),
-    "sigma_ss2d_scan_bwd_split": (c_int, [c_int] + [c_void_p] * 14 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
-    "sigma_layernorm_fwd": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_float, c_void_p]),
-    "sigma_layernorm_bwd": (c_int, [c_void_p] * 6 + [c_int64, c_int, c_float, c_void_p]),
-    "sigma_dwconv3x3_silu_fwd": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64] + [c_int] * 4 + [c_void_p]),
-    "sigma_merge_norm_gate_fwd": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
-                                          c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_float, c_void_p]),
-    "sigma_upsample2x_norm_fwd": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_float, c_void_p]),
-    "sigma_argmax_hist_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p]),
-    "sigma_patch_merge_norm_fwd": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_float, c_void_p]),
-    "sigma_pixel_shuffle_norm_fwd": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_float, c_void_p]),
-    "sigma_upsample2x_norm_head_fwd": (c_int, [c_void_p] * 4 + [c_int, c_void_p] + [c_int] * 4 + [c_float, c_void_p]),
-    "sigma_pool_avgmax_partial_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int, c_int, c_void_p]),
-    "sigma_scale_add_fwd": (c_int, [c_void_p] * 5 + [c_int64, c_int64, c_int, c_void_p]),
-    "sigma_image_pre_fwd": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_double, c_double] + [c_int] * 7 + [c_void_p] * 4),
-    "sigma_eval_exp_accumulate_fwd": (c_int, [c_void_p] * 3 + [c_int] * 11 + [c_void_p]),
-    "sigma_eval_resize_add_fwd": (c_int, [c_void_p] + [c_int] * 7 + [c_void_p, c_int, c_int, c_void_p]),
-    "sigma_eval_argmax_hist_fwd": (c_int, [c_void_p] * 5 + [c_int, c_int64, c_void_p]),
-    "sigma_linear_tf32": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p]),
-    "sigma_linear_tf32x3": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p]),
-    "sigma_conv3x3_tf32": (c_int, [c_void_p] * 4 + [c_int, c_void_p] + [c_int] * 5 + [c_void_p]),
-    "sigma_split_tf32_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
-    "sigma_linear_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int, c_int, c_void_p]),
-    "sigma_layernorm_fwd_bf16": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_float, c_void_p]),
-    "sigma_patch_merge_norm_fwd_bf16": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_float, c_void_p]),
-    "sigma_merge_norm_gate_fwd_bf16": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
-                                               c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_float, c_void_p]),
-    "sigma_dwconv3x3_silu_fwd_bf16": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64] + [c_int] * 4 + [c_void_p]),
-    "sigma_ss2d_scan_fwd_bf16": (c_int, [c_int] + [c_void_p] * 7 + [c_int] * 7 + [c_void_p, c_size_t, c_void_p]),
-    "sigma_scan_bwd_det_workspace_bytes": (c_size_t, [c_int] * 6),
-    "sigma_scan_bwd_det": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
-    "sigma_ss2d_scan_bwd_det_workspace_bytes": (c_size_t, [c_int] * 6),
-    "sigma_ss2d_scan_bwd_det": (c_int, [c_int] + [c_void_p] * 14 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
-    "sigma_ss2d_scan_bwd_saved_det": (c_int, [c_int] + [c_void_p] * 15 + [c_int] * 7 + [c_void_p, c_size_t, c_int, c_void_p]),
-    "sigma_layernorm_bwd_det_workspace_bytes": (c_size_t, [c_int64, c_int]),
-    "sigma_layernorm_bwd_det": (c_int, [c_void_p] * 6 + [c_int64, c_int, c_float, c_void_p, c_size_t, c_void_p]),
-    "sigma_upsample_bilinear_bwd": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_float, c_float, c_int, c_void_p]),
-}
+HEADER = os.path.join(os.path.dirname(_HERE), "include", "sigma_b200.h")
+_SCALARS = {"void": None, "int": c_int, "int64_t": c_int64, "uint64_t": c_uint64, "size_t": c_size_t, "float": c_float,
+            "double": c_double}
+
+
+def _ctype(decl):
+    """ctypes type of one declarator of the header ("const float *A", "int64_t *out8_host", "size_t", ...).  Every pointer is
+    passed as c_void_p except host int64 output arrays, the strides struct and the error string."""
+    decl = decl.replace("const ", "").strip()
+    if "*" not in decl:
+        return _SCALARS[decl.split()[0]]
+    base, name = (t.strip() for t in decl.split("*", 1))
+    if base == "sigma_scan_strides":
+        return ctypes.POINTER(ScanStrides)
+    if base == "int64_t" and name.endswith("_host"):
+        return ctypes.POINTER(c_int64)
+    return c_char_p if base == "char" else c_void_p
+
+
+def _signatures():
+    """name -> (restype, argtypes) of every function include/sigma_b200.h declares."""
+    src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
+    sigs = {}
+    for ret, name, args in re.findall(r"^([A-Za-z_][\w ]*?\s*\**)\s*(sigma_\w+)\s*\(([^)]*)\)\s*;", src, flags=re.M):
+        params = [a for a in args.split(",") if a.strip() not in ("", "void")]
+        sigs[name] = (_ctype(ret), [_ctype(a) for a in params])
+    return sigs
+
+
+SIGNATURES = _signatures()
 
 _lib = None
 
@@ -106,3 +76,13 @@ def check(rc, what):
 
 def launch_count():
     return int(lib().sigma_launch_count())
+
+
+def ptr(t):
+    """a tensor's device pointer as a `void *` / `float *` argument; None passes NULL"""
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def stream():
+    """torch's current CUDA stream as the `void *stream` argument"""
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)

@@ -25,58 +25,15 @@ void set_error(const char *fmt, ...) {
 }
 void count_launch(int n) { g_launches.fetch_add((uint64_t)n, std::memory_order_relaxed); }
 
-// implemented in scan_op.cu (generic) / scan_op_tma.cu (TMA-staged) / scan_op_bwd*.cu
-size_t scan_op_workspace_bytes(int batch, int dim, int dstate);
-size_t scan_op_tma_workspace_bytes(int batch, int dim, int dstate);
-size_t scan_op_bwd_workspace_bytes(int batch, int dim, int L, int N, int elem_bytes);
-size_t scan_op_bwd_tma_workspace_bytes(int batch, int dim, int L, int N, int elem_bytes);
-template <typename T>
-bool scan_op_tma_eligible(const void *u, const void *delta, const void *B, const void *C, const void *out, int dim, int L,
-                          int N, int G, const sigma_scan_strides &s);
-template <typename T>
-int scan_op_fwd_tma(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
-                    const float *bias, void *out, float *x, float *hs, int batch, int dim, int L, int N, int G, int softplus,
-                    const sigma_scan_strides &s, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream);
-template <typename T>
-int scan_op_fwd_generic(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
-                        const float *bias, void *out, float *x, float *hs, int batch, int dim, int L, int N, int G,
-                        int softplus, const sigma_scan_strides &s, void *ws, size_t ws_bytes, int force_split,
-                        cudaStream_t stream);
-template <typename T>
-int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
-                    const float *bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC, float *dD,
-                    float *dbias, int batch, int dim, int L, int N, int G, int softplus, void *ws, size_t ws_bytes,
-                    int force_split, cudaStream_t stream, void *det_ws);
-template <typename T>
-int scan_op_bwd_generic(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
-                        const float *bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC,
-                        float *dD, float *dbias, int batch, int dim, int L, int N, int G, int softplus, void *ws,
-                        size_t ws_bytes, cudaStream_t stream, void *det_ws);
-// scratch of the deterministic backward builds (det_ws != nullptr above)
-size_t scan_op_bwd_tma_det_bytes(int batch, int dim, int L, int N, int G);
-size_t scan_op_bwd_det_bytes(int batch, int dim, int L, int N, int G);
-// launch plans, host only: the launchers above plan through these very functions
-ScanOpPlan scan_op_fwd_generic_plan(int batch, int dim, int L, int N, int G, bool have_ws, int force_split);
-ScanOpPlan scan_op_fwd_tma_plan(int elem_bytes, int batch, int dim, int L, int N, int G, bool have_ws, int force_split);
-ScanOpPlan scan_op_bwd_tma_plan(int elem_bytes, int batch, int dim, int L, int N, int G, int force_split);
-
 // SIGMA_OP_GENERIC=1 forces the generic kernels (A/B timing, tests of the fallback on TMA-eligible shapes)
 static bool force_generic() {
   const char *e = getenv("SIGMA_OP_GENERIC");
   return e && atoi(e) > 0;
 }
 
-static size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 // ---- 16-bit tensors whose rows are not 16-byte aligned (L % 8 != 0, e.g. the 15 x 20 stage) cannot be TMA boxes.  When the
 // fp32 image of the call IS eligible (L % 4 == 0), it is cheaper to widen the operands into scratch, run the TMA-staged fp32
 // kernels and narrow the results than to take the generic kernels (measured: 0.2-0.6x of the reference kernel there). ----
-template <typename T> __device__ __forceinline__ float wide(T v);
-template <> __device__ __forceinline__ float wide<__half>(__half v) { return __half2float(v); }
-template <> __device__ __forceinline__ float wide<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
-template <typename T> __device__ __forceinline__ T narrow(float v);
-template <> __device__ __forceinline__ __half narrow<__half>(float v) { return __float2half_rn(v); }
-template <> __device__ __forceinline__ __nv_bfloat16 narrow<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
 // src (n0, n1, n2, L) with element strides (s0, s1, s2, 1) -> dst contiguous fp32
 template <typename T>
@@ -87,7 +44,7 @@ __global__ void widen_kernel(const T *__restrict__ src, float *__restrict__ dst,
     long long r = i / L;
     const int i2 = (int)(r % n2); r /= n2;
     const int i1 = (int)(r % n1); r /= n1;
-    dst[i] = wide<T>(src[r * s0 + i1 * s1 + i2 * s2 + l]);
+    dst[i] = to_f32(src[r * s0 + i1 * s1 + i2 * s2 + l]);
   }
 }
 // src contiguous fp32 (n0, n1, L) -> dst with strides (s0, s1, 1)
@@ -97,7 +54,7 @@ __global__ void narrow_kernel(const float *__restrict__ src, T *__restrict__ dst
     const int l = (int)(i % L);
     long long r = i / L;
     const int i1 = (int)(r % n1); r /= n1;
-    dst[r * s0 + i1 * s1 + l] = narrow<T>(src[i]);
+    dst[r * s0 + i1 * s1 + l] = from_f32<T>(src[i]);
   }
 }
 template <typename T>
@@ -347,61 +304,6 @@ int sigma_test_scan_plan(int sweep, int batch, int dim, int seqlen, int dstate, 
 // fused channels-last pipeline
 // ---------------------------------------------------------------------------------------------
 namespace sigma {
-int row_norm_launch(const RowNormParams &p, cudaStream_t stream);
-int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                         int D, float eps, cudaStream_t stream, float *part = nullptr);
-size_t layernorm_bwd_det_workspace_bytes(long long rows, int D);
-int upsample_bilinear_bwd_launch(const float *dy, float *dx, int batch, int C, int Hin, int Win, int Hout, int Wout, float rh, float rw,
-                                 int channels_last, cudaStream_t stream);
-int argmax_hist_launch(const float *logits, const void *labels, int label_bytes, unsigned long long *hist,
-                       unsigned long long *counts, unsigned char *pred_out, int batch, int ncls, long long HW, cudaStream_t stream);
-int dwconv3x3_silu_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
-                          const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
-                          cudaStream_t stream);
-size_t ss2d_scan_workspace_bytes(int kind, int batch, int D, int N);
-int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
-                  const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp, void *ws,
-                  size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave = nullptr, float *hsave = nullptr, int xc_bf16 = 0);
-size_t ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N);
-int ss2d_pick_segments_hook(long long ctas, int nw, int ntiles, int N);
-int ss2d_fwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int R, int xc_bf16, int force_split, size_t ws_bytes,
-                       long long *out8);
-int gemm_pick_bn_hook(int N, long long m_tiles);
-int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out);
-size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
-size_t ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
-int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int force_split, long long *out4);
-int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
-                  const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
-                  int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream,
-                  const float *hs_saved = nullptr, int det = 0);
-int upsample2x_norm_launch(const float *in, const float *gamma, const float *beta, const float *wcls, int ncls, float *out,
-                           int B, int Hin, int Win, int C, float eps, cudaStream_t stream);
-int pool_avgmax_partial_launch(const float *x, float *partial, int B, long long L, int C, int nslice, cudaStream_t stream);
-int scale_add_launch(const float *a, const float *sa, const float *b, const float *sb, float *out, long long rows,
-                     long long rows_per_batch, int C, cudaStream_t stream);
-int gemm_tf32_launch(const float *A, long long lda, const float *W, const float *W_lo, const float *bias, const float *residual,
-                     long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream);
-int split_tf32_launch(const float *x, float *hi, float *lo, long long n, cudaStream_t stream);
-int gemm_bf16_launch(const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
-                     const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N, int K, cudaStream_t stream);
-int dwconv3x3_silu_bf16_launch(const void *x, long long x_row_stride, long long x_batch_stride, const float *w, const float *bias,
-                               void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream);
-int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, const float *bias, int act, float *y, int B, int H, int W,
-                        int Cin, int Cout, cudaStream_t stream);
-struct ImagePreParams {
-  const unsigned char *src; float *dst; const unsigned char *lsrc; long long *ldst;
-  int H0, W0, SH, SW, OH, OW, off_y, off_x, mirror_src, mirror_out, label_pad;
-  int clip_y0, clip_x0, clip_y1, clip_x1;
-  double scale_y, scale_x, mean[3], stdv[3];
-};
-int image_pre_launch(const ImagePreParams &p, cudaStream_t stream);
-int eval_exp_accumulate_launch(const float *logits, const float *logits_flip, float *acc, int ncls, int TH, int TW, int m_top, int m_left,
-                               int vh, int vw, int AH, int AW, int ay, int ax, cudaStream_t stream);
-int eval_resize_add_launch(const float *acc, int ncls, int AH, int AW, int m_top, int m_left, int SH, int SW, double *out, int H0, int W0,
-                           cudaStream_t stream);
-int eval_argmax_hist_launch(const double *score, const unsigned char *labels, unsigned char *pred, unsigned long long *hist,
-                            unsigned long long *counts, int ncls, long long HW, cudaStream_t stream);
 static bool al16(const void *p) { return ((uintptr_t)p & 15) == 0; }
 static bool al8(const void *p) { return ((uintptr_t)p & 7) == 0; }
 }  // namespace sigma
@@ -547,10 +449,8 @@ int sigma_dwconv3x3_silu_fwd_bf16(const void *x, int64_t x_row_stride, int64_t x
 }
 
 int sigma_ss2d_padded_cp(int N, int R) {
-  const int opts[] = {4, 8, 12, 16, 24, 32, 48, 64};
-  for (int o : opts)
-    if (R <= o) return 2 * N + o;
-  return -1;
+  const int rp = pad_rp(R);
+  return rp < 0 ? -1 : 2 * N + rp;
 }
 
 size_t sigma_ss2d_scan_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
@@ -602,8 +502,8 @@ int sigma_ss2d_scan_fwd_split(int kind, const float *xc, const float *xdbl, cons
 }
 
 // test hooks (host logic only, no CUDA call): the launch heuristics, so that CPU tests can hold them to the recorded sweeps
-int sigma_test_pick_segments(long long ctas, int warps_per_cta, int ntiles, int N) { return ss2d_pick_segments_hook(ctas, warps_per_cta, ntiles, N); }
-int sigma_test_pick_bn(int N, long long m_tiles) { return gemm_pick_bn_hook(N, m_tiles); }
+int sigma_test_pick_segments(int64_t ctas, int warps_per_cta, int ntiles, int N) { return ss2d_pick_segments_hook(ctas, warps_per_cta, ntiles, N); }
+int sigma_test_pick_bn(int N, int64_t m_tiles) { return gemm_pick_bn_hook(N, m_tiles); }
 // the launch plan of sigma_linear_tf32{,x3} (conv_B = 0) or of sigma_conv3x3_tf32 (conv_B > 0: input (conv_B, conv_H, conv_W, K),
 // N output channels), SIGMA_GEMM_BN included: out6_host = {tile width, ring stages, grid, tiles, shared-memory bytes, CTAs per SM}
 int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, int64_t *out6_host) {

@@ -1,20 +1,20 @@
 // Shared device helpers and host-side error plumbing for libsigma_b200 (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 
-#include "../../include/sigma_b200.h"
+#include "internal.cuh"
 
 namespace sigma {
 
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr int kNumSMs = 132;   // H100 SXM: grid sizes and the launch cost models assume this many SMs
 
-// ---- host-side error state (thread-local string, no exceptions across the ABI) ----
-void set_error(const char *fmt, ...);
-void count_launch(int n = 1);
+// workspace carving: every sub-buffer starts on a 256-byte boundary
+inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 #define SIGMA_CHECK_ARG(cond, ...)         \
   do {                                     \
@@ -40,47 +40,29 @@ void count_launch(int n = 1);
     SIGMA_CHECK_CUDA(cudaPeekAtLastError());      \
   } while (0)
 
-// ---- shared host-side parameter blocks ----
-// Launch plan of one op-level scan sweep (scan_op*.cu): what the launcher runs and what sigma_test_scan_plan reports.
-struct ScanOpPlan {
-  int nsplit;            // L-segments
-  int tiles_per_split;   // position tiles per segment
-  int ntiles;            // position tiles of the sequence
-  int DT;                // channels per CTA
-  int nst;               // ring / pipeline stages
-};
+// ---- element conversions: fp32 <-> {fp32, fp16, bf16}; widening is exact, narrowing rounds to nearest even ----
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <typename T> __device__ __forceinline__ T from_f32(float v);
+template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
+template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+// two fp32 -> one 32-bit word holding two 16-bit T (a at the lower address)
+template <typename T> __device__ __forceinline__ uint32_t from_f32x2(float a, float b);
+template <> __device__ __forceinline__ uint32_t from_f32x2<__half>(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t *>(&h);
+}
+template <> __device__ __forceinline__ uint32_t from_f32x2<__nv_bfloat16>(float a, float b) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<const uint32_t *>(&h);
+}
 
-struct RowNormParams {
-  const float *y;          // K slabs
-  long long k_stride;      // floats between slabs
-  int K;
-  const float *gamma, *beta;
-  const float *z; long long z_row_stride;       // nullable
-  const float *gate;                            // nullable, (rows / rows_per_batch, D)
-  float *out;
-  long long rows, rows_per_batch;
-  long long in_batch_stride, out_batch_stride, out_row_stride;
-  int D;
-  float eps;
-  // row addressing mode (fast kernel only): 0 = plain rows;
-  // 1 = PatchMerging2D gather (vmamba.py:619-636): y is (batch, gH, gW, D/4), row (b,i,j) = the four pixels
-  //     (2i,2j), (2i+1,2j), (2i,2j+1), (2i+1,2j+1) concatenated, zeros beyond odd gH / gW;
-  // 2 = PatchExpand pixel shuffle (MambaDecoder.py:24-28): input rows are (b, h, w, p1, p2) sub-rows of D channels,
-  //     row lands at out (b, 2h+p1, 2w+p2)
-  int mode = 0, gH = 0, gW = 0;
-  // element types (the bf16 inference mode): 0 = y, z, out fp32; 1 = y fp32, out bf16 (LayerNorm / patch-merge LN feeding a
-  // bf16 GEMM); 2 = y, z, out bf16 (merge + out_norm + gate of the bf16 scan output).  Pointers and strides count elements.
-  int io = 0;
-};
-
-// ---- 4-element fp32 / bf16 accesses (a float4 or 8 bytes of bf16); bf16 -> fp32 is exact, fp32 -> bf16 rounds to nearest even ----
+// ---- 4-element fp32 / bf16 accesses (a float4 or 8 bytes of bf16) ----
 __device__ __forceinline__ float4 bf16x4_to_f4(uint2 u) {
   return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
                      __uint_as_float(u.y & 0xFFFF0000u));
-}
-__device__ __forceinline__ uint32_t f2_to_bf16x2(float a, float b) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<const uint32_t *>(&h);
 }
 __device__ __forceinline__ float4 ld4(const float *p) { return *reinterpret_cast<const float4 *>(p); }
 __device__ __forceinline__ float4 ld4(const __nv_bfloat16 *p) { return bf16x4_to_f4(*reinterpret_cast<const uint2 *>(p)); }
@@ -90,13 +72,8 @@ __device__ __forceinline__ float4 ld4cs(const float *p) { return __ldcs(reinterp
 __device__ __forceinline__ float4 ld4cs(const __nv_bfloat16 *p) { return bf16x4_to_f4(__ldcs(reinterpret_cast<const uint2 *>(p))); }
 __device__ __forceinline__ void st4(float *p, float4 v) { *reinterpret_cast<float4 *>(p) = v; }
 __device__ __forceinline__ void st4(__nv_bfloat16 *p, float4 v) {
-  *reinterpret_cast<uint2 *>(p) = make_uint2(f2_to_bf16x2(v.x, v.y), f2_to_bf16x2(v.z, v.w));
+  *reinterpret_cast<uint2 *>(p) = make_uint2(from_f32x2<__nv_bfloat16>(v.x, v.y), from_f32x2<__nv_bfloat16>(v.z, v.w));
 }
-__device__ __forceinline__ float to_f32(float v) { return v; }
-__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
-template <typename T> __device__ __forceinline__ T from_f32(float v);
-template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
-template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
 // ---- device math ----
 __device__ __forceinline__ float ex2(float x) {

@@ -135,9 +135,6 @@ __global__ void __launch_bounds__(DC_THREADS, 2) dwconv3x3_silu_tma_kernel(const
   }
 }
 
-int make_tmap_generic(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,
-                      const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo);   // scan_op_tma.cu
-
 template <typename T>
 static int dwconv_tma_launch(const T *x, long long x_row_stride, long long x_batch_stride, const float *w, const float *bias, T *y,
                              long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream) {
@@ -146,9 +143,8 @@ static int dwconv_tma_launch(const T *x, long long x_row_stride, long long x_bat
   const uint64_t dims[4] = {(uint64_t)D, (uint64_t)W, (uint64_t)H, (uint64_t)batch};
   const uint64_t str[3] = {(uint64_t)x_row_stride * es, (uint64_t)W * x_row_stride * es, (uint64_t)x_batch_stride * es};
   const uint32_t box[4] = {DC_CB, DC_TW + 2, DC_TH + 2, 1};
-  int rc = es == 4 ? make_tmap_f32_4d(&p.map, x, dims, str, box)
-                   : make_tmap_generic(&p.map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE,
-                                       CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+  int rc = make_tmap(&p.map, es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x, dims, str, box,
+                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
   if (rc) return rc;
   p.w = w; p.bias = bias; p.y = y; p.y_batch_stride = y_batch_stride;
   p.batch = batch; p.H = H; p.W = W; p.D = D;

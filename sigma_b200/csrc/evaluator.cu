@@ -94,17 +94,6 @@ __device__ __forceinline__ Lin8u lin8u_coef(int d, int sn, double scale) {
   return c;
 }
 
-struct ImagePreParams {
-  const unsigned char *src;   // (H0, W0, 3) uint8, HWC
-  float *dst;                 // (3, OH, OW) float32 (one image of an NCHW batch)
-  const unsigned char *lsrc;  // nullable: (H0, W0) uint8 labels
-  long long *ldst;            // nullable: (OH, OW) int64 labels
-  int H0, W0, SH, SW, OH, OW, off_y, off_x, mirror_src, mirror_out, label_pad;
-  int clip_y0, clip_x0, clip_y1, clip_x1;   // only this rectangle of the scaled image is visible (a sliding window); rest = pad
-  double scale_y, scale_x;    // source pixels per scaled pixel (cv2: 1/fy, 1/fx or H0/SH, W0/SW)
-  double mean[3], stdv[3];
-};
-
 // One output pixel per thread: out(c, oy, ox) = pad 0 outside the scaled image, else ((resized / 255) − mean) / std in
 // double like utils/transforms.py:182-187, rounded to float like np.ascontiguousarray(..., dtype=float32).
 __global__ void __launch_bounds__(256) image_pre_kernel(const ImagePreParams p) {

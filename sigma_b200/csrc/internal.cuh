@@ -1,0 +1,183 @@
+// Declarations shared between the library's translation units: every host function, kernel and parameter block that is
+// used outside the file that defines it, declared once (default arguments included).  Each defining file includes this
+// header (through common.cuh), so the compiler checks every definition against its declaration.
+#pragma once
+#include <cuda.h>
+#include <cuda_runtime.h>
+#include <stddef.h>
+#include <stdint.h>
+
+#include "../../include/sigma_b200.h"
+
+namespace sigma {
+
+// ---- parameter blocks ----
+// Launch plan of one op-level scan sweep (scan_op*.cu): what the launcher runs and what sigma_test_scan_plan reports.
+struct ScanOpPlan {
+  int nsplit;            // L-segments
+  int tiles_per_split;   // position tiles per segment
+  int ntiles;            // position tiles of the sequence
+  int DT;                // channels per CTA
+  int nst;               // ring / pipeline stages
+};
+
+struct RowNormParams {
+  const float *y;          // K slabs
+  long long k_stride;      // floats between slabs
+  int K;
+  const float *gamma, *beta;
+  const float *z; long long z_row_stride;       // nullable
+  const float *gate;                            // nullable, (rows / rows_per_batch, D)
+  float *out;
+  long long rows, rows_per_batch;
+  long long in_batch_stride, out_batch_stride, out_row_stride;
+  int D;
+  float eps;
+  // row addressing mode (fast kernel only): 0 = plain rows;
+  // 1 = PatchMerging2D gather (vmamba.py:619-636): y is (batch, gH, gW, D/4), row (b,i,j) = the four pixels
+  //     (2i,2j), (2i+1,2j), (2i,2j+1), (2i+1,2j+1) concatenated, zeros beyond odd gH / gW;
+  // 2 = PatchExpand pixel shuffle (MambaDecoder.py:24-28): input rows are (b, h, w, p1, p2) sub-rows of D channels,
+  //     row lands at out (b, 2h+p1, 2w+p2)
+  int mode = 0, gH = 0, gW = 0;
+  // element types (the bf16 inference mode): 0 = y, z, out fp32; 1 = y fp32, out bf16 (LayerNorm / patch-merge LN feeding a
+  // bf16 GEMM); 2 = y, z, out bf16 (merge + out_norm + gate of the bf16 scan output).  Pointers and strides count elements.
+  int io = 0;
+};
+
+struct ImagePreParams {
+  const unsigned char *src;   // (H0, W0, 3) uint8, HWC
+  float *dst;                 // (3, OH, OW) float32 (one image of an NCHW batch)
+  const unsigned char *lsrc;  // nullable: (H0, W0) uint8 labels
+  long long *ldst;            // nullable: (OH, OW) int64 labels
+  int H0, W0, SH, SW, OH, OW, off_y, off_x, mirror_src, mirror_out, label_pad;
+  int clip_y0, clip_x0, clip_y1, clip_x1;   // only this rectangle of the scaled image is visible (a sliding window); rest = pad
+  double scale_y, scale_x;    // source pixels per scaled pixel (cv2: 1/fy, 1/fx or H0/SH, W0/SW)
+  double mean[3], stdv[3];
+};
+
+// ---- api.cu: host-side error state (thread-local string, no exceptions across the ABI) and the launch counter ----
+void set_error(const char *fmt, ...);
+void count_launch(int n = 1);
+
+// ---- ss2d_scan_host.cu ----
+// The one tensor-map encoder: cuTensorMapEncodeTiled resolved at run time through the runtime's driver entry point (the
+// library does not link libcuda).  dims innermost first, strides_bytes for dims 1..rank-1; element strides 1, no interleave,
+// no out-of-bounds fill.  Returns 0 or SIGMA_ECUDA with the library error string set.
+int make_tmap(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,
+              const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo);
+int pad_rp(int R);   // dt_rank padded to an instantiated width (4, 8, 12, 16, 24, 32, 48, 64), -1 beyond 64
+size_t ss2d_scan_workspace_bytes(int kind, int batch, int D, int N);
+// xc_bf16 = 1: xc and y are bf16; dsave / hsave (training forward): delta' slabs and block-start states for the backward
+int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                  const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp, void *ws,
+                  size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave = nullptr, float *hsave = nullptr, int xc_bf16 = 0);
+int ss2d_pick_segments_hook(long long ctas, int nw, int ntiles, int N);
+int ss2d_fwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int R, int xc_bf16, int force_split, size_t ws_bytes,
+                       long long *out8);
+
+// ---- ss2d_scan_bwd.cu ----
+int ss2d_save_tiles(int kind, int H, int W);   // 16-position blocks of the longest walk
+size_t ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N);
+size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
+size_t ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
+int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int force_split, long long *out4);
+// hs_saved: the training forward's block-start states (no state sweep); det: the deterministic build
+int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
+                  const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
+                  int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream,
+                  const float *hs_saved = nullptr, int det = 0);
+
+// ---- scan_op.cu: generic op-level scan forward ----
+__global__ void scan_combine_kernel(float *carry, long long nrows, int nsplit, int NP);
+int scan_op_npad(int N);
+size_t scan_op_workspace_bytes(int batch, int dim, int dstate);
+ScanOpPlan scan_op_fwd_generic_plan(int batch, int dim, int L, int N, int G, bool have_ws, int force_split);
+template <typename T>
+int scan_op_fwd_generic(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
+                        const float *bias, void *out, float *x, float *hs, int batch, int dim, int L, int N, int G,
+                        int softplus, const sigma_scan_strides &s, void *ws, size_t ws_bytes, int force_split,
+                        cudaStream_t stream);
+
+// ---- scan_op_tma.cu: TMA-staged op-level scan forward ----
+cudaError_t prep_kernel_once(const void *fn);
+int pick_segments(long long ctas_base, int ntiles, long long slots, double pass_factor, int max_split);
+size_t scan_op_tma_workspace_bytes(int batch, int dim, int dstate);
+ScanOpPlan scan_op_fwd_tma_plan(int elem_bytes, int batch, int dim, int L, int N, int G, bool have_ws, int force_split);
+template <typename T>
+bool scan_op_tma_eligible(const void *u, const void *delta, const void *B, const void *C, const void *out, int dim, int L,
+                          int N, int G, const sigma_scan_strides &s);
+template <typename T>
+int scan_op_fwd_tma(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
+                    const float *bias, void *out, float *x, float *hs, int batch, int dim, int L, int N, int G, int softplus,
+                    const sigma_scan_strides &s, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream);
+
+// ---- scan_op_bwd.cu: generic op-level scan backward ----
+size_t scan_op_bwd_workspace_bytes(int batch, int dim, int L, int N, int elem_bytes);
+size_t scan_op_bwd_det_bytes(int batch, int dim, int L, int N, int G);   // scratch of the deterministic build (det_ws)
+template <typename T>
+int scan_op_bwd_generic(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
+                        const float *bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC,
+                        float *dD, float *dbias, int batch, int dim, int L, int N, int G, int softplus, void *ws,
+                        size_t ws_bytes, cudaStream_t stream, void *det_ws);
+
+// ---- scan_op_bwd_tma.cu: TMA-staged op-level scan backward ----
+__global__ void scan_combine_rev_kernel(float *carry, long long nrows, int nsplit, int NP);
+size_t scan_op_bwd_tma_workspace_bytes(int batch, int dim, int L, int N, int elem_bytes);
+size_t scan_op_bwd_tma_det_bytes(int batch, int dim, int L, int N, int G);   // scratch of the deterministic build (det_ws)
+ScanOpPlan scan_op_bwd_tma_plan(int elem_bytes, int batch, int dim, int L, int N, int G, int force_split);
+template <typename T>
+int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
+                    const float *bias, const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC, float *dD,
+                    float *dbias, int batch, int dim, int L, int N, int G, int softplus, void *ws, size_t ws_bytes,
+                    int force_split, cudaStream_t stream, void *det_ws);
+
+// ---- det_reduce.cu ----
+int sum_parts_det_launch(const float *part, int nparts, long long ncols, long long inner, long long ostride, float *out, cudaStream_t stream);
+int upsample_bilinear_bwd_launch(const float *dy, float *dx, int batch, int C, int Hin, int Win, int Hout, int Wout, float rh, float rw,
+                                 int channels_last, cudaStream_t stream);
+
+// ---- rowwise.cu ----
+int row_norm_launch(const RowNormParams &p, cudaStream_t stream);
+// part != nullptr: the deterministic build (layernorm_bwd_det_workspace_bytes of scratch)
+int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
+                         int D, float eps, cudaStream_t stream, float *part = nullptr);
+size_t layernorm_bwd_det_workspace_bytes(long long rows, int D);
+int dwconv3x3_silu_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
+                          const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
+                          cudaStream_t stream);
+int upsample2x_norm_launch(const float *in, const float *gamma, const float *beta, const float *wcls, int ncls, float *out,
+                           int B, int Hin, int Win, int C, float eps, cudaStream_t stream);
+int pool_avgmax_partial_launch(const float *x, float *partial, int B, long long L, int C, int nslice, cudaStream_t stream);
+int scale_add_launch(const float *a, const float *sa, const float *b, const float *sb, float *out, long long rows,
+                     long long rows_per_batch, int C, cudaStream_t stream);
+
+// ---- dwconv_tma.cu ----
+int dwconv3x3_silu_tma_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
+                              const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
+                              cudaStream_t stream);
+int dwconv3x3_silu_bf16_launch(const void *x, long long x_row_stride, long long x_batch_stride, const float *w, const float *bias,
+                               void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream);
+
+// ---- gemm_tf32.cu ----
+int gemm_tf32_launch(const float *A, long long lda, const float *W, const float *W_lo, const float *bias, const float *residual,
+                     long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream);
+int gemm_bf16_launch(const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
+                     const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N, int K, cudaStream_t stream);
+int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, const float *bias, int act, float *y, int B, int H, int W,
+                        int Cin, int Cout, cudaStream_t stream);
+int split_tf32_launch(const float *x, float *hi, float *lo, long long n, cudaStream_t stream);
+int gemm_pick_bn_hook(int N, long long m_tiles);
+int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out);
+
+// ---- evaluator.cu ----
+int argmax_hist_launch(const float *logits, const void *labels, int label_bytes, unsigned long long *hist,
+                       unsigned long long *counts, unsigned char *pred_out, int batch, int ncls, long long HW, cudaStream_t stream);
+int image_pre_launch(const ImagePreParams &p, cudaStream_t stream);
+int eval_exp_accumulate_launch(const float *logits, const float *logits_flip, float *acc, int ncls, int TH, int TW, int m_top, int m_left,
+                               int vh, int vw, int AH, int AW, int ay, int ax, cudaStream_t stream);
+int eval_resize_add_launch(const float *acc, int ncls, int AH, int AW, int m_top, int m_left, int SH, int SW, double *out, int H0, int W0,
+                           cudaStream_t stream);
+int eval_argmax_hist_launch(const double *score, const unsigned char *labels, unsigned char *pred, unsigned long long *hist,
+                            unsigned long long *counts, int ncls, long long HW, cudaStream_t stream);
+
+}  // namespace sigma

@@ -391,8 +391,6 @@ size_t layernorm_bwd_det_workspace_bytes(long long rows, int D) {
   return (size_t)2 * layernorm_bwd_grid(rows, D) * 8 * D * sizeof(float);
 }
 
-int sum_parts_det_launch(const float *part, int nparts, long long ncols, long long inner, long long ostride, float *out, cudaStream_t stream);
-
 // dgamma / dbeta are zeroed here and accumulated into; false if D has no instantiation (the fast forward's D set).
 // part != nullptr: the deterministic build (layernorm_bwd_det_workspace_bytes of scratch), dgamma / dbeta written by the
 // fixed-order sum over the grid's warps
@@ -497,10 +495,6 @@ __global__ void __launch_bounds__(256) dwconv3x3_silu_kernel(const float *__rest
     }
   }
 }
-
-int dwconv3x3_silu_tma_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
-                              const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
-                              cudaStream_t stream);   // dwconv_tma.cu
 
 int dwconv3x3_silu_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
                           const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,

@@ -39,6 +39,31 @@ __device__ __forceinline__ float channel_reduce(float v) {
   return v;
 }
 
+// The dB / dC reduction of the backward kernels: sum v[0..NV) over the W lanes {lane ^ x : x < W} (W a power of two <= 32).
+// Halving steps trade registers for lanes: after the step with offset OFF a lane keeps the half of the values selected by
+// (lane & OFF); when one value is left the remaining offsets are plain butterflies.  Returns the sum of value index `which`
+// (also returned) — every value index is held by W / NV lanes.
+template <int NV, int OFF>
+__device__ __forceinline__ float transpose_reduce(float (&v)[NV], int lane, int &which) {
+  if constexpr (OFF == 0) {
+    return v[0];
+  } else if constexpr (NV > 1) {
+    const bool up = (lane & OFF) != 0;
+    float w[NV / 2];
+#pragma unroll
+    for (int j = 0; j < NV / 2; ++j) {
+      const float send = up ? v[j] : v[j + NV / 2];
+      const float keep = up ? v[j + NV / 2] : v[j];
+      w[j] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
+    }
+    which = which * 2 + (up ? 1 : 0);
+    return transpose_reduce<NV / 2, OFF / 2>(w, lane, which);
+  } else {
+    float w[1] = {v[0] + __shfl_xor_sync(0xffffffffu, v[0], OFF)};
+    return transpose_reduce<1, OFF / 2>(w, lane, which);
+  }
+}
+
 // delta' for a group of 4 consecutive positions, computed ONCE per channel and shared by its LPC
 // lanes: lane q evaluates softplus for position(s) it owns, then the values are exchanged by
 // shuffle.  raw[i] must be identical across the LPC lanes of a channel.

@@ -25,15 +25,6 @@ constexpr int OP_LTP = 36;  // smem row pitch (floats)
 constexpr int OP_DT = 32;   // channels per CTA
 constexpr int OP_NST = 2;   // cp.async stages
 
-template <typename T> __device__ __forceinline__ float gen_to_f32(T v);
-template <> __device__ __forceinline__ float gen_to_f32<float>(float v) { return v; }
-template <> __device__ __forceinline__ float gen_to_f32<__half>(__half v) { return __half2float(v); }
-template <> __device__ __forceinline__ float gen_to_f32<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
-template <typename T> __device__ __forceinline__ T gen_from_f32(float v);
-template <> __device__ __forceinline__ float gen_from_f32<float>(float v) { return v; }
-template <> __device__ __forceinline__ __half gen_from_f32<__half>(float v) { return __float2half_rn(v); }
-template <> __device__ __forceinline__ __nv_bfloat16 gen_from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
-
 struct ScanOpParams {
   const void *u, *delta, *B, *C;   // element type T of the kernel instantiation
   const float *A, *D, *bias;
@@ -134,7 +125,7 @@ __global__ void __launch_bounds__(32 * LPC) scan_op_kernel(const ScanOpParams p)
         else { const int n = row - 2 * OP_DT - NP; ok = n < p.N; src = gC + (long long)n * p.C_n; }
         ok = ok && l < p.L;
         if constexpr (F32) cp_async4(sbase + row * OP_LTP + e, ok ? (const void *)(src + l) : (const void *)p.u, ok ? 4 : 0);
-        else sbase[row * OP_LTP + e] = ok ? gen_to_f32<T>(src[l]) : 0.f;   // 16-bit elements: plain load, widened on the way in
+        else sbase[row * OP_LTP + e] = ok ? to_f32(src[l]) : 0.f;   // 16-bit elements: plain load, widened on the way in
       }
     }
   };
@@ -231,7 +222,7 @@ __global__ void __launch_bounds__(32 * LPC) scan_op_kernel(const ScanOpParams p)
       } else {
         for (int rr = 0; rr < CPW; ++rr) {
           const int r = warp * CPW + rr;
-          if (r < nch && lane < npos) go[(long long)r * p.o_d + lane] = gen_from_f32<T>(sY[r * OP_LTP + lane]);
+          if (r < nch && lane < npos) go[(long long)r * p.o_d + lane] = from_f32<T>(sY[r * OP_LTP + lane]);
         }
       }
       // x checkpoints: (prod a, h) at the end of every 2048-chunk (selective_scan_fwd_kernel.cuh:181-184)

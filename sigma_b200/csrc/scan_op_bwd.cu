@@ -23,15 +23,6 @@ namespace sigma {
 
 constexpr int BW_LT = 32, BW_LTP = 36, BW_DT = 32;
 
-template <typename T> __device__ __forceinline__ float gen_to_f32(T v);
-template <> __device__ __forceinline__ float gen_to_f32<float>(float v) { return v; }
-template <> __device__ __forceinline__ float gen_to_f32<__half>(__half v) { return __half2float(v); }
-template <> __device__ __forceinline__ float gen_to_f32<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
-template <typename T> __device__ __forceinline__ T gen_from_f32(float v);
-template <> __device__ __forceinline__ float gen_from_f32<float>(float v) { return v; }
-template <> __device__ __forceinline__ __half gen_from_f32<__half>(float v) { return __float2half_rn(v); }
-template <> __device__ __forceinline__ __nv_bfloat16 gen_from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
-
 struct ScanBwdParams {
   const void *u, *delta, *B, *C, *dout;   // element type T
   const float *A, *D, *bias, *hs;
@@ -95,11 +86,11 @@ __device__ __forceinline__ void scan_op_bwd_body(const ScanBwdParams &p) {
       const int row = i >> 5, e = i & 31;
       float v = 0.f;
       if (e < npos) {
-        if (row < BW_DT) { if (row < nch) v = gen_to_f32<T>(pu[row0 + (long long)row * p.L + l0 + e]); }
-        else if (row < 2 * BW_DT) { if (row - BW_DT < nch) v = gen_to_f32<T>(pdl[row0 + (long long)(row - BW_DT) * p.L + l0 + e]); }
-        else if (row < 3 * BW_DT) { if (row - 2 * BW_DT < nch) v = gen_to_f32<T>(pdo[row0 + (long long)(row - 2 * BW_DT) * p.L + l0 + e]); }
-        else if (row < 3 * BW_DT + NP) { const int n = row - 3 * BW_DT; if (n < p.N) v = gen_to_f32<T>(pB[bc0 + (long long)n * p.L + l0 + e]); }
-        else { const int n = row - 3 * BW_DT - NP; if (n < p.N) v = gen_to_f32<T>(pC[bc0 + (long long)n * p.L + l0 + e]); }
+        if (row < BW_DT) { if (row < nch) v = to_f32(pu[row0 + (long long)row * p.L + l0 + e]); }
+        else if (row < 2 * BW_DT) { if (row - BW_DT < nch) v = to_f32(pdl[row0 + (long long)(row - BW_DT) * p.L + l0 + e]); }
+        else if (row < 3 * BW_DT) { if (row - 2 * BW_DT < nch) v = to_f32(pdo[row0 + (long long)(row - 2 * BW_DT) * p.L + l0 + e]); }
+        else if (row < 3 * BW_DT + NP) { const int n = row - 3 * BW_DT; if (n < p.N) v = to_f32(pB[bc0 + (long long)n * p.L + l0 + e]); }
+        else { const int n = row - 3 * BW_DT - NP; if (n < p.N) v = to_f32(pC[bc0 + (long long)n * p.L + l0 + e]); }
       }
       smem[row * BW_LTP + e] = v;
     }
@@ -191,7 +182,7 @@ __device__ __forceinline__ void scan_op_bwd_body(const ScanBwdParams &p) {
       const int which = i / (BW_DT * BW_LT), r = (i >> 5) % BW_DT, e = i & 31;
       if (r < nch && e < npos) {
         T *dst = (T *)(which ? p.ddelta : p.du);
-        dst[row0 + (long long)r * p.L + l0 + e] = gen_from_f32<T>((which ? sDd : sDu)[r * BW_LTP + e]);
+        dst[row0 + (long long)r * p.L + l0 + e] = from_f32<T>((which ? sDd : sDu)[r * BW_LTP + e]);
       }
     }
     for (int i = tid; i < 2 * NP * BW_LT; i += NTH) {
@@ -240,15 +231,6 @@ __global__ void __launch_bounds__(32 * LPC) scan_op_bwd_kernel(const ScanBwdPara
 template <typename T, int SPT, int LPC>
 __global__ void __launch_bounds__(32 * LPC) scan_op_bwd_det_kernel(const ScanBwdParams p) { scan_op_bwd_body<T, SPT, LPC, true>(p); }
 
-int scan_op_npad(int N);
-template <typename T>
-int scan_op_fwd_generic(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
-                        const float *bias, void *out, float *x, float *hs, int batch, int dim, int L, int N, int G,
-                        int softplus, const sigma_scan_strides &s, void *ws, size_t ws_bytes, int force_split,
-                        cudaStream_t stream);
-
-int sum_parts_det_launch(const float *part, int nparts, long long ncols, long long inner, long long ostride, float *out, cudaStream_t stream);
-
 template <typename T, int SPT, int LPC>
 static int launch_bwd(const ScanBwdParams &p, cudaStream_t stream) {
   const bool det = p.part_B != nullptr;
@@ -270,21 +252,19 @@ static int launch_bwd(const ScanBwdParams &p, cudaStream_t stream) {
   return SIGMA_OK;
 }
 
-static size_t al256g(size_t v) { return (v + 255) & ~(size_t)255; }
-
 // scratch of the deterministic build: [dB partials] [dC partials] (tiles_per_group, batch, G, N, L) [dA partials (batch, dim, N)]
 // [dD partials] [ddelta_bias partials] (batch, dim)
 size_t scan_op_bwd_det_bytes(int batch, int dim, int L, int N, int G) {
   const size_t tpg = (size_t)(dim / G + BW_DT - 1) / BW_DT;
-  return 2 * al256g(tpg * batch * G * N * L * sizeof(float)) + al256g((size_t)batch * dim * N * sizeof(float)) +
-         2 * al256g((size_t)batch * dim * sizeof(float));
+  return 2 * align256(tpg * batch * G * N * L * sizeof(float)) + align256((size_t)batch * dim * N * sizeof(float)) +
+         2 * align256((size_t)batch * dim * sizeof(float));
 }
 
 size_t scan_op_bwd_workspace_bytes(int batch, int dim, int L, int N, int elem_bytes) {
   const size_t ntiles = (L + BW_LT - 1) / BW_LT;
   const size_t hs = (size_t)batch * dim * ntiles * scan_op_npad(N) * sizeof(float);
   const size_t out = (size_t)batch * dim * L * elem_bytes;   // forward output of the recompute sweep (discarded)
-  return ((hs + 255) & ~(size_t)255) + ((out + 255) & ~(size_t)255);
+  return align256(hs) + align256(out);
 }
 
 // all tensors contiguous, element type T
@@ -301,7 +281,7 @@ int scan_op_bwd_generic(const void *u, const void *delta, const float *A, const 
   const int NP = scan_op_npad(N);
   const int ntiles = (L + BW_LT - 1) / BW_LT;
   float *hs = (float *)ws;
-  const size_t hs_b = (((size_t)batch * dim * ntiles * NP * sizeof(float)) + 255) & ~(size_t)255;
+  const size_t hs_b = align256((size_t)batch * dim * ntiles * NP * sizeof(float));
   void *out_tmp = (char *)ws + hs_b;
   sigma_scan_strides st;
   st.u_batch = st.delta_batch = st.out_batch = (int64_t)dim * L;
@@ -326,8 +306,8 @@ int scan_op_bwd_generic(const void *u, const void *delta, const float *A, const 
   p.ntiles = ntiles; p.softplus = softplus;
   p.part_B = p.part_C = p.part_dA = p.part_dD = p.part_db = nullptr;
   if (det_ws) {   // layout of scan_op_bwd_det_bytes
-    const size_t bc = al256g((size_t)p.tiles_per_group * batch * G * N * L * sizeof(float));
-    const size_t da = al256g((size_t)batch * dim * N * sizeof(float)), dd = al256g((size_t)batch * dim * sizeof(float));
+    const size_t bc = align256((size_t)p.tiles_per_group * batch * G * N * L * sizeof(float));
+    const size_t da = align256((size_t)batch * dim * N * sizeof(float)), dd = align256((size_t)batch * dim * sizeof(float));
     char *w = (char *)det_ws;
     p.part_B = (float *)w; p.part_C = (float *)(w + bc); p.part_dA = (float *)(w + 2 * bc);
     p.part_dD = (float *)(w + 2 * bc + da); p.part_db = (float *)(w + 2 * bc + da + dd);

@@ -52,35 +52,6 @@ __host__ __device__ inline size_t bwd_tma_smem_bytes(int DT, int nst) {
   return 1024 + nst * stage + bct + sh + 256;
 }
 
-// Sum v[0..NV) over the W lanes {lane ^ x : x < W} (W a power of two <= 32).  Halving steps trade registers for lanes:
-// after the step with offset OFF a lane keeps the half of the values selected by (lane & OFF); when one value is left the
-// remaining offsets are plain butterflies.  Returns the sum of value index `which` (also returned) — every value index
-// is held by W / NV lanes.
-template <int NV, int OFF>
-__device__ __forceinline__ float transpose_reduce(float (&v)[NV], int lane, int &which) {
-  if constexpr (OFF == 0) {
-    return v[0];
-  } else if constexpr (NV > 1) {
-    const bool up = (lane & OFF) != 0;
-    float w[NV / 2];
-#pragma unroll
-    for (int j = 0; j < NV / 2; ++j) {
-      const float send = up ? v[j] : v[j + NV / 2];
-      const float keep = up ? v[j + NV / 2] : v[j];
-      w[j] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
-    }
-    which = which * 2 + (up ? 1 : 0);
-    return transpose_reduce<NV / 2, OFF / 2>(w, lane, which);
-  } else {
-    float w[1] = {v[0] + __shfl_xor_sync(0xffffffffu, v[0], OFF)};
-    return transpose_reduce<1, OFF / 2>(w, lane, which);
-  }
-}
-
-__device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
 // DET: the sums across warps and CTAs go to the partials of the deterministic build (see ScanBwdTmaParams), not to atomics
 template <typename T, int NP, int MODE, bool DET>
 __device__ __forceinline__ void scan_op_bwd_tma_body(const ScanBwdTmaParams &p) {
@@ -465,29 +436,19 @@ __global__ void scan_combine_rev_kernel(float *carry, long long nrows, int nspli
 // ---- host side ----
 constexpr int kBwdMaxSplit = 64;
 
-template <typename T>
-int scan_op_fwd_tma(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D,
-                    const float *bias, void *out, float *x, float *hs, int batch, int dim, int L, int N, int G, int softplus,
-                    const sigma_scan_strides &s, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream);
-size_t scan_op_tma_workspace_bytes(int batch, int dim, int dstate);
-
-static size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
-
-int sum_parts_det_launch(const float *part, int nparts, long long ncols, long long inner, long long ostride, float *out, cudaStream_t stream);
-
 // scratch of the deterministic build: [dB partials] [dC partials] (dpg / CPW, batch, G, N, L) [dA partials (batch·64, dim, N)]
 // [dD partials] [ddelta_bias partials] (batch·64, dim)
 size_t scan_op_bwd_tma_det_bytes(int batch, int dim, int L, int N, int G) {
   const size_t cpw = N >= 16 ? 16 : 32, ntile = (size_t)(dim / G) / cpw, segs = (size_t)batch * kBwdMaxSplit;
-  return 2 * al256(ntile * batch * G * N * L * sizeof(float)) + al256(segs * dim * N * sizeof(float)) + 2 * al256(segs * dim * sizeof(float));
+  return 2 * align256(ntile * batch * G * N * L * sizeof(float)) + align256(segs * dim * N * sizeof(float)) + 2 * align256(segs * dim * sizeof(float));
 }
 
 // workspace = [hs (batch, dim, ntiles, N)] [forward-split carry] [reverse-split carry]
 size_t scan_op_bwd_tma_workspace_bytes(int batch, int dim, int L, int N, int elem_bytes) {
   (void)elem_bytes;
   const size_t nhs = (L + OPT_HS_POS - 1) / OPT_HS_POS;
-  return al256((size_t)batch * dim * nhs * N * sizeof(float)) + al256(scan_op_tma_workspace_bytes(batch, dim, N)) +
-         al256((size_t)batch * dim * kBwdMaxSplit * 2 * N * sizeof(float));
+  return align256((size_t)batch * dim * nhs * N * sizeof(float)) + align256(scan_op_tma_workspace_bytes(batch, dim, N)) +
+         align256((size_t)batch * dim * kBwdMaxSplit * 2 * N * sizeof(float));
 }
 
 template <typename T>
@@ -576,8 +537,8 @@ int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void
     return SIGMA_EWORKSPACE;
   }
   const int ntiles = (L + LT - 1) / LT;
-  const size_t hs_b = al256((size_t)batch * dim * ((L + OPT_HS_POS - 1) / OPT_HS_POS) * N * sizeof(float));
-  const size_t fc_b = al256(scan_op_tma_workspace_bytes(batch, dim, N));
+  const size_t hs_b = align256((size_t)batch * dim * ((L + OPT_HS_POS - 1) / OPT_HS_POS) * N * sizeof(float));
+  const size_t fc_b = align256(scan_op_tma_workspace_bytes(batch, dim, N));
   float *hs = (float *)ws;
   void *fcarry = (char *)ws + hs_b;
   float *rcarry = (float *)((char *)ws + hs_b + fc_b);
@@ -607,8 +568,8 @@ int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void
   p.batch = batch; p.dim = dim; p.L = L; p.N = N; p.G = G; p.dpg = dim / G; p.softplus = softplus;
   if (det_ws) {   // layout of scan_op_bwd_tma_det_bytes
     const size_t cpw = N >= 16 ? 16 : 32, ntile = (size_t)p.dpg / cpw, segs = (size_t)batch * kBwdMaxSplit;
-    const size_t bc = al256(ntile * batch * G * N * L * sizeof(float)), da = al256(segs * dim * N * sizeof(float));
-    const size_t dd = al256(segs * dim * sizeof(float));
+    const size_t bc = align256(ntile * batch * G * N * L * sizeof(float)), da = align256(segs * dim * N * sizeof(float));
+    const size_t dd = align256(segs * dim * sizeof(float));
     char *w = (char *)det_ws;
     p.part_B = (float *)w; p.part_C = (float *)(w + bc); p.part_dA = (float *)(w + 2 * bc);
     p.part_dD = (float *)(w + 2 * bc + da); p.part_db = (float *)(w + 2 * bc + da + dd);
@@ -629,16 +590,16 @@ int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void
     uint32_t box[3] = {(uint32_t)LT, (uint32_t)p.DT, 1};
     uint32_t boxw[3] = {(uint32_t)LT, (uint32_t)(32 / lpc), 1};
     const CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_64B;
-    if ((rc = make_tmap_generic(&p.m_u, OpT<T>::kType, 3, u, dims, str, box, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
-    if ((rc = make_tmap_generic(&p.m_dl, OpT<T>::kType, 3, delta, dims, str, box, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
-    if ((rc = make_tmap_generic(&p.m_do, OpT<T>::kType, 3, dout, dims, str, box, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
-    if ((rc = make_tmap_generic(&p.m_du, OpT<T>::kType, 3, du, dims, str, boxw, sw, CU_TENSOR_MAP_L2_PROMOTION_NONE))) return rc;
-    if ((rc = make_tmap_generic(&p.m_dd, OpT<T>::kType, 3, ddelta, dims, str, boxw, sw, CU_TENSOR_MAP_L2_PROMOTION_NONE))) return rc;
+    if ((rc = make_tmap(&p.m_u, OpT<T>::kType, 3, u, dims, str, box, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if ((rc = make_tmap(&p.m_dl, OpT<T>::kType, 3, delta, dims, str, box, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if ((rc = make_tmap(&p.m_do, OpT<T>::kType, 3, dout, dims, str, box, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if ((rc = make_tmap(&p.m_du, OpT<T>::kType, 3, du, dims, str, boxw, sw, CU_TENSOR_MAP_L2_PROMOTION_NONE))) return rc;
+    if ((rc = make_tmap(&p.m_dd, OpT<T>::kType, 3, ddelta, dims, str, boxw, sw, CU_TENSOR_MAP_L2_PROMOTION_NONE))) return rc;
     uint64_t dimb[4] = {(uint64_t)L, (uint64_t)N, (uint64_t)G, (uint64_t)batch};
     uint64_t strb[3] = {(uint64_t)L * sz, (uint64_t)N * L * sz, (uint64_t)G * N * L * sz};
     uint32_t boxb[4] = {(uint32_t)LT, (uint32_t)NP, 1, 1};
-    if ((rc = make_tmap_generic(&p.m_B, OpT<T>::kType, 4, B, dimb, strb, boxb, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
-    if ((rc = make_tmap_generic(&p.m_C, OpT<T>::kType, 4, C, dimb, strb, boxb, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if ((rc = make_tmap(&p.m_B, OpT<T>::kType, 4, B, dimb, strb, boxb, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if ((rc = make_tmap(&p.m_C, OpT<T>::kType, 4, C, dimb, strb, boxb, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
   }
   switch (NP) {
     case 4: return launch_bwd_tma<T, 4>(p, stream);

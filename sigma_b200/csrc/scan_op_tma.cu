@@ -22,31 +22,6 @@
 
 namespace sigma {
 
-void *get_tensor_map_encoder();   // ss2d_scan_host.cu
-
-typedef CUresult (*EncodeTiledFnG)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-int make_tmap_generic(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,
-                      const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo) {
-  EncodeTiledFnG fn = (EncodeTiledFnG)get_tensor_map_encoder();
-  if (!fn) return SIGMA_ECUDA;
-  cuuint64_t gdim[5], gstr[4];
-  cuuint32_t bdim[5], estr[5];
-  for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bdim[i] = box[i]; estr[i] = 1; }
-  for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  CUresult r = fn(map, dtype, (cuuint32_t)rank, const_cast<void *>(base), gdim, gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
-                  promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed (CUresult %d): rank=%d dims=(%llu,%llu,%llu) strides=(%llu,%llu) box=(%u,%u,%u) base=%p",
-              (int)r, rank, (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2],
-              (unsigned long long)strides_bytes[0], (unsigned long long)strides_bytes[1], box[0], box[1], box[2], base);
-    return SIGMA_ECUDA;
-  }
-  return SIGMA_OK;
-}
-
 // Opt a kernel into the full 227 KB of dynamic shared memory, once per kernel and process (cudaFuncSetAttribute on every
 // call was a measurable part of the small-batch launch floor).
 cudaError_t prep_kernel_once(const void *fn) {
@@ -300,8 +275,6 @@ __global__ void __launch_bounds__(128, OpCfg<NP>::CTAS) scan_op_tma_kernel(const
   }
 }
 
-__global__ void scan_combine_kernel(float *carry, long long nrows, int nsplit, int NP);   // scan_op.cu
-
 // ---- host side ----
 constexpr int kOpMaxSplit = 64;
 
@@ -431,17 +404,17 @@ int scan_op_fwd_tma(const void *u, const void *delta, const float *A, const void
     uint64_t st_u[2] = {(uint64_t)s.u_dim * sz, (uint64_t)s.u_batch * sz};
     uint64_t st_d[2] = {(uint64_t)s.delta_dim * sz, (uint64_t)s.delta_batch * sz};
     uint64_t st_o[2] = {(uint64_t)s.out_dim * sz, (uint64_t)s.out_batch * sz};
-    if ((rc = make_tmap_generic(&p.m_u, OpT<T>::kType, 3, u, dims, st_u, box, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
-    if ((rc = make_tmap_generic(&p.m_dl, OpT<T>::kType, 3, delta, dims, st_d, box, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if ((rc = make_tmap(&p.m_u, OpT<T>::kType, 3, u, dims, st_u, box, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if ((rc = make_tmap(&p.m_dl, OpT<T>::kType, 3, delta, dims, st_d, box, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
     uint32_t boxo[3] = {(uint32_t)LT, 32, 1};
     if (out != nullptr &&
-        (rc = make_tmap_generic(&p.m_out, OpT<T>::kType, 3, out, dims, st_o, boxo, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE))) return rc;
+        (rc = make_tmap(&p.m_out, OpT<T>::kType, 3, out, dims, st_o, boxo, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE))) return rc;
     uint64_t dimb[4] = {(uint64_t)L, (uint64_t)N, (uint64_t)G, (uint64_t)batch};
     uint32_t boxb[4] = {(uint32_t)LT, (uint32_t)NP, 1, 1};
     uint64_t st_B[3] = {(uint64_t)s.B_dstate * sz, (uint64_t)s.B_group * sz, (uint64_t)s.B_batch * sz};
     uint64_t st_C[3] = {(uint64_t)s.C_dstate * sz, (uint64_t)s.C_group * sz, (uint64_t)s.C_batch * sz};
-    if ((rc = make_tmap_generic(&p.m_B, OpT<T>::kType, 4, B, dimb, st_B, boxb, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
-    if ((rc = make_tmap_generic(&p.m_C, OpT<T>::kType, 4, C, dimb, st_C, boxb, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if ((rc = make_tmap(&p.m_B, OpT<T>::kType, 4, B, dimb, st_B, boxb, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
+    if ((rc = make_tmap(&p.m_C, OpT<T>::kType, 4, C, dimb, st_C, boxb, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))) return rc;
   }
   switch (NP) {
     case 4: return launch_tma<T, 4>(p, out != nullptr, stream);

@@ -34,11 +34,6 @@ template <> struct OpT<__nv_bfloat16> {
   static constexpr CUtensorMapDataType kType = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
 };
 
-template <typename T> __device__ __forceinline__ float opt_to_f32(T v);
-template <> __device__ __forceinline__ float opt_to_f32<float>(float v) { return v; }
-template <> __device__ __forceinline__ float opt_to_f32<__half>(__half v) { return __half2float(v); }
-template <> __device__ __forceinline__ float opt_to_f32<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
-
 // byte offset of 16-byte chunk c of row r inside a 64-byte-row tile written by TMA with CU_TENSOR_MAP_SWIZZLE_64B
 // (address bits [4,6) are XORed with bits [7,9); the tile base is 512-byte aligned)
 __device__ __forceinline__ uint32_t sw64_off(int r, int c) { return (uint32_t)(r * OPT_ROW_BYTES + ((c ^ ((r >> 1) & 3)) << 4)); }
@@ -57,23 +52,14 @@ __device__ __forceinline__ void load_group(const unsigned char *tile, int r, int
       const uint4 t = *reinterpret_cast<const uint4 *>(tile + sw64_off(r, g));
       const T *e = reinterpret_cast<const T *>(&t);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = opt_to_f32<T>(e[i]);
+      for (int i = 0; i < 8; ++i) v[i] = to_f32(e[i]);
     } else {
       const uint2 t = *reinterpret_cast<const uint2 *>(tile + sw64_off(r, g >> 1) + ((g & 1) << 3));
       const T *e = reinterpret_cast<const T *>(&t);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) v[i] = opt_to_f32<T>(e[i]);
+      for (int i = 0; i < 4; ++i) v[i] = to_f32(e[i]);
     }
   }
-}
-
-__device__ __forceinline__ uint32_t pack_half2(float a, float b, __half) {
-  const __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t *>(&h);
-}
-__device__ __forceinline__ uint32_t pack_half2(float a, float b, __nv_bfloat16) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<const uint32_t *>(&h);
 }
 
 // the inverse: G fp32 values -> T, stored at the same (swizzled) place of a tile
@@ -86,12 +72,12 @@ __device__ __forceinline__ void store_group(unsigned char *tile, int r, int g, c
   } else {
     if constexpr (G == 8) {
       uint4 t;
-      t.x = pack_half2(v[0], v[1], T()); t.y = pack_half2(v[2], v[3], T());
-      t.z = pack_half2(v[4], v[5], T()); t.w = pack_half2(v[6], v[7], T());
+      t.x = from_f32x2<T>(v[0], v[1]); t.y = from_f32x2<T>(v[2], v[3]);
+      t.z = from_f32x2<T>(v[4], v[5]); t.w = from_f32x2<T>(v[6], v[7]);
       *reinterpret_cast<uint4 *>(tile + sw64_off(r, g)) = t;
     } else {
       uint2 t;
-      t.x = pack_half2(v[0], v[1], T()); t.y = pack_half2(v[2], v[3], T());
+      t.x = from_f32x2<T>(v[0], v[1]); t.y = from_f32x2<T>(v[2], v[3]);
       *reinterpret_cast<uint2 *>(tile + sw64_off(r, g >> 1) + ((g & 1) << 3)) = t;
     }
   }
@@ -106,30 +92,11 @@ __device__ __forceinline__ void transpose_bc(const unsigned char *rawB, const un
 #pragma unroll
   for (int j = 0; j < NP / LPR; ++j) {
     const int l = lane % LT, n = j * LPR + lane / LT;
-    const float b = opt_to_f32<T>(*reinterpret_cast<const T *>(rawB + n * OPT_ROW_BYTES + l * sizeof(T)));
-    const float c = opt_to_f32<T>(*reinterpret_cast<const T *>(rawC + n * OPT_ROW_BYTES + l * sizeof(T)));
+    const float b = to_f32(*reinterpret_cast<const T *>(rawB + n * OPT_ROW_BYTES + l * sizeof(T)));
+    const float c = to_f32(*reinterpret_cast<const T *>(rawC + n * OPT_ROW_BYTES + l * sizeof(T)));
     bct[l * PITCH + n] = b;
     bct[l * PITCH + NP + n] = c;
   }
-}
-
-// generic tensor map (rank 3 or 4) with dtype / swizzle / L2 promotion; implemented in scan_op_tma.cu
-int make_tmap_generic(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,
-                      const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo);
-
-cudaError_t prep_kernel_once(const void *fn);   // scan_op_tma.cu
-int pick_segments(long long ctas_base, int ntiles, long long slots, double pass_factor, int max_split);   // scan_op_tma.cu
-
-// global <- shared, 3-D box (per-warp y / gradient rows)
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap *map, const void *smem_src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"((uint64_t)map),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(smem_u32(smem_dst)), "l"((uint64_t)map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
 }
 
 }  // namespace sigma

@@ -29,12 +29,6 @@
 
 namespace sigma {
 
-int make_tmap_f32_4d(CUtensorMap *map, const void *base, const uint64_t dims[4], const uint64_t strides_bytes[3], const uint32_t box[4]);
-int pick_segments(long long ctas_base, int ntiles, long long slots, double pass_factor, int max_split);   // scan_op_tma.cu
-cudaError_t prep_kernel_once(const void *fn);                                                            // scan_op_tma.cu
-__global__ void scan_combine_kernel(float *carry, long long nrows, int nsplit, int NP);                  // scan_op.cu
-__global__ void scan_combine_rev_kernel(float *carry, long long nrows, int nsplit, int NP);              // scan_op_bwd_tma.cu
-
 constexpr int FB_LT = 16;   // positions per tile
 constexpr int FB_DT = 64;   // channels per CTA
 
@@ -59,34 +53,6 @@ template <int N> struct FbCfg {
   static constexpr int NS = N / LPC;
   static constexpr int CPW = 32 / LPC;
 };
-
-__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap *map, const void *smem_src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"((uint64_t)map),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-
-// see scan_op_bwd_tma.cu
-template <int NV, int OFF>
-__device__ __forceinline__ float fb_transpose_reduce(float (&v)[NV], int lane, int &which) {
-  if constexpr (OFF == 0) {
-    return v[0];
-  } else if constexpr (NV > 1) {
-    const bool up = (lane & OFF) != 0;
-    float w[NV / 2];
-#pragma unroll
-    for (int j = 0; j < NV / 2; ++j) {
-      const float send = up ? v[j] : v[j + NV / 2];
-      const float keep = up ? v[j + NV / 2] : v[j];
-      w[j] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
-    }
-    which = which * 2 + (up ? 1 : 0);
-    return fb_transpose_reduce<NV / 2, OFF / 2>(w, lane, which);
-  } else {
-    float w[1] = {v[0] + __shfl_xor_sync(0xffffffffu, v[0], OFF)};
-    return fb_transpose_reduce<1, OFF / 2>(w, lane, which);
-  }
-}
 
 // everything the three kernels share: CTA coordinates, the direction's tile geometry, the ring
 struct FbWalk {
@@ -394,8 +360,8 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
       }
       // dB / dC: sum over the CPW channels of this warp that share the lane's state set, one coalesced red per row
       int wb = 0, wc = 0;
-      const float rB = fb_transpose_reduce<NS, CPW / 2>(cB, lane, wb);
-      const float rC = fb_transpose_reduce<NS, CPW / 2>(cC, lane, wc);
+      const float rB = transpose_reduce<NS, CPW / 2>(cB, lane, wb);
+      const float rC = transpose_reduce<NS, CPW / 2>(cC, lane, wc);
       constexpr int DUP = CPW / NS;
       if ((cl & (DUP - 1)) == 0) {
         const long long pos = (long long)o * p.pso[w.k] + (long long)(i0 + r) * p.psi[w.k];
@@ -471,9 +437,6 @@ __global__ void __launch_bounds__(128, 2) ss2d_bwd_det_kernel(const __grid_const
 // ---- host ----
 constexpr int kFbMaxSplit = 64;
 
-static size_t fb_al(size_t v) { return (v + 255) & ~(size_t)255; }
-
-int ss2d_save_tiles(int kind, int H, int W);
 static int fb_max_tiles(int kind, int H, int W) { return ss2d_save_tiles(kind, H, W); }
 int ss2d_save_tiles(int kind, int H, int W) {
   const long long L = (long long)H * W;
@@ -490,7 +453,7 @@ size_t ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N) {
 size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
   const int K = kind == SIGMA_DIRS_CROSS4 ? 4 : 2;
   const size_t carry = (size_t)batch * K * D * kFbMaxSplit * 2 * N * sizeof(float);
-  return fb_al((size_t)K * batch * fb_max_tiles(kind, H, W) * D * N * sizeof(float)) + 2 * fb_al(carry);
+  return align256((size_t)K * batch * fb_max_tiles(kind, H, W) * D * N * sizeof(float)) + 2 * align256(carry);
 }
 
 // the deterministic build appends [du slabs (K, batch, Lseq, D)] [dB / dC partials (D / CPW, batch, Lseq, K, 2N)]
@@ -503,10 +466,10 @@ static FbDetLayout fb_det_layout(int kind, int batch, int H, int W, int D, int N
   const size_t segs = (size_t)batch * kFbMaxSplit;
   FbDetLayout l;
   l.du = ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N);
-  l.bc = l.du + fb_al((size_t)K * batch * Lseq * D * sizeof(float));
-  l.dA = l.bc + fb_al((size_t)(D / CPW) * batch * Lseq * K * 2 * N * sizeof(float));
-  l.dD = l.dA + fb_al(segs * K * D * N * sizeof(float));
-  l.total = l.dD + 2 * fb_al(segs * K * D * sizeof(float));
+  l.bc = l.du + align256((size_t)K * batch * Lseq * D * sizeof(float));
+  l.dA = l.bc + align256((size_t)(D / CPW) * batch * Lseq * K * 2 * N * sizeof(float));
+  l.dD = l.dA + align256(segs * K * D * N * sizeof(float));
+  l.total = l.dD + 2 * align256(segs * K * D * sizeof(float));
   return l;
 }
 
@@ -540,8 +503,6 @@ int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int forc
   return SIGMA_OK;
 }
 
-int sum_parts_det_launch(const float *part, int nparts, long long ncols, long long inner, long long ostride, float *out, cudaStream_t stream);
-
 // delta / ddelta: (K, batch, Lseq, D) slabs stored at the position a value belongs to; dxc (batch, Lseq, D) and dxdbl
 // (batch, Lseq, K, Cp) are ACCUMULATED INTO after being zeroed here; dA (K·D, N), dDs (K·D), ddtb (K, D) overwritten.
 // det: the main sweep writes partials (see fb_det_layout) that sum_parts_det_kernel adds in a fixed order.
@@ -562,13 +523,17 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
   p.dxdbl = dxdbl; p.dA = dA; p.dDs = dDs; p.ddtb = ddtb;
   p.D = D; p.N = N; p.R = R; p.Cp = Cp; p.K = K; p.batch = batch; p.Lseq = Lseq;
   p.max_tiles = fb_max_tiles(kind, H, W);
-  const size_t hs_b = fb_al((size_t)K * batch * p.max_tiles * D * N * sizeof(float));
-  const size_t carry_b = fb_al((size_t)batch * K * D * kFbMaxSplit * 2 * N * sizeof(float));
+  const size_t hs_b = align256((size_t)K * batch * p.max_tiles * D * N * sizeof(float));
+  const size_t carry_b = align256((size_t)batch * K * D * kFbMaxSplit * 2 * N * sizeof(float));
   p.hs = (float *)ws;
   p.hs_in = hs_saved ? hs_saved : p.hs;   // hs_saved: the training forward already wrote delta' and the block-start states
   float *fcarry = (float *)((char *)ws + hs_b), *rcarry = (float *)((char *)ws + hs_b + carry_b);
   const int CPW = N >= 16 ? 16 : 32;
   int rc;
+  auto tmap = [](CUtensorMap *map, const void *base, const uint64_t *dims, const uint64_t *str, const uint32_t *box) {
+    return make_tmap(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+  };
   for (int k = 0; k < K; ++k) {
     const bool colmajor = kind == SIGMA_DIRS_CROSS4 && (k & 1);
     p.rev[k] = kind == SIGMA_DIRS_CROSS4 ? (k >= 2) : (k == 1);
@@ -583,18 +548,18 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
       dims[0] = D; dims[1] = H; dims[2] = W; dims[3] = batch;
       str[0] = (uint64_t)W * D * 4; str[1] = (uint64_t)D * 4; str[2] = (uint64_t)Lseq * D * 4;
     }
-    if ((rc = make_tmap_f32_4d(&p.m_xc[k], xc, dims, str, box))) return rc;
-    if ((rc = make_tmap_f32_4d(&p.m_dy[k], dy, dims, str, box))) return rc;
-    if ((rc = make_tmap_f32_4d(&p.m_dxc[k], dxc, dims, str, boxw))) return rc;
+    if ((rc = tmap(&p.m_xc[k], xc, dims, str, box))) return rc;
+    if ((rc = tmap(&p.m_dy[k], dy, dims, str, box))) return rc;
+    if ((rc = tmap(&p.m_dxc[k], dxc, dims, str, boxw))) return rc;
     dims[3] = (uint64_t)K * batch;   // slabs: image index k·batch + b
-    if ((rc = make_tmap_f32_4d(&p.m_dl[k], delta, dims, str, box))) return rc;
+    if ((rc = tmap(&p.m_dl[k], delta, dims, str, box))) return rc;
     dims[3] = batch;
     uint32_t boxd[4] = {(uint32_t)Cp, (uint32_t)FB_LT, 1, 1};
     dims[0] = Cp;
     const uint64_t pos = (uint64_t)K * Cp * 4;
     if (!colmajor) { str[0] = pos; str[1] = Lseq * pos; str[2] = Lseq * pos; }
     else { str[0] = W * pos; str[1] = pos; str[2] = Lseq * pos; }
-    if ((rc = make_tmap_f32_4d(&p.m_dbl[k], xdbl + (long long)k * Cp, dims, str, boxd))) return rc;
+    if ((rc = tmap(&p.m_dbl[k], xdbl + (long long)k * Cp, dims, str, boxd))) return rc;
   }
   const FbPlan pl = fb_plan(kind, batch, H, W, D, N, force_split);
   p.tiles_per_split = pl.tiles_per_split;
@@ -620,7 +585,7 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
         dims[0] = D; dims[1] = H; dims[2] = W; dims[3] = (uint64_t)K * batch;
         str[0] = (uint64_t)W * D * 4; str[1] = (uint64_t)D * 4; str[2] = (uint64_t)Lseq * D * 4;
       }
-      int r = make_tmap_f32_4d(maps ? &maps[k] : &p.m_dd[k], slab, dims, str, boxw);
+      int r = tmap(maps ? &maps[k] : &p.m_dd[k], slab, dims, str, boxw);
       if (r) return r;
     }
     return SIGMA_OK;

@@ -2,12 +2,13 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <string>
 
 #include "ss2d_scan.cuh"
 
 namespace sigma {
 
-// ---- tensor map creation through the runtime-resolved driver entry point ----
+// ---- tensor maps: the one caller of cuTensorMapEncodeTiled, through the runtime-resolved driver entry point ----
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -26,31 +27,31 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-void *get_tensor_map_encoder() { return (void *)get_encode_fn(); }
-
-int make_tmap_f32_4d(CUtensorMap *map, const void *base, const uint64_t dims[4], const uint64_t strides_bytes[3],
-                     const uint32_t box[4]) {
+int make_tmap(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,
+              const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return SIGMA_ECUDA;
-  cuuint64_t gdim[4] = {dims[0], dims[1], dims[2], dims[3]};
-  cuuint64_t gstr[3] = {strides_bytes[0], strides_bytes[1], strides_bytes[2]};
-  cuuint32_t bdim[4] = {box[0], box[1], box[2], box[3]};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<void *>(base), gdim, gstr, bdim, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  cuuint64_t gdim[5], gstr[4];
+  cuuint32_t bdim[5], estr[5];
+  for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bdim[i] = box[i]; estr[i] = 1; }
+  for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
+  CUresult r = fn(map, dtype, (cuuint32_t)rank, const_cast<void *>(base), gdim, gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
+                  promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed (CUresult %d): dims=(%llu,%llu,%llu,%llu) strides=(%llu,%llu,%llu) "
-              "box=(%u,%u,%u,%u) base=%p",
-              (int)r, (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2],
-              (unsigned long long)dims[3], (unsigned long long)strides_bytes[0], (unsigned long long)strides_bytes[1],
-              (unsigned long long)strides_bytes[2], box[0], box[1], box[2], box[3], base);
+    std::string d, st, bx;
+    for (int i = 0; i < rank; ++i) {
+      d += (i ? "," : "") + std::to_string(dims[i]);
+      bx += (i ? "," : "") + std::to_string(box[i]);
+      if (i + 1 < rank) st += (i ? "," : "") + std::to_string(strides_bytes[i]);
+    }
+    set_error("cuTensorMapEncodeTiled failed (CUresult %d): rank=%d dims=(%s) strides=(%s) box=(%s) base=%p", (int)r, rank, d.c_str(),
+              st.c_str(), bx.c_str(), base);
     return SIGMA_ECUDA;
   }
   return SIGMA_OK;
 }
 
-static int pad_rp(int R) {
+int pad_rp(int R) {
   const int opts[] = {4, 8, 12, 16, 24, 32, 48, 64};
   for (int o : opts)
     if (R <= o) return o;
@@ -89,8 +90,6 @@ static int pick_warps(int D, int cpt, int maxw) {
 
 constexpr int kMaxSplit = 32;
 
-int ss2d_save_tiles(int kind, int H, int W);   // ss2d_scan_bwd.cu: 16-position blocks of the longest walk
-
 // Which register budget to run (`CTAS` of ss2d_scan_kernel): the scans are MUFU / MIO-limited, so more resident warps than
 // 12 buy little; d_state 16 at dt_rank 24 (stage 2, nine blocks) is the one case that runs 16.  SIGMA_SCAN_CTAS overrides.
 static int ss2d_pick_ctas(int N, int rp) {
@@ -126,14 +125,11 @@ static int ss2d_pick_segments(long long ctas, int nw, int ntiles, int N) {
   return best_n;
 }
 
-int ss2d_pick_segments_hook(long long ctas, int nw, int ntiles, int N) { return ss2d_pick_segments(ctas, nw, ntiles, N); }   // api.cu test hook
+int ss2d_pick_segments_hook(long long ctas, int nw, int ntiles, int N) { return ss2d_pick_segments(ctas, nw, ntiles, N); }
 
 size_t ss2d_scan_workspace_bytes(int kind, int batch, int D, int N) {
   return (size_t)batch * kind_dirs(kind) * D * kMaxSplit * 2 * N * sizeof(float);
 }
-
-int make_tmap_generic(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void *base, const uint64_t *dims,
-                      const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo);   // scan_op_tma.cu
 
 // The launch plan of the forward: everything ss2d_scan_fwd decides before it builds the tensor maps.  One function, so that the
 // launch and its host-only query (sigma_test_ss2d_fwd_plan) cannot disagree.
@@ -227,7 +223,7 @@ static int ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R,
 }
 
 int ss2d_fwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int R, int xc_bf16, int force_split, size_t ws_bytes,
-                       long long *out8) {   // api.cu: sigma_test_ss2d_fwd_plan
+                       long long *out8) {
   Ss2dFwdPlan pl;
   const bool have_ws = ws_bytes > 0 && ws_bytes >= ss2d_scan_workspace_bytes(kind, batch, D, N);
   const int rc = ss2d_fwd_plan(kind, batch, H, W, D, N, R, xc_bf16, force_split, have_ws, pl);
@@ -277,17 +273,16 @@ int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw
       dims[0] = D; dims[1] = H; dims[2] = W; dims[3] = batch;
       str[0] = (uint64_t)W * D * xes; str[1] = (uint64_t)D * xes; str[2] = (uint64_t)Lseq * D * xes;
     }
-    if ((rc = xc_bf16 ? make_tmap_generic(&p.m_xc[k], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, xc, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE,
-                                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B)
-                      : make_tmap_f32_4d(&p.m_xc[k], xc, dims, str, box))) return rc;
+    if ((rc = make_tmap(&p.m_xc[k], xc_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, xc, dims, str, box,
+                        CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
     // x_dbl (batch, Lseq, K, Cp): direction k's row starts at column k·Cp
     uint32_t boxd[4] = {(uint32_t)Cp, (uint32_t)LT, 1, 1};
     dims[0] = Cp;
     const uint64_t pos = (uint64_t)K * Cp * 4;
     if (!colmajor) { str[0] = pos; str[1] = Lseq * pos; str[2] = Lseq * pos; }
     else { str[0] = W * pos; str[1] = pos; str[2] = Lseq * pos; }
-    if ((rc = make_tmap_f32_4d(&p.m_dbl[k], xdbl + (long long)(kind == SIGMA_DIRS_CROSS ? 0 : k) * Cp, dims, str, boxd)))
-      return rc;
+    if ((rc = make_tmap(&p.m_dbl[k], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, xdbl + (long long)(kind == SIGMA_DIRS_CROSS ? 0 : k) * Cp, dims,
+                        str, boxd, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
   }
   p.tiles_per_split = pl.tiles_per_split;
   p.nsplit = pl.nsplit;

@@ -1,5 +1,5 @@
-// TMA (cp.async.bulk.tensor) + mbarrier wrappers, and host-side tensor-map creation without linking
-// libcuda (the driver entry point is resolved at run time, so the .so loads on a GPU-less box).
+// TMA (cp.async.bulk.tensor) and other bulk-async / mbarrier PTX wrappers.  The host-side tensor maps they take come from
+// make_tmap (internal.cuh).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -81,7 +81,17 @@ __device__ __forceinline__ void mbar_wait_backoff(uint64_t *bar, uint32_t parity
   }
 }
 
-// global -> shared, 4-D tile, completion signalled on an mbarrier (SASS: UTMALDG)
+// global -> shared, 2-D / 3-D / 4-D tile, completion signalled on an mbarrier (SASS: UTMALDG)
+__device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+               ::"r"(smem_u32(smem_dst)), "l"((uint64_t)map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_load_3d(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+               ::"r"(smem_u32(smem_dst)), "l"((uint64_t)map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 __device__ __forceinline__ void tma_load_4d(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1,
                                             int c2, int c3) {
   asm volatile(
@@ -89,10 +99,21 @@ __device__ __forceinline__ void tma_load_4d(void *smem_dst, const CUtensorMap *m
       ::"r"(smem_u32(smem_dst)), "l"((uint64_t)map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-// shared -> global, 4-D tile, bulk-group completion (SASS: UTMASTG); out-of-bounds elements are not written
+// shared -> global, 3-D / 4-D tile, bulk-group completion (SASS: UTMASTG); out-of-bounds elements are not written
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap *map, const void *smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"((uint64_t)map),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap *map, const void *smem_src, int c0, int c1, int c2,
                                              int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"((uint64_t)map),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+// shared -> global element-wise fp32 add, 4-D tile, bulk-group completion
+__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap *map, const void *smem_src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"((uint64_t)map),
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
@@ -109,10 +130,9 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap *map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)map) : "memory");
 }
 
-// ---- host ----
-// fp32 tensor map of rank 4: dims (d0 innermost .. d3), byte strides for d1..d3, box (b0..b3).
-// Returns 0 on success; on failure sets the library error string.
-int make_tmap_f32_4d(CUtensorMap *map, const void *base, const uint64_t dims[4], const uint64_t strides_bytes[3],
-                     const uint32_t box[4]);
+// four consecutive fp32 added to global memory without a return value (one vector red per 16 bytes)
+__device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d) {
+  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
 
 }  // namespace sigma

@@ -9,14 +9,7 @@ import numpy as np
 import torch
 
 from . import _lib
-
-
-def _vp(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+from ._lib import ptr, stream
 
 
 def _cv_round(v):
@@ -34,9 +27,9 @@ def image_pre(src_u8, out, *, scaled_hw=None, scale_xy=None, off=(0, 0), mirror_
     m = (ctypes.c_double * 3)(*[float(v) for v in mean])
     sd = (ctypes.c_double * 3)(*[float(v) for v in std])
     cl = (ctypes.c_int * 4)(*[int(v) for v in clip]) if clip is not None else None
-    rc = _lib.lib().sigma_image_pre_fwd(_vp(src_u8), _vp(labels_u8), _vp(out), _vp(labels_out), H0, W0, SH, SW, float(sy), float(sx), OH, OW,
+    rc = _lib.lib().sigma_image_pre_fwd(ptr(src_u8), ptr(labels_u8), ptr(out), ptr(labels_out), H0, W0, SH, SW, float(sy), float(sx), OH, OW,
                                         int(off[0]), int(off[1]), int(bool(mirror_src)), int(bool(mirror_out)), int(label_pad), cl, m, sd,
-                                        _stream())
+                                        stream())
     _lib.check(rc, "sigma_image_pre_fwd")
 
 
@@ -135,7 +128,7 @@ class DeviceEvaluator:
         acc = torch.zeros((self.n, AH, AW), dtype=torch.float32, device=self.device)
         for i, (ay, ax, vh, vw, oy, ox, tmt, tml) in enumerate(wins):
             lf = logits[nw + i] if self.flip else None
-            rc = L_.sigma_eval_exp_accumulate_fwd(_vp(logits[i]), _vp(lf), _vp(acc), self.n, TH, TW, tmt, tml, vh, vw, AH, AW, ay, ax, _stream())
+            rc = L_.sigma_eval_exp_accumulate_fwd(ptr(logits[i]), ptr(lf), ptr(acc), self.n, TH, TW, tmt, tml, vh, vw, AH, AW, ay, ax, stream())
             _lib.check(rc, "sigma_eval_exp_accumulate_fwd")
         return acc, SH, SW
 
@@ -156,14 +149,14 @@ class DeviceEvaluator:
         L_ = _lib.lib()
         for s in self.scales:
             acc, SH, SW = self._scale(rgb_u8, x_u8, s)
-            rc = L_.sigma_eval_resize_add_fwd(_vp(acc), self.n, acc.shape[1], acc.shape[2], 0, 0, SH, SW, _vp(total), H0, W0, _stream())
+            rc = L_.sigma_eval_resize_add_fwd(ptr(acc), self.n, acc.shape[1], acc.shape[2], 0, 0, SH, SW, ptr(total), H0, W0, stream())
             _lib.check(rc, "sigma_eval_resize_add_fwd")
         pred = torch.empty((H0, W0), dtype=torch.uint8, device=self.device)
         lab = to(labels).to(self.device) if labels is not None else None
         if lab is not None and (lab.dtype != torch.uint8 or tuple(lab.shape) != (H0, W0)):
             raise ValueError("labels must be (H, W) uint8")
-        rc = L_.sigma_eval_argmax_hist_fwd(_vp(total), _vp(lab), _vp(pred), _vp(self.metric.hist), _vp(self.metric.counts), self.n,
-                                           H0 * W0, _stream())
+        rc = L_.sigma_eval_argmax_hist_fwd(ptr(total), ptr(lab), ptr(pred), ptr(self.metric.hist), ptr(self.metric.counts), self.n,
+                                           H0 * W0, stream())
         _lib.check(rc, "sigma_eval_argmax_hist_fwd")
         return pred
 

@@ -22,17 +22,10 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
+from ._lib import ptr, stream
 
 EPS = 1e-5
 _FORCE_SPLIT = 0  # test hook: force the number of L-segments of the fused scan
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 # ---------------------------------------------------------------- primitive wrappers
@@ -41,7 +34,7 @@ def layernorm(x2d, ln, dtype=torch.float32):
     rows, C = x2d.shape
     y = torch.empty((rows, C), dtype=dtype, device=x2d.device)
     fn = "sigma_layernorm_fwd_bf16" if dtype == torch.bfloat16 else "sigma_layernorm_fwd"
-    _lib.check(getattr(_lib.lib(), fn)(_p(x2d), _p(ln.weight), _p(ln.bias), _p(y), rows, C, float(ln.eps), _stream()), fn)
+    _lib.check(getattr(_lib.lib(), fn)(ptr(x2d), ptr(ln.weight), ptr(ln.bias), ptr(y), rows, C, float(ln.eps), stream()), fn)
     return y
 
 
@@ -105,7 +98,7 @@ def _split_weight(w):
     if ent is not None and ent[0]() is w and ent[1] == w._version:
         return ent[2], ent[3]
     hi, lo = torch.empty_like(w), torch.empty_like(w)
-    _lib.check(_lib.lib().sigma_split_tf32_fwd(_p(w), _p(hi), _p(lo), w.numel(), _stream()), "sigma_split_tf32_fwd")
+    _lib.check(_lib.lib().sigma_split_tf32_fwd(ptr(w), ptr(hi), ptr(lo), w.numel(), stream()), "sigma_split_tf32_fwd")
     key = id(w)
     _SPLIT[key] = (weakref.ref(w, lambda _r, k=key: _SPLIT.pop(k, None)), w._version, hi, lo)
     return hi, lo
@@ -151,13 +144,13 @@ def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="d
     w = weight if weight.is_contiguous() else weight.contiguous()
     ldr = residual.stride(0) if residual is not None else 0
     if _dense_precision() == "tf32" and kind not in _FP32_KINDS:
-        rc = _lib.lib().sigma_linear_tf32(_p(x2d), x2d.stride(0), _p(w), _p(bias), _p(residual), ldr, _p(rscale), _p(out),
-                                          out.stride(0), M, N, K, _stream())
+        rc = _lib.lib().sigma_linear_tf32(ptr(x2d), x2d.stride(0), ptr(w), ptr(bias), ptr(residual), ldr, ptr(rscale), ptr(out),
+                                          out.stride(0), M, N, K, stream())
         _lib.check(rc, "sigma_linear_tf32")
     else:
         hi, lo = _split_weight(w)
-        rc = _lib.lib().sigma_linear_tf32x3(_p(x2d), x2d.stride(0), _p(hi), _p(lo), _p(bias), _p(residual), ldr, _p(rscale), _p(out),
-                                            out.stride(0), M, N, K, _stream())
+        rc = _lib.lib().sigma_linear_tf32x3(ptr(x2d), x2d.stride(0), ptr(hi), ptr(lo), ptr(bias), ptr(residual), ldr, ptr(rscale), ptr(out),
+                                            out.stride(0), M, N, K, stream())
         _lib.check(rc, "sigma_linear_tf32x3")
     return out
 
@@ -179,8 +172,8 @@ def _linear_bf16(x2d, weight, bias, out, residual, rscale, out_dtype):
         return out
     ldr = residual.stride(0) if residual is not None else 0
     c_dtype = _lib.BF16 if out.dtype == torch.bfloat16 else _lib.F32
-    rc = _lib.lib().sigma_linear_bf16(_p(x2d), x2d.stride(0), _p(w), _p(bias), _p(residual), ldr, _p(rscale), _p(out), out.stride(0),
-                                      c_dtype, M, N, K, _stream())
+    rc = _lib.lib().sigma_linear_bf16(ptr(x2d), x2d.stride(0), ptr(w), ptr(bias), ptr(residual), ldr, ptr(rscale), ptr(out), out.stride(0),
+                                      c_dtype, M, N, K, stream())
     _lib.check(rc, "sigma_linear_bf16")
     return out
 
@@ -225,7 +218,7 @@ def conv3x3(x, conv, gelu=False):
         hi, lo = w9, None
     else:
         hi, lo = _split_weight(w9)
-    rc = _lib.lib().sigma_conv3x3_tf32(_p(x), _p(hi), _p(lo), _p(conv.bias), 1 if gelu else 0, _p(y), B, H, W, Cin, conv.out_channels, _stream())
+    rc = _lib.lib().sigma_conv3x3_tf32(ptr(x), ptr(hi), ptr(lo), ptr(conv.bias), 1 if gelu else 0, ptr(y), B, H, W, Cin, conv.out_channels, stream())
     _lib.check(rc, "sigma_conv3x3_tf32")
     return y
 
@@ -233,8 +226,8 @@ def conv3x3(x, conv, gelu=False):
 def dwconv3x3_silu(x, x_row_stride, x_batch_stride, conv, out, out_batch_stride, batch, H, W, D):
     """x and out both fp32, or both bf16 (sigma_dwconv3x3_silu_fwd_bf16)."""
     fn = "sigma_dwconv3x3_silu_fwd_bf16" if x.dtype == torch.bfloat16 else "sigma_dwconv3x3_silu_fwd"
-    _lib.check(getattr(_lib.lib(), fn)(_p(x), x_row_stride, x_batch_stride, _p(conv.weight), _p(conv.bias),
-                                       _p(out), out_batch_stride, batch, H, W, D, _stream()), fn)
+    _lib.check(getattr(_lib.lib(), fn)(ptr(x), x_row_stride, x_batch_stride, ptr(conv.weight), ptr(conv.bias),
+                                       ptr(out), out_batch_stride, batch, H, W, D, stream()), fn)
     return out
 
 
@@ -246,16 +239,16 @@ def ss2d_scan(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
     wsb = L_.sigma_ss2d_scan_workspace_bytes(kind, batch, H, W, D, N)
     ws = torch.empty(wsb, dtype=torch.uint8, device=xc.device)
     if xc.dtype == torch.bfloat16:
-        rc = L_.sigma_ss2d_scan_fwd_bf16(kind, _p(xc), _p(xdbl), _p(dtw), _p(dtb), _p(A), _p(Ds), _p(y), batch, H, W, D, N, R, Cp,
-                                         _p(ws), wsb, _stream())
+        rc = L_.sigma_ss2d_scan_fwd_bf16(kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(y), batch, H, W, D, N, R, Cp,
+                                         ptr(ws), wsb, stream())
         _lib.check(rc, "sigma_ss2d_scan_fwd_bf16")
         return y
     if _FORCE_SPLIT:
-        rc = L_.sigma_ss2d_scan_fwd_split(kind, _p(xc), _p(xdbl), _p(dtw), _p(dtb), _p(A), _p(Ds), _p(y), batch, H, W, D, N,
-                                          R, Cp, _p(ws), wsb, _FORCE_SPLIT, _stream())
+        rc = L_.sigma_ss2d_scan_fwd_split(kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(y), batch, H, W, D, N,
+                                          R, Cp, ptr(ws), wsb, _FORCE_SPLIT, stream())
     else:
-        rc = L_.sigma_ss2d_scan_fwd(kind, _p(xc), _p(xdbl), _p(dtw), _p(dtb), _p(A), _p(Ds), _p(y), batch, H, W, D, N, R, Cp,
-                                    _p(ws), wsb, _stream())
+        rc = L_.sigma_ss2d_scan_fwd(kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(y), batch, H, W, D, N, R, Cp,
+                                    ptr(ws), wsb, stream())
     _lib.check(rc, "sigma_ss2d_scan_fwd")
     return y
 
@@ -271,8 +264,8 @@ def ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
     hs = torch.empty(L_.sigma_ss2d_scan_hs_bytes(kind, batch, H, W, D, N) // 4, dtype=torch.float32, device=xc.device)
     wsb = L_.sigma_ss2d_scan_workspace_bytes(kind, batch, H, W, D, N)
     ws = torch.empty(wsb, dtype=torch.uint8, device=xc.device)
-    rc = L_.sigma_ss2d_scan_fwd_save(kind, _p(xc), _p(xdbl), _p(dtw), _p(dtb), _p(A), _p(Ds), _p(y), _p(delta), _p(hs), batch, H, W, D,
-                                     N, R, Cp, _p(ws), wsb, int(_FORCE_SPLIT or 0), _stream())
+    rc = L_.sigma_ss2d_scan_fwd_save(kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(y), ptr(delta), ptr(hs), batch, H, W, D,
+                                     N, R, Cp, ptr(ws), wsb, int(_FORCE_SPLIT or 0), stream())
     _lib.check(rc, "sigma_ss2d_scan_fwd_save")
     return y, delta, hs
 
@@ -283,8 +276,8 @@ def merge_norm_gate(y, K, k_stride, in_batch_stride, ln, z, z_row_stride, gate, 
     fn = "sigma_merge_norm_gate_fwd_bf16" if y.dtype == torch.bfloat16 else "sigma_merge_norm_gate_fwd"
     yp = ctypes.c_void_p(y.data_ptr() + y.element_size() * y_offset)
     op = ctypes.c_void_p(out.data_ptr() + out.element_size() * out_offset)
-    rc = getattr(_lib.lib(), fn)(yp, K, k_stride, in_batch_stride, _p(ln.weight), _p(ln.bias), z, z_row_stride,
-                                 _p(gate), op, out_batch_stride, out_row_stride, rows, rows_per_batch, D, float(ln.eps), _stream())
+    rc = getattr(_lib.lib(), fn)(yp, K, k_stride, in_batch_stride, ptr(ln.weight), ptr(ln.bias), z, z_row_stride,
+                                 ptr(gate), op, out_batch_stride, out_row_stride, rows, rows_per_batch, D, float(ln.eps), stream())
     _lib.check(rc, fn)
     return out
 
@@ -381,7 +374,7 @@ def patch_merging(m, x):
     xn = torch.empty((B * H2 * W2, 4 * C), dtype=torch.bfloat16 if bf16 else torch.float32, device=x.device)
     # 2x2 gather (+ zero padding of odd sizes) + LayerNorm(4C) in one kernel: no concatenated tensor
     fn = "sigma_patch_merge_norm_fwd_bf16" if bf16 else "sigma_patch_merge_norm_fwd"
-    _lib.check(getattr(_lib.lib(), fn)(_p(x), _p(m.norm.weight), _p(m.norm.bias), _p(xn), B, H, W, C, float(m.norm.eps), _stream()), fn)
+    _lib.check(getattr(_lib.lib(), fn)(ptr(x), ptr(m.norm.weight), ptr(m.norm.bias), ptr(xn), B, H, W, C, float(m.norm.eps), stream()), fn)
     return linear(xn, m.reduction.weight).view(B, H2, W2, -1)
 
 
@@ -455,8 +448,8 @@ def upsample2x_norm(x, ln):
     x = x.contiguous()
     B, H, W, C = x.shape
     y = torch.empty((B, 2 * H, 2 * W, C), dtype=torch.float32, device=x.device)
-    wp, bp, eps = (_p(ln.weight), _p(ln.bias), float(ln.eps)) if ln is not None else (None, None, 0.0)
-    _lib.check(_lib.lib().sigma_upsample2x_norm_fwd(_p(x), wp, bp, _p(y), B, H, W, C, eps, _stream()),
+    wp, bp, eps = (ptr(ln.weight), ptr(ln.bias), float(ln.eps)) if ln is not None else (None, None, 0.0)
+    _lib.check(_lib.lib().sigma_upsample2x_norm_fwd(ptr(x), wp, bp, ptr(y), B, H, W, C, eps, stream()),
                "sigma_upsample2x_norm_fwd")
     return y
 
@@ -468,8 +461,8 @@ def upsample2x_norm_head(x, ln, conv1x1):
     ncls = conv1x1.weight.shape[0]
     w = conv1x1.weight.view(ncls, C)
     out = torch.empty((B, ncls, 2 * H, 2 * W), dtype=torch.float32, device=x.device)
-    _lib.check(_lib.lib().sigma_upsample2x_norm_head_fwd(_p(x), _p(ln.weight), _p(ln.bias), _p(w), ncls, _p(out), B, H, W, C,
-                                                          float(ln.eps), _stream()), "sigma_upsample2x_norm_head_fwd")
+    _lib.check(_lib.lib().sigma_upsample2x_norm_head_fwd(ptr(x), ptr(ln.weight), ptr(ln.bias), ptr(w), ncls, ptr(out), B, H, W, C,
+                                                          float(ln.eps), stream()), "sigma_upsample2x_norm_head_fwd")
     return out
 
 
@@ -481,7 +474,7 @@ def pool_avgmax(t):
     # of them (B = 1, 30x40 map: 4 CTAs took 74 us), at least 32 positions per slice
     nslice = max(1, min(64, L // 32, max(L // 256, -(-296 // B))))
     part = torch.empty((B, nslice, 2, C), dtype=torch.float32, device=t.device)
-    _lib.check(_lib.lib().sigma_pool_avgmax_partial_fwd(_p(t), _p(part), B, L, C, nslice, _stream()), "sigma_pool_avgmax_partial_fwd")
+    _lib.check(_lib.lib().sigma_pool_avgmax_partial_fwd(ptr(t), ptr(part), B, L, C, nslice, stream()), "sigma_pool_avgmax_partial_fwd")
     return part[:, :, 0].sum(1) / L, part[:, :, 1].amax(1)
 
 
@@ -490,7 +483,7 @@ def scale_add(a, sa, b, sb, rows_per_batch):
     out = torch.empty_like(b)
     C = b.shape[-1]
     rows = b.numel() // C
-    _lib.check(_lib.lib().sigma_scale_add_fwd(_p(a), _p(sa), _p(b), _p(sb), _p(out), rows, rows_per_batch, C, _stream()),
+    _lib.check(_lib.lib().sigma_scale_add_fwd(ptr(a), ptr(sa), ptr(b), ptr(sb), ptr(out), rows, rows_per_batch, C, stream()),
                "sigma_scale_add_fwd")
     return out
 
@@ -521,8 +514,8 @@ def patch_expand(m, x):
     B, H, W, C = x.shape
     y = linear(x.reshape(B * H * W, C), m.expand.weight)             # (B·H·W, 2C) = "b h w (p1 p2 c)"
     out = torch.empty((B, 2 * H, 2 * W, C // 2), dtype=torch.float32, device=x.device)
-    _lib.check(_lib.lib().sigma_pixel_shuffle_norm_fwd(_p(y), _p(m.norm.weight), _p(m.norm.bias), _p(out), B, H, W, C // 2,
-                                                        float(m.norm.eps), _stream()), "sigma_pixel_shuffle_norm_fwd")
+    _lib.check(_lib.lib().sigma_pixel_shuffle_norm_fwd(ptr(y), ptr(m.norm.weight), ptr(m.norm.bias), ptr(out), B, H, W, C // 2,
+                                                        float(m.norm.eps), stream()), "sigma_pixel_shuffle_norm_fwd")
     return out
 
 

@@ -11,16 +11,9 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
+from ._lib import ptr, stream
 
 _DTYPE = {torch.float32: _lib.F32, torch.float16: _lib.F16, torch.bfloat16: _lib.BF16}
-
-
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def deterministic():
@@ -77,13 +70,13 @@ def selective_scan_cuda_core_fwd(u, delta, A, B, C, D=None, delta_bias=None, del
     wsb = L_.sigma_scan_fwd_workspace_bytes(batch, dim, L, N, G, dt)
     ws = torch.empty(wsb, dtype=torch.uint8, device=u.device)
     if _force_split:
-        rc = L_.sigma_scan_fwd_split(_ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C), _ptr(D), _ptr(delta_bias),
-                                     _ptr(out), _ptr(x), batch, dim, L, N, G, dt, int(bool(delta_softplus)),
-                                     ctypes.byref(st), _ptr(ws), wsb, int(_force_split), _stream())
+        rc = L_.sigma_scan_fwd_split(ptr(u), ptr(delta), ptr(A), ptr(B), ptr(C), ptr(D), ptr(delta_bias),
+                                     ptr(out), ptr(x), batch, dim, L, N, G, dt, int(bool(delta_softplus)),
+                                     ctypes.byref(st), ptr(ws), wsb, int(_force_split), stream())
     else:
-        rc = L_.sigma_scan_fwd(_ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C), _ptr(D), _ptr(delta_bias),
-                               _ptr(out), _ptr(x), batch, dim, L, N, G, dt, int(bool(delta_softplus)),
-                               ctypes.byref(st), _ptr(ws), wsb, _stream())
+        rc = L_.sigma_scan_fwd(ptr(u), ptr(delta), ptr(A), ptr(B), ptr(C), ptr(D), ptr(delta_bias),
+                               ptr(out), ptr(x), batch, dim, L, N, G, dt, int(bool(delta_softplus)),
+                               ctypes.byref(st), ptr(ws), wsb, stream())
     _lib.check(rc, "sigma_scan_fwd")
     return [out, x]
 
@@ -111,21 +104,21 @@ def selective_scan_cuda_core_bwd(u, delta, A, B, C, D, delta_bias, dout, x, delt
     if deterministic():
         wsb = L_.sigma_scan_bwd_det_workspace_bytes(batch, dim, L, N, G, dt)
         ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=u.device)
-        rc = L_.sigma_scan_bwd_det(_ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C), _ptr(D), _ptr(delta_bias), _ptr(dout),
-                                   _ptr(du), _ptr(ddelta), _ptr(dA), _ptr(dB), _ptr(dC), _ptr(dD), _ptr(dbias),
-                                   batch, dim, L, N, G, dt, int(bool(delta_softplus)), _ptr(ws), wsb, int(_force_split), _stream())
+        rc = L_.sigma_scan_bwd_det(ptr(u), ptr(delta), ptr(A), ptr(B), ptr(C), ptr(D), ptr(delta_bias), ptr(dout),
+                                   ptr(du), ptr(ddelta), ptr(dA), ptr(dB), ptr(dC), ptr(dD), ptr(dbias),
+                                   batch, dim, L, N, G, dt, int(bool(delta_softplus)), ptr(ws), wsb, int(_force_split), stream())
         _lib.check(rc, "sigma_scan_bwd_det")
         return [du, ddelta, dA, dB.to(u.dtype), dC.to(u.dtype), dD, dbias]
     wsb = L_.sigma_scan_bwd_workspace_bytes(batch, dim, L, N, G, dt)
     ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=u.device)
     if _force_split:
-        rc = L_.sigma_scan_bwd_split(_ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C), _ptr(D), _ptr(delta_bias), _ptr(dout),
-                                     _ptr(du), _ptr(ddelta), _ptr(dA), _ptr(dB), _ptr(dC), _ptr(dD), _ptr(dbias),
-                                     batch, dim, L, N, G, dt, int(bool(delta_softplus)), _ptr(ws), wsb, int(_force_split), _stream())
+        rc = L_.sigma_scan_bwd_split(ptr(u), ptr(delta), ptr(A), ptr(B), ptr(C), ptr(D), ptr(delta_bias), ptr(dout),
+                                     ptr(du), ptr(ddelta), ptr(dA), ptr(dB), ptr(dC), ptr(dD), ptr(dbias),
+                                     batch, dim, L, N, G, dt, int(bool(delta_softplus)), ptr(ws), wsb, int(_force_split), stream())
     else:
-        rc = L_.sigma_scan_bwd(_ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C), _ptr(D), _ptr(delta_bias), _ptr(dout),
-                               _ptr(du), _ptr(ddelta), _ptr(dA), _ptr(dB), _ptr(dC), _ptr(dD), _ptr(dbias),
-                               batch, dim, L, N, G, dt, int(bool(delta_softplus)), _ptr(ws), wsb, _stream())
+        rc = L_.sigma_scan_bwd(ptr(u), ptr(delta), ptr(A), ptr(B), ptr(C), ptr(D), ptr(delta_bias), ptr(dout),
+                               ptr(du), ptr(ddelta), ptr(dA), ptr(dB), ptr(dC), ptr(dD), ptr(dbias),
+                               batch, dim, L, N, G, dt, int(bool(delta_softplus)), ptr(ws), wsb, stream())
     _lib.check(rc, "sigma_scan_bwd")
     # the reference returns dB/dC cast to the input dtype (selective_scan.cpp:360)
     return [du, ddelta, dA, dB.to(u.dtype), dC.to(u.dtype), dD, dbias]
@@ -364,7 +357,7 @@ class LayerNormFn(torch.autograd.Function):
         x2 = x.contiguous().view(-1, x.shape[-1])
         y = torch.empty_like(x2)
         w, b = weight.contiguous(), bias.contiguous()
-        _lib.check(_lib.lib().sigma_layernorm_fwd(_ptr(x2), _ptr(w), _ptr(b), _ptr(y), x2.shape[0], x2.shape[1], float(eps), _stream()),
+        _lib.check(_lib.lib().sigma_layernorm_fwd(ptr(x2), ptr(w), ptr(b), ptr(y), x2.shape[0], x2.shape[1], float(eps), stream()),
                    "sigma_layernorm_fwd")
         ctx.save_for_backward(x2, w)
         ctx.eps = float(eps)
@@ -381,11 +374,11 @@ class LayerNormFn(torch.autograd.Function):
             L_ = _lib.lib()
             wsb = L_.sigma_layernorm_bwd_det_workspace_bytes(x2.shape[0], x2.shape[1])
             ws = torch.empty(max(wsb, 16), dtype=torch.uint8, device=x2.device)
-            _lib.check(L_.sigma_layernorm_bwd_det(_ptr(x2), _ptr(dy2), _ptr(w), _ptr(dx), _ptr(dw), _ptr(db), x2.shape[0], x2.shape[1],
-                                                  ctx.eps, _ptr(ws), wsb, _stream()), "sigma_layernorm_bwd_det")
+            _lib.check(L_.sigma_layernorm_bwd_det(ptr(x2), ptr(dy2), ptr(w), ptr(dx), ptr(dw), ptr(db), x2.shape[0], x2.shape[1],
+                                                  ctx.eps, ptr(ws), wsb, stream()), "sigma_layernorm_bwd_det")
             return dx.view(dy.shape), dw, db, None
-        _lib.check(_lib.lib().sigma_layernorm_bwd(_ptr(x2), _ptr(dy2), _ptr(w), _ptr(dx), _ptr(dw), _ptr(db), x2.shape[0], x2.shape[1], ctx.eps,
-                                                 _stream()), "sigma_layernorm_bwd")
+        _lib.check(_lib.lib().sigma_layernorm_bwd(ptr(x2), ptr(dy2), ptr(w), ptr(dx), ptr(dw), ptr(db), x2.shape[0], x2.shape[1], ctx.eps,
+                                                 stream()), "sigma_layernorm_bwd")
         return dx.view(dy.shape), dw, db, None
 
 
@@ -408,15 +401,15 @@ def _call_ss2d_bwd(args, saved=False, det=False):
     L_ = _lib.lib()
     if det:
         fn = L_.sigma_ss2d_scan_bwd_saved_det if saved else L_.sigma_ss2d_scan_bwd_det
-        _lib.check(fn(*args, int(fused._FORCE_SPLIT or 0), _stream()), "sigma_ss2d_scan_bwd_det")
+        _lib.check(fn(*args, int(fused._FORCE_SPLIT or 0), stream()), "sigma_ss2d_scan_bwd_det")
         return
     if saved:
-        _lib.check(L_.sigma_ss2d_scan_bwd_saved(*args, int(fused._FORCE_SPLIT or 0), _stream()), "sigma_ss2d_scan_bwd_saved")
+        _lib.check(L_.sigma_ss2d_scan_bwd_saved(*args, int(fused._FORCE_SPLIT or 0), stream()), "sigma_ss2d_scan_bwd_saved")
         return
     if fused._FORCE_SPLIT:
-        rc = L_.sigma_ss2d_scan_bwd_split(*args, int(fused._FORCE_SPLIT), _stream())
+        rc = L_.sigma_ss2d_scan_bwd_split(*args, int(fused._FORCE_SPLIT), stream())
     else:
-        rc = L_.sigma_ss2d_scan_bwd(*args, _stream())
+        rc = L_.sigma_ss2d_scan_bwd(*args, stream())
     _lib.check(rc, "sigma_ss2d_scan_bwd")
 
 
@@ -476,9 +469,9 @@ class FusedSS2DCore(torch.autograd.Function):
         det = deterministic()
         wsb = (L_.sigma_ss2d_scan_bwd_det_workspace_bytes if det else L_.sigma_ss2d_scan_bwd_workspace_bytes)(kind, B, H, W, D, N)
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-        head = (kind, _ptr(xc), _ptr(xdbl), _ptr(dtw), _ptr(dtb), _ptr(A), _ptr(Ds), _ptr(dy), _ptr(delta))
-        tail = (_ptr(dxc), _ptr(ddelta), _ptr(dxdbl), _ptr(dA), _ptr(dDs), _ptr(ddtb), B, H, W, D, N, R, Cp, _ptr(ws), wsb)
-        _call_ss2d_bwd(head + ((_ptr(hs),) if saved else ()) + tail, saved, det)
+        head = (kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(dy), ptr(delta))
+        tail = (ptr(dxc), ptr(ddelta), ptr(dxdbl), ptr(dA), ptr(dDs), ptr(ddtb), B, H, W, D, N, R, Cp, ptr(ws), wsb)
+        _call_ss2d_bwd(head + ((ptr(hs),) if saved else ()) + tail, saved, det)
         # dt_proj: d dt_r = ddelta_k · W_dt[k]  (into the dt_r columns of dxdbl),  dW_dt[k] = ddelta_k^T · dt_r_k
         xd3 = xdbl.view(B * Lseq, K, Cp)
         dW = torch.empty_like(dtw)
@@ -528,7 +521,7 @@ class UpsampleBilinearFn(torch.autograd.Function):
         fmt = torch.channels_last if cl else torch.contiguous_format
         dy = dy.float().contiguous(memory_format=fmt)
         dx = torch.empty((B, C, Hin, Win), dtype=torch.float32, device=dy.device, memory_format=fmt)
-        _lib.check(_lib.lib().sigma_upsample_bilinear_bwd(_ptr(dy), _ptr(dx), B, C, Hin, Win, Hout, Wout, rh, rw, int(cl), _stream()),
+        _lib.check(_lib.lib().sigma_upsample_bilinear_bwd(ptr(dy), ptr(dx), B, C, Hin, Win, Hout, Wout, rh, rw, int(cl), stream()),
                    "sigma_upsample_bilinear_bwd")
         return dx.to(dtype), None, None
 

@@ -30,8 +30,7 @@ def test_library_exports_every_declared_symbol(lib_path):
     assert declared, "no declarations parsed"
     assert declared <= exported, f"declared but not exported: {sorted(declared - exported)}"
     extra = {s for s in exported - declared if s.startswith("sigma_")}
-    assert extra <= {"sigma_scan_bwd_split", "sigma_ss2d_scan_fwd_split", "sigma_ss2d_scan_bwd_split",
-                     "sigma_test_pick_segments", "sigma_test_pick_bn"}, f"undeclared exports: {sorted(extra)}"
+    assert not extra, f"undeclared exports: {sorted(extra)}"
 
 
 def test_library_has_no_runtime_dependency_on_cuda_libs(lib_path):
@@ -43,10 +42,27 @@ def test_ctypes_binding_matches_header(lib_path):
     from sigma_b200 import _lib
     L = _lib.lib()
     assert L.sigma_abi_version() == 1
-    assert set(_lib.SIGNATURES) >= _declared()
+    assert set(_lib.SIGNATURES) == _declared()
     assert L.sigma_ss2d_padded_cp(16, 6) == 40 and L.sigma_ss2d_padded_cp(4, 24) == 32 and L.sigma_ss2d_padded_cp(4, 65) == -1
     assert L.sigma_scan_fwd_workspace_bytes(2, 768, 1024, 16, 4, 0) > 0
     assert L.sigma_launch_count() == 0
+
+
+def test_ctypes_types_follow_header_conventions():
+    """SIGNATURES is parsed from the header: host int64 arrays, the strides struct and the error string keep their types,
+    every other pointer is a void pointer."""
+    from ctypes import POINTER, c_char_p, c_int, c_int64, c_void_p
+    from sigma_b200 import _lib
+    S = _lib.SIGNATURES
+    assert S["sigma_test_gemm_plan"] == (c_int, [c_int64] + [c_int] * 6 + [POINTER(c_int64)])
+    assert S["sigma_image_pre_fwd"][1][3] is c_void_p                      # int64_t *labels_out: a device pointer
+    assert POINTER(_lib.ScanStrides) in S["sigma_scan_fwd"][1]
+    assert S["sigma_last_error"] == (c_char_p, [])
+    src = open(os.path.join(ROOT, "include", "sigma_b200.h")).read()
+    body = re.search(r"typedef struct sigma_scan_strides \{(.*?)\}", src, flags=re.S).group(1)
+    decls = [d.split(None, 1) for d in body.split(";") if d.strip()]
+    assert decls and all(t == "int64_t" for t, _ in decls)
+    assert _lib.ScanStrides._fields_ == [(f.strip(), c_int64) for _, names in decls for f in names.split(",")]
 
 
 def test_sm90a_tma_in_sass(lib_path):
