@@ -144,14 +144,16 @@ int sigma_ss2d_scan_fwd_bf16(int kind, const void *xc, const float *xdbl, const 
 /* ------------------------------------------------------------------------------------------
  * f1. Backward of the fused scan (training): replaces the autograd of CrossScan (vmamba.py:80-98) + the dt_proj einsum (:199) +
  * SelectiveScan (selective_scan_bwd_kernel.cuh:68-274) + CrossMerge (:100-121) without materialising the (B,4,D,L) copies.
- * kind = SIGMA_DIRS_CROSS4 or SIGMA_DIRS_SEQ2; d_state in {4, 16}; D % 64 == 0.  Inputs as the forward plus
+ * kind = SIGMA_DIRS_CROSS4, SIGMA_DIRS_SEQ2 or SIGMA_DIRS_CROSS (batch = 2·images, as the forward; K = 1 walk per image, Kw = 2
+ * weight sets); d_state in {4, 16}; D % 64 == 0.  Inputs as the forward plus
  *   dy      (batch, Lseq, D)      gradient of the MERGED output y = sum_k y_k (CrossMerge is a sum, so every direction sees dy)
  * Outputs (fp32):
  *   dxc     (batch, Lseq, D)      sum over directions of du, accumulated by TMA reduce-add (zeroed inside)
  *   ddelta  (K, batch, Lseq, D)   gradient w.r.t. the PRE-softplus dt_proj output, per direction, at the position it belongs to; the
  *                                 caller finishes d dt_r = ddelta_k · W_dt[k] and dW_dt[k] = ddelta_k^T · dt_r_k with two GEMMs
- *   dxdbl   (batch, Lseq, K, Cp)  dB in columns [0, N), dC in [N, 2N) (zeroed inside; dt_r columns left 0 for the caller)
- *   dA (K·D, N), dDs (K·D), ddtb (K, D)   overwritten
+ *   dxdbl   (batch, Lseq, K, Cp)  dB in columns [0, N), dC in [N, 2N) (zeroed inside; dt_r columns left 0 for the caller); CROSS:
+ *                                 image b's dC goes to the C columns of image (b + batch/2) mod batch, whose row supplied C
+ *   dA (Kw·D, N), dDs (Kw·D), ddtb (Kw, D)   overwritten; CROSS: rows w·D + d summed over the images of modality w
  *   delta   (K, batch, Lseq, D)   scratch: the recomputed softplus(dt_proj) slabs
  * ------------------------------------------------------------------------------------------ */
 size_t sigma_ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
@@ -163,8 +165,8 @@ int sigma_ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const floa
  * otherwise recompute in a state sweep — delta (K, batch, Lseq, D) = softplus(dt_proj) at the position it belongs to, and
  * hs (sigma_ss2d_scan_hs_bytes) = the scan state at the start of every 16-position block of each direction's walk (the role of
  * the reference's chunk states `x`, selective_scan_fwd_kernel.cuh:176-190).  `sigma_ss2d_scan_bwd_saved` consumes them (delta
- * and hs are inputs) and runs only the reverse sweep.  nsplit = 0 lets the library choose the L-segments.  CROSS4 / SEQ2,
- * d_state 4 / 16. */
+ * and hs are inputs) and runs only the reverse sweep.  nsplit = 0 lets the library choose the L-segments.  CROSS4 / SEQ2 / CROSS
+ * (even batch; one walk of ceil(L/16) blocks per image), d_state 4 / 16. */
 size_t sigma_ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N);
 int sigma_ss2d_scan_fwd_save(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                              const float *Ds, float *y, float *delta, float *hs, int batch, int H, int W, int D, int N, int R, int Cp,
@@ -177,7 +179,9 @@ int sigma_ss2d_scan_bwd_saved(int kind, const float *xc, const float *xdbl, cons
 /* Deterministic builds of the fused backward (state sweep / after sigma_ss2d_scan_fwd_save): the same outputs, bitwise
  * reproducible for the same inputs, GPU model and L-segment plan.  Each direction's du goes to a slab summed over k into dxc,
  * dB / dC are kept per warp channel tile and dA / dDs / ddtb per (image, L-segment), all in the workspace, then summed in a
- * fixed order; no float atomics and no bulk reduce.  nsplit = 0 lets the library choose the L-segments. */
+ * fixed order; no float atomics and no bulk reduce.  nsplit = 0 lets the library choose the L-segments.  CROSS4 / SEQ2 only: kind
+ * CROSS has no deterministic build (SIGMA_EINVAL; the workspace query returns 0) — under the deterministic switch CroMB trains
+ * through the op-level _det kernels. */
 size_t sigma_ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
 int sigma_ss2d_scan_bwd_det(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                             const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb,
@@ -319,8 +323,8 @@ int sigma_conv3x3_tf32(const float *x, const float *w9, const float *w9_lo, cons
 int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, int64_t *out6_host);
 
 /* L-segment plan of the fused scan backward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_bwd (nsplit = 0)
- * or sigma_ss2d_scan_bwd_split / sigma_ss2d_scan_bwd_saved with that nsplit would launch for kind CROSS4 / SEQ2 at (batch, H, W, D,
- * N).  out4_host = {segments, 16-position tiles per segment, tiles of the longest direction's walk, tiles of the shortest}.  The
+ * or sigma_ss2d_scan_bwd_split / sigma_ss2d_scan_bwd_saved with that nsplit would launch for kind CROSS4 / SEQ2 / CROSS (even
+ * batch) at (batch, H, W, D, N).  out4_host = {segments, 16-position tiles per segment, tiles of the longest direction's walk, tiles of the shortest}.  The
  * directions share the tiles per segment, so a walk shorter than the longest can end in empty segments.  For tests and tuning. */
 int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, int nsplit, int64_t *out4_host);
 

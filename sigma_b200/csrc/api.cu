@@ -518,8 +518,8 @@ int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H
 // the L-segment plan of sigma_ss2d_scan_bwd{,_split,_saved} (nsplit = 0: the library's choice):
 // out4_host = {segments, tiles per segment, tiles of the longest walk, tiles of the shortest walk}
 int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, int nsplit, int64_t *out4_host) {
-  SIGMA_CHECK_ARG(out4_host && (kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2) && batch > 0 && H > 0 && W > 0 && D > 0 &&
-                      D % 64 == 0 && (N == 4 || N == 16) && nsplit >= 0,
+  SIGMA_CHECK_ARG(out4_host && (kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2 || kind == SIGMA_DIRS_CROSS) && batch > 0 && H > 0 &&
+                      W > 0 && D > 0 && D % 64 == 0 && (N == 4 || N == 16) && nsplit >= 0 && (kind != SIGMA_DIRS_CROSS || batch % 2 == 0),
                   "sigma_test_ss2d_bwd_plan: bad arguments");
   long long out[4];
   const int rc = ss2d_bwd_plan_hook(kind, batch, H, W, D, N, nsplit, out);
@@ -546,7 +546,7 @@ int sigma_test_ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, in
 
 // training forward: the forward plus what the fused backward needs (delta' slabs, block-start states)
 size_t sigma_ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N) {
-  if (kind != SIGMA_DIRS_CROSS4 && kind != SIGMA_DIRS_SEQ2) return 0;
+  if (kind != SIGMA_DIRS_CROSS4 && kind != SIGMA_DIRS_SEQ2 && (kind != SIGMA_DIRS_CROSS || batch % 2)) return 0;
   return ss2d_scan_hs_bytes(kind, batch, H, W, D, N);
 }
 
@@ -556,17 +556,19 @@ int sigma_ss2d_scan_fwd_save(int kind, const float *xc, const float *xdbl, const
   int rc = ss2d_check(kind, xc, xdbl, dtw, dtb, A, Ds, y, batch, H, W, D, N, R, Cp);
   if (rc) return rc;
   SIGMA_CHECK_ARG(delta && hs && al16(delta) && al16(hs), "sigma_ss2d_scan_fwd_save: delta / hs must be non-null and 16-byte aligned");
-  SIGMA_CHECK_ARG(kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2, "sigma_ss2d_scan_fwd_save: kind %d unsupported (CROSS4, SEQ2)", kind);
+  SIGMA_CHECK_ARG(kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2 || kind == SIGMA_DIRS_CROSS,
+                  "sigma_ss2d_scan_fwd_save: kind %d unsupported (CROSS4, SEQ2, CROSS)", kind);
   SIGMA_CHECK_ARG(N == 4 || N == 16, "sigma_ss2d_scan_fwd_save: d_state=%d unsupported (4, 16)", N);
   return ss2d_scan_fwd(kind, xc, xdbl, dtw, dtb, A, Ds, y, batch, H, W, D, N, R, Cp, workspace, workspace_bytes, nsplit,
                        (cudaStream_t)stream, delta, hs);
 }
 
 size_t sigma_ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
-  if (kind != SIGMA_DIRS_CROSS4 && kind != SIGMA_DIRS_SEQ2) return 0;
+  if (kind != SIGMA_DIRS_CROSS4 && kind != SIGMA_DIRS_SEQ2 && (kind != SIGMA_DIRS_CROSS || batch % 2)) return 0;
   return ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N);
 }
 
+// no deterministic build of kind CROSS: under torch.use_deterministic_algorithms(True) CroMB trains through the op-level _det kernels
 size_t sigma_ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
   if ((kind != SIGMA_DIRS_CROSS4 && kind != SIGMA_DIRS_SEQ2) || (N != 4 && N != 16) || D % 64) return 0;
   return ss2d_scan_bwd_det_workspace_bytes(kind, batch, H, W, D, N);
@@ -577,7 +579,12 @@ static int ss2d_bwd_entry(int kind, const float *xc, const float *xdbl, const fl
                           int batch, int H, int W, int D, int N, int R, int Cp, void *ws, size_t wsb, int nsplit, void *stream,
                           const float *hs_saved = nullptr, int det = 0) {
   SIGMA_CHECK_ARG(xc && xdbl && dtw && dtb && A && Ds && dy && delta && dxc && ddelta && dxdbl && dA && dDs && ddtb, "sigma_ss2d_scan_bwd: null pointer");
-  SIGMA_CHECK_ARG(kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2, "sigma_ss2d_scan_bwd: kind %d unsupported (CROSS4, SEQ2)", kind);
+  SIGMA_CHECK_ARG(kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2 || kind == SIGMA_DIRS_CROSS,
+                  "sigma_ss2d_scan_bwd: kind %d unsupported (CROSS4, SEQ2, CROSS)", kind);
+  SIGMA_CHECK_ARG(kind != SIGMA_DIRS_CROSS || !det,
+                  "sigma_ss2d_scan_bwd_det: kind CROSS has no deterministic build (under the deterministic switch CroMB trains through "
+                  "the op-level _det kernels)");
+  SIGMA_CHECK_ARG(kind != SIGMA_DIRS_CROSS || batch % 2 == 0, "sigma_ss2d_scan_bwd: CROSS needs batch = 2·images (batch=%d)", batch);
   SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % 64 == 0 && R > 0, "sigma_ss2d_scan_bwd: bad sizes (D=%d must be a multiple of 64)", D);
   SIGMA_CHECK_ARG(N == 4 || N == 16, "sigma_ss2d_scan_bwd: d_state=%d unsupported (4, 16)", N);
   SIGMA_CHECK_ARG(Cp == sigma_ss2d_padded_cp(N, R), "sigma_ss2d_scan_bwd: Cp=%d must equal sigma_ss2d_padded_cp(N=%d, R=%d)", Cp, N, R);

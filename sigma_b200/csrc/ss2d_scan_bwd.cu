@@ -17,7 +17,9 @@
 //        dA, dDs, d dt_bias -> per-thread accumulators, one atomic per channel at the end.
 // Thread mapping as scan_op_bwd_tma.cu: d_state 16 -> 2 lanes per channel (8 states each), d_state 4 -> 1; a CTA = 64
 // channels of one (direction, image [, L-segment]); tiles of 16 positions through a TMA ring (full mbarrier + last-arriver
-// refill).  Kinds SIGMA_DIRS_CROSS4 and SIGMA_DIRS_SEQ2 (SS2D and ConMB); d_state in {4, 16}; D % 64 == 0.
+// refill).  Kinds SIGMA_DIRS_CROSS4 and SIGMA_DIRS_SEQ2 (SS2D and ConMB) and SIGMA_DIRS_CROSS (CroMB: one row-major walk per
+// image of a 2·images batch, per-modality weights, C from the other modality; separate *_cross_kernel instances, no
+// deterministic build); d_state in {4, 16}; D % 64 == 0.
 #include <stdlib.h>
 #include <string.h>
 
@@ -84,8 +86,10 @@ __device__ __forceinline__ FbWalk fb_walk(const Ss2dBwdParams &p) {
 // ---------------------------------------------------------------------------------------------------------------------
 // 1. state sweep: delta' slabs + tile-start states (walk order)
 // ---------------------------------------------------------------------------------------------------------------------
-template <int N, int MODE>
-__global__ void __launch_bounds__(128, 3) ss2d_state_kernel(const __grid_constant__ Ss2dBwdParams p) {
+// CROSS: image b runs with weight set kw = [b >= batch/2] (its rows of W_dt, bias and A); the state sweep needs only its own
+// x_dbl row (B, dt_r), so the walk itself is kind SEQ2's first direction
+template <int N, int MODE, bool CROSS>
+__device__ __forceinline__ void ss2d_state_body(const Ss2dBwdParams &p) {
   constexpr int LPC = FbCfg<N>::LPC, NS = FbCfg<N>::NS, CPW = FbCfg<N>::CPW, NT = FB_DT * LPC;
   // delta' does not depend on the state: the pass that sees a position FIRST (MODE_SERIAL, or MODE_SUMMARY when the walk is
   // cut into L-segments) computes it and stores the slab tile; MODE_APPLY reads it back instead of repeating the dot product
@@ -103,6 +107,7 @@ __global__ void __launch_bounds__(128, 3) ss2d_state_kernel(const __grid_constan
   const int half = lane / CPW, cl = lane - half * CPW, c = warp * CPW + cl, n0 = half * NS;
   const FbWalk w = fb_walk(p);
   const int d = w.d0 + c;
+  const int kw = CROSS ? (w.b >= (p.batch >> 1) ? 1 : 0) : w.k;   // weight set
   if (tid == 0) {
     for (int s = 0; s < NST; ++s) { mbar_init(&full[s], 1); done[s] = 0; }
     fence_mbar_init();
@@ -110,7 +115,7 @@ __global__ void __launch_bounds__(128, 3) ss2d_state_kernel(const __grid_constan
   if (COMPUTE) {
     for (int i = tid; i < FB_DT * R; i += NT) {
       const int cc = i / R, r = i - cc * R;
-      sW[cc * (R + 1) + r] = p.dtw[((long long)w.k * p.D + w.d0 + cc) * R + r];
+      sW[cc * (R + 1) + r] = p.dtw[((long long)kw * p.D + w.d0 + cc) * R + r];
     }
   }
   __syncthreads();
@@ -128,7 +133,7 @@ __global__ void __launch_bounds__(128, 3) ss2d_state_kernel(const __grid_constan
   if (tid == 0) for (int tau = w.t0; tau < min(w.t1, w.t0 + NST); ++tau) request_tile(tau, tau - w.t0);
 
   float h[NS], a2[NS];
-  const long long wd = (long long)w.k * p.D + d;
+  const long long wd = (long long)kw * p.D + d;
 #pragma unroll
   for (int s = 0; s < NS; ++s) { a2[s] = p.A[wd * N + n0 + s] * kLog2e; h[s] = 0.f; }
   const float bias = p.dtb[wd];
@@ -206,12 +211,21 @@ __global__ void __launch_bounds__(128, 3) ss2d_state_kernel(const __grid_constan
   }
 }
 
+template <int N, int MODE>
+__global__ void __launch_bounds__(128, 3) ss2d_state_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_state_body<N, MODE, false>(p); }
+
+template <int N, int MODE>
+__global__ void __launch_bounds__(128, 3) ss2d_state_cross_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_state_body<N, MODE, true>(p); }
+
 // ---------------------------------------------------------------------------------------------------------------------
 // 2 + 3. reverse summaries (MODE_SUMMARY) and the main backward sweep (MODE_SERIAL / MODE_APPLY)
 // ---------------------------------------------------------------------------------------------------------------------
-// DET: every sum across CTAs goes to the partials of the deterministic build (see Ss2dBwdParams) instead of an atomic
-template <int N, int MODE, bool DET>
+// DET: every sum across CTAs goes to the partials of the deterministic build (see Ss2dBwdParams) instead of an atomic.
+// CROSS: image b runs with weight set kw = [b >= batch/2] and reads C from image bC = the other modality's (as the forward):
+// the stage holds bC's x_dbl tile too, dC goes to the C columns of bC's dxdbl rows, dA / dDs / d dt_bias to rows kw·D + d.
+template <int N, int MODE, bool DET, bool CROSS>
 __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
+  static_assert(!(DET && CROSS), "no deterministic build of the CROSS backward");
   constexpr int LPC = FbCfg<N>::LPC, NS = FbCfg<N>::NS, CPW = FbCfg<N>::CPW, NT = FB_DT * LPC;
   constexpr bool MAIN = MODE != MODE_SUMMARY;
   constexpr float kLn2 = 0.6931471805599453f;
@@ -219,7 +233,7 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
   float *smem = reinterpret_cast<float *>(smem_raw);
   const int NST = p.nst, Cp = p.Cp;
   const int xc_fl = FB_LT * FB_DT, dbl_fl = FB_LT * Cp;
-  const int stage_fl = (MAIN ? 3 : 2) * xc_fl + dbl_fl;            // [xc] dy dl dbl
+  const int stage_fl = (MAIN ? 3 : 2) * xc_fl + (CROSS ? 2 : 1) * dbl_fl;   // [xc] dy dl dbl [dbl of image bC]
   float *stage_all = smem + NST * stage_fl;                        // per-warp staging: du [16][CPW], ddelta [16][CPW]
   float4 *sH = reinterpret_cast<float4 *>(stage_all + (MAIN ? (NT / 32) * 2 * FB_LT * CPW : 0));   // [16][NS/4][NT]
   uint64_t *full = reinterpret_cast<uint64_t *>(sH + (MAIN ? FB_LT * (NS / 4) * NT : 0));
@@ -229,6 +243,9 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
   const int half = lane / CPW, cl = lane - half * CPW, c = warp * CPW + cl, n0 = half * NS;
   const FbWalk w = fb_walk(p);
   const int d = w.d0 + c;
+  const int half_b = p.batch >> 1;
+  const int kw = CROSS ? (w.b >= half_b ? 1 : 0) : w.k;
+  const int bC = CROSS ? (w.b >= half_b ? w.b - half_b : w.b + half_b) : w.b;
   if (tid == 0) {
     for (int s = 0; s < NST; ++s) { mbar_init(&full[s], 1); done[s] = 0; }
     fence_mbar_init();
@@ -262,11 +279,12 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
     tma_load_4d(dst, &p.m_dy[w.k], &full[st], w.d0, i0, o, w.b);
     tma_load_4d(dst + xc_fl, &p.m_dl[w.k], &full[st], w.d0, i0, o, w.k * p.batch + w.b);
     tma_load_4d(dst + 2 * xc_fl, &p.m_dbl[w.k], &full[st], 0, i0, o, w.b);
+    if (CROSS) tma_load_4d(dst + 2 * xc_fl + dbl_fl, &p.m_dbl[w.k], &full[st], 0, i0, o, bC);
   };
   if (tid == 0) for (int kk = 0; kk < min(ntl, NST); ++kk) request_tile(kk, kk);
 
   float a2[NS], dh[NS], dAacc[NS];
-  const long long wd = (long long)w.k * p.D + d;
+  const long long wd = (long long)kw * p.D + d;
 #pragma unroll
   for (int s = 0; s < NS; ++s) { a2[s] = p.A[wd * N + n0 + s] * kLog2e; dh[s] = 0.f; dAacc[s] = 0.f; }
   float *carry_row = p.carry + ((((long long)w.b * p.K + w.k) * p.D + d) * p.nsplit + w.split) * 2 * N;
@@ -279,6 +297,7 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
   float *sdu = stage_all + warp * 2 * FB_LT * CPW, *sdd = sdu + FB_LT * CPW;
   float4 *sHt = sH + tid;
   float *dxrow0 = p.dxdbl + (long long)w.b * p.Lseq * p.K * Cp + (long long)w.k * Cp;   // + pos·K·Cp
+  float *dxrowC = CROSS ? p.dxdbl + (long long)bC * p.Lseq * p.K * Cp + (long long)w.k * Cp : dxrow0;
 
   int st = 0, ph = 0;
   for (int kk = 0; kk < ntl; ++kk) {
@@ -288,6 +307,7 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
     mbar_spin(&full[st], (uint32_t)ph);
     const float *base = smem + st * stage_fl;
     const float *sXC = base, *sDY = base + (MAIN ? xc_fl : 0), *sDL = sDY + xc_fl, *sDB = sDL + xc_fl;
+    const float *sDC = CROSS ? sDB + dbl_fl : sDB;   // the x_dbl tile C is read from
 
     if (MAIN) {
       // ---- forward inside the tile from its start state (walk order), h after every step -> shared memory ----
@@ -321,11 +341,11 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
     for (int s = npos - 1; s >= 0; --s) {
       const int r = w.rev ? npos - 1 - s : s;
       const float dl = sDL[r * FB_DT + c], dy = sDY[r * FB_DT + c];
-      const float *row = sDB + r * Cp + n0;
+      const float *row = sDB + r * Cp + n0, *rowC = sDC + r * Cp + n0;
       if (!MAIN) {
 #pragma unroll
         for (int q = 0; q < NS / 4; ++q) {
-          const float4 cv = *reinterpret_cast<const float4 *>(row + N + 4 * q);
+          const float4 cv = *reinterpret_cast<const float4 *>(rowC + N + 4 * q);
           dh[4 * q] = fmaf(dy, cv.x, dh[4 * q]) * ex2(dl * a2[4 * q]);
           dh[4 * q + 1] = fmaf(dy, cv.y, dh[4 * q + 1]) * ex2(dl * a2[4 * q + 1]);
           dh[4 * q + 2] = fmaf(dy, cv.z, dh[4 * q + 2]) * ex2(dl * a2[4 * q + 2]);
@@ -341,7 +361,7 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
 #pragma unroll
       for (int q = 0; q < NS / 4; ++q) {
         const float4 bv = *reinterpret_cast<const float4 *>(row + 4 * q);
-        const float4 cv = *reinterpret_cast<const float4 *>(row + N + 4 * q);
+        const float4 cv = *reinterpret_cast<const float4 *>(rowC + N + 4 * q);
         const float4 hv = sHt[(s * (NS / 4) + q) * NT];
         const float Bq[4] = {bv.x, bv.y, bv.z, bv.w}, Cq[4] = {cv.x, cv.y, cv.z, cv.w}, Hq[4] = {hv.x, hv.y, hv.z, hv.w};
 #pragma unroll
@@ -372,8 +392,9 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
           dst[N + n0 + wb] = rC;
         } else {
           float *dst = dxrow0 + pos * p.K * Cp;
+          float *dstC = CROSS ? dxrowC + pos * p.K * Cp : dst;
           atomicAdd(dst + n0 + wb, rB);
-          atomicAdd(dst + N + n0 + wb, rC);
+          atomicAdd(dstC + N + n0 + wb, rC);
         }
       }
       if (LPC == 2) {
@@ -429,29 +450,37 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
 }
 
 template <int N, int MODE>
-__global__ void __launch_bounds__(128, 2) ss2d_bwd_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, false>(p); }
+__global__ void __launch_bounds__(128, 2) ss2d_bwd_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, false, false>(p); }
 
 template <int N, int MODE>
-__global__ void __launch_bounds__(128, 2) ss2d_bwd_det_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, true>(p); }
+__global__ void __launch_bounds__(128, 2) ss2d_bwd_det_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, true, false>(p); }
+
+template <int N, int MODE>
+__global__ void __launch_bounds__(128, 2) ss2d_bwd_cross_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, false, true>(p); }
 
 // ---- host ----
 constexpr int kFbMaxSplit = 64;
+
+// walks per image K (x_dbl rows per position) and parameter sets (K, or the 2 modalities of CROSS)
+static int fb_dirs(int kind) { return kind == SIGMA_DIRS_CROSS4 ? 4 : (kind == SIGMA_DIRS_SEQ2 ? 2 : 1); }
+static int fb_wsets(int kind) { return kind == SIGMA_DIRS_CROSS ? 2 : fb_dirs(kind); }
 
 static int fb_max_tiles(int kind, int H, int W) { return ss2d_save_tiles(kind, H, W); }
 int ss2d_save_tiles(int kind, int H, int W) {
   const long long L = (long long)H * W;
   if (kind == SIGMA_DIRS_SEQ2) return (int)((2 * L + FB_LT - 1) / FB_LT);
+  if (kind == SIGMA_DIRS_CROSS) return (int)((L + FB_LT - 1) / FB_LT);   // one row-major walk
   return (int)std::max<long long>((L + FB_LT - 1) / FB_LT, (long long)W * ((H + FB_LT - 1) / FB_LT));
 }
 
 size_t ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N) {
-  const int K = kind == SIGMA_DIRS_CROSS4 ? 4 : 2;
+  const int K = fb_dirs(kind);
   return (size_t)K * batch * fb_max_tiles(kind, H, W) * D * N * sizeof(float);
 }
 
 // workspace = [hs (K, batch, max_tiles, D, N)] [forward carries] [reverse carries]
 size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
-  const int K = kind == SIGMA_DIRS_CROSS4 ? 4 : 2;
+  const int K = fb_dirs(kind);
   const size_t carry = (size_t)batch * K * D * kFbMaxSplit * 2 * N * sizeof(float);
   return align256((size_t)K * batch * fb_max_tiles(kind, H, W) * D * N * sizeof(float)) + 2 * align256(carry);
 }
@@ -482,7 +511,7 @@ size_t ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int 
 struct FbPlan { int nsplit, tiles_per_split, max_tiles, min_tiles; };
 
 static FbPlan fb_plan(int kind, int batch, int H, int W, int D, int N, int force_split) {
-  const int K = kind == SIGMA_DIRS_CROSS4 ? 4 : 2;
+  const int K = fb_dirs(kind);
   const long long Lseq = kind == SIGMA_DIRS_SEQ2 ? 2LL * H * W : (long long)H * W;
   const int row_tiles = (int)((Lseq + FB_LT - 1) / FB_LT), col_tiles = W * ((H + FB_LT - 1) / FB_LT);
   FbPlan pl;
@@ -515,9 +544,10 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
     set_error("sigma_ss2d_scan_bwd: workspace too small (%zu < %zu)", ws_bytes, need);
     return SIGMA_EWORKSPACE;
   }
+  const bool cross = kind == SIGMA_DIRS_CROSS;   // never with det (the entry points reject it)
   Ss2dBwdParams p;
   memset(&p, 0, sizeof(p));
-  const int K = kind == SIGMA_DIRS_CROSS4 ? 4 : 2;
+  const int K = fb_dirs(kind), Kw = fb_wsets(kind);
   const long long Lseq = kind == SIGMA_DIRS_SEQ2 ? 2LL * H * W : (long long)H * W;
   p.dtw = dtw; p.dtb = dtb; p.A = A; p.Ds = Ds;
   p.dxdbl = dxdbl; p.dA = dA; p.dDs = dDs; p.ddtb = ddtb;
@@ -568,9 +598,9 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
 
   SIGMA_CHECK_CUDA(cudaMemsetAsync(dxc, 0, (size_t)batch * Lseq * D * sizeof(float), stream));
   SIGMA_CHECK_CUDA(cudaMemsetAsync(dxdbl, 0, (size_t)batch * Lseq * K * Cp * sizeof(float), stream));
-  SIGMA_CHECK_CUDA(cudaMemsetAsync(dA, 0, (size_t)K * D * N * sizeof(float), stream));
-  SIGMA_CHECK_CUDA(cudaMemsetAsync(dDs, 0, (size_t)K * D * sizeof(float), stream));
-  SIGMA_CHECK_CUDA(cudaMemsetAsync(ddtb, 0, (size_t)K * D * sizeof(float), stream));
+  SIGMA_CHECK_CUDA(cudaMemsetAsync(dA, 0, (size_t)Kw * D * N * sizeof(float), stream));
+  SIGMA_CHECK_CUDA(cudaMemsetAsync(dDs, 0, (size_t)Kw * D * sizeof(float), stream));
+  SIGMA_CHECK_CUDA(cudaMemsetAsync(ddtb, 0, (size_t)Kw * D * sizeof(float), stream));
 
   // the state sweep stores delta' through m_dd (per-warp boxes over the delta slabs); the main sweep re-points it at ddelta
   auto make_dd = [&](float *slab, CUtensorMap *maps = nullptr) -> int {
@@ -610,33 +640,41 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
     dim3 grid(D / FB_DT, K * pm.nsplit, batch), block(NT);
     const long long nrows = (long long)batch * K * D, tot = nrows * NN;
     const size_t st_smem = ((size_t)pm.nst * (2 * FB_LT * FB_DT + FB_LT * Cp) + FB_DT * (R + 1) + 2 + (NT / 32) * FB_LT * CPWc) * sizeof(float) + 256;
-    const size_t sm_smem = ((size_t)pm.nst * (2 * FB_LT * FB_DT + FB_LT * Cp)) * sizeof(float) + 256;
-    const size_t mn_smem = ((size_t)pm.nst * (3 * FB_LT * FB_DT + FB_LT * Cp) + (NT / 32) * 2 * FB_LT * CPWc + (size_t)FB_LT * NS * NT) * sizeof(float) + 256;
+    const size_t dbl_tiles = cross ? 2 : 1;   // the reverse sweeps of CROSS also stage the C image's x_dbl tile
+    const size_t sm_smem = ((size_t)pm.nst * (2 * FB_LT * FB_DT + dbl_tiles * FB_LT * Cp)) * sizeof(float) + 256;
+    const size_t mn_smem = ((size_t)pm.nst * (3 * FB_LT * FB_DT + dbl_tiles * FB_LT * Cp) + (NT / 32) * 2 * FB_LT * CPWc + (size_t)FB_LT * NS * NT) * sizeof(float) + 256;
     auto run = [&](auto kern, const Ss2dBwdParams &pp, size_t smem) -> int {
       SIGMA_CHECK_CUDA(prep_kernel_once((const void *)kern));
       kern<<<grid, block, smem, stream>>>(pp);
       SIGMA_CHECK_LAUNCH();
       return SIGMA_OK;
     };
+    using Kern = void (*)(Ss2dBwdParams);
+    const Kern st_serial = cross ? ss2d_state_cross_kernel<NN, MODE_SERIAL> : ss2d_state_kernel<NN, MODE_SERIAL>;
+    const Kern st_summary = cross ? ss2d_state_cross_kernel<NN, MODE_SUMMARY> : ss2d_state_kernel<NN, MODE_SUMMARY>;
+    const Kern st_apply = cross ? ss2d_state_cross_kernel<NN, MODE_APPLY> : ss2d_state_kernel<NN, MODE_APPLY>;
+    const Kern bw_serial = cross ? ss2d_bwd_cross_kernel<NN, MODE_SERIAL> : ss2d_bwd_kernel<NN, MODE_SERIAL>;
+    const Kern bw_summary = cross ? ss2d_bwd_cross_kernel<NN, MODE_SUMMARY> : ss2d_bwd_kernel<NN, MODE_SUMMARY>;
+    const Kern bw_apply = cross ? ss2d_bwd_cross_kernel<NN, MODE_APPLY> : ss2d_bwd_kernel<NN, MODE_APPLY>;
     int r;
     ps.carry = fcarry;
     if (hs_saved != nullptr) {
       // nothing to recompute
     } else if (pm.nsplit == 1) {
-      if ((r = run(ss2d_state_kernel<NN, MODE_SERIAL>, ps, st_smem))) return r;
+      if ((r = run(st_serial, ps, st_smem))) return r;
     } else {
-      if ((r = run(ss2d_state_kernel<NN, MODE_SUMMARY>, ps, st_smem))) return r;
+      if ((r = run(st_summary, ps, st_smem))) return r;
       scan_combine_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(fcarry, nrows, pm.nsplit, NN);
       SIGMA_CHECK_LAUNCH();
-      if ((r = run(ss2d_state_kernel<NN, MODE_APPLY>, ps, st_smem))) return r;
+      if ((r = run(st_apply, ps, st_smem))) return r;
     }
     pm.carry = rcarry;
     if (!det) {
-      if (pm.nsplit == 1) return run(ss2d_bwd_kernel<NN, MODE_SERIAL>, pm, mn_smem);
-      if ((r = run(ss2d_bwd_kernel<NN, MODE_SUMMARY>, pm, sm_smem))) return r;
+      if (pm.nsplit == 1) return run(bw_serial, pm, mn_smem);
+      if ((r = run(bw_summary, pm, sm_smem))) return r;
       scan_combine_rev_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(rcarry, nrows, pm.nsplit, NN);
       SIGMA_CHECK_LAUNCH();
-      return run(ss2d_bwd_kernel<NN, MODE_APPLY>, pm, mn_smem);
+      return run(bw_apply, pm, mn_smem);
     }
     if (pm.nsplit == 1) {
       if ((r = run(ss2d_bwd_det_kernel<NN, MODE_SERIAL>, pm, mn_smem))) return r;

@@ -257,7 +257,7 @@ def ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
     """Training forward: ss2d_scan that also returns delta' (K, batch, Lseq, D) and the block-start states `hs` for
     sigma_ss2d_scan_bwd_saved (no state sweep in the backward)."""
     L_ = _lib.lib()
-    ndir = {_lib.DIRS_CROSS4: 4, _lib.DIRS_SEQ2: 2}[kind]
+    ndir = {_lib.DIRS_CROSS4: 4, _lib.DIRS_SEQ2: 2, _lib.DIRS_CROSS: 1}[kind]
     Lseq = 2 * H * W if kind == _lib.DIRS_SEQ2 else H * W
     y = torch.empty((ndir, batch, Lseq, D), dtype=torch.float32, device=xc.device)
     delta = torch.empty_like(y)

@@ -358,9 +358,23 @@ class CrossMambaFusion_SS2D_SSM(nn.Module):
             from . import fused
             return fused.cromb_ss2d(self, x_rgb, x_e, residual=residual)
         B, H, W, _ = x_rgb.shape
-        c_r = self.act(self.conv2d(self.in_proj(x_rgb).permute(0, 3, 1, 2).contiguous()))
-        c_e = self.act(self.conv2d(self.in_proj_modalx(x_e).permute(0, 3, 1, 2).contiguous()))
-        y_r, y_e = self.CMA_ssm(c_r.flatten(2).transpose(1, 2), c_e.flatten(2).transpose(1, 2))
+        if ops.fused_core_ok(x_rgb, self.d_inner, self.d_state) and not ops.deterministic():
+            # training through the fused core (f1), kind CROSS: both modalities as one 2·B batch, channels-last throughout.  Under
+            # the deterministic switch the composed path below runs (the op-level _det kernels; CROSS has no _det build)
+            from . import _lib
+            D, cm = self.d_inner, self.CMA_ssm
+            t = torch.cat([self.in_proj(x_rgb), self.in_proj_modalx(x_e)], dim=0)             # (2B, H, W, D)
+            xc = self.act(self.conv2d(t.permute(0, 3, 1, 2))).permute(0, 2, 3, 1).reshape(2 * B, H * W, D)   # one shared conv
+            y = ops.FusedSS2DCore.apply(xc, torch.stack([cm.x_proj_1.weight, cm.x_proj_2.weight]),
+                                        torch.stack([cm.dt_proj_1.weight, cm.dt_proj_2.weight]),
+                                        torch.stack([cm.dt_proj_1.bias, cm.dt_proj_2.bias]), torch.cat([cm.A_log_1, cm.A_log_2]),
+                                        torch.cat([cm.D_1, cm.D_2]), _lib.DIRS_CROSS, H, W)                # (2B, L, D)
+            y_r = ops.layer_norm(cm.out_norm_1, y[:B])
+            y_e = ops.layer_norm(cm.out_norm_2, y[B:])
+        else:
+            c_r = self.act(self.conv2d(self.in_proj(x_rgb).permute(0, 3, 1, 2).contiguous()))
+            c_e = self.act(self.conv2d(self.in_proj_modalx(x_e).permute(0, 3, 1, 2).contiguous()))
+            y_r, y_e = self.CMA_ssm(c_r.flatten(2).transpose(1, 2), c_e.flatten(2).transpose(1, 2))
         o_r = self.dropout_rgb(self.out_proj_rgb(y_r.view(B, H, W, -1)))
         o_e = self.dropout_e(self.out_proj_e(y_e.view(B, H, W, -1)))
         return (x_rgb + o_r, x_e + o_e) if residual else (o_r, o_e)

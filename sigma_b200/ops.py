@@ -419,19 +419,32 @@ class FusedSS2DCore(torch.autograd.Function):
     the position it belongs to (CrossMerge).  Forward = the inference kernels (x_proj GEMM + the fused scan) in their state-saving
     build (sigma_ss2d_scan_fwd_save: also keeps delta' and the scan state entering every 16-position block); backward =
     sigma_ss2d_scan_bwd_saved (one reverse sweep; no CrossScan / CrossMerge tensors) + the x_proj / dt_proj weight-gradient GEMMs.
-    With FUSED_SAVE_STATES = False the plain forward runs and sigma_ss2d_scan_bwd recomputes both in a state sweep."""
+    With FUSED_SAVE_STATES = False the plain forward runs and sigma_ss2d_scan_bwd recomputes both in a state sweep.
+    Kind CROSS is Cross_Mamba_Attention_SSM.forward (vmamba.py:1508-1545): xc (2·images, L, D) modality-major, the parameters of
+    the two modalities stacked (x_proj_weight (2, R+2N, D), dt_projs_weight (2, D, R), dt_projs_bias (2, D), A_logs (2D, N), Ds
+    (2D)); each half runs its own x_proj and weights and reads C from the other half.  It has no deterministic backward."""
 
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
     def forward(ctx, xc, x_proj_weight, dt_projs_weight, dt_projs_bias, A_logs, Ds, kind, H, W):
         from . import fused
-        K, _, D = x_proj_weight.shape
+        Kw, _, D = x_proj_weight.shape
+        cross = kind == _lib.DIRS_CROSS
+        K = 1 if cross else Kw                   # x_dbl rows per position
         N, R = A_logs.shape[1], dt_projs_weight.shape[2]
         Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
         xc = xc.contiguous()
         B, Lseq, _ = xc.shape
-        xw = torch.cat([fused._pack_xproj(x_proj_weight[k], N, R, Cp) for k in range(K)], dim=0).contiguous()      # (K·Cp, D)
-        xdbl = fused.linear(xc.view(B * Lseq, D), xw, kind="x_proj")                                                # (B·Lseq, K·Cp)
+        xw = torch.cat([fused._pack_xproj(x_proj_weight[k], N, R, Cp) for k in range(Kw)], dim=0).contiguous()     # (Kw·Cp, D)
+        if cross:   # each modality's half of the batch through its own x_proj
+            if B % 2:
+                raise RuntimeError(f"FusedSS2DCore: kind CROSS needs a batch of 2·images, got {B}")
+            n = B // 2 * Lseq
+            xdbl = torch.empty((B * Lseq, Cp), dtype=torch.float32, device=xc.device)
+            for m in range(2):
+                fused.linear(xc.view(B * Lseq, D)[m * n:(m + 1) * n], xw[m * Cp:(m + 1) * Cp], out=xdbl[m * n:(m + 1) * n], kind="x_proj")
+        else:
+            xdbl = fused.linear(xc.view(B * Lseq, D), xw, kind="x_proj")                                            # (B·Lseq, K·Cp)
         dtw, dtb = dt_projs_weight.contiguous(), dt_projs_bias.contiguous()
         A = (-torch.exp(A_logs)).contiguous()
         Dsc = Ds.contiguous()
@@ -442,7 +455,7 @@ class FusedSS2DCore(torch.autograd.Function):
             y = fused.ss2d_scan(kind, xc, xdbl, dtw, dtb, A, Dsc, B, H, W, D, N, R, Cp)                              # (K, B, Lseq, D)
             ctx.save_for_backward(xc, xdbl, xw, dtw, dtb, A, Dsc)
         ctx.meta = (kind, H, W, K, D, N, R, Cp)
-        return y.sum(0)
+        return y[0] if cross else y.sum(0)
 
     @staticmethod
     @torch.amp.custom_bwd(device_type="cuda")
@@ -454,6 +467,12 @@ class FusedSS2DCore(torch.autograd.Function):
         else:
             xc, xdbl, xw, dtw, dtb, A, Ds = ctx.saved_tensors
         kind, H, W, K, D, N, R, Cp = ctx.meta
+        cross = kind == _lib.DIRS_CROSS
+        Kw = 2 if cross else K                   # parameter sets
+        det = deterministic()
+        if cross and det:
+            raise RuntimeError("FusedSS2DCore: kind CROSS has no deterministic backward; under torch.use_deterministic_algorithms(True) "
+                               "CroMB trains through the op-level _det kernels (CrossMambaFusion_SS2D_SSM routes there itself)")
         B, Lseq, _ = xc.shape
         dy = dy.contiguous().float()
         dev = xc.device
@@ -462,16 +481,29 @@ class FusedSS2DCore(torch.autograd.Function):
         ddelta = torch.empty_like(delta)
         dxc = torch.empty((B, Lseq, D), dtype=torch.float32, device=dev)
         dxdbl = torch.empty((B * Lseq, K, Cp), dtype=torch.float32, device=dev)
-        dA = torch.empty((K * D, N), dtype=torch.float32, device=dev)
-        dDs = torch.empty(K * D, dtype=torch.float32, device=dev)
-        ddtb = torch.empty((K, D), dtype=torch.float32, device=dev)
+        dA = torch.empty((Kw * D, N), dtype=torch.float32, device=dev)
+        dDs = torch.empty(Kw * D, dtype=torch.float32, device=dev)
+        ddtb = torch.empty((Kw, D), dtype=torch.float32, device=dev)
         L_ = _lib.lib()
-        det = deterministic()
         wsb = (L_.sigma_ss2d_scan_bwd_det_workspace_bytes if det else L_.sigma_ss2d_scan_bwd_workspace_bytes)(kind, B, H, W, D, N)
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
         head = (kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(dy), ptr(delta))
         tail = (ptr(dxc), ptr(ddelta), ptr(dxdbl), ptr(dA), ptr(dDs), ptr(ddtb), B, H, W, D, N, R, Cp, ptr(ws), wsb)
-        _call_ss2d_bwd(head + ((ptr(hs),) if saved else ()) + tail, saved, det)
+        args = head + ((ptr(hs),) if saved else ()) + tail
+        # det only when set: bench.py --mode train brackets this call with a wrapper that takes (args, saved)
+        _call_ss2d_bwd(args, saved, True) if det else _call_ss2d_bwd(args, saved)
+        if cross:   # the same two steps per modality half m (its rows of dxdbl / ddelta / xc, its weight set)
+            n = B // 2 * Lseq
+            xd, dxd, dd = xdbl.view(2, n, Cp), dxdbl.view(2, n, Cp), ddelta.view(2, n, D)
+            xcm, dxcm, xw3 = xc.view(2, n, D), dxc.view(2, n, D), xw.view(2, Cp, D)
+            dW, dxw = torch.empty_like(dtw), torch.empty_like(xw3)
+            for m in range(2):
+                dxd[m, :, 2 * N:2 * N + R].copy_(dd[m] @ dtw[m])
+                dW[m] = dd[m].t() @ xd[m, :, 2 * N:2 * N + R]
+                dxcm[m].addmm_(dxd[m], xw3[m])
+                dxw[m] = dxd[m].t() @ xcm[m]
+            dxpw = torch.cat([dxw[:, 2 * N:2 * N + R], dxw[:, 0:N], dxw[:, N:2 * N]], dim=1)
+            return dxc, dxpw, dW, ddtb, dA * A, dDs, None, None, None
         # dt_proj: d dt_r = ddelta_k · W_dt[k]  (into the dt_r columns of dxdbl),  dW_dt[k] = ddelta_k^T · dt_r_k
         xd3 = xdbl.view(B * Lseq, K, Cp)
         dW = torch.empty_like(dtw)
