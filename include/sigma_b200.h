@@ -136,7 +136,7 @@ int sigma_ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const floa
                         void *workspace, size_t workspace_bytes, void *stream);
 
 /* bf16 inference mode: the same scan with xc and y in bf16 (x_dbl, the parameters, the state and the recurrence fp32; y rounded once
- * on its store).  D % 8 == 0.  Not for training: there is no bf16 counterpart of sigma_ss2d_scan_fwd_save.                      */
+ * on its store).  D % 8 == 0.  Training has its own pair: sigma_ss2d_scan_fwd_save_bf16 / sigma_ss2d_scan_bwd_saved_bf16.        */
 int sigma_ss2d_scan_fwd_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                              const float *Ds, void *y, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                              size_t workspace_bytes, void *stream);
@@ -176,6 +176,20 @@ int sigma_ss2d_scan_bwd_saved(int kind, const float *xc, const float *xdbl, cons
                               float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                               size_t workspace_bytes, int nsplit, void *stream);
 
+/* bf16 training mode of the pair above: xc, y, delta and dy are bf16 (16-byte aligned, D % 8 == 0 for the forward, D % 64 == 0 for
+ * the backward); x_dbl, hs, the parameters, the state, every accumulator and dxc / ddelta / dxdbl / dA / dDs / ddtb stay fp32
+ * (dxc is the fp32 accumulator of the directions' TMA reduce-adds; the caller rounds it once after adding dxdbl · xw).
+ * delta = softplus(dt_proj) is rounded to bf16 (nearest even) BEFORE the forward's recurrence uses it, so the backward recomputes
+ * exp(delta·A) from exactly the value the forward ran on; y is rounded once on its store.  Same workspace and hs queries, same
+ * nsplit convention, same kinds; d_state 4 / 16 (8: SIGMA_EUNSUPPORTED).  No deterministic build. */
+int sigma_ss2d_scan_fwd_save_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                  const float *Ds, void *y, void *delta, float *hs, int batch, int H, int W, int D, int N, int R, int Cp,
+                                  void *workspace, size_t workspace_bytes, int nsplit, void *stream);
+int sigma_ss2d_scan_bwd_saved_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                   const float *Ds, const void *dy, const void *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl,
+                                   float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                                   size_t workspace_bytes, int nsplit, void *stream);
+
 /* Deterministic builds of the fused backward (state sweep / after sigma_ss2d_scan_fwd_save): the same outputs, bitwise
  * reproducible for the same inputs, GPU model and L-segment plan.  Each direction's du goes to a slab summed over k into dxc,
  * dB / dC are kept per warp channel tile and dA / dDs / ddtb per (image, L-segment), all in the workspace, then summed in a
@@ -200,12 +214,18 @@ int sigma_layernorm_fwd(const float *x, const float *w, const float *b, float *y
                         int C, float eps, void *stream);
 /* bf16 inference mode: the same LayerNorm (fp32 statistics) with y stored as bf16 (8-byte aligned), to feed sigma_linear_bf16. */
 int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream);
+/* bf16 training mode: x and y both bf16 (8-byte aligned rows), fp32 statistics, w and b. */
+int sigma_layernorm_fwd_bf16io(const void *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream);
 
 /* Backward of sigma_layernorm_fwd (training path; the reference's autograd of nn.LayerNorm): dx (rows, C); dw (C) = sum over rows
  * of dy·xhat, db (C) = sum over rows of dy — both zeroed inside, then accumulated.  mean / rstd are recomputed from x.
  * C/4 must be one of {8, 16, 24, 32, 48, 64, 96, 128, 192, 256, 384} (every Sigma width up to 1536); else SIGMA_EUNSUPPORTED. */
 int sigma_layernorm_bwd(const float *x, const float *dy, const float *w, float *dx, float *dw, float *db, int64_t rows, int C,
                         float eps, void *stream);
+/* The same with bf16 x, dy and dx (8-byte aligned rows; the backward of sigma_layernorm_fwd_bf16io): statistics, dw and db fp32.
+ * No deterministic build. */
+int sigma_layernorm_bwd_bf16(const void *x, const void *dy, const float *w, void *dx, float *dw, float *db, int64_t rows, int C,
+                             float eps, void *stream);
 /* Deterministic build: dw / db kept per warp in the (16-byte aligned) workspace and summed in warp order; no float atomics. */
 size_t sigma_layernorm_bwd_det_workspace_bytes(int64_t rows, int C);
 int sigma_layernorm_bwd_det(const float *x, const float *dy, const float *w, float *dx, float *dw, float *db, int64_t rows, int C,
@@ -325,11 +345,13 @@ int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H
 /* L-segment plan of the fused scan backward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_bwd (nsplit = 0)
  * or sigma_ss2d_scan_bwd_split / sigma_ss2d_scan_bwd_saved with that nsplit would launch for kind CROSS4 / SEQ2 / CROSS (even
  * batch) at (batch, H, W, D, N).  out4_host = {segments, 16-position tiles per segment, tiles of the longest direction's walk, tiles of the shortest}.  The
- * directions share the tiles per segment, so a walk shorter than the longest can end in empty segments.  For tests and tuning. */
+ * directions share the tiles per segment, so a walk shorter than the longest can end in empty segments.  The plan does not depend
+ * on the element type: sigma_ss2d_scan_bwd_saved_bf16 launches the same segments.  For tests and tuning. */
 int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, int nsplit, int64_t *out4_host);
 
 /* Launch plan of the fused scan forward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_fwd (force_split = 0),
- * sigma_ss2d_scan_fwd_split (force_split > 0) or, with bf16 = 1, sigma_ss2d_scan_fwd_bf16 would launch for any kind at (batch, H,
+ * sigma_ss2d_scan_fwd_split (force_split > 0) or, with bf16 = 1, sigma_ss2d_scan_fwd_bf16 (bf16 = 2: sigma_ss2d_scan_fwd_save_bf16
+ * with nsplit = force_split; d_state 8 is SIGMA_EUNSUPPORTED there) would launch for any kind at (batch, H,
  * W, D, N, R) given a workspace of workspace_bytes (0: none), under the current environment (SIGMA_SCAN_WARPS, SIGMA_SCAN_NST,
  * SIGMA_SCAN_CTAS, SIGMA_SCAN_SPLIT_RULE).  out8_host = {segments, LT-position tiles per segment, tiles of the longest direction's
  * walk, tiles of the shortest, warps per CTA, TMA ring depth, register budget (the CTAs per SM the kernel build assumes: 3 or 4),

@@ -220,7 +220,7 @@ using namespace sigma;
 extern "C" {
 #pragma GCC visibility push(default)
 
-int sigma_abi_version(void) { return 1; }
+int sigma_abi_version(void) { return 1; }   // additions only since 1: every existing call is unchanged
 const char *sigma_last_error(void) { return g_err; }
 uint64_t sigma_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
@@ -327,6 +327,23 @@ int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, voi
   RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
   p.io = 1;
   return row_norm_launch(p, (cudaStream_t)stream);
+}
+
+int sigma_layernorm_fwd_bf16io(const void *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
+  SIGMA_CHECK_ARG(x && w && b && y, "sigma_layernorm_fwd_bf16io: null pointer");
+  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd_bf16io: C=%d must be a positive multiple of 4", C);
+  SIGMA_CHECK_ARG(al8(x) && al16(w) && al16(b) && al8(y), "sigma_layernorm_fwd_bf16io: w, b must be 16-byte and x, y 8-byte aligned");
+  RowNormParams p{(const float *)x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
+  p.io = 2;
+  return row_norm_launch(p, (cudaStream_t)stream);
+}
+
+int sigma_layernorm_bwd_bf16(const void *x, const void *dy, const float *w, void *dx, float *dw, float *db, int64_t rows, int C, float eps,
+                             void *stream) {
+  SIGMA_CHECK_ARG(x && dy && w && dx && dw && db, "sigma_layernorm_bwd_bf16: null pointer");
+  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_bwd_bf16: C=%d must be a positive multiple of 4", C);
+  SIGMA_CHECK_ARG(al8(x) && al8(dy) && al16(w) && al8(dx), "sigma_layernorm_bwd_bf16: w must be 16-byte and x, dy, dx 8-byte aligned");
+  return layernorm_bwd_launch((const float *)x, (const float *)dy, w, (float *)dx, dw, db, rows, C, eps, (cudaStream_t)stream, nullptr, true);
 }
 
 int sigma_layernorm_bwd(const float *x, const float *dy, const float *w, float *dx, float *dw, float *db, int64_t rows, int C, float eps,
@@ -528,7 +545,8 @@ int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, in
   return SIGMA_OK;
 }
 
-// the launch plan of sigma_ss2d_scan_fwd{,_split,_bf16} (force_split = 0: the library's choice), environment overrides included:
+// the launch plan of sigma_ss2d_scan_fwd{,_split,_bf16} and, with bf16 = 2, of sigma_ss2d_scan_fwd_save_bf16 (force_split = 0: the
+// library's choice), environment overrides included:
 // out8_host = {segments, tiles per segment, tiles of the longest walk, of the shortest, warps per CTA, ring depth, register
 // budget (CTAs per SM the kernel build assumes), dynamic shared-memory bytes}
 int sigma_test_ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R, int bf16, int force_split, size_t workspace_bytes,
@@ -537,6 +555,10 @@ int sigma_test_ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, in
                       H > 0 && W > 0 && D > 0 && D % (bf16 ? 8 : 4) == 0 && R > 0 && force_split >= 0 &&
                       (kind != SIGMA_DIRS_CROSS || batch % 2 == 0),
                   "sigma_test_ss2d_fwd_plan: bad arguments");
+  if (bf16 == 2 && N != 4 && N != 16) {
+    set_error("sigma_test_ss2d_fwd_plan: d_state=%d unsupported by the bf16 training forward (4, 16)", N);
+    return SIGMA_EUNSUPPORTED;
+  }
   long long out[8];
   const int rc = ss2d_fwd_plan_hook(kind, batch, H, W, D, N, R, bf16 ? 1 : 0, force_split, workspace_bytes, out);
   if (rc) return rc;
@@ -563,6 +585,23 @@ int sigma_ss2d_scan_fwd_save(int kind, const float *xc, const float *xdbl, const
                        (cudaStream_t)stream, delta, hs);
 }
 
+// the bf16 training mode: xc, y and delta are bf16, and delta is rounded before the recurrence uses it
+int sigma_ss2d_scan_fwd_save_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                  const float *Ds, void *y, void *delta, float *hs, int batch, int H, int W, int D, int N, int R, int Cp,
+                                  void *workspace, size_t workspace_bytes, int nsplit, void *stream) {
+  if (N == 8) {
+    set_error("sigma_ss2d_scan_fwd_save_bf16: d_state=8 unsupported (4, 16)");
+    return SIGMA_EUNSUPPORTED;
+  }
+  int rc = ss2d_check(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp);
+  if (rc) return rc;
+  SIGMA_CHECK_ARG(D % 8 == 0, "sigma_ss2d_scan_fwd_save_bf16: D=%d must be a multiple of 8 (16-byte TMA rows)", D);
+  SIGMA_CHECK_ARG(delta && hs && al16(delta) && al16(hs), "sigma_ss2d_scan_fwd_save_bf16: delta / hs must be non-null and 16-byte aligned");
+  SIGMA_CHECK_ARG(nsplit >= 0, "sigma_ss2d_scan_fwd_save_bf16: nsplit=%d < 0", nsplit);
+  return ss2d_scan_fwd(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp, workspace, workspace_bytes,
+                       nsplit, (cudaStream_t)stream, (float *)delta, hs, 1);
+}
+
 size_t sigma_ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
   if (kind != SIGMA_DIRS_CROSS4 && kind != SIGMA_DIRS_SEQ2 && (kind != SIGMA_DIRS_CROSS || batch % 2)) return 0;
   return ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N);
@@ -577,7 +616,7 @@ size_t sigma_ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W
 static int ss2d_bwd_entry(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                           const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb,
                           int batch, int H, int W, int D, int N, int R, int Cp, void *ws, size_t wsb, int nsplit, void *stream,
-                          const float *hs_saved = nullptr, int det = 0) {
+                          const float *hs_saved = nullptr, int det = 0, int bf16 = 0) {
   SIGMA_CHECK_ARG(xc && xdbl && dtw && dtb && A && Ds && dy && delta && dxc && ddelta && dxdbl && dA && dDs && ddtb, "sigma_ss2d_scan_bwd: null pointer");
   SIGMA_CHECK_ARG(kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2 || kind == SIGMA_DIRS_CROSS,
                   "sigma_ss2d_scan_bwd: kind %d unsupported (CROSS4, SEQ2, CROSS)", kind);
@@ -591,7 +630,7 @@ static int ss2d_bwd_entry(int kind, const float *xc, const float *xdbl, const fl
   SIGMA_CHECK_ARG(al16(xc) && al16(xdbl) && al16(dy) && al16(delta) && al16(dxc) && al16(ddelta) && al16(dxdbl), "sigma_ss2d_scan_bwd: pointers must be 16-byte aligned");
   SIGMA_CHECK_ARG(hs_saved == nullptr || al16(hs_saved), "sigma_ss2d_scan_bwd_saved: hs must be 16-byte aligned");
   return ss2d_scan_bwd(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, ws, wsb, nsplit,
-                       (cudaStream_t)stream, hs_saved, det);
+                       (cudaStream_t)stream, hs_saved, det, bf16);
 }
 
 // backward after sigma_ss2d_scan_fwd_save: `delta` and `hs` are INPUTS (what that call wrote); no state sweep runs
@@ -602,6 +641,21 @@ int sigma_ss2d_scan_bwd_saved(int kind, const float *xc, const float *xdbl, cons
   SIGMA_CHECK_ARG(hs != nullptr, "sigma_ss2d_scan_bwd_saved: null hs");
   return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, const_cast<float *>(delta), dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R,
                         Cp, workspace, workspace_bytes, nsplit, stream, hs);
+}
+
+// backward after sigma_ss2d_scan_fwd_save_bf16: xc, dy and delta are bf16; dxc and every other output fp32
+int sigma_ss2d_scan_bwd_saved_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                   const float *Ds, const void *dy, const void *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl,
+                                   float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                                   size_t workspace_bytes, int nsplit, void *stream) {
+  SIGMA_CHECK_ARG(hs != nullptr, "sigma_ss2d_scan_bwd_saved_bf16: null hs");
+  SIGMA_CHECK_ARG(nsplit >= 0, "sigma_ss2d_scan_bwd_saved_bf16: nsplit=%d < 0", nsplit);
+  if (N == 8) {
+    set_error("sigma_ss2d_scan_bwd_saved_bf16: d_state=8 unsupported (4, 16)");
+    return SIGMA_EUNSUPPORTED;
+  }
+  return ss2d_bwd_entry(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (const float *)dy, (float *)const_cast<void *>(delta), dxc, ddelta, dxdbl,
+                        dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace, workspace_bytes, nsplit, stream, hs, 0, 1);
 }
 
 int sigma_ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,

@@ -250,9 +250,10 @@ int row_norm_launch(const RowNormParams &p, cudaStream_t stream) {
 // atomicAdd per column (torch's GammaBetaBackwardCUDAKernel spent 5.9 ms per Sigma-tiny training step on this reduction).
 // DET: instead of the atomics, warp w of the grid writes its column sums to part[w·D ...] (dgamma) and
 // part[(nwarps + w)·D ...] (dbeta); sum_parts_det_kernel adds them in warp order.
-template <int LPR, int V, bool DET>
-__device__ __forceinline__ void layernorm_bwd_body(const float *__restrict__ x, const float *__restrict__ dy, const float *__restrict__ gamma,
-                                                   float *__restrict__ dx, float *__restrict__ dgamma, float *__restrict__ dbeta,
+// T: element type of x, dy and dx (float; __nv_bfloat16 for bf16 activations — gamma, the statistics, dgamma and dbeta stay fp32)
+template <int LPR, int V, bool DET, typename T = float>
+__device__ __forceinline__ void layernorm_bwd_body(const T *__restrict__ x, const T *__restrict__ dy, const float *__restrict__ gamma,
+                                                   T *__restrict__ dx, float *__restrict__ dgamma, float *__restrict__ dbeta,
                                                    long long rows, int D, float eps, float *__restrict__ part) {
   constexpr int RPW = 32 / LPR;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane / LPR, l = lane % LPR;
@@ -272,10 +273,16 @@ __device__ __forceinline__ void layernorm_bwd_body(const float *__restrict__ x, 
     const long long row_raw = step * RPW + sub;
     const bool valid = row_raw < rows;
     const long long row = valid ? row_raw : rows - 1;
-    const float4 *xr = reinterpret_cast<const float4 *>(x + row * D), *dr = reinterpret_cast<const float4 *>(dy + row * D);
     float4 xv[V], dv[V];
+    if constexpr (sizeof(T) == 4) {
+      const float4 *xr = reinterpret_cast<const float4 *>(x + row * D), *dr = reinterpret_cast<const float4 *>(dy + row * D);
 #pragma unroll
-    for (int v = 0; v < V; ++v) { xv[v] = __ldcs(xr + l + LPR * v); dv[v] = __ldcs(dr + l + LPR * v); }
+      for (int v = 0; v < V; ++v) { xv[v] = __ldcs(xr + l + LPR * v); dv[v] = __ldcs(dr + l + LPR * v); }
+    } else {
+      const T *xr = x + row * D, *dr = dy + row * D;
+#pragma unroll
+      for (int v = 0; v < V; ++v) { xv[v] = ld4cs(xr + 4 * (l + LPR * v)); dv[v] = ld4cs(dr + 4 * (l + LPR * v)); }
+    }
     float s = 0.f;
 #pragma unroll
     for (int v = 0; v < V; ++v) s += (xv[v].x + xv[v].y) + (xv[v].z + xv[v].w);
@@ -306,7 +313,7 @@ __device__ __forceinline__ void layernorm_bwd_body(const float *__restrict__ x, 
       s2 += __shfl_xor_sync(0xffffffffu, s2, o);
     }
     const float m1 = s1 * invD, m2 = s2 * invD;
-    float4 *outr = reinterpret_cast<float4 *>(dx + row * D);
+    float4 *outr = reinterpret_cast<float4 *>(dx + row * D);   // bf16: only the row's address (st4 below)
 #pragma unroll
     for (int v = 0; v < V; ++v) {
       const float4 gv = GREG ? g[GREG ? v : 0] : __ldg(gp + LPR * v);
@@ -316,7 +323,8 @@ __device__ __forceinline__ void layernorm_bwd_body(const float *__restrict__ x, 
       o.z = rstd * (gv.z * dv[v].z - m1 - xv[v].z * m2);
       o.w = rstd * (gv.w * dv[v].w - m1 - xv[v].w * m2);
       if (valid) {
-        outr[l + LPR * v] = o;
+        if constexpr (sizeof(T) == 4) outr[l + LPR * v] = o;
+        else st4(dx + row * D + 4 * (l + LPR * v), o);
         dg[v].x = fmaf(dv[v].x, xv[v].x, dg[v].x); dg[v].y = fmaf(dv[v].y, xv[v].y, dg[v].y);
         dg[v].z = fmaf(dv[v].z, xv[v].z, dg[v].z); dg[v].w = fmaf(dv[v].w, xv[v].w, dg[v].w);
         db[v].x += dv[v].x; db[v].y += dv[v].y; db[v].z += dv[v].z; db[v].w += dv[v].w;
@@ -369,6 +377,14 @@ __global__ void __launch_bounds__(256) layernorm_bwd_det_kernel(const float *__r
   layernorm_bwd_body<LPR, V, true>(x, dy, gamma, dx, nullptr, nullptr, rows, D, eps, part);
 }
 
+template <int LPR, int V>
+__global__ void __launch_bounds__(256) layernorm_bwd_bf16_kernel(const __nv_bfloat16 *__restrict__ x, const __nv_bfloat16 *__restrict__ dy,
+                                                                  const float *__restrict__ gamma, __nv_bfloat16 *__restrict__ dx,
+                                                                  float *__restrict__ dgamma, float *__restrict__ dbeta, long long rows,
+                                                                  int D, float eps) {
+  layernorm_bwd_body<LPR, V, false, __nv_bfloat16>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, nullptr);
+}
+
 // enough CTAs to fill the machine, few enough that the 2·D atomics per warp stay negligible (a warp walks >= 4 steps);
 // lanes per row as in the instantiation table of layernorm_bwd_launch
 static unsigned layernorm_bwd_grid(long long rows, int D) {
@@ -379,10 +395,12 @@ static unsigned layernorm_bwd_grid(long long rows, int D) {
 
 template <int LPR, int V>
 static void layernorm_bwd_k(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                            int D, float eps, float *part, cudaStream_t stream) {
+                            int D, float eps, float *part, cudaStream_t stream, bool bf16) {
+  using bf = __nv_bfloat16;
   const int warps = 8;
   const unsigned grid = layernorm_bwd_grid(rows, D);
-  if (part) layernorm_bwd_det_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>(x, dy, gamma, dx, rows, D, eps, part);
+  if (bf16) layernorm_bwd_bf16_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>((const bf *)x, (const bf *)dy, gamma, (bf *)dx, dgamma, dbeta, rows, D, eps);
+  else if (part) layernorm_bwd_det_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>(x, dy, gamma, dx, rows, D, eps, part);
   else layernorm_bwd_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps);
 }
 
@@ -393,9 +411,9 @@ size_t layernorm_bwd_det_workspace_bytes(long long rows, int D) {
 
 // dgamma / dbeta are zeroed here and accumulated into; false if D has no instantiation (the fast forward's D set).
 // part != nullptr: the deterministic build (layernorm_bwd_det_workspace_bytes of scratch), dgamma / dbeta written by the
-// fixed-order sum over the grid's warps
+// fixed-order sum over the grid's warps.  bf16 (never with part): x, dy and dx are bf16 behind the float pointers
 int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                         int D, float eps, cudaStream_t stream, float *part) {
+                         int D, float eps, cudaStream_t stream, float *part, bool bf16) {
   if (D & 3) { set_error("layernorm_bwd: D=%d must be a multiple of 4", D); return SIGMA_EUNSUPPORTED; }
   if (rows == 0 && !part) return SIGMA_OK;
   if (rows == 0) {
@@ -409,7 +427,7 @@ int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, fl
   }
   const int nvec = D >> 2;
   bool ok = false;
-#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) { layernorm_bwd_k<LPR, V>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, part, stream); SIGMA_CHECK_LAUNCH(); ok = true; }
+#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) { layernorm_bwd_k<LPR, V>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, part, stream, bf16); SIGMA_CHECK_LAUNCH(); ok = true; }
   TRY(8, 1) TRY(8, 2) TRY(8, 3) TRY(8, 4)
   TRY(16, 3) TRY(16, 4)
   TRY(32, 3) TRY(32, 4) TRY(32, 6) TRY(32, 8) TRY(32, 12)

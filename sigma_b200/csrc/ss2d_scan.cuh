@@ -25,6 +25,8 @@
 // the current one (software pipelining across tile boundaries: the only serial dependency is h = a·h + b).
 #pragma once
 #include "scan_core.cuh"
+#include <type_traits>
+
 #include "tma.cuh"
 
 namespace sigma {
@@ -59,7 +61,8 @@ struct alignas(64) Ss2dParams {
   int nst;     // TMA ring depth: as many LT-position stages as fit next to CTAS-1 other CTAs in shared memory
   int ablate;  // timing experiments, only in builds with -DSIGMA_SCAN_ABLATION (SIGMA_SCAN_ABLATE env):
                // 1 = no y store, 2 = no per-group prologue, 4 = no TMA reload
-  int xc_bf16; // 1: xc and y are bf16 (the bf16 inference mode, non-SAVE kernels only); x_dbl, the state and the recurrence stay fp32
+  int xc_bf16; // 1: xc and y are bf16; x_dbl, the state and the recurrence stay fp32.  With hsave (the bf16 training mode) the
+               // delta' slabs are bf16 too and the recurrence runs on the rounded delta'
 };
 
 #ifdef SIGMA_SCAN_ABLATION
@@ -100,7 +103,9 @@ __device__ __forceinline__ unsigned long long mul2_raw(unsigned long long a, uns
 // dt_r part of the first row) and whose xc values start at `xrow` (this thread's first channel).  dt_r is read
 // once per position (broadcast LDS.128) and used for all CPT channels; the dot product runs on fma2 pairs
 // (one accumulator chain up to RP = 12, two beyond), softplus is branch-free (common.cuh).
-template <int N, int CPT, int RP, int G, typename XT>
+// RND (the bf16 training mode): delta' is rounded to bf16 here, before the recurrence uses it, so that the value the forward
+// runs on is exactly the value it saves for the backward.
+template <int N, int CPT, int RP, int G, bool RND = false, typename XT>
 __device__ __forceinline__ void group_prologue(const Ss2dThread<N, CPT, RP> &t, const XT *xrow, const float *drow, int DT,
                                                float (&dl)[CPT][G], float (&u)[CPT][G]) {
   constexpr int Cp = 2 * N + RP;  // x_dbl row length: [B | C | dt_r padded to RP] (sigma_ss2d_padded_cp)
@@ -140,7 +145,8 @@ __device__ __forceinline__ void group_prologue(const Ss2dThread<N, CPT, RP> &t, 
 #pragma unroll
     for (int e = 0; e < G; e += 2) {
       const f2 sp = softplus20x2(dl[c][e], dl[c][e + 1]);
-      dl[c][e] = sp.x; dl[c][e + 1] = sp.y;
+      dl[c][e] = RND ? to_f32(from_f32<__nv_bfloat16>(sp.x)) : sp.x;
+      dl[c][e + 1] = RND ? to_f32(from_f32<__nv_bfloat16>(sp.y)) : sp.y;
     }
   }
 }
@@ -152,10 +158,10 @@ __device__ __forceinline__ void group_prologue(const Ss2dThread<N, CPT, RP> &t, 
 // channel lies beyond D walks a one-element sink instead (kernel prologue), so there is no branch around the store.
 // Per position B and C are read ONCE (2·N/4 broadcast LDS.128) and reused by the CPT channels of the thread;
 // per channel and state pair: mul2 (exp arguments), 2 x MUFU.EX2, mul2 (delta·u·B), fma2 (h), fma2 (C·h).
-template <int N, int CPT, int RP, int G, bool WITH_Y, bool REV, bool FULL, bool SAVE = false, typename XT = float>
+template <int N, int CPT, int RP, int G, bool WITH_Y, bool REV, bool FULL, bool SAVE = false, typename XT = float, typename ST = float>
 __device__ __forceinline__ void group_body(Ss2dThread<N, CPT, RP> &t, const float *rb, const float *rc, XT *yq,
                                            int ystep, int ycstride, const float (&dl)[CPT][G],
-                                           const float (&u)[CPT][G], int cnt, float *dq = nullptr) {
+                                           const float (&u)[CPT][G], int cnt, ST *dq = nullptr) {
   constexpr int Cp = 2 * N + RP;
   constexpr int NCH = N >= 8 ? 2 : 1;   // independent C·h accumulator chains per channel
 #pragma unroll
@@ -197,7 +203,7 @@ __device__ __forceinline__ void group_body(Ss2dThread<N, CPT, RP> &t, const floa
           if (NCH == 2) y += yacc[c][1].x + yacc[c][1].y;
           if (SIGMA_ABL(t.ablate, 1)) t.sumdl[c] += y;
           else yq[c * ycstride] = from_f32<XT>(fmaf(t.Dv[c], u[c][i], y));
-          if (SAVE) dq[c * ycstride] = dl[c][i];
+          if (SAVE) dq[c * ycstride] = from_f32<ST>(dl[c][i]);
         } else {
           t.sumdl[c] += dl[c][i];
         }
@@ -209,7 +215,7 @@ __device__ __forceinline__ void group_body(Ss2dThread<N, CPT, RP> &t, const floa
 }
 
 // Everything a warp needs to walk its CTA's tiles; filled once in the kernel.
-template <int N, int CPT, int RP, typename XT = float>
+template <int N, int CPT, int RP, typename XT = float, typename ST = float>
 struct Ss2dWalk {
   float *stages;
   uint64_t *full;
@@ -217,7 +223,7 @@ struct Ss2dWalk {
   XT *ybase;
   long long istride, ostride;
   int ystep;   // y elements from one walked position to the next (sign follows the walk direction; 0 on the sink)
-  float *dbase;        // SAVE: this thread's channel in the delta' slab of (k, b) (same addressing as ybase)
+  ST *dbase;           // SAVE: this thread's channel in the delta' slab of (k, b) (same addressing as ybase)
   float *hs_base;      // SAVE: hsave + (((k·batch + b)·save_tiles)·D + d)·N; tile tau16 adds tau16·D·N
   long long hs_stride; // D·N (0 on the sink)
   int TPO16, ntiles16; // 16-position blocks per inner walk line / in the whole walk (the backward's tile geometry)
@@ -229,15 +235,15 @@ struct Ss2dWalk {
 // The tile loop of one warp.  The software pipeline over groups of G positions runs ACROSS tiles: while the
 // recurrence of group g runs, delta'/u of group g+1 are computed — from the next tile's ring slot when g is the
 // last group of its tile — so no prologue is exposed at a tile boundary and none is computed twice.
-template <int N, int CPT, int RP, bool WITH_Y, bool REV, bool SAVE, typename XT, typename Request>
-__device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2dWalk<N, CPT, RP, XT> &w, Request &&request_tile) {
+template <int N, int CPT, int RP, bool WITH_Y, bool REV, bool SAVE, bool RND, typename XT, typename ST, typename Request>
+__device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2dWalk<N, CPT, RP, XT, ST> &w, Request &&request_tile) {
   constexpr int G = Ss2dCfg<N>::G, LT = Ss2dCfg<N>::LT;
   constexpr int Cp = 2 * N + RP;
   const int ycs = w.DT / CPT;
 
   // ring slot / phase and (outer index, inner tile) of the tile being opened advance incrementally: no division
   // or modulo per tile.  Tiles are walked in ascending tau; reversed directions map tau -> ntiles-1-tau.
-  struct Tile { const XT *sXC; const float *sDB, *sDC; XT *ystart; float *dstart; int npos, ng, tm16; };   // ystart: y of the tile's first WALKED group start
+  struct Tile { const XT *sXC; const float *sDB, *sDC; XT *ystart; ST *dstart; int npos, ng, tm16; };   // ystart: y of the tile's first WALKED group start
   int ost = 0, oph = 0;                                  // slot and phase parity of the next tile to open
   int tm0 = w.rev ? w.ntiles - 1 - w.t0 : w.t0;          // memory-order tile index of tile t0
   int oo = tm0 / w.TPO, oti = tm0 - oo * w.TPO;          // its (outer index, inner tile)
@@ -264,12 +270,12 @@ __device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2d
   Tile cur = open_tile();
   int j = REV ? cur.ng - 1 : 0;   // walking backwards, a ragged group (npos % G) comes first
   float dl[CPT][G], u[CPT][G];
-  group_prologue<N, CPT, RP, G>(t, cur.sXC + j * G * w.DT + w.ch, cur.sDB + j * G * Cp + 2 * N, w.DT, dl, u);
+  group_prologue<N, CPT, RP, G, RND>(t, cur.sXC + j * G * w.DT + w.ch, cur.sDB + j * G * Cp + 2 * N, w.DT, dl, u);
 
   int rst = 0;                    // ring slot of the tile being processed
   const int gstep = G * w.ystep;  // y elements from one group's first walked position to the next group's
   XT *yp = cur.ystart;            // running y pointer: first walked position of the current group
-  float *dp = cur.dstart;
+  ST *dp = cur.dstart;
   for (int tau = w.t0; tau < w.t1; ++tau) {
     Tile nxt = cur;
     int jn = j;
@@ -308,17 +314,17 @@ __device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2d
         }
       }
       if (cnt >= G) {
-        if (!SIGMA_ABL(t.ablate, 2)) group_prologue<N, CPT, RP, G>(t, px, pd, w.DT, dln, un);
+        if (!SIGMA_ABL(t.ablate, 2)) group_prologue<N, CPT, RP, G, RND>(t, px, pd, w.DT, dln, un);
         else {
 #pragma unroll
           for (int c = 0; c < CPT; ++c)
 #pragma unroll
             for (int i = 0; i < G; ++i) { dln[c][i] = dl[c][i] * 1.0001f; un[c][i] = u[c][i]; }
         }
-        group_body<N, CPT, RP, G, WITH_Y, REV, true, SAVE>(t, rb, rc, yp, w.ystep, ycs, dl, u, G, dp);
+        group_body<N, CPT, RP, G, WITH_Y, REV, true, SAVE, XT, ST>(t, rb, rc, yp, w.ystep, ycs, dl, u, G, dp);
       } else {
-        group_prologue<N, CPT, RP, G>(t, px, pd, w.DT, dln, un);
-        group_body<N, CPT, RP, G, WITH_Y, REV, false, SAVE>(t, rb, rc, yp, w.ystep, ycs, dl, u, cnt, dp);
+        group_prologue<N, CPT, RP, G, RND>(t, px, pd, w.DT, dln, un);
+        group_body<N, CPT, RP, G, WITH_Y, REV, false, SAVE, XT, ST>(t, rb, rc, yp, w.ystep, ycs, dl, u, cnt, dp);
       }
 #pragma unroll
       for (int c = 0; c < CPT; ++c)
@@ -341,11 +347,15 @@ __device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2d
   }
 }
 
-// XT: element type of xc and y (float; __nv_bfloat16 in the bf16 inference mode, not with SAVE)
-template <int N, int CPT, int RP, int MODE, int CTAS, bool SAVE = false, typename XT = float>
-__global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(const __grid_constant__ Ss2dParams p) {
+// XT: element type of xc and y (float; __nv_bfloat16 in the bf16 inference and training modes).
+// TRAIN16 (the bf16 training mode, XT = __nv_bfloat16): delta' is rounded to bf16 before the recurrence uses it — in the
+// summary pass too, whose carries must describe the same recurrence — and the SAVE passes store that bf16 delta'.
+template <int N, int CPT, int RP, int MODE, bool SAVE, typename XT, bool TRAIN16>
+__device__ __forceinline__ void ss2d_scan_body(const Ss2dParams &p) {
   static_assert(!SAVE || MODE != MODE_SUMMARY, "the summary pass has no final states to save");
-  static_assert(!SAVE || sizeof(XT) == 4, "the training forward stores fp32");
+  static_assert(!SAVE || sizeof(XT) == 4 || TRAIN16, "the fp32 training forward stores fp32");
+  static_assert(!TRAIN16 || sizeof(XT) == 2, "the bf16 training mode reads and writes bf16");
+  using ST = std::conditional_t<TRAIN16, __nv_bfloat16, float>;   // element type of the saved delta' slabs
   constexpr int LT = Ss2dCfg<N>::LT;
   constexpr bool WITH_Y = MODE != MODE_SUMMARY;
   const int NST = p.nst;
@@ -435,7 +445,7 @@ __global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(
     }
   }
 
-  Ss2dWalk<N, CPT, RP, XT> w;
+  Ss2dWalk<N, CPT, RP, XT, ST> w;
   w.stages = stages; w.full = full; w.done = done;
   static_assert(CPT == 1, "the sink redirection below assumes one channel per thread");
   if (t.ok[0]) {
@@ -448,7 +458,7 @@ __global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(
   w.ystep = (int)(rev ? -w.istride : w.istride);
   w.dbase = nullptr; w.hs_base = nullptr; w.hs_stride = 0; w.TPO16 = 0; w.ntiles16 = 0;
   if (SAVE) {
-    w.dbase = t.ok[0] ? p.dsave + (w.ybase - reinterpret_cast<XT *>(p.y)) : reinterpret_cast<float *>(w.ybase);          // same (K, batch, Lseq, D) addressing as y; sink otherwise
+    w.dbase = t.ok[0] ? reinterpret_cast<ST *>(p.dsave) + (w.ybase - reinterpret_cast<XT *>(p.y)) : reinterpret_cast<ST *>(w.ybase);          // same (K, batch, Lseq, D) addressing as y; sink otherwise
     w.TPO16 = (I + 15) >> 4;
     w.ntiles16 = O * w.TPO16;
     w.hs_stride = (long long)p.D * N;
@@ -459,8 +469,8 @@ __global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(
   w.t0 = t0; w.t1 = t1; w.TPO = TPO; w.ntiles = ntiles; w.I = I; w.nst = NST;
   w.cross = cross; w.rev = rev;
 
-  if (rev) walk_tiles<N, CPT, RP, WITH_Y, true, SAVE>(t, w, request_tile);
-  else     walk_tiles<N, CPT, RP, WITH_Y, false, SAVE>(t, w, request_tile);
+  if (rev) walk_tiles<N, CPT, RP, WITH_Y, true, SAVE, TRAIN16>(t, w, request_tile);
+  else     walk_tiles<N, CPT, RP, WITH_Y, false, SAVE, TRAIN16>(t, w, request_tile);
 
   if (MODE == MODE_SUMMARY || SIGMA_ABL(p.ablate, 1)) {
 #pragma unroll
@@ -474,6 +484,18 @@ __global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(
       }
     }
   }
+}
+
+template <int N, int CPT, int RP, int MODE, int CTAS, bool SAVE = false, typename XT = float>
+__global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(const __grid_constant__ Ss2dParams p) {
+  static_assert(!SAVE || sizeof(XT) == 4, "the bf16 training forward is ss2d_scan_train16_kernel");
+  ss2d_scan_body<N, CPT, RP, MODE, SAVE, XT, false>(p);
+}
+
+// the bf16 training mode: bf16 xc / y and a bf16 delta' that the recurrence itself runs on (see ss2d_scan_body)
+template <int N, int CPT, int RP, int MODE, int CTAS, bool SAVE>
+__global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_train16_kernel(const __grid_constant__ Ss2dParams p) {
+  ss2d_scan_body<N, CPT, RP, MODE, SAVE, __nv_bfloat16, true>(p);
 }
 
 // host-side launcher for one (N, CPT, RP) instantiation; defined per RP in ss2d_scan_rp*.cu.

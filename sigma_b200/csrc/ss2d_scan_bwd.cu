@@ -223,16 +223,19 @@ __global__ void __launch_bounds__(128, 3) ss2d_state_cross_kernel(const __grid_c
 // DET: every sum across CTAs goes to the partials of the deterministic build (see Ss2dBwdParams) instead of an atomic.
 // CROSS: image b runs with weight set kw = [b >= batch/2] and reads C from image bC = the other modality's (as the forward):
 // the stage holds bC's x_dbl tile too, dC goes to the C columns of bC's dxdbl rows, dA / dDs / d dt_bias to rows kw·D + d.
-template <int N, int MODE, bool DET, bool CROSS>
+// XT: element type of the xc, dy and delta' tiles (float; __nv_bfloat16 in the bf16 training mode, which widens them on the read
+// from the stage and keeps everything else — x_dbl, hs, every accumulator, du / ddelta and their TMA stores — fp32).
+template <int N, int MODE, bool DET, bool CROSS, typename XT = float>
 __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
   static_assert(!(DET && CROSS), "no deterministic build of the CROSS backward");
+  static_assert(!DET || sizeof(XT) == 4, "no deterministic build of the bf16 backward");
   constexpr int LPC = FbCfg<N>::LPC, NS = FbCfg<N>::NS, CPW = FbCfg<N>::CPW, NT = FB_DT * LPC;
   constexpr bool MAIN = MODE != MODE_SUMMARY;
   constexpr float kLn2 = 0.6931471805599453f;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   float *smem = reinterpret_cast<float *>(smem_raw);
   const int NST = p.nst, Cp = p.Cp;
-  const int xc_fl = FB_LT * FB_DT, dbl_fl = FB_LT * Cp;
+  const int xc_fl = FB_LT * FB_DT * (int)sizeof(XT) / 4, dbl_fl = FB_LT * Cp;   // tile sizes in floats (bf16 tiles: half)
   const int stage_fl = (MAIN ? 3 : 2) * xc_fl + (CROSS ? 2 : 1) * dbl_fl;   // [xc] dy dl dbl [dbl of image bC]
   float *stage_all = smem + NST * stage_fl;                        // per-warp staging: du [16][CPW], ddelta [16][CPW]
   float4 *sH = reinterpret_cast<float4 *>(stage_all + (MAIN ? (NT / 32) * 2 * FB_LT * CPW : 0));   // [16][NS/4][NT]
@@ -306,7 +309,9 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
     w.tile(tau, o, i0, npos);
     mbar_spin(&full[st], (uint32_t)ph);
     const float *base = smem + st * stage_fl;
-    const float *sXC = base, *sDY = base + (MAIN ? xc_fl : 0), *sDL = sDY + xc_fl, *sDB = sDL + xc_fl;
+    const XT *sXC = reinterpret_cast<const XT *>(base), *sDY = reinterpret_cast<const XT *>(base + (MAIN ? xc_fl : 0));
+    const XT *sDL = reinterpret_cast<const XT *>(base + (MAIN ? 2 : 1) * xc_fl);
+    const float *sDB = base + (MAIN ? 3 : 2) * xc_fl;
     const float *sDC = CROSS ? sDB + dbl_fl : sDB;   // the x_dbl tile C is read from
 
     if (MAIN) {
@@ -318,8 +323,8 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
 #pragma unroll 1
       for (int s = 0; s < npos; ++s) {
         const int r = w.rev ? npos - 1 - s : s;
-        const float dl = sDL[r * FB_DT + c];
-        const float du = dl * sXC[r * FB_DT + c];
+        const float dl = to_f32(sDL[r * FB_DT + c]);
+        const float du = dl * to_f32(sXC[r * FB_DT + c]);
         const float *row = sDB + r * Cp + n0;
 #pragma unroll
         for (int q = 0; q < NS / 4; ++q) {
@@ -340,7 +345,7 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
 #pragma unroll 1
     for (int s = npos - 1; s >= 0; --s) {
       const int r = w.rev ? npos - 1 - s : s;
-      const float dl = sDL[r * FB_DT + c], dy = sDY[r * FB_DT + c];
+      const float dl = to_f32(sDL[r * FB_DT + c]), dy = to_f32(sDY[r * FB_DT + c]);
       const float *row = sDB + r * Cp + n0, *rowC = sDC + r * Cp + n0;
       if (!MAIN) {
 #pragma unroll
@@ -354,7 +359,7 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
         sumdl += dl;
         continue;
       }
-      const float u = sXC[r * FB_DT + c];
+      const float u = to_f32(sXC[r * FB_DT + c]);
       const float dlu = dl * u;
       float cB[NS], cC[NS];
       float s1 = 0.f, s2 = 0.f;     // Σ dh·B and Σ t·a2 over this lane's states
@@ -458,6 +463,13 @@ __global__ void __launch_bounds__(128, 2) ss2d_bwd_det_kernel(const __grid_const
 template <int N, int MODE>
 __global__ void __launch_bounds__(128, 2) ss2d_bwd_cross_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, false, true>(p); }
 
+// the bf16 training mode (non-deterministic only): bf16 xc / dy / delta' tiles
+template <int N, int MODE>
+__global__ void __launch_bounds__(128, 2) ss2d_bwd_bf16_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, false, false, __nv_bfloat16>(p); }
+
+template <int N, int MODE>
+__global__ void __launch_bounds__(128, 2) ss2d_bwd_cross_bf16_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, false, true, __nv_bfloat16>(p); }
+
 // ---- host ----
 constexpr int kFbMaxSplit = 64;
 
@@ -538,13 +550,15 @@ int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int forc
 int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                   const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
                   int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream,
-                  const float *hs_saved, int det) {
+                  const float *hs_saved, int det, int bf16) {
   const size_t need = det ? ss2d_scan_bwd_det_workspace_bytes(kind, batch, H, W, D, N) : ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N);
   if (ws == nullptr || ws_bytes < need) {
     set_error("sigma_ss2d_scan_bwd: workspace too small (%zu < %zu)", ws_bytes, need);
     return SIGMA_EWORKSPACE;
   }
   const bool cross = kind == SIGMA_DIRS_CROSS;   // never with det (the entry points reject it)
+  // bf16 (never with det, always with hs_saved; the entry point checks): xc, dy and delta are bf16 behind the float pointers
+  const uint64_t xes = bf16 ? 2 : 4;             // bytes per xc / dy / delta element
   Ss2dBwdParams p;
   memset(&p, 0, sizeof(p));
   const int K = fb_dirs(kind), Kw = fb_wsets(kind);
@@ -560,14 +574,15 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
   float *fcarry = (float *)((char *)ws + hs_b), *rcarry = (float *)((char *)ws + hs_b + carry_b);
   const int CPW = N >= 16 ? 16 : 32;
   int rc;
-  auto tmap = [](CUtensorMap *map, const void *base, const uint64_t *dims, const uint64_t *str, const uint32_t *box) {
-    return make_tmap(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+  auto tmap = [](CUtensorMap *map, const void *base, const uint64_t *dims, const uint64_t *str, const uint32_t *box,
+                 CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT32) {
+    return make_tmap(map, dtype, 4, base, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
   };
+  const CUtensorMapDataType xdt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   for (int k = 0; k < K; ++k) {
     const bool colmajor = kind == SIGMA_DIRS_CROSS4 && (k & 1);
     p.rev[k] = kind == SIGMA_DIRS_CROSS4 ? (k >= 2) : (k == 1);
-    uint64_t dims[4], str[3];
+    uint64_t dims[4], str[3], strx[3];   // str: fp32 rows (dxc); strx: rows of xc / dy / delta
     uint32_t box[4] = {(uint32_t)FB_DT, (uint32_t)FB_LT, 1, 1}, boxw[4] = {(uint32_t)CPW, (uint32_t)FB_LT, 1, 1};
     if (!colmajor) {
       p.I[k] = (int)Lseq; p.O[k] = 1; p.psi[k] = 1; p.pso[k] = 0;
@@ -578,11 +593,12 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
       dims[0] = D; dims[1] = H; dims[2] = W; dims[3] = batch;
       str[0] = (uint64_t)W * D * 4; str[1] = (uint64_t)D * 4; str[2] = (uint64_t)Lseq * D * 4;
     }
-    if ((rc = tmap(&p.m_xc[k], xc, dims, str, box))) return rc;
-    if ((rc = tmap(&p.m_dy[k], dy, dims, str, box))) return rc;
+    for (int i = 0; i < 3; ++i) strx[i] = str[i] / 4 * xes;
+    if ((rc = tmap(&p.m_xc[k], xc, dims, strx, box, xdt))) return rc;
+    if ((rc = tmap(&p.m_dy[k], dy, dims, strx, box, xdt))) return rc;
     if ((rc = tmap(&p.m_dxc[k], dxc, dims, str, boxw))) return rc;
     dims[3] = (uint64_t)K * batch;   // slabs: image index k·batch + b
-    if ((rc = tmap(&p.m_dl[k], delta, dims, str, box))) return rc;
+    if ((rc = tmap(&p.m_dl[k], delta, dims, strx, box, xdt))) return rc;
     dims[3] = batch;
     uint32_t boxd[4] = {(uint32_t)Cp, (uint32_t)FB_LT, 1, 1};
     dims[0] = Cp;
@@ -620,7 +636,7 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
     }
     return SIGMA_OK;
   };
-  if ((rc = make_dd(delta))) return rc;
+  if (!bf16 && (rc = make_dd(delta))) return rc;   // (the bf16 mode runs no state sweep: its delta slabs are an input)
   Ss2dBwdParams ps = p;
   if ((rc = make_dd(ddelta))) return rc;
   const FbDetLayout dl = fb_det_layout(kind, batch, H, W, D, N);
@@ -641,8 +657,9 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
     const long long nrows = (long long)batch * K * D, tot = nrows * NN;
     const size_t st_smem = ((size_t)pm.nst * (2 * FB_LT * FB_DT + FB_LT * Cp) + FB_DT * (R + 1) + 2 + (NT / 32) * FB_LT * CPWc) * sizeof(float) + 256;
     const size_t dbl_tiles = cross ? 2 : 1;   // the reverse sweeps of CROSS also stage the C image's x_dbl tile
-    const size_t sm_smem = ((size_t)pm.nst * (2 * FB_LT * FB_DT + dbl_tiles * FB_LT * Cp)) * sizeof(float) + 256;
-    const size_t mn_smem = ((size_t)pm.nst * (3 * FB_LT * FB_DT + dbl_tiles * FB_LT * Cp) + (NT / 32) * 2 * FB_LT * CPWc + (size_t)FB_LT * NS * NT) * sizeof(float) + 256;
+    const size_t xt_fl = FB_LT * FB_DT * xes / 4;   // an xc / dy / delta tile, in floats
+    const size_t sm_smem = ((size_t)pm.nst * (2 * xt_fl + dbl_tiles * FB_LT * Cp)) * sizeof(float) + 256;
+    const size_t mn_smem = ((size_t)pm.nst * (3 * xt_fl + dbl_tiles * FB_LT * Cp) + (NT / 32) * 2 * FB_LT * CPWc + (size_t)FB_LT * NS * NT) * sizeof(float) + 256;
     auto run = [&](auto kern, const Ss2dBwdParams &pp, size_t smem) -> int {
       SIGMA_CHECK_CUDA(prep_kernel_once((const void *)kern));
       kern<<<grid, block, smem, stream>>>(pp);
@@ -653,9 +670,12 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
     const Kern st_serial = cross ? ss2d_state_cross_kernel<NN, MODE_SERIAL> : ss2d_state_kernel<NN, MODE_SERIAL>;
     const Kern st_summary = cross ? ss2d_state_cross_kernel<NN, MODE_SUMMARY> : ss2d_state_kernel<NN, MODE_SUMMARY>;
     const Kern st_apply = cross ? ss2d_state_cross_kernel<NN, MODE_APPLY> : ss2d_state_kernel<NN, MODE_APPLY>;
-    const Kern bw_serial = cross ? ss2d_bwd_cross_kernel<NN, MODE_SERIAL> : ss2d_bwd_kernel<NN, MODE_SERIAL>;
-    const Kern bw_summary = cross ? ss2d_bwd_cross_kernel<NN, MODE_SUMMARY> : ss2d_bwd_kernel<NN, MODE_SUMMARY>;
-    const Kern bw_apply = cross ? ss2d_bwd_cross_kernel<NN, MODE_APPLY> : ss2d_bwd_kernel<NN, MODE_APPLY>;
+    const Kern bw_serial = bf16 ? (cross ? ss2d_bwd_cross_bf16_kernel<NN, MODE_SERIAL> : ss2d_bwd_bf16_kernel<NN, MODE_SERIAL>)
+                                : (cross ? ss2d_bwd_cross_kernel<NN, MODE_SERIAL> : ss2d_bwd_kernel<NN, MODE_SERIAL>);
+    const Kern bw_summary = bf16 ? (cross ? ss2d_bwd_cross_bf16_kernel<NN, MODE_SUMMARY> : ss2d_bwd_bf16_kernel<NN, MODE_SUMMARY>)
+                                 : (cross ? ss2d_bwd_cross_kernel<NN, MODE_SUMMARY> : ss2d_bwd_kernel<NN, MODE_SUMMARY>);
+    const Kern bw_apply = bf16 ? (cross ? ss2d_bwd_cross_bf16_kernel<NN, MODE_APPLY> : ss2d_bwd_bf16_kernel<NN, MODE_APPLY>)
+                               : (cross ? ss2d_bwd_cross_kernel<NN, MODE_APPLY> : ss2d_bwd_kernel<NN, MODE_APPLY>);
     int r;
     ps.carry = fcarry;
     if (hs_saved != nullptr) {

@@ -4,7 +4,10 @@
 (csrc/selective_scan/selective_scan.cpp:364-367); `sigma_b200/dropin/selective_scan_cuda_core.py`
 re-exports them under the reference's module name.
 """
+import contextlib
 import ctypes
+import functools
+import os
 
 import numpy as np
 import torch
@@ -343,22 +346,65 @@ def fused_core_ok(xc, D, N):
     return FUSED_TRAINING and xc.is_cuda and N in (4, 16) and D % 64 == 0
 
 
+# ---- bf16 training mode of the fused core (opt-in) ----
+# On, the fused core and the LayerNorm pair keep bf16 activations under bf16 autocast instead of widening them to fp32: bf16 xc, y,
+# dy, dxc and saved delta' (x_dbl, the states, every accumulator and every parameter gradient stay fp32).  Off (the default), autocast
+# does not change those two autograd nodes.  SIGMA_BF16_TRAINING_CORE=1 sets the initial value.
+BF16_TRAINING_CORE = os.environ.get("SIGMA_BF16_TRAINING_CORE", "0") == "1"
+
+
+@contextlib.contextmanager
+def bf16_training_core(on=True):
+    """Switch the bf16 training mode of the fused core on (or off) inside the block."""
+    global BF16_TRAINING_CORE
+    prev, BF16_TRAINING_CORE = BF16_TRAINING_CORE, bool(on)
+    try:
+        yield
+    finally:
+        BF16_TRAINING_CORE = prev
+
+
+def _bf16_autocast():
+    return (BF16_TRAINING_CORE and torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16
+            and not deterministic())
+
+
+def _bf16_mode_fwd(takes_bf16):
+    """torch.amp.custom_fwd(cast_inputs=torch.float32) for an autograd forward, except when `takes_bf16(ctx, *args)` holds under
+    the bf16 training mode: then the arguments are passed as they are (autocast off inside, as custom_fwd does) and
+    ctx.bf16_mode is True."""
+    def decorate(fwd):
+        widened = torch.amp.custom_fwd(fwd, device_type="cuda", cast_inputs=torch.float32)
+
+        @functools.wraps(fwd)
+        def wrapper(ctx, *args):
+            ctx.bf16_mode = _bf16_autocast() and takes_bf16(ctx, *args)
+            if not ctx.bf16_mode:
+                return widened(ctx, *args)
+            ctx._dtype, ctx._fwd_used_autocast = torch.get_autocast_dtype("cuda"), False    # what custom_bwd reads
+            with torch.autocast("cuda", enabled=False):
+                return fwd(ctx, *args)
+        return wrapper
+    return decorate
+
+
 _LN_WIDTHS = {32, 64, 96, 128, 192, 256, 384, 512, 768, 1024, 1536}   # C with an instantiation of sigma_layernorm_bwd
 FUSED_LAYERNORM = True
 
 
 class LayerNormFn(torch.autograd.Function):
     """nn.LayerNorm over the last dim under autograd: forward = sigma_layernorm_fwd, backward = sigma_layernorm_bwd (dx, dweight, dbias in
-    one pass over x and dy; nothing saved but x).  Numerics as F.layer_norm in fp32."""
+    one pass over x and dy; nothing saved but x).  Numerics as F.layer_norm in fp32.  In the bf16 training mode a bf16 x stays bf16
+    (sigma_layernorm_fwd_bf16io / sigma_layernorm_bwd_bf16: bf16 x, y, dy, dx; fp32 statistics, parameters and their gradients)."""
 
     @staticmethod
-    @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
+    @_bf16_mode_fwd(lambda ctx, x, weight, bias, eps: x.dtype == torch.bfloat16 and weight.dtype == torch.float32)
     def forward(ctx, x, weight, bias, eps):
         x2 = x.contiguous().view(-1, x.shape[-1])
         y = torch.empty_like(x2)
         w, b = weight.contiguous(), bias.contiguous()
-        _lib.check(_lib.lib().sigma_layernorm_fwd(ptr(x2), ptr(w), ptr(b), ptr(y), x2.shape[0], x2.shape[1], float(eps), stream()),
-                   "sigma_layernorm_fwd")
+        fn = "sigma_layernorm_fwd_bf16io" if ctx.bf16_mode else "sigma_layernorm_fwd"
+        _lib.check(getattr(_lib.lib(), fn)(ptr(x2), ptr(w), ptr(b), ptr(y), x2.shape[0], x2.shape[1], float(eps), stream()), fn)
         ctx.save_for_backward(x2, w)
         ctx.eps = float(eps)
         return y.view(x.shape)
@@ -367,9 +413,14 @@ class LayerNormFn(torch.autograd.Function):
     @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, dy):
         x2, w = ctx.saved_tensors
-        dy2 = dy.contiguous().float().view(-1, x2.shape[1])
         dx = torch.empty_like(x2)
         dw, db = torch.empty_like(w), torch.empty_like(w)
+        if ctx.bf16_mode:
+            dy2 = dy.contiguous().to(torch.bfloat16).view(-1, x2.shape[1])
+            _lib.check(_lib.lib().sigma_layernorm_bwd_bf16(ptr(x2), ptr(dy2), ptr(w), ptr(dx), ptr(dw), ptr(db), x2.shape[0], x2.shape[1],
+                                                          ctx.eps, stream()), "sigma_layernorm_bwd_bf16")
+            return dx.view(dy.shape), dw, db, None
+        dy2 = dy.contiguous().float().view(-1, x2.shape[1])
         if deterministic():
             L_ = _lib.lib()
             wsb = L_.sigma_layernorm_bwd_det_workspace_bytes(x2.shape[0], x2.shape[1])
@@ -395,10 +446,17 @@ def layer_norm(norm, x):
 FUSED_SAVE_STATES = True      # training forward keeps delta' and the block-start states, so the backward runs no state sweep
 
 
+_SAVED_BF16 = 2               # `saved` of _call_ss2d_bwd: the arguments are those of sigma_ss2d_scan_bwd_saved_bf16
+
+
 def _call_ss2d_bwd(args, saved=False, det=False):
-    """The native call of the fused backward (a module-level function so that bench.py can bracket it with events)."""
+    """The native call of the fused backward (a module-level function so that bench.py can bracket it with events, through a
+    wrapper that passes (args, saved) on: so the bf16 training mode is a value of `saved`, not another argument)."""
     from . import fused
     L_ = _lib.lib()
+    if saved == _SAVED_BF16:
+        _lib.check(L_.sigma_ss2d_scan_bwd_saved_bf16(*args, int(fused._FORCE_SPLIT or 0), stream()), "sigma_ss2d_scan_bwd_saved_bf16")
+        return
     if det:
         fn = L_.sigma_ss2d_scan_bwd_saved_det if saved else L_.sigma_ss2d_scan_bwd_det
         _lib.check(fn(*args, int(fused._FORCE_SPLIT or 0), stream()), "sigma_ss2d_scan_bwd_det")
@@ -422,10 +480,15 @@ class FusedSS2DCore(torch.autograd.Function):
     With FUSED_SAVE_STATES = False the plain forward runs and sigma_ss2d_scan_bwd recomputes both in a state sweep.
     Kind CROSS is Cross_Mamba_Attention_SSM.forward (vmamba.py:1508-1545): xc (2·images, L, D) modality-major, the parameters of
     the two modalities stacked (x_proj_weight (2, R+2N, D), dt_projs_weight (2, D, R), dt_projs_bias (2, D), A_logs (2D, N), Ds
-    (2D)); each half runs its own x_proj and weights and reads C from the other half.  It has no deterministic backward."""
+    (2D)); each half runs its own x_proj and weights and reads C from the other half.  It has no deterministic backward.
+    The bf16 training mode (BF16_TRAINING_CORE, bf16 autocast, FUSED_SAVE_STATES, not deterministic, some input needs a gradient):
+    xc is taken (or cast to) bf16 and never widened, x_proj runs the bf16 GEMM with fp32 x_dbl out, sigma_ss2d_scan_fwd_save_bf16
+    writes bf16 y and the bf16 delta' its own recurrence ran on, and the backward (sigma_ss2d_scan_bwd_saved_bf16) takes a bf16 dy
+    and returns a bf16 dxc rounded once from the fp32 sum of the directions and the x_proj term; parameter gradients are fp32."""
 
     @staticmethod
-    @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
+    @_bf16_mode_fwd(lambda ctx, xc, *a: FUSED_SAVE_STATES and any(ctx.needs_input_grad) and fused_core_ok(xc, xc.shape[-1], a[3].shape[1])
+                    and all(t.dtype == torch.float32 for t in a[:5]))
     def forward(ctx, xc, x_proj_weight, dt_projs_weight, dt_projs_bias, A_logs, Ds, kind, H, W):
         from . import fused
         Kw, _, D = x_proj_weight.shape
@@ -434,6 +497,8 @@ class FusedSS2DCore(torch.autograd.Function):
         N, R = A_logs.shape[1], dt_projs_weight.shape[2]
         Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
         xc = xc.contiguous()
+        if ctx.bf16_mode:
+            xc = xc.to(torch.bfloat16)           # a bf16 xc (the conv + SiLU under autocast) passes through untouched
         B, Lseq, _ = xc.shape
         xw = torch.cat([fused._pack_xproj(x_proj_weight[k], N, R, Cp) for k in range(Kw)], dim=0).contiguous()     # (Kw·Cp, D)
         if cross:   # each modality's half of the batch through its own x_proj
@@ -474,11 +539,12 @@ class FusedSS2DCore(torch.autograd.Function):
             raise RuntimeError("FusedSS2DCore: kind CROSS has no deterministic backward; under torch.use_deterministic_algorithms(True) "
                                "CroMB trains through the op-level _det kernels (CrossMambaFusion_SS2D_SSM routes there itself)")
         B, Lseq, _ = xc.shape
-        dy = dy.contiguous().float()
+        bf16 = ctx.bf16_mode
+        dy = dy.contiguous().to(torch.bfloat16) if bf16 else dy.contiguous().float()
         dev = xc.device
         if not saved:
             delta = torch.empty((K, B, Lseq, D), dtype=torch.float32, device=dev)
-        ddelta = torch.empty_like(delta)
+        ddelta = torch.empty((K, B, Lseq, D), dtype=torch.float32, device=dev)
         dxc = torch.empty((B, Lseq, D), dtype=torch.float32, device=dev)
         dxdbl = torch.empty((B * Lseq, K, Cp), dtype=torch.float32, device=dev)
         dA = torch.empty((Kw * D, N), dtype=torch.float32, device=dev)
@@ -491,7 +557,11 @@ class FusedSS2DCore(torch.autograd.Function):
         tail = (ptr(dxc), ptr(ddelta), ptr(dxdbl), ptr(dA), ptr(dDs), ptr(ddtb), B, H, W, D, N, R, Cp, ptr(ws), wsb)
         args = head + ((ptr(hs),) if saved else ()) + tail
         # det only when set: bench.py --mode train brackets this call with a wrapper that takes (args, saved)
-        _call_ss2d_bwd(args, saved, True) if det else _call_ss2d_bwd(args, saved)
+        if bf16:
+            _call_ss2d_bwd(args, _SAVED_BF16)
+            xc = xc.float()                      # only the x_proj weight gradient below (a torch matmul) needs the widened copy
+        else:
+            _call_ss2d_bwd(args, saved, True) if det else _call_ss2d_bwd(args, saved)
         if cross:   # the same two steps per modality half m (its rows of dxdbl / ddelta / xc, its weight set)
             n = B // 2 * Lseq
             xd, dxd, dd = xdbl.view(2, n, Cp), dxdbl.view(2, n, Cp), ddelta.view(2, n, D)
@@ -503,7 +573,7 @@ class FusedSS2DCore(torch.autograd.Function):
                 dxcm[m].addmm_(dxd[m], xw3[m])
                 dxw[m] = dxd[m].t() @ xcm[m]
             dxpw = torch.cat([dxw[:, 2 * N:2 * N + R], dxw[:, 0:N], dxw[:, N:2 * N]], dim=1)
-            return dxc, dxpw, dW, ddtb, dA * A, dDs, None, None, None
+            return (dxc.to(torch.bfloat16) if bf16 else dxc), dxpw, dW, ddtb, dA * A, dDs, None, None, None
         # dt_proj: d dt_r = ddelta_k · W_dt[k]  (into the dt_r columns of dxdbl),  dW_dt[k] = ddelta_k^T · dt_r_k
         xd3 = xdbl.view(B * Lseq, K, Cp)
         dW = torch.empty_like(dtw)
@@ -517,7 +587,7 @@ class FusedSS2DCore(torch.autograd.Function):
         dxc2.addmm_(d2, xw)
         dxw = (d2.t() @ xc.view(B * Lseq, D)).view(K, Cp, D)
         dxpw = torch.cat([dxw[:, 2 * N:2 * N + R], dxw[:, 0:N], dxw[:, N:2 * N]], dim=1)          # back to [dt | B | C] rows
-        return dxc, dxpw, dW, ddtb, dA * A, dDs, None, None, None
+        return (dxc.to(torch.bfloat16) if bf16 else dxc), dxpw, dW, ddtb, dA * A, dDs, None, None, None
 
 
 # ---- deterministic training: bilinear upsampling and cross-entropy ----

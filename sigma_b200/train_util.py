@@ -52,14 +52,18 @@ def wrap_ddp(model, device_index=None, single_bucket=False):
 
 class TrainStep:
     """One iteration of train.py:164-172: loss = model(imgs, modal_xs, gts); zero_grad; backward; optimizer.step.
-    `amp_dtype` = torch.bfloat16 runs the dense layers under autocast (the scan casts itself to fp32, vmamba.py:36)."""
+    `amp_dtype` = torch.bfloat16 runs the dense layers under autocast (the scan casts itself to fp32, vmamba.py:36).
+    `bf16_core` = True switches the bf16 training mode of the fused core on around the step (ops.bf16_training_core); False
+    leaves ops.BF16_TRAINING_CORE as it is."""
 
-    def __init__(self, model, optimizer, amp_dtype=None, device_type="cuda"):
+    def __init__(self, model, optimizer, amp_dtype=None, device_type="cuda", bf16_core=False):
         self.model, self.opt, self.amp, self.device_type = model, optimizer, amp_dtype, device_type
+        self.bf16_core = bf16_core
 
     def __call__(self, rgb, modal_x, label, sync=True):
+        from . import ops
         ctx = self.model.no_sync() if (not sync and hasattr(self.model, "no_sync")) else contextlib.nullcontext()
-        with ctx:
+        with ctx, (ops.bf16_training_core() if self.bf16_core else contextlib.nullcontext()):
             with torch.autocast(self.device_type, dtype=self.amp, enabled=self.amp is not None):
                 loss = self.model(rgb, modal_x, label)
             self.opt.zero_grad(set_to_none=True)
