@@ -44,7 +44,17 @@ rounded once, and a compiler-contracted FMA rounds less often than the separate 
     one term of the deterministic warp-order sum) per warp.  Over more than 16 roundings the bound uses the probabilistic model of
     Higham & Mary (SIAM J. Sci. Comput. 2019): n roundings of partial sums bounded by S err by at most 4·sqrt(n)·u·S, S = sum |terms|.
 Every first-order bound is multiplied by SAFETY = 1.25 for the second-order products of the itemised errors (each below 1e-4 of
-the first-order total on these inputs).  Every bound is per element; none is a fraction of a tensor's maximum."""
+the first-order total on these inputs).  Every bound is per element; none is a fraction of a tensor's maximum.
+
+bf16 instances (RowNormParams::io = 1: fp32 in, bf16 out; io = 2: bf16 y / z in, bf16 out; layernorm_bwd with bf16 x, dy, dx;
+dwconv3x3_silu_tma_kernel<__nv_bfloat16>).  Every bf16 operand is widened exactly and all arithmetic is the fp32 kernel's, so the
+inputs are rounded to bf16 first and the reference and its fp32 bound e are computed from those exact values: operand rounding
+never enters the comparison.  A bf16 store rounds the kernel's fp32 value v, |v - ref| <= e, to nearest even, which moves it by at
+most BF16_RN·|v| <= BF16_RN·(|ref| + e) (BF16_RN = 2^-8: 8 significand bits; bf16 has fp32's exponent range):
+  * bf16_store_bound(ref, e) = e + BF16_RN·(|ref| + e), once per store; dgamma / dbeta of the bf16 backward stay fp32 (e alone).
+A constant row of dyadic k/8 (exact in bf16) still normalises to beta exactly, stored as bf16(beta).  hard_rows(bf16=True) builds
+the var_eps rows around a mean of order 2^-6, where bf16's spacing (<= 2^-14) still resolves a sigma of ~3e-3; at a mean of order
+1 (spacing 2^-8) rounding would leave a few distinct values per row."""
 import math
 
 import torch
@@ -54,11 +64,14 @@ E_RSQRT = 2.0 ** -22      # rsqrtf / rsqrt.approx.f32: 2 ulp (CUDA C++ Programmi
 E2 = 2.0 ** -22           # ex2.approx.f32 relative error (PTX ISA)
 E_FDIV = 2.0 ** -22       # __fdividef: 2 ulp
 SAFETY = 1.25
+BF16_RN = 2.0 ** -8       # relative error of a round-to-nearest bf16 store (= oracle/ss2d_ref64.BF16_RN)
 NUM_SMS = 132             # kNumSMs of common.cuh: the grid caps of layernorm_bwd and scale_add
 
 # rowwise.cu's instantiation tables: (lanes per row, float4 per lane)
 ROW_FAST = [(8, 2), (8, 3), (8, 4), (16, 3), (16, 4), (32, 3), (32, 4), (32, 6), (32, 8), (32, 12), (32, 16)]
 ROW_FAST_K = (1, 2, 4)
+# row_norm_fast_k's dispatch per io (0: fp32, 1: fp32 in / bf16 out, 2: bf16 in and out): mode -> the K with a fast instance
+ROW_FAST_IO = {0: {0: ROW_FAST_K, 1: (1,), 2: (1,)}, 1: {0: (1,), 1: (1,)}, 2: {0: ROW_FAST_K}}
 HEAD_FAST = [(8, 2), (8, 3), (8, 4), (16, 3), (16, 4)]
 HEAD_FAST_MAX_NCLS = 24
 HEAD_NCLS = [2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 16, 19, 20, 21, 37, 40, 41]
@@ -74,11 +87,12 @@ def _maxv(nvec, cap=32):
     raise ValueError(f"{4 * nvec} channels: no generic instantiation")
 
 
-def row_plan(D, K=1, mode=0):
-    """(lanes, float4 per lane, fast) of row_norm_launch for D channels, K directions, mode 0 / 1 (gather) / 2 (pixel shuffle)"""
+def row_plan(D, K=1, mode=0, io=0):
+    """(lanes, float4 per lane, fast) of row_norm_launch for D channels, K directions, mode 0 / 1 (gather) / 2 (pixel shuffle) and
+    element types io (ROW_FAST_IO)"""
     nvec = D // 4
     for lpr, v in ROW_FAST:
-        if nvec == lpr * v and (K in ROW_FAST_K if mode == 0 else K == 1):
+        if nvec == lpr * v and K in ROW_FAST_IO[io].get(mode, ()):
             return lpr, v, True
     if mode != 0:
         raise ValueError(f"mode {mode}: D={D} has no fast instantiation")
@@ -128,6 +142,11 @@ def bound_fraction(got, ref, bound):
     err = (got.to(ref.device, torch.float64) - ref).abs()
     frac = torch.where(bound > 0, err / bound.clamp_min(1e-300), torch.where(err > 0, math.inf, 0.0))
     return float(frac.max()) if frac.numel() else 0.0
+
+
+def bf16_store_bound(ref, e):
+    """bound of a bf16 store of a value the fp32 bound e holds to ref (module docstring): e + BF16_RN·(|ref| + e)"""
+    return e + BF16_RN * (_f(ref).abs() + e)
 
 
 def _f(t):
@@ -390,13 +409,14 @@ def layernorm_bwd_bound(x, dy, gamma, eps):
 ROW_FAMILIES = ("ordinary", "large_mean", "var_eps", "constant", "outlier")
 
 
-def hard_rows(seed, rows, D, eps=1e-5, families=ROW_FAMILIES, device="cpu"):
+def hard_rows(seed, rows, D, eps=1e-5, families=ROW_FAMILIES, device="cpu", bf16=False):
     """(rows, D) fp32 on `device` (its own generator, seeded), row i of family families[i % len(families)]:
       ordinary     N(0, 1) scaled by a per-row sigma in [0.5, 2]
       large_mean   mean = ±(30..100)·sigma: the one-pass variance's cancellation
-      var_eps      sigma^2 in [0.5, 2]·eps around a mean of order 1: where eps's placement matters
+      var_eps      sigma^2 in [0.5, 2]·eps around a mean of order 1 (bf16: of order 2^-6): where eps's placement matters
       constant     a dyadic constant k/8 (every partial sum exact): the output must be beta exactly
-      outlier      N(0, 1) with one channel at ±(20..40)"""
+      outlier      N(0, 1) with one channel at ±(20..40)
+    bf16: the same draws, var_eps's mean scaled by 2^-6, returned rounded to bf16 (module docstring)"""
     g = torch.Generator(device=device).manual_seed(seed)
     kw = dict(generator=g, device=device)
     n = torch.randn(rows, D, dtype=torch.float32, **kw)
@@ -416,7 +436,7 @@ def hard_rows(seed, rows, D, eps=1e-5, families=ROW_FAMILIES, device="cpu"):
         elif name == "large_mean":
             out[m] = (n[m] + big[m]) * sig[m]
         elif name == "var_eps":
-            out[m] = mu[m] + n[m] * sig_eps[m]
+            out[m] = mu[m] * (2.0 ** -6 if bf16 else 1.0) + n[m] * sig_eps[m]
         elif name == "constant":
             out[m] = kconst[m].expand(-1, D)
         elif name == "outlier":
@@ -425,7 +445,7 @@ def hard_rows(seed, rows, D, eps=1e-5, families=ROW_FAMILIES, device="cpu"):
             out[m] = o
         else:
             raise ValueError(name)
-    return out
+    return out.to(torch.bfloat16) if bf16 else out
 
 
 def constant_rows(rows, families=ROW_FAMILIES, device="cpu"):

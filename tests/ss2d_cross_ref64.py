@@ -9,20 +9,25 @@ relative to one walk of ss2d_ref64:
   * dA, dDs and d dt_bias are sums over the images of one modality, into rows w·D + d of (2D, N), (2D) and (2, D).
 `mistake` computes the result of a plausible kernel bug instead (for tests that the bound tells it apart): "dC_own" credits dC to
 the image's own row, "wset" sends dA / dDs / d dt_bias to the other weight set's rows, "C_own" reads C from the image's own half.
+`delta` runs the forward and the backward on a given delta' (the bf16 training mode's saved one), through
+tests/ss2d_delta_ref64.ss2d_fwd_ref64 as ss2d_delta_ref64.ss2d_ref64 does for cross4 / seq2; without it the forward is the
+oracle's, bit for bit.
 """
 import math
 
 import torch
 
+import ss2d_delta_ref64 as RD
 from oracle import ss2d_ref64 as R
 
 MISTAKES = ("dC_own", "wset", "C_own")
 
 
-def ss2d_cross_ref64(xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None, mistake=None):
+def ss2d_cross_ref64(xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None, mistake=None, delta=None):
     """The inputs of ss2d_fwd_ref64 for kind "cross" (xc (Bt, L, D), xdbl (Bt, L, 1, Cp), dtw (2, D, R), dtb (2, D), A (2D, N), Ds
     (2D)) and dy (Bt, L, D).  Returns (ref, bound) as ss2d_ref64 does: y / delta / ddelta (1, Bt, L, D), hs (1, Bt, ceil(L/16), D,
-    N), dxc (Bt, L, D), dB / dC (Bt, L, 1, N), dA (2D, N), dDs (2D), ddtb (2, D)."""
+    N), dxc (Bt, L, D), dB / dC (Bt, L, 1, N), dA (2D, N), dDs (2D), ddtb (2, D).
+    delta (1, Bt, L, D): the delta' to run with instead of the softplus (taken as exact; ref["delta"] is then it, bound 0)."""
     assert mistake in (None,) + MISTAKES, mistake
     dev = torch.device(device) if device is not None else xc.device
     Bt, Lseq, D = xc.shape
@@ -136,7 +141,7 @@ def ss2d_cross_ref64(xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None, mistake=N
         ref["ddtb"][ws] = dd_k.sum((0, 1, 2))
         bnd["ddtb"][ws] = R.tile_rss(edd_k.sum(2)) + R._acc(dd_k.sum(2), (dd_k.abs() + edd_k).sum(2), Lseq)
 
-    y, ey = R.ss2d_fwd_ref64("cross", xc, xdbl, dtw, dtb, A, Ds, H, W, device=dev, on_walk=backward)
+    y, ey = RD.ss2d_fwd_ref64("cross", xc, xdbl, dtw, dtb, A, Ds, H, W, device=dev, on_walk=backward, delta=delta)
     bnd["dxc"] += U * dxc_mag
     for key in ("delta", "dxc", "ddelta", "dB", "dC"):
         sl = (slice(None), slice(0, Lseq)) if key in ("dxc", "dB", "dC") else (slice(None), slice(None), slice(0, Lseq))

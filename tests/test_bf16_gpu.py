@@ -7,9 +7,6 @@ rounding does not enter.  u = 2^-24; mag = (|A|·|W|^T)_ij or (|x| ⊛ |w|); K =
   GEMM     bf16 x bf16 products are exact in fp32; the fp32 accumulation adds at most K·2^-23·mag (one truncating addition per
            product of a partial sum <= mag), + 2^-20·mag of slack, and the epilogue rounds twice: 2u·(mag + |bias| + |res·rscale|).
            A bf16 output is then rounded once more: + 2^-8·|ref| (round to nearest even, 8 significand bits).
-  Row-wise LayerNorm statistics and the normalisation in fp32 (relative error ~ a few u), SiLU through ex2.approx (~2^-22
-           relative): + 1e-5·max|ref| absolute, then the one bf16 rounding: + 2^-8·|ref|.
-  dwconv   9 fp32 FMAs: 9·2^-23·mag, SiLU as above, then + 2^-8·|ref|.
   Scan     the bf16 instance runs the same fp32 recurrence on the same (bf16-exact) xc values as the fp32 kernel; y is rounded once
            on its store, so |y_bf16 - y_fp32| <= 2^-8·|y_fp32| (+ 1e-6 for the sink of ties at tiny values).
 Outputs sit inside NaN-filled buffers whose guard elements must stay bit-identical.
@@ -159,108 +156,31 @@ def test_bf16_gemm_epilogues_strided_multiwave(extras, out_dtype, monkeypatch):
               tag=f"bf16gemm-epi/{extras}")
 
 
-# ---------------------------------------------------------------- row-wise kernels
-def _ln64(x, w, b, eps):
-    x = x.double()
-    m = x.mean(-1, keepdim=True)
-    v = ((x - m) ** 2).mean(-1, keepdim=True)
-    return (x - m) / torch.sqrt(v + eps) * w.double() + b.double()
-
-
-def _rowwise_bound(ref):
-    return BU * ref.abs() + 1e-5 * float(ref.abs().max()) + 1e-7
-
-
-@pytest.mark.parametrize("C", [96, 192, 384, 768, 100])
-def test_bf16_layernorm(C):
-    from sigma_b200 import fused
-    rows = 74 * 40 + 3
-    x = P.randn(S, f"ln/{C}/x", (rows, C), 2.0, 0.5).cuda()
-    ln = torch.nn.LayerNorm(C).cuda()
-    with torch.no_grad():
-        ln.weight.copy_(P.randn(S, f"ln/{C}/w", (C,), 0.5, 1.0))
-        ln.bias.copy_(P.randn(S, f"ln/{C}/b", (C,), 0.2))
-    buf = _nan((rows + 2, C), BF)
-    got = buf[:rows]
-    from sigma_b200 import _lib
-    _lib.check(_lib.lib().sigma_layernorm_fwd_bf16(_p(x), _p(ln.weight), _p(ln.bias), _p(got), rows, C, float(ln.eps), _stream()), "ln")
-    torch.cuda.synchronize()
-    _guard_ok(buf[rows:], "rows past the end")
-    ref = _ln64(x, ln.weight.detach(), ln.bias.detach(), ln.eps)
-    _ratio(f"ln C={C}", got, ref, _rowwise_bound(ref))
-    assert torch.equal(fused.layernorm(x, ln, BF), got)
-
-
-@pytest.mark.parametrize("H,W,C", [(120, 160, 96), (45, 61, 192), (15, 21, 384)])
-def test_bf16_patch_merge_norm(H, W, C):
-    from sigma_b200 import _lib
-    B = 3
-    x = P.randn(S, f"pm/{H}/x", (B, H, W, C)).cuda()
-    w = P.randn(S, f"pm/{H}/w", (4 * C,), 0.5, 1.0).cuda()
-    b = P.randn(S, f"pm/{H}/b", (4 * C,), 0.2).cuda()
-    H2, W2 = (H + 1) // 2, (W + 1) // 2
-    rows = B * H2 * W2
-    buf = _nan((rows + 2, 4 * C), BF)
-    _lib.check(_lib.lib().sigma_patch_merge_norm_fwd_bf16(_p(x), _p(w), _p(b), _p(buf), B, H, W, C, 1e-5, _stream()), "pm")
-    torch.cuda.synchronize()
-    _guard_ok(buf[rows:], "rows past the end")
-    xp = torch.nn.functional.pad(x, (0, 0, 0, W % 2, 0, H % 2))
-    cat = torch.cat([xp[:, 0::2, 0::2], xp[:, 1::2, 0::2], xp[:, 0::2, 1::2], xp[:, 1::2, 1::2]], -1).reshape(rows, 4 * C)
-    ref = _ln64(cat, w, b, 1e-5)
-    _ratio(f"patch-merge {H}x{W}", buf[:rows], ref, _rowwise_bound(ref))
-
-
-@pytest.mark.parametrize("K", [1, 2, 4])
-@pytest.mark.parametrize("with_z,with_gate", [(False, False), (True, False), (False, True), (True, True)])
-def test_bf16_merge_norm_gate(K, with_z, with_gate):
-    from sigma_b200 import _lib
-    D, Bn, L = 384, 3, 1200
-    rows = Bn * L
-    tag = f"mng/{K}/{with_z}/{with_gate}"
-    y = P.randn(S, tag + "/y", (K, rows, D)).to(BF).cuda()
-    zbuf = P.randn(S, tag + "/z", (rows, 2 * D)).to(BF).cuda()         # z = the second half of [x | z] rows
-    gate = P.randn(S, tag + "/g", (Bn, D), 0.5, 1.0).cuda() if with_gate else None
-    g = P.randn(S, tag + "/w", (D,), 0.5, 1.0).cuda()
-    bb = P.randn(S, tag + "/bb", (D,), 0.2).cuda()
-    obuf = _nan((rows + 2, D + 8), BF)
-    zp = ctypes.c_void_p(zbuf.data_ptr() + 2 * D) if with_z else None
-    _lib.check(_lib.lib().sigma_merge_norm_gate_fwd_bf16(_p(y), K, rows * D, L * D, _p(g), _p(bb), zp, 2 * D if with_z else 0,
-                                                         _p(gate), _p(obuf), L * (D + 8), D + 8, rows, L, D, 1e-5, _stream()), "mng")
-    torch.cuda.synchronize()
-    _guard_ok(obuf[:, D:], "columns past D")
-    _guard_ok(obuf[rows:], "rows past the end")
-    ref = _ln64(y.double().sum(0), g, bb, 1e-5)
-    if with_z:
-        z = zbuf[:, D:].double()
-        ref = ref * z * torch.sigmoid(z)
-    if with_gate:
-        ref = ref * gate.double().repeat_interleave(L, 0)
-    _ratio(tag, obuf[:rows, :D], ref, _rowwise_bound(ref))
-
+# The bf16 row-wise kernels (LayerNorm, patch-merge, merge + norm + gate) are compared with fp64 in tests/test_rowwise_fp64_gpu.py
+# (io axis); the bf16 depthwise conv at Sigma's widths and production layouts in tests/test_gemm_waves_gpu.py (test_dwconv_silu_bf16).
 
 # ---------------------------------------------------------------- depthwise conv
 def test_bf16_dwconv_ring_wraps():
-    """Every CTA walks >= 9 tiles (the 4-slot ring wraps twice), ragged H / W, x a strided view ([x | z] rows)."""
+    """D = 64 (two 32-channel blocks): every CTA walks >= 9 tiles (the 4-slot ring wraps twice), ragged H / W, x a strided view
+    ([x | z] rows).  Element by element against fp64 on the bf16 input's exact values, inside the fp32 kernel's per-element bound
+    (test_gemm_waves_gpu._dwconv_ref) plus one bf16 store (rowwise_ref64.bf16_store_bound)."""
     from sigma_b200 import _lib
+    from oracle import rowwise_ref64 as RR
+    from test_gemm_waves_gpu import _dwconv_check, _dwconv_ref
     Bn, H, W, D = 7, 121, 161, 64
     tiles = Bn * -(-W // 16) * -(-H // 8)
     assert tiles >= 9 * (132 * 2 // (D // 32))
     xz = P.randn(S, "dw/x", (Bn, H, W, 2 * D)).to(BF).cuda()
-    conv = torch.nn.Conv2d(D, D, 3, padding=1, groups=D).cuda()
-    with torch.no_grad():
-        conv.weight.copy_(P.randn(S, "dw/w", (D, 1, 3, 3), 0.3))
-        conv.bias.copy_(P.randn(S, "dw/b", (D,), 0.1))
+    w = P.randn(S, "dw/w", (D, 1, 3, 3), 0.3).cuda()
+    b = P.randn(S, "dw/b", (D,), 0.1).cuda()
     buf = _nan((Bn * H * W + 5, D), BF)
-    _lib.check(_lib.lib().sigma_dwconv3x3_silu_fwd_bf16(_p(xz), 2 * D, H * W * 2 * D, _p(conv.weight), _p(conv.bias), _p(buf),
-                                                        H * W * D, Bn, H, W, D, _stream()), "dw")
+    _lib.check(_lib.lib().sigma_dwconv3x3_silu_fwd_bf16(_p(xz), 2 * D, H * W * 2 * D, _p(w), _p(b), _p(buf), H * W * D, Bn, H, W, D,
+                                                        _stream()), "dw")
     torch.cuda.synchronize()
     _guard_ok(buf[Bn * H * W:], "past the end")
-    x64 = xz[..., :D].permute(0, 3, 1, 2).double()
-    pre = torch.nn.functional.conv2d(x64, conv.weight.double(), conv.bias.double(), padding=1, groups=D)
-    mag = torch.nn.functional.conv2d(x64.abs(), conv.weight.double().abs(), padding=1, groups=D) + conv.bias.double().abs().view(1, D, 1, 1)
-    ref = (pre * torch.sigmoid(pre)).permute(0, 2, 3, 1).reshape(-1, D)
-    mag = mag.permute(0, 2, 3, 1).reshape(-1, D)
-    _ratio("dwconv bf16", buf[:Bn * H * W], ref, BU * ref.abs() + 9 * 2.0 ** -23 * mag + 2.0 ** -21 * mag + 1e-6)
+    ref, e = _dwconv_ref(xz[..., :D], w, b)
+    worst = _dwconv_check("dwconv bf16", buf[:Bn * H * W].view(Bn, H, W, D), ref, RR.bf16_store_bound(ref, e))
+    record("bf16_dwconv", case="ring", max_err_over_bound=worst)
 
 
 # ---------------------------------------------------------------- scan

@@ -1,5 +1,6 @@
 """GPU: the wgmma GEMM (sigma_linear_tf32 / sigma_linear_tf32x3 through fused.linear), its implicit-GEMM 3x3 convolution
-(sigma_conv3x3_tf32) and the depthwise conv (sigma_dwconv3x3_silu_fwd) in the regime the model runs them in: persistent CTAs
+(sigma_conv3x3_tf32) and the depthwise conv (sigma_dwconv3x3_silu_fwd, and its bf16 instance at Sigma's widths in its three
+production stride layouts) in the regime the model runs them in: persistent CTAs
 that walk several tiles each — so the producer runs ahead across tile boundaries, the mbarrier ring carries its phase from tile to
 tile and the accumulators restart per tile — at every tile width (SIGMA_GEMM_BN), with ragged M / N / K / channel counts and
 every epilogue, against fp64 ELEMENT BY ELEMENT, with the memory around each output filled with NaN and checked untouched.
@@ -351,14 +352,72 @@ def test_dwconv_silu_ring_wraps(B, H, W, D):
     _assert_nan_untouched(img[:, H * W * D:], f"{tag}: gaps between images")
     _assert_nan_untouched(buf[B * ybs:], f"{tag}: after the last image")
     y = img[:, :H * W * D].reshape(B, H, W, D)
-    xn = xz[..., :D].permute(0, 3, 1, 2).double()
+    ref, bound = _dwconv_ref(xz[..., :D], w, b)
+    record("dwconv_ring", case=tag, max_err_over_bound=_dwconv_check(tag, y, ref, bound))
+
+
+def _dwconv_ref(x, w, b):
+    """fp64 conv + bias + SiLU of x (B, H, W, D) and the per-element bound of the fp32 kernel: 9 FMAs + bias (<= 10u·mag), then
+    SiLU (|SiLU'| <= 1.1, ex2.approx / fast division within a few ulp)"""
+    D = x.shape[-1]
+    xn = x.permute(0, 3, 1, 2).double()
     pre = torch.nn.functional.conv2d(xn, w.double(), b.double(), padding=1, groups=D).permute(0, 2, 3, 1)
     mag = torch.nn.functional.conv2d(xn.abs(), w.double().abs(), b.double().abs(), padding=1, groups=D).permute(0, 2, 3, 1)
     ref = torch.nn.functional.silu(pre)
-    assert bool(torch.isfinite(y).all())
+    return ref, 1.1 * 10 * U * mag + 2.0 ** -19 * ref.abs() + 1e-12
+
+
+def _dwconv_check(tag, y, ref, bound):
+    assert bool(torch.isfinite(y).all()), f"{tag}: non-finite output (not written?)"
     err = (y.double() - ref).abs()
-    bound = 1.1 * 10 * U * mag + 2.0 ** -19 * ref.abs() + 1e-12
     bad = err > bound
     assert not bool(bad.any()), (f"{tag}: {int(bad.sum())}/{bad.numel()} elements out of bound; max err {float(err.max()):.3e}, "
                                  f"worst err/bound {float((err / bound).max()):.2f}")
-    record("dwconv_ring", case=tag, max_err_over_bound=float((err / bound).max()))
+    return float((err / bound).max())
+
+
+# (D, H, W): Sigma's d_inner at its 480 x 640 stages, Sigma-base's widest (2048 at 720 x 960), and D = 136: a partial 32-channel block
+DW_BF16 = [(192, 120, 160), (384, 60, 80), (768, 30, 40), (1536, 15, 20), (2048, 23, 30), (136, 57, 75)]
+NAN16 = 0x7FC0
+
+
+@pytest.mark.parametrize("layout", ["ss2d", "cromb", "conmb"])
+@pytest.mark.parametrize("D,H,W", DW_BF16)
+def test_dwconv_silu_bf16(D, H, W, layout):
+    """sigma_dwconv3x3_silu_fwd_bf16 (dwconv3x3_silu_tma_kernel<__nv_bfloat16>) with the strides of its production calls:
+      ss2d   x the x half of in_proj's [x | z] rows (row stride 2D), out (B, L, D)                      (fused.ss2d)
+      cromb  x (2, B·L, D) modality-major, one call over the 2B images, out (2B, L, D)                  (fused.cromb_ss2d)
+      conmb  x (B·L, D), out the second half of seq (B, 2L, D): offset L·D, image stride 2L·D           (fused.conmb_ss2d)
+    with enough images that every CTA walks >= 9 tiles.  x is bf16 and the reference runs on its exact values; the bound is the fp32
+    one plus one bf16 store (rowwise_ref64.bf16_store_bound).  The first half of every conmb image (NaN gaps between the images)
+    and the guards around the buffer stay NaN."""
+    from oracle import rowwise_ref64 as RR
+    L = _lib()
+    step = 2 if layout == "cromb" else 1
+    B = step
+    while True:
+        _, ny, ntiles = _dwconv_grid(B, H, W, D)
+        if ntiles // ny >= 9:
+            break
+        B += step
+    tag = f"dw16/{layout}/{B}/{H}/{W}/{D}"
+    dev = "cuda"
+    HW = H * W
+    xin = P.randn(S, tag + "/x", (B, H, W, 2 * D if layout == "ss2d" else D)).to(dev).to(torch.bfloat16)
+    w = P.randn(S, tag + "/w", (D, 1, 3, 3), 0.4).to(dev)
+    b = P.randn(S, tag + "/b", (D,), 0.2).to(dev)
+    xrs = 2 * D if layout == "ss2d" else D
+    ybs, yoff = (2 * HW * D, HW * D) if layout == "conmb" else (HW * D, 0)
+    g = 64
+    buf = torch.full((B * ybs + 2 * g,), float("nan"), dtype=torch.bfloat16, device=dev)
+    yp = ctypes.c_void_p(buf.data_ptr() + 2 * (g + yoff))
+    L.check(L.lib().sigma_dwconv3x3_silu_fwd_bf16(_p(xin), xrs, HW * xrs, _p(w), _p(b), yp, ybs, B, H, W, D, _stream()), tag)
+    torch.cuda.synchronize()
+    bits = buf.view(torch.int16)
+    gaps = [bits[:g], bits[g + B * ybs:]] + ([bits[g:g + B * ybs].view(B, ybs)[:, :HW * D]] if layout == "conmb" else [])
+    bad = sum(int((t != NAN16).sum()) for t in gaps)
+    assert bad == 0, f"{tag}: {bad} elements written outside the output"
+    y = buf[g:g + B * ybs].view(B, ybs)[:, yoff:yoff + HW * D].reshape(B, H, W, D)
+    ref, e = _dwconv_ref(xin[..., :D], w, b)
+    worst = _dwconv_check(tag, y, ref, RR.bf16_store_bound(ref, e))
+    record("dwconv_bf16", case=tag, tiles_per_cta=ntiles // ny, max_err_over_bound=worst)

@@ -13,10 +13,16 @@ per-element error bounds, at every instantiation and at Sigma's shapes.
 * pool_avgmax (forced slice counts with empty trailing slices, idle threads), scale_add past 3 grid-stride passes, layernorm_bwd
   past its grid cap (the deterministic build bitwise repeatable);
 * the benchmark's batch of 74: every image of the LayerNorm and of the head bit-identical to a batch-1 run of it.
+* The bf16 instances (rowwise_ref64's docstring: inputs rounded to bf16 first, the fp32 bound plus one bf16 store) on the same
+  cases through an io axis: io 1 (fp32 in, bf16 out: sigma_layernorm_fwd_bf16 at every width and the benchmark's batch, the
+  patch-merge gather at every width it takes, and fused.layernorm's routing to both), io 2 (bf16 in and out:
+  sigma_layernorm_fwd_bf16io at every width, merge + norm + gate at K = 1..8 and the three production calls); hard rows in their
+  bf16 form; constant rows give bf16(beta) exactly.  sigma_layernorm_bwd_bf16 at every instantiation past its grid cap.
 Outputs sit in NaN-filled buffers (helpers.guarded): every interior element must be written, every guard stay untouched.  Inputs
 are generated on the GPU from fixed seeds; the references run there in torch float64.  Worst bound fractions go to
 helpers.record."""
 import ctypes
+import types
 
 import pytest
 import torch
@@ -32,8 +38,14 @@ SIGMA_EUNSUPPORTED = -4
 LN_FAST_D = [64, 96, 128, 192, 256, 384, 512, 768, 1024, 1536, 2048]
 LN_GENERIC_D = [32, 200, 400, 1000, 2000, 4000, 4096]
 MERGE_K = [1, 2, 3, 4, 5, 6, 7, 8]
-MERGE_D = [96, 192, 384, 768, 1536, 256, 512, 1024, 2048]
-PATCH_MERGE_C = [96, 192, 384, 128, 256, 512]
+MERGE_D = [96, 192, 384, 768, 1536, 256, 512, 1024, 2048, 64, 128]
+PATCH_MERGE_C = [96, 192, 384, 128, 256, 512, 16, 24, 32, 48, 64]
+# element types (RowNormParams::io) each test runs: 0 fp32, 1 fp32 in / bf16 out, 2 bf16 in and out
+LN_IO = [0, 1, 2]
+MERGE_IO = [0, 2]
+PATCH_MERGE_IO = [0, 1]
+BWD_BF16_D = [32, 64, 96, 128, 192, 256, 384, 512, 768, 1024, 1536]
+BF = torch.bfloat16
 PATCH_MERGE_UNSUPPORTED_C = 40
 SHUFFLE_D = [384, 512] + [d for d in LN_FAST_D if d not in (384, 512)]
 UPSAMPLE_C = [48, 192, 384, 1024]
@@ -77,11 +89,39 @@ def _check(tag, got, ref, bnd, worst, key):
     assert frac <= 1.0, f"{tag}: {frac:.3f} of the per-element bound"
 
 
-def _layernorm(x, g, b):
+def _with_io(cases, ios):
+    """pytest parameters (*case, io): io 0 keeps the fp32 test's ids, a bf16 io is appended to them as -io1 / -io2"""
+    out = []
+    for io in ios:
+        for c in cases:
+            c = c if isinstance(c, tuple) else (c,)
+            ident = "-".join(str(v) for v in c)
+            out.append(pytest.param(*c, io, id=ident if io == 0 else f"{ident}-io{io}"))
+    return out
+
+
+def _rows(seed, rows, D, io, **kw):
+    """hard_rows as the instance reads them: bf16 (their bf16 form) when y is bf16 (io 2)"""
+    return R.hard_rows(seed, rows, D, device="cuda", bf16=io == 2, **kw)
+
+
+def _bound(io, ref, e):
+    """the fp32 bound e, plus the bf16 store of a bf16 output"""
+    return R.bf16_store_bound(ref, e) if io else e
+
+
+def _out_dtype(io):
+    return BF if io else torch.float32
+
+
+_LN_FN = {0: "sigma_layernorm_fwd", 1: "sigma_layernorm_fwd_bf16", 2: "sigma_layernorm_fwd_bf16io"}
+
+
+def _layernorm(x, g, b, io=0):
     rows, D = x.shape
-    buf, y = guarded((rows, D))
-    _call("sigma_layernorm_fwd", ptr(x), ptr(g), ptr(b), ptr(y), rows, D, EPS, stream())
-    guard_ok(buf, f"layernorm {rows}x{D}")
+    buf, y = guarded((rows, D), _out_dtype(io))
+    _call(_LN_FN[io], ptr(x), ptr(g), ptr(b), ptr(y), rows, D, EPS, stream())
+    guard_ok(buf, f"layernorm io={io} {rows}x{D}")
     return y
 
 
@@ -92,132 +132,140 @@ def _ln_counts(D):
     return [1, 8 * rpw * 5 + rpw - 1 if rpw > 1 else 8 * 5 + 3, WAVE_WARPS * rpw + 5]
 
 
-@pytest.mark.parametrize("D", LN_FAST_D + LN_GENERIC_D)
-def test_layernorm(D):
-    plan = R.row_plan(D)
+@pytest.mark.parametrize("D,io", _with_io(LN_FAST_D + LN_GENERIC_D, LN_IO))
+def test_layernorm(D, io):
+    from sigma_b200 import fused
+    plan = R.row_plan(D, io=io)
     g, b = _affine(S + D, D)
     worst = {}
     for rows in _ln_counts(D):
-        x = R.hard_rows(S * D + rows, rows, D, device="cuda")
-        y = _layernorm(x, g, b)
-        _check(f"D={D} rows={rows}", y, R.layer_norm_ref64(x, g, b, EPS), R.layer_norm_bound(x, g, b, EPS, plan), worst, "y")
+        x = _rows(S * D + rows, rows, D, io)
+        y = _layernorm(x, g, b, io)
+        ref = R.layer_norm_ref64(x, g, b, EPS)
+        _check(f"D={D} io={io} rows={rows}", y, ref, _bound(io, ref, R.layer_norm_bound(x, g, b, EPS, plan)), worst, "y")
         const = R.constant_rows(rows, device="cuda")
-        assert torch.equal(y[const], b.expand(int(const.sum()), D)), f"D={D}: constant rows must give beta exactly"
-    record("rowwise_fp64/layernorm", D=D, plan=list(plan), rows=_ln_counts(D), bound_used=worst["y"])
+        assert torch.equal(y[const], b.to(y.dtype).expand(int(const.sum()), D)), f"D={D} io={io}: constant rows must give beta exactly"
+        if io < 2:      # fused.layernorm routes an fp32 row block to the instance of the output dtype: the same bits
+            assert torch.equal(fused.layernorm(x, types.SimpleNamespace(weight=g, bias=b, eps=EPS), y.dtype), y), f"D={D} io={io}"
+    record("rowwise_fp64/layernorm", D=D, io=io, plan=list(plan), rows=_ln_counts(D), bound_used=worst["y"])
 
 
 # ---------------------------------------------------------------- merge + norm + gate
-def _merge_inputs(seed, K, rows, D):
-    y = torch.stack([R.hard_rows(seed + k, rows, D, device="cuda") for k in range(K)])
+def _merge_inputs(seed, K, rows, D, io=0):
+    y = torch.stack([_rows(seed + k, rows, D, io) for k in range(K)])
     xz = _randn(seed + 100, (rows, 2 * D), 2.0)
-    return y, xz
+    return y, xz.to(BF) if io == 2 else xz
 
 
-@pytest.mark.parametrize("D", MERGE_D)
-@pytest.mark.parametrize("K", MERGE_K)
-def test_merge_norm_gate(K, D):
+def _merge(io, *args):
+    _call("sigma_merge_norm_gate_fwd_bf16" if io else "sigma_merge_norm_gate_fwd", *args)
+
+
+@pytest.mark.parametrize("K,D,io", _with_io([(K, D) for K in MERGE_K for D in MERGE_D], MERGE_IO))
+def test_merge_norm_gate(K, D, io):
     """y (K, B·L, D) in direction-major slabs, z the second half of [x | z] rows, out rows padded to D + 8 per row"""
     Bn, L = 3, 407
     rows, ld = Bn * L, D + 8
-    y, xz = _merge_inputs(S + 10 * K + D, K, rows, D)
+    y, xz = _merge_inputs(S + 10 * K + D, K, rows, D, io)
     gate = _randn(S + K + D, (Bn, D), 0.5, 1.0)
     g, b = _affine(S + 2 * D + K, D)
-    plan = R.row_plan(D, K)
+    plan = R.row_plan(D, K, io=io)
     worst = {}
     for with_z in (False, True):
         for with_gate in (False, True):
-            tag = f"K={K} D={D} z={with_z} gate={with_gate}"
-            buf, o = guarded((rows, ld))
+            tag = f"K={K} D={D} io={io} z={with_z} gate={with_gate}"
+            buf, o = guarded((rows, ld), _out_dtype(io))
             z = xz[:, D:] if with_z else None
             gt = gate if with_gate else None
-            _call("sigma_merge_norm_gate_fwd", ptr(y), K, rows * D, L * D, ptr(g), ptr(b), _off(xz, D) if with_z else None,
-                  2 * D if with_z else 0, ptr(gt), ptr(o), L * ld, ld, rows, L, D, EPS, stream())
+            _merge(io, ptr(y), K, rows * D, L * D, ptr(g), ptr(b), _off(xz, D) if with_z else None, 2 * D if with_z else 0, ptr(gt),
+                   ptr(o), L * ld, ld, rows, L, D, EPS, stream())
             guard_ok(buf, tag)
             assert bool(o[:, D:].isnan().all()), f"{tag}: row padding written"
-            _check(tag, o[:, :D], R.merge_norm_ref64(y, g, b, EPS, z, gt, L),
-                   R.merge_norm_bound(y, g, b, EPS, plan, z, gt, L), worst, "y")
-    record("rowwise_fp64/merge_norm_gate", K=K, D=D, plan=list(plan), bound_used=worst["y"])
+            ref = R.merge_norm_ref64(y, g, b, EPS, z, gt, L)
+            _check(tag, o[:, :D], ref, _bound(io, ref, R.merge_norm_bound(y, g, b, EPS, plan, z, gt, L)), worst, "y")
+    record("rowwise_fp64/merge_norm_gate", K=K, D=D, io=io, plan=list(plan), bound_used=worst["y"])
 
 
-@pytest.mark.parametrize("B,H,W,D", [(2, 30, 40, 192), (3, 15, 20, 384), (1, 15, 20, 1536)])
-def test_merge_ss2d_call(B, H, W, D):
+@pytest.mark.parametrize("B,H,W,D,io", _with_io([(2, 30, 40, 192), (3, 15, 20, 384), (1, 15, 20, 1536)], MERGE_IO))
+def test_merge_ss2d_call(B, H, W, D, io):
     """fused.ss2d: K = 4 slabs of B·L rows, z from [x | z] rows, one dense output"""
     L = H * W
     rows = B * L
-    y, xz = _merge_inputs(S + D, 4, rows, D)
+    y, xz = _merge_inputs(S + D, 4, rows, D, io)
     g, b = _affine(S + D + 1, D)
-    buf, o = guarded((rows, D))
-    _call("sigma_merge_norm_gate_fwd", ptr(y), 4, B * L * D, 0, ptr(g), ptr(b), _off(xz, D), 2 * D, None, ptr(o), 0, D, rows,
-          rows, D, EPS, stream())
+    buf, o = guarded((rows, D), _out_dtype(io))
+    _merge(io, ptr(y), 4, B * L * D, 0, ptr(g), ptr(b), _off(xz, D), 2 * D, None, ptr(o), 0, D, rows, rows, D, EPS, stream())
     guard_ok(buf, "ss2d merge")
     worst = {}
-    _check("ss2d merge", o, R.merge_norm_ref64(y, g, b, EPS, xz[:, D:]),
-           R.merge_norm_bound(y, g, b, EPS, R.row_plan(D, 4), xz[:, D:]), worst, "y")
-    record("rowwise_fp64/merge_ss2d", B=B, H=H, W=W, D=D, bound_used=worst["y"])
+    ref = R.merge_norm_ref64(y, g, b, EPS, xz[:, D:])
+    _check(f"ss2d merge io={io}", o, ref, _bound(io, ref, R.merge_norm_bound(y, g, b, EPS, R.row_plan(D, 4, io=io), xz[:, D:])),
+           worst, "y")
+    record("rowwise_fp64/merge_ss2d", B=B, H=H, W=W, D=D, io=io, bound_used=worst["y"])
 
 
-@pytest.mark.parametrize("B,H,W,D", [(2, 30, 40, 192), (1, 15, 20, 768)])
-def test_merge_cromb_calls(B, H, W, D):
+@pytest.mark.parametrize("B,H,W,D,io", _with_io([(2, 30, 40, 192), (1, 15, 20, 768)], MERGE_IO))
+def test_merge_cromb_calls(B, H, W, D, io):
     """fused.cromb_ss2d: y (1, 2B, L, D) modality-major; two K = 1 launches, the second at offsets B·L·D of y and out"""
     L = H * W
     rows = B * L
-    y = R.hard_rows(S + D + 2, 2 * rows, D, device="cuda")
+    y = _rows(S + D + 2, 2 * rows, D, io)
     (g1, b1), (g2, b2) = _affine(S + 3, D), _affine(S + 4, D)
-    buf, o = guarded((2, rows, D))
-    _call("sigma_merge_norm_gate_fwd", ptr(y), 1, 0, 0, ptr(g1), ptr(b1), None, 0, None, ptr(o), 0, D, rows, rows, D, EPS, stream())
+    buf, o = guarded((2, rows, D), _out_dtype(io))
+    _merge(io, ptr(y), 1, 0, 0, ptr(g1), ptr(b1), None, 0, None, ptr(o), 0, D, rows, rows, D, EPS, stream())
     assert bool(o[1].isnan().all()), "cromb: the first launch wrote the second modality's half"
-    _call("sigma_merge_norm_gate_fwd", _off(y, rows * D), 1, 0, 0, ptr(g2), ptr(b2), None, 0, None, _off(o, rows * D), 0, D, rows,
-          rows, D, EPS, stream())
+    _merge(io, _off(y, rows * D), 1, 0, 0, ptr(g2), ptr(b2), None, 0, None, _off(o, rows * D), 0, D, rows, rows, D, EPS, stream())
     guard_ok(buf, "cromb merge")
-    plan, worst = R.row_plan(D), {}
+    plan, worst = R.row_plan(D, io=io), {}
     for m, (g, b) in enumerate(((g1, b1), (g2, b2))):
         ym = y[m * rows:(m + 1) * rows]
-        _check(f"cromb modality {m}", o[m], R.layer_norm_ref64(ym, g, b, EPS), R.layer_norm_bound(ym, g, b, EPS, plan), worst, "y")
-    record("rowwise_fp64/merge_cromb", B=B, H=H, W=W, D=D, bound_used=worst["y"])
+        ref = R.layer_norm_ref64(ym, g, b, EPS)
+        _check(f"cromb io={io} modality {m}", o[m], ref, _bound(io, ref, R.layer_norm_bound(ym, g, b, EPS, plan)), worst, "y")
+    record("rowwise_fp64/merge_cromb", B=B, H=H, W=W, D=D, io=io, bound_used=worst["y"])
 
 
-@pytest.mark.parametrize("B,H,W,D", [(2, 30, 40, 192), (3, 15, 20, 384), (1, 15, 20, 768)])
-def test_merge_conmb_calls(B, H, W, D):
+@pytest.mark.parametrize("B,H,W,D,io", _with_io([(2, 30, 40, 192), (3, 15, 20, 384), (1, 15, 20, 768)], MERGE_IO))
+def test_merge_conmb_calls(B, H, W, D, io):
     """fused.conmb_ss2d: y (2, B, 2L, D) = two directions over [rgb ‖ x]; out rows [rgb half | x half] of 2D; K = 2,
     rows_per_batch = L, in_batch_stride 2·L·D, out_row_stride 2D, the second launch at y offset L·D and out offset D, gates
     crosswise per image"""
     L = H * W
     rows = B * L
-    y = torch.stack([R.hard_rows(S + D + k, B * 2 * L, D, device="cuda") for k in range(2)])       # (2, B·2L, D)
+    y = torch.stack([_rows(S + D + k, B * 2 * L, D, io) for k in range(2)])                        # (2, B·2L, D)
     g_e, g_r = _randn(S + 5, (B, D), 0.5, 1.0), _randn(S + 6, (B, D), 0.5, 1.0)
     (w1, b1), (w2, b2) = _affine(S + 7, D), _affine(S + 8, D)
     ks = B * 2 * L * D
-    buf, o = guarded((rows, 2 * D))
-    _call("sigma_merge_norm_gate_fwd", ptr(y), 2, ks, 2 * L * D, ptr(w1), ptr(b1), None, 0, ptr(g_e), ptr(o), L * 2 * D, 2 * D, rows,
-          L, D, EPS, stream())
+    buf, o = guarded((rows, 2 * D), _out_dtype(io))
+    _merge(io, ptr(y), 2, ks, 2 * L * D, ptr(w1), ptr(b1), None, 0, ptr(g_e), ptr(o), L * 2 * D, 2 * D, rows, L, D, EPS, stream())
     assert bool(o[:, D:].isnan().all()), "conmb: the first launch wrote the second launch's half"
-    _call("sigma_merge_norm_gate_fwd", _off(y, L * D), 2, ks, 2 * L * D, ptr(w2), ptr(b2), None, 0, ptr(g_r), _off(o, D), L * 2 * D,
-          2 * D, rows, L, D, EPS, stream())
+    _merge(io, _off(y, L * D), 2, ks, 2 * L * D, ptr(w2), ptr(b2), None, 0, ptr(g_r), _off(o, D), L * 2 * D, 2 * D, rows, L, D, EPS,
+           stream())
     guard_ok(buf, "conmb merge")
     yv = y.view(2, B, 2, L, D)
-    plan, worst = R.row_plan(D, 2), {}
+    plan, worst = R.row_plan(D, 2, io=io), {}
     for half, (w, b, gate) in enumerate(((w1, b1, g_e), (w2, b2, g_r))):
         yh = yv[:, :, half].reshape(2, rows, D)
-        _check(f"conmb half {half}", o[:, half * D:(half + 1) * D], R.merge_norm_ref64(yh, w, b, EPS, None, gate, L),
-               R.merge_norm_bound(yh, w, b, EPS, plan, None, gate, L), worst, "y")
-    record("rowwise_fp64/merge_conmb", B=B, H=H, W=W, D=D, bound_used=worst["y"])
+        ref = R.merge_norm_ref64(yh, w, b, EPS, None, gate, L)
+        _check(f"conmb io={io} half {half}", o[:, half * D:(half + 1) * D], ref,
+               _bound(io, ref, R.merge_norm_bound(yh, w, b, EPS, plan, None, gate, L)), worst, "y")
+    record("rowwise_fp64/merge_conmb", B=B, H=H, W=W, D=D, io=io, bound_used=worst["y"])
 
 
 # ---------------------------------------------------------------- patch merge, pixel shuffle
-@pytest.mark.parametrize("C", PATCH_MERGE_C)
-def test_patch_merge_norm(C):
+@pytest.mark.parametrize("C,io", _with_io(PATCH_MERGE_C, PATCH_MERGE_IO))
+def test_patch_merge_norm(C, io):
     g, b = _affine(S + C, 4 * C)
-    plan, worst = R.row_plan(4 * C, mode=1), {}
+    plan, worst = R.row_plan(4 * C, mode=1, io=io), {}
+    fn = "sigma_patch_merge_norm_fwd_bf16" if io else "sigma_patch_merge_norm_fwd"
     for B, H, W in ((1, 45, 60), (3, 16, 22), (3, 15, 21), (1, 1, 1)):
         x = R.hard_rows(S + C + H, B * H * W, C, device="cuda").view(B, H, W, C)
         rows = B * ((H + 1) // 2) * ((W + 1) // 2)
-        buf, y = guarded((rows, 4 * C))
-        _call("sigma_patch_merge_norm_fwd", ptr(x), ptr(g), ptr(b), ptr(y), B, H, W, C, EPS, stream())
-        guard_ok(buf, f"patch merge {B}x{H}x{W}x{C}")
+        buf, y = guarded((rows, 4 * C), _out_dtype(io))
+        _call(fn, ptr(x), ptr(g), ptr(b), ptr(y), B, H, W, C, EPS, stream())
+        guard_ok(buf, f"patch merge io={io} {B}x{H}x{W}x{C}")
         cat = R.patch_merge_gather64(x)
-        _check(f"patch merge {B}x{H}x{W}x{C}", y, R.layer_norm_ref64(cat, g, b, EPS), R.layer_norm_bound(cat, g, b, EPS, plan),
-               worst, "y")
-    record("rowwise_fp64/patch_merge", C=C, bound_used=worst["y"])
+        ref = R.layer_norm_ref64(cat, g, b, EPS)
+        _check(f"patch merge io={io} {B}x{H}x{W}x{C}", y, ref, _bound(io, ref, R.layer_norm_bound(cat, g, b, EPS, plan)), worst, "y")
+    record("rowwise_fp64/patch_merge", C=C, io=io, bound_used=worst["y"])
 
 
 def test_patch_merge_without_instantiation_is_refused():
@@ -425,25 +473,55 @@ def test_layernorm_bwd_past_grid_cap():
     record("rowwise_fp64/layernorm_bwd", rows=rows, C=C, warps=nw, steps_per_warp=steps, bound_used=worst)
 
 
+@pytest.mark.parametrize("D", BWD_BF16_D)
+def test_layernorm_bwd_bf16(D):
+    """sigma_layernorm_bwd_bf16 (bf16 x, dy and dx; fp32 gamma, dgamma, dbeta) at every instantiation, its grid capped and every
+    warp walking 5 steps, on the bf16 form of every hard_rows family: dx inside layernorm_bwd_bound plus its bf16 store, dgamma /
+    dbeta inside the unchanged fp32 bound"""
+    lpr = R.bwd_plan(1, D)[0]
+    rows = 5 * R.NUM_SMS * 8 * 32 * (32 // lpr) // 4 - 3          # the last warp step ragged where a step holds several rows
+    _, _, nw, steps = R.bwd_plan(rows, D)
+    assert nw == R.NUM_SMS * 8 * 8 and steps == 5, "premise: the grid is capped and every warp walks 5 steps"
+    x = R.hard_rows(S + 31 + D, rows, D, device="cuda", bf16=True)
+    dy = _randn(S + 32 + D, (rows, D)).to(BF)
+    g, _ = _affine(S + 33 + D, D)
+    bx, dx = guarded((rows, D), BF)
+    bg, dg = guarded((D,))
+    bb, db = guarded((D,))
+    _call("sigma_layernorm_bwd_bf16", ptr(x), ptr(dy), ptr(g), ptr(dx), ptr(dg), ptr(db), rows, D, EPS, stream())
+    for buf, what in ((bx, "dx"), (bg, "dgamma"), (bb, "dbeta")):
+        guard_ok(buf, f"layernorm_bwd_bf16 D={D} {what}")
+    ref = R.layernorm_bwd_ref64(x, dy, g, EPS)
+    bnd = list(R.layernorm_bwd_bound(x, dy, g, EPS))
+    bnd[0] = R.bf16_store_bound(ref[0], bnd[0])
+    worst = {}
+    for name, got, rf, bd in zip(("dx", "dgamma", "dbeta"), (dx, dg, db), ref, bnd):
+        _check(f"layernorm_bwd_bf16 D={D} {name}", got, rf, bd, worst, name)
+    record("rowwise_fp64/layernorm_bwd_bf16", rows=rows, D=D, warps=nw, steps_per_warp=steps, bound_used=worst)
+
+
 # ---------------------------------------------------------------- the benchmark's batch
 BENCH_B = 74
 CHECK_IMAGES = (0, 37, 73)
 
 
 def test_bench_batch_layernorm():
-    """C = 96 on 74 x 19200 rows (120 x 160 maps): every image bit-identical to a batch-1 run; images 0, 37, 73 against fp64"""
+    """C = 96 on 74 x 19200 rows (120 x 160 maps), fp32 and bf16 out (sigma_layernorm_fwd_bf16, the bf16 inference mode's): every
+    image bit-identical to a batch-1 run; images 0, 37, 73 against fp64"""
     C, L = 96, 120 * 160
     x = R.hard_rows(S + 21, BENCH_B * L, C, device="cuda")
     g, b = _affine(S + 22, C)
-    y = _layernorm(x, g, b)
-    for i in range(BENCH_B):
-        assert torch.equal(_layernorm(x[i * L:(i + 1) * L].contiguous(), g, b), y[i * L:(i + 1) * L]), f"image {i}"
     worst = {}
-    for i in CHECK_IMAGES:
-        xi = x[i * L:(i + 1) * L]
-        _check(f"bench ln image {i}", y[i * L:(i + 1) * L], R.layer_norm_ref64(xi, g, b, EPS),
-               R.layer_norm_bound(xi, g, b, EPS, R.row_plan(C)), worst, "y")
-    record("rowwise_fp64/bench_layernorm", B=BENCH_B, bound_used=worst["y"])
+    for io in (0, 1):
+        y = _layernorm(x, g, b, io)
+        for i in range(BENCH_B):
+            assert torch.equal(_layernorm(x[i * L:(i + 1) * L].contiguous(), g, b, io), y[i * L:(i + 1) * L]), f"io={io} image {i}"
+        for i in CHECK_IMAGES:
+            xi = x[i * L:(i + 1) * L]
+            ref = R.layer_norm_ref64(xi, g, b, EPS)
+            _check(f"bench ln io={io} image {i}", y[i * L:(i + 1) * L], ref,
+                   _bound(io, ref, R.layer_norm_bound(xi, g, b, EPS, R.row_plan(C, io=io))), worst, f"y_io{io}")
+    record("rowwise_fp64/bench_layernorm", B=BENCH_B, bound_used=worst["y_io0"], bound_used_bf16=worst["y_io1"])
 
 
 def test_bench_batch_head():

@@ -20,6 +20,7 @@ from helpers import record
 from oracle import rowwise_ref64 as R
 
 F32 = torch.float32
+BF = torch.bfloat16
 LOG2E_F32 = torch.tensor(1.4426950408889634, dtype=F32)
 EPS = 1e-5
 SRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "sigma_b200", "csrc", "rowwise.cu")
@@ -52,27 +53,41 @@ def _silu(z):
     return (z.double() / (1.0 + e).double() * (1 - R.E_FDIV)).float()
 
 
+def _bf(t):
+    """fp32 -> bf16 -> fp32, round to nearest even (the kernels' st4 / __floats2bfloat162_rn)"""
+    return t.to(BF).float()
+
+
+def _bf_rz(t):
+    """fp32 -> bf16 rounding toward zero (the low 16 bits dropped), as fp32"""
+    return (t.contiguous().view(torch.int32) & -65536).view(F32)
+
+
 def emu_norm(y, gamma, beta, eps, plan, z=None, gate_r=None, mut=()):
     """row_norm_{fast_,}kernel on y (K, rows, D) fp32: the K-sum, the lane-ordered mean / variance, rsqrtf, the fmaf epilogue,
     SiLU(z) and the gate (gate_r: the gate row of every row).  Also the normalisation of the head / upsample kernels.
-    mut: "one_pass" (var = E[x^2] - mean^2), "eps_on_sigma" (rstd = 1/(sqrt(var) + eps))"""
+    mut: "one_pass" (var = E[x^2] - mean^2), "eps_on_sigma" (rstd = 1/(sqrt(var) + eps)), "k_sum_bf16" (each partial K-sum rounded
+    to bf16), "stats_bf16" (mean and variance from a bf16-rounded copy of the row)"""
     K, rows, D = y.shape
     lanes, vecs = plan[:2]
     a = y[0].clone()
     for k in range(1, K):
         a = a + y[k]
+        if "k_sum_bf16" in mut:
+            a = _bf(a)
     Dp = 4 * lanes * vecs
     xp = torch.zeros(rows, Dp, dtype=F32)
     xp[:, :D] = a
     mask = torch.zeros(Dp, dtype=F32)
     mask[:D] = 1
     view = lambda t: t.view(rows, vecs, lanes, 4)
-    mean = _lane_sum(view(xp), lanes) / float(D)
+    xs = _bf(xp) if "stats_bf16" in mut else xp
+    mean = _lane_sum(view(xs), lanes) / float(D)
     d = xp - mean[:, None]
     if "one_pass" in mut:
         var = _lane_sum(view(xp * xp), lanes) / float(D) - mean * mean
     else:
-        dm = d * mask
+        dm = (xs - mean[:, None]) * mask
         var = _lane_sum(view(dm * dm), lanes) / float(D)
     if "eps_on_sigma" in mut:
         rstd = (1.0 / (torch.sqrt(var.clamp_min(0)) + eps)).float()
@@ -162,8 +177,9 @@ def emu_pool(x, nslice, mut=()):
     return tot / float(div), torch.stack(maxs, 1).amax(1), torch.stack(sums, 1)
 
 
-def emu_ln_bwd(x, dy, gamma, eps):
-    """layernorm_bwd_body: dx of every row, dgamma / dbeta as the grid's warps accumulate them (rows in warp order)"""
+def emu_ln_bwd(x, dy, gamma, eps, mut=()):
+    """layernorm_bwd_body: dx of every row, dgamma / dbeta as the grid's warps accumulate them (rows in warp order).
+    mut: "dx_bf16_before_rstd" (dx = bf16(bf16(gamma dy - m1 - xhat m2)·rstd): a bf16 kernel rounding before the last product)"""
     rows, D = x.shape
     lpr, vecs, nw, _ = R.bwd_plan(rows, D)
     view = lambda t: t.view(rows, vecs, lpr, 4)
@@ -175,7 +191,8 @@ def emu_ln_bwd(x, dy, gamma, eps):
     a = gamma * dy
     m1 = _lane_sum(view(a), lpr) * invD
     m2 = _lane_sum(view(a * xh), lpr) * invD
-    dx = rstd[:, None] * (a - m1[:, None] - xh * m2[:, None])
+    inner = a - m1[:, None] - xh * m2[:, None]
+    dx = _bf(rstd[:, None] * _bf(inner)) if "dx_bf16_before_rstd" in mut else rstd[:, None] * inner
     rpw = 32 // lpr
     steps = -(-rows // rpw)
     dg, db = torch.zeros(D, dtype=F32), torch.zeros(D, dtype=F32)
@@ -346,6 +363,66 @@ def test_layernorm_bwd_bound_covers_fp32_emulation(D):
         assert frac <= 1.0, name
 
 
+def _bf16_case(io, K, D, rows=60, seed=70):
+    """inputs of a bf16 instance as its GPU test draws them: y (K, rows, D) bf16-exact for io 2 (fp32 for io 1, K = 1), z bf16-exact"""
+    y = torch.stack([R.hard_rows(seed + k, rows, D, bf16=io == 2).float() for k in range(K)])
+    z = _bf(torch.randn(rows, D, generator=torch.Generator().manual_seed(seed)) * 3) if io == 2 else None
+    return y, z
+
+
+@pytest.mark.parametrize("io,K,D", [(1, 1, 96), (1, 1, 200), (1, 1, 2048), (2, 1, 64), (2, 2, 384), (2, 3, 200), (2, 4, 96), (2, 8, 1000)])
+def test_bf16_norm_bound_covers_fp32_then_bf16_emulation(io, K, D):
+    """the fp32 emulation on bf16-exact inputs, its output rounded to bf16 once: inside bf16_store_bound of the fp32 bound; a constant
+    row gives bf16(beta) exactly"""
+    rows, rpb = 60, 7
+    y, z = _bf16_case(io, K, D, rows)
+    gate = torch.randn(-(-rows // rpb), D) if io == 2 else None
+    g, b = R.affine(71, D)
+    plan = R.row_plan(D, K, io=io)
+    got = emu_norm(y, g, b, EPS, plan, z, gate[torch.arange(rows) // rpb] if gate is not None else None).to(BF)
+    ref = R.merge_norm_ref64(y, g, b, EPS, z, gate, rpb)
+    frac = R.bound_fraction(got, ref, R.bf16_store_bound(ref, R.merge_norm_bound(y, g, b, EPS, plan, z, gate, rpb)))
+    record("rowwise_ref64_cpu/bf16_soundness", io=io, K=K, D=D, bound_used=frac)
+    assert frac <= 1.0
+    const = R.constant_rows(rows)
+    got_c = emu_norm(y, g, b, EPS, plan).to(BF)[const]
+    assert torch.equal(got_c, b.to(BF).expand(int(const.sum()), D)), "a constant row must give bf16(beta) exactly"
+
+
+def test_bf16_hard_rows_stay_hard():
+    """the bf16 form of hard_rows: var_eps rows keep sigma^2 ~ eps after rounding (not flattened to a few values), constant rows
+    stay constant and exact"""
+    D = 384
+    x = R.hard_rows(72, 50, D, bf16=True)
+    assert x.dtype == BF
+    fam = torch.arange(50) % len(R.ROW_FAMILIES)
+    var = x.double().var(-1, unbiased=False)
+    ve = var[fam == R.ROW_FAMILIES.index("var_eps")]
+    assert bool((ve > 0.3 * EPS).all() and (ve < 3 * EPS).all()), ve
+    distinct = [len(torch.unique(r)) for r in x[fam == R.ROW_FAMILIES.index("var_eps")]]
+    assert min(distinct) >= 20, distinct
+    x32 = R.hard_rows(72, 50, D)
+    const = R.constant_rows(50)
+    assert torch.equal(x[const].float(), x32[const])
+
+
+@pytest.mark.parametrize("D", [32, 96, 384])
+def test_layernorm_bwd_bf16_bound_covers_emulation(D):
+    """sigma_layernorm_bwd_bf16: bf16-exact x and dy, the fp32 body, dx rounded once: dx inside bf16_store_bound, dgamma / dbeta
+    inside the unchanged fp32 bound"""
+    rows = 203
+    x = R.hard_rows(80 + D, rows, D, bf16=True).float()
+    g, _ = R.affine(81, D)
+    dy = _bf(torch.randn(rows, D, generator=torch.Generator().manual_seed(82)))
+    dx, dg, db = emu_ln_bwd(x, dy, g, EPS)
+    ref = R.layernorm_bwd_ref64(x, dy, g, EPS)
+    bnd = R.layernorm_bwd_bound(x, dy, g, EPS)
+    for name, gt, rf, bd in zip(("dx", "dgamma", "dbeta"), (dx.to(BF), dg, db), ref, (R.bf16_store_bound(ref[0], bnd[0]),) + bnd[1:]):
+        frac = R.bound_fraction(gt, rf, bd)
+        record("rowwise_ref64_cpu/ln_bwd_bf16_soundness", D=D, out=name, bound_used=frac)
+        assert frac <= 1.0, name
+
+
 # ---------------------------------------------------------------- sharpness: plausible mistakes land outside the bound
 def _outside(got, ref, bound, what):
     frac = R.bound_fraction(got, ref, bound)
@@ -361,6 +438,33 @@ def test_variance_mistakes_are_rejected(mut, family):
     plan = R.row_plan(D)
     _outside(emu_norm(x[None], g, b, EPS, plan, mut=(mut,)), R.layer_norm_ref64(x, g, b, EPS),
              R.layer_norm_bound(x, g, b, EPS, plan), mut)
+
+
+@pytest.mark.parametrize("mut,io,K,family", [("round_toward_zero", 2, 1, "ordinary"), ("k_sum_bf16", 2, 4, "ordinary"),
+                                             ("stats_bf16", 1, 1, "large_mean")])
+def test_bf16_norm_mistakes_are_rejected(mut, io, K, family):
+    """a bf16 store that truncates, the K-direction sum kept in bf16, statistics taken from a bf16-rounded copy of an fp32 row"""
+    D = 96
+    y = torch.stack([R.hard_rows(90 + k, 40, D, families=(family,), bf16=io == 2).float() for k in range(K)])
+    g, b = R.affine(91, D)
+    plan = R.row_plan(D, K, io=io)
+    o = emu_norm(y, g, b, EPS, plan, mut=(mut,))
+    got = _bf_rz(o) if mut == "round_toward_zero" else o.to(BF)
+    ref = R.merge_norm_ref64(y, g, b, EPS)
+    bound = R.bf16_store_bound(ref, R.merge_norm_bound(y, g, b, EPS, plan))
+    assert R.bound_fraction(emu_norm(y, g, b, EPS, plan).to(BF), ref, bound) <= 1.0
+    _outside(got, ref, bound, mut)
+
+
+def test_bf16_ln_bwd_double_rounding_is_rejected():
+    """dx rounded to bf16 before the final rstd product (and again on the store)"""
+    D, rows = 96, 203
+    x = R.hard_rows(92, rows, D, families=("ordinary",), bf16=True).float()
+    g, _ = R.affine(93, D)
+    dy = _bf(torch.randn(rows, D, generator=torch.Generator().manual_seed(94)))
+    ref = R.layernorm_bwd_ref64(x, dy, g, EPS)
+    bound = R.bf16_store_bound(ref[0], R.layernorm_bwd_bound(x, dy, g, EPS)[0])
+    _outside(emu_ln_bwd(x, dy, g, EPS, mut=("dx_bf16_before_rstd",))[0], ref[0], bound, "dx rounded before rstd")
 
 
 def test_gate_and_z_mistakes_are_rejected():
@@ -456,3 +560,40 @@ def test_instantiation_tables_are_covered():
     assert {R.head_plan(C, 0)[1] for C in G.UPSAMPLE_C} == {1, 2, 4, 8}
     assert all(R.row_plan(4 * c, mode=1)[2] for c in G.PATCH_MERGE_C) and not any(4 * G.PATCH_MERGE_UNSUPPORTED_C == 4 * l * v for l, v in row)
     assert {4 * l * v for l, v in row} <= set(G.SHUFFLE_D)
+
+
+_IO = {("float", "float"): 0, ("float", "bf16"): 1, ("bf16", "bf16"): 2}
+
+
+def _io(ti, to):
+    return _IO[tuple("bf16" if t == "__nv_bfloat16" else t for t in (ti, to))]
+
+
+def test_io_dispatch_is_the_oracles_and_covered():
+    """row_norm_fast_k's (io, mode, K) instances and row_norm_launch's generic (io, MAXV) ones, parsed from rowwise.cu, are the
+    oracle's (ROW_FAST_IO, MAXV_GENERIC), and the GPU test's parameter lists reach every one of them at every fast width; the bf16
+    LayerNorm backward exists and its GPU test runs every BWD_FAST width"""
+    src = open(SRC).read()
+    i = src.index("static bool row_norm_fast_k(")
+    fast = {(_io(ti, to), int(mode), int(k))
+            for k, mode, ti, to in re.findall(r"row_norm_fast_kernel<LPR, V, (\d), (\d), (\w+), (\w+)>", src[i:src.index("\n}\n", i)])}
+    assert fast == {(io, mode, k) for io, modes in R.ROW_FAST_IO.items() for mode, ks in modes.items() for k in ks}
+    i = src.index("int row_norm_launch(")
+    body = src[i:src.index("\n}\n", i)]
+    gen_io = {_io(ti, to) for ti, to in re.findall(r"row_norm_kernel<MV, (\w+), (\w+)>", body)}
+    maxv = [int(m) for m in re.findall(r"LAUNCH\((\d+)\);", body)]
+    assert gen_io == {0, 1, 2} and tuple(maxv) == R.MAXV_GENERIC
+    # what the GPU cases reach: fast (io, mode, K, lanes, vecs) and generic (io, MAXV)
+    cases = [(D, 1, 0, io) for D in G.LN_FAST_D + G.LN_GENERIC_D for io in G.LN_IO]
+    cases += [(D, K, 0, io) for K in G.MERGE_K for D in G.MERGE_D for io in G.MERGE_IO]
+    cases += [(4 * C, 1, 1, io) for C in G.PATCH_MERGE_C for io in G.PATCH_MERGE_IO]
+    cases += [(D, 1, 2, 0) for D in G.SHUFFLE_D]
+    reached = set()
+    for D, K, mode, io in cases:
+        lanes, vecs, is_fast = R.row_plan(D, K, mode, io)
+        reached.add((io, mode, K, lanes, vecs) if is_fast else (io, vecs))
+    want = {(io, mode, k, l, v) for io, mode, k in fast for l, v in R.ROW_FAST} | {(io, mv) for io in gen_io for mv in maxv}
+    assert want <= reached, sorted(want - reached)
+    i = src.index("static void layernorm_bwd_k(")
+    assert "layernorm_bwd_bf16_kernel<LPR, V>" in src[i:src.index("\n}\n", i)]
+    assert set(G.BWD_BF16_D) == {4 * l * v for l, v in R.BWD_FAST}

@@ -7,12 +7,12 @@ activations) against fp64.
   rounding tie never turns into a false failure and nothing is loosened.  Kinds cross4 / seq2 at d_state 4 and 16, every padded
   dt_rank Sigma trains with, ragged maps, batch 1 / 2 / 3, L-segments 1, 2, 7, the library's choice, the cap, and a forward cut
   differently from its backward; outputs inside NaN-filled guards; the dt_r and padding columns of dxdbl 0.
-* Kind cross (CroMB): delta' and the forward the same way (the fp64 forward runs on the kernel's delta').  Its fp64 backward
-  reference (tests/ss2d_cross_ref64.py) takes no delta', so the backward is held to it in the max norm: 1e-2 of each output's scale,
-  which is what rounding delta' to 8 significand bits leaves (measured: 1.4e-3 .. 2.3e-3); the element-wise check of the backward
-  body is the cross4 / seq2 one, which shares every line but the source of C.
+* Kind cross (CroMB) the same way, element by element: delta' against the softplus, everything else against
+  tests/ss2d_cross_ref64.py run on the kernel's delta' (delta=), at CroMB's training shapes at d_state 4 with 1-3 images
+  (test_ss2d_cross_bwd_fp64_gpu.CASES) and at d_state 16.
 * FusedSS2DCore.apply with the switch on under bf16 autocast: bf16 output, bf16 saved xc and delta', the saved bytes, all six
-  gradients against the fp64 chain; with the switch off, and under the deterministic switch, the fp32 entry points run.
+  gradients against the fp64 chain (kind cross chained per modality half); with the switch off, and under the deterministic
+  switch, the fp32 entry points run.
 * LayerNormFn with bf16 activations against fp64 at every width of ops._LN_WIDTHS."""
 import math
 
@@ -23,6 +23,7 @@ import procedural as P
 from helpers import guard_ok as _guard_ok, guarded as _guarded, ptr as _p, record, ss2d_kind as _kid, ss2d_params, stream as _stream
 import ss2d_delta_ref64 as RD
 from oracle import ss2d_ref64 as R64
+from test_ss2d_cross_bwd_fp64_gpu import CASES as CROSS_CASES          # (H, W, D, R, images) of CroMB's training shapes
 
 pytestmark = pytest.mark.gpu
 S = 211
@@ -133,29 +134,33 @@ def test_bf16_pair_matches_fp64(kind, B, H, W, D, N, R):
     record(f"ss2d bf16 train fp64 {tag}", **worst)
 
 
-@pytest.mark.parametrize("B,H,W,D,N,R", [(2, 30, 40, 768, 4, 24), (4, 15, 20, 1536, 4, 48), (2, 60, 80, 384, 16, 12), (4, 23, 30, 192, 16, 6)])
+# Bt = 2·images, H, W, D, N, R: CroMB's training shapes at d_state 4 with 1-3 images, and two d_state 16 cases
+CROSS = [(2 * im, H, W, D, 4, R) for H, W, D, R, im in CROSS_CASES] + [(2, 60, 80, 384, 16, 12), (4, 23, 30, 192, 16, 6)]
+
+
+@pytest.mark.parametrize("B,H,W,D,N,R", CROSS)
 def test_bf16_pair_cross(B, H, W, D, N, R):
+    """kind cross: delta' against the fp64 softplus; every other output element by element against tests/ss2d_cross_ref64.py run on
+    the kernel's saved delta' (one reference: delta' must not depend on the L-segment cut)"""
     from ss2d_cross_ref64 import ss2d_cross_ref64
     kind, tag = "cross", f"cross/{B}/{H}x{W}/D{D}/N{N}/R{R}"
     args16, Cp = _args16(kind, B, H, W, D, N, R, tag)
     xc, xdbl, dtw, dtb, A, Ds, dy = args16
     dref, dbnd = _delta_ref(kind, xdbl, dtw, dtb, N, R)
-    cref, _ = ss2d_cross_ref64(xc.float(), xdbl, dtw, dtb, A, Ds, dy.float(), H, W)
-    worst = {}
+    worst, key, ref = {}, None, None
     for fs, bs in [(0, 0), (1, 1), (3, 7), (100, 100)]:
         t = f"{tag} fwd={fs} bwd={bs}"
-        bufs, outs, (head, tail) = _pair(kind, B, H, W, D, N, R, Cp, args16, fs, bs)
+        bufs, outs, _ = _pair(kind, B, H, W, D, N, R, Cp, args16, fs, bs)
         _check(t, "delta", outs["delta"], dref, dbnd, worst)
-        yr, yb = RD.ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, delta=outs["delta"].double())
-        _check(t, "y", outs["y"], yr, yb, worst)
-        for n in ("dxc", "ddelta", "dA", "dDs", "ddtb"):
-            err = float((outs[n].double() - cref[n]).abs().max()) / float(cref[n].abs().max())
-            worst["maxnorm/" + n] = max(worst.get("maxnorm/" + n, 0.0), err)
-            assert err <= 1e-2, f"{t} {n}: {err:.3e} of its scale"
+        if key is None:
+            key = outs["delta"].view(torch.int16).clone()
+            ref, bnd = ss2d_cross_ref64(xc, xdbl, dtw, dtb, A, Ds, dy.float(), H, W, delta=outs["delta"].double())
+        assert torch.equal(outs["delta"].view(torch.int16), key), f"{t}: delta' depends on the L-segment cut"
+        for name in ("y", "hs", "dxc", "ddelta", "dA", "dDs", "ddtb"):
+            _check(t, name, outs[name], ref[name], bnd[name], worst)
         dx = outs["dxdbl"]
-        for n, got in (("dB", dx[..., :N]), ("dC", dx[..., N:2 * N])):
-            err = float((got.double() - cref[n]).abs().max()) / float(cref[n].abs().max())
-            assert err <= 1e-2, f"{t} {n}: {err:.3e} of its scale"
+        _check(t, "dB", dx[..., :N], ref["dB"], bnd["dB"], worst)
+        _check(t, "dC", dx[..., N:2 * N], ref["dC"], bnd["dC"], worst)
         assert bool((dx[..., 2 * N:] == 0).all()), f"{t}: the dt_r / padding columns of dxdbl must stay 0"
         for name, buf in bufs.items():
             _guard_ok(buf, f"{t} {name}")
@@ -166,22 +171,26 @@ def _bf(t):
     return t.to(BF).float()
 
 
-@pytest.mark.parametrize("kind,B,H,W,D,N,R", [("cross4", 2, 60, 80, 384, 16, 12), ("seq2", 2, 15, 20, 1536, 4, 48), ("cross4", 2, 30, 40, 768, 4, 24)])
+@pytest.mark.parametrize("kind,B,H,W,D,N,R", [("cross4", 2, 60, 80, 384, 16, 12), ("seq2", 2, 15, 20, 1536, 4, 48), ("cross4", 2, 30, 40, 768, 4, 24),
+                                               ("cross", 4, 30, 40, 768, 4, 24)])
 def test_fused_core_autograd_bf16_mode(kind, B, H, W, D, N, R, monkeypatch):
     from sigma_b200 import _lib, fused, ops
+    from ss2d_cross_ref64 import ss2d_cross_ref64
+    from test_ss2d_bwd_fp64_gpu import core_chain64, core_xdbl
     monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
-    K = 4 if kind == "cross4" else 2
+    K = {"cross4": 4, "seq2": 2, "cross": 1}[kind]            # x_dbl rows per position
+    Kw = 2 if kind == "cross" else K                          # parameter sets
     Lseq = H * W * (2 if kind == "seq2" else 1)
     Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
     tag = f"ag16/{kind}/{B}/{H}x{W}/D{D}/N{N}/R{R}"
     xc0 = P.randn(S, tag + "/xc", (B, Lseq, D)).cuda().to(BF)
     wgt = _bf(P.randn(S, tag + "/w", (B, Lseq, D)).cuda())
-    xpw = _bf(P.randn(S, tag + "/xpw", (K, R + 2 * N, D), D ** -0.5).cuda())          # exact in the bf16 x_proj GEMM
-    dtw = P.rand(S, tag + "/dtw", (K, D, R), -R ** -0.5, R ** -0.5).cuda()
-    dt = torch.exp(P.rand(S, tag + "/dt", (K, D), math.log(1e-3), math.log(0.1)))
+    xpw = _bf(P.randn(S, tag + "/xpw", (Kw, R + 2 * N, D), D ** -0.5).cuda())         # exact in the bf16 x_proj GEMM
+    dtw = P.rand(S, tag + "/dtw", (Kw, D, R), -R ** -0.5, R ** -0.5).cuda()
+    dt = torch.exp(P.rand(S, tag + "/dt", (Kw, D), math.log(1e-3), math.log(0.1)))
     dtb = (dt + torch.log(-torch.expm1(-dt))).cuda()
-    Al = (torch.log(torch.arange(1, N + 1, dtype=torch.float32)).repeat(K * D, 1) + P.rand(S, tag + "/A", (K * D, N), -0.2, 0.2)).cuda()
-    Ds = P.randn(S, tag + "/Ds", (K * D,), 0.1, 1.0).cuda()
+    Al = (torch.log(torch.arange(1, N + 1, dtype=torch.float32)).repeat(Kw * D, 1) + P.rand(S, tag + "/A", (Kw * D, N), -0.2, 0.2)).cuda()
+    Ds = P.randn(S, tag + "/Ds", (Kw * D,), 0.1, 1.0).cuda()
 
     def run(on):
         leaves = [t.clone().requires_grad_(True) for t in (xc0, xpw, dtw, dtb, Al, Ds)]
@@ -215,29 +224,20 @@ def test_fused_core_autograd_bf16_mode(kind, B, H, W, D, N, R, monkeypatch):
     slabs = [t for t in saved if t.shape == (K, B, Lseq, D)]
     assert len(slabs) == 1 and slabs[0].dtype == BF and [t.dtype for t in saved if t.shape == (B, Lseq, D)] == [BF]
     hs_bytes = _lib.lib().sigma_ss2d_scan_hs_bytes(_kid(kind), B, H, W, D, N)
-    want = (B * Lseq * D * 2 + K * B * Lseq * D * 2 + B * Lseq * K * Cp * 4 + K * Cp * D * 4 + K * D * R * 4 + K * D * 4 + K * D * N * 4
-            + K * D * 4 + hs_bytes)               # xc, delta' (bf16); x_dbl, xw, W_dt, bias, A, Ds, hs (fp32)
+    want = (B * Lseq * D * 2 + K * B * Lseq * D * 2 + B * Lseq * K * Cp * 4 + Kw * Cp * D * 4 + Kw * D * R * 4 + Kw * D * 4
+            + Kw * D * N * 4 + Kw * D * 4 + hs_bytes)          # xc, delta' (bf16); x_dbl, xw, W_dt, bias, A, Ds, hs (fp32)
     assert sum(t.numel() * t.element_size() for t in saved) == want
     # the fp64 chain on the delta' the forward saved
     with torch.no_grad():
-        xw = torch.cat([fused._pack_xproj(xpw[k], N, R, Cp) for k in range(K)], dim=0).contiguous()
-        xdbl = fused.linear(xc0.view(B * Lseq, D), xw, kind="x_proj").view(B, Lseq, K, Cp)
+        xdbl, xw = core_xdbl(kind, xc0, xpw, N, R, Cp)                # the forward's own x_proj GEMM calls
         A = -torch.exp(Al)
-        ref, _ = RD.ss2d_ref64(kind, xc0, xdbl, dtw, dtb, A, Ds, wgt, H, W, delta=slabs[0].double())
-        d = lambda t: t.double()
-        BL = B * Lseq
-        dxd = torch.zeros(B, Lseq, K, Cp, dtype=torch.float64, device="cuda")
-        dxd[..., :N], dxd[..., N:2 * N] = ref["dB"], ref["dC"]
-        dW = []
-        for k in range(K):
-            dd = ref["ddelta"][k].reshape(BL, D)
-            dxd[:, :, k, 2 * N:2 * N + R] = (dd @ d(dtw[k])).view(B, Lseq, R)
-            dW.append(dd.t() @ d(xdbl[:, :, k, 2 * N:2 * N + R]).reshape(BL, R))
-        d2 = dxd.view(BL, K * Cp)
-        dxc = ref["dxc"] + (d2 @ d(xw)).view(B, Lseq, D)
-        dxw = (d2.t() @ d(xc0).view(BL, D)).view(K, Cp, D)
-        order = lambda t: torch.cat([t[:, 2 * N:2 * N + R], t[:, 0:N], t[:, N:2 * N]], dim=1)
-        want = [dxc, order(dxw), torch.stack(dW), ref["ddtb"], ref["dA"] * d(A), ref["dDs"]]
+        if kind == "cross":
+            ref, _ = ss2d_cross_ref64(xc0, xdbl, dtw, dtb, A, Ds, wgt, H, W, delta=slabs[0].double())
+        else:
+            ref, _ = RD.ss2d_ref64(kind, xc0, xdbl, dtw, dtb, A, Ds, wgt, H, W, delta=slabs[0].double())
+        want, _ = core_chain64(kind, ref, None, xc0, xdbl, xw, dtw, N, R, Cp)
+        want[4] = want[4] * A.double()
+        dxc = want[0]
         worst = {}
         # y: K directions each rounded to bf16, added in fp32, rounded once more; dxc: one rounding of the fp32 sum
         yr = ref["y"].sum(0)

@@ -9,7 +9,7 @@ that module's per-element error bounds, at Sigma's training shapes:
 * every output inside NaN-filled memory whose guard elements must stay bit-identical, the dt_r and padding columns of dxdbl 0;
 * y, delta' and the tile-start states hs of the training forward too, and of the state sweep (its workspace).
 At the autograd level FusedSS2DCore.apply is checked through all six gradients against the reference chained with the fp64
-x_proj / dt_proj algebra of its backward.  Parameters: dt log-uniform in [1e-3, 0.1] through the inverse softplus, A = -exp(A_log)
+x_proj / dt_proj algebra of its backward, kind cross (CroMB, tests/ss2d_cross_ref64.py) included, chained per modality half.  Parameters: dt log-uniform in [1e-3, 0.1] through the inverse softplus, A = -exp(A_log)
 around the S4D-real init, Ds near 1; one widened set (dt up to 0.5, |A| up to 4x).  Worst bound fractions go to helpers.record."""
 import ctypes
 import math
@@ -173,20 +173,63 @@ def _mm_bound_positions(aT, eaT, b):
     return rss + R64.LAMBDA * R64.U * math.sqrt(n) * ((aT @ b).abs() + ((aT * aT) @ (b * b)).sqrt())
 
 
-@pytest.mark.parametrize("kind,B,H,W,D,N,R", [("cross4", 2, 120, 160, 192, 16, 6), ("seq2", 2, 15, 20, 1536, 4, 48),
-                                               ("cross4", 2, 15, 20, 1536, 16, 48)])
-@pytest.mark.parametrize("save", [True, False])
-def test_fused_core_autograd_matches_fp64(kind, B, H, W, D, N, R, save, monkeypatch):
-    """FusedSS2DCore.apply: y and all six gradients against the reference chained with the fp64 x_proj / dt_proj algebra.  The
-    reference takes the very x_dbl the forward computed (the same deterministic GEMM call), so only the scan and the backward's
-    own fp32 GEMMs are under test; this pins the [dt | B | C] row order and the dA·A step at a real shape."""
-    from sigma_b200 import _lib, fused, ops
-    monkeypatch.setattr(ops, "FUSED_SAVE_STATES", save)
-    monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
-    K = 4 if kind == "cross4" else 2
+def core_chain64(kind, ref, bnd, xc, xdbl, xw, dtw, N, R, Cp):
+    """FusedSS2DCore's backward after the scan, in fp64: the six gradients (dxc, dx_proj_weight, ddt_projs_weight, ddt_projs_bias,
+    the scan's dA (the caller applies the dA·A step of dA_logs), dDs) from the scan reference `ref` (oracle/ss2d_ref64 or
+    tests/ss2d_cross_ref64 layouts), and with `bnd` their per-element bounds (else None).  dxdbl = [dB | dC | ddelta · W_dt | 0] per direction (cross: per modality half, its own
+    W_dt), then dxc += dxdbl · xw and d xw = dxdbl^T · xc per x_proj GEMM (cross: one per half, its own xw rows)."""
+    d = lambda t: t.double()
+    B, Lseq, K, _ = xdbl.shape
+    D = xc.shape[-1]
+    BL = B * Lseq
+    cross = kind == "cross"
+    Kw = 2 if cross else K
+    n = BL // 2
+    # (positions, x_dbl row, weight set) of each dt_proj step; (positions, xw rows) of each x_proj GEMM
+    steps = [(slice(m * n, (m + 1) * n), 0, m) for m in range(2)] if cross else [(slice(None), k, k) for k in range(K)]
+    gemms = [(slice(m * n, (m + 1) * n), slice(m * Cp, (m + 1) * Cp)) for m in range(2)] if cross else [(slice(None), slice(None))]
+    withb = bnd is not None
+    z = lambda *s: torch.zeros(s, dtype=torch.float64, device=xc.device)
+    dxd, edxd = z(BL, K, Cp), z(BL, K, Cp)
+    dxd[..., :N], dxd[..., N:2 * N] = ref["dB"].reshape(BL, K, N), ref["dC"].reshape(BL, K, N)
+    if withb:
+        edxd[..., :N], edxd[..., N:2 * N] = bnd["dB"].reshape(BL, K, N), bnd["dC"].reshape(BL, K, N)
+    dW, edW = z(Kw, D, R), z(Kw, D, R)
+    xd = d(xdbl).view(BL, K, Cp)
+    for rs, k, w in steps:
+        dd = ref["ddelta"][k].reshape(BL, D)[rs]
+        dtr = xd[rs, k, 2 * N:2 * N + R]
+        dxd[rs, k, 2 * N:2 * N + R] = dd @ d(dtw[w])
+        dW[w] = dd.t() @ dtr
+        if withb:
+            edd = bnd["ddelta"][k].reshape(BL, D)[rs]
+            edxd[rs, k, 2 * N:2 * N + R] = _mm_bound(dd, edd, d(dtw[w]), D)
+            edW[w] = _mm_bound_positions(dd.t(), edd.t(), dtr)
+    d2, e2 = dxd.view(BL, K * Cp), edxd.view(BL, K * Cp)
+    x2 = d(xc).reshape(BL, D)
+    dxc = ref["dxc"].reshape(BL, D).clone()
+    edxc = bnd["dxc"].reshape(BL, D).clone() if withb else None
+    dxw, edxw = z(Kw * Cp, D), z(Kw * Cp, D)
+    for rs, cs in gemms:
+        a, w = d2[rs], d(xw[cs])
+        dxc[rs] += a @ w
+        dxw[cs] = a.t() @ x2[rs]
+        if withb:
+            edxc[rs] += _mm_bound(a, e2[rs], w, a.shape[1])
+            edxw[cs] = _mm_bound_positions(a.t(), e2[rs].t(), x2[rs])
+    order = lambda t: torch.cat([t[:, 2 * N:2 * N + R], t[:, 0:N], t[:, N:2 * N]], dim=1)
+    want = [dxc.view(B, Lseq, D), order(dxw.view(Kw, Cp, D)), dW, ref["ddtb"], ref["dA"], ref["dDs"]]
+    if not withb:
+        return want, None
+    edxc += R64.U * dxc.abs()
+    return want, [edxc.view(B, Lseq, D), order(edxw.view(Kw, Cp, D)), edW, bnd["ddtb"], bnd["dA"], bnd["dDs"]]
+
+
+def core_inputs(kind, B, H, W, D, N, R, tag):
+    """leaves of FusedSS2DCore (xc, x_proj_weight, dt_projs_weight, dt_projs_bias, A_logs, Ds) and the output weight, fp32: one
+    parameter set per direction, or per modality for cross"""
+    K = {"cross4": 4, "seq2": 2, "cross": 2}[kind]
     Lseq = H * W * (2 if kind == "seq2" else 1)
-    Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
-    tag = f"ag/{kind}/{B}/{H}x{W}/D{D}/N{N}/R{R}"
     xc0 = P.randn(S, tag + "/xc", (B, Lseq, D)).cuda()
     wgt = P.randn(S, tag + "/w", (B, Lseq, D)).cuda()
     xpw = P.randn(S, tag + "/xpw", (K, R + 2 * N, D), D ** -0.5).cuda()
@@ -195,43 +238,58 @@ def test_fused_core_autograd_matches_fp64(kind, B, H, W, D, N, R, save, monkeypa
     dtb = (dt + torch.log(-torch.expm1(-dt))).cuda()
     Al = (torch.log(torch.arange(1, N + 1, dtype=torch.float32)).repeat(K * D, 1) + P.rand(S, tag + "/A", (K * D, N), -0.2, 0.2)).cuda()
     Ds = P.randn(S, tag + "/Ds", (K * D,), 0.1, 1.0).cuda()
+    return [xc0, xpw, dtw, dtb, Al, Ds], wgt
+
+
+def core_xdbl(kind, xc, xpw, N, R, Cp):
+    """x_dbl as FusedSS2DCore's forward computes it (the same GEMM calls): (B, Lseq, K, Cp), and the packed x_proj rows xw"""
+    from sigma_b200 import fused
+    B, Lseq, D = xc.shape
+    xw = torch.cat([fused._pack_xproj(xpw[k], N, R, Cp) for k in range(xpw.shape[0])], dim=0).contiguous()
+    if kind != "cross":
+        return fused.linear(xc.reshape(B * Lseq, D), xw, kind="x_proj").view(B, Lseq, -1, Cp), xw
+    n = B // 2 * Lseq
+    xdbl = torch.empty((B * Lseq, Cp), dtype=torch.float32, device=xc.device)
+    for m in range(2):
+        fused.linear(xc.reshape(B * Lseq, D)[m * n:(m + 1) * n], xw[m * Cp:(m + 1) * Cp], out=xdbl[m * n:(m + 1) * n], kind="x_proj")
+    return xdbl.view(B, Lseq, 1, Cp), xw
+
+
+@pytest.mark.parametrize("kind,B,H,W,D,N,R", [("cross4", 2, 120, 160, 192, 16, 6), ("seq2", 2, 15, 20, 1536, 4, 48),
+                                               ("cross4", 2, 15, 20, 1536, 16, 48), ("cross", 4, 30, 40, 768, 4, 24)])
+@pytest.mark.parametrize("save", [True, False])
+def test_fused_core_autograd_matches_fp64(kind, B, H, W, D, N, R, save, monkeypatch):
+    """FusedSS2DCore.apply: y and all six gradients against the reference chained with the fp64 x_proj / dt_proj algebra.  The
+    reference takes the very x_dbl the forward computed (the same deterministic GEMM calls), so only the scan and the backward's
+    own fp32 GEMMs are under test; this pins the [dt | B | C] row order and the dA·A step at a real shape.  Kind cross (CroMB, 2
+    images): the x_proj GEMMs, dt_proj steps and weight gradients per modality half, dC credited to the other half's rows."""
+    from sigma_b200 import _lib, ops
+    from ss2d_cross_ref64 import ss2d_cross_ref64
+    monkeypatch.setattr(ops, "FUSED_SAVE_STATES", save)
+    monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
+    K = {"cross4": 4, "seq2": 2, "cross": 1}[kind]
+    Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
+    tag = f"ag/{kind}/{B}/{H}x{W}/D{D}/N{N}/R{R}"
+    (xc0, xpw, dtw, dtb, Al, Ds), wgt = core_inputs(kind, B, H, W, D, N, R, tag)
     leaves = [t.clone().requires_grad_(True) for t in (xc0, xpw, dtw, dtb, Al, Ds)]
     y = ops.FusedSS2DCore.apply(*leaves, _kid(kind), H, W)
     (y * wgt).sum().backward()
     got = [t.grad for t in leaves]
     with torch.no_grad():
-        xw = torch.cat([fused._pack_xproj(xpw[k], N, R, Cp) for k in range(K)], dim=0).contiguous()
-        xdbl = fused.linear(xc0.view(B * Lseq, D), xw, kind="x_proj").view(B, Lseq, K, Cp)
+        xdbl, xw = core_xdbl(kind, xc0, xpw, N, R, Cp)
         A = -torch.exp(Al)
-        ref, bnd = R64.ss2d_ref64(kind, xc0, xdbl, dtw, dtb, A, Ds, wgt, H, W)
-        d = lambda t: t.double()
-        BL = B * Lseq
+        if kind == "cross":
+            ref, bnd = ss2d_cross_ref64(xc0, xdbl, dtw, dtb, A, Ds, wgt, H, W)
+        else:
+            ref, bnd = R64.ss2d_ref64(kind, xc0, xdbl, dtw, dtb, A, Ds, wgt, H, W)
         worst = {}
         yr = ref["y"].sum(0)
-        yb = bnd["y"].sum(0) + K * R64.U * ref["y"].abs().sum(0)
+        yb = bnd["y"].sum(0) + (K if K > 1 else 0) * R64.U * ref["y"].abs().sum(0)     # the directions' fp32 sum
         _check(tag, "y", y.detach(), yr, yb, worst)
-        # dxdbl = [dB | dC | ddelta_k · W_dt[k] | 0] (fp32 GEMM per direction), then dxc += dxdbl · xw, d xw = dxdbl^T · xc
-        dxd, edxd = torch.zeros(B, Lseq, K, Cp, dtype=torch.float64, device="cuda"), torch.zeros(B, Lseq, K, Cp, dtype=torch.float64, device="cuda")
-        dxd[..., :N], dxd[..., N:2 * N] = ref["dB"], ref["dC"]
-        edxd[..., :N], edxd[..., N:2 * N] = bnd["dB"], bnd["dC"]
-        dW, edW = [], []
-        for k in range(K):
-            dd, edd = ref["ddelta"][k].reshape(BL, D), bnd["ddelta"][k].reshape(BL, D)
-            dxd[:, :, k, 2 * N:2 * N + R] = (dd @ d(dtw[k])).view(B, Lseq, R)
-            edxd[:, :, k, 2 * N:2 * N + R] = _mm_bound(dd, edd, d(dtw[k]), D).view(B, Lseq, R)
-            dtr = d(xdbl[:, :, k, 2 * N:2 * N + R]).reshape(BL, R)
-            dW.append(dd.t() @ dtr)
-            edW.append(_mm_bound_positions(dd.t(), edd.t(), dtr))
-        d2, e2 = dxd.view(BL, K * Cp), edxd.view(BL, K * Cp)
-        dxc = ref["dxc"] + (d2 @ d(xw)).view(B, Lseq, D)
-        edxc = bnd["dxc"] + _mm_bound(d2, e2, d(xw), K * Cp).view(B, Lseq, D) + R64.U * dxc.abs()
-        dxw = (d2.t() @ d(xc0).view(BL, D)).view(K, Cp, D)
-        edxw = _mm_bound_positions(d2.t(), e2.t(), d(xc0).view(BL, D)).view(K, Cp, D)
-        order = lambda t: torch.cat([t[:, 2 * N:2 * N + R], t[:, 0:N], t[:, N:2 * N]], dim=1)
-        A64 = d(A)
-        want = [(dxc, edxc), (order(dxw), order(edxw)), (torch.stack(dW), torch.stack(edW)), (ref["ddtb"], bnd["ddtb"]),
-                (ref["dA"] * A64, bnd["dA"] * A64.abs() + 2 * R64.U * (ref["dA"] * A64).abs()), (ref["dDs"], bnd["dDs"])]
-        for name, g, (r, b) in zip(["dxc", "dx_proj_weight", "ddt_projs_weight", "ddt_projs_bias", "dA_logs", "dDs"], got, want):
+        want, bounds = core_chain64(kind, ref, bnd, xc0, xdbl, xw, dtw, N, R, Cp)
+        A64 = A.double()
+        want[4], bounds[4] = want[4] * A64, bounds[4] * A64.abs() + 2 * R64.U * (want[4] * A64).abs()
+        for name, g, r, b in zip(["dxc", "dx_proj_weight", "ddt_projs_weight", "ddt_projs_bias", "dA_logs", "dDs"], got, want, bounds):
             _check(f"{tag} save={save}", name, g, r, b, worst)
             # the weight gradients contract the scan's per-element bounds over all B·L positions, which leaves their propagated
             # bound looser than 1e-3 of scale at the largest element: there the max-norm bar holds as well

@@ -1,7 +1,8 @@
 """CPU: the fp64 reference of the CROSS (CroMB) scan backward (tests/ss2d_cross_ref64.py) that the fused backward's GPU tests compare
 with, and the backward's launch plan for kind CROSS.
 * every output and the tile-start states against torch.autograd in fp64 through a literal restatement of CroMB's two scans (each
-  modality's half with its own weights and B, C from the other half; a loop over L), at ragged maps and at L > 2048;
+  modality's half with its own weights and B, C from the other half; a loop over L), at ragged maps and at L > 2048; the same on a
+  given (bf16-rounded) delta' through delta=, and without delta' the same bits as on the oracle's own forward;
 * its error bound against an fp32 emulation whose decays are perturbed by the ex2.approx bound and whose forward runs in L-segments
   with carries formed as the summary pass forms them (an fp32 sum of delta'): the emulation must stay inside the bound;
 * three plausible kernel mistakes (dC credited to the image's own row, the other weight set's rows for dA / dDs / d dt_bias, C read
@@ -37,9 +38,10 @@ def _inputs(Bt, H, W, D, N, R, tag, wide=False):
     return xc, xdbl, dtw, dtb, A, Ds, dy
 
 
-def _literal(xc, xdbl, dtw, dtb, A, Ds, dy, H, W):
+def _literal(xc, xdbl, dtw, dtb, A, Ds, dy, H, W, delta=None):
     """CroMB's two scans restated (vmamba.py:1530,1536): fp64 autograd over a loop along L; the state entering every 16-position
-    block too"""
+    block too.  delta (1, Bt, L, D): run on this delta' instead of the softplus; ddelta is then the gradient at delta' times the
+    softplus derivative 1 - exp(-delta') and d dt_bias its sum, as the backward kernel forms them"""
     t = [v.double().clone().requires_grad_(True) for v in (xc, xdbl, dtw, dtb, A, Ds)]
     xc_, xdbl_, dtw_, dtb_, A_, Ds_ = t
     Bt, L, D = xc.shape
@@ -49,9 +51,12 @@ def _literal(xc, xdbl, dtw, dtb, A, Ds, dy, H, W):
     hs = torch.full((1, Bt, -(-L // 16), D, N), float("nan"), dtype=torch.float64)
     for m in range(2):
         sl, osl = slice(m * h2, (m + 1) * h2), slice((1 - m) * h2, (2 - m) * h2)
-        pre = xdbl_[sl, :, 0, 2 * N:2 * N + R] @ dtw_[m].t() + dtb_[m]
-        pre.retain_grad()
-        dl = torch.nn.functional.softplus(pre)
+        if delta is None:
+            pre = xdbl_[sl, :, 0, 2 * N:2 * N + R] @ dtw_[m].t() + dtb_[m]
+            pre.retain_grad()
+            dl = torch.nn.functional.softplus(pre)
+        else:
+            dl = pre = delta[0, sl].double().clone().requires_grad_(True)
         Am, Dm = A_[m * D:(m + 1) * D], Ds_[m * D:(m + 1) * D]
         u, Bm, Cm = xc_[sl], xdbl_[sl, :, 0, :N], xdbl_[osl, :, 0, N:2 * N]
         h = torch.zeros(h2, D, N, dtype=torch.float64)
@@ -66,9 +71,10 @@ def _literal(xc, xdbl, dtw, dtb, A, Ds, dy, H, W):
     total.backward()
     ddelta = torch.zeros(1, Bt, L, D, dtype=torch.float64)
     for sl, pre in pres:
-        ddelta[0, sl] = pre.grad
+        ddelta[0, sl] = pre.grad if delta is None else pre.grad * -torch.expm1(-pre.detach())
     g = xdbl_.grad
-    return dict(dxc=xc_.grad, ddelta=ddelta, dB=g[..., :N], dC=g[..., N:2 * N], dA=A_.grad, dDs=Ds_.grad, ddtb=dtb_.grad), hs
+    ddtb = dtb_.grad if delta is None else torch.stack([ddelta[0, :h2].sum((0, 1)), ddelta[0, h2:].sum((0, 1))])
+    return dict(dxc=xc_.grad, ddelta=ddelta, dB=g[..., :N], dC=g[..., N:2 * N], dA=A_.grad, dDs=Ds_.grad, ddtb=ddtb), hs
 
 
 @pytest.mark.parametrize("H,W,N,Bt", [(5, 7, 4, 2), (9, 11, 4, 4), (9, 11, 16, 2), (1, 9, 16, 4), (42, 50, 4, 2)])
@@ -83,6 +89,42 @@ def test_backward_and_states_match_autograd(H, W, N, Bt):
     assert float((ref["hs"] - hs).abs().max()) <= 1e-12 * float(hs.abs().max())
     y, by = R64.ss2d_fwd_ref64("cross", *args[:6], H, W)                   # the forward is the oracle's, bit for bit
     assert torch.equal(y, ref["y"]) and torch.equal(by, bnd["y"])
+
+
+@pytest.mark.parametrize("H,W,N,Bt", [(5, 7, 4, 2), (9, 11, 16, 4)])
+def test_given_delta_matches_the_literal_loop(H, W, N, Bt):
+    """delta=: every output against the literal loop run on the same delta' (a softplus value rounded to bf16, as the bf16 training
+    mode saves it); ref["delta"] is the given one with bound 0; and with delta' = the fp64 softplus, the delta= path agrees with
+    the reference that forms delta' itself"""
+    D, R = 8, 3
+    args = _inputs(Bt, H, W, D, N, R, f"d/{H}/{W}/{N}/{Bt}")
+    full, _ = ss2d_cross_ref64(*args, H, W)
+    given = full["delta"].to(torch.bfloat16).double()
+    ref, bnd = ss2d_cross_ref64(*args, H, W, delta=given)
+    want, hs = _literal(*args, H, W, delta=given)
+    for name, w in want.items():
+        err = float((ref[name] - w).abs().max()) / float(w.abs().max())
+        assert err < 1e-12, f"{name}: {err:.2e}"
+    assert float((ref["hs"] - hs).abs().max()) <= 1e-12 * float(hs.abs().max())
+    assert torch.equal(ref["delta"], given) and not bool(bnd["delta"].any())
+    same, _ = ss2d_cross_ref64(*args, H, W, delta=full["delta"])
+    for name in ("y", "dxc", "ddelta", "dB", "dC", "dA", "dDs", "ddtb"):
+        err = float((same[name] - full[name]).abs().max()) / float(full[name].abs().max())
+        assert err < 1e-12, f"{name}: {err:.2e}"
+
+
+def test_without_delta_the_oracle_forward_bit_for_bit(monkeypatch):
+    """without delta the reference is what it was when it ran on oracle/ss2d_ref64.ss2d_fwd_ref64: every output and bound the same
+    bits"""
+    import ss2d_cross_ref64 as C
+    H, W, N, Bt, D, R = 9, 11, 4, 4, 16, 6
+    args = _inputs(Bt, H, W, D, N, R, "bits")
+    ref, bnd = ss2d_cross_ref64(*args, H, W)
+    monkeypatch.setattr(C.RD, "ss2d_fwd_ref64", lambda *a, delta=None, **kw: R64.ss2d_fwd_ref64(*a, **kw))
+    ref0, bnd0 = ss2d_cross_ref64(*args, H, W)
+    for name in ref:
+        assert torch.equal(ref[name].nan_to_num(7.0), ref0[name].nan_to_num(7.0)), name
+        assert torch.equal(bnd[name].nan_to_num(7.0), bnd0[name].nan_to_num(7.0)), name
 
 
 def _emulate32(xc, xdbl, dtw, dtb, A, Ds, dy, H, W, seed, nseg):
