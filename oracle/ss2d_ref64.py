@@ -1,12 +1,15 @@
-"""fp64 reference of the fused SS2D scan core (sigma_ss2d_scan_fwd{,_split,_bf16,_save}, sigma_ss2d_scan_bwd{,_saved}) with a
-per-element error bound for each output of the fp32 kernels.  ORACLE — test infrastructure only.  Plain torch float64,
+"""fp64 reference of the fused SS2D scan core (sigma_ss2d_scan_fwd{,_split,_bf16,_save{,_bf16}}, sigma_ss2d_scan_bwd{,_saved{,_bf16}})
+with a per-element error bound for each output of the fp32 kernels.  ORACLE — test infrastructure only.  Plain torch float64,
 device-agnostic.  ss2d_fwd_ref64 is the forward alone (y and its bound, every kind, fp32 or bf16 xc); ss2d_ref64 runs it and
-adds the backward (kinds "cross4" and "seq2").
+adds the backward (every kind).
 
 Operation (kind "cross4": four directions over an H x W map; "seq2": forward and reversed walks over [rgb ‖ x], Lseq = 2·H·W;
 "cross": the cross-modality scan, one row-major walk over the batch Bt = 2·images, images [0, Bt/2) of modality 0 and
 [Bt/2, Bt) of modality 1: image b runs with weight set w = [b >= Bt/2] (its rows of A, Ds, dt_proj and bias, A (2·D, N)) and its
-own B and dt_r, but takes C from the other modality's image (b + Bt/2) mod Bt (vmamba.py:1530,1536)).
+own B and dt_r, but takes C from the other modality's image b' = (b + Bt/2) mod Bt (vmamba.py:1530,1536)).  walk_groups lists
+the walks: (direction, images, weight set, images C is read from).  Each walk's backward credits dB and dxc to its own images,
+dC to the images that supplied C (under "cross" the other half's rows of dxdbl), and dA, dDs and d dt_bias to its weight set's
+rows: K sets for "cross4" / "seq2", the two modalities' for "cross" (dA (2D, N), dDs (2D), ddtb (2, D)).
 For direction k, walk step l visits position p = idx_k[l] (row-major, column-major l = w·H + h, and their reverses):
     delta'_l = softplus(dt_r[p] · W_dt[k]^T + bias[k])                  (K, B, Lseq, D) slabs, stored at position p
     h_l = exp(delta'_l · A) ⊙ h_{l-1} + delta'_l · u_l · B_l,  y_l = C_l · h_l + Ds · u_l
@@ -58,6 +61,15 @@ u = 2^-24 (fp32 rounding) and E2 = 2^-22 (the relative error bound the PTX ISA d
 All first-order terms are multiplied by SAFETY = 1.5 to cover second-order terms and the few roundings not itemised above (the
 combine kernels, whose carry is a product of decays applied to a segment's start state rather than to each step's state).  Every
 bound is per element; none is a fraction of the tensor's maximum.
+
+A given delta' (delta=, the bf16 training mode: its kernels round delta' = softplus(dt_proj) to bf16 before the recurrence uses it
+and save that value).  The recurrence and the backward then run on an fp64 copy of the given values, taken as exact: err(delta') =
+0 in every term above, and the softplus derivative is 1 - exp(-delta') of the given value, as the backward kernel forms it.  delta'
+itself is checked apart, against the softplus and inside its fp32 bound + BF16_RN·|delta'| (delta_ref64, delta_bound_bf16).
+
+`mistake` (kind "cross" only) computes the result of a plausible kernel bug instead, for tests that the bound tells it apart:
+"dC_own" credits dC to the image's own row, "wset" sends dA / dDs / d dt_bias to the other weight set's rows, "C_own" reads C from
+the image's own half.
 """
 import math
 import types
@@ -73,6 +85,7 @@ SAFETY = 1.5
 LAMBDA = 6.0
 LT = 16
 KINDS = {"cross4": 4, "seq2": 2, "cross": 1}     # directions (x_dbl rows per position)
+MISTAKES = ("dC_own", "wset", "C_own")
 
 
 def dir_index(kind, H, W):
@@ -169,13 +182,43 @@ def _pad(t):
     return torch.cat([t, torch.zeros_like(t[:, :1])], 1)          # position Lseq = the padding's zero row
 
 
-def ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, device=None, on_walk=None):
+def _softplus64(dtr, dtw, dtb):
+    """delta' = softplus(dt_r · W_dt^T + bias) in fp64 (dt_r (..., R), dtw (D, R), dtb (D)), the sigmoid of its argument, and
+    delta''s first-order error bound in the fp32 kernels (before SAFETY)"""
+    pre = dtr @ dtw.t() + dtb
+    Tm = dtr.abs() @ dtw.abs().t() + dtb.abs()
+    dl = torch.nn.functional.softplus(pre)
+    sig = torch.sigmoid(pre)
+    return dl, sig, sig * (dtr.shape[-1] + 2) * U * Tm + SP * dl
+
+
+def delta_ref64(kind, xdbl, dtw, dtb, N):
+    """delta' (K, B, Lseq, D) at every position in fp64 and its per-element bound (SAFETY applied), for checking a kernel's delta'
+    on its own; xdbl (B, Lseq, K, Cp) and the weights as ss2d_fwd_ref64 takes them"""
+    f = lambda t: t.detach().double()
+    xdbl, dtw, dtb = f(xdbl), f(dtw), f(dtb)
+    Bt, Lseq, K, _ = xdbl.shape
+    D, R = dtw.shape[1], dtw.shape[2]
+    dl, bnd = (torch.empty((K, Bt, Lseq, D), dtype=torch.float64, device=xdbl.device) for _ in range(2))
+    for k, bs, kw, _ in walk_groups(kind, Bt):
+        dl[k, bs], _, e = _softplus64(xdbl[bs, :, k, 2 * N:2 * N + R], dtw[kw], dtb[kw])
+        bnd[k, bs] = SAFETY * e
+    return dl, bnd
+
+
+def delta_bound_bf16(ref_delta, bnd_delta):
+    """per-element bound of a delta' the kernel rounded to bf16, from the fp64 softplus and its fp32 bound (SAFETY applied)"""
+    return bnd_delta + BF16_RN * (ref_delta.abs() + bnd_delta)
+
+
+def ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, device=None, on_walk=None, delta=None):
     """The forward alone.  kind "cross4" / "seq2" / "cross"; xc (B, Lseq, D) fp32 or bf16, xdbl (B, Lseq, K, Cp) = [B | C | dt_r |
     padding], dtw (Kw, D, R), dtb (Kw, D), A (Kw·D, N), Ds (Kw·D), Kw = K or 2 (modalities) for "cross".  Returns (y, bound), float64
     (K, B, Lseq, D): direction k's output at the position it belongs to, and its per-element bound (SAFETY applied; with bf16 xc it
     includes the final rounding to bf16).
-    on_walk(g): called after each walk with its tensors (tiles, inputs, delta', the states at every step and their bounds); the
-    states are only kept when it is given.  ss2d_ref64 runs its backward from there."""
+    on_walk(g): called after each walk with its tensors (walk group, tiles, inputs, delta', the states at every step and their
+    bounds); the states are only kept when it is given.  ss2d_ref64 runs its backward from there.
+    delta (K, B, Lseq, D): the delta' to run the recurrence with instead of the softplus (taken as exact)."""
     bf16 = xc.dtype == torch.bfloat16
     dev = torch.device(device) if device is not None else xc.device
     f = lambda t: t.detach().to(dev, torch.float64)
@@ -187,6 +230,7 @@ def ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, device=None, on_walk=N
     z = lambda *s: torch.zeros(s, dtype=torch.float64, device=dev)
     y, ey = z(K, Bt, Lseq + 1, D), z(K, Bt, Lseq + 1, D)
     xcp, xdp = _pad(xc), _pad(xdbl)
+    dgiven = _pad(f(delta).flatten(0, 1)).view(K, Bt, Lseq + 1, D) if delta is not None else None
     for k, bs, kw, cs in walk_groups(kind, Bt):
         blk = torch.from_numpy(tiles[k]).to(dev)
         nb = blk.shape[0]
@@ -194,14 +238,16 @@ def ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, device=None, on_walk=N
         p = torch.where(blk >= 0, blk, torch.full_like(blk, Lseq))
         u = xcp[bs][:, p]                                                       # (b, nb, 16, D)
         xk = xdp[bs][:, p, k]
-        Bm, dtr = xk[..., :N], xk[..., 2 * N:2 * N + R]
+        Bm = xk[..., :N]
         Cm = xdp[cs][:, p, k, N:2 * N]
-        pre = dtr @ dtw[kw].t() + dtb[kw]
-        Tm = dtr.abs() @ dtw[kw].abs().t() + dtb[kw].abs()
-        dl = torch.nn.functional.softplus(pre) * m
-        sig = torch.sigmoid(pre)
-        edl = (sig * (R + 2) * U * Tm + SP * dl) * m
-        del Tm, dtr, xk
+        if dgiven is None:
+            dl, sig, edl = _softplus64(xk[..., 2 * N:2 * N + R], dtw[kw], dtb[kw])
+            dl, edl = dl * m, edl * m
+        else:
+            dl = dgiven[k, bs][:, p] * m
+            edl = torch.zeros_like(dl)
+            sig = -torch.expm1(-dl)
+        del xk
         Ak, Dk = A[kw * D:(kw + 1) * D], Ds[kw * D:(kw + 1) * D]
         dlu = dl * u
         absA = Ak.abs()
@@ -252,8 +298,8 @@ def ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, device=None, on_walk=N
         ey[k, bs].index_copy_(1, pf, eyk.reshape(b, nb * LT, D))
         del yk, eyk
         if keep:
-            on_walk(types.SimpleNamespace(k=k, nb=nb, m=m, p=p, pf=pf, u=u, Bm=Bm, Cm=Cm, dl=dl, edl=edl, sig=sig, Ak=Ak, Dk=Dk,
-                                          absA=absA, slot=slot, P=P, h0=h0, e0=e0, h_all=h_all, e_all=e_all))
+            on_walk(types.SimpleNamespace(k=k, bs=bs, kw=kw, cs=cs, nb=nb, m=m, p=p, pf=pf, u=u, Bm=Bm, Cm=Cm, dl=dl, edl=edl, sig=sig,
+                                          Ak=Ak, Dk=Dk, absA=absA, slot=slot, P=P, h0=h0, e0=e0, h_all=h_all, e_all=e_all))
             del h_all, e_all
     y, ey = y[:, :, :Lseq].contiguous(), ey[:, :, :Lseq] * SAFETY
     if bf16:
@@ -261,32 +307,41 @@ def ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, device=None, on_walk=N
     return y, ey.contiguous()
 
 
-def ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None):
-    """kind "cross4" / "seq2"; the inputs of ss2d_fwd_ref64 (fp32) and dy (B, Lseq, D).  Returns (ref, bound): two dicts of float64
-    tensors with keys y, delta, hs, dxc, ddelta, dB, dC, dA, dDs, ddtb.  y / delta / ddelta (K, B, Lseq, D), hs (K, B, max_tiles, D,
-    N), dB / dC (B, Lseq, K, N).  y and its bound are ss2d_fwd_ref64's, bit for bit."""
-    assert kind in ("cross4", "seq2"), "the fused backward covers CROSS4 and SEQ2"
+def ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None, delta=None, mistake=None):
+    """The inputs of ss2d_fwd_ref64 (fp32 xc) and dy (B, Lseq, D).  Returns (ref, bound): two dicts of float64 tensors with keys y,
+    delta, hs, dxc, ddelta, dB, dC, dA, dDs, ddtb.  y / delta / ddelta (K, B, Lseq, D), hs (K, B, max_tiles, D, N), dxc (B, Lseq, D),
+    dB / dC (B, Lseq, K, N), dA (Kw·D, N), dDs (Kw·D), ddtb (Kw, D).  y and its bound are ss2d_fwd_ref64's, bit for bit.
+    delta: as in ss2d_fwd_ref64; the forward and the backward both run on it (ref["delta"] is then the given one, bound 0).
+    mistake: one of MISTAKES (kind "cross")."""
+    assert mistake is None or (kind == "cross" and mistake in MISTAKES), mistake
     dev = torch.device(device) if device is not None else xc.device
     Bt, Lseq, D = xc.shape
-    K, N = xdbl.shape[2], A.shape[1]
+    K, N, Kw = xdbl.shape[2], A.shape[1], dtw.shape[0]
+    if mistake == "C_own":   # swap the halves' C columns: the forward then reads each image's own C
+        hb = Bt // 2
+        xdbl = xdbl.clone()
+        xdbl[:, :, :, N:2 * N] = torch.cat([xdbl[hb:, :, :, N:2 * N], xdbl[:hb, :, :, N:2 * N]])
     T = max(t.shape[0] for t in walk_tiles(kind, H, W))
     z = lambda *s: torch.zeros(s, dtype=torch.float64, device=dev)
     ref = dict(delta=z(K, Bt, Lseq + 1, D), hs=torch.full((K, Bt, T, D, N), math.nan, dtype=torch.float64, device=dev),
-               dxc=z(Bt, Lseq + 1, D), ddelta=z(K, Bt, Lseq + 1, D), dB=z(Bt, Lseq + 1, K, N), dC=z(Bt, Lseq + 1, K, N), dA=z(K * D, N),
-               dDs=z(K * D), ddtb=z(K, D))
+               dxc=z(Bt, Lseq + 1, D), ddelta=z(K, Bt, Lseq + 1, D), dB=z(Bt, Lseq + 1, K, N), dC=z(Bt, Lseq + 1, K, N), dA=z(Kw * D, N),
+               dDs=z(Kw * D), ddtb=z(Kw, D))
     bnd = {k: torch.zeros_like(v) for k, v in ref.items()}
     bnd["hs"].fill_(math.nan)
     dxc_mag = z(Bt, Lseq + 1, D)
     dyp = _pad(dy.detach().to(dev, torch.float64))
 
-    def backward(g):
-        k, nb, m, p, pf, u, Bm, Cm, dl, edl, sig = g.k, g.nb, g.m, g.p, g.pf, g.u, g.Bm, g.Cm, g.dl, g.edl, g.sig
-        Ak, Dk, absA, slot, P, h0, h_all, e_all = g.Ak, g.Dk, g.absA, g.slot, g.P, g.h0, g.h_all, g.e_all
-        sh = (Bt, nb, D, N)
-        put = lambda dst, src: dst.index_copy_(1, pf, src.reshape(Bt, nb * LT, *src.shape[3:]))
-        ref["hs"][k, :, :nb], bnd["hs"][k, :, :nb] = h0, g.e0
-        put(ref["delta"][k], dl); put(bnd["delta"][k], edl)
-        dyk = dyp[:, p]
+    def backward(wk):
+        k, bs, nb, m, p, pf, u, Bm, Cm, dl, edl, sig = wk.k, wk.bs, wk.nb, wk.m, wk.p, wk.pf, wk.u, wk.Bm, wk.Cm, wk.dl, wk.edl, wk.sig
+        Ak, Dk, absA, slot, P, h0, h_all, e_all = wk.Ak, wk.Dk, wk.absA, wk.slot, wk.P, wk.h0, wk.h_all, wk.e_all
+        ws = 1 - wk.kw if mistake == "wset" else wk.kw              # rows the weight set's sums go to
+        cdst = bs if mistake == "dC_own" else wk.cs                 # images whose dxdbl C columns receive dC
+        b = u.shape[0]
+        sh = (b, nb, D, N)
+        put = lambda dst, src: dst.index_copy_(1, pf, src.reshape(b, nb * LT, *src.shape[3:]))
+        ref["hs"][k, bs, :nb], bnd["hs"][k, bs, :nb] = h0, wk.e0
+        put(ref["delta"][k, bs], dl); put(bnd["delta"][k, bs], edl)
+        dyk = dyp[bs][:, p]
 
         # ---- backward: q = a·g entering each step from the right, and its error, tile by tile from the right ----
         def wslot(s):
@@ -308,22 +363,19 @@ def ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None):
         q, eq = q0, eq0
         dd_k, edd_k = torch.empty_like(u), torch.empty_like(u)
         du_k, edu_k, dum_k = torch.empty_like(u), torch.empty_like(u), torch.empty_like(u)
-        dB_k, dC_k = z(Bt, nb, LT, N), z(Bt, nb, LT, N)
-        edB_k, edC_k = z(Bt, nb, LT, N), z(Bt, nb, LT, N)
-        dA_k, edA_k = z(D, N), z(*sh)
-        dA_tot, dA_abs = z(*sh), z(*sh)
+        dB_k, dC_k, edB_k, edC_k = z(b, nb, LT, N), z(b, nb, LT, N), z(b, nb, LT, N), z(b, nb, LT, N)
+        dA_k, edA_k, dA_tot, dA_abs = z(D, N), z(*sh), z(*sh), z(*sh)
         gD = _gt(D)
         for s in range(LT - 1, -1, -1):
             a, rho, v, _ = slot(s)
-            w = wslot(s)
-            g = w + q
+            g = wslot(s) + q
             G = g.abs()
             eg = eq + U * G
             h, eh = h_all[:, :, s], e_all[:, :, s].double()
             hp = h_all[:, :, s - 1] if s > 0 else h0
             Mh, Mp = h.abs(), hp.abs()
             dys, us, ds, es = dyk[:, :, s, :, None], u[:, :, s, :, None], dl[:, :, s, :, None], edl[:, :, s, :, None]
-            Bs, Cs = Bm[:, :, s, None, :], Cm[:, :, s, None, :]
+            Bs = Bm[:, :, s, None, :]
             # dC = sum_d dy h,  dB = sum_d g delta' u
             dC_k[:, :, s] = (dys * h).sum(2)
             edC_k[:, :, s] = chan(dys.abs() * (eh + U * Mh)) + gD * (dys.abs() * Mh).sum(2)
@@ -357,23 +409,24 @@ def ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy, H, W, device=None):
             dA_abs += (t * ds).abs()
             edA_k += ds * et + tm * es + U * ds * tm
             q, eq = a * g, a * eg + a * rho * G + U * a * G
-        put(ref["ddelta"][k], dd_k * m); put(bnd["ddelta"][k], edd_k)
-        ref["dB"][:, :, k].index_copy_(1, pf, dB_k.reshape(Bt, nb * LT, N)); bnd["dB"][:, :, k].index_copy_(1, pf, edB_k.reshape(Bt, nb * LT, N))
-        ref["dC"][:, :, k].index_copy_(1, pf, dC_k.reshape(Bt, nb * LT, N)); bnd["dC"][:, :, k].index_copy_(1, pf, edC_k.reshape(Bt, nb * LT, N))
-        mm = m.expand_as(u).reshape(Bt, nb * LT, D)
-        ref["dxc"].index_add_(1, pf, (du_k.reshape(Bt, nb * LT, D) * mm))
-        bnd["dxc"].index_add_(1, pf, (edu_k.reshape(Bt, nb * LT, D) * mm))
-        dxc_mag.index_add_(1, pf, (dum_k.reshape(Bt, nb * LT, D) * mm))
-        ref["dA"][k * D:(k + 1) * D] = dA_k
-        bnd["dA"][k * D:(k + 1) * D] = tile_rss(edA_k) + _acc(dA_tot, dA_abs, Lseq)
+        put(ref["ddelta"][k, bs], dd_k * m); put(bnd["ddelta"][k, bs], edd_k)
+        put(ref["dB"][bs, :, k], dB_k); put(bnd["dB"][bs, :, k], edB_k)
+        put(ref["dC"][cdst, :, k], dC_k); put(bnd["dC"][cdst, :, k], edC_k)
+        mm = m.expand_as(u).reshape(b, nb * LT, D)
+        ref["dxc"][bs].index_add_(1, pf, du_k.reshape(b, nb * LT, D) * mm)
+        bnd["dxc"][bs].index_add_(1, pf, edu_k.reshape(b, nb * LT, D) * mm)
+        dxc_mag[bs].index_add_(1, pf, dum_k.reshape(b, nb * LT, D) * mm)
+        rows = slice(ws * D, (ws + 1) * D)
+        ref["dA"][rows] = dA_k
+        bnd["dA"][rows] = tile_rss(edA_k) + _acc(dA_tot, dA_abs, Lseq)
         dyu = dyk * u
-        ref["dDs"][k * D:(k + 1) * D] = dyu.sum((0, 1, 2))
-        bnd["dDs"][k * D:(k + 1) * D] = U * dyu.abs().sum((0, 1, 2)) + _acc(dyu.sum(2), dyu.abs().sum(2), Lseq)
+        ref["dDs"][rows] = dyu.sum((0, 1, 2))
+        bnd["dDs"][rows] = U * dyu.abs().sum((0, 1, 2)) + _acc(dyu.sum(2), dyu.abs().sum(2), Lseq)
         dd_k *= m
-        ref["ddtb"][k] = dd_k.sum((0, 1, 2))
-        bnd["ddtb"][k] = tile_rss(edd_k.sum(2)) + _acc(dd_k.sum(2), (dd_k.abs() + edd_k).sum(2), Lseq)
+        ref["ddtb"][ws] = dd_k.sum((0, 1, 2))
+        bnd["ddtb"][ws] = tile_rss(edd_k.sum(2)) + _acc(dd_k.sum(2), (dd_k.abs() + edd_k).sum(2), Lseq)
 
-    y, ey = ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, device=dev, on_walk=backward)
+    y, ey = ss2d_fwd_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, H, W, device=dev, on_walk=backward, delta=delta)
     bnd["dxc"] += K * U * dxc_mag
     for key in ("delta", "dxc", "ddelta", "dB", "dC"):
         sl = (slice(None), slice(0, Lseq)) if key in ("dxc", "dB", "dC") else (slice(None), slice(None), slice(0, Lseq))

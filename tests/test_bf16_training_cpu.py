@@ -3,10 +3,6 @@
 * the forward planner reports the plan of sigma_ss2d_scan_fwd_save_bf16 (bf16 = 2) and refuses d_state 8 there; the backward's plan does
   not depend on the element type;
 * argument validation of the new pair returns its codes before any CUDA call;
-* the fp64 reference on a given delta' (tests/ss2d_delta_ref64.py): with the reference's own delta' it changes nothing beyond the delta' error terms it
-  drops, and with a bf16-rounded delta' every output matches fp64 autograd through a restatement of the op that runs on that delta'
-  with the rounding passed straight through and the softplus derivative taken from the rounded value (the gradient the backward
-  kernel computes);
 * the switch: default off, the context manager restores it;
 * `cuobjdump -sass` of the built library: the fp32 training-forward / backward kernels and the bf16 inference kernels are still there
   under their names, and the bf16 training kernels are separate symbols."""
@@ -16,11 +12,6 @@ import subprocess
 import pytest
 import torch
 
-import procedural as P
-import ss2d_delta_ref64 as RD
-from oracle import ss2d_ref64 as R64
-
-S = 131
 NEW = ("sigma_ss2d_scan_fwd_save_bf16", "sigma_ss2d_scan_bwd_saved_bf16", "sigma_layernorm_fwd_bf16io", "sigma_layernorm_bwd_bf16")
 
 
@@ -82,101 +73,6 @@ def test_switch_is_off_by_default_and_restored():
         assert ops.BF16_TRAINING_CORE is True
     assert ops.BF16_TRAINING_CORE is False
     assert train_util.TrainStep(None, None).bf16_core is False
-
-
-def _inputs(kind, B, H, W, D, N, R, tag):
-    K = R64.KINDS[kind]
-    Lseq = H * W * (2 if kind == "seq2" else 1)
-    Cp = 2 * N + R + 3
-    bf = lambda t: t.bfloat16().float()
-    xc = bf(P.randn(S, tag + "/xc", (B, Lseq, D)))
-    xdbl = P.randn(S, tag + "/xdbl", (B, Lseq, K, Cp))
-    xdbl[..., 2 * N + R:] = 0.0
-    dtw = P.rand(S, tag + "/dtw", (K, D, R), -R ** -0.5, R ** -0.5)
-    dt = torch.exp(P.rand(S, tag + "/dt", (K, D), -6.9, -2.3))
-    dtb = dt + torch.log(-torch.expm1(-dt))
-    A = -torch.arange(1, N + 1, dtype=torch.float32).repeat(K * D, 1) * P.rand(S, tag + "/A", (K * D, N), 0.8, 1.25)
-    Ds = P.randn(S, tag + "/Ds", (K * D,), 0.1, 1.0)
-    dy = bf(P.randn(S, tag + "/dy", (B, Lseq, D)))
-    return xc, xdbl, dtw, dtb, A, Ds, dy
-
-
-class _SoftplusRounded(torch.autograd.Function):
-    """softplus rounded to bf16; backward as the kernel forms it: the derivative 1 - exp(-delta') of the ROUNDED delta', the
-    rounding itself passed straight through"""
-
-    @staticmethod
-    def forward(ctx, x):
-        dl = torch.nn.functional.softplus(x).float().bfloat16().double()
-        ctx.save_for_backward(dl)
-        return dl
-
-    @staticmethod
-    def backward(ctx, g):
-        return g * -torch.expm1(-ctx.saved_tensors[0])
-
-
-def _literal(kind, xc, xdbl, dtw, dtb, A, Ds, dy, H, W):
-    """the op restated on a delta' rounded to bf16 before use: per direction gather, a loop over the walk, scatter; fp64 autograd"""
-    t = [v.double().clone().requires_grad_(True) for v in (xc, xdbl, dtw, dtb, A, Ds)]
-    xc_, xdbl_, dtw_, dtb_, A_, Ds_ = t
-    Bt, Lseq, D = xc.shape
-    N, R = A.shape[1], dtw.shape[2]
-    total, pres, deltas = 0.0, [], []
-    for k, idx in enumerate(R64.dir_index(kind, H, W)):
-        u, xk = xc_[:, idx], xdbl_[:, idx, k]
-        pre = xk[..., 2 * N:2 * N + R] @ dtw_[k].t() + dtb_[k]
-        pre.retain_grad()
-        dl = _SoftplusRounded.apply(pre)
-        Ak, Dk = A_[k * D:(k + 1) * D], Ds_[k * D:(k + 1) * D]
-        h = torch.zeros(Bt, D, N, dtype=torch.float64)
-        ys = []
-        for l in range(Lseq):
-            h = torch.exp(dl[:, l, :, None] * Ak) * h + (dl[:, l] * u[:, l])[..., None] * xk[:, l, None, :N]
-            ys.append((h * xk[:, l, None, N:2 * N]).sum(-1) + Dk * u[:, l])
-        yk = torch.stack(ys, 1)
-        total = total + (yk * dy.double()[:, idx]).sum()
-        inv = torch.empty(Lseq, dtype=torch.long)
-        inv[torch.from_numpy(idx.copy())] = torch.arange(Lseq)
-        pres.append((pre, inv))
-        deltas.append(dl.detach()[:, inv])
-    total.backward()
-    return t, pres, torch.stack(deltas)
-
-
-@pytest.mark.parametrize("kind,H,W,N", [("cross4", 5, 7, 16), ("seq2", 5, 7, 4), ("cross4", 17, 3, 4)])
-def test_oracle_with_a_given_delta_matches_autograd(kind, H, W, N):
-    B, D, R = 2, 8, 3
-    args = _inputs(kind, B, H, W, D, N, R, f"bf16train/{kind}/{H}x{W}/N{N}")
-    (xc_, xdbl_, dtw_, dtb_, A_, Ds_), pres, delta = _literal(kind, *args, H, W)
-    plain, pb = R64.ss2d_ref64(kind, *args, H, W)
-    # the rounded delta' lies inside the bound the GPU test holds the kernel's delta' to
-    assert R64.bound_fraction(delta, plain["delta"], RD.delta_bound_bf16(plain["delta"], pb["delta"])) <= 1.0
-    assert float((delta - plain["delta"]).abs().max()) > 0                        # and the rounding is really there
-    ref, bnd = RD.ss2d_ref64(kind, *args, H, W, delta=delta)
-    assert torch.equal(ref["delta"], delta) and float(bnd["delta"].abs().max()) == 0.0
-    close = lambda a, b: float((a - b).abs().max()) <= 1e-11 * (1.0 + float(b.abs().max()))
-    assert close(ref["dxc"], xc_.grad)
-    assert close(ref["dB"], xdbl_.grad[..., :N]) and close(ref["dC"], xdbl_.grad[..., N:2 * N])
-    assert close(ref["dA"], A_.grad) and close(ref["dDs"], Ds_.grad) and close(ref["ddtb"], dtb_.grad)
-    for k, (pre, inv) in enumerate(pres):
-        assert close(ref["ddelta"][k], pre.grad[:, inv]), k
-    # the bounds only lose the delta' error terms
-    for key in ("y", "dxc", "ddelta", "dA"):
-        assert bool((bnd[key] >= 0).all()) and float(bnd[key].max()) <= 1.5 * float(pb[key].max()), key
-
-
-def test_given_own_delta_changes_nothing():
-    args = _inputs("cross4", 2, 5, 7, 8, 4, 3, "bf16train/self")
-    plain, _ = R64.ss2d_ref64("cross4", *args, 5, 7)
-    again, _ = RD.ss2d_ref64("cross4", *args, 5, 7, delta=plain["delta"])
-    for key in ("y", "dxc", "dB", "dC", "dA", "dDs"):
-        assert float((again[key] - plain[key]).abs().max()) <= 1e-12 * (1.0 + float(plain[key].abs().max())), key
-    # and without a delta' the module is the oracle, values and bounds, bit for bit
-    same, sb = RD.ss2d_ref64("cross4", *args, 5, 7)
-    _, pb = R64.ss2d_ref64("cross4", *args, 5, 7)
-    for key in plain:
-        assert torch.equal(same[key].nan_to_num(7.0), plain[key].nan_to_num(7.0)) and torch.equal(sb[key].nan_to_num(7.0), pb[key].nan_to_num(7.0)), key
 
 
 @pytest.fixture(scope="module")

@@ -7,7 +7,10 @@
   every plan is launchable — grid within the tile count, 2-8 ring stages, shared memory within the H100's limits.
 * the fused scan forward's whole launch plan (through sigma_test_ss2d_fwd_plan) at every Sigma inference shape and 1, 2, 8 and 74
   images: segments capped at 32 and never empty for the longest walk by choice, one segment without a workspace, the 4-CTA register
-  budget only where it is built and chosen, a ring of 2-8 stages whose shared memory fits the CTAs the budget puts on an SM."""
+  budget only where it is built and chosen, a ring of 2-8 stages whose shared memory fits the CTAs the budget puts on an SM.
+* the fused scan backward's plan for kind CROSS (sigma_test_ss2d_bwd_plan), its state and workspace sizes at every CroMB training
+  shape and 1, 2, 3, 8 images, and the rejection of an odd batch."""
+import ctypes
 import os
 import re
 
@@ -377,3 +380,41 @@ def test_op_scan_plan_segments(monkeypatch):
         scan_plan("bwd", 2, 192, 19200, 4, 1, ws_bytes=0)
     # the drop-in CroMB stage-0 call runs L-segments by default, forward and backward
     assert scan_plan("fwd", 2, 192, 19200, 4, 1)["nsplit"] > 1 and scan_plan("bwd", 2, 192, 19200, 4, 1)["nsplit"] > 1
+
+
+# CroMB's training shapes (one block per encoder stage; d_inner = 2·C): Sigma-tiny / small at 480 x 640 and Sigma-base at 720 x 960
+CROMB = [(120, 160, 192, 6), (60, 80, 384, 12), (30, 40, 768, 24), (15, 20, 1536, 48), (180, 240, 256, 8), (23, 30, 2048, 64)]
+
+
+def _lib():
+    from sigma_b200 import _lib
+    return _lib
+
+
+@pytest.mark.parametrize("H,W,D,R", CROMB)
+@pytest.mark.parametrize("images", [1, 2, 3, 8])
+def test_cross_backward_plan_and_sizes(H, W, D, R, images):
+    L_, lib = _lib().lib(), _lib()
+    Bt, N, L = 2 * images, 4, H * W
+    tiles = -(-L // 16)
+    for force in (0, 1, 2, 7, 64, 100):
+        out = (ctypes.c_int64 * 4)()
+        lib.check(L_.sigma_test_ss2d_bwd_plan(lib.DIRS_CROSS, Bt, H, W, D, N, force, out), "sigma_test_ss2d_bwd_plan")
+        nsplit, tps, mx, mn = (int(v) for v in out)
+        assert mx == mn == tiles                                          # one row-major walk of ceil(L / 16) tiles
+        assert 1 <= nsplit <= 64 and nsplit * tps >= tiles and (nsplit - 1) * tps < tiles, (force, nsplit, tps)
+        if force:
+            assert nsplit == len(range(0, tiles, -(-tiles // min(force, 64, tiles))))
+    hsb = L_.sigma_ss2d_scan_hs_bytes(lib.DIRS_CROSS, Bt, H, W, D, N)
+    assert hsb == Bt * tiles * D * N * 4
+    assert L_.sigma_ss2d_scan_bwd_workspace_bytes(lib.DIRS_CROSS, Bt, H, W, D, N) >= hsb
+    assert L_.sigma_ss2d_scan_bwd_det_workspace_bytes(lib.DIRS_CROSS, Bt, H, W, D, N) == 0     # no deterministic build
+
+
+def test_cross_backward_rejects_an_odd_batch():
+    L_, lib = _lib().lib(), _lib()
+    out = (ctypes.c_int64 * 4)()
+    assert L_.sigma_test_ss2d_bwd_plan(lib.DIRS_CROSS, 3, 30, 40, 768, 4, 0, out) != 0
+    assert L_.sigma_test_ss2d_bwd_plan(lib.DIRS_CROSS, 4, 30, 40, 768, 4, 0, out) == 0
+    assert L_.sigma_ss2d_scan_hs_bytes(lib.DIRS_CROSS, 3, 30, 40, 768, 4) == 0
+    assert L_.sigma_ss2d_scan_bwd_workspace_bytes(lib.DIRS_CROSS, 3, 30, 40, 768, 4) == 0

@@ -1,15 +1,13 @@
 """GPU: the bf16 training mode of the fused core (sigma_ss2d_scan_fwd_save_bf16 + sigma_ss2d_scan_bwd_saved_bf16, LayerNormFn on bf16
 activations) against fp64.
-* The C-ABI pair, element by element inside the per-element bounds of oracle/ss2d_ref64.py, whose error model tests/ss2d_delta_ref64.py applies to a
-  given delta'.  Inputs are drawn, then xc and dy are
-  rounded to bf16, so the reference sees the exact values.  The kernel's delta' is checked on its own against the fp64 softplus
-  inside `fp32 bound + 2^-8·|delta'|`; everything downstream is checked against the reference run on THAT delta' (`delta=`), so a
+* The C-ABI pair, element by element inside the per-element bounds of oracle/ss2d_ref64.py run on a given delta'.  Inputs are
+  drawn, then xc and dy are rounded to bf16, so the reference sees the exact values.  The kernel's delta' is checked on its own
+  against the fp64 softplus inside `fp32 bound + 2^-8·|delta'|`; everything downstream is checked against the reference run on THAT delta' (`delta=`), so a
   rounding tie never turns into a false failure and nothing is loosened.  Kinds cross4 / seq2 at d_state 4 and 16, every padded
   dt_rank Sigma trains with, ragged maps, batch 1 / 2 / 3, L-segments 1, 2, 7, the library's choice, the cap, and a forward cut
   differently from its backward; outputs inside NaN-filled guards; the dt_r and padding columns of dxdbl 0.
-* Kind cross (CroMB) the same way, element by element: delta' against the softplus, everything else against
-  tests/ss2d_cross_ref64.py run on the kernel's delta' (delta=), at CroMB's training shapes at d_state 4 with 1-3 images
-  (test_ss2d_cross_bwd_fp64_gpu.CASES) and at d_state 16.
+* Kind cross (CroMB) the same way, element by element, at CroMB's training shapes at d_state 4 with 1-3 images
+  (test_ss2d_bwd_fp64_gpu.CROSS_CASES) and at d_state 16.
 * FusedSS2DCore.apply with the switch on under bf16 autocast: bf16 output, bf16 saved xc and delta', the saved bytes, all six
   gradients against the fp64 chain (kind cross chained per modality half); with the switch off, and under the deterministic
   switch, the fp32 entry points run.
@@ -21,34 +19,18 @@ import torch
 
 import procedural as P
 from helpers import guard_ok as _guard_ok, guarded as _guarded, ptr as _p, record, ss2d_kind as _kid, ss2d_params, stream as _stream
-import ss2d_delta_ref64 as RD
 from oracle import ss2d_ref64 as R64
-from test_ss2d_cross_bwd_fp64_gpu import CASES as CROSS_CASES          # (H, W, D, R, images) of CroMB's training shapes
+from test_ss2d_bwd_fp64_gpu import CROSS_CASES
 
 pytestmark = pytest.mark.gpu
 S = 211
 BF = torch.bfloat16
 
 
-def _delta_ref(kind, xdbl, dtw, dtb, N, R):
+def _delta_ref(kind, xdbl, dtw, dtb, N):
     """fp64 softplus(dt_proj) slabs (K, B, Lseq, D) and the bound of a kernel delta' rounded to bf16"""
-    Bt, Lseq, K, _ = xdbl.shape
-    ref, bnd = [], []
-    for k in range(K):
-        dtr = xdbl[:, :, k, 2 * N:2 * N + R].double()
-        if kind == "cross":
-            w = torch.arange(Bt, device=xdbl.device) >= Bt // 2
-            Wk, bk = dtw.double()[w.long()], dtb.double()[w.long()][:, None]           # (Bt, D, R), (Bt, 1, D)
-            pre = torch.einsum("blr,bdr->bld", dtr, Wk) + bk
-            Tm = torch.einsum("blr,bdr->bld", dtr.abs(), Wk.abs()) + bk.abs()
-        else:
-            pre = dtr @ dtw[k].double().t() + dtb[k].double()
-            Tm = dtr.abs() @ dtw[k].double().abs().t() + dtb[k].double().abs()
-        dl = torch.nn.functional.softplus(pre)
-        e32 = R64.SAFETY * (torch.sigmoid(pre) * (R + 2) * R64.U * Tm + R64.SP * dl)
-        ref.append(dl)
-        bnd.append(RD.delta_bound_bf16(dl, e32))
-    return torch.stack(ref), torch.stack(bnd)
+    ref, bnd = R64.delta_ref64(kind, xdbl, dtw, dtb, N)
+    return ref, R64.delta_bound_bf16(ref, bnd)
 
 
 def _check(tag, name, got, ref, bnd, worst):
@@ -110,7 +92,7 @@ def test_bf16_pair_matches_fp64(kind, B, H, W, D, N, R):
     tag = f"{kind}/{B}/{H}x{W}/D{D}/N{N}/R{R}"
     args16, Cp = _args16(kind, B, H, W, D, N, R, tag)
     xc, xdbl, dtw, dtb, A, Ds, dy = args16
-    dref, dbnd = _delta_ref(kind, xdbl, dtw, dtb, N, R)
+    dref, dbnd = _delta_ref(kind, xdbl, dtw, dtb, N)
     worst, refs = {}, {}
     for fs, bs in SPLITS:
         t = f"{tag} fwd={fs} bwd={bs}"
@@ -119,7 +101,7 @@ def test_bf16_pair_matches_fp64(kind, B, H, W, D, N, R):
         key = outs["delta"].view(torch.int16).clone()
         hit = [v for kk, v in refs.values() if torch.equal(kk, key)]       # delta' does not depend on the cut: one reference run
         if not hit:
-            refs[fs] = (key, RD.ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy.float(), H, W, delta=outs["delta"].double()))
+            refs[fs] = (key, R64.ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy.float(), H, W, delta=outs["delta"].double()))
             hit = [refs[fs][1]]
         ref, bnd = hit[0]
         for name in ("y", "hs", "dxc", "ddelta", "dA", "dDs", "ddtb"):
@@ -135,18 +117,17 @@ def test_bf16_pair_matches_fp64(kind, B, H, W, D, N, R):
 
 
 # Bt = 2·images, H, W, D, N, R: CroMB's training shapes at d_state 4 with 1-3 images, and two d_state 16 cases
-CROSS = [(2 * im, H, W, D, 4, R) for H, W, D, R, im in CROSS_CASES] + [(2, 60, 80, 384, 16, 12), (4, 23, 30, 192, 16, 6)]
+CROSS = [(B, H, W, D, N, R) for _, B, H, W, D, N, R in CROSS_CASES] + [(2, 60, 80, 384, 16, 12), (4, 23, 30, 192, 16, 6)]
 
 
 @pytest.mark.parametrize("B,H,W,D,N,R", CROSS)
 def test_bf16_pair_cross(B, H, W, D, N, R):
-    """kind cross: delta' against the fp64 softplus; every other output element by element against tests/ss2d_cross_ref64.py run on
-    the kernel's saved delta' (one reference: delta' must not depend on the L-segment cut)"""
-    from ss2d_cross_ref64 import ss2d_cross_ref64
+    """kind cross: delta' against the fp64 softplus; every other output element by element against the reference run on the
+    kernel's saved delta' (one reference: delta' must not depend on the L-segment cut)"""
     kind, tag = "cross", f"cross/{B}/{H}x{W}/D{D}/N{N}/R{R}"
     args16, Cp = _args16(kind, B, H, W, D, N, R, tag)
     xc, xdbl, dtw, dtb, A, Ds, dy = args16
-    dref, dbnd = _delta_ref(kind, xdbl, dtw, dtb, N, R)
+    dref, dbnd = _delta_ref(kind, xdbl, dtw, dtb, N)
     worst, key, ref = {}, None, None
     for fs, bs in [(0, 0), (1, 1), (3, 7), (100, 100)]:
         t = f"{tag} fwd={fs} bwd={bs}"
@@ -154,7 +135,7 @@ def test_bf16_pair_cross(B, H, W, D, N, R):
         _check(t, "delta", outs["delta"], dref, dbnd, worst)
         if key is None:
             key = outs["delta"].view(torch.int16).clone()
-            ref, bnd = ss2d_cross_ref64(xc, xdbl, dtw, dtb, A, Ds, dy.float(), H, W, delta=outs["delta"].double())
+            ref, bnd = R64.ss2d_ref64(kind, xc, xdbl, dtw, dtb, A, Ds, dy.float(), H, W, delta=outs["delta"].double())
         assert torch.equal(outs["delta"].view(torch.int16), key), f"{t}: delta' depends on the L-segment cut"
         for name in ("y", "hs", "dxc", "ddelta", "dA", "dDs", "ddtb"):
             _check(t, name, outs[name], ref[name], bnd[name], worst)
@@ -175,7 +156,6 @@ def _bf(t):
                                                ("cross", 4, 30, 40, 768, 4, 24)])
 def test_fused_core_autograd_bf16_mode(kind, B, H, W, D, N, R, monkeypatch):
     from sigma_b200 import _lib, fused, ops
-    from ss2d_cross_ref64 import ss2d_cross_ref64
     from test_ss2d_bwd_fp64_gpu import core_chain64, core_xdbl
     monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
     K = {"cross4": 4, "seq2": 2, "cross": 1}[kind]            # x_dbl rows per position
@@ -231,10 +211,7 @@ def test_fused_core_autograd_bf16_mode(kind, B, H, W, D, N, R, monkeypatch):
     with torch.no_grad():
         xdbl, xw = core_xdbl(kind, xc0, xpw, N, R, Cp)                # the forward's own x_proj GEMM calls
         A = -torch.exp(Al)
-        if kind == "cross":
-            ref, _ = ss2d_cross_ref64(xc0, xdbl, dtw, dtb, A, Ds, wgt, H, W, delta=slabs[0].double())
-        else:
-            ref, _ = RD.ss2d_ref64(kind, xc0, xdbl, dtw, dtb, A, Ds, wgt, H, W, delta=slabs[0].double())
+        ref, _ = R64.ss2d_ref64(kind, xc0, xdbl, dtw, dtb, A, Ds, wgt, H, W, delta=slabs[0].double())
         want, _ = core_chain64(kind, ref, None, xc0, xdbl, xw, dtw, N, R, Cp)
         want[4] = want[4] * A.double()
         dxc = want[0]
