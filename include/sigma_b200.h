@@ -80,8 +80,11 @@ int sigma_scan_fwd(const void *u, const void *delta, const float *A, const void 
  * Replaces `selective_scan_cuda_core.bwd(u, delta, A, B, C, D, delta_bias, dout, x,
  * delta_softplus, nrows) -> [du, ddelta, dA, dB, dC, dD, ddelta_bias]`
  * (selective_scan.cpp:251-362, selective_scan_bwd_kernel.cuh:68-274).
- * All tensors contiguous (d_state <= 16), fp16 / bf16 natively.  `workspace` holds the forward states of the recompute sweep
- * (one every 16 positions) and the L-segment carries of both directions;
+ * All tensors contiguous, d_state <= 256, fp16 / bf16 natively.  `workspace` holds the forward states of the recompute sweep
+ * (one every 16 positions) and the L-segment carries of both directions;  for 16 < d_state <= 256 ONE deterministic kernel
+ * (no float atomics; csrc/scan_op_bwd_wide.cu) serves sigma_scan_bwd, sigma_scan_bwd_split and sigma_scan_bwd_det alike: no
+ * L-segments (nsplit has no effect), the same bits from all three, and the workspace (the same size from both queries) holds
+ * the states at every 32-position tile and the partial sums;
  * the reference's `x` is not needed.  du, ddelta: (batch, dim, seqlen) in `dtype`; dA (dim, dstate),
  * dD, ddelta_bias (dim) fp32 — OVERWRITTEN (not accumulated); dB, dC (batch, ngroups, dstate,
  * seqlen) fp32, overwritten.  dD / ddelta_bias may be NULL when D / delta_bias are NULL.

@@ -279,8 +279,18 @@ int sigma_test_scan_plan(int sweep, int batch, int dim, int seqlen, int dstate, 
                       ngroups > 0 && dim % ngroups == 0 && nsplit >= 0 &&
                       (dtype == SIGMA_F32 || dtype == SIGMA_F16 || dtype == SIGMA_BF16),
                   "sigma_test_scan_plan: bad arguments");
+  if (sweep > 0 && dstate > 16) {   // the wide-state kernel: one walk per CTA after a serial state sweep, both sweeps alike
+    const size_t need = sigma_scan_bwd_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype);
+    if (workspace_bytes < need) {
+      set_error("sigma_scan_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+      return SIGMA_EWORKSPACE;
+    }
+    const ScanOpPlan main = scan_op_bwd_wide_plan(seqlen), state = scan_op_fwd_generic_plan(batch, dim, seqlen, dstate, ngroups, false, 1);
+    const long long v[8] = {ROUTE_GENERIC, main.nsplit, main.tiles_per_split, main.ntiles, main.DT, main.nst, state.nsplit, state.tiles_per_split};
+    for (int i = 0; i < 8; ++i) out8_host[i] = v[i];
+    return SIGMA_OK;
+  }
   if (sweep > 0) {   // what scan_bwd_entry checks before it dispatches
-    if (dstate > 16) { set_error("sigma_scan_bwd: d_state=%d > 16 is not supported by the backward kernels", dstate); return SIGMA_EUNSUPPORTED; }
     const size_t base = sigma_scan_bwd_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype);
     const size_t need = sweep == 2 ? sigma_scan_bwd_det_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype) : base;
     if (workspace_bytes < need) {
@@ -736,6 +746,7 @@ int sigma_scale_add_fwd(const float *a, const float *sa, const float *b, const f
 }
 
 size_t sigma_scan_bwd_workspace_bytes(int batch, int dim, int seqlen, int dstate, int ngroups, int dtype) {
+  if (dstate > 16) return scan_op_bwd_wide_workspace_bytes(batch, dim, seqlen, dstate, ngroups);   // 0 beyond 256
   const int eb = dtype == SIGMA_F32 ? 4 : 2;
   size_t w = align256(std::max(scan_op_bwd_workspace_bytes(batch, dim, seqlen, dstate, eb),
                                scan_op_bwd_tma_workspace_bytes(batch, dim, seqlen, std::min(dstate, 16), eb)));
@@ -745,6 +756,7 @@ size_t sigma_scan_bwd_workspace_bytes(int batch, int dim, int seqlen, int dstate
 
 // the deterministic build appends the partials of whichever kernel runs (TMA-staged or generic) to the workspace
 size_t sigma_scan_bwd_det_workspace_bytes(int batch, int dim, int seqlen, int dstate, int ngroups, int dtype) {
+  if (dstate > 16) return scan_op_bwd_wide_workspace_bytes(batch, dim, seqlen, dstate, ngroups);   // one kernel for both builds
   if (batch <= 0 || dim <= 0 || seqlen <= 0 || dstate <= 0 || dstate > 16 || ngroups <= 0 || dim % ngroups) return 0;
   return align256(sigma_scan_bwd_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype)) +
          std::max(scan_op_bwd_tma_det_bytes(batch, dim, seqlen, dstate, ngroups), scan_op_bwd_det_bytes(batch, dim, seqlen, dstate, ngroups));
@@ -761,12 +773,22 @@ static int scan_bwd_entry(const void *u, const void *delta, const float *A, cons
   SIGMA_CHECK_ARG(batch > 0 && dim > 0 && seqlen > 0 && dstate > 0 && ngroups > 0 && dim % ngroups == 0,
                   "sigma_scan_bwd: bad sizes (batch=%d dim=%d seqlen=%d dstate=%d ngroups=%d)", batch, dim, seqlen, dstate, ngroups);
   SIGMA_CHECK_ARG(dtype == SIGMA_F32 || dtype == SIGMA_F16 || dtype == SIGMA_BF16, "sigma_scan_bwd: unknown dtype %d", dtype);
-  if (dstate > 16) { set_error("sigma_scan_bwd: d_state=%d > 16 is not supported by the backward kernels", dstate); return SIGMA_EUNSUPPORTED; }
+  if (dstate > 256) { set_error("sigma_scan_bwd: d_state=%d > 256 is not supported (selective_scan.cpp:290)", dstate); return SIGMA_EUNSUPPORTED; }
   const size_t need = det ? sigma_scan_bwd_det_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype)
                           : sigma_scan_bwd_workspace_bytes(batch, dim, seqlen, dstate, ngroups, dtype);
   if (workspace == nullptr || workspace_bytes < need) {
     set_error("sigma_scan_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
     return SIGMA_EWORKSPACE;
+  }
+  if (dstate > 16) {   // one deterministic kernel for every entry point; nsplit has no effect (scan_op_bwd_wide.cu)
+    if (dtype == SIGMA_F32)
+      return scan_op_bwd_wide<float>(u, delta, A, B, C, D, delta_bias, dout, du, ddelta, dA, dB, dC, dD, ddelta_bias, batch, dim, seqlen,
+                                     dstate, ngroups, delta_softplus, workspace, workspace_bytes, stream);
+    if (dtype == SIGMA_F16)
+      return scan_op_bwd_wide<__half>(u, delta, A, B, C, D, delta_bias, dout, du, ddelta, dA, dB, dC, dD, ddelta_bias, batch, dim,
+                                      seqlen, dstate, ngroups, delta_softplus, workspace, workspace_bytes, stream);
+    return scan_op_bwd_wide<__nv_bfloat16>(u, delta, A, B, C, D, delta_bias, dout, du, ddelta, dA, dB, dC, dD, ddelta_bias, batch, dim,
+                                           seqlen, dstate, ngroups, delta_softplus, workspace, workspace_bytes, stream);
   }
   void *det_ws = nullptr;
   if (det) {   // the kernels see only the plain workspace; the partials follow it

@@ -133,6 +133,14 @@ int scan_op_bwd_tma(const void *u, const void *delta, const float *A, const void
                     float *dbias, int batch, int dim, int L, int N, int G, int softplus, void *ws, size_t ws_bytes,
                     int force_split, cudaStream_t stream, void *det_ws);
 
+// ---- scan_op_bwd_wide.cu: op-level scan backward for 16 < d_state <= 256 (deterministic, every entry point) ----
+size_t scan_op_bwd_wide_workspace_bytes(int batch, int dim, int L, int N, int G);   // 0 for a call it does not take
+ScanOpPlan scan_op_bwd_wide_plan(int L);
+template <typename T>
+int scan_op_bwd_wide(const void *u, const void *delta, const float *A, const void *B, const void *C, const float *D, const float *bias,
+                     const void *dout, void *du, void *ddelta, float *dA, float *dB, float *dC, float *dD, float *dbias, int batch,
+                     int dim, int L, int N, int G, int softplus, void *ws, size_t ws_bytes, cudaStream_t stream);
+
 // ---- det_reduce.cu ----
 int sum_parts_det_launch(const float *part, int nparts, long long ncols, long long inner, long long ostride, float *out, cudaStream_t stream);
 int upsample_bilinear_bwd_launch(const float *dy, float *dx, int batch, int C, int Hin, int Win, int Hout, int Wout, float rh, float rw,

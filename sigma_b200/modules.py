@@ -89,6 +89,16 @@ def _fused_ok(*tensors):
     return all(t.dtype == torch.float32 for t in tensors)
 
 
+FUSED_SCAN_STATES = (4, 8, 16)   # the d_state values the fused channels-last scan is built for
+
+
+def _fused_block_ok(op, *tensors):
+    """The fused inference path of a Mamba block (SS2D, ConMB_SS2D, CrossMambaFusion_SS2D_SSM and the blocks around them): taken
+    under _fused_ok when the block's scan `op` has a d_state the fused scan is built for; any other d_state (d_state="auto" at
+    most widths) runs the composed path, as under composed_path()."""
+    return _fused_ok(*tensors) and op.d_state in FUSED_SCAN_STATES
+
+
 # --------------------------------------------------------------------------------------------
 # SSM parameter initialisers (vmamba.py:728-782; identical in SS2D / ConMB_SS2D / CMA_SSM)
 # --------------------------------------------------------------------------------------------
@@ -190,7 +200,7 @@ class SS2D(nn.Module):
     forward_corev2 = forward_core
 
     def forward(self, x, residual=None, **kwargs):
-        if _fused_ok(x) and isinstance(self.dropout, nn.Identity):
+        if _fused_block_ok(self, x) and isinstance(self.dropout, nn.Identity):
             from . import fused
             return fused.ss2d(self, x, residual=residual)
         xz = self.in_proj(x)
@@ -259,7 +269,7 @@ class ConMB_SS2D(nn.Module):
             self.out_norm1, self.out_norm2, nrows=nrows)
 
     def forward(self, x_rgb, x_e, residual=None):
-        if _fused_ok(x_rgb, x_e) and isinstance(self.dropout, nn.Identity):
+        if _fused_block_ok(self, x_rgb, x_e) and isinstance(self.dropout, nn.Identity):
             from . import fused
             return fused.conmb_ss2d(self, x_rgb, x_e, residual=residual)
         t_r = self.in_proj(x_rgb).permute(0, 3, 1, 2).contiguous()
@@ -354,7 +364,7 @@ class CrossMambaFusion_SS2D_SSM(nn.Module):
                                                  dt_scale=dt_scale, dt_init_floor=dt_init_floor, **kwargs)
 
     def forward(self, x_rgb, x_e, residual=False):
-        if _fused_ok(x_rgb, x_e) and isinstance(self.dropout_rgb, nn.Identity):
+        if _fused_block_ok(self, x_rgb, x_e) and isinstance(self.dropout_rgb, nn.Identity):
             from . import fused
             return fused.cromb_ss2d(self, x_rgb, x_e, residual=residual)
         B, H, W, _ = x_rgb.shape
@@ -426,7 +436,7 @@ class VSSBlock(nn.Module):
             self.mlp = Mlp(in_features=hidden_dim, hidden_features=int(hidden_dim * mlp_ratio), act_layer=act_layer, drop=drop)
 
     def _forward(self, input):
-        if _fused_ok(input) and not self.mlp_branch:
+        if _fused_block_ok(self.op, input) and not self.mlp_branch:
             from . import fused
             return fused.vss_block(self, input)
         x = input + self.drop_path(self.op(ops.layer_norm(self.norm, input)))
@@ -490,7 +500,7 @@ class CVSSDecoderBlock(nn.Module):
         self.scale2 = nn.Parameter(torch.ones(hidden_dim))
 
     def _forward(self, input):
-        if _fused_ok(input):
+        if _fused_block_ok(self.op, input):
             from . import fused
             return fused.cvss_decoder_block(self, input)
         x = input * self.scale1 + self.drop_path(self.op(ops.layer_norm(self.norm1, input)))
@@ -522,7 +532,7 @@ class CrossMambaFusionBlock(nn.Module):
             self.mlp = Mlp(in_features=hidden_dim, hidden_features=int(hidden_dim * mlp_ratio), act_layer=act_layer, drop=drop)
 
     def _forward(self, x_rgb, x_e):
-        if _fused_ok(x_rgb, x_e):
+        if _fused_block_ok(self.op, x_rgb, x_e):
             return self.op(x_rgb, x_e, residual=True)
         c_r, c_e = self.op(x_rgb, x_e)
         return x_rgb + self.drop_path1(c_r), x_e + self.drop_path2(c_e)
@@ -551,7 +561,7 @@ class ConcatMambaFusionBlock(nn.Module):
             self.mlp = Mlp(in_features=hidden_dim, hidden_features=int(hidden_dim * mlp_ratio), act_layer=act_layer, drop=drop)
 
     def _forward(self, x_rgb, x_e):
-        if _fused_ok(x_rgb, x_e) and not self.mlp_branch:
+        if _fused_block_ok(self.op, x_rgb, x_e) and not self.mlp_branch:
             return self.op(x_rgb, x_e, residual=x_rgb + x_e)     # the sum is added in the out_proj GEMM epilogue
         x = x_rgb + x_e + self.drop_path(self.op(x_rgb, x_e))
         if self.mlp_branch:

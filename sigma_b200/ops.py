@@ -288,10 +288,12 @@ class CrossMerge_multimodal(torch.autograd.Function):
         return xs
 
 
-def _pick_nrows(D, nrows):
+def _pick_nrows(D, nrows, N=1):
+    """vmamba.py:183-191's automatic rows per block, stopping at a count whose d_state bound (N <= 256 / nrows,
+    selective_scan.cpp:198) the call meets: d_state="auto" past 64 states runs instead of failing the check.  Unchanged for N <= 64."""
     if nrows >= 1:
         return nrows
-    return 4 if D % 4 == 0 else 3 if D % 3 == 0 else 2 if D % 2 == 0 else 1
+    return next(r for r in (4, 3, 2, 1) if D % r == 0 and N <= 256 // r)
 
 
 def _scan_core(xs, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, nrows, delta_softplus):
@@ -313,7 +315,7 @@ def cross_selective_scan(x, x_proj_weight=None, x_proj_bias=None, dt_projs_weigh
                          A_logs=None, Ds=None, out_norm=None, softmax_version=False, nrows=-1, delta_softplus=True):
     """vmamba.py:165-226 (composed path: used when autograd is recording)."""
     B, D, H, W = x.shape
-    nrows = _pick_nrows(D, nrows)
+    nrows = _pick_nrows(D, nrows, A_logs.shape[1])
     ys = _scan_core(CrossScan.apply(x), x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds,
                     nrows, delta_softplus)
     y = CrossMerge.apply(ys.view(B, 4, D, H, W))
@@ -328,7 +330,7 @@ def cross_selective_scan_multimodal_k2(x_rgb, x_e, x_proj_weight=None, x_proj_bi
                                        softmax_version=False, nrows=-1, delta_softplus=True):
     """vmamba.py:369-430 (composed path)."""
     B, D, H, W = x_rgb.shape
-    nrows = _pick_nrows(D, nrows)
+    nrows = _pick_nrows(D, nrows, A_logs.shape[1])
     ys = _scan_core(CrossScan_multimodal.apply(x_rgb, x_e), x_proj_weight, x_proj_bias, dt_projs_weight,
                     dt_projs_bias, A_logs, Ds, nrows, delta_softplus)
     y_r, y_e = CrossMerge_multimodal.apply(ys)
