@@ -329,6 +329,41 @@ int sigma_split_tf32_fwd(const float *x, float *hi, float *lo, int64_t n, void *
 int sigma_linear_bf16(const void *A, int64_t lda, const void *W, const float *bias, const float *residual, int64_t ldr,
                       const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * FP8 inference mode (sigma_b200.fused.fp8_inference): e4m3 operands with fp32 scales.
+ * Quantizing a row x[0..C) (an activation row, or a weight's output channel) — every step one IEEE fp32 operation, round to
+ * nearest even:
+ *     amax = max_i |x_i|                     (fp32 values as the producer computed them, before any bf16 rounding)
+ *     amax == 0:  s = 1,  q_i = 0
+ *     otherwise:  inv = min(448 / amax, FLT_MAX),  s = amax / 448,
+ *                 q_i = cvt.rn.satfinite.e4m3(x_i · inv)   (round to nearest even, subnormals kept, |q| clamped to 448)
+ * so that x_i ≈ q_i · s.  The GEMM multiplies its fp32 accumulator by s_a[row] · s_w[col] (in that order) before the bias and
+ * residual epilogue.
+ * ------------------------------------------------------------------------------------------ */
+/* C[M,N] = (A[M,K]·Wq[N,K]^T)·sa[m]·sw[n] (+ bias[N]) (+ residual[M,N] (· rscale[N])) on the e4m3 tensor cores (`wgmma ...
+ * k32.f32.e4m3.e4m3`): A (M, K) e4m3 rows lda bytes apart, Wq (N, K) e4m3 contiguous, sa (M) and sw (N) fp32; each 128-wide
+ * k-block accumulates separately and is added to fp32 accumulators in registers.  C rows ldc elements apart, fp32 (c_dtype =
+ * SIGMA_F32) or bf16 (SIGMA_BF16); bias / residual / rscale fp32.  K, lda % 16 == 0; N, ldc, ldr % 4 == 0; A, Wq, C, bias,
+ * residual, rscale 16-byte aligned.                                                                                              */
+int sigma_linear_fp8(const void *A, int64_t lda, const float *sa, const void *Wq, const float *sw, const float *bias, const float *residual,
+                     int64_t ldr, const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream);
+/* Row quantizer (the formula above): x (rows, C) fp32 (x_dtype = SIGMA_F32, 16-byte aligned) or bf16 (SIGMA_BF16, 8-byte aligned)
+ * rows ldx elements apart -> q (rows, C) e4m3 rows ldq bytes apart (4-byte aligned) and scale (rows) fp32.  C, ldx, ldq % 4 == 0.
+ * Weights are quantized per output channel with it; so are activations that no row-wise producer below emits.               */
+int sigma_quantize_e4m3_rows(const void *x, int x_dtype, int64_t ldx, void *q, int64_t ldq, float *scale, int64_t rows, int C, void *stream);
+/* The producers of the FP8 mode that hold a whole row in registers, with a quantizing output: the same arithmetic as
+ * sigma_layernorm_fwd, sigma_patch_merge_norm_fwd and sigma_merge_norm_gate_fwd_bf16 (K = 1 or 4 there), the fp32 result quantized
+ * by the formula above into q (e4m3, the output layout of the plain call, in bytes; 4-byte aligned) and scale[r] for row r (the
+ * row index of the call: b·rows_per_batch + i for the merge).                                                                  */
+int sigma_layernorm_fwd_fp8(const float *x, const float *w, const float *b, void *q, float *scale, int64_t rows, int C, float eps,
+                            void *stream);
+int sigma_patch_merge_norm_fwd_fp8(const float *x, const float *w, const float *b, void *q, float *scale, int batch, int H, int W, int C,
+                                   float eps, void *stream);
+int sigma_merge_norm_gate_fwd_fp8(const void *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
+                                  const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *q, float *scale,
+                                  int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
+                                  int D, float eps, void *stream);
+
 /* Dense 3x3 convolution (pad 1, stride 1) of the ChannelAttentionBlock (vmamba.py:1749-1752), channels-last, as an implicit GEMM on
  * the same wgmma kernel: y (batch, H, W, Cout) = conv(x (batch, H, W, Cin), w9) + bias, act = 1 applies the exact (erf) GELU of
  * nn.GELU() in the epilogue.  w9 = the nn.Conv2d weight (Cout, Cin, 3, 3) re-ordered to (3·3, Cout, Cin); every tap's input patch
@@ -342,7 +377,8 @@ int sigma_conv3x3_tf32(const float *x, const float *w9, const float *w9_lo, cons
  * the current environment.  out6_host = {tile width, ring stages, persistent grid, output tiles, dynamic shared memory bytes, CTAs
  * per SM}.  The environment variable SIGMA_GEMM_BN=<w> forces the tile width of both calls (a multiple of 32 in [32, 256], read
  * per call; any other value makes the calls and this query return SIGMA_EINVAL).  For tests and tuning.
- * x3 selects the instance: 0 = tf32, 1 = tf32x3, 2 = sigma_linear_bf16 (conv_B must be 0); other values are SIGMA_EINVAL.      */
+ * x3 selects the instance: 0 = tf32, 1 = tf32x3, 2 = sigma_linear_bf16, 4 = sigma_linear_fp8 (conv_B must be 0 for 2 and 4; the
+ * e4m3 tiles are 32 or 64 wide, and forcing a wider one is SIGMA_EINVAL); other values (3 included) are SIGMA_EINVAL.        */
 int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, int64_t *out6_host);
 
 /* L-segment plan of the fused scan backward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_bwd (nsplit = 0)

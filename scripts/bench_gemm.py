@@ -1,7 +1,10 @@
 """Dense-projection GEMMs of Sigma-tiny at `--images` per GPU: our wgmma kernel vs cuBLAS (torch.mm), in the precision of
 `--precision` (tf32: one TF32 MMA per k-step, cuBLAS TF32; tf32x3: three TF32 MMAs per k-step, cuBLAS fp32).
 Reports ms, effective GB/s over (A read once + C written once [+ residual read]) and TFLOP/s over 2·M·N·K; for our tf32x3
-kernel also the TF32 tensor-core rate, 3 x 2·M·N·K (A_lo·W_hi + A_hi·W_lo + A_hi·W_hi)."""
+kernel also the TF32 tensor-core rate, 3 x 2·M·N·K (A_lo·W_hi + A_hi·W_lo + A_hi·W_hi).
+--precision fp8 times, at the GEMMs the FP8 inference mode quantizes (in_proj, out_proj, the patch-merge reduction), our
+bf16 instance (bf16 A, as in the bf16 mode) against our e4m3 instance (A already quantized, as the fused producers emit it);
+bytes count A at 2 or 1 byte per element (+ 4 per row of scales), C fp32."""
 import argparse
 import os
 import sys
@@ -14,7 +17,7 @@ from sigma_b200 import fused  # noqa: E402
 ap = argparse.ArgumentParser()
 ap.add_argument("--images", type=int, default=16)
 ap.add_argument("--only", nargs="*", default=None)
-ap.add_argument("--precision", default="tf32", choices=["tf32", "tf32x3"])
+ap.add_argument("--precision", default="tf32", choices=["tf32", "tf32x3", "fp8"])
 a = ap.parse_args()
 torch.backends.cuda.matmul.allow_tf32 = a.precision == "tf32"
 S = 2 * a.images
@@ -30,6 +33,30 @@ print(f"precision {fused.precision()}, {torch.cuda.get_device_name()}", flush=Tr
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 for name, M, N, K, res in SHAPES:
     if a.only and name not in a.only:
+        continue
+    if a.precision == "fp8":
+        if "x_proj" in name:                         # x_proj stays bf16 in the FP8 mode
+            continue
+        A = torch.randn(M, K, device="cuda")
+        W = torch.randn(N, K, device="cuda") * K ** -0.5
+        R = torch.randn(M, N, device="cuda") if res else None
+        out = torch.empty(M, N, device="cuda")
+        operands = {"bf16": A.to(torch.bfloat16), "e4m3": fused.quantize_rows(A)}
+        line = f"{name:11s} M={M:7d} N={N:5d} K={K:5d}: "
+        for mode, op in operands.items():
+            byt = (2 if mode == "bf16" else 1) * M * K + (4 * M if mode == "e4m3" else 0) + 4 * M * N * (2 if res else 1)
+            ts = []
+            for _ in range(7):
+                flush.zero_()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                fused.linear(op, W, None, out=out, residual=R)
+                e1.record()
+                torch.cuda.synchronize()
+                ts.append(e0.elapsed_time(e1))
+            ms = sorted(ts[1:])[3]
+            line += f"{mode} {ms:7.3f} ms {byt / ms / 1e6:7.1f} GB/s {2 * M * N * K / ms / 1e9:6.1f} TFLOP/s   "
+        print(line, flush=True)
         continue
     A = torch.randn(M, K, device="cuda")
     W = torch.randn(N, K, device="cuda") * K ** -0.5

@@ -1,5 +1,6 @@
-"""Sigma-tiny 480x640 inference at B = 74 by CUDA-graph replay in the fused path's three modes — tf32x3 (default), tf32
-(torch.backends.cuda.matmul.allow_tf32) and bf16 (torch.autocast("cuda", dtype=torch.bfloat16)) — alternating in one process
+"""Sigma-tiny 480x640 inference at B = 74 by CUDA-graph replay in the fused path's four modes — tf32x3 (default), tf32
+(torch.backends.cuda.matmul.allow_tf32), bf16 (torch.autocast("cuda", dtype=torch.bfloat16)) and fp8
+(sigma_b200.fused.fp8_inference()) — alternating in one process
 after warm-up.  Prints one JSON line: images/s per mode (median of the rounds), each mode's logits error against tf32x3 on
 the same seeded inputs (max |diff| / max |logit|), peak memory per mode, and the card name and power limit read in the same run.
 
@@ -31,7 +32,10 @@ def _card():
 
 
 def _mode_ctx(mode):
+    from sigma_b200 import fused
     torch.backends.cuda.matmul.allow_tf32 = mode == "tf32"
+    if mode == "fp8":
+        return fused.fp8_inference()
     return torch.autocast("cuda", dtype=torch.bfloat16) if mode == "bf16" else contextlib.nullcontext()
 
 
@@ -55,9 +59,11 @@ def main():
     model = model.cuda().eval()
     rgb = P.randn(7, "bench/rgb", (B, 3, H, W)).cuda()
     x = P.randn(7, "bench/x", (B, 3, H, W)).cuda()
-    modes = ["tf32x3", "tf32", "bf16"]
+    modes = ["tf32x3", "tf32", "bf16", "fp8"]
     graphs, outs, peak = {}, {}, {}
     stream = torch.cuda.Stream()
+    pool = torch.cuda.graph_pool_handle()            # one memory pool for the four graphs (replayed one at a time): four
+                                                     # private pools of a B = 74 forward do not fit in 80 GB
     for m in modes:
         torch.cuda.synchronize()
         torch.cuda.reset_peak_memory_stats()
@@ -67,7 +73,7 @@ def main():
                 model(rgb, x)
             stream.synchronize()
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=stream):
+            with torch.cuda.graph(g, stream=stream, pool=pool):
                 outs[m] = model(rgb, x)
         stream.synchronize()
         graphs[m] = g
@@ -87,6 +93,12 @@ def main():
                 e1.record(stream)
                 e1.synchronize()
                 times[m].append(e0.elapsed_time(e1) / args.steps)
+        final = {}
+        for m in modes:                              # a graph's output can share pool memory with another's intermediates:
+            graphs[m].replay()                       # read each right after its own replay
+            final[m] = outs[m].float().clone()
+        stream.synchronize()
+    outs = final
     ref = outs["tf32x3"].float()
     scale = float(ref.abs().max())
     name, limit = _card()

@@ -339,6 +339,16 @@ int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, voi
   return row_norm_launch(p, (cudaStream_t)stream);
 }
 
+int sigma_layernorm_fwd_fp8(const float *x, const float *w, const float *b, void *q, float *scale, int64_t rows, int C, float eps,
+                            void *stream) {
+  SIGMA_CHECK_ARG(x && w && b && q && scale, "sigma_layernorm_fwd_fp8: null pointer");
+  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd_fp8: C=%d must be a positive multiple of 4", C);
+  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && ((uintptr_t)q & 3) == 0, "sigma_layernorm_fwd_fp8: x, w, b must be 16-byte and q 4-byte aligned");
+  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)q, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
+  p.io = 3; p.qscale = scale;
+  return row_norm_launch(p, (cudaStream_t)stream);
+}
+
 int sigma_layernorm_fwd_bf16io(const void *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
   SIGMA_CHECK_ARG(x && w && b && y, "sigma_layernorm_fwd_bf16io: null pointer");
   SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd_bf16io: C=%d must be a positive multiple of 4", C);
@@ -410,6 +420,18 @@ int sigma_patch_merge_norm_fwd_bf16(const float *x, const float *w, const float 
   return row_norm_launch(p, (cudaStream_t)stream);
 }
 
+int sigma_patch_merge_norm_fwd_fp8(const float *x, const float *w, const float *b, void *q, float *scale, int batch, int H, int W, int C,
+                                   float eps, void *stream) {
+  SIGMA_CHECK_ARG(x && w && b && q && scale, "sigma_patch_merge_norm_fwd_fp8: null pointer");
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "sigma_patch_merge_norm_fwd_fp8: bad sizes");
+  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && ((uintptr_t)q & 3) == 0,
+                  "sigma_patch_merge_norm_fwd_fp8: x, w, b must be 16-byte and q 4-byte aligned");
+  const int64_t rows = (int64_t)batch * ((H + 1) / 2) * ((W + 1) / 2);
+  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)q, rows, rows, 0, 0, 4 * C, 4 * C, eps};
+  p.mode = 1; p.gH = H; p.gW = W; p.io = 3; p.qscale = scale;
+  return row_norm_launch(p, (cudaStream_t)stream);
+}
+
 int sigma_pixel_shuffle_norm_fwd(const float *x, const float *w, const float *b, float *y, int batch, int H, int W, int C,
                                  float eps, void *stream) {
   SIGMA_CHECK_ARG(x && w && b && y, "sigma_pixel_shuffle_norm_fwd: null pointer");
@@ -435,6 +457,23 @@ int sigma_merge_norm_gate_fwd(const float *y, int K, int64_t k_stride, int64_t i
                   "sigma_merge_norm_gate_fwd: pointers / strides must be 16-byte aligned");
   RowNormParams p{y, k_stride, K, gamma, beta, z, z_row_stride, gate, out, rows, rows_per_batch, in_batch_stride,
                   out_batch_stride, out_row_stride, D, eps};
+  return row_norm_launch(p, (cudaStream_t)stream);
+}
+
+int sigma_merge_norm_gate_fwd_fp8(const void *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
+                                  const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *q, float *scale,
+                                  int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
+                                  int D, float eps, void *stream) {
+  SIGMA_CHECK_ARG(y && gamma && beta && q && scale, "sigma_merge_norm_gate_fwd_fp8: null pointer");
+  SIGMA_CHECK_ARG((K == 1 || K == 4) && D > 0 && D % 4 == 0 && rows >= 0 && rows_per_batch > 0,
+                  "sigma_merge_norm_gate_fwd_fp8: bad sizes K=%d (1 or 4) D=%d rows=%lld rows_per_batch=%lld", K, D, (long long)rows,
+                  (long long)rows_per_batch);
+  SIGMA_CHECK_ARG(al8(y) && al16(gamma) && al16(beta) && ((uintptr_t)q & 3) == 0 && al8(z) && al16(gate) && k_stride % 4 == 0 &&
+                      in_batch_stride % 4 == 0 && out_batch_stride % 4 == 0 && out_row_stride % 4 == 0 && z_row_stride % 4 == 0,
+                  "sigma_merge_norm_gate_fwd_fp8: y / z must be 8-byte, q 4-byte and gamma / beta / gate 16-byte aligned, strides multiples of 4");
+  RowNormParams p{(const float *)y, k_stride, K, gamma, beta, (const float *)z, z_row_stride, gate, (float *)q, rows, rows_per_batch,
+                  in_batch_stride, out_batch_stride, out_row_stride, D, eps};
+  p.io = 4; p.qscale = scale;
   return row_norm_launch(p, (cudaStream_t)stream);
 }
 
@@ -857,6 +896,29 @@ int sigma_linear_bf16(const void *A, int64_t lda, const void *W, const float *bi
                   "sigma_linear_bf16: pointers must be 16-byte aligned");
   SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "sigma_linear_bf16: rscale without residual");
   return gemm_bf16_launch(A, lda, W, bias, residual, ldr, rscale, C, ldc, c_dtype == SIGMA_BF16, M, N, K, (cudaStream_t)stream);
+}
+
+int sigma_linear_fp8(const void *A, int64_t lda, const float *sa, const void *Wq, const float *sw, const float *bias, const float *residual,
+                     int64_t ldr, const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream) {
+  SIGMA_CHECK_ARG(A && sa && Wq && sw && C, "sigma_linear_fp8: null pointer");
+  SIGMA_CHECK_ARG(c_dtype == SIGMA_F32 || c_dtype == SIGMA_BF16, "sigma_linear_fp8: c_dtype %d (SIGMA_F32 or SIGMA_BF16)", c_dtype);
+  SIGMA_CHECK_ARG(M >= 0 && M < (1LL << 31) && N > 0 && K > 0, "sigma_linear_fp8: bad sizes M=%lld N=%d K=%d", (long long)M, N, K);
+  SIGMA_CHECK_ARG(K % 16 == 0 && lda % 16 == 0 && N % 4 == 0 && ldc % 4 == 0 && (residual == nullptr || ldr % 4 == 0) && lda >= K && ldc >= N,
+                  "sigma_linear_fp8: K and lda must be multiples of 16 (16-byte e4m3 TMA rows); N, ldc, ldr multiples of 4");
+  SIGMA_CHECK_ARG(al16(A) && al16(Wq) && al16(C) && al16(bias) && al16(residual) && al16(rscale) && al8(sw),
+                  "sigma_linear_fp8: A, Wq, C, bias, residual, rscale must be 16-byte and sw 8-byte aligned");
+  SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "sigma_linear_fp8: rscale without residual");
+  return gemm_fp8_launch(A, lda, sa, Wq, sw, bias, residual, ldr, rscale, C, ldc, c_dtype == SIGMA_BF16, M, N, K, (cudaStream_t)stream);
+}
+
+int sigma_quantize_e4m3_rows(const void *x, int x_dtype, int64_t ldx, void *q, int64_t ldq, float *scale, int64_t rows, int C, void *stream) {
+  SIGMA_CHECK_ARG(x && q && scale, "sigma_quantize_e4m3_rows: null pointer");
+  SIGMA_CHECK_ARG(x_dtype == SIGMA_F32 || x_dtype == SIGMA_BF16, "sigma_quantize_e4m3_rows: x_dtype %d (SIGMA_F32 or SIGMA_BF16)", x_dtype);
+  SIGMA_CHECK_ARG(rows >= 0 && C > 0 && C % 4 == 0 && ldx >= C && ldq >= C && ldx % 4 == 0 && ldq % 4 == 0,
+                  "sigma_quantize_e4m3_rows: C=%d, ldx, ldq must be multiples of 4 with ldx, ldq >= C", C);
+  SIGMA_CHECK_ARG((x_dtype == SIGMA_F32 ? al16(x) : al8(x)) && ((uintptr_t)q & 3) == 0,
+                  "sigma_quantize_e4m3_rows: x must be 16-byte (fp32) or 8-byte (bf16) and q 4-byte aligned");
+  return quantize_e4m3_rows_launch(x, x_dtype == SIGMA_BF16, ldx, q, ldq, scale, rows, C, (cudaStream_t)stream);
 }
 
 int sigma_linear_tf32x3(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias, const float *residual,

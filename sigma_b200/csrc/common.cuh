@@ -75,6 +75,24 @@ __device__ __forceinline__ void st4(__nv_bfloat16 *p, float4 v) {
   *reinterpret_cast<uint2 *>(p) = make_uint2(from_f32x2<__nv_bfloat16>(v.x, v.y), from_f32x2<__nv_bfloat16>(v.z, v.w));
 }
 
+// ---- e4m3 rows with one fp32 scale per row (the FP8 inference mode; the formula is stated in sigma_b200.h) ----
+// Output-type tag of the row-wise kernels: `out` holds e4m3 bytes, RowNormParams::qscale one scale per row.
+struct E4M3Rows {};
+// 448 / amax, the factor that maps a row onto e4m3's finite range; amax = 0 -> 1 (the row quantizes to zeros, scale 1);
+// clamped to FLT_MAX so that a row of tiny values cannot make it infinite
+__device__ __forceinline__ float e4m3_inv_scale(float amax) {
+  return amax == 0.f ? 1.f : fminf(__fdiv_rn(448.f, amax), 3.4028234663852886e38f);
+}
+__device__ __forceinline__ float e4m3_scale(float amax) { return amax == 0.f ? 1.f : __fdiv_rn(amax, 448.f); }
+// four fp32 -> four e4m3 bytes of v·inv (x at the lowest address), round to nearest even, saturating to ±448
+__device__ __forceinline__ uint32_t e4m3x4(float4 v, float inv) {
+  uint16_t lo, hi;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(__fmul_rn(v.y, inv)), "f"(__fmul_rn(v.x, inv)));
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(__fmul_rn(v.w, inv)), "f"(__fmul_rn(v.z, inv)));
+  return (uint32_t)lo | ((uint32_t)hi << 16);
+}
+__device__ __forceinline__ float amax4(float4 v) { return fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))); }
+
 // ---- device math ----
 __device__ __forceinline__ float ex2(float x) {
   float y;

@@ -41,7 +41,10 @@ struct RowNormParams {
   int mode = 0, gH = 0, gW = 0;
   // element types (the bf16 inference mode): 0 = y, z, out fp32; 1 = y fp32, out bf16 (LayerNorm / patch-merge LN feeding a
   // bf16 GEMM); 2 = y, z, out bf16 (merge + out_norm + gate of the bf16 scan output).  Pointers and strides count elements.
+  // The FP8 inference mode: 3 = y fp32, out e4m3 (LayerNorm / patch-merge LN feeding sigma_linear_fp8); 4 = y, z bf16, out e4m3
+  // (merge + out_norm + gate).  Both write row r's scale to qscale[r].
   int io = 0;
+  float *qscale = nullptr;
 };
 
 struct ImagePreParams {
@@ -148,6 +151,8 @@ int upsample_bilinear_bwd_launch(const float *dy, float *dx, int batch, int C, i
 
 // ---- rowwise.cu ----
 int row_norm_launch(const RowNormParams &p, cudaStream_t stream);
+int quantize_e4m3_rows_launch(const void *x, bool bf16, long long ldx, void *q, long long ldq, float *scale, long long rows, int C,
+                              cudaStream_t stream);
 // part != nullptr: the deterministic build (layernorm_bwd_det_workspace_bytes of scratch)
 int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
                          int D, float eps, cudaStream_t stream, float *part = nullptr, bool bf16 = false);
@@ -173,6 +178,9 @@ int gemm_tf32_launch(const float *A, long long lda, const float *W, const float 
                      long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream);
 int gemm_bf16_launch(const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
                      const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N, int K, cudaStream_t stream);
+int gemm_fp8_launch(const void *A, long long lda, const float *sa, const void *W, const float *sw, const float *bias,
+                    const float *residual, long long ldr, const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N,
+                    int K, cudaStream_t stream);
 int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, const float *bias, int act, float *y, int B, int H, int W,
                         int Cin, int Cout, cudaStream_t stream);
 int split_tf32_launch(const float *x, float *hi, float *lo, long long n, cudaStream_t stream);

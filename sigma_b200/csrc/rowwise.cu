@@ -6,6 +6,7 @@
 // All are HBM-bound; loads/stores are 16-byte, rows are contiguous in the channel dimension.
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -18,7 +19,27 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
-// TI: element type of y and z, TO: of out (RowNormParams::io); gamma, beta, gate and all arithmetic are fp32
+// (x - mean)·rstd·gamma + beta [· SiLU(z)] [· gate] of float4 idx of a row: the arithmetic of the stores below, for the e4m3
+// instances, which hold the whole row before they store it
+__device__ __forceinline__ float4 norm_gate4(float4 x, float mean, float rstd, const RowNormParams &p, int idx, float4 z, bool has_z,
+                                             const float *gate_row) {
+  const float4 g = __ldg(reinterpret_cast<const float4 *>(p.gamma) + idx);
+  const float4 b = __ldg(reinterpret_cast<const float4 *>(p.beta) + idx);
+  float4 o;
+  o.x = fmaf((x.x - mean) * rstd, g.x, b.x);
+  o.y = fmaf((x.y - mean) * rstd, g.y, b.y);
+  o.z = fmaf((x.z - mean) * rstd, g.z, b.z);
+  o.w = fmaf((x.w - mean) * rstd, g.w, b.w);
+  if (has_z) { o.x *= silu(z.x); o.y *= silu(z.y); o.z *= silu(z.z); o.w *= silu(z.w); }
+  if (gate_row) {
+    const float4 gg = __ldg(reinterpret_cast<const float4 *>(gate_row) + idx);
+    o.x *= gg.x; o.y *= gg.y; o.z *= gg.z; o.w *= gg.w;
+  }
+  return o;
+}
+
+// TI: element type of y and z, TO: of out (RowNormParams::io; E4M3Rows: e4m3 bytes + p.qscale); gamma, beta, gate and all
+// arithmetic are fp32
 template <int MAXV, typename TI, typename TO>
 __global__ void __launch_bounds__(256) row_norm_kernel(const RowNormParams p) {
   const int lane = threadIdx.x & 31;
@@ -56,6 +77,26 @@ __global__ void __launch_bounds__(256) row_norm_kernel(const RowNormParams p) {
   TO *out = reinterpret_cast<TO *>(p.out) + bi * p.out_batch_stride + ri * p.out_row_stride;
   const TI *zr = p.z ? reinterpret_cast<const TI *>(p.z) + row * p.z_row_stride : nullptr;
   const float *gr = p.gate ? p.gate + bi * p.D : nullptr;
+  if constexpr (std::is_same<TO, E4M3Rows>::value) {   // the whole row first (its amax sets the scale), then e4m3
+    float am = 0.f;
+#pragma unroll
+    for (int v = 0; v < MAXV; ++v) {
+      const int idx = lane + 32 * v;
+      if (idx < nvec) {
+        x[v] = norm_gate4(x[v], mean, rstd, p, idx, zr ? ld4g(zr + 4 * idx) : make_float4(0.f, 0.f, 0.f, 0.f), zr != nullptr, gr);
+        am = fmaxf(am, amax4(x[v]));
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, o));
+    const float inv = e4m3_inv_scale(am);
+#pragma unroll
+    for (int v = 0; v < MAXV; ++v) {
+      const int idx = lane + 32 * v;
+      if (idx < nvec) reinterpret_cast<uint32_t *>(out)[idx] = e4m3x4(x[v], inv);
+    }
+    if (lane == 0) p.qscale[row] = e4m3_scale(am);
+  } else {
 #pragma unroll
   for (int v = 0; v < MAXV; ++v) {
     const int idx = lane + 32 * v;
@@ -77,6 +118,7 @@ __global__ void __launch_bounds__(256) row_norm_kernel(const RowNormParams p) {
       }
       st4(out + 4 * idx, o);
     }
+  }
   }
 }
 
@@ -151,6 +193,22 @@ __global__ void __launch_bounds__(256) row_norm_fast_kernel(const RowNormParams 
     out = reinterpret_cast<TO *>(p.out) + (((b * 2 * p.gH + 2 * h + p1) * 2 * p.gW) + 2 * w + p2) * p.D;
   }
   const float4 *gr = p.gate ? reinterpret_cast<const float4 *>(p.gate + bi * p.D) : nullptr;
+  if constexpr (std::is_same<TO, E4M3Rows>::value) {   // the whole row first (its amax sets the scale), then e4m3
+    float am = 0.f;
+#pragma unroll
+    for (int v = 0; v < V; ++v) {
+      x[v] = norm_gate4(x[v], mean, rstd, p, l + LPR * v, zz[v], has_z, reinterpret_cast<const float *>(gr));
+      am = fmaxf(am, amax4(x[v]));
+    }
+#pragma unroll
+    for (int o = LPR / 2; o > 0; o >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, o));
+    const float inv = e4m3_inv_scale(am);
+    if (valid) {
+#pragma unroll
+      for (int v = 0; v < V; ++v) reinterpret_cast<uint32_t *>(out)[l + LPR * v] = e4m3x4(x[v], inv);
+      if (l == 0) p.qscale[row] = e4m3_scale(am);
+    }
+  } else {
 #pragma unroll
   for (int v = 0; v < V; ++v) {
     const int idx = l + LPR * v;
@@ -167,6 +225,7 @@ __global__ void __launch_bounds__(256) row_norm_fast_kernel(const RowNormParams 
       o.x *= gg.x; o.y *= gg.y; o.z *= gg.z; o.w *= gg.w;
     }
     if (valid) st4(out + 4 * idx, o);
+  }
   }
 }
 
@@ -215,8 +274,60 @@ static bool row_norm_fast(const RowNormParams &p, cudaStream_t stream) {
   return false;
 }
 
+// The e4m3-output instances (io 3, 4: the FP8 inference mode), at the fast widths of row_norm_fast and, for other widths up to
+// 1024 channels, the generic kernel (a wider row held in registers would spill).
+template <int LPR, int V>
+static bool row_norm_e4m3_fast_k(const RowNormParams &p, cudaStream_t stream) {
+  using bf16 = __nv_bfloat16;
+  const int warps = 8, rows_per_cta = warps * (32 / LPR);
+  const unsigned grid = (unsigned)((p.rows + rows_per_cta - 1) / rows_per_cta);
+  if (p.io == 3) {   // LayerNorm / patch-merge LayerNorm
+    if (p.K != 1) return false;
+    if (p.mode == 0) { row_norm_fast_kernel<LPR, V, 1, 0, float, E4M3Rows><<<grid, warps * 32, 0, stream>>>(p); return true; }
+    if (p.mode == 1) { row_norm_fast_kernel<LPR, V, 1, 1, float, E4M3Rows><<<grid, warps * 32, 0, stream>>>(p); return true; }
+    return false;
+  }
+  if (p.mode != 0) return false;   // io 4: merge + norm + gate, bf16 in
+  if (p.K == 1) { row_norm_fast_kernel<LPR, V, 1, 0, bf16, E4M3Rows><<<grid, warps * 32, 0, stream>>>(p); return true; }
+  if (p.K == 4) { row_norm_fast_kernel<LPR, V, 4, 0, bf16, E4M3Rows><<<grid, warps * 32, 0, stream>>>(p); return true; }
+  return false;
+}
+
+static int row_norm_e4m3_launch(const RowNormParams &p, cudaStream_t stream) {
+  const int nvec = p.D >> 2;
+  bool ok = false;
+  if (!((p.D & 3) || (p.k_stride & 3) || (p.in_batch_stride & 3) || (p.out_row_stride & 3) || (p.out_batch_stride & 3) ||
+        (p.z_row_stride & 3))) {
+#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) ok = row_norm_e4m3_fast_k<LPR, V>(p, stream)
+    TRY(8, 2); TRY(8, 3); TRY(8, 4);
+    TRY(16, 3); TRY(16, 4);
+    TRY(32, 3); TRY(32, 4); TRY(32, 6); TRY(32, 8); TRY(32, 12); TRY(32, 16);
+#undef TRY
+  }
+  if (!ok) {
+    if (p.mode != 0 || nvec > 256 || (p.io == 4 && p.K != 1 && p.K != 4)) {
+      set_error("row_norm: no e4m3-output instance for D=%d, mode %d, K=%d (fast widths, or D <= 1024 plain rows)", p.D, p.mode, p.K);
+      return SIGMA_EUNSUPPORTED;
+    }
+    const unsigned grid = (unsigned)((p.rows + 7) / 8);
+#define LAUNCH_E4M3(MV)                                                                                                  \
+    do {                                                                                                                 \
+      if (p.io == 3) row_norm_kernel<MV, float, E4M3Rows><<<grid, 256, 0, stream>>>(p);                                  \
+      else row_norm_kernel<MV, __nv_bfloat16, E4M3Rows><<<grid, 256, 0, stream>>>(p);                                    \
+    } while (0)
+    if (nvec <= 32) LAUNCH_E4M3(1);
+    else if (nvec <= 64) LAUNCH_E4M3(2);
+    else if (nvec <= 128) LAUNCH_E4M3(4);
+    else LAUNCH_E4M3(8);
+#undef LAUNCH_E4M3
+  }
+  SIGMA_CHECK_LAUNCH();
+  return SIGMA_OK;
+}
+
 int row_norm_launch(const RowNormParams &p, cudaStream_t stream) {
   if (p.rows == 0) return SIGMA_OK;
+  if (p.io >= 3) return row_norm_e4m3_launch(p, stream);
   if (row_norm_fast(p, stream)) {
     SIGMA_CHECK_LAUNCH();
     return SIGMA_OK;
@@ -239,6 +350,38 @@ int row_norm_launch(const RowNormParams &p, cudaStream_t stream) {
   else if (nvec <= 1024) LAUNCH(32);
   else { set_error("row_norm: D=%d > 4096 unsupported", p.D); return SIGMA_EUNSUPPORTED; }
 #undef LAUNCH
+  SIGMA_CHECK_LAUNCH();
+  return SIGMA_OK;
+}
+
+// ---- standalone e4m3 row quantizer (the FP8 inference mode: weights per output channel, and activations no producer holds a
+// row of): one warp per row, an amax pass and a quantizing pass over the row (the second one from L1 / L2) ----
+template <typename TI>
+__global__ void __launch_bounds__(256) quantize_e4m3_rows_kernel(const TI *__restrict__ x, long long ldx, unsigned char *__restrict__ q,
+                                                                  long long ldq, float *__restrict__ scale, long long rows, int C) {
+  const int lane = threadIdx.x & 31;
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const TI *xr = x + row * ldx;
+  const int nvec = C >> 2;
+  float am = 0.f;
+  for (int i = lane; i < nvec; i += 32) am = fmaxf(am, amax4(ld4g(xr + 4 * i)));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, o));
+  const float inv = e4m3_inv_scale(am);
+  uint32_t *qr = reinterpret_cast<uint32_t *>(q + row * ldq);
+  for (int i = lane; i < nvec; i += 32) qr[i] = e4m3x4(ld4g(xr + 4 * i), inv);
+  if (lane == 0) scale[row] = e4m3_scale(am);
+}
+
+int quantize_e4m3_rows_launch(const void *x, bool bf16, long long ldx, void *q, long long ldq, float *scale, long long rows, int C,
+                              cudaStream_t stream) {
+  if (rows == 0) return SIGMA_OK;
+  const unsigned grid = (unsigned)((rows + 7) / 8);
+  if (bf16)
+    quantize_e4m3_rows_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16 *)x, ldx, (unsigned char *)q, ldq, scale, rows, C);
+  else
+    quantize_e4m3_rows_kernel<float><<<grid, 256, 0, stream>>>((const float *)x, ldx, (unsigned char *)q, ldq, scale, rows, C);
   SIGMA_CHECK_LAUNCH();
   return SIGMA_OK;
 }

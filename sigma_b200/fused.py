@@ -15,8 +15,17 @@ x_dbl stays fp32 (it carries dt, B and C into softplus and exp, and it is small)
 out_proj, the PatchMerging reduction and x_proj write fp32, so their residual and rscale epilogues read fp32.  Everything
 else (the decoder's CAB convs, patch embed, PatchExpand, UpsampleExpand, the final head, the pools) runs in the dense mode
 torch's matmul switch selects, with autocast switched off around the torch ops the fused path calls.
+
+The FP8 mode (`precision() == "fp8"`, selected by `fp8_inference()` with autograd off, autocast or not) stores exactly what the
+bf16 mode stores, and runs the in_proj / in_proj_modalx and out_proj / out_proj_rgb / out_proj_e GEMMs of SS2D, ConMB and CroMB
+and the PatchMerging2D reduction on e4m3 operands (sigma_linear_fp8): activations with one fp32 scale per row, weights with one
+per output channel (the formula in include/sigma_b200.h).  The LayerNorms in front of in_proj, the patch-merge LayerNorm and
+SS2D's / CroMB's merge + norm + gate emit the e4m3 rows and scales themselves; ConMB's and CroMB's in_proj operands and ConMB's
+two-part ycat go through the standalone row quantizer.  x_proj stays bf16 (it feeds softplus and exp).
 """
+import contextlib
 import ctypes
+from typing import NamedTuple
 
 import torch
 import torch.nn.functional as F
@@ -29,9 +38,39 @@ _FORCE_SPLIT = 0  # test hook: force the number of L-segments of the fused scan
 
 
 # ---------------------------------------------------------------- primitive wrappers
-def layernorm(x2d, ln, dtype=torch.float32):
-    """nn.LayerNorm over the last dim of a contiguous (rows, C) fp32 tensor; dtype=torch.bfloat16 stores the output as bf16."""
+class E4M3Rows(NamedTuple):
+    """An FP8-mode GEMM operand: q (rows, ...) torch.float8_e4m3fn and one fp32 scale per row, s (rows,); row r is q[r]·s[r]."""
+    q: torch.Tensor
+    s: torch.Tensor
+
+    def view(self, *shape):
+        return E4M3Rows(self.q.view(*shape), self.s)
+
+
+def _e4m3_empty(rows, C, device):
+    return E4M3Rows(torch.empty((rows, C), dtype=torch.float8_e4m3fn, device=device),
+                    torch.empty((rows,), dtype=torch.float32, device=device))
+
+
+def quantize_rows(x2d, out=None):
+    """(rows, C) fp32 or bf16 with unit column stride -> E4M3Rows (sigma_quantize_e4m3_rows; per-row scale)."""
     rows, C = x2d.shape
+    out = out if out is not None else _e4m3_empty(rows, C, x2d.device)
+    xd = _lib.BF16 if x2d.dtype == torch.bfloat16 else _lib.F32
+    _lib.check(_lib.lib().sigma_quantize_e4m3_rows(ptr(x2d), xd, x2d.stride(0), ptr(out.q), out.q.stride(0), ptr(out.s), rows, C,
+                                                   stream()), "sigma_quantize_e4m3_rows")
+    return out
+
+
+def layernorm(x2d, ln, dtype=torch.float32):
+    """nn.LayerNorm over the last dim of a contiguous (rows, C) fp32 tensor; dtype=torch.bfloat16 stores the output as bf16,
+    dtype=torch.float8_e4m3fn returns E4M3Rows (sigma_layernorm_fwd_fp8: the fp32 result quantized per row)."""
+    rows, C = x2d.shape
+    if dtype == torch.float8_e4m3fn:
+        y = _e4m3_empty(rows, C, x2d.device)
+        _lib.check(_lib.lib().sigma_layernorm_fwd_fp8(ptr(x2d), ptr(ln.weight), ptr(ln.bias), ptr(y.q), ptr(y.s), rows, C, float(ln.eps),
+                                                      stream()), "sigma_layernorm_fwd_fp8")
+        return y
     y = torch.empty((rows, C), dtype=dtype, device=x2d.device)
     fn = "sigma_layernorm_fwd_bf16" if dtype == torch.bfloat16 else "sigma_layernorm_fwd"
     _lib.check(getattr(_lib.lib(), fn)(ptr(x2d), ptr(ln.weight), ptr(ln.bias), ptr(y), rows, C, float(ln.eps), stream()), fn)
@@ -41,8 +80,25 @@ def layernorm(x2d, ln, dtype=torch.float32):
 USE_OWN_GEMM = True  # False: cuBLAS through torch (library GEMM, precision by torch's switch), kept for A/B timing only
 
 
+FP8_INFERENCE = False
+
+
+@contextlib.contextmanager
+def fp8_inference(on=True):
+    """Switch the FP8 inference mode of the fused path on (or off) inside the block: with autograd off, precision() is "fp8"."""
+    global FP8_INFERENCE
+    prev, FP8_INFERENCE = FP8_INFERENCE, bool(on)
+    try:
+        yield
+    finally:
+        FP8_INFERENCE = prev
+
+
 def precision():
-    """Precision of the fused path.  With autograd off and torch.autocast("cuda", dtype=torch.bfloat16) active it is "bf16": the
+    """Precision of the fused path.  Inside fp8_inference() with autograd off it is "fp8": the bf16 mode's storage, with the
+    in_proj / out_proj / PatchMerging GEMMs on e4m3 operands scaled per row and per output channel (module docstring); logits
+    within 2x the error of the reference's layers under bf16 autocast with the same e4m3 quantize-dequantize at those GEMMs.
+    With autograd off and torch.autocast("cuda", dtype=torch.bfloat16) active it is "bf16": the
     SS2D / ConMB / CroMB / PatchMerging interiors store bf16 and their GEMMs run bf16 wgmma (module docstring); logits within
     2x the error of the reference's own layers under the same autocast.  Autocast with fp16 is not a mode of the fused path: it
     keeps the fp32 modes below.  With autograd on (training) autocast does not change the fused core either.
@@ -53,6 +109,8 @@ def precision():
           with the reference's fp32 results to ~1e-6 of their scale (1e-3 bar);
       torch.backends.cuda.matmul.allow_tf32 = True -> "tf32": the same kernel, one TF32 MMA per k-step (10-bit mantissa
           operands, fp32 accumulate in registers); logits within ~3e-3 of the reference's (1e-2 bar)."""
+    if not torch.is_grad_enabled() and FP8_INFERENCE:
+        return "fp8"
     if not torch.is_grad_enabled() and torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16:
         return "bf16"
     return _dense_precision()
@@ -69,17 +127,23 @@ def logits_bar(composed_err=None):
     """Parity bar for end-to-end logits of the fused path, as a fraction of the logit scale (tests state it through this).
     bf16 has no fixed bar: it is 2 x `composed_err` + BF16_FLOOR, where `composed_err` is the error (same fraction of the
     scale) of the reference's op composition (modules.composed_path()) on the same inputs under the same autocast — so the
-    caller measures it first (tests/test_bf16_gpu.py)."""
+    caller measures it first (tests/test_bf16_gpu.py).  fp8 likewise, with the composed path run under bf16 autocast and the
+    mode's e4m3 quantize-dequantize at the GEMMs it quantizes (tests/test_fp8_gpu.py)."""
     mode = precision()
-    if mode == "bf16":
+    if mode in ("bf16", "fp8"):
         if composed_err is None:
-            raise ValueError("logits_bar(): the bf16 bar is relative; pass the composed path's error under the same autocast")
+            raise ValueError(f"logits_bar(): the {mode} bar is relative; pass the composed path's error under the same autocast")
         return 2.0 * composed_err + BF16_FLOOR
     return 1e-2 if mode == "tf32" else 1e-3
 
 
 def _bf16_mode():
-    return precision() == "bf16"
+    """bf16 interior storage: the bf16 and the FP8 modes"""
+    return precision() in ("bf16", "fp8")
+
+
+def _fp8_mode():
+    return precision() == "fp8"
 
 
 def _no_autocast():
@@ -89,7 +153,8 @@ def _no_autocast():
 
 _FP32_KINDS = set()   # experiment hook (scripts/tf32_error_budget.py): kinds of projections forced to full precision in tf32 mode
 _SPLIT = {}           # id(weight) -> (weakref, version, W_hi, W_lo): the tf32x3 operand split of a weight, made once per version
-_BF16 = {}            # id(weight) -> (weakref, version, W_bf16): the bf16 copy of a weight, made once per version
+_LOWP = {}            # id(weight) -> (weakref, version, {form: copy}): the bf16 copy ("bf16") and the per-channel e4m3 rows
+                      # and scales ("e4m3") of a weight, each made once per version
 
 
 def _split_weight(w):
@@ -104,15 +169,27 @@ def _split_weight(w):
     return hi, lo
 
 
-def _bf16_weight(w):
+def _lowp_weight(w, form):
     import weakref
-    ent = _BF16.get(id(w))
-    if ent is not None and ent[0]() is w and ent[1] == w._version:
-        return ent[2]
-    wb = w.detach().to(torch.bfloat16).contiguous()
-    key = id(w)
-    _BF16[key] = (weakref.ref(w, lambda _r, k=key: _BF16.pop(k, None)), w._version, wb)
-    return wb
+    ent = _LOWP.get(id(w))
+    if ent is None or ent[0]() is not w or ent[1] != w._version:
+        key = id(w)
+        ent = (weakref.ref(w, lambda _r, k=key: _LOWP.pop(k, None)), w._version, {})
+        _LOWP[key] = ent
+    forms = ent[2]
+    if form not in forms:
+        wc = w.detach().contiguous()
+        forms[form] = wc.to(torch.bfloat16) if form == "bf16" else quantize_rows(wc.float() if wc.dtype != torch.float32 else wc)
+    return forms[form]
+
+
+def _bf16_weight(w):
+    return _lowp_weight(w, "bf16")
+
+
+def _e4m3_weight(w):
+    """E4M3Rows of a (N, K) weight: one scale per output channel"""
+    return _lowp_weight(w, "e4m3")
 
 
 def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="dense", out_dtype=torch.float32):
@@ -126,7 +203,12 @@ def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="d
 
     A bf16 x2d runs the bf16 instance (sigma_linear_bf16: bf16 operands, fp32 accumulation) whatever `precision()` says, with a
     bf16 copy of the weight cached on `_version` exactly like the tf32x3 split (same `.data` limitation); the output is fp32 or
-    (out_dtype=torch.bfloat16) bf16.  Rows whose byte stride is not a multiple of 16 go to torch.mm."""
+    (out_dtype=torch.bfloat16) bf16.  Rows whose byte stride is not a multiple of 16 go to torch.mm.
+
+    An E4M3Rows x2d runs the e4m3 instance (sigma_linear_fp8) with the weight's per-channel e4m3 rows, cached the same way; K and
+    the row stride must be multiples of 16 and N of 4 (there is no other path for it)."""
+    if isinstance(x2d, E4M3Rows):
+        return _linear_fp8(x2d, weight, bias, out, residual, rscale, out_dtype)
     M, K = x2d.shape
     N = weight.shape[0]
     if x2d.dtype == torch.bfloat16:
@@ -175,6 +257,23 @@ def _linear_bf16(x2d, weight, bias, out, residual, rscale, out_dtype):
     rc = _lib.lib().sigma_linear_bf16(ptr(x2d), x2d.stride(0), ptr(w), ptr(bias), ptr(residual), ldr, ptr(rscale), ptr(out), out.stride(0),
                                       c_dtype, M, N, K, stream())
     _lib.check(rc, "sigma_linear_bf16")
+    return out
+
+
+def _linear_fp8(xq, weight, bias, out, residual, rscale, out_dtype):
+    q = xq.q
+    M, K = q.shape
+    N = weight.shape[0]
+    if K % 16 or q.stride(1) != 1 or q.stride(0) % 16 or N % 4:
+        raise ValueError(f"fused.linear: the e4m3 GEMM needs K and the row stride % 16 == 0 and N % 4 == 0 (K={K}, N={N})")
+    if out is None:
+        out = torch.empty((M, N), dtype=out_dtype, device=q.device)
+    w = _e4m3_weight(weight)
+    ldr = residual.stride(0) if residual is not None else 0
+    c_dtype = _lib.BF16 if out.dtype == torch.bfloat16 else _lib.F32
+    rc = _lib.lib().sigma_linear_fp8(ptr(q), q.stride(0), ptr(xq.s), ptr(w.q), ptr(w.s), ptr(bias), ptr(residual), ldr, ptr(rscale),
+                                     ptr(out), out.stride(0), c_dtype, M, N, K, stream())
+    _lib.check(rc, "sigma_linear_fp8")
     return out
 
 
@@ -274,9 +373,18 @@ def ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
 
 def merge_norm_gate(y, K, k_stride, in_batch_stride, ln, z, z_row_stride, gate, out, out_batch_stride, out_row_stride,
                     rows, rows_per_batch, D, y_offset=0, out_offset=0):
-    """y, z and out all fp32, or all bf16 (sigma_merge_norm_gate_fwd_bf16); offsets and strides count elements."""
-    fn = "sigma_merge_norm_gate_fwd_bf16" if y.dtype == torch.bfloat16 else "sigma_merge_norm_gate_fwd"
+    """y, z and out all fp32, or all bf16 (sigma_merge_norm_gate_fwd_bf16); offsets and strides count elements.  out = E4M3Rows
+    (y, z bf16): sigma_merge_norm_gate_fwd_fp8, whose row r's scale lands at out.s[out_offset / out_row_stride + r]."""
     yp = ctypes.c_void_p(y.data_ptr() + y.element_size() * y_offset)
+    if isinstance(out, E4M3Rows):
+        qp = ctypes.c_void_p(out.q.data_ptr() + out_offset)
+        sp = ctypes.c_void_p(out.s.data_ptr() + 4 * (out_offset // out_row_stride))
+        rc = _lib.lib().sigma_merge_norm_gate_fwd_fp8(yp, K, k_stride, in_batch_stride, ptr(ln.weight), ptr(ln.bias), z, z_row_stride,
+                                                      ptr(gate), qp, sp, out_batch_stride, out_row_stride, rows, rows_per_batch, D,
+                                                      float(ln.eps), stream())
+        _lib.check(rc, "sigma_merge_norm_gate_fwd_fp8")
+        return out
+    fn = "sigma_merge_norm_gate_fwd_bf16" if y.dtype == torch.bfloat16 else "sigma_merge_norm_gate_fwd"
     op = ctypes.c_void_p(out.data_ptr() + out.element_size() * out_offset)
     rc = getattr(_lib.lib(), fn)(yp, K, k_stride, in_batch_stride, ptr(ln.weight), ptr(ln.bias), z, z_row_stride,
                                  ptr(gate), op, out_batch_stride, out_row_stride, rows, rows_per_batch, D, float(ln.eps), stream())
@@ -339,16 +447,23 @@ def ss2d(m, x, residual=None, rscale=None):
     """SS2D.forward (vmamba.py:1067-1089); x (B,H,W,C) contiguous.  Returns (B,H,W,C) [+ residual (· rscale)], the
     residual being added in the out_proj GEMM epilogue."""
     dt = torch.bfloat16 if _bf16_mode() else torch.float32     # storage of the block's interior (module docstring)
-    x = x.to(dt).contiguous()
-    B, H, W, C = x.shape
+    fp8 = _fp8_mode()
+    if isinstance(x, E4M3Rows):                                 # the FP8 mode's LayerNorm output (vss_block, cvss_decoder_block)
+        B, H, W, C = x.q.shape
+        xa = x.view(B * H * W, C)
+    else:
+        x = x.contiguous() if fp8 else x.to(dt).contiguous()
+        B, H, W, C = x.shape
+        xa = quantize_rows(x.view(B * H * W, C)) if fp8 else x.view(B * H * W, C)
     D, N, R, L = m.d_inner, m.d_state, m.dt_rank, H * W
     c = _ssm_params(m)
-    xz = linear(x.view(B * L, C), m.in_proj.weight, m.in_proj.bias, kind="in_proj", out_dtype=dt)      # (BL, 2D): [x | z]
-    xc = torch.empty((B, L, D), dtype=dt, device=x.device)
+    dev = xa.q.device if fp8 else xa.device
+    xz = linear(xa, m.in_proj.weight, m.in_proj.bias, kind="in_proj", out_dtype=dt)                   # (BL, 2D): [x | z]
+    xc = torch.empty((B, L, D), dtype=dt, device=dev)
     dwconv3x3_silu(xz, 2 * D, L * 2 * D, m.conv2d, xc, L * D, B, H, W, D)
     xdbl = linear(xc.view(B * L, D), c["xproj"], kind="x_proj")                                        # (BL, 4·Cp) fp32
     y = ss2d_scan(_lib.DIRS_CROSS4, xc, xdbl, c["dtw"], c["dtb"], c["A"], c["Ds"], B, H, W, D, N, R, c["Cp"])
-    yg = torch.empty((B * L, D), dtype=dt, device=x.device)
+    yg = _e4m3_empty(B * L, D, dev) if fp8 else torch.empty((B * L, D), dtype=dt, device=dev)
     z = ctypes.c_void_p(xz.data_ptr() + xz.element_size() * D)
     merge_norm_gate(y, 4, B * L * D, 0, m.out_norm, z, 2 * D, None, yg, 0, D, B * L, B * L, D)
     res2d = residual.reshape(B * L, C) if residual is not None else None
@@ -359,11 +474,16 @@ def _interior_dtype():
     return torch.bfloat16 if _bf16_mode() else torch.float32
 
 
+def _ln_out_dtype():
+    """the dtype of a LayerNorm output that feeds in_proj: E4M3Rows in the FP8 mode, else the interior storage"""
+    return torch.float8_e4m3fn if _fp8_mode() else _interior_dtype()
+
+
 def vss_block(blk, x):
     """VSSBlock._forward (vmamba.py:1712-1716), mlp_ratio = 0."""
     x = x.contiguous()
     B, H, W, C = x.shape
-    xn = layernorm(x.view(-1, C), blk.norm, _interior_dtype()).view(B, H, W, C)
+    xn = layernorm(x.view(-1, C), blk.norm, _ln_out_dtype()).view(B, H, W, C)
     return ss2d(blk.op, xn, residual=x)
 
 
@@ -373,6 +493,11 @@ def patch_merging(m, x):
     B, H, W, C = x.shape
     H2, W2 = (H + 1) // 2, (W + 1) // 2
     bf16 = _bf16_mode()
+    if _fp8_mode():                                                  # the same kernel, quantizing its rows
+        xq = _e4m3_empty(B * H2 * W2, 4 * C, x.device)
+        _lib.check(_lib.lib().sigma_patch_merge_norm_fwd_fp8(ptr(x), ptr(m.norm.weight), ptr(m.norm.bias), ptr(xq.q), ptr(xq.s), B, H, W, C,
+                                                             float(m.norm.eps), stream()), "sigma_patch_merge_norm_fwd_fp8")
+        return linear(xq, m.reduction.weight).view(B, H2, W2, -1)
     xn = torch.empty((B * H2 * W2, 4 * C), dtype=torch.bfloat16 if bf16 else torch.float32, device=x.device)
     # 2x2 gather (+ zero padding of odd sizes) + LayerNorm(4C) in one kernel: no concatenated tensor
     fn = "sigma_patch_merge_norm_fwd_bf16" if bf16 else "sigma_patch_merge_norm_fwd"
@@ -390,23 +515,31 @@ def cromb_ss2d(m, x_rgb, x_e, residual=False):
     c = _cma_params(cm)
     dev = x_rgb.device
     dt = _interior_dtype()
-    a_r, a_e = x_rgb.to(dt), x_e.to(dt)                                        # GEMM operands (the residuals below stay fp32)
+    fp8 = _fp8_mode()
+    if fp8:                                                                    # GEMM operands (the residuals below stay fp32)
+        a_r, a_e = quantize_rows(x_rgb.view(B * L, C)), quantize_rows(x_e.view(B * L, C))
+    else:
+        a_r, a_e = x_rgb.to(dt).view(B * L, C), x_e.to(dt).view(B * L, C)
     xp = torch.empty((2, B * L, D), dtype=dt, device=dev)                     # modality-major
-    linear(a_r.view(B * L, C), m.in_proj.weight, m.in_proj.bias, out=xp[0])
-    linear(a_e.view(B * L, C), m.in_proj_modalx.weight, m.in_proj_modalx.bias, out=xp[1])
+    linear(a_r, m.in_proj.weight, m.in_proj.bias, out=xp[0])
+    linear(a_e, m.in_proj_modalx.weight, m.in_proj_modalx.bias, out=xp[1])
     xc = torch.empty((2 * B, L, D), dtype=dt, device=dev)
     dwconv3x3_silu(xp, D, L * D, m.conv2d, xc, L * D, 2 * B, H, W, D)         # ONE conv for both modalities (:1629-1630)
     xdbl = torch.empty((2, B * L, c["Cp"]), dtype=torch.float32, device=dev)
     linear(xc[:B].view(B * L, D), c["xproj1"], out=xdbl[0], kind="x_proj")
     linear(xc[B:].view(B * L, D), c["xproj2"], out=xdbl[1], kind="x_proj")
     y = ss2d_scan(_lib.DIRS_CROSS, xc, xdbl, c["dtw"], c["dtb"], c["A"], c["Ds"], 2 * B, H, W, D, N, R, c["Cp"])  # (1,2B,L,D)
-    yn = torch.empty((2, B * L, D), dtype=dt, device=dev)
+    yn = _e4m3_empty(2 * B * L, D, dev) if fp8 else torch.empty((2 * B * L, D), dtype=dt, device=dev)
     merge_norm_gate(y, 1, 0, 0, cm.out_norm_1, None, 0, None, yn, 0, D, B * L, B * L, D)
     merge_norm_gate(y, 1, 0, 0, cm.out_norm_2, None, 0, None, yn, 0, D, B * L, B * L, D, y_offset=B * L * D, out_offset=B * L * D)
+    if fp8:
+        yn_r, yn_e = E4M3Rows(yn.q[:B * L], yn.s[:B * L]), E4M3Rows(yn.q[B * L:], yn.s[B * L:])
+    else:
+        yn_r, yn_e = yn[:B * L], yn[B * L:]
     r_r = x_rgb.view(B * L, C) if residual else None
     r_e = x_e.view(B * L, C) if residual else None
-    o_r = linear(yn[0], m.out_proj_rgb.weight, m.out_proj_rgb.bias, residual=r_r).view(B, H, W, C)
-    o_e = linear(yn[1], m.out_proj_e.weight, m.out_proj_e.bias, residual=r_e).view(B, H, W, C)
+    o_r = linear(yn_r, m.out_proj_rgb.weight, m.out_proj_rgb.bias, residual=r_r).view(B, H, W, C)
+    o_e = linear(yn_e, m.out_proj_e.weight, m.out_proj_e.bias, residual=r_e).view(B, H, W, C)
     return o_r, o_e
 
 
@@ -418,8 +551,13 @@ def conmb_ss2d(m, x_rgb, x_e, residual=None):
     c = _ssm_params(m)
     dev = x_rgb.device
     dt = _interior_dtype()
-    tr = linear(x_rgb.to(dt).view(B * L, C), m.in_proj.weight, m.in_proj.bias, out_dtype=dt)
-    te = linear(x_e.to(dt).view(B * L, C), m.in_proj_modalx.weight, m.in_proj_modalx.bias, out_dtype=dt)
+    fp8 = _fp8_mode()
+    if fp8:
+        a_r, a_e = quantize_rows(x_rgb.view(B * L, C)), quantize_rows(x_e.view(B * L, C))
+    else:
+        a_r, a_e = x_rgb.to(dt).view(B * L, C), x_e.to(dt).view(B * L, C)
+    tr = linear(a_r, m.in_proj.weight, m.in_proj.bias, out_dtype=dt)
+    te = linear(a_e, m.in_proj_modalx.weight, m.in_proj_modalx.bias, out_dtype=dt)
     seq = torch.empty((B, 2 * L, D), dtype=dt, device=dev)                    # [rgb ‖ x] along L (vmamba.py:130)
     dwconv3x3_silu(tr, D, L * D, m.conv2d, seq, 2 * L * D, B, H, W, D)
     dwconv3x3_silu(te, D, L * D, m.conv2d_modalx, seq[:, L:], 2 * L * D, B, H, W, D)
@@ -435,6 +573,8 @@ def conmb_ss2d(m, x_rgb, x_e, residual=None):
     merge_norm_gate(y, 2, ks, 2 * L * D, m.out_norm2, None, 0, g_r, ycat, L * 2 * D, 2 * D, B * L, L, D,
                     y_offset=L * D, out_offset=D)
     res2d = residual.reshape(B * L, C) if residual is not None else None
+    if fp8:                                                                   # the two halves come from two calls: quantize the row here
+        ycat = quantize_rows(ycat)
     return linear(ycat, m.out_proj.weight, m.out_proj.bias, residual=res2d).view(B, H, W, C)
 
 
@@ -494,7 +634,7 @@ def cvss_decoder_block(blk, x):
     """CVSSDecoderBlock._forward (vmamba.py:1800-1805) with ChannelAttentionBlock (vmamba.py:1725-1757)."""
     x = x.contiguous()
     B, H, W, C = x.shape
-    xn = layernorm(x.view(-1, C), blk.norm1, _interior_dtype()).view(B, H, W, C)
+    xn = layernorm(x.view(-1, C), blk.norm1, _ln_out_dtype()).view(B, H, W, C)
     x1 = ss2d(blk.op, xn, residual=x, rscale=blk.scale1)            # x·scale1 + SS2D(LN(x)) in the GEMM epilogue
     xn2 = layernorm(x1.view(-1, C), blk.norm2).view(B, H, W, C)
     cab = blk.conv_blk.cab

@@ -31,11 +31,14 @@ class InferencePipeline:
     version counters and re-captures the graph, so stale packed copies are never replayed.
 
     amp_dtype=torch.bfloat16 runs the forward (warm-up, capture and any re-capture) under torch.autocast("cuda", dtype=amp_dtype),
-    so the captured graph is the one of the fused path's bf16 mode (sigma_b200.fused.precision); None runs it as called."""
+    so the captured graph is the one of the fused path's bf16 mode (sigma_b200.fused.precision); None runs it as called.
+    fp8=True runs them inside sigma_b200.fused.fp8_inference(), so the graph is the one of the FP8 mode (the per-channel e4m3
+    weights it reads are re-quantized, like the packed SSM tensors, when a re-capture follows a weight change)."""
 
-    def __init__(self, model, batch, height, width, use_graph=True, amp_dtype=None):
+    def __init__(self, model, batch, height, width, use_graph=True, amp_dtype=None, fp8=False):
         self.model = model
         self.amp_dtype = amp_dtype
+        self.fp8 = fp8
         p = next(model.parameters())
         if p.device.type != "cuda":
             raise RuntimeError("sigma_b200.InferencePipeline needs the model on a CUDA device (there is no CPU path)")
@@ -64,7 +67,14 @@ class InferencePipeline:
         return sum(p._version for p in self.model.parameters())
 
     def _autocast(self):
-        return torch.autocast("cuda", dtype=self.amp_dtype) if self.amp_dtype is not None else contextlib.nullcontext()
+        """the forward's precision context: autocast (amp_dtype) and / or the FP8 mode"""
+        from . import fused
+        stack = contextlib.ExitStack()
+        if self.amp_dtype is not None:
+            stack.enter_context(torch.autocast("cuda", dtype=self.amp_dtype))
+        if self.fp8:
+            stack.enter_context(fused.fp8_inference())
+        return stack
 
     def _capture(self):
         with torch.cuda.stream(self.compute), torch.no_grad(), self._autocast():
