@@ -377,9 +377,16 @@ int sigma_conv3x3_tf32(const float *x, const float *w9, const float *w9_lo, cons
  * the current environment.  out6_host = {tile width, ring stages, persistent grid, output tiles, dynamic shared memory bytes, CTAs
  * per SM}.  The environment variable SIGMA_GEMM_BN=<w> forces the tile width of both calls (a multiple of 32 in [32, 256], read
  * per call; any other value makes the calls and this query return SIGMA_EINVAL).  For tests and tuning.
- * x3 selects the instance: 0 = tf32, 1 = tf32x3, 2 = sigma_linear_bf16, 4 = sigma_linear_fp8 (conv_B must be 0 for 2 and 4; the
- * e4m3 tiles are 32 or 64 wide, and forcing a wider one is SIGMA_EINVAL); other values (3 included) are SIGMA_EINVAL.        */
+ * x3 selects the instance: 0 = tf32, 1 = tf32x3 with register-stored output tiles (the conv and
+ * sigma_test_linear_tf32x3_regs), 2 = sigma_linear_bf16, 4 = sigma_linear_fp8, 5 = tf32x3 with TMA-stored output tiles
+ * (sigma_linear_tf32x3); conv_B must be 0 for 2, 4 and 5; the e4m3 tiles are 32 or 64 wide, and forcing a wider one is
+ * SIGMA_EINVAL; other values (3 included) are SIGMA_EINVAL.                                                                   */
 int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, int64_t *out6_host);
+/* sigma_linear_tf32x3 (same arguments and checks) with the output tiles stored from registers instead of through shared memory
+ * and TMA: the same products and epilogue operations, so the same bits.  For tests.                                          */
+int sigma_test_linear_tf32x3_regs(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias,
+                                  const float *residual, int64_t ldr, const float *rscale, float *C, int64_t ldc, int64_t M, int N,
+                                  int K, void *stream);
 
 /* L-segment plan of the fused scan backward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_bwd (nsplit = 0)
  * or sigma_ss2d_scan_bwd_split / sigma_ss2d_scan_bwd_saved with that nsplit would launch for kind CROSS4 / SEQ2 / CROSS (even

@@ -921,8 +921,8 @@ int sigma_quantize_e4m3_rows(const void *x, int x_dtype, int64_t ldx, void *q, i
   return quantize_e4m3_rows_launch(x, x_dtype == SIGMA_BF16, ldx, q, ldq, scale, rows, C, (cudaStream_t)stream);
 }
 
-int sigma_linear_tf32x3(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias, const float *residual,
-                        int64_t ldr, const float *rscale, float *C, int64_t ldc, int64_t M, int N, int K, void *stream) {
+static int linear_tf32x3(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias, const float *residual,
+                         int64_t ldr, const float *rscale, float *C, int64_t ldc, int64_t M, int N, int K, void *stream, bool reg_epilogue) {
   SIGMA_CHECK_ARG(A && W_hi && W_lo && C, "sigma_linear_tf32x3: null pointer");
   SIGMA_CHECK_ARG(M >= 0 && M < (1LL << 31) && N > 0 && K > 0, "sigma_linear_tf32x3: bad sizes M=%lld N=%d K=%d", (long long)M, N, K);
   SIGMA_CHECK_ARG(K % 4 == 0 && N % 4 == 0 && lda % 4 == 0 && ldc % 4 == 0 && (residual == nullptr || ldr % 4 == 0) && lda >= K && ldc >= N,
@@ -930,7 +930,18 @@ int sigma_linear_tf32x3(const float *A, int64_t lda, const float *W_hi, const fl
   SIGMA_CHECK_ARG(al16(A) && al16(W_hi) && al16(W_lo) && al16(C) && al16(bias) && al16(residual) && al16(rscale),
                   "sigma_linear_tf32x3: pointers must be 16-byte aligned");
   SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "sigma_linear_tf32x3: rscale without residual");
-  return gemm_tf32_launch(A, lda, W_hi, W_lo, bias, residual, ldr, rscale, C, ldc, M, N, K, (cudaStream_t)stream);
+  return gemm_tf32_launch(A, lda, W_hi, W_lo, bias, residual, ldr, rscale, C, ldc, M, N, K, (cudaStream_t)stream, reg_epilogue);
+}
+
+int sigma_linear_tf32x3(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias, const float *residual,
+                        int64_t ldr, const float *rscale, float *C, int64_t ldc, int64_t M, int N, int K, void *stream) {
+  return linear_tf32x3(A, lda, W_hi, W_lo, bias, residual, ldr, rscale, C, ldc, M, N, K, stream, false);
+}
+
+int sigma_test_linear_tf32x3_regs(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias,
+                                  const float *residual, int64_t ldr, const float *rscale, float *C, int64_t ldc, int64_t M, int N,
+                                  int K, void *stream) {
+  return linear_tf32x3(A, lda, W_hi, W_lo, bias, residual, ldr, rscale, C, ldc, M, N, K, stream, true);
 }
 
 int sigma_conv3x3_tf32(const float *x, const float *w9, const float *w9_lo, const float *bias, int act, float *y, int batch, int H, int W,

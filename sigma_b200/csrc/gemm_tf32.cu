@@ -9,7 +9,8 @@
 // 128 x BN tile (its own A half, all of W) and issuing the MMAs for them; warp 8 = TMA producer.  Persistent CTAs loop over
 // 128 x BN output tiles (BN a multiple of 32 up to 256, one template instance per width, chosen per call); the producer
 // runs ahead across tile boundaries, so the loads of the next tile overlap the epilogue of the current one.  The epilogue
-// adds bias / residual·rscale to the register accumulators and stores them directly (each warp store covers 8 rows x 32 B).
+// adds bias / residual·rscale to the register accumulators and stores them directly (each warp store covers 8 rows x 32 B);
+// the tf32x3 linear instance (gemm_x3_tma_kernel) stages them in shared memory and stores them with TMA instead (TMA_C).
 // These GEMMs are HBM-bound at the Sigma shapes (K = 96..1536): what matters is one pass over A and one over C.
 //
 // X3 = true ("tf32x3", sigma_linear_tf32x3): fp32-grade products on the TF32 tensor pipe by error compensation,
@@ -47,7 +48,21 @@ struct alignas(64) GemmParams {
   int c_bf16;       // BF16: 1 = C is stored as bf16 (bias / residual / rscale stay fp32)
   int cH, cW, tiles_w, tiles_hw, kbc, act;   // CONV: image size, 8x16 patches per row / per image, Cin blocks per tap, activation
   const float *sa, *sw;   // FP8: per-row scales of A, per-output-channel scales of W
+  CUtensorMap m_c, m_r;   // TMA_C: C and (if any) the residual, GM_CHUNK x 64 boxes
 };
+
+// One ring stage holds a k-block's K-major, 128-byte-swizzled operand tiles, each 1024-aligned: [A | W].  tf32x3 adds W_lo:
+// the register-stored epilogue's stage is [A | W][A_lo | W_lo], whose A_lo tile nothing writes (A is split in registers), and
+// the TMA-stored epilogue's is [A | W_hi | W_lo].  gemm_body's offsets and plan_gemm's sizes both come from here.
+__host__ __device__ constexpr int gemm_w_bytes(int bn) { return (bn * GM_BK * 4 + 1023) & ~1023; }
+__host__ __device__ constexpr int gemm_stage_bytes(int bn, bool x3, bool tma_c) {
+  return tma_c ? GM_BM * GM_BK * 4 + 2 * gemm_w_bytes(bn) : (GM_BM * GM_BK * 4 + gemm_w_bytes(bn)) * (x3 ? 2 : 1);
+}
+// TMA-stored epilogue: each consumer warpgroup stages its 64 rows in chunks of GM_CHUNK columns (one 128-byte swizzle row per
+// row, 8 KB) through two buffers after the ring
+constexpr int GM_CHUNK = 32;
+constexpr int GM_CHUNK_BYTES = 64 * GM_CHUNK * 4;
+constexpr int GM_STAGING_BYTES = 2 * 2 * GM_CHUNK_BYTES;
 
 constexpr int CV_TH = 8, CV_TW = 16;   // pixel patch of one M tile (8 x 16 = GM_BM)
 
@@ -615,22 +630,41 @@ template <> __device__ __forceinline__ void wgmma_e4m3<64>(float (&d)[32], uint6
       : "l"(da), "l"(db), "r"(scale_d));
 }
 
+// shared -> global, 2-D tile, bulk-group completion (SASS: UTMASTG); out-of-bounds elements are not written
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void *smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"((uint64_t)map),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+
+// TMA_C: residual chunk number e of a warpgroup, columns col.. and rows row.. of the residual, into staging buffer e % 2
+__device__ __forceinline__ void load_residual_chunk(const GemmParams &p, unsigned char *stg, uint64_t *rfull, uint32_t e, int col,
+                                                    int row) {
+  mbar_arrive_expect_tx(&rfull[e & 1], GM_CHUNK_BYTES);
+  tma_load_2d(stg + (e & 1) * GM_CHUNK_BYTES, &p.m_r, &rfull[e & 1], col, row);
+}
+
 // The body of every instance.  FP8 (gemm_fp8_kernel): e4m3 operands, 128 per k-block; each k-block's four k32 MMAs accumulate
 // into a zeroed fragment that is then added to the fp32 accumulators in registers (the tensor core's e4m3 accumulation keeps
 // fewer bits than fp32, DESIGN §5.4), and the epilogue scales acc[row, col] by sa[row]·sw[col] before the bias / residual.
-template <int BN, bool X3, bool CONV, bool BF16, bool FP8>
+// TMA_C (gemm_x3_tma_kernel): the epilogue stages each warpgroup's output in GM_CHUNK-column chunks in shared memory and
+// stores them with TMA, asynchronously, so the consumers go on to the next tile's MMAs while the stores drain; the residual
+// chunks arrive by TMA as well, the first two during the tile's k-loop.
+template <int BN, bool X3, bool CONV, bool BF16, bool FP8, bool TMA_C = false>
 __device__ __forceinline__ void gemm_body(const GemmParams &p) {
   static_assert(!BF16 || (!X3 && !CONV), "the bf16 instance is a plain GEMM");
   static_assert(!FP8 || (!X3 && !CONV && !BF16), "the e4m3 instance is a plain GEMM");
+  static_assert(!TMA_C || (X3 && !CONV), "the TMA-stored epilogue is the tf32x3 linear instance's");
   constexpr int KB = FP8 ? 4 * GM_BK : BF16 ? 2 * GM_BK : GM_BK;   // elements per k-block: one 128-byte swizzle row in every case
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const int S = p.stages;
   constexpr int a_bytes = GM_BM * GM_BK * 4, b_bytes = BN * GM_BK * 4;
   constexpr int a_half = a_bytes / 2;                                // one warpgroup's 64 rows
-  constexpr int half_bytes = a_bytes + ((b_bytes + 1023) & ~1023);   // [A | W] ; X3: a second [A_lo | W_lo] follows
-  constexpr int stage_bytes = X3 ? 2 * half_bytes : half_bytes;
-  uint64_t *full = reinterpret_cast<uint64_t *>(smem_raw + (size_t)S * stage_bytes);
+  constexpr int stage_bytes = gemm_stage_bytes(BN, X3, TMA_C);
+  constexpr int wlo_off = TMA_C ? a_bytes + gemm_w_bytes(BN) : stage_bytes / 2 + a_bytes;   // X3: the W_lo tile in a stage
+  uint64_t *full = reinterpret_cast<uint64_t *>(smem_raw + (size_t)S * stage_bytes + (TMA_C ? GM_STAGING_BYTES : 0));
   uint64_t *empty = full + S;
+  uint64_t *rfull = empty + S;   // TMA_C: residual chunk loaded, one per staging buffer
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nkb = CONV ? 9 * p.kbc : (p.K + KB - 1) / KB;
@@ -642,6 +676,7 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
     tma_prefetch_desc(&p.m_a);
     tma_prefetch_desc(&p.m_w);
     for (int s = 0; s < S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+    if (TMA_C) for (int i = 0; i < 4; ++i) mbar_init(&rfull[i], 1);
     fence_mbar_init();
   }
   __syncthreads();
@@ -665,11 +700,11 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
             // the tap's input patch: shifted by (dy-1, dx-1); rows / columns outside the image arrive as zeros = the padding
             tma_load_4d(sa, &p.m_a, &full[st], kc * GM_BK, tx * CV_TW + dx - 1, ty * CV_TH + dy - 1, b);
             tma_load_2d(sa + a_bytes, &p.m_w, &full[st], kc * GM_BK, tap * p.N + n0);
-            if (X3) tma_load_2d(sa + half_bytes + a_bytes, &p.m_wlo, &full[st], kc * GM_BK, tap * p.N + n0);
+            if (X3) tma_load_2d(sa + wlo_off, &p.m_wlo, &full[st], kc * GM_BK, tap * p.N + n0);
           } else {
             tma_load_2d(sa, &p.m_a, &full[st], kb * KB, m0);
             tma_load_2d(sa + a_bytes, &p.m_w, &full[st], kb * KB, n0);
-            if (X3) tma_load_2d(sa + half_bytes + a_bytes, &p.m_wlo, &full[st], kb * GM_BK, n0);
+            if (X3) tma_load_2d(sa + wlo_off, &p.m_wlo, &full[st], kb * GM_BK, n0);
           }
         }
       }
@@ -685,7 +720,25 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
   // chunk c ^ (r % 8), which also puts the 8 rows of each matrix in distinct banks.
   const uint32_t a_lane = (uint32_t)(16 * (warp & 3) + 8 * ((lane >> 3) & 1) + (lane & 7)) * 128u + (uint32_t)(((lane >> 4) ^ (lane & 7)) << 4);
   long long it = 0;
+  // TMA_C: this warpgroup's two staging buffers; chunk number e (counted over the CTA's tiles) uses buffer e % 2, whose
+  // (e / 2)-th residual load completes phase (e / 2) % 2 of rfull[2·wg + e % 2].  Thread t = 0 issues and waits for the bulk
+  // copies of the warpgroup.
+  unsigned char *stg = smem_raw + (size_t)S * stage_bytes + wg * 2 * GM_CHUNK_BYTES;
+  uint32_t ec = 0;
+  // TMA_C: the warpgroup's 64 x BN block of a tile starts at row m0, column n0; nch of its chunks hold any of C (none when
+  // its rows are past M)
+  const auto block = [&](long long tile, int &m0, int &n0) {
+    m0 = (int)(tile / num_n) * GM_BM + 64 * wg;
+    n0 = (int)(tile % num_n) * BN;
+    return m0 < p.M ? min(BN / GM_CHUNK, (p.N - n0 + GM_CHUNK - 1) / GM_CHUNK) : 0;
+  };
   for (long long tile = blockIdx.x; tile < total; tile += gridDim.x) {
+    if (TMA_C && p.residual && t == 0) {
+      int m0, n0;
+      const int nch = block(tile, m0, n0);
+      tma_store_wait_read<0>();                 // the previous tile's stores have left both buffers
+      for (int c = 0; c < min(nch, 2); ++c) load_residual_chunk(p, stg, &rfull[2 * wg], ec + c, n0 + GM_CHUNK * c, m0);
+    }
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -698,10 +751,9 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
         // A from registers, W_hi / W_lo from shared memory.  Per k8 step, two commit groups, small terms first: {A_lo·W_hi}
         // and {A_hi·W_lo, A_hi·W_hi}.  Each group's fragment is loaded from the stage and split just before it is issued, after
         // a wait_group 1 has retired the group before the previous one, so at most 8 fragment registers are live (the
-        // 2-CTA-per-SM widths have 96 registers for 64 accumulators) while one group is always queued.  The stage keeps its
-        // [A | W][A_lo | W_lo] layout, which the launch plan sizes, but its A_lo tile is no longer written.
+        // 2-CTA-per-SM widths have 96 registers for 64 accumulators) while one group is always queued.
         const uint32_t a_frag = smem_u32(sa + wg * a_half) + a_lane;
-        const uint64_t db = wgmma_desc_sw128(sa + a_bytes), dbl = wgmma_desc_sw128(sa + half_bytes + a_bytes);
+        const uint64_t db = wgmma_desc_sw128(sa + a_bytes), dbl = wgmma_desc_sw128(sa + wlo_off);
 #pragma unroll
         for (int k = 0; k < GM_BK / GM_UK; ++k) {
           const uint32_t addr = a_frag ^ (uint32_t)(32 * k);   // the stage is 1024-aligned: bits 4-6 of a_frag are the row's XOR
@@ -766,6 +818,57 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
     acc_fence(acc);
     if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
 
+    if constexpr (TMA_C) {
+      // per chunk: bias / residual·rscale added in registers (the register-stored epilogue's operations, in its order) into
+      // the staging buffer in the C map's 128-byte-swizzled box layout, then one TMA store; TMA clips the M tail and the
+      // columns past N.  The buffer a chunk writes was last stored from two chunks earlier: t = 0 waits for that store to be
+      // read out before the warpgroup barrier that precedes the next chunk's writes (with a residual, before its reload).
+      int m0, c_n0;
+      const int nch = block(tile, m0, c_n0);
+      const int rr = 16 * (warp & 3) + (lane >> 2);   // this lane's rows rr, rr + 8 of the block
+#pragma unroll
+      for (int c = 0; c < BN / GM_CHUNK; ++c) {
+        if (c >= nch) break;
+        const uint32_t e = ec + c;
+        const uint32_t buf = smem_u32(stg) + (e & 1) * GM_CHUNK_BYTES;
+        if (p.residual) mbar_wait(&rfull[2 * wg + (e & 1)], (e >> 1) & 1);
+#pragma unroll
+        for (int i = 0; i < GM_CHUNK / 8; ++i) {
+          const int n = c_n0 + GM_CHUNK * c + 8 * i + 2 * (lane & 3);
+          const bool in = n < p.N;                     // N is even, so a column pair is all-in or all-out
+          const float2 b = p.bias && in ? __ldg(reinterpret_cast<const float2 *>(p.bias + n)) : make_float2(0.f, 0.f);
+          const float2 sc = p.rscale && in ? __ldg(reinterpret_cast<const float2 *>(p.rscale + n)) : make_float2(0.f, 0.f);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = rr + 8 * h;
+            const uint32_t q = buf + r * 128 + (((2 * i + ((lane & 3) >> 1)) ^ (r & 7)) << 4) + ((lane & 1) << 3);
+            float2 o = make_float2(acc[4 * (GM_CHUNK / 8 * c + i) + 2 * h], acc[4 * (GM_CHUNK / 8 * c + i) + 2 * h + 1]);
+            if (p.bias) { o.x += b.x; o.y += b.y; }
+            if (p.residual) {
+              float2 rv;
+              asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(rv.x), "=f"(rv.y) : "r"(q) : "memory");
+              if (p.rscale) { o.x = fmaf(rv.x, sc.x, o.x); o.y = fmaf(rv.y, sc.y, o.y); }
+              else { o.x += rv.x; o.y += rv.y; }
+            }
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(q), "f"(o.x), "f"(o.y) : "memory");
+          }
+        }
+        fence_proxy_async();
+        if (t == 0) tma_store_wait_read<0>();
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+        if (t == 0) {
+          tma_store_2d(&p.m_c, stg + (e & 1) * GM_CHUNK_BYTES, c_n0 + GM_CHUNK * c, m0);
+          tma_store_commit();
+          if (p.residual && c + 2 < nch) {
+            tma_store_wait_read<0>();
+            load_residual_chunk(p, stg, &rfull[2 * wg], e + 2, c_n0 + GM_CHUNK * (c + 2), m0);
+          }
+        }
+      }
+      ec += nch;
+      continue;
+    }
+
     // epilogue: accumulator fragment (m64nBN, f32): acc[4i + 2h + j] = row 16·(warp % 4) + lane / 4 + 8h,
     // column 8i + 2·(lane % 4) + j of this warpgroup's 64 x BN block
     const int mt = (int)(tile / num_n), n0 = (int)(tile % num_n) * BN;
@@ -825,11 +928,19 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
       }
     }
   }
+  if (TMA_C && t == 0) tma_store_wait_all<0>();   // the shared memory the stores read stays until they are done
 }
 
 template <int BN, bool X3, bool CONV, bool BF16 = false>
 __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_tf32_kernel(const __grid_constant__ GemmParams p) {
   gemm_body<BN, X3, CONV, BF16, false>(p);
+}
+
+// The tf32x3 linear instance with the TMA-stored epilogue: fp32 C (and residual) whose rows a tensor map can describe.
+// Widths up to 96 run two CTAs per SM; from 128 on, the staging buffers leave room for one (plan_gemm) and its registers.
+template <int BN>
+__global__ void __launch_bounds__(GM_THREADS, BN < 128 ? 2 : 1) gemm_x3_tma_kernel(const __grid_constant__ GemmParams p) {
+  gemm_body<BN, true, false, false, false, true>(p);
 }
 
 // The FP8 instance.  Its two accumulator sets (acc and the k-block fragment) need BN registers per thread; at BN <= kFp8MaxBn
@@ -923,8 +1034,10 @@ static int forced_bn() {
 constexpr int kFp8MaxBn = 64;
 
 // conv_B > 0: the implicit-GEMM 3x3 convolution of a (conv_B, conv_H, conv_W, K) input with N output channels (M unused).
-// fp8: the e4m3 instance (widths up to kFp8MaxBn, two CTAs per SM)
-static int plan_gemm(long long M, int N, int K, bool x3, int conv_B, int conv_H, int conv_W, GemmPlan *pl, bool fp8 = false) {
+// fp8: the e4m3 instance (widths up to kFp8MaxBn, two CTAs per SM).  tma_c: the tf32x3 linear instance with the TMA-stored
+// epilogue, whose staging buffers come out of the budget before the ring.
+static int plan_gemm(long long M, int N, int K, bool x3, int conv_B, int conv_H, int conv_W, GemmPlan *pl, bool fp8 = false,
+                     bool tma_c = false) {
   (void)K;   // the K loop does not enter the plan
   const bool conv = conv_B > 0;
   const long long m_tiles = conv ? (long long)conv_B * ((conv_W + CV_TW - 1) / CV_TW) * ((conv_H + CV_TH - 1) / CV_TH)
@@ -942,40 +1055,43 @@ static int plan_gemm(long long M, int N, int K, bool x3, int conv_B, int conv_H,
   if (fbn > 0) bn = fbn;
   pl->BN = bn;
   pl->tiles = m_tiles * ((N + bn - 1) / bn);
-  const int a_bytes = GM_BM * GM_BK * 4, b_bytes = bn * GM_BK * 4;
-  const int stage_bytes = (a_bytes + ((b_bytes + 1023) & ~1023)) * (x3 ? 2 : 1);
+  const int stage_bytes = gemm_stage_bytes(bn, x3, tma_c), staging = tma_c ? GM_STAGING_BYTES : 0;
   // up to 227 KB per block; tiles of <= 128 columns keep the ring small enough for two CTAs per SM (their register budget)
-  const int regs_ctas = bn <= (fp8 ? 64 : 128) ? 2 : 1;
-  const int budget = (regs_ctas == 2 ? 112 * 1024 : 226 * 1024) - 1024;
-  pl->stages = std::max(2, std::min(8, budget / stage_bytes));
-  pl->smem = (size_t)pl->stages * stage_bytes + 1024 /*barriers*/;
+  int regs_ctas = bn <= (fp8 ? 64 : 128) ? 2 : 1;
+  const auto ring = [&](int ctas) { return ((ctas == 2 ? 112 * 1024 : 226 * 1024) - 1024 - staging) / stage_bytes; };
+  // TMA-stored: where the staging and a two-stage ring no longer fit twice per SM, one CTA with a deeper ring
+  if (tma_c && regs_ctas == 2 && 2 * (2 * stage_bytes + staging + 2048) > 228 * 1024) regs_ctas = 1;
+  pl->stages = std::max(2, std::min(8, ring(regs_ctas)));
+  pl->smem = (size_t)pl->stages * stage_bytes + staging + 1024 /*barriers*/;
   pl->ctas_per_sm = std::max(1, std::min(regs_ctas, (int)((228 * 1024) / (pl->smem + 1024))));
   pl->grid = (unsigned)std::min<long long>(pl->tiles, (long long)kNumSMs * pl->ctas_per_sm);
   return SIGMA_OK;
 }
 
-// api.cu test hook: out = {BN, stages, grid, tiles, smem bytes, CTAs per SM}.  x3: 0 = tf32, 1 = tf32x3, 2 = bf16 (the bf16
-// instance stages the same bytes per k-block as tf32 — 128-byte rows — so its plan is the tf32 plan), 4 = e4m3 (the same stage
-// bytes too, narrower widths); 3 is not a mode
+// api.cu test hook: out = {BN, stages, grid, tiles, smem bytes, CTAs per SM}.  x3: 0 = tf32, 1 = tf32x3 with the register-stored
+// epilogue (the conv, and sigma_test_linear_tf32x3_regs), 2 = bf16 (the bf16 instance stages the
+// same bytes per k-block as tf32 — 128-byte rows — so its plan is the tf32 plan), 4 = e4m3 (the same stage bytes too, narrower
+// widths), 5 = tf32x3 with the TMA-stored epilogue (linear only); 3 is not a mode
 int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out) {
   GemmPlan pl;
-  if (x3 < 0 || x3 > 4 || x3 == 3 || (x3 >= 2 && conv_B > 0)) {
-    set_error("gemm plan: mode %d (0 tf32, 1 tf32x3, 2 bf16, 4 e4m3; bf16 and e4m3 have no conv)", x3);
+  if (x3 < 0 || x3 > 5 || x3 == 3 || (x3 >= 2 && conv_B > 0)) {
+    set_error("gemm plan: mode %d (0 tf32, 1 tf32x3, 2 bf16, 4 e4m3, 5 tf32x3 TMA-stored; only 0 and 1 have a conv)", x3);
     return SIGMA_EINVAL;
   }
-  const int rc = plan_gemm(M, N, K, x3 == 1, conv_B, conv_H, conv_W, &pl, x3 == 4);
+  const int rc = plan_gemm(M, N, K, x3 == 1 || x3 == 5, conv_B, conv_H, conv_W, &pl, x3 == 4, x3 == 5);
   if (rc) return rc;
   out[0] = pl.BN; out[1] = pl.stages; out[2] = pl.grid; out[3] = pl.tiles; out[4] = (long long)pl.smem; out[5] = pl.ctas_per_sm;
   return SIGMA_OK;
 }
 
 // The launch of the instance for pl.BN.
-template <bool X3, bool CONV, bool BF16 = false>
+template <bool X3, bool CONV, bool BF16 = false, bool TMA_C = false>
 static int launch_gemm(GemmParams &p, const GemmPlan &pl, cudaStream_t stream) {
   p.stages = pl.stages;
   const void *kern = nullptr;
   switch (p.BN) {
-#define SIGMA_GEMM_BN(bn) case bn: kern = (const void *)gemm_tf32_kernel<bn, X3, CONV, BF16>; break;
+#define SIGMA_GEMM_BN(bn) \
+  case bn: kern = TMA_C ? (const void *)gemm_x3_tma_kernel<bn> : (const void *)gemm_tf32_kernel<bn, X3, CONV, BF16>; break;
     SIGMA_GEMM_BN(32) SIGMA_GEMM_BN(64) SIGMA_GEMM_BN(96) SIGMA_GEMM_BN(128)
     SIGMA_GEMM_BN(160) SIGMA_GEMM_BN(192) SIGMA_GEMM_BN(224) SIGMA_GEMM_BN(256)
 #undef SIGMA_GEMM_BN
@@ -988,14 +1104,17 @@ static int launch_gemm(GemmParams &p, const GemmPlan &pl, cudaStream_t stream) {
   return SIGMA_OK;
 }
 
-// W_lo == nullptr: plain TF32 (one MMA per k-step); else tf32x3 with W = W_hi
+// W_lo == nullptr: plain TF32 (one MMA per k-step); else tf32x3 with W = W_hi, whose output tiles go out through TMA
+// (gemm_x3_tma_kernel) unless reg_epilogue
 int gemm_tf32_launch(const float *A, long long lda, const float *W, const float *W_lo, const float *bias, const float *residual,
-                     long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream) {
+                     long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream,
+                     bool reg_epilogue) {
   if (M == 0) return SIGMA_OK;
   const bool x3 = W_lo != nullptr;
+  const bool tma_c = x3 && !reg_epilogue;
   GemmPlan pl;
   int rc;
-  if ((rc = plan_gemm(M, N, K, x3, 0, 0, 0, &pl))) return rc;
+  if ((rc = plan_gemm(M, N, K, x3, 0, 0, 0, &pl, false, tma_c))) return rc;
   GemmParams p;
   memset(&p, 0, sizeof(p));
   p.bias = bias; p.residual = residual; p.rscale = rscale; p.C = C; p.ldr = ldr; p.ldc = ldc;
@@ -1004,6 +1123,15 @@ int gemm_tf32_launch(const float *A, long long lda, const float *W, const float 
   if ((rc = make_tmap_2d_sw128(&p.m_a, A, M, K, lda, GM_BM))) return rc;
   if ((rc = make_tmap_2d_sw128(&p.m_w, W, N, K, K, p.BN))) return rc;
   if (x3 && (rc = make_tmap_2d_sw128(&p.m_wlo, W_lo, N, K, K, p.BN))) return rc;
+  if (tma_c) {
+    const uint64_t dims[2] = {(uint64_t)N, (uint64_t)M}, str_c[1] = {(uint64_t)ldc * 4}, str_r[1] = {(uint64_t)ldr * 4};
+    const uint32_t box[2] = {GM_CHUNK, 64};
+    if ((rc = make_tmap(&p.m_c, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, C, dims, str_c, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                        CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
+    if (residual && (rc = make_tmap(&p.m_r, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, residual, dims, str_r, box,
+                                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
+    return launch_gemm<true, false, false, true>(p, pl, stream);
+  }
   return x3 ? launch_gemm<true, false>(p, pl, stream) : launch_gemm<false, false>(p, pl, stream);
 }
 

@@ -174,8 +174,12 @@ int dwconv3x3_silu_bf16_launch(const void *x, long long x_row_stride, long long 
                                void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream);
 
 // ---- gemm_tf32.cu ----
+// tf32x3 (W_lo != nullptr) stores its output tiles with TMA; reg_epilogue = true stores them from registers instead (the
+// TMA-stored epilogue's reference in the tests, sigma_test_linear_tf32x3_regs).  C and the residual: 16-byte-aligned base and
+// row stride (sigma_linear_tf32{,x3} check it).
 int gemm_tf32_launch(const float *A, long long lda, const float *W, const float *W_lo, const float *bias, const float *residual,
-                     long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream);
+                     long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream,
+                     bool reg_epilogue = false);
 int gemm_bf16_launch(const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
                      const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N, int K, cudaStream_t stream);
 int gemm_fp8_launch(const void *A, long long lda, const float *sa, const void *W, const float *sw, const float *bias,
