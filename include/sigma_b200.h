@@ -145,10 +145,16 @@ int sigma_ss2d_scan_fwd_bf16(int kind, const void *xc, const float *xdbl, const 
                              size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------
- * f1. Backward of the fused scan (training): replaces the autograd of CrossScan (vmamba.py:80-98) + the dt_proj einsum (:199) +
- * SelectiveScan (selective_scan_bwd_kernel.cuh:68-274) + CrossMerge (:100-121) without materialising the (B,4,D,L) copies.
- * kind = SIGMA_DIRS_CROSS4, SIGMA_DIRS_SEQ2 or SIGMA_DIRS_CROSS (batch = 2·images, as the forward; K = 1 walk per image, Kw = 2
- * weight sets); d_state in {4, 16}; D % 64 == 0.  Inputs as the forward plus
+ * f1. Training pair of the fused scan.  `sigma_ss2d_scan_fwd_save` is sigma_ss2d_scan_fwd that also writes what its backward
+ * needs: delta (K, batch, Lseq, D) = softplus(dt_proj) at the position it belongs to, and hs (sigma_ss2d_scan_hs_bytes) = the
+ * scan state at the start of every 16-position block of each direction's walk (the role of the reference's chunk states `x`,
+ * selective_scan_fwd_kernel.cuh:176-190).  `sigma_ss2d_scan_bwd_saved` consumes them (delta and hs are inputs) in one reverse
+ * sweep and replaces the autograd of CrossScan (vmamba.py:80-98) + the dt_proj einsum (:199) + SelectiveScan
+ * (selective_scan_bwd_kernel.cuh:68-274) + CrossMerge (:100-121) without materialising the (B,4,D,L) copies.
+ * kind = SIGMA_DIRS_CROSS4, SIGMA_DIRS_SEQ2 or SIGMA_DIRS_CROSS (batch = 2·images, as the forward; K = 1 walk of ceil(L/16)
+ * blocks per image, Kw = 2 weight sets); d_state in {4, 16}; D % 64 == 0 for the backward.  nsplit = 0 lets the library choose
+ * the L-segments; otherwise it forces their count (the forward caps it at 32, the backward at 64, both at the tile count of the
+ * longest walk), and the two calls may be cut differently.  The backward's inputs are the forward's, delta, hs and
  *   dy      (batch, Lseq, D)      gradient of the MERGED output y = sum_k y_k (CrossMerge is a sum, so every direction sees dy)
  * Outputs (fp32):
  *   dxc     (batch, Lseq, D)      sum over directions of du, accumulated by TMA reduce-add (zeroed inside)
@@ -157,20 +163,9 @@ int sigma_ss2d_scan_fwd_bf16(int kind, const void *xc, const float *xdbl, const 
  *   dxdbl   (batch, Lseq, K, Cp)  dB in columns [0, N), dC in [N, 2N) (zeroed inside; dt_r columns left 0 for the caller); CROSS:
  *                                 image b's dC goes to the C columns of image (b + batch/2) mod batch, whose row supplied C
  *   dA (Kw·D, N), dDs (Kw·D), ddtb (Kw, D)   overwritten; CROSS: rows w·D + d summed over the images of modality w
- *   delta   (K, batch, Lseq, D)   scratch: the recomputed softplus(dt_proj) slabs
  * ------------------------------------------------------------------------------------------ */
-size_t sigma_ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
-int sigma_ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
-                        const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
-                        int H, int W, int D, int N, int R, int Cp, void *workspace, size_t workspace_bytes, void *stream);
-
-/* Training forward + its backward: `sigma_ss2d_scan_fwd_save` is sigma_ss2d_scan_fwd that also writes what the backward would
- * otherwise recompute in a state sweep — delta (K, batch, Lseq, D) = softplus(dt_proj) at the position it belongs to, and
- * hs (sigma_ss2d_scan_hs_bytes) = the scan state at the start of every 16-position block of each direction's walk (the role of
- * the reference's chunk states `x`, selective_scan_fwd_kernel.cuh:176-190).  `sigma_ss2d_scan_bwd_saved` consumes them (delta
- * and hs are inputs) and runs only the reverse sweep.  nsplit = 0 lets the library choose the L-segments.  CROSS4 / SEQ2 / CROSS
- * (even batch; one walk of ceil(L/16) blocks per image), d_state 4 / 16. */
 size_t sigma_ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N);
+size_t sigma_ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
 int sigma_ss2d_scan_fwd_save(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                              const float *Ds, float *y, float *delta, float *hs, int batch, int H, int W, int D, int N, int R, int Cp,
                              void *workspace, size_t workspace_bytes, int nsplit, void *stream);
@@ -193,17 +188,13 @@ int sigma_ss2d_scan_bwd_saved_bf16(int kind, const void *xc, const float *xdbl, 
                                    float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                                    size_t workspace_bytes, int nsplit, void *stream);
 
-/* Deterministic builds of the fused backward (state sweep / after sigma_ss2d_scan_fwd_save): the same outputs, bitwise
+/* Deterministic build of the fused backward (after sigma_ss2d_scan_fwd_save): the same outputs, bitwise
  * reproducible for the same inputs, GPU model and L-segment plan.  Each direction's du goes to a slab summed over k into dxc,
  * dB / dC are kept per warp channel tile and dA / dDs / ddtb per (image, L-segment), all in the workspace, then summed in a
  * fixed order; no float atomics and no bulk reduce.  nsplit = 0 lets the library choose the L-segments.  CROSS4 / SEQ2 only: kind
  * CROSS has no deterministic build (SIGMA_EINVAL; the workspace query returns 0) — under the deterministic switch CroMB trains
  * through the op-level _det kernels. */
 size_t sigma_ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
-int sigma_ss2d_scan_bwd_det(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
-                            const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb,
-                            int batch, int H, int W, int D, int N, int R, int Cp, void *workspace, size_t workspace_bytes, int nsplit,
-                            void *stream);
 int sigma_ss2d_scan_bwd_saved_det(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                                   const float *Ds, const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl,
                                   float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
@@ -388,8 +379,8 @@ int sigma_test_linear_tf32x3_regs(const float *A, int64_t lda, const float *W_hi
                                   const float *residual, int64_t ldr, const float *rscale, float *C, int64_t ldc, int64_t M, int N,
                                   int K, void *stream);
 
-/* L-segment plan of the fused scan backward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_bwd (nsplit = 0)
- * or sigma_ss2d_scan_bwd_split / sigma_ss2d_scan_bwd_saved with that nsplit would launch for kind CROSS4 / SEQ2 / CROSS (even
+/* L-segment plan of the fused scan backward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_bwd_saved with
+ * that nsplit (0: the library's choice) would launch for kind CROSS4 / SEQ2 / CROSS (even
  * batch) at (batch, H, W, D, N).  out4_host = {segments, 16-position tiles per segment, tiles of the longest direction's walk, tiles of the shortest}.  The
  * directions share the tiles per segment, so a walk shorter than the longest can end in empty segments.  The plan does not depend
  * on the element type: sigma_ss2d_scan_bwd_saved_bf16 launches the same segments.  For tests and tuning. */
@@ -437,12 +428,6 @@ int sigma_scan_bwd_split(const void *u, const void *delta, const float *A, const
  * the longest walk).  nsplit > 1 without a large enough workspace is SIGMA_EWORKSPACE.                                         */
 int sigma_ss2d_scan_fwd_split(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                               const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
-                              size_t workspace_bytes, int nsplit, void *stream);
-/* sigma_ss2d_scan_bwd with a forced number of L-segments (nsplit = 0: the library's choice; capped at 64 and at the tile count of
- * the longest walk).                                                                                                           */
-int sigma_ss2d_scan_bwd_split(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
-                              const float *Ds, const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA,
-                              float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                               size_t workspace_bytes, int nsplit, void *stream);
 /* Host only (no CUDA call, works without a GPU): the L-segment count the fused scan forward picks for a grid of `ctas` CTAs of
  * warps_per_cta warps walking ntiles tiles at d_state N, and the GEMM tile width for N output columns and m_tiles 128-row tiles. */

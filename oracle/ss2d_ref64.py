@@ -1,4 +1,4 @@
-"""fp64 reference of the fused SS2D scan core (sigma_ss2d_scan_fwd{,_split,_bf16,_save{,_bf16}}, sigma_ss2d_scan_bwd{,_saved{,_bf16}})
+"""fp64 reference of the fused SS2D scan core (sigma_ss2d_scan_fwd{,_split,_bf16,_save{,_bf16}}, sigma_ss2d_scan_bwd_saved{,_bf16,_det})
 with a per-element error bound for each output of the fp32 kernels.  ORACLE — test infrastructure only.  Plain torch float64,
 device-agnostic.  ss2d_fwd_ref64 is the forward alone (y and its bound, every kind, fp32 or bf16 xc); ss2d_ref64 runs it and
 adds the backward (every kind).

@@ -220,7 +220,7 @@ using namespace sigma;
 extern "C" {
 #pragma GCC visibility push(default)
 
-int sigma_abi_version(void) { return 1; }   // additions only since 1: every existing call is unchanged
+int sigma_abi_version(void) { return 2; }   // 2 removed sigma_ss2d_scan_bwd{,_split,_det}; additions only since 2
 const char *sigma_last_error(void) { return g_err; }
 uint64_t sigma_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
@@ -581,7 +581,7 @@ int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H
   return SIGMA_OK;
 }
 
-// the L-segment plan of sigma_ss2d_scan_bwd{,_split,_saved} (nsplit = 0: the library's choice):
+// the L-segment plan of sigma_ss2d_scan_bwd_saved{,_bf16,_det} (nsplit = 0: the library's choice):
 // out4_host = {segments, tiles per segment, tiles of the longest walk, tiles of the shortest walk}
 int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, int nsplit, int64_t *out4_host) {
   SIGMA_CHECK_ARG(out4_host && (kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2 || kind == SIGMA_DIRS_CROSS) && batch > 0 && H > 0 &&
@@ -663,33 +663,34 @@ size_t sigma_ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W
 }
 
 static int ss2d_bwd_entry(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
-                          const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb,
-                          int batch, int H, int W, int D, int N, int R, int Cp, void *ws, size_t wsb, int nsplit, void *stream,
-                          const float *hs_saved = nullptr, int det = 0, int bf16 = 0) {
-  SIGMA_CHECK_ARG(xc && xdbl && dtw && dtb && A && Ds && dy && delta && dxc && ddelta && dxdbl && dA && dDs && ddtb, "sigma_ss2d_scan_bwd: null pointer");
+                          const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl, float *dA,
+                          float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *ws, size_t wsb, int nsplit,
+                          void *stream, int det = 0, int bf16 = 0) {
+  SIGMA_CHECK_ARG(xc && xdbl && dtw && dtb && A && Ds && dy && delta && dxc && ddelta && dxdbl && dA && dDs && ddtb,
+                  "sigma_ss2d_scan_bwd_saved: null pointer");
   SIGMA_CHECK_ARG(kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2 || kind == SIGMA_DIRS_CROSS,
-                  "sigma_ss2d_scan_bwd: kind %d unsupported (CROSS4, SEQ2, CROSS)", kind);
+                  "sigma_ss2d_scan_bwd_saved: kind %d unsupported (CROSS4, SEQ2, CROSS)", kind);
   SIGMA_CHECK_ARG(kind != SIGMA_DIRS_CROSS || !det,
-                  "sigma_ss2d_scan_bwd_det: kind CROSS has no deterministic build (under the deterministic switch CroMB trains through "
-                  "the op-level _det kernels)");
-  SIGMA_CHECK_ARG(kind != SIGMA_DIRS_CROSS || batch % 2 == 0, "sigma_ss2d_scan_bwd: CROSS needs batch = 2·images (batch=%d)", batch);
-  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % 64 == 0 && R > 0, "sigma_ss2d_scan_bwd: bad sizes (D=%d must be a multiple of 64)", D);
-  SIGMA_CHECK_ARG(N == 4 || N == 16, "sigma_ss2d_scan_bwd: d_state=%d unsupported (4, 16)", N);
-  SIGMA_CHECK_ARG(Cp == sigma_ss2d_padded_cp(N, R), "sigma_ss2d_scan_bwd: Cp=%d must equal sigma_ss2d_padded_cp(N=%d, R=%d)", Cp, N, R);
-  SIGMA_CHECK_ARG(al16(xc) && al16(xdbl) && al16(dy) && al16(delta) && al16(dxc) && al16(ddelta) && al16(dxdbl), "sigma_ss2d_scan_bwd: pointers must be 16-byte aligned");
-  SIGMA_CHECK_ARG(hs_saved == nullptr || al16(hs_saved), "sigma_ss2d_scan_bwd_saved: hs must be 16-byte aligned");
-  return ss2d_scan_bwd(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, ws, wsb, nsplit,
-                       (cudaStream_t)stream, hs_saved, det, bf16);
+                  "sigma_ss2d_scan_bwd_saved_det: kind CROSS has no deterministic build (under the deterministic switch CroMB trains "
+                  "through the op-level _det kernels)");
+  SIGMA_CHECK_ARG(kind != SIGMA_DIRS_CROSS || batch % 2 == 0, "sigma_ss2d_scan_bwd_saved: CROSS needs batch = 2·images (batch=%d)", batch);
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % 64 == 0 && R > 0, "sigma_ss2d_scan_bwd_saved: bad sizes (D=%d must be a multiple of 64)", D);
+  SIGMA_CHECK_ARG(N == 4 || N == 16, "sigma_ss2d_scan_bwd_saved: d_state=%d unsupported (4, 16)", N);
+  SIGMA_CHECK_ARG(Cp == sigma_ss2d_padded_cp(N, R), "sigma_ss2d_scan_bwd_saved: Cp=%d must equal sigma_ss2d_padded_cp(N=%d, R=%d)", Cp, N, R);
+  SIGMA_CHECK_ARG(al16(xc) && al16(xdbl) && al16(dy) && al16(delta) && al16(dxc) && al16(ddelta) && al16(dxdbl), "sigma_ss2d_scan_bwd_saved: pointers must be 16-byte aligned");
+  SIGMA_CHECK_ARG(al16(hs), "sigma_ss2d_scan_bwd_saved: hs must be 16-byte aligned");
+  return ss2d_scan_bwd(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, hs, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, ws, wsb,
+                       nsplit, (cudaStream_t)stream, det, bf16);
 }
 
-// backward after sigma_ss2d_scan_fwd_save: `delta` and `hs` are INPUTS (what that call wrote); no state sweep runs
+// backward after sigma_ss2d_scan_fwd_save: `delta` and `hs` are INPUTS (what that call wrote)
 int sigma_ss2d_scan_bwd_saved(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                               const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl, float *dA,
                               float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                               size_t workspace_bytes, int nsplit, void *stream) {
   SIGMA_CHECK_ARG(hs != nullptr, "sigma_ss2d_scan_bwd_saved: null hs");
-  return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, const_cast<float *>(delta), dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R,
-                        Cp, workspace, workspace_bytes, nsplit, stream, hs);
+  return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, hs, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp,
+                        workspace, workspace_bytes, nsplit, stream);
 }
 
 // backward after sigma_ss2d_scan_fwd_save_bf16: xc, dy and delta are bf16; dxc and every other output fp32
@@ -703,44 +704,19 @@ int sigma_ss2d_scan_bwd_saved_bf16(int kind, const void *xc, const float *xdbl, 
     set_error("sigma_ss2d_scan_bwd_saved_bf16: d_state=8 unsupported (4, 16)");
     return SIGMA_EUNSUPPORTED;
   }
-  return ss2d_bwd_entry(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (const float *)dy, (float *)const_cast<void *>(delta), dxc, ddelta, dxdbl,
-                        dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace, workspace_bytes, nsplit, stream, hs, 0, 1);
+  return ss2d_bwd_entry(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (const float *)dy, (const float *)delta, hs, dxc, ddelta, dxdbl,
+                        dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace, workspace_bytes, nsplit, stream, 0, 1);
 }
 
-int sigma_ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
-                        const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
-                        int H, int W, int D, int N, int R, int Cp, void *workspace, size_t workspace_bytes, void *stream) {
-  return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace,
-                        workspace_bytes, 0, stream);
-}
-
-// test hook: force the number of L-segments
-int sigma_ss2d_scan_bwd_split(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
-                              const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb,
-                              int batch, int H, int W, int D, int N, int R, int Cp, void *workspace, size_t workspace_bytes, int nsplit,
-                              void *stream) {
-  return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace,
-                        workspace_bytes, nsplit, stream);
-}
-
-// deterministic builds of sigma_ss2d_scan_bwd_split / sigma_ss2d_scan_bwd_saved (nsplit = 0: the library's choice)
-int sigma_ss2d_scan_bwd_det(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
-                            const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb,
-                            int batch, int H, int W, int D, int N, int R, int Cp, void *workspace, size_t workspace_bytes, int nsplit,
-                            void *stream) {
-  SIGMA_CHECK_ARG(nsplit >= 0, "sigma_ss2d_scan_bwd_det: nsplit=%d < 0", nsplit);
-  return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace,
-                        workspace_bytes, nsplit, stream, nullptr, 1);
-}
-
+// the deterministic build of sigma_ss2d_scan_bwd_saved (nsplit = 0: the library's choice)
 int sigma_ss2d_scan_bwd_saved_det(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                                   const float *Ds, const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl,
                                   float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                                   size_t workspace_bytes, int nsplit, void *stream) {
   SIGMA_CHECK_ARG(hs != nullptr, "sigma_ss2d_scan_bwd_saved_det: null hs");
   SIGMA_CHECK_ARG(nsplit >= 0, "sigma_ss2d_scan_bwd_saved_det: nsplit=%d < 0", nsplit);
-  return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, const_cast<float *>(delta), dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R,
-                        Cp, workspace, workspace_bytes, nsplit, stream, hs, 1);
+  return ss2d_bwd_entry(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, hs, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp,
+                        workspace, workspace_bytes, nsplit, stream, 1);
 }
 
 int sigma_upsample2x_norm_fwd(const float *x, const float *w, const float *b, float *y, int batch, int H, int W, int C,

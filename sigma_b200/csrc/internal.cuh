@@ -85,12 +85,12 @@ size_t ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N);
 size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
 size_t ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
 int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int force_split, long long *out4);
-// hs_saved: the training forward's block-start states (no state sweep); det: the deterministic build; bf16 (needs hs_saved,
-// excludes det): xc, dy and delta are bf16 behind the float pointers
+// delta / hs: the delta' slabs and block-start states the training forward wrote; det: the deterministic build; bf16 (excludes
+// det): xc, dy and delta are bf16 behind the float pointers
 int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
-                  const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
-                  int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream,
-                  const float *hs_saved = nullptr, int det = 0, int bf16 = 0);
+                  const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs,
+                  float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split,
+                  cudaStream_t stream, int det = 0, int bf16 = 0);
 
 // ---- scan_op.cu: generic op-level scan forward ----
 __global__ void scan_combine_kernel(float *carry, long long nrows, int nsplit, int NP);

@@ -48,7 +48,7 @@ struct alignas(64) Ss2dParams {
   CUtensorMap m_xc[4], m_dbl[4];
   const float *dtw, *dtb, *A, *Ds;
   float *y, *carry;
-  // training forward (SAVE kernels): what the fused backward (ss2d_scan_bwd.cu) would otherwise recompute in its state sweep —
+  // training forward (SAVE kernels): what the fused backward (ss2d_scan_bwd.cu) reads instead of recomputing it —
   // delta' = softplus(dt_proj) slabs (K, batch, Lseq, D), stored like y, and the state at the start of every 16-position block
   // of the walk, hsave (K, batch, save_tiles, D, N) indexed by the backward's walk-order tile number
   float *dsave, *hsave;

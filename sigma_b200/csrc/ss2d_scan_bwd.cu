@@ -1,13 +1,13 @@
-// f1 — backward of the FUSED multi-direction SS2D scan, channels-last (see include/sigma_b200.h: sigma_ss2d_scan_bwd).
+// f1 — backward of the FUSED multi-direction SS2D scan, channels-last (see include/sigma_b200.h: sigma_ss2d_scan_bwd_saved).
 //
 // Replaces, for training, the autograd of CrossScan + dt_proj einsum + SelectiveScan + CrossMerge
 // (vmamba.py:80-121, 195-215 and selective_scan_bwd_kernel.cuh:68-274) without ever materialising CrossScan's (B,4,D,L)
-// copy: every direction is the same 4-D TMA walk over the channels-last tensors that the forward uses.  Three sweeps:
-//   1. state sweep  (ss2d_state_kernel, walk order): delta' = softplus(dt_r·W_dt + bias) -> `delta` slabs (K,B,L,D), and the
-//      state h at the start of every 16-position tile -> `hs`; L-segments by MODE_SUMMARY -> scan_combine_kernel -> MODE_APPLY;
-//   2. reverse summaries (ss2d_bwd_kernel<MODE_SUMMARY>, only with L-segments) + scan_combine_rev_kernel: the dh entering
+// copy: every direction is the same 4-D TMA walk over the channels-last tensors that the forward uses.  The training forward
+// (sigma_ss2d_scan_fwd_save) has already written delta' = softplus(dt_r·W_dt + bias) -> `delta` slabs (K,B,L,D), and the state
+// h at the start of every 16-position tile -> `hs`; both are inputs here.  Two sweeps:
+//   1. reverse summaries (ss2d_bwd_kernel<MODE_SUMMARY>, only with L-segments) + scan_combine_rev_kernel: the dh entering
 //      every segment (L-parallel reverse sweep);
-//   3. main sweep (ss2d_bwd_kernel, tiles walked BACKWARDS): per tile recompute h at every position from the tile's start
+//   2. main sweep (ss2d_bwd_kernel, tiles walked BACKWARDS): per tile recompute h at every position from the tile's start
 //      state into shared memory, then the reverse recurrence dh_l = a_{l+1}·dh_{l+1} + dy_l·C_l producing
 //        du      -> TMA REDUCE-ADD (cp.reduce.async.bulk.tensor .add.f32) straight into dxc (B,L,D): the four directions'
 //                   contributions meet in L2, no (B,4,D,L) gradient tensor and no CrossScan backward;
@@ -37,8 +37,8 @@ constexpr int FB_DT = 64;   // channels per CTA
 struct alignas(64) Ss2dBwdParams {
   CUtensorMap m_xc[4], m_dy[4], m_dl[4], m_dbl[4];    // loads: boxes {64 ch, 16 pos} / {Cp, 16 pos}
   CUtensorMap m_dxc[4], m_dd[4];                      // per-warp outputs: boxes {CPW ch, 16 pos}
-  const float *dtw, *dtb, *A, *Ds, *hs_in;
-  float *hs, *dxdbl, *dA, *dDs, *ddtb, *carry;
+  const float *dtw, *dtb, *A, *Ds, *hs;
+  float *dxdbl, *dA, *dDs, *ddtb, *carry;
   int D, N, R, Cp, K, batch;
   long long Lseq;
   int I[4], O[4], rev[4];
@@ -56,7 +56,7 @@ template <int N> struct FbCfg {
   static constexpr int CPW = 32 / LPC;
 };
 
-// everything the three kernels share: CTA coordinates, the direction's tile geometry, the ring
+// everything both sweeps share: CTA coordinates, the direction's tile geometry, the ring
 struct FbWalk {
   int k, split, b, d0, t0, t1, I, TPO, ntiles;
   bool rev;
@@ -84,141 +84,7 @@ __device__ __forceinline__ FbWalk fb_walk(const Ss2dBwdParams &p) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// 1. state sweep: delta' slabs + tile-start states (walk order)
-// ---------------------------------------------------------------------------------------------------------------------
-// CROSS: image b runs with weight set kw = [b >= batch/2] (its rows of W_dt, bias and A); the state sweep needs only its own
-// x_dbl row (B, dt_r), so the walk itself is kind SEQ2's first direction
-template <int N, int MODE, bool CROSS>
-__device__ __forceinline__ void ss2d_state_body(const Ss2dBwdParams &p) {
-  constexpr int LPC = FbCfg<N>::LPC, NS = FbCfg<N>::NS, CPW = FbCfg<N>::CPW, NT = FB_DT * LPC;
-  // delta' does not depend on the state: the pass that sees a position FIRST (MODE_SERIAL, or MODE_SUMMARY when the walk is
-  // cut into L-segments) computes it and stores the slab tile; MODE_APPLY reads it back instead of repeating the dot product
-  constexpr bool COMPUTE = MODE != MODE_APPLY, STATES = MODE != MODE_SUMMARY;
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  float *smem = reinterpret_cast<float *>(smem_raw);
-  const int NST = p.nst, Cp = p.Cp, R = p.R;
-  const int xc_fl = FB_LT * FB_DT, dbl_fl = FB_LT * Cp, stage_fl = xc_fl + dbl_fl + (COMPUTE ? 0 : xc_fl);   // xc | dbl | [delta']
-  float *stage_all = smem + NST * stage_fl;                // per-warp delta staging [16][CPW] (TMA store source: keep it aligned)
-  float *sW = stage_all + (NT / 32) * FB_LT * CPW;         // W_dt rows of this CTA's channels, pitch R + 1
-  uint64_t *full = reinterpret_cast<uint64_t *>(sW + ((FB_DT * (R + 1) + 1) & ~1));
-  uint32_t *done = reinterpret_cast<uint32_t *>(full + NST);
-
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = NT >> 5;
-  const int half = lane / CPW, cl = lane - half * CPW, c = warp * CPW + cl, n0 = half * NS;
-  const FbWalk w = fb_walk(p);
-  const int d = w.d0 + c;
-  const int kw = CROSS ? (w.b >= (p.batch >> 1) ? 1 : 0) : w.k;   // weight set
-  if (tid == 0) {
-    for (int s = 0; s < NST; ++s) { mbar_init(&full[s], 1); done[s] = 0; }
-    fence_mbar_init();
-  }
-  if (COMPUTE) {
-    for (int i = tid; i < FB_DT * R; i += NT) {
-      const int cc = i / R, r = i - cc * R;
-      sW[cc * (R + 1) + r] = p.dtw[((long long)kw * p.D + w.d0 + cc) * R + r];
-    }
-  }
-  __syncthreads();
-  if (w.t0 >= w.t1) return;
-  const uint32_t tx = (uint32_t)(stage_fl * sizeof(float));
-  auto request_tile = [&](int tau, int st) {
-    int o, i0, npos;
-    w.tile(tau, o, i0, npos);
-    float *dst = smem + st * stage_fl;
-    mbar_arrive_expect_tx(&full[st], tx);
-    tma_load_4d(dst, &p.m_xc[w.k], &full[st], w.d0, i0, o, w.b);
-    tma_load_4d(dst + xc_fl, &p.m_dbl[w.k], &full[st], 0, i0, o, w.b);
-    if (!COMPUTE) tma_load_4d(dst + xc_fl + dbl_fl, &p.m_dl[w.k], &full[st], w.d0, i0, o, w.k * p.batch + w.b);
-  };
-  if (tid == 0) for (int tau = w.t0; tau < min(w.t1, w.t0 + NST); ++tau) request_tile(tau, tau - w.t0);
-
-  float h[NS], a2[NS];
-  const long long wd = (long long)kw * p.D + d;
-#pragma unroll
-  for (int s = 0; s < NS; ++s) { a2[s] = p.A[wd * N + n0 + s] * kLog2e; h[s] = 0.f; }
-  const float bias = p.dtb[wd];
-  float sumdl = 0.f;
-  float *carry_row = p.carry + ((((long long)w.b * p.K + w.k) * p.D + d) * p.nsplit + w.split) * 2 * N;
-  if (MODE == MODE_APPLY) {
-#pragma unroll
-    for (int s = 0; s < NS; ++s) h[s] = carry_row[N + n0 + s];
-  }
-  const float *wrow = sW + c * (R + 1);
-  float *stg = stage_all + warp * FB_LT * CPW;
-
-  int st = 0, ph = 0;
-  for (int tau = w.t0; tau < w.t1; ++tau) {
-    int o, i0, npos;
-    w.tile(tau, o, i0, npos);
-    mbar_spin(&full[st], (uint32_t)ph);
-    const float *sXC = smem + st * stage_fl, *sDB = sXC + xc_fl, *sDL = sDB + dbl_fl;
-    if (STATES) {   // state at the start of the tile (walk order)
-      float4 *hp = reinterpret_cast<float4 *>(p.hs + (((((long long)w.k * p.batch + w.b) * p.max_tiles + tau) * p.D + d) * N + n0));
-#pragma unroll
-      for (int q = 0; q < NS / 4; ++q) hp[q] = make_float4(h[4 * q], h[4 * q + 1], h[4 * q + 2], h[4 * q + 3]);
-    }
-#pragma unroll 1
-    for (int s = 0; s < npos; ++s) {
-      const int r = w.rev ? npos - 1 - s : s;
-      const float *row = sDB + r * Cp;
-      float dl;
-      if (COMPUTE) {
-        dl = 0.f;
-        if (half == 0) {           // one lane per channel evaluates dt_proj + softplus; its partner lane (d_state 16) receives it
-          float acc = bias;
-          for (int q = 0; q < R; ++q) acc = fmaf(wrow[q], row[2 * N + q], acc);
-          dl = softplus20(acc);
-          stg[r * CPW + cl] = dl;
-        }
-        if (LPC == 2) dl = __shfl_sync(0xffffffffu, dl, cl);
-      } else {
-        dl = sDL[r * FB_DT + c];
-      }
-      const float du = dl * sXC[r * FB_DT + c];
-#pragma unroll
-      for (int q = 0; q < NS / 4; ++q) {
-        const float4 bv = *reinterpret_cast<const float4 *>(row + n0 + 4 * q);
-        h[4 * q] = fmaf(ex2(dl * a2[4 * q]), h[4 * q], du * bv.x);
-        h[4 * q + 1] = fmaf(ex2(dl * a2[4 * q + 1]), h[4 * q + 1], du * bv.y);
-        h[4 * q + 2] = fmaf(ex2(dl * a2[4 * q + 2]), h[4 * q + 2], du * bv.z);
-        h[4 * q + 3] = fmaf(ex2(dl * a2[4 * q + 3]), h[4 * q + 3], du * bv.w);
-      }
-      sumdl += dl;
-    }
-    if (COMPUTE) {
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        tma_store_4d(&p.m_dd[w.k], stg, w.d0 + warp * CPW, i0, o, w.k * p.batch + w.b);   // m_dd doubles as the delta-slab map here
-        tma_store_commit();
-        tma_store_wait_read<0>();
-      }
-    }
-    __syncwarp();
-    if (lane == 0 && tau + NST < w.t1) {
-      const uint32_t old = smem_inc_acq_rel(&done[st]);
-      if ((old + 1) % (uint32_t)nwarps == 0) request_tile(tau + NST, st);
-    }
-    if (++st == NST) { st = 0; ph ^= 1; }
-  }
-  if (COMPUTE && lane == 0) tma_store_wait_all<0>();
-  if (MODE == MODE_SUMMARY) {
-#pragma unroll
-    for (int s = 0; s < NS; ++s) {
-      carry_row[n0 + s] = ex2(a2[s] * sumdl);
-      carry_row[N + n0 + s] = h[s];
-    }
-  }
-}
-
-template <int N, int MODE>
-__global__ void __launch_bounds__(128, 3) ss2d_state_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_state_body<N, MODE, false>(p); }
-
-template <int N, int MODE>
-__global__ void __launch_bounds__(128, 3) ss2d_state_cross_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_state_body<N, MODE, true>(p); }
-
-// ---------------------------------------------------------------------------------------------------------------------
-// 2 + 3. reverse summaries (MODE_SUMMARY) and the main backward sweep (MODE_SERIAL / MODE_APPLY)
+// 1 + 2. reverse summaries (MODE_SUMMARY) and the main backward sweep (MODE_SERIAL / MODE_APPLY)
 // ---------------------------------------------------------------------------------------------------------------------
 // DET: every sum across CTAs goes to the partials of the deterministic build (see Ss2dBwdParams) instead of an atomic.
 // CROSS: image b runs with weight set kw = [b >= batch/2] and reads C from image bC = the other modality's (as the forward):
@@ -317,7 +183,7 @@ __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
     if (MAIN) {
       // ---- forward inside the tile from its start state (walk order), h after every step -> shared memory ----
       float h[NS];
-      const float4 *hp = reinterpret_cast<const float4 *>(p.hs_in + (((((long long)w.k * p.batch + w.b) * p.max_tiles + tau) * p.D + d) * N + n0));
+      const float4 *hp = reinterpret_cast<const float4 *>(p.hs +(((((long long)w.k * p.batch + w.b) * p.max_tiles + tau) * p.D + d) * N + n0));
 #pragma unroll
       for (int q = 0; q < NS / 4; ++q) { const float4 v = hp[q]; h[4 * q] = v.x; h[4 * q + 1] = v.y; h[4 * q + 2] = v.z; h[4 * q + 3] = v.w; }
 #pragma unroll 1
@@ -490,11 +356,9 @@ size_t ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N) {
   return (size_t)K * batch * fb_max_tiles(kind, H, W) * D * N * sizeof(float);
 }
 
-// workspace = [hs (K, batch, max_tiles, D, N)] [forward carries] [reverse carries]
+// workspace = [reverse carries (batch, K, D, 64 segments, 2N)]
 size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
-  const int K = fb_dirs(kind);
-  const size_t carry = (size_t)batch * K * D * kFbMaxSplit * 2 * N * sizeof(float);
-  return align256((size_t)K * batch * fb_max_tiles(kind, H, W) * D * N * sizeof(float)) + 2 * align256(carry);
+  return align256((size_t)batch * fb_dirs(kind) * D * kFbMaxSplit * 2 * N * sizeof(float));
 }
 
 // the deterministic build appends [du slabs (K, batch, Lseq, D)] [dB / dC partials (D / CPW, batch, Lseq, K, 2N)]
@@ -518,7 +382,7 @@ size_t ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int 
   return fb_det_layout(kind, batch, H, W, D, N).total;
 }
 
-// The L-segment plan of the three sweeps.  All directions share tiles_per_split, so a direction with fewer tiles than the
+// The L-segment plan of both sweeps.  All directions share tiles_per_split, so a direction with fewer tiles than the
 // longest walk (min_tiles < max_tiles) can get empty trailing segments.  force_split > 0 overrides the count (capped at 64).
 struct FbPlan { int nsplit, tiles_per_split, max_tiles, min_tiles; };
 
@@ -548,30 +412,26 @@ int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int forc
 // (batch, Lseq, K, Cp) are ACCUMULATED INTO after being zeroed here; dA (K·D, N), dDs (K·D), ddtb (K, D) overwritten.
 // det: the main sweep writes partials (see fb_det_layout) that sum_parts_det_kernel adds in a fixed order.
 int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
-                  const float *dy, float *delta, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch,
-                  int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split, cudaStream_t stream,
-                  const float *hs_saved, int det, int bf16) {
+                  const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs,
+                  float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split,
+                  cudaStream_t stream, int det, int bf16) {
   const size_t need = det ? ss2d_scan_bwd_det_workspace_bytes(kind, batch, H, W, D, N) : ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N);
   if (ws == nullptr || ws_bytes < need) {
-    set_error("sigma_ss2d_scan_bwd: workspace too small (%zu < %zu)", ws_bytes, need);
+    set_error("sigma_ss2d_scan_bwd_saved: workspace too small (%zu < %zu)", ws_bytes, need);
     return SIGMA_EWORKSPACE;
   }
   const bool cross = kind == SIGMA_DIRS_CROSS;   // never with det (the entry points reject it)
-  // bf16 (never with det, always with hs_saved; the entry point checks): xc, dy and delta are bf16 behind the float pointers
+  // bf16 (never with det; the entry point checks): xc, dy and delta are bf16 behind the float pointers
   const uint64_t xes = bf16 ? 2 : 4;             // bytes per xc / dy / delta element
   Ss2dBwdParams p;
   memset(&p, 0, sizeof(p));
   const int K = fb_dirs(kind), Kw = fb_wsets(kind);
   const long long Lseq = kind == SIGMA_DIRS_SEQ2 ? 2LL * H * W : (long long)H * W;
-  p.dtw = dtw; p.dtb = dtb; p.A = A; p.Ds = Ds;
+  p.dtw = dtw; p.dtb = dtb; p.A = A; p.Ds = Ds; p.hs = hs;
   p.dxdbl = dxdbl; p.dA = dA; p.dDs = dDs; p.ddtb = ddtb;
   p.D = D; p.N = N; p.R = R; p.Cp = Cp; p.K = K; p.batch = batch; p.Lseq = Lseq;
   p.max_tiles = fb_max_tiles(kind, H, W);
-  const size_t hs_b = align256((size_t)K * batch * p.max_tiles * D * N * sizeof(float));
-  const size_t carry_b = align256((size_t)batch * K * D * kFbMaxSplit * 2 * N * sizeof(float));
-  p.hs = (float *)ws;
-  p.hs_in = hs_saved ? hs_saved : p.hs;   // hs_saved: the training forward already wrote delta' and the block-start states
-  float *fcarry = (float *)((char *)ws + hs_b), *rcarry = (float *)((char *)ws + hs_b + carry_b);
+  p.carry = (float *)ws;
   const int CPW = N >= 16 ? 16 : 32;
   int rc;
   auto tmap = [](CUtensorMap *map, const void *base, const uint64_t *dims, const uint64_t *str, const uint32_t *box,
@@ -618,7 +478,7 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
   SIGMA_CHECK_CUDA(cudaMemsetAsync(dDs, 0, (size_t)Kw * D * sizeof(float), stream));
   SIGMA_CHECK_CUDA(cudaMemsetAsync(ddtb, 0, (size_t)Kw * D * sizeof(float), stream));
 
-  // the state sweep stores delta' through m_dd (per-warp boxes over the delta slabs); the main sweep re-points it at ddelta
+  // per-warp boxes over (K, batch, Lseq, D) slabs: m_dd over ddelta, and for det m_dxc over the du slabs
   auto make_dd = [&](float *slab, CUtensorMap *maps = nullptr) -> int {
     for (int k = 0; k < K; ++k) {
       const bool colmajor = kind == SIGMA_DIRS_CROSS4 && (k & 1);
@@ -636,8 +496,6 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
     }
     return SIGMA_OK;
   };
-  if (!bf16 && (rc = make_dd(delta))) return rc;   // (the bf16 mode runs no state sweep: its delta slabs are an input)
-  Ss2dBwdParams ps = p;
   if ((rc = make_dd(ddelta))) return rc;
   const FbDetLayout dl = fb_det_layout(kind, batch, H, W, D, N);
   float *du_slabs = (float *)((char *)ws + dl.du);
@@ -648,28 +506,22 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
     p.part_dD = (float *)((char *)ws + dl.dD);
     p.part_db = p.part_dD + (size_t)batch * kFbMaxSplit * K * D;
   }
-  Ss2dBwdParams pm = p;
-  // ps holds m_dd -> delta (state sweep), pm holds m_dd -> ddelta (main sweep)
   auto go = [&](auto tag) -> int {
     constexpr int NN = decltype(tag)::value;
     constexpr int LPC = FbCfg<NN>::LPC, NS = FbCfg<NN>::NS, CPWc = FbCfg<NN>::CPW, NT = FB_DT * LPC;
-    dim3 grid(D / FB_DT, K * pm.nsplit, batch), block(NT);
+    dim3 grid(D / FB_DT, K * p.nsplit, batch), block(NT);
     const long long nrows = (long long)batch * K * D, tot = nrows * NN;
-    const size_t st_smem = ((size_t)pm.nst * (2 * FB_LT * FB_DT + FB_LT * Cp) + FB_DT * (R + 1) + 2 + (NT / 32) * FB_LT * CPWc) * sizeof(float) + 256;
     const size_t dbl_tiles = cross ? 2 : 1;   // the reverse sweeps of CROSS also stage the C image's x_dbl tile
     const size_t xt_fl = FB_LT * FB_DT * xes / 4;   // an xc / dy / delta tile, in floats
-    const size_t sm_smem = ((size_t)pm.nst * (2 * xt_fl + dbl_tiles * FB_LT * Cp)) * sizeof(float) + 256;
-    const size_t mn_smem = ((size_t)pm.nst * (3 * xt_fl + dbl_tiles * FB_LT * Cp) + (NT / 32) * 2 * FB_LT * CPWc + (size_t)FB_LT * NS * NT) * sizeof(float) + 256;
-    auto run = [&](auto kern, const Ss2dBwdParams &pp, size_t smem) -> int {
+    const size_t sm_smem = ((size_t)p.nst * (2 * xt_fl + dbl_tiles * FB_LT * Cp)) * sizeof(float) + 256;
+    const size_t mn_smem = ((size_t)p.nst * (3 * xt_fl + dbl_tiles * FB_LT * Cp) + (NT / 32) * 2 * FB_LT * CPWc + (size_t)FB_LT * NS * NT) * sizeof(float) + 256;
+    auto run = [&](auto kern, size_t smem) -> int {
       SIGMA_CHECK_CUDA(prep_kernel_once((const void *)kern));
-      kern<<<grid, block, smem, stream>>>(pp);
+      kern<<<grid, block, smem, stream>>>(p);
       SIGMA_CHECK_LAUNCH();
       return SIGMA_OK;
     };
     using Kern = void (*)(Ss2dBwdParams);
-    const Kern st_serial = cross ? ss2d_state_cross_kernel<NN, MODE_SERIAL> : ss2d_state_kernel<NN, MODE_SERIAL>;
-    const Kern st_summary = cross ? ss2d_state_cross_kernel<NN, MODE_SUMMARY> : ss2d_state_kernel<NN, MODE_SUMMARY>;
-    const Kern st_apply = cross ? ss2d_state_cross_kernel<NN, MODE_APPLY> : ss2d_state_kernel<NN, MODE_APPLY>;
     const Kern bw_serial = bf16 ? (cross ? ss2d_bwd_cross_bf16_kernel<NN, MODE_SERIAL> : ss2d_bwd_bf16_kernel<NN, MODE_SERIAL>)
                                 : (cross ? ss2d_bwd_cross_kernel<NN, MODE_SERIAL> : ss2d_bwd_kernel<NN, MODE_SERIAL>);
     const Kern bw_summary = bf16 ? (cross ? ss2d_bwd_cross_bf16_kernel<NN, MODE_SUMMARY> : ss2d_bwd_bf16_kernel<NN, MODE_SUMMARY>)
@@ -677,41 +529,29 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
     const Kern bw_apply = bf16 ? (cross ? ss2d_bwd_cross_bf16_kernel<NN, MODE_APPLY> : ss2d_bwd_bf16_kernel<NN, MODE_APPLY>)
                                : (cross ? ss2d_bwd_cross_kernel<NN, MODE_APPLY> : ss2d_bwd_kernel<NN, MODE_APPLY>);
     int r;
-    ps.carry = fcarry;
-    if (hs_saved != nullptr) {
-      // nothing to recompute
-    } else if (pm.nsplit == 1) {
-      if ((r = run(st_serial, ps, st_smem))) return r;
-    } else {
-      if ((r = run(st_summary, ps, st_smem))) return r;
-      scan_combine_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(fcarry, nrows, pm.nsplit, NN);
-      SIGMA_CHECK_LAUNCH();
-      if ((r = run(st_apply, ps, st_smem))) return r;
-    }
-    pm.carry = rcarry;
     if (!det) {
-      if (pm.nsplit == 1) return run(bw_serial, pm, mn_smem);
-      if ((r = run(bw_summary, pm, sm_smem))) return r;
-      scan_combine_rev_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(rcarry, nrows, pm.nsplit, NN);
+      if (p.nsplit == 1) return run(bw_serial, mn_smem);
+      if ((r = run(bw_summary, sm_smem))) return r;
+      scan_combine_rev_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(p.carry, nrows, p.nsplit, NN);
       SIGMA_CHECK_LAUNCH();
-      return run(bw_apply, pm, mn_smem);
+      return run(bw_apply, mn_smem);
     }
-    if (pm.nsplit == 1) {
-      if ((r = run(ss2d_bwd_det_kernel<NN, MODE_SERIAL>, pm, mn_smem))) return r;
+    if (p.nsplit == 1) {
+      if ((r = run(ss2d_bwd_det_kernel<NN, MODE_SERIAL>, mn_smem))) return r;
     } else {
-      if ((r = run(ss2d_bwd_kernel<NN, MODE_SUMMARY>, pm, sm_smem))) return r;
-      scan_combine_rev_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(rcarry, nrows, pm.nsplit, NN);
+      if ((r = run(ss2d_bwd_kernel<NN, MODE_SUMMARY>, sm_smem))) return r;
+      scan_combine_rev_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(p.carry, nrows, p.nsplit, NN);
       SIGMA_CHECK_LAUNCH();
-      if ((r = run(ss2d_bwd_det_kernel<NN, MODE_APPLY>, pm, mn_smem))) return r;
+      if ((r = run(ss2d_bwd_det_kernel<NN, MODE_APPLY>, mn_smem))) return r;
     }
     // fixed-order sums: du over directions k, dB / dC over warp channel tiles, dA / dDs / d dt_bias over (image, segment)
-    const int segs = batch * pm.nsplit;
+    const int segs = batch * p.nsplit;
     const long long KD = (long long)K * D;
     if ((r = sum_parts_det_launch(du_slabs, K, (long long)batch * Lseq * D, (long long)batch * Lseq * D, 0, dxc, stream))) return r;
-    if ((r = sum_parts_det_launch(pm.part_bc, D / CPWc, (long long)batch * Lseq * K * 2 * NN, 2 * NN, Cp, dxdbl, stream))) return r;
-    if ((r = sum_parts_det_launch(pm.part_dA, segs, KD * NN, KD * NN, 0, dA, stream))) return r;
-    if ((r = sum_parts_det_launch(pm.part_dD, segs, KD, KD, 0, dDs, stream))) return r;
-    return sum_parts_det_launch(pm.part_db, segs, KD, KD, 0, ddtb, stream);
+    if ((r = sum_parts_det_launch(p.part_bc, D / CPWc, (long long)batch * Lseq * K * 2 * NN, 2 * NN, Cp, dxdbl, stream))) return r;
+    if ((r = sum_parts_det_launch(p.part_dA, segs, KD * NN, KD * NN, 0, dA, stream))) return r;
+    if ((r = sum_parts_det_launch(p.part_dD, segs, KD, KD, 0, dDs, stream))) return r;
+    return sum_parts_det_launch(p.part_db, segs, KD, KD, 0, ddtb, stream);
   };
   if (N == 16) return go(std::integral_constant<int, 16>{});
   return go(std::integral_constant<int, 4>{});

@@ -445,32 +445,17 @@ def layer_norm(norm, x):
     return norm(x)
 
 
-FUSED_SAVE_STATES = True      # training forward keeps delta' and the block-start states, so the backward runs no state sweep
-
-
 _SAVED_BF16 = 2               # `saved` of _call_ss2d_bwd: the arguments are those of sigma_ss2d_scan_bwd_saved_bf16
 
 
-def _call_ss2d_bwd(args, saved=False, det=False):
-    """The native call of the fused backward (a module-level function so that bench.py can bracket it with events, through a
-    wrapper that passes (args, saved) on: so the bf16 training mode is a value of `saved`, not another argument)."""
+def _call_ss2d_bwd(args, saved=True, det=False):
+    """The native call of the fused backward, sigma_ss2d_scan_bwd_saved (_det when det; _bf16 when saved is _SAVED_BF16).  A
+    module-level function so that bench.py can bracket it with events, through a wrapper that passes (args, saved) on: so the
+    bf16 training mode is a value of `saved`, not another argument."""
     from . import fused
-    L_ = _lib.lib()
-    if saved == _SAVED_BF16:
-        _lib.check(L_.sigma_ss2d_scan_bwd_saved_bf16(*args, int(fused._FORCE_SPLIT or 0), stream()), "sigma_ss2d_scan_bwd_saved_bf16")
-        return
-    if det:
-        fn = L_.sigma_ss2d_scan_bwd_saved_det if saved else L_.sigma_ss2d_scan_bwd_det
-        _lib.check(fn(*args, int(fused._FORCE_SPLIT or 0), stream()), "sigma_ss2d_scan_bwd_det")
-        return
-    if saved:
-        _lib.check(L_.sigma_ss2d_scan_bwd_saved(*args, int(fused._FORCE_SPLIT or 0), stream()), "sigma_ss2d_scan_bwd_saved")
-        return
-    if fused._FORCE_SPLIT:
-        rc = L_.sigma_ss2d_scan_bwd_split(*args, int(fused._FORCE_SPLIT), stream())
-    else:
-        rc = L_.sigma_ss2d_scan_bwd(*args, stream())
-    _lib.check(rc, "sigma_ss2d_scan_bwd")
+    fn = ("sigma_ss2d_scan_bwd_saved_bf16" if saved == _SAVED_BF16 else
+          "sigma_ss2d_scan_bwd_saved_det" if det else "sigma_ss2d_scan_bwd_saved")
+    _lib.check(getattr(_lib.lib(), fn)(*args, int(fused._FORCE_SPLIT or 0), stream()), fn)
 
 
 class FusedSS2DCore(torch.autograd.Function):
@@ -479,17 +464,16 @@ class FusedSS2DCore(torch.autograd.Function):
     the position it belongs to (CrossMerge).  Forward = the inference kernels (x_proj GEMM + the fused scan) in their state-saving
     build (sigma_ss2d_scan_fwd_save: also keeps delta' and the scan state entering every 16-position block); backward =
     sigma_ss2d_scan_bwd_saved (one reverse sweep; no CrossScan / CrossMerge tensors) + the x_proj / dt_proj weight-gradient GEMMs.
-    With FUSED_SAVE_STATES = False the plain forward runs and sigma_ss2d_scan_bwd recomputes both in a state sweep.
     Kind CROSS is Cross_Mamba_Attention_SSM.forward (vmamba.py:1508-1545): xc (2·images, L, D) modality-major, the parameters of
     the two modalities stacked (x_proj_weight (2, R+2N, D), dt_projs_weight (2, D, R), dt_projs_bias (2, D), A_logs (2D, N), Ds
     (2D)); each half runs its own x_proj and weights and reads C from the other half.  It has no deterministic backward.
-    The bf16 training mode (BF16_TRAINING_CORE, bf16 autocast, FUSED_SAVE_STATES, not deterministic, some input needs a gradient):
+    The bf16 training mode (BF16_TRAINING_CORE, bf16 autocast, not deterministic, some input needs a gradient):
     xc is taken (or cast to) bf16 and never widened, x_proj runs the bf16 GEMM with fp32 x_dbl out, sigma_ss2d_scan_fwd_save_bf16
     writes bf16 y and the bf16 delta' its own recurrence ran on, and the backward (sigma_ss2d_scan_bwd_saved_bf16) takes a bf16 dy
     and returns a bf16 dxc rounded once from the fp32 sum of the directions and the x_proj term; parameter gradients are fp32."""
 
     @staticmethod
-    @_bf16_mode_fwd(lambda ctx, xc, *a: FUSED_SAVE_STATES and any(ctx.needs_input_grad) and fused_core_ok(xc, xc.shape[-1], a[3].shape[1])
+    @_bf16_mode_fwd(lambda ctx, xc, *a: any(ctx.needs_input_grad) and fused_core_ok(xc, xc.shape[-1], a[3].shape[1])
                     and all(t.dtype == torch.float32 for t in a[:5]))
     def forward(ctx, xc, x_proj_weight, dt_projs_weight, dt_projs_bias, A_logs, Ds, kind, H, W):
         from . import fused
@@ -515,12 +499,8 @@ class FusedSS2DCore(torch.autograd.Function):
         dtw, dtb = dt_projs_weight.contiguous(), dt_projs_bias.contiguous()
         A = (-torch.exp(A_logs)).contiguous()
         Dsc = Ds.contiguous()
-        if FUSED_SAVE_STATES:
-            y, delta, hs = fused.ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Dsc, B, H, W, D, N, R, Cp)
-            ctx.save_for_backward(xc, xdbl, xw, dtw, dtb, A, Dsc, delta, hs)
-        else:
-            y = fused.ss2d_scan(kind, xc, xdbl, dtw, dtb, A, Dsc, B, H, W, D, N, R, Cp)                              # (K, B, Lseq, D)
-            ctx.save_for_backward(xc, xdbl, xw, dtw, dtb, A, Dsc)
+        y, delta, hs = fused.ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Dsc, B, H, W, D, N, R, Cp)                  # y (K, B, Lseq, D)
+        ctx.save_for_backward(xc, xdbl, xw, dtw, dtb, A, Dsc, delta, hs)
         ctx.meta = (kind, H, W, K, D, N, R, Cp)
         return y[0] if cross else y.sum(0)
 
@@ -528,11 +508,7 @@ class FusedSS2DCore(torch.autograd.Function):
     @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, dy):
         from . import fused
-        saved = len(ctx.saved_tensors) == 9
-        if saved:
-            xc, xdbl, xw, dtw, dtb, A, Ds, delta, hs = ctx.saved_tensors
-        else:
-            xc, xdbl, xw, dtw, dtb, A, Ds = ctx.saved_tensors
+        xc, xdbl, xw, dtw, dtb, A, Ds, delta, hs = ctx.saved_tensors
         kind, H, W, K, D, N, R, Cp = ctx.meta
         cross = kind == _lib.DIRS_CROSS
         Kw = 2 if cross else K                   # parameter sets
@@ -544,8 +520,6 @@ class FusedSS2DCore(torch.autograd.Function):
         bf16 = ctx.bf16_mode
         dy = dy.contiguous().to(torch.bfloat16) if bf16 else dy.contiguous().float()
         dev = xc.device
-        if not saved:
-            delta = torch.empty((K, B, Lseq, D), dtype=torch.float32, device=dev)
         ddelta = torch.empty((K, B, Lseq, D), dtype=torch.float32, device=dev)
         dxc = torch.empty((B, Lseq, D), dtype=torch.float32, device=dev)
         dxdbl = torch.empty((B * Lseq, K, Cp), dtype=torch.float32, device=dev)
@@ -555,15 +529,14 @@ class FusedSS2DCore(torch.autograd.Function):
         L_ = _lib.lib()
         wsb = (L_.sigma_ss2d_scan_bwd_det_workspace_bytes if det else L_.sigma_ss2d_scan_bwd_workspace_bytes)(kind, B, H, W, D, N)
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-        head = (kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(dy), ptr(delta))
-        tail = (ptr(dxc), ptr(ddelta), ptr(dxdbl), ptr(dA), ptr(dDs), ptr(ddtb), B, H, W, D, N, R, Cp, ptr(ws), wsb)
-        args = head + ((ptr(hs),) if saved else ()) + tail
+        args = (kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(dy), ptr(delta), ptr(hs),
+                ptr(dxc), ptr(ddelta), ptr(dxdbl), ptr(dA), ptr(dDs), ptr(ddtb), B, H, W, D, N, R, Cp, ptr(ws), wsb)
         # det only when set: bench.py --mode train brackets this call with a wrapper that takes (args, saved)
         if bf16:
             _call_ss2d_bwd(args, _SAVED_BF16)
             xc = xc.float()                      # only the x_proj weight gradient below (a torch matmul) needs the widened copy
         else:
-            _call_ss2d_bwd(args, saved, True) if det else _call_ss2d_bwd(args, saved)
+            _call_ss2d_bwd(args, True, True) if det else _call_ss2d_bwd(args, True)
         if cross:   # the same two steps per modality half m (its rows of dxdbl / ddelta / xc, its weight set)
             n = B // 2 * Lseq
             xd, dxd, dd = xdbl.view(2, n, Cp), dxdbl.view(2, n, Cp), ddelta.view(2, n, D)

@@ -26,7 +26,7 @@ def _cases():
 @pytest.mark.parametrize("name", ["grad_vssblock", "grad_cromb", "grad_conmb", "grad_cvss_dec"])
 @pytest.mark.parametrize("core", ["fused", "composed"])
 def test_block_gradients_match_reference_autograd(name, core, monkeypatch):
-    """core = fused: SS2D / ConMB train through ops.FusedSS2DCore (f1: sigma_ss2d_scan_bwd); composed: CrossScan + einsums +
+    """core = fused: SS2D / ConMB train through ops.FusedSS2DCore (f1: sigma_ss2d_scan_bwd_saved); composed: CrossScan + einsums +
     the op-level scan kernels.  CroMB always uses the composed path (its scans read the other modality's C)."""
     from sigma_b200 import ops
     monkeypatch.setattr(ops, "FUSED_TRAINING", core == "fused")

@@ -41,7 +41,7 @@ def test_library_has_no_runtime_dependency_on_cuda_libs(lib_path):
 def test_ctypes_binding_matches_header(lib_path):
     from sigma_b200 import _lib
     L = _lib.lib()
-    assert L.sigma_abi_version() == 1
+    assert L.sigma_abi_version() == 2
     assert set(_lib.SIGNATURES) == _declared()
     assert L.sigma_ss2d_padded_cp(16, 6) == 40 and L.sigma_ss2d_padded_cp(4, 24) == 32 and L.sigma_ss2d_padded_cp(4, 65) == -1
     assert L.sigma_scan_fwd_workspace_bytes(2, 768, 1024, 16, 4, 0) > 0

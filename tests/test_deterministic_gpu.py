@@ -2,7 +2,7 @@
 
 * Bitwise repeatability of every `_det` backward: three calls on the same inputs, one of them while another stream keeps the SMs
   busy with GEMMs, must give torch.equal outputs.  The fused SS2D backward at the training shapes and dt_ranks of
-  test_ss2d_bwd_fp64_gpu (state sweep and saved entries, auto and forced L-segment plans); the op-level backward in fp32 / fp16 /
+  test_ss2d_bwd_fp64_gpu (after the training forward, auto and forced L-segment plans); the op-level backward in fp32 / fp16 /
   bf16 at d_state 4, 8, 16 and the generic kernel at L = 690; LayerNorm at every instantiated width; bilinear upsampling at
   Sigma's x2, x4 and size= cases.
 * Accuracy: the fused `_det` outputs inside the per-element fp64 bounds of oracle/ss2d_ref64.py; the op-level ones at the
@@ -67,7 +67,7 @@ def _equal3(outs, tag):
 
 
 # ---- fused SS2D backward ----
-def _ss2d_det(kind, B, H, W, D, N, R, Cp, args, nsplit, saved):
+def _ss2d_det(kind, B, H, W, D, N, R, Cp, args, nsplit):
     from sigma_b200 import _lib
     L_ = _lib.lib()
     xc, xdbl, dtw, dtb, A, Ds, dy = args
@@ -84,15 +84,12 @@ def _ss2d_det(kind, B, H, W, D, N, R, Cp, args, nsplit, saved):
     ws = torch.full((wsb // 4,), float("nan"), device="cuda")
     head = (kid, F64._p(xc), F64._p(xdbl), F64._p(dtw), F64._p(dtb), F64._p(A), F64._p(Ds))
     tail = tuple(F64._p(outs[n]) for n in ("dxc", "ddelta", "dxdbl", "dA", "dDs", "ddtb")) + (B, H, W, D, N, R, Cp, F64._p(ws), wsb)
-    if saved:
-        fwb = L_.sigma_ss2d_scan_workspace_bytes(kid, B, H, W, D, N)
-        fws = torch.zeros(max(fwb, 4), dtype=torch.uint8, device="cuda")
-        _lib.check(L_.sigma_ss2d_scan_fwd_save(*head, F64._p(outs["y"]), F64._p(outs["delta"]), F64._p(outs["hs"]), B, H, W, D, N, R, Cp,
-                                               F64._p(fws), fwb, 0, F64._stream()), "sigma_ss2d_scan_fwd_save")
-        rc = L_.sigma_ss2d_scan_bwd_saved_det(*head, F64._p(dy), F64._p(outs["delta"]), F64._p(outs["hs"]), *tail, nsplit, F64._stream())
-    else:
-        rc = L_.sigma_ss2d_scan_bwd_det(*head, F64._p(dy), F64._p(outs["delta"]), *tail, nsplit, F64._stream())
-    _lib.check(rc, "sigma_ss2d_scan_bwd_det")
+    fwb = L_.sigma_ss2d_scan_workspace_bytes(kid, B, H, W, D, N)
+    fws = torch.zeros(max(fwb, 4), dtype=torch.uint8, device="cuda")
+    _lib.check(L_.sigma_ss2d_scan_fwd_save(*head, F64._p(outs["y"]), F64._p(outs["delta"]), F64._p(outs["hs"]), B, H, W, D, N, R, Cp,
+                                           F64._p(fws), fwb, 0, F64._stream()), "sigma_ss2d_scan_fwd_save")
+    _lib.check(L_.sigma_ss2d_scan_bwd_saved_det(*head, F64._p(dy), F64._p(outs["delta"]), F64._p(outs["hs"]), *tail, nsplit, F64._stream()),
+               "sigma_ss2d_scan_bwd_saved_det")
     torch.cuda.synchronize()
     for name, buf in bufs.items():
         F64._guard_ok(buf, f"{kind} det {name}")
@@ -106,14 +103,14 @@ def test_fused_bwd_det_repeatable_and_within_fp64_bounds(kind, B, H, W, D, N, R)
     ref, bnd = R64.ss2d_ref64(kind, *args, H, W)
     worst = {}
     names = ("dxc", "ddelta", "dA", "dDs", "ddtb")
-    plans = [(0, True), (0, False), (7, True), (1, False)]
+    plans = [0, 7, 1]
     if (H, W) == (15, 20):
-        plans.append((20, True))                 # the shorter walks end in an empty segment (asserted in test_ss2d_bwd_fp64_gpu)
-    for nsplit, saved in plans:
-        t = f"{tag} split={nsplit} saved={saved}"
-        runs = _three(lambda: [o for n, o in _ss2d_det(kind, B, H, W, D, N, R, Cp, args, nsplit, saved).items() if n != "y" or saved])
+        plans.append(20)                         # the shorter walks end in an empty segment (asserted in test_ss2d_bwd_fp64_gpu)
+    for nsplit in plans:
+        t = f"{tag} split={nsplit}"
+        runs = _three(lambda: list(_ss2d_det(kind, B, H, W, D, N, R, Cp, args, nsplit).values()))
         _equal3(runs, t)
-        outs = _ss2d_det(kind, B, H, W, D, N, R, Cp, args, nsplit, saved)
+        outs = _ss2d_det(kind, B, H, W, D, N, R, Cp, args, nsplit)
         for name in names:
             F64._check(t, name, outs[name], ref[name], bnd[name], worst)
         dx = outs["dxdbl"]

@@ -407,7 +407,8 @@ def test_cross_backward_plan_and_sizes(H, W, D, R, images):
             assert nsplit == len(range(0, tiles, -(-tiles // min(force, 64, tiles))))
     hsb = L_.sigma_ss2d_scan_hs_bytes(lib.DIRS_CROSS, Bt, H, W, D, N)
     assert hsb == Bt * tiles * D * N * 4
-    assert L_.sigma_ss2d_scan_bwd_workspace_bytes(lib.DIRS_CROSS, Bt, H, W, D, N) >= hsb
+    for kind, K in ((lib.DIRS_CROSS, 1), (lib.DIRS_CROSS4, 4), (lib.DIRS_SEQ2, 2)):   # the reverse carries of 64 segments, no more
+        assert L_.sigma_ss2d_scan_bwd_workspace_bytes(kind, Bt, H, W, D, N) == -(-Bt * K * D * 64 * 2 * N * 4 // 256) * 256
     assert L_.sigma_ss2d_scan_bwd_det_workspace_bytes(lib.DIRS_CROSS, Bt, H, W, D, N) == 0     # no deterministic build
 
 

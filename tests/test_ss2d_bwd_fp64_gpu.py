@@ -1,17 +1,15 @@
-"""GPU: the fused SS2D scan backward (sigma_ss2d_scan_bwd / _bwd_split with its state sweep, and the training pair
-sigma_ss2d_scan_fwd_save + sigma_ss2d_scan_bwd_saved) against the fp64 reference of oracle/ss2d_ref64.py, element by element inside
-that module's per-element error bounds, at Sigma's training shapes:
-* every padded dt_rank Sigma trains with (6 .. 64), so every x_dbl tile size and state-sweep shared-memory layout runs;
+"""GPU: the fused SS2D scan's training pair (sigma_ss2d_scan_fwd_save + sigma_ss2d_scan_bwd_saved) against the fp64 reference of
+oracle/ss2d_ref64.py, element by element inside that module's per-element error bounds, at Sigma's training shapes:
+* every padded dt_rank Sigma trains with (6 .. 64), so every x_dbl tile size and shared-memory layout runs;
 * ragged maps (15 x 20: every column tile has 15 rows; 23 x 30 odd in both), batch 1, 2 and 3;
 * kind CROSS (CroMB) at its training shapes (d_state 4): Sigma-tiny / small 120x160/192/R6, 60x80/384/12, 30x40/768/24,
   15x20/1536/48 and Sigma-base 180x240/256/8, 23x30/2048/64, with 1, 2 and 3 images (a batch of 2·images);
-* L-segments 1, 2, 7, the library's choice and the 64 cap, a count that leaves the shorter walks an empty trailing segment, and a
-  training forward cut differently from its backward.  The premises (more than one segment at stage 0 by default, the empty
-  segment) are asserted through the backward's planner (sigma_test_ss2d_bwd_plan);
+* backward L-segments 1, 2, 7, the library's choice and the 64 cap, a count that leaves the shorter walks an empty trailing
+  segment, and a training forward cut differently from its backward.  The premises (more than one segment at stage 0 by default,
+  the empty segment) are asserted through the backward's planner (sigma_test_ss2d_bwd_plan);
 * every output inside NaN-filled memory whose guard elements must stay bit-identical, the dt_r and padding columns of dxdbl 0, and
   NaN-filled workspaces;
-* y, delta' and the tile-start states hs of the training forward too, and of the state sweep (its workspace), and the training
-  forward's delta' and hs against the state sweep's.
+* y, delta' and the tile-start states hs of the training forward too.
 At the autograd level FusedSS2DCore.apply is checked through all six gradients against the reference chained with the fp64
 x_proj / dt_proj algebra of its backward, kind cross included, chained per modality half.  Parameters: dt log-uniform in [1e-3, 0.1]
 through the inverse softplus, A = -exp(A_log) around the S4D-real init, Ds near 1; one widened set (dt up to 0.5, |A| up to 4x).
@@ -69,9 +67,9 @@ def _finish(tag, worst, tight=True):
     assert not (tight and loose), f"{tag}: bound at the largest element looser than 1e-3 of scale: {loose}"
 
 
-def _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, tag, worst, split=None, saved=None):
-    """split: the state-sweep backward with that L-segment count (0: the library's choice).  saved = (fwd_split, bwd_split): the
-    training forward followed by the backward that consumes its delta' and states.  Returns (delta, hs) as the route left them."""
+def _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, tag, worst, fwd_split=0, bwd_split=0):
+    """the training forward with fwd_split L-segments followed by the backward with bwd_split (0: the library's choice) that
+    consumes its delta' and states"""
     from sigma_b200 import _lib
     L_ = _lib.lib()
     xc, xdbl, dtw, dtb, A, Ds, dy = args
@@ -89,33 +87,21 @@ def _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, tag, worst, split=None,
     tail = (_p(outs["dxc"]), _p(outs["ddelta"]), _p(outs["dxdbl"]), _p(outs["dA"]), _p(outs["dDs"]), _p(outs["ddtb"]), B, H, W, D, N, R, Cp,
             _p(ws), wsb)
     head = (_kid(kind), _p(xc), _p(xdbl), _p(dtw), _p(dtb), _p(A), _p(Ds))
-    if saved is None:
-        if split:
-            rc = L_.sigma_ss2d_scan_bwd_split(*head, _p(dy), _p(outs["delta"]), *tail, split, _stream())
-        else:
-            rc = L_.sigma_ss2d_scan_bwd(*head, _p(dy), _p(outs["delta"]), *tail, _stream())
-        _lib.check(rc, "sigma_ss2d_scan_bwd")
-        hs = ws[:K * B * T * D * N].view(K, B, T, D, N)
-        names = ("delta", "hs", "dxc", "ddelta", "dA", "dDs", "ddtb")
-    else:
-        fwb = L_.sigma_ss2d_scan_workspace_bytes(_kid(kind), B, H, W, D, N)
-        fws = torch.full((max(fwb, 4) // 4,), float("nan"), device="cuda")
-        _lib.check(L_.sigma_ss2d_scan_fwd_save(*head, _p(outs["y"]), _p(outs["delta"]), _p(outs["hs"]), B, H, W, D, N, R, Cp, _p(fws), fwb,
-                                               saved[0], _stream()), "sigma_ss2d_scan_fwd_save")
-        _lib.check(L_.sigma_ss2d_scan_bwd_saved(*head, _p(dy), _p(outs["delta"]), _p(outs["hs"]), *tail, saved[1], _stream()),
-                   "sigma_ss2d_scan_bwd_saved")
-        hs = outs["hs"]
-        names = OUTS
+    fwb = L_.sigma_ss2d_scan_workspace_bytes(_kid(kind), B, H, W, D, N)
+    fws = torch.full((max(fwb, 4) // 4,), float("nan"), device="cuda")
+    _lib.check(L_.sigma_ss2d_scan_fwd_save(*head, _p(outs["y"]), _p(outs["delta"]), _p(outs["hs"]), B, H, W, D, N, R, Cp, _p(fws), fwb,
+                                           fwd_split, _stream()), "sigma_ss2d_scan_fwd_save")
+    _lib.check(L_.sigma_ss2d_scan_bwd_saved(*head, _p(dy), _p(outs["delta"]), _p(outs["hs"]), *tail, bwd_split, _stream()),
+               "sigma_ss2d_scan_bwd_saved")
     torch.cuda.synchronize()
-    for name in names:
-        _check(tag, name, hs if name == "hs" else outs[name], ref[name], bnd[name], worst)
+    for name in OUTS:
+        _check(tag, name, outs[name], ref[name], bnd[name], worst)
     dx = outs["dxdbl"]
     _check(tag, "dB", dx[..., :N], ref["dB"], bnd["dB"], worst)
     _check(tag, "dC", dx[..., N:2 * N], ref["dC"], bnd["dC"], worst)
     assert bool((dx[..., 2 * N:] == 0).all()), f"{tag}: the dt_r / padding columns of dxdbl must stay 0"
     for name, buf in bufs.items():
         _guard_ok(buf, f"{tag} {name}")
-    return outs["delta"].clone(), hs.clone()
 
 
 # kind, B, H, W, D, N, R
@@ -152,18 +138,8 @@ def test_fused_bwd_matches_fp64(kind, B, H, W, D, N, R):
         if pl["min_tiles"] < pl["max_tiles"]:
             assert (pl["nsplit"] - 1) * pl["tiles_per_split"] >= pl["min_tiles"]   # the shorter walks end in an empty segment
             splits.append(20)
-    for sp in splits:
-        got = _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, f"{tag} split={sp}", worst, split=sp)
-        if sp == 1:
-            d0, h0 = got
-    for fs, bs in [(0, 0), (3, 7), (1, 2)]:
-        delta, hs = _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, f"{tag} saved fwd={fs} bwd={bs}", worst, saved=(fs, bs))
-        # the training forward keeps what the state sweep would recompute: the same delta' and tile-start states, within the bound
-        for name, a, b in (("delta", delta, d0), ("hs", hs, h0)):
-            ok = ~ref[name].isnan()
-            frac = R64.bound_fraction(a[ok], b[ok].double(), 2 * bnd[name][ok])
-            worst["fwd_vs_sweep/" + name] = max(worst.get("fwd_vs_sweep/" + name, 0.0), frac)
-            assert frac <= 1.0, f"{tag} fwd={fs}: {name} of the training forward vs the state sweep: {frac:.3f} of twice the bound"
+    for fs, bs in [(0, sp) for sp in splits] + [(3, 7), (1, 2)]:
+        _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, f"{tag} fwd={fs} bwd={bs}", worst, fs, bs)
     # CroMB's bound at the largest element is recorded; only the other kinds are held to 1e-3 of scale there
     _finish(f"ss2d bwd fp64 {tag}", worst, tight=kind != "cross")
 
@@ -177,8 +153,7 @@ def test_fused_bwd_matches_fp64_widened(kind, B, H, W, D, N, R):
     ref, bnd = R64.ss2d_ref64(kind, *args, H, W)
     worst = {}
     for sp in [1, 0, 7]:
-        _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, f"{tag} split={sp}", worst, split=sp)
-    _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, f"{tag} saved", worst, saved=(0, 0))
+        _run_bwd(kind, B, H, W, D, N, R, Cp, args, ref, bnd, f"{tag} bwd={sp}", worst, bwd_split=sp)
     _finish(f"ss2d bwd fp64 {tag}", worst)
 
 
@@ -284,14 +259,12 @@ def core_xdbl(kind, xc, xpw, N, R, Cp):
 
 @pytest.mark.parametrize("kind,B,H,W,D,N,R", [("cross4", 2, 120, 160, 192, 16, 6), ("seq2", 2, 15, 20, 1536, 4, 48),
                                                ("cross4", 2, 15, 20, 1536, 16, 48), ("cross", 4, 30, 40, 768, 4, 24)])
-@pytest.mark.parametrize("save", [True, False])
-def test_fused_core_autograd_matches_fp64(kind, B, H, W, D, N, R, save, monkeypatch):
+def test_fused_core_autograd_matches_fp64(kind, B, H, W, D, N, R, monkeypatch):
     """FusedSS2DCore.apply: y and all six gradients against the reference chained with the fp64 x_proj / dt_proj algebra.  The
     reference takes the very x_dbl the forward computed (the same deterministic GEMM calls), so only the scan and the backward's
     own fp32 GEMMs are under test; this pins the [dt | B | C] row order and the dA·A step at a real shape.  Kind cross (CroMB, 2
     images): the x_proj GEMMs, dt_proj steps and weight gradients per modality half, dC credited to the other half's rows."""
     from sigma_b200 import _lib, ops
-    monkeypatch.setattr(ops, "FUSED_SAVE_STATES", save)
     monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
     K = {"cross4": 4, "seq2": 2, "cross": 1}[kind]
     Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
@@ -313,21 +286,22 @@ def test_fused_core_autograd_matches_fp64(kind, B, H, W, D, N, R, save, monkeypa
         A64 = A.double()
         want[4], bounds[4] = want[4] * A64, bounds[4] * A64.abs() + 2 * R64.U * (want[4] * A64).abs()
         for name, g, r, b in zip(["dxc", "dx_proj_weight", "ddt_projs_weight", "ddt_projs_bias", "dA_logs", "dDs"], got, want, bounds):
-            _check(f"{tag} save={save}", name, g, r, b, worst)
+            _check(tag, name, g, r, b, worst)
             # the weight gradients contract the scan's per-element bounds over all B·L positions, which leaves their propagated
             # bound looser than 1e-3 of scale at the largest element: there the max-norm bar holds as well
             err = float((g.double() - r).abs().max()) / float(r.abs().max())
-            assert err <= 1e-3, f"{tag} save={save} {name}: {err:.2e} of its scale"
-    _finish(f"ss2d autograd fp64 {tag} save={save}", worst, tight=False)
+            assert err <= 1e-3, f"{tag} {name}: {err:.2e} of its scale"
+    _finish(f"ss2d autograd fp64 {tag}", worst, tight=False)
 
 
 def test_cross_instances_exist_without_local_memory():
     from sigma_b200 import build
     out = subprocess.run(["cuobjdump", "-res-usage", build.LIB], capture_output=True, text=True, check=True).stdout
     use = dict(re.findall(r"Function (\S+):\s*\n\s*(REG:.*)", out))
-    names = [f"_ZN5sigma{len(k)}{k}ILi{n}ELi{m}EEEvNS_13Ss2dBwdParamsE" for k in ("ss2d_bwd_cross_kernel", "ss2d_state_cross_kernel")
-             for n in (4, 16) for m in (0, 1, 2)]
+    names = [f"_ZN5sigma21ss2d_bwd_cross_kernelILi{n}ELi{m}EEEvNS_13Ss2dBwdParamsE" for n in (4, 16) for m in (0, 1, 2)]
     for n in names:
         assert n in use, f"missing CROSS kernel {n}"
         assert re.search(r"\bSTACK:0\b", use[n]) and re.search(r"\bLOCAL:0\b", use[n]), f"{n}: {use[n]}"
     assert not [n for n in use if "cross" in n and "_det" in n]
+    # the backward recomputes no states (the training forward saved them): every kernel of its parameter block is a reverse sweep
+    assert all(n.startswith("_ZN5sigma") and "ss2d_bwd" in n for n in use if "Ss2dBwdParams" in n)
