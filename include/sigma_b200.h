@@ -143,6 +143,11 @@ int sigma_ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const floa
 int sigma_ss2d_scan_fwd_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                              const float *Ds, void *y, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                              size_t workspace_bytes, void *stream);
+/* fp16 inference mode (sigma_b200.fused.fp16_inference): the same with xc and y in fp16 and the launch plan of the bf16 call.
+ * Every fp16 store below rounds once to nearest even; a value past ±65504 is stored as ±inf, as torch's .half() does.        */
+int sigma_ss2d_scan_fwd_fp16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                             const float *Ds, void *y, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                             size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * f1. Training pair of the fused scan.  `sigma_ss2d_scan_fwd_save` is sigma_ss2d_scan_fwd that also writes what its backward
@@ -208,6 +213,8 @@ int sigma_layernorm_fwd(const float *x, const float *w, const float *b, float *y
                         int C, float eps, void *stream);
 /* bf16 inference mode: the same LayerNorm (fp32 statistics) with y stored as bf16 (8-byte aligned), to feed sigma_linear_bf16. */
 int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream);
+/* fp16 inference mode: the same with y stored as fp16, to feed sigma_linear_fp16. */
+int sigma_layernorm_fwd_fp16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream);
 /* bf16 training mode: x and y both bf16 (8-byte aligned rows), fp32 statistics, w and b. */
 int sigma_layernorm_fwd_bf16io(const void *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream);
 
@@ -241,6 +248,9 @@ int sigma_patch_merge_norm_fwd(const float *x, const float *w, const float *b, f
 /* bf16 inference mode: the same gather + LayerNorm with y stored as bf16 (8-byte aligned).                                      */
 int sigma_patch_merge_norm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int batch, int H, int W, int C,
                                     float eps, void *stream);
+/* fp16 inference mode: the same with y stored as fp16. */
+int sigma_patch_merge_norm_fwd_fp16(const float *x, const float *w, const float *b, void *y, int batch, int H, int W, int C,
+                                    float eps, void *stream);
 
 /* PatchExpand back half (MambaDecoder.py:24-30): x is the expand Linear's output (batch,H,W,2,2,C) ("b h w (p1 p2 c)"),
  * y[b,2h+p1,2w+p2,:] = LayerNorm(x[b,h,w,p1,p2,:]); y (batch,2H,2W,C).  The pixel shuffle is the store address.   */
@@ -258,6 +268,9 @@ int sigma_dwconv3x3_silu_fwd(const float *x, int64_t x_row_stride, int64_t x_bat
  * x strides multiples of 8 elements (TMA); y 8-byte aligned, y_batch_stride % 4 == 0.                                          */
 int sigma_dwconv3x3_silu_fwd_bf16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
                                   void *y, int64_t y_batch_stride, int batch, int H, int W, int D, void *stream);
+/* fp16 inference mode: the same with x and y fp16. */
+int sigma_dwconv3x3_silu_fwd_fp16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
+                                  void *y, int64_t y_batch_stride, int batch, int H, int W, int D, void *stream);
 
 /* CrossMerge sum + out_norm LayerNorm + gates (vmamba.py:217-224,1077; ConMB: 423-428,1280-1281):
  *   out[r,:] = (LN(Σ_k y[k][r,:])·gamma+beta) · (z ? SiLU(z[r,:]) : 1) · (gate ? gate[r / rows_per_batch, :] : 1)
@@ -271,6 +284,11 @@ int sigma_merge_norm_gate_fwd(const float *y, int K, int64_t k_stride, int64_t i
 /* bf16 inference mode: the same merge + LayerNorm + gates with y, z and out bf16 (8-byte aligned); gamma, beta, gate and the
  * statistics fp32.  Strides count elements.                                                                                   */
 int sigma_merge_norm_gate_fwd_bf16(const void *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
+                                   const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *out,
+                                   int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
+                                   int D, float eps, void *stream);
+/* fp16 inference mode: the same with y, z and out fp16. */
+int sigma_merge_norm_gate_fwd_fp16(const void *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
                                    const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *out,
                                    int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
                                    int D, float eps, void *stream);
@@ -318,6 +336,10 @@ int sigma_split_tf32_fwd(const float *x, float *hi, float *lo, int64_t n, void *
  * A (M, K) bf16 rows lda elements apart, W (N, K) bf16 contiguous; C rows ldc elements apart, stored as fp32 (c_dtype = SIGMA_F32)
  * or bf16 (SIGMA_BF16, rounded once); bias / residual / rscale fp32.  K, lda % 8 == 0; N, ldc, ldr % 4 == 0; 16-byte aligned.   */
 int sigma_linear_bf16(const void *A, int64_t lda, const void *W, const float *bias, const float *residual, int64_t ldr,
+                      const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream);
+/* fp16 inference mode: the same GEMM on fp16 operands (`wgmma ... k16.f32.f16.f16`), the same tile widths and launch plan; C fp32
+ * (c_dtype = SIGMA_F32) or fp16 (SIGMA_F16, rounded once: past ±65504 it is ±inf).                                             */
+int sigma_linear_fp16(const void *A, int64_t lda, const void *W, const float *bias, const float *residual, int64_t ldr,
                       const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream);
 
 /* ------------------------------------------------------------------------------------------
@@ -370,8 +392,8 @@ int sigma_conv3x3_tf32(const float *x, const float *w9, const float *w9_lo, cons
  * per call; any other value makes the calls and this query return SIGMA_EINVAL).  For tests and tuning.
  * x3 selects the instance: 0 = tf32, 1 = tf32x3 with register-stored output tiles (the conv and
  * sigma_test_linear_tf32x3_regs), 2 = sigma_linear_bf16, 4 = sigma_linear_fp8, 5 = tf32x3 with TMA-stored output tiles
- * (sigma_linear_tf32x3); conv_B must be 0 for 2, 4 and 5; the e4m3 tiles are 32 or 64 wide, and forcing a wider one is
- * SIGMA_EINVAL; other values (3 included) are SIGMA_EINVAL.                                                                   */
+ * (sigma_linear_tf32x3), 7 = sigma_linear_fp16 (the plan of 2); conv_B must be 0 for 2, 4, 5 and 7; the e4m3 tiles are 32 or 64
+ * wide, and forcing a wider one is SIGMA_EINVAL; other values (3 and 6 included) are SIGMA_EINVAL.                            */
 int sigma_test_gemm_plan(int64_t M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, int64_t *out6_host);
 /* sigma_linear_tf32x3 (same arguments and checks) with the output tiles stored from registers instead of through shared memory
  * and TMA: the same products and epilogue operations, so the same bits.  For tests.                                          */
@@ -388,7 +410,7 @@ int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, in
 
 /* Launch plan of the fused scan forward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_fwd (force_split = 0),
  * sigma_ss2d_scan_fwd_split (force_split > 0) or, with bf16 = 1, sigma_ss2d_scan_fwd_bf16 (bf16 = 2: sigma_ss2d_scan_fwd_save_bf16
- * with nsplit = force_split; d_state 8 is SIGMA_EUNSUPPORTED there) would launch for any kind at (batch, H,
+ * with nsplit = force_split; d_state 8 is SIGMA_EUNSUPPORTED there; bf16 = 3: sigma_ss2d_scan_fwd_fp16) would launch for any kind at (batch, H,
  * W, D, N, R) given a workspace of workspace_bytes (0: none), under the current environment (SIGMA_SCAN_WARPS, SIGMA_SCAN_NST,
  * SIGMA_SCAN_CTAS, SIGMA_SCAN_SPLIT_RULE).  out8_host = {segments, LT-position tiles per segment, tiles of the longest direction's
  * walk, tiles of the shortest, warps per CTA, TMA ring depth, register budget (the CTAs per SM the kernel build assumes: 3 or 4),

@@ -1,6 +1,6 @@
-"""Sigma-tiny 480x640 inference at B = 74 by CUDA-graph replay in the fused path's four modes — tf32x3 (default), tf32
-(torch.backends.cuda.matmul.allow_tf32), bf16 (torch.autocast("cuda", dtype=torch.bfloat16)) and fp8
-(sigma_b200.fused.fp8_inference()) — alternating in one process
+"""Sigma-tiny 480x640 inference at B = 74 by CUDA-graph replay in the fused path's five modes — tf32x3 (default), tf32
+(torch.backends.cuda.matmul.allow_tf32), bf16 (torch.autocast("cuda", dtype=torch.bfloat16)), fp8
+(sigma_b200.fused.fp8_inference()) and fp16 (sigma_b200.fused.fp16_inference()) — alternating in one process
 after warm-up.  Prints one JSON line: images/s per mode (median of the rounds), each mode's logits error against tf32x3 on
 the same seeded inputs (max |diff| / max |logit|), peak memory per mode, and the card name and power limit read in the same run.
 
@@ -36,6 +36,8 @@ def _mode_ctx(mode):
     torch.backends.cuda.matmul.allow_tf32 = mode == "tf32"
     if mode == "fp8":
         return fused.fp8_inference()
+    if mode == "fp16":
+        return fused.fp16_inference()
     return torch.autocast("cuda", dtype=torch.bfloat16) if mode == "bf16" else contextlib.nullcontext()
 
 
@@ -59,10 +61,10 @@ def main():
     model = model.cuda().eval()
     rgb = P.randn(7, "bench/rgb", (B, 3, H, W)).cuda()
     x = P.randn(7, "bench/x", (B, 3, H, W)).cuda()
-    modes = ["tf32x3", "tf32", "bf16", "fp8"]
+    modes = ["tf32x3", "tf32", "bf16", "fp8", "fp16"]
     graphs, outs, peak = {}, {}, {}
     stream = torch.cuda.Stream()
-    pool = torch.cuda.graph_pool_handle()            # one memory pool for the four graphs (replayed one at a time): four
+    pool = torch.cuda.graph_pool_handle()            # one memory pool for the five graphs (replayed one at a time): five
                                                      # private pools of a B = 74 forward do not fit in 80 GB
     for m in modes:
         torch.cuda.synchronize()

@@ -330,13 +330,75 @@ int sigma_layernorm_fwd(const float *x, const float *w, const float *b, float *y
   return row_norm_launch(p, (cudaStream_t)stream);
 }
 
-int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && y, "sigma_layernorm_fwd_bf16: null pointer");
-  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd_bf16: C=%d must be a positive multiple of 4", C);
-  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al8(y), "sigma_layernorm_fwd_bf16: x, w, b must be 16-byte and y 8-byte aligned");
+// The bf16 and fp16 twins of one entry point share a body: `fn` names the entry point in its error strings, dtype (SIGMA_BF16 or
+// SIGMA_F16) is the 16-bit element type.
+static int layernorm_fwd_16bit(const char *fn, int dtype, const float *x, const float *w, const float *b, void *y, int64_t rows, int C,
+                               float eps, void *stream) {
+  SIGMA_CHECK_ARG(x && w && b && y, "%s: null pointer", fn);
+  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "%s: C=%d must be a positive multiple of 4", fn, C);
+  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al8(y), "%s: x, w, b must be 16-byte and y 8-byte aligned", fn);
   RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
-  p.io = 1;
+  p.io = dtype == SIGMA_F16 ? 5 : 1;
   return row_norm_launch(p, (cudaStream_t)stream);
+}
+
+static int patch_merge_norm_fwd_16bit(const char *fn, int dtype, const float *x, const float *w, const float *b, void *y, int batch, int H,
+                                      int W, int C, float eps, void *stream) {
+  SIGMA_CHECK_ARG(x && w && b && y, "%s: null pointer", fn);
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "%s: bad sizes", fn);
+  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al8(y), "%s: x, w, b must be 16-byte and y 8-byte aligned", fn);
+  const int64_t rows = (int64_t)batch * ((H + 1) / 2) * ((W + 1) / 2);
+  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows, 0, 0, 4 * C, 4 * C, eps};
+  p.mode = 1; p.gH = H; p.gW = W; p.io = dtype == SIGMA_F16 ? 5 : 1;
+  return row_norm_launch(p, (cudaStream_t)stream);
+}
+
+static int merge_norm_gate_fwd_16bit(const char *fn, int dtype, const void *y, int K, int64_t k_stride, int64_t in_batch_stride,
+                                     const float *gamma, const float *beta, const void *z, int64_t z_row_stride, const float *gate,
+                                     void *out, int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
+                                     int D, float eps, void *stream) {
+  SIGMA_CHECK_ARG(y && gamma && beta && out, "%s: null pointer", fn);
+  SIGMA_CHECK_ARG(K >= 1 && K <= 8 && D > 0 && D % 4 == 0 && rows >= 0 && rows_per_batch > 0,
+                  "%s: bad sizes K=%d D=%d rows=%lld rows_per_batch=%lld", fn, K, D, (long long)rows, (long long)rows_per_batch);
+  SIGMA_CHECK_ARG(al8(y) && al16(gamma) && al16(beta) && al8(out) && al8(z) && al16(gate) && k_stride % 4 == 0 &&
+                      in_batch_stride % 4 == 0 && out_batch_stride % 4 == 0 && out_row_stride % 4 == 0 && z_row_stride % 4 == 0,
+                  "%s: y / z / out must be 8-byte and gamma / beta / gate 16-byte aligned, strides multiples of 4", fn);
+  RowNormParams p{(const float *)y, k_stride, K, gamma, beta, (const float *)z, z_row_stride, gate, (float *)out, rows, rows_per_batch,
+                  in_batch_stride, out_batch_stride, out_row_stride, D, eps};
+  p.io = dtype == SIGMA_F16 ? 6 : 2;
+  return row_norm_launch(p, (cudaStream_t)stream);
+}
+
+static int dwconv3x3_silu_fwd_16bit(const char *fn, int dtype, const void *x, int64_t x_row_stride, int64_t x_batch_stride,
+                                    const float *w, const float *bias, void *y, int64_t y_batch_stride, int batch, int H, int W, int D,
+                                    void *stream) {
+  SIGMA_CHECK_ARG(x && w && y, "%s: null pointer", fn);
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % 4 == 0, "%s: bad sizes", fn);
+  SIGMA_CHECK_ARG(al16(x) && al8(y) && x_row_stride % 8 == 0 && x_batch_stride % 8 == 0 && y_batch_stride % 4 == 0,
+                  "%s: x must be 16-byte aligned with strides multiples of 8 elements (TMA), y 8-byte aligned", fn);
+  return dwconv3x3_silu_16bit_launch(dtype, x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D,
+                                     (cudaStream_t)stream);
+}
+
+static int linear_16bit(const char *fn, int dtype, const void *A, int64_t lda, const void *W, const float *bias, const float *residual,
+                        int64_t ldr, const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream) {
+  const bool f16 = dtype == SIGMA_F16;
+  SIGMA_CHECK_ARG(A && W && C, "%s: null pointer", fn);
+  SIGMA_CHECK_ARG(c_dtype == SIGMA_F32 || c_dtype == dtype, "%s: c_dtype %d (SIGMA_F32 or %s)", fn, c_dtype, f16 ? "SIGMA_F16" : "SIGMA_BF16");
+  SIGMA_CHECK_ARG(M >= 0 && M < (1LL << 31) && N > 0 && K > 0, "%s: bad sizes M=%lld N=%d K=%d", fn, (long long)M, N, K);
+  SIGMA_CHECK_ARG(K % 8 == 0 && lda % 8 == 0 && N % 4 == 0 && ldc % 4 == 0 && (residual == nullptr || ldr % 4 == 0) && lda >= K && ldc >= N,
+                  "%s: K and lda must be multiples of 8 (16-byte %s TMA rows); N, ldc, ldr multiples of 4", fn, f16 ? "fp16" : "bf16");
+  SIGMA_CHECK_ARG(al16(A) && al16(W) && al16(C) && al16(bias) && al16(residual) && al16(rscale), "%s: pointers must be 16-byte aligned", fn);
+  SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "%s: rscale without residual", fn);
+  return gemm_16bit_launch(dtype, A, lda, W, bias, residual, ldr, rscale, C, ldc, c_dtype == dtype, M, N, K, (cudaStream_t)stream);
+}
+
+int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
+  return layernorm_fwd_16bit("sigma_layernorm_fwd_bf16", SIGMA_BF16, x, w, b, y, rows, C, eps, stream);
+}
+
+int sigma_layernorm_fwd_fp16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
+  return layernorm_fwd_16bit("sigma_layernorm_fwd_fp16", SIGMA_F16, x, w, b, y, rows, C, eps, stream);
 }
 
 int sigma_layernorm_fwd_fp8(const float *x, const float *w, const float *b, void *q, float *scale, int64_t rows, int C, float eps,
@@ -411,13 +473,12 @@ int sigma_patch_merge_norm_fwd(const float *x, const float *w, const float *b, f
 
 int sigma_patch_merge_norm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int batch, int H, int W, int C,
                                     float eps, void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && y, "sigma_patch_merge_norm_fwd_bf16: null pointer");
-  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "sigma_patch_merge_norm_fwd_bf16: bad sizes");
-  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al8(y), "sigma_patch_merge_norm_fwd_bf16: x, w, b must be 16-byte and y 8-byte aligned");
-  const int64_t rows = (int64_t)batch * ((H + 1) / 2) * ((W + 1) / 2);
-  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows, 0, 0, 4 * C, 4 * C, eps};
-  p.mode = 1; p.gH = H; p.gW = W; p.io = 1;
-  return row_norm_launch(p, (cudaStream_t)stream);
+  return patch_merge_norm_fwd_16bit("sigma_patch_merge_norm_fwd_bf16", SIGMA_BF16, x, w, b, y, batch, H, W, C, eps, stream);
+}
+
+int sigma_patch_merge_norm_fwd_fp16(const float *x, const float *w, const float *b, void *y, int batch, int H, int W, int C,
+                                    float eps, void *stream) {
+  return patch_merge_norm_fwd_16bit("sigma_patch_merge_norm_fwd_fp16", SIGMA_F16, x, w, b, y, batch, H, W, C, eps, stream);
 }
 
 int sigma_patch_merge_norm_fwd_fp8(const float *x, const float *w, const float *b, void *q, float *scale, int batch, int H, int W, int C,
@@ -481,17 +542,16 @@ int sigma_merge_norm_gate_fwd_bf16(const void *y, int K, int64_t k_stride, int64
                                    const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *out,
                                    int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
                                    int D, float eps, void *stream) {
-  SIGMA_CHECK_ARG(y && gamma && beta && out, "sigma_merge_norm_gate_fwd_bf16: null pointer");
-  SIGMA_CHECK_ARG(K >= 1 && K <= 8 && D > 0 && D % 4 == 0 && rows >= 0 && rows_per_batch > 0,
-                  "sigma_merge_norm_gate_fwd_bf16: bad sizes K=%d D=%d rows=%lld rows_per_batch=%lld", K, D, (long long)rows,
-                  (long long)rows_per_batch);
-  SIGMA_CHECK_ARG(al8(y) && al16(gamma) && al16(beta) && al8(out) && al8(z) && al16(gate) && k_stride % 4 == 0 &&
-                      in_batch_stride % 4 == 0 && out_batch_stride % 4 == 0 && out_row_stride % 4 == 0 && z_row_stride % 4 == 0,
-                  "sigma_merge_norm_gate_fwd_bf16: y / z / out must be 8-byte and gamma / beta / gate 16-byte aligned, strides multiples of 4");
-  RowNormParams p{(const float *)y, k_stride, K, gamma, beta, (const float *)z, z_row_stride, gate, (float *)out, rows, rows_per_batch,
-                  in_batch_stride, out_batch_stride, out_row_stride, D, eps};
-  p.io = 2;
-  return row_norm_launch(p, (cudaStream_t)stream);
+  return merge_norm_gate_fwd_16bit("sigma_merge_norm_gate_fwd_bf16", SIGMA_BF16, y, K, k_stride, in_batch_stride, gamma, beta, z,
+                                   z_row_stride, gate, out, out_batch_stride, out_row_stride, rows, rows_per_batch, D, eps, stream);
+}
+
+int sigma_merge_norm_gate_fwd_fp16(const void *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
+                                   const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *out,
+                                   int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
+                                   int D, float eps, void *stream) {
+  return merge_norm_gate_fwd_16bit("sigma_merge_norm_gate_fwd_fp16", SIGMA_F16, y, K, k_stride, in_batch_stride, gamma, beta, z,
+                                   z_row_stride, gate, out, out_batch_stride, out_row_stride, rows, rows_per_batch, D, eps, stream);
 }
 
 int sigma_dwconv3x3_silu_fwd(const float *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w,
@@ -507,11 +567,14 @@ int sigma_dwconv3x3_silu_fwd(const float *x, int64_t x_row_stride, int64_t x_bat
 
 int sigma_dwconv3x3_silu_fwd_bf16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
                                   void *y, int64_t y_batch_stride, int batch, int H, int W, int D, void *stream) {
-  SIGMA_CHECK_ARG(x && w && y, "sigma_dwconv3x3_silu_fwd_bf16: null pointer");
-  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % 4 == 0, "sigma_dwconv3x3_silu_fwd_bf16: bad sizes");
-  SIGMA_CHECK_ARG(al16(x) && al8(y) && x_row_stride % 8 == 0 && x_batch_stride % 8 == 0 && y_batch_stride % 4 == 0,
-                  "sigma_dwconv3x3_silu_fwd_bf16: x must be 16-byte aligned with strides multiples of 8 elements (TMA), y 8-byte aligned");
-  return dwconv3x3_silu_bf16_launch(x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D, (cudaStream_t)stream);
+  return dwconv3x3_silu_fwd_16bit("sigma_dwconv3x3_silu_fwd_bf16", SIGMA_BF16, x, x_row_stride, x_batch_stride, w, bias, y,
+                                  y_batch_stride, batch, H, W, D, stream);
+}
+
+int sigma_dwconv3x3_silu_fwd_fp16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
+                                  void *y, int64_t y_batch_stride, int batch, int H, int W, int D, void *stream) {
+  return dwconv3x3_silu_fwd_16bit("sigma_dwconv3x3_silu_fwd_fp16", SIGMA_F16, x, x_row_stride, x_batch_stride, w, bias, y,
+                                  y_batch_stride, batch, H, W, D, stream);
 }
 
 int sigma_ss2d_padded_cp(int N, int R) {
@@ -538,6 +601,16 @@ static int ss2d_check(int kind, const float *xc, const float *xdbl, const float 
   return SIGMA_OK;
 }
 
+static int ss2d_scan_fwd_16bit(const char *fn, int dtype, int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb,
+                               const float *A, const float *Ds, void *y, int batch, int H, int W, int D, int N, int R, int Cp,
+                               void *workspace, size_t workspace_bytes, void *stream) {
+  int rc = ss2d_check(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp);
+  if (rc) return rc;
+  SIGMA_CHECK_ARG(D % 8 == 0, "%s: D=%d must be a multiple of 8 (16-byte TMA rows)", fn, D);
+  return ss2d_scan_fwd(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp, workspace, workspace_bytes,
+                       0, (cudaStream_t)stream, nullptr, nullptr, dtype);
+}
+
 int sigma_ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb,
                         const float *A, const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp,
                         void *workspace, size_t workspace_bytes, void *stream) {
@@ -550,11 +623,15 @@ int sigma_ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const floa
 int sigma_ss2d_scan_fwd_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                              const float *Ds, void *y, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                              size_t workspace_bytes, void *stream) {
-  int rc = ss2d_check(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp);
-  if (rc) return rc;
-  SIGMA_CHECK_ARG(D % 8 == 0, "sigma_ss2d_scan_fwd_bf16: D=%d must be a multiple of 8 (16-byte TMA rows)", D);
-  return ss2d_scan_fwd(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp, workspace, workspace_bytes,
-                       0, (cudaStream_t)stream, nullptr, nullptr, 1);
+  return ss2d_scan_fwd_16bit("sigma_ss2d_scan_fwd_bf16", SIGMA_BF16, kind, xc, xdbl, dtw, dtb, A, Ds, y, batch, H, W, D, N, R, Cp,
+                             workspace, workspace_bytes, stream);
+}
+
+int sigma_ss2d_scan_fwd_fp16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                             const float *Ds, void *y, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                             size_t workspace_bytes, void *stream) {
+  return ss2d_scan_fwd_16bit("sigma_ss2d_scan_fwd_fp16", SIGMA_F16, kind, xc, xdbl, dtw, dtb, A, Ds, y, batch, H, W, D, N, R, Cp,
+                             workspace, workspace_bytes, stream);
 }
 
 // test hook: force the number of L-segments
@@ -594,8 +671,8 @@ int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, in
   return SIGMA_OK;
 }
 
-// the launch plan of sigma_ss2d_scan_fwd{,_split,_bf16} and, with bf16 = 2, of sigma_ss2d_scan_fwd_save_bf16 (force_split = 0: the
-// library's choice), environment overrides included:
+// the launch plan of sigma_ss2d_scan_fwd{,_split,_bf16}, with bf16 = 2 of sigma_ss2d_scan_fwd_save_bf16 and with bf16 = 3 of
+// sigma_ss2d_scan_fwd_fp16 (force_split = 0: the library's choice), environment overrides included:
 // out8_host = {segments, tiles per segment, tiles of the longest walk, of the shortest, warps per CTA, ring depth, register
 // budget (CTAs per SM the kernel build assumes), dynamic shared-memory bytes}
 int sigma_test_ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R, int bf16, int force_split, size_t workspace_bytes,
@@ -609,7 +686,8 @@ int sigma_test_ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, in
     return SIGMA_EUNSUPPORTED;
   }
   long long out[8];
-  const int rc = ss2d_fwd_plan_hook(kind, batch, H, W, D, N, R, bf16 ? 1 : 0, force_split, workspace_bytes, out);
+  const int rc = ss2d_fwd_plan_hook(kind, batch, H, W, D, N, R, bf16 == 3 ? SIGMA_F16 : bf16 ? SIGMA_BF16 : SIGMA_F32, force_split,
+                                    workspace_bytes, out);
   if (rc) return rc;
   for (int i = 0; i < 8; ++i) out8_host[i] = out[i];
   return SIGMA_OK;
@@ -648,7 +726,7 @@ int sigma_ss2d_scan_fwd_save_bf16(int kind, const void *xc, const float *xdbl, c
   SIGMA_CHECK_ARG(delta && hs && al16(delta) && al16(hs), "sigma_ss2d_scan_fwd_save_bf16: delta / hs must be non-null and 16-byte aligned");
   SIGMA_CHECK_ARG(nsplit >= 0, "sigma_ss2d_scan_fwd_save_bf16: nsplit=%d < 0", nsplit);
   return ss2d_scan_fwd(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp, workspace, workspace_bytes,
-                       nsplit, (cudaStream_t)stream, (float *)delta, hs, 1);
+                       nsplit, (cudaStream_t)stream, (float *)delta, hs, SIGMA_BF16);
 }
 
 size_t sigma_ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
@@ -863,15 +941,12 @@ int sigma_linear_tf32(const float *A, int64_t lda, const float *W, const float *
 
 int sigma_linear_bf16(const void *A, int64_t lda, const void *W, const float *bias, const float *residual, int64_t ldr,
                       const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream) {
-  SIGMA_CHECK_ARG(A && W && C, "sigma_linear_bf16: null pointer");
-  SIGMA_CHECK_ARG(c_dtype == SIGMA_F32 || c_dtype == SIGMA_BF16, "sigma_linear_bf16: c_dtype %d (SIGMA_F32 or SIGMA_BF16)", c_dtype);
-  SIGMA_CHECK_ARG(M >= 0 && M < (1LL << 31) && N > 0 && K > 0, "sigma_linear_bf16: bad sizes M=%lld N=%d K=%d", (long long)M, N, K);
-  SIGMA_CHECK_ARG(K % 8 == 0 && lda % 8 == 0 && N % 4 == 0 && ldc % 4 == 0 && (residual == nullptr || ldr % 4 == 0) && lda >= K && ldc >= N,
-                  "sigma_linear_bf16: K and lda must be multiples of 8 (16-byte bf16 TMA rows); N, ldc, ldr multiples of 4");
-  SIGMA_CHECK_ARG(al16(A) && al16(W) && al16(C) && al16(bias) && al16(residual) && al16(rscale),
-                  "sigma_linear_bf16: pointers must be 16-byte aligned");
-  SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "sigma_linear_bf16: rscale without residual");
-  return gemm_bf16_launch(A, lda, W, bias, residual, ldr, rscale, C, ldc, c_dtype == SIGMA_BF16, M, N, K, (cudaStream_t)stream);
+  return linear_16bit("sigma_linear_bf16", SIGMA_BF16, A, lda, W, bias, residual, ldr, rscale, C, ldc, c_dtype, M, N, K, stream);
+}
+
+int sigma_linear_fp16(const void *A, int64_t lda, const void *W, const float *bias, const float *residual, int64_t ldr,
+                      const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream) {
+  return linear_16bit("sigma_linear_fp16", SIGMA_F16, A, lda, W, bias, residual, ldr, rscale, C, ldc, c_dtype, M, N, K, stream);
 }
 
 int sigma_linear_fp8(const void *A, int64_t lda, const float *sa, const void *Wq, const float *sw, const float *bias, const float *residual,

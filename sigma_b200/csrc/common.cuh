@@ -59,7 +59,7 @@ template <> __device__ __forceinline__ uint32_t from_f32x2<__nv_bfloat16>(float 
   return *reinterpret_cast<const uint32_t *>(&h);
 }
 
-// ---- 4-element fp32 / bf16 accesses (a float4 or 8 bytes of bf16) ----
+// ---- 4-element fp32 / bf16 / fp16 accesses (a float4 or 8 bytes of bf16 / fp16) ----
 __device__ __forceinline__ float4 bf16x4_to_f4(uint2 u) {
   return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
                      __uint_as_float(u.y & 0xFFFF0000u));
@@ -73,6 +73,17 @@ __device__ __forceinline__ float4 ld4cs(const __nv_bfloat16 *p) { return bf16x4_
 __device__ __forceinline__ void st4(float *p, float4 v) { *reinterpret_cast<float4 *>(p) = v; }
 __device__ __forceinline__ void st4(__nv_bfloat16 *p, float4 v) {
   *reinterpret_cast<uint2 *>(p) = make_uint2(from_f32x2<__nv_bfloat16>(v.x, v.y), from_f32x2<__nv_bfloat16>(v.z, v.w));
+}
+// the same for fp16 (the fp16 inference mode); a store past ±65504 gives ±inf, as torch's .half()
+__device__ __forceinline__ float4 f16x4_to_f4(uint2 u) {
+  const float2 a = __half22float2(*reinterpret_cast<const __half2 *>(&u.x)), b = __half22float2(*reinterpret_cast<const __half2 *>(&u.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ float4 ld4(const __half *p) { return f16x4_to_f4(*reinterpret_cast<const uint2 *>(p)); }
+__device__ __forceinline__ float4 ld4g(const __half *p) { return f16x4_to_f4(__ldg(reinterpret_cast<const uint2 *>(p))); }
+__device__ __forceinline__ float4 ld4cs(const __half *p) { return f16x4_to_f4(__ldcs(reinterpret_cast<const uint2 *>(p))); }
+__device__ __forceinline__ void st4(__half *p, float4 v) {
+  *reinterpret_cast<uint2 *>(p) = make_uint2(from_f32x2<__half>(v.x, v.y), from_f32x2<__half>(v.z, v.w));
 }
 
 // ---- e4m3 rows with one fp32 scale per row (the FP8 inference mode; the formula is stated in sigma_b200.h) ----

@@ -11,6 +11,7 @@
 // The first version of this kernel read its window straight from global memory through L1 (18 loads per 4
 // outputs, no prefetch across loop iterations) and reached ~35 % of the HBM roofline.
 #include <algorithm>
+#include <type_traits>
 #include "common.cuh"
 #include "tma.cuh"
 
@@ -29,8 +30,8 @@ struct DwTmaParams {
   long long ntiles;
 };
 
-// T: element type of x and y (float, or __nv_bfloat16 in the bf16 inference mode: same tiles at half the bytes; weights, bias
-// and the accumulation stay fp32)
+// T: element type of x and y (float, or __nv_bfloat16 / __half in the bf16 / fp16 inference modes: same tiles at half the bytes;
+// weights, bias and the accumulation stay fp32)
 template <typename T>
 __global__ void __launch_bounds__(DC_THREADS, 2) dwconv3x3_silu_tma_kernel(const __grid_constant__ DwTmaParams p) {
   constexpr int DC_TILE_BYTES = DC_TILE_FL * (int)sizeof(T);
@@ -143,8 +144,9 @@ static int dwconv_tma_launch(const T *x, long long x_row_stride, long long x_bat
   const uint64_t dims[4] = {(uint64_t)D, (uint64_t)W, (uint64_t)H, (uint64_t)batch};
   const uint64_t str[3] = {(uint64_t)x_row_stride * es, (uint64_t)W * x_row_stride * es, (uint64_t)x_batch_stride * es};
   const uint32_t box[4] = {DC_CB, DC_TW + 2, DC_TH + 2, 1};
-  int rc = make_tmap(&p.map, es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x, dims, str, box,
-                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+  const CUtensorMapDataType dt = es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  int rc = make_tmap(&p.map, dt, 4, x, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
   if (rc) return rc;
   p.w = w; p.bias = bias; p.y = y; p.y_batch_stride = y_batch_stride;
   p.batch = batch; p.H = H; p.W = W; p.D = D;
@@ -174,9 +176,13 @@ int dwconv3x3_silu_tma_launch(const float *x, long long x_row_stride, long long 
   return dwconv_tma_launch<float>(x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D, stream);
 }
 
-// bf16 x and y (the caller checks the 16-byte stride / alignment TMA needs: there is no direct bf16 kernel to fall back to)
-int dwconv3x3_silu_bf16_launch(const void *x, long long x_row_stride, long long x_batch_stride, const float *w, const float *bias,
-                               void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream) {
+// 16-bit x and y, dtype SIGMA_BF16 or SIGMA_F16 (the caller checks the 16-byte stride / alignment TMA needs: there is no direct
+// 16-bit kernel to fall back to)
+int dwconv3x3_silu_16bit_launch(int dtype, const void *x, long long x_row_stride, long long x_batch_stride, const float *w,
+                                const float *bias, void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream) {
+  if (dtype == SIGMA_F16)
+    return dwconv_tma_launch<__half>((const __half *)x, x_row_stride, x_batch_stride, w, bias, (__half *)y, y_batch_stride, batch, H,
+                                     W, D, stream);
   return dwconv_tma_launch<__nv_bfloat16>((const __nv_bfloat16 *)x, x_row_stride, x_batch_stride, w, bias, (__nv_bfloat16 *)y,
                                           y_batch_stride, batch, H, W, D, stream);
 }

@@ -45,7 +45,7 @@ struct alignas(64) GemmParams {
   float *C;
   long long ldr, ldc;
   int M, N, K, BN, stages;   // BN: host-side choice of the template instance
-  int c_bf16;       // BF16: 1 = C is stored as bf16 (bias / residual / rscale stay fp32)
+  int c_bf16;       // BF16, FP8: 1 = C is stored as bf16; F16: as fp16 (bias / residual / rscale stay fp32)
   int cH, cW, tiles_w, tiles_hw, kbc, act;   // CONV: image size, 8x16 patches per row / per image, Cin blocks per tap, activation
   const float *sa, *sw;   // FP8: per-row scales of A, per-output-channel scales of W
   CUtensorMap m_c, m_r;   // TMA_C: C and (if any) the residual, GM_CHUNK x 64 boxes
@@ -602,6 +602,174 @@ template <> __device__ __forceinline__ void wgmma_bf16<256>(float (&d)[128], uin
       : "l"(da), "l"(db), "r"(scale_d));
 }
 
+// the same in fp16 (F16 instance, gemm_fp16_kernel): `k16.f32.f16.f16`, the same stage layout and descriptor advance
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_f16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_f16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_f16<96>(float (&d)[48], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+      "%48, %49, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_f16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_f16<160>(float (&d)[80], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %82, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n160k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
+      "%80, %81, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_f16<192>(float (&d)[96], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %98, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n192k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
+      "%96, %97, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_f16<224>(float (&d)[112], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %114, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n224k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111}, "
+      "%112, %113, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_f16<256>(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+
 // D[64 x N] (+)= A[64 x 32] · B[N x 32]^T in e4m3 (FP8 instance): a k32 e4m3 step is 32 bytes, like a k8 tf32 step, so the
 // swizzled stage layout and the +32 B descriptor advance are shared; both operands K-major (the only layout e4m3 wgmma takes)
 template <int N>
@@ -650,12 +818,14 @@ __device__ __forceinline__ void load_residual_chunk(const GemmParams &p, unsigne
 // TMA_C (gemm_x3_tma_kernel): the epilogue stages each warpgroup's output in GM_CHUNK-column chunks in shared memory and
 // stores them with TMA, asynchronously, so the consumers go on to the next tile's MMAs while the stores drain; the residual
 // chunks arrive by TMA as well, the first two during the tile's k-loop.
-template <int BN, bool X3, bool CONV, bool BF16, bool FP8, bool TMA_C = false>
+// F16 (gemm_fp16_kernel): the BF16 instance on fp16 operands, C fp32 or (p.c_bf16) fp16.
+template <int BN, bool X3, bool CONV, bool BF16, bool FP8, bool TMA_C = false, bool F16 = false>
 __device__ __forceinline__ void gemm_body(const GemmParams &p) {
   static_assert(!BF16 || (!X3 && !CONV), "the bf16 instance is a plain GEMM");
   static_assert(!FP8 || (!X3 && !CONV && !BF16), "the e4m3 instance is a plain GEMM");
+  static_assert(!F16 || (!X3 && !CONV && !BF16 && !FP8), "the fp16 instance is a plain GEMM");
   static_assert(!TMA_C || (X3 && !CONV), "the TMA-stored epilogue is the tf32x3 linear instance's");
-  constexpr int KB = FP8 ? 4 * GM_BK : BF16 ? 2 * GM_BK : GM_BK;   // elements per k-block: one 128-byte swizzle row in every case
+  constexpr int KB = FP8 ? 4 * GM_BK : (BF16 || F16) ? 2 * GM_BK : GM_BK;   // elements per k-block: one 128-byte swizzle row in every case
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const int S = p.stages;
   constexpr int a_bytes = GM_BM * GM_BK * 4, b_bytes = BN * GM_BK * 4;
@@ -804,7 +974,8 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < GM_BK / GM_UK; ++k) {   // +32 B along K inside the swizzle row = +2 in 16-byte units
-          if (BF16) wgmma_bf16<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
+          if constexpr (F16) wgmma_f16<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
+          else if (BF16) wgmma_bf16<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
           else wgmma_tf32<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
         }
         wgmma_commit();
@@ -881,7 +1052,7 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;   // row inside the 128-row tile
-      long long coff;   // element offset of the row in C (fp32 or, (BF16 || FP8) && p.c_bf16, bf16)
+      long long coff;   // element offset of the row in C (fp32 or, (BF16 || FP8 || F16) && p.c_bf16, bf16 / fp16)
       const float *rrow = nullptr;
       float srow = 1.f;   // FP8: the activation row's scale
       if (CONV) {   // row r = pixel (r / 16, r % 16) of the 8 x 16 patch
@@ -921,7 +1092,9 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
           o.x = 0.5f * o.x * (1.f + erff(o.x * 0.70710678118654752f));
           o.y = 0.5f * o.y * (1.f + erff(o.y * 0.70710678118654752f));
         }
-        if ((BF16 || FP8) && p.c_bf16)
+        if (F16 && p.c_bf16)
+          *reinterpret_cast<__half2 *>(reinterpret_cast<__half *>(p.C) + coff + n) = __floats2half2_rn(o.x, o.y);
+        else if ((BF16 || FP8) && p.c_bf16)
           *reinterpret_cast<__nv_bfloat162 *>(reinterpret_cast<__nv_bfloat16 *>(p.C) + coff + n) = __floats2bfloat162_rn(o.x, o.y);
         else
           *reinterpret_cast<float2 *>(p.C + coff + n) = o;
@@ -950,14 +1123,24 @@ __global__ void __launch_bounds__(GM_THREADS, 2) gemm_fp8_kernel(const __grid_co
   gemm_body<BN, false, false, false, true>(p);
 }
 
+// The fp16 instance: the bf16 instance's widths, ring and occupancy with `k16.f32.f16.f16` MMAs (a separate kernel, so that
+// gemm_tf32_kernel<..., BF16> stays as it was)
+template <int BN>
+__global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_fp16_kernel(const __grid_constant__ GemmParams p) {
+  gemm_body<BN, false, false, false, false, false, true>(p);
+}
+
 // ---- host ----
-// K-major operand map: 128-byte box rows (GM_BK fp32 or, bf16 = true, 2·GM_BK bf16 elements) with the 128-byte swizzle
+// K-major operand map: 128-byte box rows (GM_BK fp32 or, dtype SIGMA_BF16 / SIGMA_F16, 2·GM_BK 16-bit elements) with the
+// 128-byte swizzle
 static int make_tmap_2d_sw128(CUtensorMap *map, const void *base, long long rows, long long cols, long long ld, int box_rows,
-                              bool bf16 = false) {
-  const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows}, str[1] = {(uint64_t)ld * (bf16 ? 2 : 4)};
-  const uint32_t box[2] = {(uint32_t)(bf16 ? 2 * GM_BK : GM_BK), (uint32_t)box_rows};
-  return make_tmap(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, dims, str, box,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+                              int dtype = SIGMA_F32) {
+  const bool h = dtype != SIGMA_F32;
+  const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows}, str[1] = {(uint64_t)ld * (h ? 2 : 4)};
+  const uint32_t box[2] = {(uint32_t)(h ? 2 * GM_BK : GM_BK), (uint32_t)box_rows};
+  const CUtensorMapDataType dt = dtype == SIGMA_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                 : dtype == SIGMA_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  return make_tmap(map, dt, 2, base, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 // the same for e4m3 operands: 128 one-byte elements per box row
 static int make_tmap_2d_sw128_u8(CUtensorMap *map, const void *base, long long rows, long long cols, long long ld, int box_rows) {
@@ -1071,11 +1254,11 @@ static int plan_gemm(long long M, int N, int K, bool x3, int conv_B, int conv_H,
 // api.cu test hook: out = {BN, stages, grid, tiles, smem bytes, CTAs per SM}.  x3: 0 = tf32, 1 = tf32x3 with the register-stored
 // epilogue (the conv, and sigma_test_linear_tf32x3_regs), 2 = bf16 (the bf16 instance stages the
 // same bytes per k-block as tf32 — 128-byte rows — so its plan is the tf32 plan), 4 = e4m3 (the same stage bytes too, narrower
-// widths), 5 = tf32x3 with the TMA-stored epilogue (linear only); 3 is not a mode
+// widths), 5 = tf32x3 with the TMA-stored epilogue (linear only), 7 = fp16 (the bf16 plan); 3 and 6 are not modes
 int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out) {
   GemmPlan pl;
-  if (x3 < 0 || x3 > 5 || x3 == 3 || (x3 >= 2 && conv_B > 0)) {
-    set_error("gemm plan: mode %d (0 tf32, 1 tf32x3, 2 bf16, 4 e4m3, 5 tf32x3 TMA-stored; only 0 and 1 have a conv)", x3);
+  if (x3 < 0 || x3 > 7 || x3 == 3 || x3 == 6 || (x3 >= 2 && conv_B > 0)) {
+    set_error("gemm plan: mode %d (0 tf32, 1 tf32x3, 2 bf16, 4 e4m3, 5 tf32x3 TMA-stored, 7 fp16; only 0 and 1 have a conv)", x3);
     return SIGMA_EINVAL;
   }
   const int rc = plan_gemm(M, N, K, x3 == 1 || x3 == 5, conv_B, conv_H, conv_W, &pl, x3 == 4, x3 == 5);
@@ -1084,14 +1267,17 @@ int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, in
   return SIGMA_OK;
 }
 
-// The launch of the instance for pl.BN.
-template <bool X3, bool CONV, bool BF16 = false, bool TMA_C = false>
+// The launch of the instance for pl.BN (F16: gemm_fp16_kernel).
+template <bool X3, bool CONV, bool BF16 = false, bool TMA_C = false, bool F16 = false>
 static int launch_gemm(GemmParams &p, const GemmPlan &pl, cudaStream_t stream) {
   p.stages = pl.stages;
   const void *kern = nullptr;
   switch (p.BN) {
-#define SIGMA_GEMM_BN(bn) \
-  case bn: kern = TMA_C ? (const void *)gemm_x3_tma_kernel<bn> : (const void *)gemm_tf32_kernel<bn, X3, CONV, BF16>; break;
+#define SIGMA_GEMM_BN(bn)                                                                                                        \
+  case bn:                                                                                                                       \
+    kern = F16 ? (const void *)gemm_fp16_kernel<bn>                                                                              \
+               : TMA_C ? (const void *)gemm_x3_tma_kernel<bn> : (const void *)gemm_tf32_kernel<bn, X3, CONV, BF16>;             \
+    break;
     SIGMA_GEMM_BN(32) SIGMA_GEMM_BN(64) SIGMA_GEMM_BN(96) SIGMA_GEMM_BN(128)
     SIGMA_GEMM_BN(160) SIGMA_GEMM_BN(192) SIGMA_GEMM_BN(224) SIGMA_GEMM_BN(256)
 #undef SIGMA_GEMM_BN
@@ -1135,20 +1321,22 @@ int gemm_tf32_launch(const float *A, long long lda, const float *W, const float 
   return x3 ? launch_gemm<true, false>(p, pl, stream) : launch_gemm<false, false>(p, pl, stream);
 }
 
-// bf16 operands (A (M, K) row stride lda, W (N, K)), fp32 accumulation, C fp32 or (c_bf16) bf16; bias / residual / rscale fp32
-int gemm_bf16_launch(const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
-                     const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N, int K, cudaStream_t stream) {
+// bf16 (dtype SIGMA_BF16) or fp16 (SIGMA_F16) operands (A (M, K) row stride lda, W (N, K)), fp32 accumulation, C fp32 or (c_16)
+// the operands' type; bias / residual / rscale fp32.  Both instances stage the same bytes, so both run the tf32 plan.
+int gemm_16bit_launch(int dtype, const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
+                      const float *rscale, void *C, long long ldc, int c_16, long long M, int N, int K, cudaStream_t stream) {
   if (M == 0) return SIGMA_OK;
   GemmPlan pl;
   int rc;
   if ((rc = plan_gemm(M, N, K, false, 0, 0, 0, &pl))) return rc;
   GemmParams p;
   memset(&p, 0, sizeof(p));
-  p.bias = bias; p.residual = residual; p.rscale = rscale; p.C = (float *)C; p.ldr = ldr; p.ldc = ldc; p.c_bf16 = c_bf16;
+  p.bias = bias; p.residual = residual; p.rscale = rscale; p.C = (float *)C; p.ldr = ldr; p.ldc = ldc; p.c_bf16 = c_16;
   p.M = (int)M; p.N = N; p.K = K;
   p.BN = pl.BN;
-  if ((rc = make_tmap_2d_sw128(&p.m_a, A, M, K, lda, GM_BM, true))) return rc;
-  if ((rc = make_tmap_2d_sw128(&p.m_w, W, N, K, K, p.BN, true))) return rc;
+  if ((rc = make_tmap_2d_sw128(&p.m_a, A, M, K, lda, GM_BM, dtype))) return rc;
+  if ((rc = make_tmap_2d_sw128(&p.m_w, W, N, K, K, p.BN, dtype))) return rc;
+  if (dtype == SIGMA_F16) return launch_gemm<false, false, false, false, true>(p, pl, stream);
   return launch_gemm<false, false, true>(p, pl, stream);
 }
 

@@ -43,6 +43,7 @@ struct RowNormParams {
   // bf16 GEMM); 2 = y, z, out bf16 (merge + out_norm + gate of the bf16 scan output).  Pointers and strides count elements.
   // The FP8 inference mode: 3 = y fp32, out e4m3 (LayerNorm / patch-merge LN feeding sigma_linear_fp8); 4 = y, z bf16, out e4m3
   // (merge + out_norm + gate).  Both write row r's scale to qscale[r].
+  // The fp16 inference mode: 5 = y fp32, out fp16 (as 1); 6 = y, z, out fp16 (as 2).
   int io = 0;
   float *qscale = nullptr;
 };
@@ -70,13 +71,14 @@ int make_tmap(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void 
               const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo);
 int pad_rp(int R);   // dt_rank padded to an instantiated width (4, 8, 12, 16, 24, 32, 48, 64), -1 beyond 64
 size_t ss2d_scan_workspace_bytes(int kind, int batch, int D, int N);
-// xc_bf16 = 1: xc and y are bf16; dsave / hsave (training forward): delta' slabs and block-start states for the backward
-// (both: the bf16 training mode, whose delta' slabs are bf16 too)
+// xc_dtype: element type of xc and y, SIGMA_F32, SIGMA_BF16 or (inference only) SIGMA_F16; dsave / hsave (training forward):
+// delta' slabs and block-start states for the backward (with SIGMA_BF16: the bf16 training mode, whose delta' slabs are bf16 too)
 int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                   const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp, void *ws,
-                  size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave = nullptr, float *hsave = nullptr, int xc_bf16 = 0);
+                  size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave = nullptr, float *hsave = nullptr,
+                  int xc_dtype = SIGMA_F32);
 int ss2d_pick_segments_hook(long long ctas, int nw, int ntiles, int N);
-int ss2d_fwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int R, int xc_bf16, int force_split, size_t ws_bytes,
+int ss2d_fwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int R, int xc_dtype, int force_split, size_t ws_bytes,
                        long long *out8);
 
 // ---- ss2d_scan_bwd.cu ----
@@ -170,8 +172,9 @@ int scale_add_launch(const float *a, const float *sa, const float *b, const floa
 int dwconv3x3_silu_tma_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
                               const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
                               cudaStream_t stream);
-int dwconv3x3_silu_bf16_launch(const void *x, long long x_row_stride, long long x_batch_stride, const float *w, const float *bias,
-                               void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream);
+// dtype: SIGMA_BF16 or SIGMA_F16 x and y
+int dwconv3x3_silu_16bit_launch(int dtype, const void *x, long long x_row_stride, long long x_batch_stride, const float *w,
+                                const float *bias, void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream);
 
 // ---- gemm_tf32.cu ----
 // tf32x3 (W_lo != nullptr) stores its output tiles with TMA; reg_epilogue = true stores them from registers instead (the
@@ -180,8 +183,9 @@ int dwconv3x3_silu_bf16_launch(const void *x, long long x_row_stride, long long 
 int gemm_tf32_launch(const float *A, long long lda, const float *W, const float *W_lo, const float *bias, const float *residual,
                      long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream,
                      bool reg_epilogue = false);
-int gemm_bf16_launch(const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
-                     const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N, int K, cudaStream_t stream);
+// dtype: SIGMA_BF16 or SIGMA_F16 operands; c_16 = 1: C stored in that type (else fp32)
+int gemm_16bit_launch(int dtype, const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
+                      const float *rscale, void *C, long long ldc, int c_16, long long M, int N, int K, cudaStream_t stream);
 int gemm_fp8_launch(const void *A, long long lda, const float *sa, const void *W, const float *sw, const float *bias,
                     const float *residual, long long ldr, const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N,
                     int K, cudaStream_t stream);

@@ -325,8 +325,63 @@ static int row_norm_e4m3_launch(const RowNormParams &p, cudaStream_t stream) {
   return SIGMA_OK;
 }
 
+// The fp16 instances (io 5, 6: the fp16 inference mode): io 1 / 2's kernels with __half for bf16, at the same fast widths and, for
+// other widths, the generic kernel.
+template <int LPR, int V>
+static bool row_norm_fp16_fast_k(const RowNormParams &p, cudaStream_t stream) {
+  using f16 = __half;
+  const int warps = 8, rows_per_cta = warps * (32 / LPR);
+  const unsigned grid = (unsigned)((p.rows + rows_per_cta - 1) / rows_per_cta);
+  if (p.io == 5) {   // LayerNorm / patch-merge LayerNorm with fp16 output
+    if (p.K != 1) return false;
+    if (p.mode == 0) { row_norm_fast_kernel<LPR, V, 1, 0, float, f16><<<grid, warps * 32, 0, stream>>>(p); return true; }
+    if (p.mode == 1) { row_norm_fast_kernel<LPR, V, 1, 1, float, f16><<<grid, warps * 32, 0, stream>>>(p); return true; }
+    return false;
+  }
+  if (p.mode != 0) return false;   // io 6: merge + norm + gate, fp16 in and out
+  switch (p.K) {
+    case 1: row_norm_fast_kernel<LPR, V, 1, 0, f16, f16><<<grid, warps * 32, 0, stream>>>(p); return true;
+    case 2: row_norm_fast_kernel<LPR, V, 2, 0, f16, f16><<<grid, warps * 32, 0, stream>>>(p); return true;
+    case 4: row_norm_fast_kernel<LPR, V, 4, 0, f16, f16><<<grid, warps * 32, 0, stream>>>(p); return true;
+  }
+  return false;
+}
+
+static int row_norm_fp16_launch(const RowNormParams &p, cudaStream_t stream) {
+  const int nvec = p.D >> 2;
+  bool ok = false;
+  if (!((p.D & 3) || (p.k_stride & 3) || (p.in_batch_stride & 3) || (p.out_row_stride & 3) || (p.out_batch_stride & 3) ||
+        (p.z_row_stride & 3))) {
+#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) ok = row_norm_fp16_fast_k<LPR, V>(p, stream)
+    TRY(8, 2); TRY(8, 3); TRY(8, 4);
+    TRY(16, 3); TRY(16, 4);
+    TRY(32, 3); TRY(32, 4); TRY(32, 6); TRY(32, 8); TRY(32, 12); TRY(32, 16);
+#undef TRY
+  }
+  if (!ok) {
+    if (p.mode != 0) { set_error("row_norm: gather / pixel-shuffle modes need D = 4·LPR·V (D=%d has no fast instantiation)", p.D); return SIGMA_EUNSUPPORTED; }
+    const unsigned grid = (unsigned)((p.rows + 7) / 8);
+#define LAUNCH_F16(MV)                                                                                                   \
+    do {                                                                                                                 \
+      if (p.io == 5) row_norm_kernel<MV, float, __half><<<grid, 256, 0, stream>>>(p);                                    \
+      else row_norm_kernel<MV, __half, __half><<<grid, 256, 0, stream>>>(p);                                             \
+    } while (0)
+    if (nvec <= 32) LAUNCH_F16(1);
+    else if (nvec <= 64) LAUNCH_F16(2);
+    else if (nvec <= 128) LAUNCH_F16(4);
+    else if (nvec <= 256) LAUNCH_F16(8);
+    else if (nvec <= 512) LAUNCH_F16(16);
+    else if (nvec <= 1024) LAUNCH_F16(32);
+    else { set_error("row_norm: D=%d > 4096 unsupported", p.D); return SIGMA_EUNSUPPORTED; }
+#undef LAUNCH_F16
+  }
+  SIGMA_CHECK_LAUNCH();
+  return SIGMA_OK;
+}
+
 int row_norm_launch(const RowNormParams &p, cudaStream_t stream) {
   if (p.rows == 0) return SIGMA_OK;
+  if (p.io == 5 || p.io == 6) return row_norm_fp16_launch(p, stream);
   if (p.io >= 3) return row_norm_e4m3_launch(p, stream);
   if (row_norm_fast(p, stream)) {
     SIGMA_CHECK_LAUNCH();

@@ -61,8 +61,8 @@ struct alignas(64) Ss2dParams {
   int nst;     // TMA ring depth: as many LT-position stages as fit next to CTAS-1 other CTAs in shared memory
   int ablate;  // timing experiments, only in builds with -DSIGMA_SCAN_ABLATION (SIGMA_SCAN_ABLATE env):
                // 1 = no y store, 2 = no per-group prologue, 4 = no TMA reload
-  int xc_bf16; // 1: xc and y are bf16; x_dbl, the state and the recurrence stay fp32.  With hsave (the bf16 training mode) the
-               // delta' slabs are bf16 too and the recurrence runs on the rounded delta'
+  int xc_dtype; // SIGMA_BF16 / SIGMA_F16: xc and y are bf16 / fp16; x_dbl, the state and the recurrence stay fp32.  With hsave
+                // (the bf16 training mode, SIGMA_BF16 only) the delta' slabs are bf16 too and the recurrence runs on the rounded delta'
 };
 
 #ifdef SIGMA_SCAN_ABLATION
@@ -71,7 +71,7 @@ struct alignas(64) Ss2dParams {
 #define SIGMA_ABL(flags, m) false
 #endif
 
-// xc_bytes: element size of the staged xc tile (4, or 2 for bf16)
+// xc_bytes: element size of the staged xc tile (4, or 2 for bf16 / fp16)
 __host__ __device__ inline size_t ss2d_smem_bytes(int LT, int DT, int NST, int Cp, bool cross, int xc_bytes = 4) {
   const size_t stage = (size_t)LT * DT * xc_bytes + (size_t)LT * Cp * (cross ? 2 : 1) * sizeof(float);
   return NST * stage + 128 /*barriers + counters*/;
@@ -347,7 +347,7 @@ __device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2d
   }
 }
 
-// XT: element type of xc and y (float; __nv_bfloat16 in the bf16 inference and training modes).
+// XT: element type of xc and y (float; __nv_bfloat16 in the bf16 inference and training modes, __half in the fp16 inference mode).
 // TRAIN16 (the bf16 training mode, XT = __nv_bfloat16): delta' is rounded to bf16 before the recurrence uses it — in the
 // summary pass too, whose carries must describe the same recurrence — and the SAVE passes store that bf16 delta'.
 template <int N, int CPT, int RP, int MODE, bool SAVE, typename XT, bool TRAIN16>

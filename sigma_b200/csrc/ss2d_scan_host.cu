@@ -143,7 +143,7 @@ struct Ss2dFwdPlan {
 };
 
 // have_ws: the caller passed a workspace of at least ss2d_scan_workspace_bytes
-static int ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R, int xc_bf16, int force_split, bool have_ws,
+static int ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R, int xc_dtype, int force_split, bool have_ws,
                          Ss2dFwdPlan &pl) {
   if (N != 4 && N != 8 && N != 16) {
     set_error("sigma_ss2d_scan_fwd: d_state=%d unsupported by the fused kernel (4, 8, 16)", N);
@@ -154,7 +154,7 @@ static int ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R,
     return SIGMA_EUNSUPPORTED;
   }
   const int Cp = 2 * N + pad_rp(R);
-  const int xes = xc_bf16 ? 2 : 4;   // bytes per xc / y element
+  const int xes = xc_dtype == SIGMA_F32 ? 4 : 2;   // bytes per xc / y element
   const int ndir = kind_dirs(kind);
   const long long Lseq = kind == SIGMA_DIRS_SEQ2 ? 2LL * H * W : (long long)H * W;
   const int LT = lt_for(N);
@@ -203,7 +203,7 @@ static int ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R,
   // register budget (ss2d_scan.cuh): which `__launch_bounds__(128, CTAS)` build runs.  SIGMA_SCAN_CTAS overrides.
   int rbud = ss2d_pick_ctas(N, pad_rp(R));
   if (const char *e = getenv("SIGMA_SCAN_CTAS")) rbud = std::max(3, std::min(5, atoi(e)));
-  if (N != 16 || xc_bf16) rbud = 3;   // bf16: only the 3-CTA budget is built (ss2d_scan_inst.inc)
+  if (N != 16 || xc_dtype != SIGMA_F32) rbud = 3;   // bf16 / fp16: only the 3-CTA budget is built (ss2d_scan_inst.inc)
   rbud = std::min(rbud, 4);
   pl.rbud = rbud;
   {
@@ -222,29 +222,32 @@ static int ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R,
   return SIGMA_OK;
 }
 
-int ss2d_fwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int R, int xc_bf16, int force_split, size_t ws_bytes,
+int ss2d_fwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int R, int xc_dtype, int force_split, size_t ws_bytes,
                        long long *out8) {
   Ss2dFwdPlan pl;
   const bool have_ws = ws_bytes > 0 && ws_bytes >= ss2d_scan_workspace_bytes(kind, batch, D, N);
-  const int rc = ss2d_fwd_plan(kind, batch, H, W, D, N, R, xc_bf16, force_split, have_ws, pl);
+  const int rc = ss2d_fwd_plan(kind, batch, H, W, D, N, R, xc_dtype, force_split, have_ws, pl);
   if (rc) return rc;
   const long long v[8] = {pl.nsplit, pl.tiles_per_split, pl.max_tiles, pl.min_tiles, pl.nw, pl.nst, pl.rbud, (long long)pl.smem};
   for (int i = 0; i < 8; ++i) out8[i] = v[i];
   return SIGMA_OK;
 }
 
-// xc_bf16 = 1: xc and y are bf16 (passed through the float pointers); x_dbl, the parameters and the recurrence stay fp32
+// xc_dtype SIGMA_BF16 / SIGMA_F16: xc and y are bf16 / fp16 (passed through the float pointers); x_dbl, the parameters and the
+// recurrence stay fp32
 int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                   const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp, void *ws,
-                  size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave, float *hsave, int xc_bf16) {
+                  size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave, float *hsave, int xc_dtype) {
   Ss2dFwdPlan pl;
-  int rc = ss2d_fwd_plan(kind, batch, H, W, D, N, R, xc_bf16, force_split,
+  int rc = ss2d_fwd_plan(kind, batch, H, W, D, N, R, xc_dtype, force_split,
                          ws != nullptr && ws_bytes >= ss2d_scan_workspace_bytes(kind, batch, D, N), pl);
   if (rc) return rc;
   Ss2dParams p;
   memset(&p, 0, sizeof(p));
-  p.xc_bf16 = xc_bf16;
-  const int xes = xc_bf16 ? 2 : 4;   // bytes per xc / y element
+  p.xc_dtype = xc_dtype;
+  const int xes = xc_dtype == SIGMA_F32 ? 4 : 2;   // bytes per xc / y element
+  const CUtensorMapDataType xdt = xc_dtype == SIGMA_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                  : xc_dtype == SIGMA_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   p.dtw = dtw; p.dtb = dtb; p.A = A; p.Ds = Ds; p.y = y; p.carry = (float *)ws;
   p.D = D; p.N = N; p.R = R; p.Cp = Cp; p.kind = kind; p.batch = batch;
   p.dsave = dsave; p.hsave = hsave; p.save_tiles = hsave ? ss2d_save_tiles(kind, H, W) : 0;
@@ -273,8 +276,8 @@ int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw
       dims[0] = D; dims[1] = H; dims[2] = W; dims[3] = batch;
       str[0] = (uint64_t)W * D * xes; str[1] = (uint64_t)D * xes; str[2] = (uint64_t)Lseq * D * xes;
     }
-    if ((rc = make_tmap(&p.m_xc[k], xc_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, xc, dims, str, box,
-                        CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
+    if ((rc = make_tmap(&p.m_xc[k], xdt, 4, xc, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B)))
+      return rc;
     // x_dbl (batch, Lseq, K, Cp): direction k's row starts at column k·Cp
     uint32_t boxd[4] = {(uint32_t)Cp, (uint32_t)LT, 1, 1};
     dims[0] = Cp;

@@ -22,6 +22,11 @@ and the PatchMerging2D reduction on e4m3 operands (sigma_linear_fp8): activation
 per output channel (the formula in include/sigma_b200.h).  The LayerNorms in front of in_proj, the patch-merge LayerNorm and
 SS2D's / CroMB's merge + norm + gate emit the e4m3 rows and scales themselves; ConMB's and CroMB's in_proj operands and ConMB's
 two-part ycat go through the standalone row quantizer.  x_proj stays bf16 (it feeds softplus and exp).
+
+The fp16 mode (`precision() == "fp16"`, selected by `fp16_inference()` with autograd off, autocast or not) stores exactly what
+the bf16 mode stores, in fp16 instead of bf16, and runs the same GEMMs on fp16 operands (sigma_linear_fp16).  fp16 keeps 11
+significant bits where bf16 keeps 8, but its range ends at ±65504: a stored value past it becomes ±inf, as torch's .half() does
+(there is no saturating conversion).  torch.autocast with fp16 is not this mode: it keeps the fp32 path.
 """
 import contextlib
 import ctypes
@@ -62,9 +67,14 @@ def quantize_rows(x2d, out=None):
     return out
 
 
+def _entry(fn, dtype):
+    """the entry point of `fn` for an element type: fp32 `fn`, bf16 `fn`_bf16, fp16 `fn`_fp16"""
+    return fn + {torch.bfloat16: "_bf16", torch.float16: "_fp16"}.get(dtype, "")
+
+
 def layernorm(x2d, ln, dtype=torch.float32):
-    """nn.LayerNorm over the last dim of a contiguous (rows, C) fp32 tensor; dtype=torch.bfloat16 stores the output as bf16,
-    dtype=torch.float8_e4m3fn returns E4M3Rows (sigma_layernorm_fwd_fp8: the fp32 result quantized per row)."""
+    """nn.LayerNorm over the last dim of a contiguous (rows, C) fp32 tensor; dtype=torch.bfloat16 / torch.float16 stores the
+    output as bf16 / fp16, dtype=torch.float8_e4m3fn returns E4M3Rows (sigma_layernorm_fwd_fp8: the fp32 result quantized per row)."""
     rows, C = x2d.shape
     if dtype == torch.float8_e4m3fn:
         y = _e4m3_empty(rows, C, x2d.device)
@@ -72,7 +82,7 @@ def layernorm(x2d, ln, dtype=torch.float32):
                                                       stream()), "sigma_layernorm_fwd_fp8")
         return y
     y = torch.empty((rows, C), dtype=dtype, device=x2d.device)
-    fn = "sigma_layernorm_fwd_bf16" if dtype == torch.bfloat16 else "sigma_layernorm_fwd"
+    fn = _entry("sigma_layernorm_fwd", dtype)
     _lib.check(getattr(_lib.lib(), fn)(ptr(x2d), ptr(ln.weight), ptr(ln.bias), ptr(y), rows, C, float(ln.eps), stream()), fn)
     return y
 
@@ -81,6 +91,7 @@ USE_OWN_GEMM = True  # False: cuBLAS through torch (library GEMM, precision by t
 
 
 FP8_INFERENCE = False
+FP16_INFERENCE = False
 
 
 @contextlib.contextmanager
@@ -94,14 +105,29 @@ def fp8_inference(on=True):
         FP8_INFERENCE = prev
 
 
+@contextlib.contextmanager
+def fp16_inference(on=True):
+    """Switch the fp16 inference mode of the fused path on (or off) inside the block: with autograd off, precision() is "fp16"
+    (module docstring; values past ±65504 become ±inf where the mode stores fp16)."""
+    global FP16_INFERENCE
+    prev, FP16_INFERENCE = FP16_INFERENCE, bool(on)
+    try:
+        yield
+    finally:
+        FP16_INFERENCE = prev
+
+
 def precision():
     """Precision of the fused path.  Inside fp8_inference() with autograd off it is "fp8": the bf16 mode's storage, with the
     in_proj / out_proj / PatchMerging GEMMs on e4m3 operands scaled per row and per output channel (module docstring); logits
     within 2x the error of the reference's layers under bf16 autocast with the same e4m3 quantize-dequantize at those GEMMs.
     With autograd off and torch.autocast("cuda", dtype=torch.bfloat16) active it is "bf16": the
     SS2D / ConMB / CroMB / PatchMerging interiors store bf16 and their GEMMs run bf16 wgmma (module docstring); logits within
-    2x the error of the reference's own layers under the same autocast.  Autocast with fp16 is not a mode of the fused path: it
-    keeps the fp32 modes below.  With autograd on (training) autocast does not change the fused core either.
+    2x the error of the reference's own layers under the same autocast.  Inside fp16_inference() with autograd off it is "fp16",
+    with or without autocast: the bf16 mode's storage and GEMMs in fp16 (11 significant bits, range ±65504); logits within 2x the
+    error of the reference's layers under fp16 autocast.  fp16_inference() and fp8_inference() together are a ValueError.
+    torch.autocast with fp16 is not a mode of the fused path: it keeps the fp32 modes below.  With autograd on (training) neither
+    autocast nor the contexts change the fused core.
     Otherwise the dense-projection precision (the scan, LayerNorms and the convolutions' accumulation are fp32 regardless)
     follows torch's own switch, exactly like the reference's nn.Linear layers do:
       torch.backends.cuda.matmul.allow_tf32 = False (torch's default) -> "tf32x3": fp32-GRADE products on the tensor cores — the
@@ -109,8 +135,12 @@ def precision():
           with the reference's fp32 results to ~1e-6 of their scale (1e-3 bar);
       torch.backends.cuda.matmul.allow_tf32 = True -> "tf32": the same kernel, one TF32 MMA per k-step (10-bit mantissa
           operands, fp32 accumulate in registers); logits within ~3e-3 of the reference's (1e-2 bar)."""
+    if not torch.is_grad_enabled() and FP8_INFERENCE and FP16_INFERENCE:
+        raise ValueError("fused.precision(): fp8_inference() and fp16_inference() are both on; choose one")
     if not torch.is_grad_enabled() and FP8_INFERENCE:
         return "fp8"
+    if not torch.is_grad_enabled() and FP16_INFERENCE:
+        return "fp16"
     if not torch.is_grad_enabled() and torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16:
         return "bf16"
     return _dense_precision()
@@ -128,18 +158,14 @@ def logits_bar(composed_err=None):
     bf16 has no fixed bar: it is 2 x `composed_err` + BF16_FLOOR, where `composed_err` is the error (same fraction of the
     scale) of the reference's op composition (modules.composed_path()) on the same inputs under the same autocast — so the
     caller measures it first (tests/test_bf16_gpu.py).  fp8 likewise, with the composed path run under bf16 autocast and the
-    mode's e4m3 quantize-dequantize at the GEMMs it quantizes (tests/test_fp8_gpu.py)."""
+    mode's e4m3 quantize-dequantize at the GEMMs it quantizes (tests/test_fp8_gpu.py); fp16 with the composed path under fp16
+    autocast (tests/test_fp16_gpu.py)."""
     mode = precision()
-    if mode in ("bf16", "fp8"):
+    if mode in ("bf16", "fp8", "fp16"):
         if composed_err is None:
             raise ValueError(f"logits_bar(): the {mode} bar is relative; pass the composed path's error under the same autocast")
         return 2.0 * composed_err + BF16_FLOOR
     return 1e-2 if mode == "tf32" else 1e-3
-
-
-def _bf16_mode():
-    """bf16 interior storage: the bf16 and the FP8 modes"""
-    return precision() in ("bf16", "fp8")
 
 
 def _fp8_mode():
@@ -153,8 +179,8 @@ def _no_autocast():
 
 _FP32_KINDS = set()   # experiment hook (scripts/tf32_error_budget.py): kinds of projections forced to full precision in tf32 mode
 _SPLIT = {}           # id(weight) -> (weakref, version, W_hi, W_lo): the tf32x3 operand split of a weight, made once per version
-_LOWP = {}            # id(weight) -> (weakref, version, {form: copy}): the bf16 copy ("bf16") and the per-channel e4m3 rows
-                      # and scales ("e4m3") of a weight, each made once per version
+_LOWP = {}            # id(weight) -> (weakref, version, {form: copy}): the bf16 / fp16 copies ("bf16", "fp16") and the
+                      # per-channel e4m3 rows and scales ("e4m3") of a weight, each made once per version
 
 
 def _split_weight(w):
@@ -179,12 +205,19 @@ def _lowp_weight(w, form):
     forms = ent[2]
     if form not in forms:
         wc = w.detach().contiguous()
-        forms[form] = wc.to(torch.bfloat16) if form == "bf16" else quantize_rows(wc.float() if wc.dtype != torch.float32 else wc)
+        if form == "e4m3":
+            forms[form] = quantize_rows(wc.float() if wc.dtype != torch.float32 else wc)
+        else:
+            forms[form] = wc.to(torch.bfloat16 if form == "bf16" else torch.float16)
     return forms[form]
 
 
 def _bf16_weight(w):
     return _lowp_weight(w, "bf16")
+
+
+def _fp16_weight(w):
+    return _lowp_weight(w, "fp16")
 
 
 def _e4m3_weight(w):
@@ -203,7 +236,8 @@ def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="d
 
     A bf16 x2d runs the bf16 instance (sigma_linear_bf16: bf16 operands, fp32 accumulation) whatever `precision()` says, with a
     bf16 copy of the weight cached on `_version` exactly like the tf32x3 split (same `.data` limitation); the output is fp32 or
-    (out_dtype=torch.bfloat16) bf16.  Rows whose byte stride is not a multiple of 16 go to torch.mm.
+    (out_dtype=torch.bfloat16) bf16.  Rows whose byte stride is not a multiple of 16 go to torch.mm.  An fp16 x2d likewise runs the
+    fp16 instance (sigma_linear_fp16) with a cached fp16 copy of the weight; its output is fp32 or (out_dtype=torch.float16) fp16.
 
     An E4M3Rows x2d runs the e4m3 instance (sigma_linear_fp8) with the weight's per-channel e4m3 rows, cached the same way; K and
     the row stride must be multiples of 16 and N of 4 (there is no other path for it)."""
@@ -211,8 +245,8 @@ def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="d
         return _linear_fp8(x2d, weight, bias, out, residual, rscale, out_dtype)
     M, K = x2d.shape
     N = weight.shape[0]
-    if x2d.dtype == torch.bfloat16:
-        return _linear_bf16(x2d, weight, bias, out, residual, rscale, out_dtype)
+    if x2d.dtype in (torch.bfloat16, torch.float16):
+        return _linear_16bit(x2d, weight, bias, out, residual, rscale, out_dtype)
     if out is None:
         out = torch.empty((M, N), dtype=torch.float32, device=x2d.device)
     if not USE_OWN_GEMM or K % 4 or x2d.stride(1) != 1 or x2d.stride(0) % 4 or N % 4:
@@ -237,15 +271,17 @@ def linear(x2d, weight, bias=None, out=None, residual=None, rscale=None, kind="d
     return out
 
 
-def _linear_bf16(x2d, weight, bias, out, residual, rscale, out_dtype):
+def _linear_16bit(x2d, weight, bias, out, residual, rscale, out_dtype):
+    """the bf16 or fp16 instance, by the dtype of x2d"""
     M, K = x2d.shape
     N = weight.shape[0]
+    f16 = x2d.dtype == torch.float16
     if out is None:
         out = torch.empty((M, N), dtype=out_dtype, device=x2d.device)
-    w = _bf16_weight(weight)
+    w = _fp16_weight(weight) if f16 else _bf16_weight(weight)
     if not USE_OWN_GEMM or K % 8 or x2d.stride(1) != 1 or x2d.stride(0) % 8 or N % 4 or out.stride(0) % 4:
         with _no_autocast():
-            t = torch.mm(x2d.float(), w.float().t())              # bf16 values are exact in fp32 (and in TF32)
+            t = torch.mm(x2d.float(), w.float().t())              # bf16 / fp16 values are exact in fp32
             if bias is not None:
                 t += bias
             if residual is not None:
@@ -253,10 +289,11 @@ def _linear_bf16(x2d, weight, bias, out, residual, rscale, out_dtype):
             out.copy_(t)
         return out
     ldr = residual.stride(0) if residual is not None else 0
-    c_dtype = _lib.BF16 if out.dtype == torch.bfloat16 else _lib.F32
-    rc = _lib.lib().sigma_linear_bf16(ptr(x2d), x2d.stride(0), ptr(w), ptr(bias), ptr(residual), ldr, ptr(rscale), ptr(out), out.stride(0),
-                                      c_dtype, M, N, K, stream())
-    _lib.check(rc, "sigma_linear_bf16")
+    c_dtype = {torch.bfloat16: _lib.BF16, torch.float16: _lib.F16}.get(out.dtype, _lib.F32)
+    fn = "sigma_linear_fp16" if f16 else "sigma_linear_bf16"
+    rc = getattr(_lib.lib(), fn)(ptr(x2d), x2d.stride(0), ptr(w), ptr(bias), ptr(residual), ldr, ptr(rscale), ptr(out), out.stride(0),
+                                 c_dtype, M, N, K, stream())
+    _lib.check(rc, fn)
     return out
 
 
@@ -323,8 +360,8 @@ def conv3x3(x, conv, gelu=False):
 
 
 def dwconv3x3_silu(x, x_row_stride, x_batch_stride, conv, out, out_batch_stride, batch, H, W, D):
-    """x and out both fp32, or both bf16 (sigma_dwconv3x3_silu_fwd_bf16)."""
-    fn = "sigma_dwconv3x3_silu_fwd_bf16" if x.dtype == torch.bfloat16 else "sigma_dwconv3x3_silu_fwd"
+    """x and out both fp32, both bf16 (sigma_dwconv3x3_silu_fwd_bf16) or both fp16 (sigma_dwconv3x3_silu_fwd_fp16)."""
+    fn = _entry("sigma_dwconv3x3_silu_fwd", x.dtype)
     _lib.check(getattr(_lib.lib(), fn)(ptr(x), x_row_stride, x_batch_stride, ptr(conv.weight), ptr(conv.bias),
                                        ptr(out), out_batch_stride, batch, H, W, D, stream()), fn)
     return out
@@ -334,13 +371,14 @@ def ss2d_scan(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
     L_ = _lib.lib()
     ndir = {_lib.DIRS_CROSS4: 4, _lib.DIRS_SEQ2: 2, _lib.DIRS_CROSS: 1}[kind]
     Lseq = 2 * H * W if kind == _lib.DIRS_SEQ2 else H * W
-    y = torch.empty((ndir, batch, Lseq, D), dtype=xc.dtype, device=xc.device)      # bf16 xc -> bf16 y
+    y = torch.empty((ndir, batch, Lseq, D), dtype=xc.dtype, device=xc.device)      # bf16 / fp16 xc -> bf16 / fp16 y
     wsb = L_.sigma_ss2d_scan_workspace_bytes(kind, batch, H, W, D, N)
     ws = torch.empty(wsb, dtype=torch.uint8, device=xc.device)
-    if xc.dtype == torch.bfloat16:
-        rc = L_.sigma_ss2d_scan_fwd_bf16(kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(y), batch, H, W, D, N, R, Cp,
-                                         ptr(ws), wsb, stream())
-        _lib.check(rc, "sigma_ss2d_scan_fwd_bf16")
+    if xc.dtype in (torch.bfloat16, torch.float16):
+        fn = _entry("sigma_ss2d_scan_fwd", xc.dtype)
+        rc = getattr(L_, fn)(kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(y), batch, H, W, D, N, R, Cp,
+                             ptr(ws), wsb, stream())
+        _lib.check(rc, fn)
         return y
     if _FORCE_SPLIT:
         rc = L_.sigma_ss2d_scan_fwd_split(kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(y), batch, H, W, D, N,
@@ -373,7 +411,8 @@ def ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
 
 def merge_norm_gate(y, K, k_stride, in_batch_stride, ln, z, z_row_stride, gate, out, out_batch_stride, out_row_stride,
                     rows, rows_per_batch, D, y_offset=0, out_offset=0):
-    """y, z and out all fp32, or all bf16 (sigma_merge_norm_gate_fwd_bf16); offsets and strides count elements.  out = E4M3Rows
+    """y, z and out all fp32, all bf16 (sigma_merge_norm_gate_fwd_bf16) or all fp16 (sigma_merge_norm_gate_fwd_fp16); offsets
+    and strides count elements.  out = E4M3Rows
     (y, z bf16): sigma_merge_norm_gate_fwd_fp8, whose row r's scale lands at out.s[out_offset / out_row_stride + r]."""
     yp = ctypes.c_void_p(y.data_ptr() + y.element_size() * y_offset)
     if isinstance(out, E4M3Rows):
@@ -384,7 +423,7 @@ def merge_norm_gate(y, K, k_stride, in_batch_stride, ln, z, z_row_stride, gate, 
                                                       float(ln.eps), stream())
         _lib.check(rc, "sigma_merge_norm_gate_fwd_fp8")
         return out
-    fn = "sigma_merge_norm_gate_fwd_bf16" if y.dtype == torch.bfloat16 else "sigma_merge_norm_gate_fwd"
+    fn = _entry("sigma_merge_norm_gate_fwd", y.dtype)
     op = ctypes.c_void_p(out.data_ptr() + out.element_size() * out_offset)
     rc = getattr(_lib.lib(), fn)(yp, K, k_stride, in_batch_stride, ptr(ln.weight), ptr(ln.bias), z, z_row_stride,
                                  ptr(gate), op, out_batch_stride, out_row_stride, rows, rows_per_batch, D, float(ln.eps), stream())
@@ -446,7 +485,7 @@ def _cma_params(cm):
 def ss2d(m, x, residual=None, rscale=None):
     """SS2D.forward (vmamba.py:1067-1089); x (B,H,W,C) contiguous.  Returns (B,H,W,C) [+ residual (· rscale)], the
     residual being added in the out_proj GEMM epilogue."""
-    dt = torch.bfloat16 if _bf16_mode() else torch.float32     # storage of the block's interior (module docstring)
+    dt = _interior_dtype()                                      # storage of the block's interior (module docstring)
     fp8 = _fp8_mode()
     if isinstance(x, E4M3Rows):                                 # the FP8 mode's LayerNorm output (vss_block, cvss_decoder_block)
         B, H, W, C = x.q.shape
@@ -471,7 +510,8 @@ def ss2d(m, x, residual=None, rscale=None):
 
 
 def _interior_dtype():
-    return torch.bfloat16 if _bf16_mode() else torch.float32
+    mode = precision()
+    return torch.bfloat16 if mode in ("bf16", "fp8") else torch.float16 if mode == "fp16" else torch.float32
 
 
 def _ln_out_dtype():
@@ -492,15 +532,15 @@ def patch_merging(m, x):
     x = x.contiguous()
     B, H, W, C = x.shape
     H2, W2 = (H + 1) // 2, (W + 1) // 2
-    bf16 = _bf16_mode()
     if _fp8_mode():                                                  # the same kernel, quantizing its rows
         xq = _e4m3_empty(B * H2 * W2, 4 * C, x.device)
         _lib.check(_lib.lib().sigma_patch_merge_norm_fwd_fp8(ptr(x), ptr(m.norm.weight), ptr(m.norm.bias), ptr(xq.q), ptr(xq.s), B, H, W, C,
                                                              float(m.norm.eps), stream()), "sigma_patch_merge_norm_fwd_fp8")
         return linear(xq, m.reduction.weight).view(B, H2, W2, -1)
-    xn = torch.empty((B * H2 * W2, 4 * C), dtype=torch.bfloat16 if bf16 else torch.float32, device=x.device)
+    dt = _interior_dtype()
+    xn = torch.empty((B * H2 * W2, 4 * C), dtype=dt, device=x.device)
     # 2x2 gather (+ zero padding of odd sizes) + LayerNorm(4C) in one kernel: no concatenated tensor
-    fn = "sigma_patch_merge_norm_fwd_bf16" if bf16 else "sigma_patch_merge_norm_fwd"
+    fn = _entry("sigma_patch_merge_norm_fwd", dt)
     _lib.check(getattr(_lib.lib(), fn)(ptr(x), ptr(m.norm.weight), ptr(m.norm.bias), ptr(xn), B, H, W, C, float(m.norm.eps), stream()), fn)
     return linear(xn, m.reduction.weight).view(B, H2, W2, -1)
 

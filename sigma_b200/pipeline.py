@@ -33,12 +33,17 @@ class InferencePipeline:
     amp_dtype=torch.bfloat16 runs the forward (warm-up, capture and any re-capture) under torch.autocast("cuda", dtype=amp_dtype),
     so the captured graph is the one of the fused path's bf16 mode (sigma_b200.fused.precision); None runs it as called.
     fp8=True runs them inside sigma_b200.fused.fp8_inference(), so the graph is the one of the FP8 mode (the per-channel e4m3
-    weights it reads are re-quantized, like the packed SSM tensors, when a re-capture follows a weight change)."""
+    weights it reads are re-quantized, like the packed SSM tensors, when a re-capture follows a weight change).  fp16=True runs
+    them inside sigma_b200.fused.fp16_inference() (the fp16 mode; its fp16 weight copies are refreshed the same way); fp8 and fp16
+    together are a ValueError."""
 
-    def __init__(self, model, batch, height, width, use_graph=True, amp_dtype=None, fp8=False):
+    def __init__(self, model, batch, height, width, use_graph=True, amp_dtype=None, fp8=False, fp16=False):
+        if fp8 and fp16:
+            raise ValueError("sigma_b200.InferencePipeline: fp8=True and fp16=True select two modes; choose one")
         self.model = model
         self.amp_dtype = amp_dtype
         self.fp8 = fp8
+        self.fp16 = fp16
         p = next(model.parameters())
         if p.device.type != "cuda":
             raise RuntimeError("sigma_b200.InferencePipeline needs the model on a CUDA device (there is no CPU path)")
@@ -67,13 +72,15 @@ class InferencePipeline:
         return sum(p._version for p in self.model.parameters())
 
     def _autocast(self):
-        """the forward's precision context: autocast (amp_dtype) and / or the FP8 mode"""
+        """the forward's precision context: autocast (amp_dtype) and / or the FP8 or fp16 mode"""
         from . import fused
         stack = contextlib.ExitStack()
         if self.amp_dtype is not None:
             stack.enter_context(torch.autocast("cuda", dtype=self.amp_dtype))
         if self.fp8:
             stack.enter_context(fused.fp8_inference())
+        if self.fp16:
+            stack.enter_context(fused.fp16_inference())
         return stack
 
     def _capture(self):
