@@ -193,6 +193,21 @@ int sigma_ss2d_scan_bwd_saved_bf16(int kind, const void *xc, const float *xdbl, 
                                    float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                                    size_t workspace_bytes, int nsplit, void *stream);
 
+/* fp16 training mode of the pair (fp16 autocast with a loss scaler such as torch.amp.GradScaler): the _bf16 pair's arguments,
+ * validation, workspace / hs queries, kinds and d_state set, with xc, y, delta and dy in fp16.  Every fp16 store rounds once to
+ * nearest even and nothing saturates: a value past ±65504 is stored as ±inf, as torch's .half() does, and an inf or NaN in xc or
+ * dy reaches the outputs (a loss scaler needs to see it to skip the step).  delta is rounded to fp16 before the forward's
+ * recurrence uses it, in the summary pass of an L-segmented walk too; a delta below 2^-14 is stored subnormal and the recurrence
+ * runs on that same value, so the backward recomputes exp(delta·A) from exactly what the forward used.  dxc and every other
+ * backward output are fp32 (the caller rounds dxc once).  No deterministic build. */
+int sigma_ss2d_scan_fwd_save_fp16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                  const float *Ds, void *y, void *delta, float *hs, int batch, int H, int W, int D, int N, int R, int Cp,
+                                  void *workspace, size_t workspace_bytes, int nsplit, void *stream);
+int sigma_ss2d_scan_bwd_saved_fp16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                   const float *Ds, const void *dy, const void *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl,
+                                   float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                                   size_t workspace_bytes, int nsplit, void *stream);
+
 /* Deterministic build of the fused backward (after sigma_ss2d_scan_fwd_save): the same outputs, bitwise
  * reproducible for the same inputs, GPU model and L-segment plan.  Each direction's du goes to a slab summed over k into dxc,
  * dB / dC are kept per warp channel tile and dA / dDs / ddtb per (image, L-segment), all in the workspace, then summed in a
@@ -217,6 +232,8 @@ int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, voi
 int sigma_layernorm_fwd_fp16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream);
 /* bf16 training mode: x and y both bf16 (8-byte aligned rows), fp32 statistics, w and b. */
 int sigma_layernorm_fwd_bf16io(const void *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream);
+/* fp16 training mode: x and y both fp16 (8-byte aligned rows), fp32 statistics, w and b; y rounds once, past ±65504 to ±inf. */
+int sigma_layernorm_fwd_fp16io(const void *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream);
 
 /* Backward of sigma_layernorm_fwd (training path; the reference's autograd of nn.LayerNorm): dx (rows, C); dw (C) = sum over rows
  * of dy·xhat, db (C) = sum over rows of dy — both zeroed inside, then accumulated.  mean / rstd are recomputed from x.
@@ -226,6 +243,10 @@ int sigma_layernorm_bwd(const float *x, const float *dy, const float *w, float *
 /* The same with bf16 x, dy and dx (8-byte aligned rows; the backward of sigma_layernorm_fwd_bf16io): statistics, dw and db fp32.
  * No deterministic build. */
 int sigma_layernorm_bwd_bf16(const void *x, const void *dy, const float *w, void *dx, float *dw, float *db, int64_t rows, int C,
+                             float eps, void *stream);
+/* The same with fp16 x, dy and dx (the backward of sigma_layernorm_fwd_fp16io): dx rounds once, past ±65504 to ±inf, and an inf or
+ * NaN in x or dy reaches dx, dw and db.  No deterministic build. */
+int sigma_layernorm_bwd_fp16(const void *x, const void *dy, const float *w, void *dx, float *dw, float *db, int64_t rows, int C,
                              float eps, void *stream);
 /* Deterministic build: dw / db kept per warp in the (16-byte aligned) workspace and summed in warp order; no float atomics. */
 size_t sigma_layernorm_bwd_det_workspace_bytes(int64_t rows, int C);
@@ -405,12 +426,13 @@ int sigma_test_linear_tf32x3_regs(const float *A, int64_t lda, const float *W_hi
  * that nsplit (0: the library's choice) would launch for kind CROSS4 / SEQ2 / CROSS (even
  * batch) at (batch, H, W, D, N).  out4_host = {segments, 16-position tiles per segment, tiles of the longest direction's walk, tiles of the shortest}.  The
  * directions share the tiles per segment, so a walk shorter than the longest can end in empty segments.  The plan does not depend
- * on the element type: sigma_ss2d_scan_bwd_saved_bf16 launches the same segments.  For tests and tuning. */
+ * on the element type: sigma_ss2d_scan_bwd_saved_bf16 / _fp16 launch the same segments.  For tests and tuning. */
 int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, int nsplit, int64_t *out4_host);
 
 /* Launch plan of the fused scan forward, host only (no CUDA call, works without a GPU): what sigma_ss2d_scan_fwd (force_split = 0),
  * sigma_ss2d_scan_fwd_split (force_split > 0) or, with bf16 = 1, sigma_ss2d_scan_fwd_bf16 (bf16 = 2: sigma_ss2d_scan_fwd_save_bf16
- * with nsplit = force_split; d_state 8 is SIGMA_EUNSUPPORTED there; bf16 = 3: sigma_ss2d_scan_fwd_fp16) would launch for any kind at (batch, H,
+ * with nsplit = force_split; d_state 8 is SIGMA_EUNSUPPORTED there; bf16 = 3: sigma_ss2d_scan_fwd_fp16; bf16 = 4:
+ * sigma_ss2d_scan_fwd_save_fp16, whose plan is that of bf16 = 2 and which refuses d_state 8 as well) would launch for any kind at (batch, H,
  * W, D, N, R) given a workspace of workspace_bytes (0: none), under the current environment (SIGMA_SCAN_WARPS, SIGMA_SCAN_NST,
  * SIGMA_SCAN_CTAS, SIGMA_SCAN_SPLIT_RULE).  out8_host = {segments, LT-position tiles per segment, tiles of the longest direction's
  * walk, tiles of the shortest, warps per CTA, TMA ring depth, register budget (the CTAs per SM the kernel build assumes: 3 or 4),

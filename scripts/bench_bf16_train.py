@@ -1,12 +1,14 @@
 """Measure the bf16 training mode of the fused core (ops.BF16_TRAINING_CORE) against the default under bf16 autocast, in one process,
 alternating the two after warming both up: median and spread of `--rounds` rounds of `--steps` steps, timed with CUDA events.
+With --amp fp16, the fp16 training mode (ops.FP16_TRAINING_CORE) against the default under fp16 autocast, both arms stepping through
+a torch.amp.GradScaler (fp16 autocast's usual recipe).
 
-    python scripts/bench_bf16_train.py [--out DIR] [--rounds 5] [--steps 10] [--models sigma_small,sigma_tiny] [--profile]
+    python scripts/bench_bf16_train.py [--amp bf16|fp16] [--out DIR] [--rounds 5] [--steps 10] [--models sigma_small,sigma_tiny] [--profile]
 
 * whole training step (forward + backward + AdamW) at 480 x 640, batch 2: step time, peak memory (torch.cuda.max_memory_allocated)
   and the loss of both modes on the same seeded batch;
-* per call at the four stage shapes of Sigma-tiny (SS2D, d_state 16): the core's forward-save and backward, fp32 and bf16, with the
-  ALGORITHMIC bytes computed from the shapes below and the GB/s that follow from them (not a measured memory traffic);
+* per call at the four stage shapes of Sigma-tiny (SS2D, d_state 16): the core's forward-save and backward, fp32 and bf16 (fp16
+  with --amp fp16), with the ALGORITHMIC bytes computed from the shapes below and the GB/s that follow from them (not a measured memory traffic);
 * the card's name and power limit, queried in the same run (nothing is set);
 * --profile: a separate torch.profiler pass of one step per mode, top kernels by time, written under --out.
 Needs a GPU: there is no CPU fallback."""
@@ -27,7 +29,7 @@ STAGES = [(120, 160, 192, 6), (60, 80, 384, 12), (30, 40, 768, 24), (15, 20, 153
 
 def core_bytes(B, H, W, D, N, R, Cp, K, bf16):
     """algorithmic bytes of one forward-save and one backward of the core (kind CROSS4): every tensor once per direction that
-    reads or writes it.  e = bytes of an xc / y / delta' / dy element."""
+    reads or writes it.  e = bytes of an xc / y / delta' / dy element (bf16: any 16-bit element type)."""
     e = 2 if bf16 else 4
     pos = B * H * W
     hs = K * B * -(-H * W // 16) * D * N * 4                      # one state per 16-position block and direction (upper bound: row tiles)
@@ -69,7 +71,11 @@ def bench_steps(a, backbone, out):
     rgb = torch.randn(2, 3, 480, 640, device="cuda", generator=g)
     mx = torch.randn(2, 3, 480, 640, device="cuda", generator=g)
     gt = torch.randint(0, 40, (2, 480, 640), device="cuda", generator=g)
-    steps = {on: train_util.TrainStep(model, opt, amp_dtype=torch.bfloat16, bf16_core=on) for on in (False, True)}
+    if a.amp == "fp16":
+        steps = {on: train_util.TrainStep(model, opt, amp_dtype=torch.float16, fp16_core=on, scaler=torch.amp.GradScaler("cuda"))
+                 for on in (False, True)}
+    else:
+        steps = {on: train_util.TrainStep(model, opt, amp_dtype=torch.bfloat16, bf16_core=on) for on in (False, True)}
     state = {k: v.clone() for k, v in model.state_dict().items()}
     res = {}
     for on in (False, True):      # the loss of both modes from the same weights on the same batch, and their peak memory
@@ -91,11 +97,11 @@ def bench_steps(a, backbone, out):
             with profile(activities=[ProfilerActivity.CUDA]) as prof:
                 steps[on](rgb, mx, gt)
                 torch.cuda.synchronize()
-            with open(os.path.join(out, f"profile_{backbone}_{'bf16core' if on else 'default'}.txt"), "w") as f:
+            with open(os.path.join(out, f"profile_{backbone}_{a.amp + 'core' if on else 'default'}.txt"), "w") as f:
                 f.write(prof.key_averages().table(sort_by="cuda_time_total", row_limit=30, max_name_column_width=90))
     del model, opt, steps
     torch.cuda.empty_cache()
-    return {"default": res[False], "bf16_core": res[True]}
+    return {"default": res[False], f"{a.amp}_core": res[True]}
 
 
 def bench_calls(a):
@@ -119,11 +125,11 @@ def bench_calls(a):
         outs = (f32(B, H * W, D), f32(K, B, H * W, D), f32(B * H * W, K, Cp), f32(K * D, N), f32(K * D), f32(K, D))
         row = {"stage": f"{H}x{W} D{D} R{R}"}
         for bf16 in (False, True):
-            dt = torch.bfloat16 if bf16 else torch.float32
+            dt = (torch.float16 if a.amp == "fp16" else torch.bfloat16) if bf16 else torch.float32
             xc, dy = rn(B, H * W, D).to(dt), rn(B, H * W, D).to(dt)
             y, delta, hs = fused.ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Ds, B, H, W, D, N, R, Cp)
             fwd = lambda: fused.ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Ds, B, H, W, D, N, R, Cp)
-            fn = L_.sigma_ss2d_scan_bwd_saved_bf16 if bf16 else L_.sigma_ss2d_scan_bwd_saved
+            fn = getattr(L_, f"sigma_ss2d_scan_bwd_saved_{a.amp}") if bf16 else L_.sigma_ss2d_scan_bwd_saved
             bwd = lambda: _lib.check(fn(kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(dy), ptr(delta), ptr(hs),
                                         *(ptr(o) for o in outs), B, H, W, D, N, R, Cp, ptr(ws), wsb, 0, stream()), "bwd")
             fb, bb = core_bytes(B, H, W, D, N, R, Cp, K, bf16)
@@ -131,13 +137,14 @@ def bench_calls(a):
                 timed(call, 5)
                 t = [timed(call, max(a.steps, 20)) for _ in range(a.rounds)]
                 m = statistics.median(t)
-                row[f"{name}_{'bf16' if bf16 else 'f32'}"] = {**med(t), "algorithmic_MB": round(nb / 1e6, 1), "algorithmic_GBps": round(nb / m / 1e6, 1)}
+                row[f"{name}_{a.amp if bf16 else 'f32'}"] = {**med(t), "algorithmic_MB": round(nb / 1e6, 1), "algorithmic_GBps": round(nb / m / 1e6, 1)}
         rows.append(row)
     return rows
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--amp", choices=("bf16", "fp16"), default="bf16", help="autocast dtype, and the 16-bit training mode compared")
     ap.add_argument("--out", default=None, help="directory for the JSON result and the profiles (default: a temporary directory)")
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--steps", type=int, default=10)
@@ -161,9 +168,11 @@ def main():
     torch.backends.cuda.matmul.allow_tf32 = True
     torch.backends.cudnn.allow_tf32 = True
     res = {"card": card(), "rounds": a.rounds, "steps_per_round": a.steps, "calls": bench_calls(a), "steps": {}}
+    if a.amp == "fp16":
+        res["amp"] = "fp16 autocast, GradScaler in both arms"
     for m in [m for m in a.models.split(",") if m]:
         res["steps"][m] = bench_steps(a, m, out)
-    with open(os.path.join(out, "bench_bf16_train.json"), "w") as f:
+    with open(os.path.join(out, "bench_bf16_train.json" if a.amp == "bf16" else "bench_fp16_train.json"), "w") as f:
         json.dump(res, f, indent=1)
     print(json.dumps(res))
 

@@ -425,7 +425,25 @@ int sigma_layernorm_bwd_bf16(const void *x, const void *dy, const float *w, void
   SIGMA_CHECK_ARG(x && dy && w && dx && dw && db, "sigma_layernorm_bwd_bf16: null pointer");
   SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_bwd_bf16: C=%d must be a positive multiple of 4", C);
   SIGMA_CHECK_ARG(al8(x) && al8(dy) && al16(w) && al8(dx), "sigma_layernorm_bwd_bf16: w must be 16-byte and x, dy, dx 8-byte aligned");
-  return layernorm_bwd_launch((const float *)x, (const float *)dy, w, (float *)dx, dw, db, rows, C, eps, (cudaStream_t)stream, nullptr, true);
+  return layernorm_bwd_launch((const float *)x, (const float *)dy, w, (float *)dx, dw, db, rows, C, eps, (cudaStream_t)stream, nullptr, SIGMA_BF16);
+}
+
+// the fp16 training mode: x and y fp16 (merge + norm + gate's fp16 in / out instance with one input and no gate)
+int sigma_layernorm_fwd_fp16io(const void *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
+  SIGMA_CHECK_ARG(x && w && b && y, "sigma_layernorm_fwd_fp16io: null pointer");
+  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd_fp16io: C=%d must be a positive multiple of 4", C);
+  SIGMA_CHECK_ARG(al8(x) && al16(w) && al16(b) && al8(y), "sigma_layernorm_fwd_fp16io: w, b must be 16-byte and x, y 8-byte aligned");
+  RowNormParams p{(const float *)x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
+  p.io = 6;
+  return row_norm_launch(p, (cudaStream_t)stream);
+}
+
+int sigma_layernorm_bwd_fp16(const void *x, const void *dy, const float *w, void *dx, float *dw, float *db, int64_t rows, int C, float eps,
+                             void *stream) {
+  SIGMA_CHECK_ARG(x && dy && w && dx && dw && db, "sigma_layernorm_bwd_fp16: null pointer");
+  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_bwd_fp16: C=%d must be a positive multiple of 4", C);
+  SIGMA_CHECK_ARG(al8(x) && al8(dy) && al16(w) && al8(dx), "sigma_layernorm_bwd_fp16: w must be 16-byte and x, dy, dx 8-byte aligned");
+  return layernorm_bwd_launch((const float *)x, (const float *)dy, w, (float *)dx, dw, db, rows, C, eps, (cudaStream_t)stream, nullptr, SIGMA_F16);
 }
 
 int sigma_layernorm_bwd(const float *x, const float *dy, const float *w, float *dx, float *dw, float *db, int64_t rows, int C, float eps,
@@ -671,8 +689,9 @@ int sigma_test_ss2d_bwd_plan(int kind, int batch, int H, int W, int D, int N, in
   return SIGMA_OK;
 }
 
-// the launch plan of sigma_ss2d_scan_fwd{,_split,_bf16}, with bf16 = 2 of sigma_ss2d_scan_fwd_save_bf16 and with bf16 = 3 of
-// sigma_ss2d_scan_fwd_fp16 (force_split = 0: the library's choice), environment overrides included:
+// the launch plan of sigma_ss2d_scan_fwd{,_split,_bf16}, with bf16 = 2 of sigma_ss2d_scan_fwd_save_bf16, with bf16 = 3 of
+// sigma_ss2d_scan_fwd_fp16 and with bf16 = 4 of sigma_ss2d_scan_fwd_save_fp16 (force_split = 0: the library's choice), environment
+// overrides included:
 // out8_host = {segments, tiles per segment, tiles of the longest walk, of the shortest, warps per CTA, ring depth, register
 // budget (CTAs per SM the kernel build assumes), dynamic shared-memory bytes}
 int sigma_test_ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, int R, int bf16, int force_split, size_t workspace_bytes,
@@ -681,13 +700,13 @@ int sigma_test_ss2d_fwd_plan(int kind, int batch, int H, int W, int D, int N, in
                       H > 0 && W > 0 && D > 0 && D % (bf16 ? 8 : 4) == 0 && R > 0 && force_split >= 0 &&
                       (kind != SIGMA_DIRS_CROSS || batch % 2 == 0),
                   "sigma_test_ss2d_fwd_plan: bad arguments");
-  if (bf16 == 2 && N != 4 && N != 16) {
-    set_error("sigma_test_ss2d_fwd_plan: d_state=%d unsupported by the bf16 training forward (4, 16)", N);
+  if ((bf16 == 2 || bf16 == 4) && N != 4 && N != 16) {
+    set_error("sigma_test_ss2d_fwd_plan: d_state=%d unsupported by the %s training forward (4, 16)", N, bf16 == 4 ? "fp16" : "bf16");
     return SIGMA_EUNSUPPORTED;
   }
   long long out[8];
-  const int rc = ss2d_fwd_plan_hook(kind, batch, H, W, D, N, R, bf16 == 3 ? SIGMA_F16 : bf16 ? SIGMA_BF16 : SIGMA_F32, force_split,
-                                    workspace_bytes, out);
+  const int rc = ss2d_fwd_plan_hook(kind, batch, H, W, D, N, R, bf16 == 3 || bf16 == 4 ? SIGMA_F16 : bf16 ? SIGMA_BF16 : SIGMA_F32,
+                                    force_split, workspace_bytes, out);
   if (rc) return rc;
   for (int i = 0; i < 8; ++i) out8_host[i] = out[i];
   return SIGMA_OK;
@@ -712,21 +731,36 @@ int sigma_ss2d_scan_fwd_save(int kind, const float *xc, const float *xdbl, const
                        (cudaStream_t)stream, delta, hs);
 }
 
-// the bf16 training mode: xc, y and delta are bf16, and delta is rounded before the recurrence uses it
-int sigma_ss2d_scan_fwd_save_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
-                                  const float *Ds, void *y, void *delta, float *hs, int batch, int H, int W, int D, int N, int R, int Cp,
-                                  void *workspace, size_t workspace_bytes, int nsplit, void *stream) {
+// The bf16 and fp16 training modes share a body: `fn` names the entry point in its error strings, dtype is SIGMA_BF16 or SIGMA_F16.
+// xc, y and delta are 16-bit, and delta is rounded before the recurrence uses it.
+static int ss2d_scan_fwd_save_16bit(const char *fn, int dtype, int kind, const void *xc, const float *xdbl, const float *dtw,
+                                    const float *dtb, const float *A, const float *Ds, void *y, void *delta, float *hs, int batch, int H,
+                                    int W, int D, int N, int R, int Cp, void *workspace, size_t workspace_bytes, int nsplit, void *stream) {
   if (N == 8) {
-    set_error("sigma_ss2d_scan_fwd_save_bf16: d_state=8 unsupported (4, 16)");
+    set_error("%s: d_state=8 unsupported (4, 16)", fn);
     return SIGMA_EUNSUPPORTED;
   }
   int rc = ss2d_check(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp);
   if (rc) return rc;
-  SIGMA_CHECK_ARG(D % 8 == 0, "sigma_ss2d_scan_fwd_save_bf16: D=%d must be a multiple of 8 (16-byte TMA rows)", D);
-  SIGMA_CHECK_ARG(delta && hs && al16(delta) && al16(hs), "sigma_ss2d_scan_fwd_save_bf16: delta / hs must be non-null and 16-byte aligned");
-  SIGMA_CHECK_ARG(nsplit >= 0, "sigma_ss2d_scan_fwd_save_bf16: nsplit=%d < 0", nsplit);
+  SIGMA_CHECK_ARG(D % 8 == 0, "%s: D=%d must be a multiple of 8 (16-byte TMA rows)", fn, D);
+  SIGMA_CHECK_ARG(delta && hs && al16(delta) && al16(hs), "%s: delta / hs must be non-null and 16-byte aligned", fn);
+  SIGMA_CHECK_ARG(nsplit >= 0, "%s: nsplit=%d < 0", fn, nsplit);
   return ss2d_scan_fwd(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (float *)y, batch, H, W, D, N, R, Cp, workspace, workspace_bytes,
-                       nsplit, (cudaStream_t)stream, (float *)delta, hs, SIGMA_BF16);
+                       nsplit, (cudaStream_t)stream, (float *)delta, hs, dtype);
+}
+
+int sigma_ss2d_scan_fwd_save_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                  const float *Ds, void *y, void *delta, float *hs, int batch, int H, int W, int D, int N, int R, int Cp,
+                                  void *workspace, size_t workspace_bytes, int nsplit, void *stream) {
+  return ss2d_scan_fwd_save_16bit("sigma_ss2d_scan_fwd_save_bf16", SIGMA_BF16, kind, xc, xdbl, dtw, dtb, A, Ds, y, delta, hs, batch, H, W,
+                                  D, N, R, Cp, workspace, workspace_bytes, nsplit, stream);
+}
+
+int sigma_ss2d_scan_fwd_save_fp16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                  const float *Ds, void *y, void *delta, float *hs, int batch, int H, int W, int D, int N, int R, int Cp,
+                                  void *workspace, size_t workspace_bytes, int nsplit, void *stream) {
+  return ss2d_scan_fwd_save_16bit("sigma_ss2d_scan_fwd_save_fp16", SIGMA_F16, kind, xc, xdbl, dtw, dtb, A, Ds, y, delta, hs, batch, H, W,
+                                  D, N, R, Cp, workspace, workspace_bytes, nsplit, stream);
 }
 
 size_t sigma_ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N) {
@@ -743,7 +777,7 @@ size_t sigma_ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W
 static int ss2d_bwd_entry(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                           const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl, float *dA,
                           float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *ws, size_t wsb, int nsplit,
-                          void *stream, int det = 0, int bf16 = 0) {
+                          void *stream, int det = 0, int xdtype = SIGMA_F32) {
   SIGMA_CHECK_ARG(xc && xdbl && dtw && dtb && A && Ds && dy && delta && dxc && ddelta && dxdbl && dA && dDs && ddtb,
                   "sigma_ss2d_scan_bwd_saved: null pointer");
   SIGMA_CHECK_ARG(kind == SIGMA_DIRS_CROSS4 || kind == SIGMA_DIRS_SEQ2 || kind == SIGMA_DIRS_CROSS,
@@ -758,7 +792,7 @@ static int ss2d_bwd_entry(int kind, const float *xc, const float *xdbl, const fl
   SIGMA_CHECK_ARG(al16(xc) && al16(xdbl) && al16(dy) && al16(delta) && al16(dxc) && al16(ddelta) && al16(dxdbl), "sigma_ss2d_scan_bwd_saved: pointers must be 16-byte aligned");
   SIGMA_CHECK_ARG(al16(hs), "sigma_ss2d_scan_bwd_saved: hs must be 16-byte aligned");
   return ss2d_scan_bwd(kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, hs, dxc, ddelta, dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, ws, wsb,
-                       nsplit, (cudaStream_t)stream, det, bf16);
+                       nsplit, (cudaStream_t)stream, det, xdtype);
 }
 
 // backward after sigma_ss2d_scan_fwd_save: `delta` and `hs` are INPUTS (what that call wrote)
@@ -771,19 +805,36 @@ int sigma_ss2d_scan_bwd_saved(int kind, const float *xc, const float *xdbl, cons
                         workspace, workspace_bytes, nsplit, stream);
 }
 
-// backward after sigma_ss2d_scan_fwd_save_bf16: xc, dy and delta are bf16; dxc and every other output fp32
+// backward after sigma_ss2d_scan_fwd_save_bf16 / _fp16 (dtype SIGMA_BF16 / SIGMA_F16): xc, dy and delta are 16-bit; dxc and every
+// other output fp32
+static int ss2d_bwd_saved_16bit(const char *fn, int dtype, int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb,
+                                const float *A, const float *Ds, const void *dy, const void *delta, const float *hs, float *dxc,
+                                float *ddelta, float *dxdbl, float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N,
+                                int R, int Cp, void *workspace, size_t workspace_bytes, int nsplit, void *stream) {
+  SIGMA_CHECK_ARG(hs != nullptr, "%s: null hs", fn);
+  SIGMA_CHECK_ARG(nsplit >= 0, "%s: nsplit=%d < 0", fn, nsplit);
+  if (N == 8) {
+    set_error("%s: d_state=8 unsupported (4, 16)", fn);
+    return SIGMA_EUNSUPPORTED;
+  }
+  return ss2d_bwd_entry(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (const float *)dy, (const float *)delta, hs, dxc, ddelta, dxdbl,
+                        dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace, workspace_bytes, nsplit, stream, 0, dtype);
+}
+
 int sigma_ss2d_scan_bwd_saved_bf16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                                    const float *Ds, const void *dy, const void *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl,
                                    float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
                                    size_t workspace_bytes, int nsplit, void *stream) {
-  SIGMA_CHECK_ARG(hs != nullptr, "sigma_ss2d_scan_bwd_saved_bf16: null hs");
-  SIGMA_CHECK_ARG(nsplit >= 0, "sigma_ss2d_scan_bwd_saved_bf16: nsplit=%d < 0", nsplit);
-  if (N == 8) {
-    set_error("sigma_ss2d_scan_bwd_saved_bf16: d_state=8 unsupported (4, 16)");
-    return SIGMA_EUNSUPPORTED;
-  }
-  return ss2d_bwd_entry(kind, (const float *)xc, xdbl, dtw, dtb, A, Ds, (const float *)dy, (const float *)delta, hs, dxc, ddelta, dxdbl,
-                        dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace, workspace_bytes, nsplit, stream, 0, 1);
+  return ss2d_bwd_saved_16bit("sigma_ss2d_scan_bwd_saved_bf16", SIGMA_BF16, kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, hs, dxc, ddelta,
+                              dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace, workspace_bytes, nsplit, stream);
+}
+
+int sigma_ss2d_scan_bwd_saved_fp16(int kind, const void *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
+                                   const float *Ds, const void *dy, const void *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl,
+                                   float *dA, float *dDs, float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *workspace,
+                                   size_t workspace_bytes, int nsplit, void *stream) {
+  return ss2d_bwd_saved_16bit("sigma_ss2d_scan_bwd_saved_fp16", SIGMA_F16, kind, xc, xdbl, dtw, dtb, A, Ds, dy, delta, hs, dxc, ddelta,
+                              dxdbl, dA, dDs, ddtb, batch, H, W, D, N, R, Cp, workspace, workspace_bytes, nsplit, stream);
 }
 
 // the deterministic build of sigma_ss2d_scan_bwd_saved (nsplit = 0: the library's choice)

@@ -71,8 +71,8 @@ int make_tmap(CUtensorMap *map, CUtensorMapDataType dtype, int rank, const void 
               const uint64_t *strides_bytes, const uint32_t *box, CUtensorMapSwizzle swz, CUtensorMapL2promotion promo);
 int pad_rp(int R);   // dt_rank padded to an instantiated width (4, 8, 12, 16, 24, 32, 48, 64), -1 beyond 64
 size_t ss2d_scan_workspace_bytes(int kind, int batch, int D, int N);
-// xc_dtype: element type of xc and y, SIGMA_F32, SIGMA_BF16 or (inference only) SIGMA_F16; dsave / hsave (training forward):
-// delta' slabs and block-start states for the backward (with SIGMA_BF16: the bf16 training mode, whose delta' slabs are bf16 too)
+// xc_dtype: element type of xc and y, SIGMA_F32, SIGMA_BF16 or SIGMA_F16; dsave / hsave (training forward): delta' slabs and
+// block-start states for the backward (with SIGMA_BF16 / SIGMA_F16: the bf16 / fp16 training modes, whose delta' slabs are 16-bit too)
 int ss2d_scan_fwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A,
                   const float *Ds, float *y, int batch, int H, int W, int D, int N, int R, int Cp, void *ws,
                   size_t ws_bytes, int force_split, cudaStream_t stream, float *dsave = nullptr, float *hsave = nullptr,
@@ -87,12 +87,12 @@ size_t ss2d_scan_hs_bytes(int kind, int batch, int H, int W, int D, int N);
 size_t ss2d_scan_bwd_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
 size_t ss2d_scan_bwd_det_workspace_bytes(int kind, int batch, int H, int W, int D, int N);
 int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int force_split, long long *out4);
-// delta / hs: the delta' slabs and block-start states the training forward wrote; det: the deterministic build; bf16 (excludes
-// det): xc, dy and delta are bf16 behind the float pointers
+// delta / hs: the delta' slabs and block-start states the training forward wrote; det: the deterministic build; xdtype
+// SIGMA_BF16 / SIGMA_F16 (excludes det): xc, dy and delta are bf16 / fp16 behind the float pointers
 int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                   const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs,
                   float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split,
-                  cudaStream_t stream, int det = 0, int bf16 = 0);
+                  cudaStream_t stream, int det = 0, int xdtype = SIGMA_F32);
 
 // ---- scan_op.cu: generic op-level scan forward ----
 __global__ void scan_combine_kernel(float *carry, long long nrows, int nsplit, int NP);
@@ -155,9 +155,10 @@ int upsample_bilinear_bwd_launch(const float *dy, float *dx, int batch, int C, i
 int row_norm_launch(const RowNormParams &p, cudaStream_t stream);
 int quantize_e4m3_rows_launch(const void *x, bool bf16, long long ldx, void *q, long long ldq, float *scale, long long rows, int C,
                               cudaStream_t stream);
-// part != nullptr: the deterministic build (layernorm_bwd_det_workspace_bytes of scratch)
+// part != nullptr: the deterministic build (layernorm_bwd_det_workspace_bytes of scratch); xdtype SIGMA_BF16 / SIGMA_F16 (excludes
+// part): x, dy and dx are bf16 / fp16 behind the float pointers
 int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                         int D, float eps, cudaStream_t stream, float *part = nullptr, bool bf16 = false);
+                         int D, float eps, cudaStream_t stream, float *part = nullptr, int xdtype = SIGMA_F32);
 size_t layernorm_bwd_det_workspace_bytes(long long rows, int D);
 int dwconv3x3_silu_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
                           const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,

@@ -448,7 +448,8 @@ int quantize_e4m3_rows_launch(const void *x, bool bf16, long long ldx, void *q, 
 // atomicAdd per column (torch's GammaBetaBackwardCUDAKernel spent 5.9 ms per Sigma-tiny training step on this reduction).
 // DET: instead of the atomics, warp w of the grid writes its column sums to part[w·D ...] (dgamma) and
 // part[(nwarps + w)·D ...] (dbeta); sum_parts_det_kernel adds them in warp order.
-// T: element type of x, dy and dx (float; __nv_bfloat16 for bf16 activations — gamma, the statistics, dgamma and dbeta stay fp32)
+// T: element type of x, dy and dx (float; __nv_bfloat16 / __half for bf16 / fp16 activations — gamma, the statistics, dgamma and
+// dbeta stay fp32)
 template <int LPR, int V, bool DET, typename T = float>
 __device__ __forceinline__ void layernorm_bwd_body(const T *__restrict__ x, const T *__restrict__ dy, const float *__restrict__ gamma,
                                                    T *__restrict__ dx, float *__restrict__ dgamma, float *__restrict__ dbeta,
@@ -583,6 +584,14 @@ __global__ void __launch_bounds__(256) layernorm_bwd_bf16_kernel(const __nv_bflo
   layernorm_bwd_body<LPR, V, false, __nv_bfloat16>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, nullptr);
 }
 
+template <int LPR, int V>
+__global__ void __launch_bounds__(256) layernorm_bwd_fp16_kernel(const __half *__restrict__ x, const __half *__restrict__ dy,
+                                                                  const float *__restrict__ gamma, __half *__restrict__ dx,
+                                                                  float *__restrict__ dgamma, float *__restrict__ dbeta, long long rows,
+                                                                  int D, float eps) {
+  layernorm_bwd_body<LPR, V, false, __half>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, nullptr);
+}
+
 // enough CTAs to fill the machine, few enough that the 2·D atomics per warp stay negligible (a warp walks >= 4 steps);
 // lanes per row as in the instantiation table of layernorm_bwd_launch
 static unsigned layernorm_bwd_grid(long long rows, int D) {
@@ -593,11 +602,12 @@ static unsigned layernorm_bwd_grid(long long rows, int D) {
 
 template <int LPR, int V>
 static void layernorm_bwd_k(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                            int D, float eps, float *part, cudaStream_t stream, bool bf16) {
+                            int D, float eps, float *part, cudaStream_t stream, int xdtype) {
   using bf = __nv_bfloat16;
   const int warps = 8;
   const unsigned grid = layernorm_bwd_grid(rows, D);
-  if (bf16) layernorm_bwd_bf16_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>((const bf *)x, (const bf *)dy, gamma, (bf *)dx, dgamma, dbeta, rows, D, eps);
+  if (xdtype == SIGMA_F16) layernorm_bwd_fp16_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>((const __half *)x, (const __half *)dy, gamma, (__half *)dx, dgamma, dbeta, rows, D, eps);
+  else if (xdtype == SIGMA_BF16) layernorm_bwd_bf16_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>((const bf *)x, (const bf *)dy, gamma, (bf *)dx, dgamma, dbeta, rows, D, eps);
   else if (part) layernorm_bwd_det_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>(x, dy, gamma, dx, rows, D, eps, part);
   else layernorm_bwd_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps);
 }
@@ -609,9 +619,10 @@ size_t layernorm_bwd_det_workspace_bytes(long long rows, int D) {
 
 // dgamma / dbeta are zeroed here and accumulated into; false if D has no instantiation (the fast forward's D set).
 // part != nullptr: the deterministic build (layernorm_bwd_det_workspace_bytes of scratch), dgamma / dbeta written by the
-// fixed-order sum over the grid's warps.  bf16 (never with part): x, dy and dx are bf16 behind the float pointers
+// fixed-order sum over the grid's warps.  xdtype SIGMA_BF16 / SIGMA_F16 (never with part): x, dy and dx are bf16 / fp16 behind the
+// float pointers
 int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                         int D, float eps, cudaStream_t stream, float *part, bool bf16) {
+                         int D, float eps, cudaStream_t stream, float *part, int xdtype) {
   if (D & 3) { set_error("layernorm_bwd: D=%d must be a multiple of 4", D); return SIGMA_EUNSUPPORTED; }
   if (rows == 0 && !part) return SIGMA_OK;
   if (rows == 0) {
@@ -625,7 +636,7 @@ int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, fl
   }
   const int nvec = D >> 2;
   bool ok = false;
-#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) { layernorm_bwd_k<LPR, V>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, part, stream, bf16); SIGMA_CHECK_LAUNCH(); ok = true; }
+#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) { layernorm_bwd_k<LPR, V>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, part, stream, xdtype); SIGMA_CHECK_LAUNCH(); ok = true; }
   TRY(8, 1) TRY(8, 2) TRY(8, 3) TRY(8, 4)
   TRY(16, 3) TRY(16, 4)
   TRY(32, 3) TRY(32, 4) TRY(32, 6) TRY(32, 8) TRY(32, 12)

@@ -62,7 +62,7 @@ struct alignas(64) Ss2dParams {
   int ablate;  // timing experiments, only in builds with -DSIGMA_SCAN_ABLATION (SIGMA_SCAN_ABLATE env):
                // 1 = no y store, 2 = no per-group prologue, 4 = no TMA reload
   int xc_dtype; // SIGMA_BF16 / SIGMA_F16: xc and y are bf16 / fp16; x_dbl, the state and the recurrence stay fp32.  With hsave
-                // (the bf16 training mode, SIGMA_BF16 only) the delta' slabs are bf16 too and the recurrence runs on the rounded delta'
+                // (the bf16 / fp16 training modes) the delta' slabs are bf16 / fp16 too and the recurrence runs on the rounded delta'
 };
 
 #ifdef SIGMA_SCAN_ABLATION
@@ -103,8 +103,8 @@ __device__ __forceinline__ unsigned long long mul2_raw(unsigned long long a, uns
 // dt_r part of the first row) and whose xc values start at `xrow` (this thread's first channel).  dt_r is read
 // once per position (broadcast LDS.128) and used for all CPT channels; the dot product runs on fma2 pairs
 // (one accumulator chain up to RP = 12, two beyond), softplus is branch-free (common.cuh).
-// RND (the bf16 training mode): delta' is rounded to bf16 here, before the recurrence uses it, so that the value the forward
-// runs on is exactly the value it saves for the backward.
+// RND (the bf16 / fp16 training modes): delta' is rounded to XT (bf16 / fp16) here, before the recurrence uses it, so that the
+// value the forward runs on is exactly the value it saves for the backward.
 template <int N, int CPT, int RP, int G, bool RND = false, typename XT>
 __device__ __forceinline__ void group_prologue(const Ss2dThread<N, CPT, RP> &t, const XT *xrow, const float *drow, int DT,
                                                float (&dl)[CPT][G], float (&u)[CPT][G]) {
@@ -145,8 +145,8 @@ __device__ __forceinline__ void group_prologue(const Ss2dThread<N, CPT, RP> &t, 
 #pragma unroll
     for (int e = 0; e < G; e += 2) {
       const f2 sp = softplus20x2(dl[c][e], dl[c][e + 1]);
-      dl[c][e] = RND ? to_f32(from_f32<__nv_bfloat16>(sp.x)) : sp.x;
-      dl[c][e + 1] = RND ? to_f32(from_f32<__nv_bfloat16>(sp.y)) : sp.y;
+      dl[c][e] = RND ? to_f32(from_f32<XT>(sp.x)) : sp.x;
+      dl[c][e + 1] = RND ? to_f32(from_f32<XT>(sp.y)) : sp.y;
     }
   }
 }
@@ -347,15 +347,16 @@ __device__ __forceinline__ void walk_tiles(Ss2dThread<N, CPT, RP> &t, const Ss2d
   }
 }
 
-// XT: element type of xc and y (float; __nv_bfloat16 in the bf16 inference and training modes, __half in the fp16 inference mode).
-// TRAIN16 (the bf16 training mode, XT = __nv_bfloat16): delta' is rounded to bf16 before the recurrence uses it — in the
-// summary pass too, whose carries must describe the same recurrence — and the SAVE passes store that bf16 delta'.
+// XT: element type of xc and y (float; __nv_bfloat16 in the bf16 inference and training modes, __half in the fp16 inference and
+// training modes).
+// TRAIN16 (the bf16 / fp16 training modes, XT = __nv_bfloat16 / __half): delta' is rounded to XT before the recurrence uses it —
+// in the summary pass too, whose carries must describe the same recurrence — and the SAVE passes store that rounded delta'.
 template <int N, int CPT, int RP, int MODE, bool SAVE, typename XT, bool TRAIN16>
 __device__ __forceinline__ void ss2d_scan_body(const Ss2dParams &p) {
   static_assert(!SAVE || MODE != MODE_SUMMARY, "the summary pass has no final states to save");
   static_assert(!SAVE || sizeof(XT) == 4 || TRAIN16, "the fp32 training forward stores fp32");
-  static_assert(!TRAIN16 || sizeof(XT) == 2, "the bf16 training mode reads and writes bf16");
-  using ST = std::conditional_t<TRAIN16, __nv_bfloat16, float>;   // element type of the saved delta' slabs
+  static_assert(!TRAIN16 || sizeof(XT) == 2, "the 16-bit training modes read and write 16-bit elements");
+  using ST = std::conditional_t<TRAIN16, XT, float>;   // element type of the saved delta' slabs
   constexpr int LT = Ss2dCfg<N>::LT;
   constexpr bool WITH_Y = MODE != MODE_SUMMARY;
   const int NST = p.nst;
@@ -488,7 +489,7 @@ __device__ __forceinline__ void ss2d_scan_body(const Ss2dParams &p) {
 
 template <int N, int CPT, int RP, int MODE, int CTAS, bool SAVE = false, typename XT = float>
 __global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(const __grid_constant__ Ss2dParams p) {
-  static_assert(!SAVE || sizeof(XT) == 4, "the bf16 training forward is ss2d_scan_train16_kernel");
+  static_assert(!SAVE || sizeof(XT) == 4, "the 16-bit training forwards are ss2d_scan_train16_kernel / ss2d_scan_train_fp16_kernel");
   ss2d_scan_body<N, CPT, RP, MODE, SAVE, XT, false>(p);
 }
 
@@ -496,6 +497,13 @@ __global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_kernel(
 template <int N, int CPT, int RP, int MODE, int CTAS, bool SAVE>
 __global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_train16_kernel(const __grid_constant__ Ss2dParams p) {
   ss2d_scan_body<N, CPT, RP, MODE, SAVE, __nv_bfloat16, true>(p);
+}
+
+// the fp16 training mode: the same with fp16 xc / y / delta' (a delta' below 2^-14 is stored subnormal and the recurrence runs on
+// that value; past ±65504 a store gives ±inf)
+template <int N, int CPT, int RP, int MODE, int CTAS, bool SAVE>
+__global__ void __launch_bounds__(32 * Ss2dCfg<N>::MAXW, CTAS) ss2d_scan_train_fp16_kernel(const __grid_constant__ Ss2dParams p) {
+  ss2d_scan_body<N, CPT, RP, MODE, SAVE, __half, true>(p);
 }
 
 // host-side launcher for one (N, CPT, RP) instantiation; defined per RP in ss2d_scan_rp*.cu.

@@ -89,12 +89,12 @@ __device__ __forceinline__ FbWalk fb_walk(const Ss2dBwdParams &p) {
 // DET: every sum across CTAs goes to the partials of the deterministic build (see Ss2dBwdParams) instead of an atomic.
 // CROSS: image b runs with weight set kw = [b >= batch/2] and reads C from image bC = the other modality's (as the forward):
 // the stage holds bC's x_dbl tile too, dC goes to the C columns of bC's dxdbl rows, dA / dDs / d dt_bias to rows kw·D + d.
-// XT: element type of the xc, dy and delta' tiles (float; __nv_bfloat16 in the bf16 training mode, which widens them on the read
-// from the stage and keeps everything else — x_dbl, hs, every accumulator, du / ddelta and their TMA stores — fp32).
+// XT: element type of the xc, dy and delta' tiles (float; __nv_bfloat16 / __half in the bf16 / fp16 training modes, which widen
+// them on the read from the stage and keep everything else — x_dbl, hs, every accumulator, du / ddelta and their TMA stores — fp32).
 template <int N, int MODE, bool DET, bool CROSS, typename XT = float>
 __device__ __forceinline__ void ss2d_bwd_body(const Ss2dBwdParams &p) {
   static_assert(!(DET && CROSS), "no deterministic build of the CROSS backward");
-  static_assert(!DET || sizeof(XT) == 4, "no deterministic build of the bf16 backward");
+  static_assert(!DET || sizeof(XT) == 4, "no deterministic build of the 16-bit backwards");
   constexpr int LPC = FbCfg<N>::LPC, NS = FbCfg<N>::NS, CPW = FbCfg<N>::CPW, NT = FB_DT * LPC;
   constexpr bool MAIN = MODE != MODE_SUMMARY;
   constexpr float kLn2 = 0.6931471805599453f;
@@ -336,6 +336,13 @@ __global__ void __launch_bounds__(128, 2) ss2d_bwd_bf16_kernel(const __grid_cons
 template <int N, int MODE>
 __global__ void __launch_bounds__(128, 2) ss2d_bwd_cross_bf16_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, false, true, __nv_bfloat16>(p); }
 
+// the fp16 training mode (non-deterministic only): fp16 xc / dy / delta' tiles
+template <int N, int MODE>
+__global__ void __launch_bounds__(128, 2) ss2d_bwd_fp16_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, false, false, __half>(p); }
+
+template <int N, int MODE>
+__global__ void __launch_bounds__(128, 2) ss2d_bwd_cross_fp16_kernel(const __grid_constant__ Ss2dBwdParams p) { ss2d_bwd_body<N, MODE, false, true, __half>(p); }
+
 // ---- host ----
 constexpr int kFbMaxSplit = 64;
 
@@ -411,18 +418,19 @@ int ss2d_bwd_plan_hook(int kind, int batch, int H, int W, int D, int N, int forc
 // delta / ddelta: (K, batch, Lseq, D) slabs stored at the position a value belongs to; dxc (batch, Lseq, D) and dxdbl
 // (batch, Lseq, K, Cp) are ACCUMULATED INTO after being zeroed here; dA (K·D, N), dDs (K·D), ddtb (K, D) overwritten.
 // det: the main sweep writes partials (see fb_det_layout) that sum_parts_det_kernel adds in a fixed order.
+// xdtype: element type of xc, dy and delta (SIGMA_F32, or SIGMA_BF16 / SIGMA_F16 behind the float pointers; never with det, the
+// entry points check)
 int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw, const float *dtb, const float *A, const float *Ds,
                   const float *dy, const float *delta, const float *hs, float *dxc, float *ddelta, float *dxdbl, float *dA, float *dDs,
                   float *ddtb, int batch, int H, int W, int D, int N, int R, int Cp, void *ws, size_t ws_bytes, int force_split,
-                  cudaStream_t stream, int det, int bf16) {
+                  cudaStream_t stream, int det, int xdtype) {
   const size_t need = det ? ss2d_scan_bwd_det_workspace_bytes(kind, batch, H, W, D, N) : ss2d_scan_bwd_workspace_bytes(kind, batch, H, W, D, N);
   if (ws == nullptr || ws_bytes < need) {
     set_error("sigma_ss2d_scan_bwd_saved: workspace too small (%zu < %zu)", ws_bytes, need);
     return SIGMA_EWORKSPACE;
   }
   const bool cross = kind == SIGMA_DIRS_CROSS;   // never with det (the entry points reject it)
-  // bf16 (never with det; the entry point checks): xc, dy and delta are bf16 behind the float pointers
-  const uint64_t xes = bf16 ? 2 : 4;             // bytes per xc / dy / delta element
+  const uint64_t xes = xdtype == SIGMA_F32 ? 4 : 2;   // bytes per xc / dy / delta element
   Ss2dBwdParams p;
   memset(&p, 0, sizeof(p));
   const int K = fb_dirs(kind), Kw = fb_wsets(kind);
@@ -432,13 +440,22 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
   p.D = D; p.N = N; p.R = R; p.Cp = Cp; p.K = K; p.batch = batch; p.Lseq = Lseq;
   p.max_tiles = fb_max_tiles(kind, H, W);
   p.carry = (float *)ws;
+  // The zeroing comes before the tensor maps: it is the call's first runtime API call, which binds the device's primary context
+  // to a thread that has none yet (autograd runs a backward that starts at this node on its own thread), and
+  // cuTensorMapEncodeTiled fails without a current context.
+  SIGMA_CHECK_CUDA(cudaMemsetAsync(dxc, 0, (size_t)batch * Lseq * D * sizeof(float), stream));
+  SIGMA_CHECK_CUDA(cudaMemsetAsync(dxdbl, 0, (size_t)batch * Lseq * K * Cp * sizeof(float), stream));
+  SIGMA_CHECK_CUDA(cudaMemsetAsync(dA, 0, (size_t)Kw * D * N * sizeof(float), stream));
+  SIGMA_CHECK_CUDA(cudaMemsetAsync(dDs, 0, (size_t)Kw * D * sizeof(float), stream));
+  SIGMA_CHECK_CUDA(cudaMemsetAsync(ddtb, 0, (size_t)Kw * D * sizeof(float), stream));
   const int CPW = N >= 16 ? 16 : 32;
   int rc;
   auto tmap = [](CUtensorMap *map, const void *base, const uint64_t *dims, const uint64_t *str, const uint32_t *box,
                  CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT32) {
     return make_tmap(map, dtype, 4, base, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
   };
-  const CUtensorMapDataType xdt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  const CUtensorMapDataType xdt = xdtype == SIGMA_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                  : xdtype == SIGMA_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   for (int k = 0; k < K; ++k) {
     const bool colmajor = kind == SIGMA_DIRS_CROSS4 && (k & 1);
     p.rev[k] = kind == SIGMA_DIRS_CROSS4 ? (k >= 2) : (k == 1);
@@ -471,12 +488,6 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
   p.tiles_per_split = pl.tiles_per_split;
   p.nsplit = pl.nsplit;
   p.nst = 2;
-
-  SIGMA_CHECK_CUDA(cudaMemsetAsync(dxc, 0, (size_t)batch * Lseq * D * sizeof(float), stream));
-  SIGMA_CHECK_CUDA(cudaMemsetAsync(dxdbl, 0, (size_t)batch * Lseq * K * Cp * sizeof(float), stream));
-  SIGMA_CHECK_CUDA(cudaMemsetAsync(dA, 0, (size_t)Kw * D * N * sizeof(float), stream));
-  SIGMA_CHECK_CUDA(cudaMemsetAsync(dDs, 0, (size_t)Kw * D * sizeof(float), stream));
-  SIGMA_CHECK_CUDA(cudaMemsetAsync(ddtb, 0, (size_t)Kw * D * sizeof(float), stream));
 
   // per-warp boxes over (K, batch, Lseq, D) slabs: m_dd over ddelta, and for det m_dxc over the du slabs
   auto make_dd = [&](float *slab, CUtensorMap *maps = nullptr) -> int {
@@ -522,12 +533,15 @@ int ss2d_scan_bwd(int kind, const float *xc, const float *xdbl, const float *dtw
       return SIGMA_OK;
     };
     using Kern = void (*)(Ss2dBwdParams);
-    const Kern bw_serial = bf16 ? (cross ? ss2d_bwd_cross_bf16_kernel<NN, MODE_SERIAL> : ss2d_bwd_bf16_kernel<NN, MODE_SERIAL>)
-                                : (cross ? ss2d_bwd_cross_kernel<NN, MODE_SERIAL> : ss2d_bwd_kernel<NN, MODE_SERIAL>);
-    const Kern bw_summary = bf16 ? (cross ? ss2d_bwd_cross_bf16_kernel<NN, MODE_SUMMARY> : ss2d_bwd_bf16_kernel<NN, MODE_SUMMARY>)
-                                 : (cross ? ss2d_bwd_cross_kernel<NN, MODE_SUMMARY> : ss2d_bwd_kernel<NN, MODE_SUMMARY>);
-    const Kern bw_apply = bf16 ? (cross ? ss2d_bwd_cross_bf16_kernel<NN, MODE_APPLY> : ss2d_bwd_bf16_kernel<NN, MODE_APPLY>)
-                               : (cross ? ss2d_bwd_cross_kernel<NN, MODE_APPLY> : ss2d_bwd_kernel<NN, MODE_APPLY>);
+    auto pick = [&](auto mode) -> Kern {
+      constexpr int M = decltype(mode)::value;
+      if (xdtype == SIGMA_BF16) return cross ? ss2d_bwd_cross_bf16_kernel<NN, M> : ss2d_bwd_bf16_kernel<NN, M>;
+      if (xdtype == SIGMA_F16) return cross ? ss2d_bwd_cross_fp16_kernel<NN, M> : ss2d_bwd_fp16_kernel<NN, M>;
+      return cross ? ss2d_bwd_cross_kernel<NN, M> : ss2d_bwd_kernel<NN, M>;
+    };
+    const Kern bw_serial = pick(std::integral_constant<int, MODE_SERIAL>{});
+    const Kern bw_summary = pick(std::integral_constant<int, MODE_SUMMARY>{});
+    const Kern bw_apply = pick(std::integral_constant<int, MODE_APPLY>{});
     int r;
     if (!det) {
       if (p.nsplit == 1) return run(bw_serial, mn_smem);

@@ -392,8 +392,8 @@ def ss2d_scan(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
 
 def ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
     """Training forward: ss2d_scan that also returns delta' (K, batch, Lseq, D) and the block-start states `hs` for
-    sigma_ss2d_scan_bwd_saved (no state sweep in the backward).  A bf16 xc runs the bf16 training mode: y and delta' are bf16
-    too, and delta' is the rounded value the recurrence itself used (sigma_ss2d_scan_fwd_save_bf16)."""
+    sigma_ss2d_scan_bwd_saved (no state sweep in the backward).  A bf16 (fp16) xc runs the bf16 (fp16) training mode: y and delta'
+    are bf16 (fp16) too, and delta' is the rounded value the recurrence itself used (sigma_ss2d_scan_fwd_save_bf16 / _fp16)."""
     L_ = _lib.lib()
     ndir = {_lib.DIRS_CROSS4: 4, _lib.DIRS_SEQ2: 2, _lib.DIRS_CROSS: 1}[kind]
     Lseq = 2 * H * W if kind == _lib.DIRS_SEQ2 else H * W
@@ -402,7 +402,7 @@ def ss2d_scan_save(kind, xc, xdbl, dtw, dtb, A, Ds, batch, H, W, D, N, R, Cp):
     hs = torch.empty(L_.sigma_ss2d_scan_hs_bytes(kind, batch, H, W, D, N) // 4, dtype=torch.float32, device=xc.device)
     wsb = L_.sigma_ss2d_scan_workspace_bytes(kind, batch, H, W, D, N)
     ws = torch.empty(wsb, dtype=torch.uint8, device=xc.device)
-    fn = "sigma_ss2d_scan_fwd_save_bf16" if xc.dtype == torch.bfloat16 else "sigma_ss2d_scan_fwd_save"
+    fn = _entry("sigma_ss2d_scan_fwd_save", xc.dtype)
     rc = getattr(L_, fn)(kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(y), ptr(delta), ptr(hs), batch, H, W, D,
                          N, R, Cp, ptr(ws), wsb, int(_FORCE_SPLIT or 0), stream())
     _lib.check(rc, fn)

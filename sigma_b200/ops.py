@@ -366,24 +366,49 @@ def bf16_training_core(on=True):
         BF16_TRAINING_CORE = prev
 
 
-def _bf16_autocast():
-    return (BF16_TRAINING_CORE and torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16
-            and not deterministic())
+# ---- fp16 training mode of the fused core (opt-in) ----
+# The same under fp16 autocast, with fp16 in place of bf16.  fp16 keeps 11 significant bits where bf16 keeps 8, but its range ends at
+# ±65504: a store past it gives ±inf (nothing saturates), so the mode is meant to run with a loss scaler (torch.amp.GradScaler), which
+# sees the inf and skips the step.  SIGMA_FP16_TRAINING_CORE=1 sets the initial value.  The two switches are independent; the
+# autocast dtype decides which of them can apply.
+FP16_TRAINING_CORE = os.environ.get("SIGMA_FP16_TRAINING_CORE", "0") == "1"
 
 
-def _bf16_mode_fwd(takes_bf16):
-    """torch.amp.custom_fwd(cast_inputs=torch.float32) for an autograd forward, except when `takes_bf16(ctx, *args)` holds under
-    the bf16 training mode: then the arguments are passed as they are (autocast off inside, as custom_fwd does) and
-    ctx.bf16_mode is True."""
+@contextlib.contextmanager
+def fp16_training_core(on=True):
+    """Switch the fp16 training mode of the fused core on (or off) inside the block."""
+    global FP16_TRAINING_CORE
+    prev, FP16_TRAINING_CORE = FP16_TRAINING_CORE, bool(on)
+    try:
+        yield
+    finally:
+        FP16_TRAINING_CORE = prev
+
+
+def _autocast_mode16():
+    """the 16-bit training mode in effect: torch.bfloat16 / torch.float16 when autocast on CUDA runs that dtype and its switch is
+    on, outside the deterministic switch; else None"""
+    if not torch.is_autocast_enabled("cuda") or deterministic():
+        return None
+    dt = torch.get_autocast_dtype("cuda")
+    on = {torch.bfloat16: BF16_TRAINING_CORE, torch.float16: FP16_TRAINING_CORE}.get(dt, False)
+    return dt if on else None
+
+
+def _mode16_fwd(takes16):
+    """torch.amp.custom_fwd(cast_inputs=torch.float32) for an autograd forward, except when `takes16(ctx, dtype, *args)` holds
+    under a 16-bit training mode of that dtype: then the arguments are passed as they are (autocast off inside, as custom_fwd
+    does) and ctx.mode16 is the dtype (None otherwise)."""
     def decorate(fwd):
         widened = torch.amp.custom_fwd(fwd, device_type="cuda", cast_inputs=torch.float32)
 
         @functools.wraps(fwd)
         def wrapper(ctx, *args):
-            ctx.bf16_mode = _bf16_autocast() and takes_bf16(ctx, *args)
-            if not ctx.bf16_mode:
+            dt = _autocast_mode16()
+            ctx.mode16 = dt if dt is not None and takes16(ctx, dt, *args) else None
+            if ctx.mode16 is None:
                 return widened(ctx, *args)
-            ctx._dtype, ctx._fwd_used_autocast = torch.get_autocast_dtype("cuda"), False    # what custom_bwd reads
+            ctx._dtype, ctx._fwd_used_autocast = dt, False    # what custom_bwd reads
             with torch.autocast("cuda", enabled=False):
                 return fwd(ctx, *args)
         return wrapper
@@ -396,16 +421,17 @@ FUSED_LAYERNORM = True
 
 class LayerNormFn(torch.autograd.Function):
     """nn.LayerNorm over the last dim under autograd: forward = sigma_layernorm_fwd, backward = sigma_layernorm_bwd (dx, dweight, dbias in
-    one pass over x and dy; nothing saved but x).  Numerics as F.layer_norm in fp32.  In the bf16 training mode a bf16 x stays bf16
-    (sigma_layernorm_fwd_bf16io / sigma_layernorm_bwd_bf16: bf16 x, y, dy, dx; fp32 statistics, parameters and their gradients)."""
+    one pass over x and dy; nothing saved but x).  Numerics as F.layer_norm in fp32.  In the bf16 (fp16) training mode a bf16 (fp16)
+    x stays 16-bit (sigma_layernorm_fwd_bf16io / sigma_layernorm_bwd_bf16, or the _fp16io / _fp16 pair: 16-bit x, y, dy, dx; fp32
+    statistics, parameters and their gradients)."""
 
     @staticmethod
-    @_bf16_mode_fwd(lambda ctx, x, weight, bias, eps: x.dtype == torch.bfloat16 and weight.dtype == torch.float32)
+    @_mode16_fwd(lambda ctx, dt, x, weight, bias, eps: x.dtype == dt and weight.dtype == torch.float32)
     def forward(ctx, x, weight, bias, eps):
         x2 = x.contiguous().view(-1, x.shape[-1])
         y = torch.empty_like(x2)
         w, b = weight.contiguous(), bias.contiguous()
-        fn = "sigma_layernorm_fwd_bf16io" if ctx.bf16_mode else "sigma_layernorm_fwd"
+        fn = {torch.bfloat16: "sigma_layernorm_fwd_bf16io", torch.float16: "sigma_layernorm_fwd_fp16io"}.get(ctx.mode16, "sigma_layernorm_fwd")
         _lib.check(getattr(_lib.lib(), fn)(ptr(x2), ptr(w), ptr(b), ptr(y), x2.shape[0], x2.shape[1], float(eps), stream()), fn)
         ctx.save_for_backward(x2, w)
         ctx.eps = float(eps)
@@ -417,10 +443,11 @@ class LayerNormFn(torch.autograd.Function):
         x2, w = ctx.saved_tensors
         dx = torch.empty_like(x2)
         dw, db = torch.empty_like(w), torch.empty_like(w)
-        if ctx.bf16_mode:
-            dy2 = dy.contiguous().to(torch.bfloat16).view(-1, x2.shape[1])
-            _lib.check(_lib.lib().sigma_layernorm_bwd_bf16(ptr(x2), ptr(dy2), ptr(w), ptr(dx), ptr(dw), ptr(db), x2.shape[0], x2.shape[1],
-                                                          ctx.eps, stream()), "sigma_layernorm_bwd_bf16")
+        if ctx.mode16 is not None:
+            dy2 = dy.contiguous().to(ctx.mode16).view(-1, x2.shape[1])
+            fn = "sigma_layernorm_bwd_bf16" if ctx.mode16 == torch.bfloat16 else "sigma_layernorm_bwd_fp16"
+            _lib.check(getattr(_lib.lib(), fn)(ptr(x2), ptr(dy2), ptr(w), ptr(dx), ptr(dw), ptr(db), x2.shape[0], x2.shape[1], ctx.eps,
+                                               stream()), fn)
             return dx.view(dy.shape), dw, db, None
         dy2 = dy.contiguous().float().view(-1, x2.shape[1])
         if deterministic():
@@ -446,14 +473,16 @@ def layer_norm(norm, x):
 
 
 _SAVED_BF16 = 2               # `saved` of _call_ss2d_bwd: the arguments are those of sigma_ss2d_scan_bwd_saved_bf16
+_SAVED_FP16 = 3               # ... of sigma_ss2d_scan_bwd_saved_fp16 (the same layout)
 
 
 def _call_ss2d_bwd(args, saved=True, det=False):
-    """The native call of the fused backward, sigma_ss2d_scan_bwd_saved (_det when det; _bf16 when saved is _SAVED_BF16).  A
-    module-level function so that bench.py can bracket it with events, through a wrapper that passes (args, saved) on: so the
-    bf16 training mode is a value of `saved`, not another argument."""
+    """The native call of the fused backward, sigma_ss2d_scan_bwd_saved (_det when det; _bf16 / _fp16 when saved is _SAVED_BF16 /
+    _SAVED_FP16).  A module-level function so that bench.py can bracket it with events, through a wrapper that passes (args, saved)
+    on: so the 16-bit training modes are values of `saved`, not another argument."""
     from . import fused
     fn = ("sigma_ss2d_scan_bwd_saved_bf16" if saved == _SAVED_BF16 else
+          "sigma_ss2d_scan_bwd_saved_fp16" if saved == _SAVED_FP16 else
           "sigma_ss2d_scan_bwd_saved_det" if det else "sigma_ss2d_scan_bwd_saved")
     _lib.check(getattr(_lib.lib(), fn)(*args, int(fused._FORCE_SPLIT or 0), stream()), fn)
 
@@ -470,11 +499,13 @@ class FusedSS2DCore(torch.autograd.Function):
     The bf16 training mode (BF16_TRAINING_CORE, bf16 autocast, not deterministic, some input needs a gradient):
     xc is taken (or cast to) bf16 and never widened, x_proj runs the bf16 GEMM with fp32 x_dbl out, sigma_ss2d_scan_fwd_save_bf16
     writes bf16 y and the bf16 delta' its own recurrence ran on, and the backward (sigma_ss2d_scan_bwd_saved_bf16) takes a bf16 dy
-    and returns a bf16 dxc rounded once from the fp32 sum of the directions and the x_proj term; parameter gradients are fp32."""
+    and returns a bf16 dxc rounded once from the fp32 sum of the directions and the x_proj term; parameter gradients are fp32.
+    The fp16 training mode (FP16_TRAINING_CORE, fp16 autocast, the same conditions) is the same with fp16 for bf16: the x_proj GEMM is
+    sigma_linear_fp16, the pair sigma_ss2d_scan_fwd_save_fp16 / sigma_ss2d_scan_bwd_saved_fp16; a dxc past ±65504 becomes ±inf."""
 
     @staticmethod
-    @_bf16_mode_fwd(lambda ctx, xc, *a: any(ctx.needs_input_grad) and fused_core_ok(xc, xc.shape[-1], a[3].shape[1])
-                    and all(t.dtype == torch.float32 for t in a[:5]))
+    @_mode16_fwd(lambda ctx, dt, xc, *a: any(ctx.needs_input_grad) and fused_core_ok(xc, xc.shape[-1], a[3].shape[1])
+                 and all(t.dtype == torch.float32 for t in a[:5]))
     def forward(ctx, xc, x_proj_weight, dt_projs_weight, dt_projs_bias, A_logs, Ds, kind, H, W):
         from . import fused
         Kw, _, D = x_proj_weight.shape
@@ -483,8 +514,8 @@ class FusedSS2DCore(torch.autograd.Function):
         N, R = A_logs.shape[1], dt_projs_weight.shape[2]
         Cp = _lib.lib().sigma_ss2d_padded_cp(N, R)
         xc = xc.contiguous()
-        if ctx.bf16_mode:
-            xc = xc.to(torch.bfloat16)           # a bf16 xc (the conv + SiLU under autocast) passes through untouched
+        if ctx.mode16 is not None:
+            xc = xc.to(ctx.mode16)               # a 16-bit xc of that dtype (the conv + SiLU under autocast) passes through untouched
         B, Lseq, _ = xc.shape
         xw = torch.cat([fused._pack_xproj(x_proj_weight[k], N, R, Cp) for k in range(Kw)], dim=0).contiguous()     # (Kw·Cp, D)
         if cross:   # each modality's half of the batch through its own x_proj
@@ -517,8 +548,8 @@ class FusedSS2DCore(torch.autograd.Function):
             raise RuntimeError("FusedSS2DCore: kind CROSS has no deterministic backward; under torch.use_deterministic_algorithms(True) "
                                "CroMB trains through the op-level _det kernels (CrossMambaFusion_SS2D_SSM routes there itself)")
         B, Lseq, _ = xc.shape
-        bf16 = ctx.bf16_mode
-        dy = dy.contiguous().to(torch.bfloat16) if bf16 else dy.contiguous().float()
+        m16 = ctx.mode16
+        dy = dy.contiguous().to(m16) if m16 is not None else dy.contiguous().float()
         dev = xc.device
         ddelta = torch.empty((K, B, Lseq, D), dtype=torch.float32, device=dev)
         dxc = torch.empty((B, Lseq, D), dtype=torch.float32, device=dev)
@@ -532,8 +563,8 @@ class FusedSS2DCore(torch.autograd.Function):
         args = (kind, ptr(xc), ptr(xdbl), ptr(dtw), ptr(dtb), ptr(A), ptr(Ds), ptr(dy), ptr(delta), ptr(hs),
                 ptr(dxc), ptr(ddelta), ptr(dxdbl), ptr(dA), ptr(dDs), ptr(ddtb), B, H, W, D, N, R, Cp, ptr(ws), wsb)
         # det only when set: bench.py --mode train brackets this call with a wrapper that takes (args, saved)
-        if bf16:
-            _call_ss2d_bwd(args, _SAVED_BF16)
+        if m16 is not None:
+            _call_ss2d_bwd(args, _SAVED_BF16 if m16 == torch.bfloat16 else _SAVED_FP16)
             xc = xc.float()                      # only the x_proj weight gradient below (a torch matmul) needs the widened copy
         else:
             _call_ss2d_bwd(args, True, True) if det else _call_ss2d_bwd(args, True)
@@ -548,7 +579,7 @@ class FusedSS2DCore(torch.autograd.Function):
                 dxcm[m].addmm_(dxd[m], xw3[m])
                 dxw[m] = dxd[m].t() @ xcm[m]
             dxpw = torch.cat([dxw[:, 2 * N:2 * N + R], dxw[:, 0:N], dxw[:, N:2 * N]], dim=1)
-            return (dxc.to(torch.bfloat16) if bf16 else dxc), dxpw, dW, ddtb, dA * A, dDs, None, None, None
+            return (dxc.to(m16) if m16 is not None else dxc), dxpw, dW, ddtb, dA * A, dDs, None, None, None
         # dt_proj: d dt_r = ddelta_k · W_dt[k]  (into the dt_r columns of dxdbl),  dW_dt[k] = ddelta_k^T · dt_r_k
         xd3 = xdbl.view(B * Lseq, K, Cp)
         dW = torch.empty_like(dtw)
@@ -562,7 +593,7 @@ class FusedSS2DCore(torch.autograd.Function):
         dxc2.addmm_(d2, xw)
         dxw = (d2.t() @ xc.view(B * Lseq, D)).view(K, Cp, D)
         dxpw = torch.cat([dxw[:, 2 * N:2 * N + R], dxw[:, 0:N], dxw[:, N:2 * N]], dim=1)          # back to [dt | B | C] rows
-        return (dxc.to(torch.bfloat16) if bf16 else dxc), dxpw, dW, ddtb, dA * A, dDs, None, None, None
+        return (dxc.to(m16) if m16 is not None else dxc), dxpw, dW, ddtb, dA * A, dDs, None, None, None
 
 
 # ---- deterministic training: bilinear upsampling and cross-entropy ----

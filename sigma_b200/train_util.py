@@ -54,21 +54,34 @@ class TrainStep:
     """One iteration of train.py:164-172: loss = model(imgs, modal_xs, gts); zero_grad; backward; optimizer.step.
     `amp_dtype` = torch.bfloat16 runs the dense layers under autocast (the scan casts itself to fp32, vmamba.py:36).
     `bf16_core` = True switches the bf16 training mode of the fused core on around the step (ops.bf16_training_core); False
-    leaves ops.BF16_TRAINING_CORE as it is."""
+    leaves ops.BF16_TRAINING_CORE as it is.  `fp16_core` does the same for the fp16 training mode (ops.fp16_training_core), which
+    applies under amp_dtype = torch.float16.
+    `scaler` (a torch.amp.GradScaler, the usual companion of fp16 autocast): the step back-propagates the scaled loss and lets the
+    scaler unscale the gradients, skip the optimizer step when one of them is inf / NaN, and update its scale.  The returned loss
+    is unscaled either way."""
 
-    def __init__(self, model, optimizer, amp_dtype=None, device_type="cuda", bf16_core=False):
+    def __init__(self, model, optimizer, amp_dtype=None, device_type="cuda", bf16_core=False, fp16_core=False, scaler=None):
         self.model, self.opt, self.amp, self.device_type = model, optimizer, amp_dtype, device_type
         self.bf16_core = bf16_core
+        self.fp16_core, self.scaler = fp16_core, scaler
 
     def __call__(self, rgb, modal_x, label, sync=True):
         from . import ops
         ctx = self.model.no_sync() if (not sync and hasattr(self.model, "no_sync")) else contextlib.nullcontext()
-        with ctx, (ops.bf16_training_core() if self.bf16_core else contextlib.nullcontext()):
+        with ctx, (ops.bf16_training_core() if self.bf16_core else contextlib.nullcontext()), \
+                (ops.fp16_training_core() if self.fp16_core else contextlib.nullcontext()):
             with torch.autocast(self.device_type, dtype=self.amp, enabled=self.amp is not None):
                 loss = self.model(rgb, modal_x, label)
             self.opt.zero_grad(set_to_none=True)
-            loss.backward()
-        self.opt.step()
+            if self.scaler is None:
+                loss.backward()
+            else:
+                self.scaler.scale(loss).backward()
+        if self.scaler is None:
+            self.opt.step()
+        else:
+            self.scaler.step(self.opt)
+            self.scaler.update()
         return loss
 
 
