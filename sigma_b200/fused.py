@@ -183,6 +183,14 @@ _LOWP = {}            # id(weight) -> (weakref, version, {form: copy}): the bf16
                       # per-channel e4m3 rows and scales ("e4m3") of a weight, each made once per version
 
 
+def weights_updated(tensors):
+    """Record that `tensors` (parameters) were written in place where autograd did not see it, as a replayed CUDA graph's
+    optimizer step does (train_util.GraphedTrainStep calls this after every replay).  It bumps each tensor's `_version`, the key
+    of every derived-weight cache here (_SPLIT, _LOWP, _W9, the packed SSM parameters of _cache) and of InferencePipeline's
+    re-capture, so the next inference forward rebuilds them from the new values.  One host call for the list; no kernel runs."""
+    torch.autograd.graph.increment_version(tensors)
+
+
 def _split_weight(w):
     import weakref
     ent = _SPLIT.get(id(w))

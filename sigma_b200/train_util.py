@@ -27,10 +27,12 @@ def group_weight(module, lr, norm_layer=nn.BatchNorm2d):
     return [dict(params=decay, lr=lr), dict(params=no_decay, weight_decay=0.0, lr=lr)]
 
 
-def make_optimizer(model, lr=6e-5, weight_decay=0.01, capturable=False):
+def make_optimizer(model, lr=6e-5, weight_decay=0.01, capturable=False, fused=False):
     """train.py:84-93 with configs/config_MFNet.py:53-59 (AdamW, lr 6e-5, betas (0.9, 0.999), weight decay 0.01).
-    capturable=True keeps the step counters on the device so the whole step can live in a CUDA graph."""
-    return torch.optim.AdamW(group_weight(model, lr), lr=lr, betas=(0.9, 0.999), weight_decay=weight_decay, capturable=capturable)
+    capturable=True keeps the step counters on the device so the whole step can live in a CUDA graph.  fused=True runs torch's
+    fused AdamW, which also takes a GradScaler's scale and inf flag on the device (what GraphedTrainStep needs with a scaler)."""
+    return torch.optim.AdamW(group_weight(model, lr), lr=lr, betas=(0.9, 0.999), weight_decay=weight_decay, capturable=capturable,
+                             fused=fused or None)
 
 
 def wrap_ddp(model, device_index=None, single_bucket=False):
@@ -83,6 +85,118 @@ class TrainStep:
             self.scaler.step(self.opt)
             self.scaler.update()
         return loss
+
+
+class GraphedTrainStep:
+    """TrainStep replayed from one CUDA graph: forward, backward and optimizer step (with a scaler, also its unscale / inf check,
+    the skipped or applied step and the scale update) are captured once and each call replays them, so the host issues one graph
+    launch per step instead of every kernel.  Same arguments as TrainStep, plus `example` = (rgb, modal_x, label), a batch whose
+    shapes, dtypes and device every later batch must have.
+
+    Construction copies the example into static input buffers, runs `warmup` eager steps on a side stream (lazy optimizer and
+    scaler state, cuBLAS / cuDNN handles, kernel attributes), captures one step, then puts back the parameters, gradients,
+    buffers, optimizer state and scaler state it found, so the first replay is the first step.  Random draws (DropPath) are not
+    put back; each replay draws fresh ones from torch's generator.
+
+    Conditions, each a ValueError: every param group of the optimizer is capturable=True or fused=True (make_optimizer(capturable=
+    True) builds one); with an enabled scaler the optimizer is fused=True, whose kernel unscales and skips the step on the device;
+    the model is not DistributedDataParallel (its all-reduce is not captured); a call's batch matches the example; and the capture
+    itself succeeds (there is no eager fallback).  Hyper-parameters given as Python numbers (lr, betas, weight decay) are fixed at
+    capture.
+
+    A call returns the unscaled loss as a new device tensor and never waits for the GPU.  After each replay the updated tensors'
+    `_version` is bumped (fused.weights_updated), so the fused inference forward, InferencePipeline and DeviceEvaluator see the new
+    weights."""
+
+    def __init__(self, model, optimizer, example, amp_dtype=None, bf16_core=False, fp16_core=False, scaler=None, warmup=3):
+        from torch.nn.parallel import DistributedDataParallel
+        if isinstance(model, DistributedDataParallel):
+            raise ValueError("GraphedTrainStep: a DistributedDataParallel model cannot be captured (its gradient all-reduce is not "
+                             "part of the graph); train multi-GPU with TrainStep")
+        groups = optimizer.param_groups
+        if not all(g.get("capturable") or g.get("fused") for g in groups):
+            raise ValueError(f"GraphedTrainStep: {type(optimizer).__name__} cannot be captured: every param group needs "
+                             "capturable=True or fused=True (make_optimizer(model, capturable=True))")
+        if scaler is not None and scaler.is_enabled() and not getattr(optimizer, "_step_supports_amp_scaling", False):
+            raise ValueError("GraphedTrainStep: with a GradScaler the optimizer must take the scale and inf flag on the device "
+                             "(fused=True, e.g. make_optimizer(model, capturable=True, fused=True)); otherwise scaler.step "
+                             "reads the inf flag on the host")
+        if warmup < 1:
+            raise ValueError("GraphedTrainStep: warmup must be >= 1 (the optimizer's and scaler's state must exist before the capture, "
+                             "or the graph would re-initialise it on every replay)")
+        if len(example) != 3 or not all(torch.is_tensor(t) and t.is_cuda for t in example) or len({t.device for t in example}) != 1:
+            raise ValueError("GraphedTrainStep: the example batch must be three CUDA tensors (rgb, modal_x, label) on one device")
+        for g in groups:
+            if g.get("fused"):
+                g["capturable"] = True   # fused kernels keep `step` on the device either way; torch's capture check reads the flag
+        self.model, self.opt, self.scaler = model, optimizer, scaler
+        self.static = tuple(t.detach().clone() for t in example)
+        self.step = TrainStep(model, optimizer, amp_dtype=amp_dtype, bf16_core=bf16_core, fp16_core=fp16_core, scaler=scaler)
+        self.updated = [p for g in groups for p in g["params"]]
+        saved = self._snapshot()
+        side = torch.cuda.Stream(device=self.static[0].device)
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(warmup):
+                self.step(*self.static)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        try:
+            with torch.cuda.graph(self.graph):
+                self.loss = self.step(*self.static).detach()
+        except Exception as e:
+            raise ValueError(f"GraphedTrainStep: capturing the step failed ({type(e).__name__}: {e})") from e
+        torch.cuda.synchronize()
+        self._restore(saved)
+
+    def _snapshot(self):
+        clone = lambda t: None if t is None else t.detach().clone()   # noqa: E731
+        sc = self.scaler
+        return dict(params=[clone(p) for p in self.model.parameters()], grads=[clone(p.grad) for p in self.model.parameters()],
+                    buffers=[clone(b) for b in self.model.buffers()],
+                    opt={p: {k: clone(v) if torch.is_tensor(v) else v for k, v in self.opt.state[p].items()}
+                         for p in self.updated if p in self.opt.state},
+                    scaler=None if sc is None or getattr(sc, "_scale", None) is None else (clone(sc._scale), clone(sc._growth_tracker)))
+
+    @torch.no_grad()
+    def _restore(self, saved):
+        """Put back what _snapshot saw, in place (the graph reads and writes these very tensors).  State that did not exist then
+        (a fresh optimizer's moments and step, a fresh scaler) goes back to the values its lazy initialisation gives: zeros and the
+        initial scale."""
+        for p, v in zip(self.model.parameters(), saved["params"]):
+            p.copy_(v)
+        for p, g in zip(self.model.parameters(), saved["grads"]):
+            if p.grad is not None:
+                p.grad.copy_(g) if g is not None else p.grad.zero_()
+        for b, v in zip(self.model.buffers(), saved["buffers"]):
+            b.copy_(v)
+        for p in self.updated:
+            old = saved["opt"].get(p)
+            for k, v in self.opt.state[p].items():
+                if torch.is_tensor(v):
+                    v.copy_(old[k]) if old is not None else v.zero_()
+        sc = self.scaler
+        if sc is not None and getattr(sc, "_scale", None) is not None:
+            if saved["scaler"] is not None:
+                sc._scale.copy_(saved["scaler"][0])
+                sc._growth_tracker.copy_(saved["scaler"][1])
+            else:
+                sc._scale.fill_(sc._init_scale)
+                sc._growth_tracker.fill_(sc._init_growth_tracker)
+        torch.cuda.synchronize()
+
+    def __call__(self, rgb, modal_x, label):
+        from . import fused
+        for name, t, s in zip(("rgb", "modal_x", "label"), (rgb, modal_x, label), self.static):
+            if not torch.is_tensor(t) or t.shape != s.shape or t.dtype != s.dtype or t.device != s.device:
+                got = (tuple(t.shape), t.dtype, t.device) if torch.is_tensor(t) else type(t).__name__
+                raise ValueError(f"GraphedTrainStep: {name} is {got}; the graph was captured for {(tuple(s.shape), s.dtype, s.device)}")
+            if t is not s:
+                s.copy_(t, non_blocking=True)
+        self.graph.replay()
+        fused.weights_updated(self.updated)
+        return self.loss.clone()
 
 
 def grad_bytes(model):
