@@ -293,6 +293,29 @@ int sigma_dwconv3x3_silu_fwd_bf16(const void *x, int64_t x_row_stride, int64_t x
 int sigma_dwconv3x3_silu_fwd_fp16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
                                   void *y, int64_t y_batch_stride, int batch, int H, int W, int D, void *stream);
 
+/* Backward of sigma_dwconv3x3_silu_fwd (training: the autograd of nn.Conv2d(D, D, 3, padding=1, groups=D) + SiLU).  With
+ * pre = conv(x) + b recomputed from x and s = sigmoid(pre):
+ *   g = dy·s·(1 + pre·(1 − s)),  dx = the transposed stencil of g (flipped taps),
+ *   dw[c, tap] = Σ over images and pixels of g·(x at the tap's shift),  dbias = Σ g.
+ * x as in the forward (position rows x_row_stride elements apart, images x_batch_stride apart); dy and dx (H·W, D) rows per image,
+ * images dy_batch_stride / dx_batch_stride elements apart; dw (D,1,3,3) and dbias (D) fp32, overwritten.  bias and dbias may be
+ * NULL together.  Deterministic by construction (no float atomics): each CTA sums its tiles in a fixed order into one partial row
+ * of the caller's workspace (sigma_dwconv3x3_silu_bwd_workspace_bytes, 16-byte aligned), and the rows are added in order, so the
+ * same inputs give the same bits with or without a deterministic mode.  D % 4 == 0; x, dy, dx 16-byte aligned, strides multiples
+ * of 4 elements.                                                                                                              */
+size_t sigma_dwconv3x3_silu_bwd_workspace_bytes(int batch, int H, int W, int D);
+int sigma_dwconv3x3_silu_bwd(const float *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
+                             const float *dy, int64_t dy_batch_stride, float *dx, int64_t dx_batch_stride, float *dw, float *dbias,
+                             int batch, int H, int W, int D, void *workspace, size_t workspace_bytes, void *stream);
+/* bf16 / fp16 training: the same with x, dy and dx 16-bit (D % 8 == 0, strides multiples of 8 elements).  g, every sum, dw and
+ * dbias are fp32; dx rounds once (fp16: past ±65504 to ±inf).  The same workspace.                                             */
+int sigma_dwconv3x3_silu_bwd_bf16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
+                                  const void *dy, int64_t dy_batch_stride, void *dx, int64_t dx_batch_stride, float *dw, float *dbias,
+                                  int batch, int H, int W, int D, void *workspace, size_t workspace_bytes, void *stream);
+int sigma_dwconv3x3_silu_bwd_fp16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
+                                  const void *dy, int64_t dy_batch_stride, void *dx, int64_t dx_batch_stride, float *dw, float *dbias,
+                                  int batch, int H, int W, int D, void *workspace, size_t workspace_bytes, void *stream);
+
 /* CrossMerge sum + out_norm LayerNorm + gates (vmamba.py:217-224,1077; ConMB: 423-428,1280-1281):
  *   out[r,:] = (LN(Σ_k y[k][r,:])·gamma+beta) · (z ? SiLU(z[r,:]) : 1) · (gate ? gate[r / rows_per_batch, :] : 1)
  * Row r = (b, i) with b = r / rows_per_batch: input row at y + k·k_stride + b·in_batch_stride + i·D,

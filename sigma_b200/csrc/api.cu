@@ -595,6 +595,50 @@ int sigma_dwconv3x3_silu_fwd_fp16(const void *x, int64_t x_row_stride, int64_t x
                                   y_batch_stride, batch, H, W, D, stream);
 }
 
+size_t sigma_dwconv3x3_silu_bwd_workspace_bytes(int batch, int H, int W, int D) {
+  if (batch <= 0 || H <= 0 || W <= 0 || D <= 0) return 0;
+  return dwconv3x3_silu_bwd_workspace_bytes(batch, H, W, D);
+}
+
+static int dwconv3x3_silu_bwd_any(const char *fn, int dtype, const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w,
+                                  const float *bias, const void *dy, int64_t dy_batch_stride, void *dx, int64_t dx_batch_stride, float *dw,
+                                  float *dbias, int batch, int H, int W, int D, void *workspace, size_t workspace_bytes, void *stream) {
+  const int q = dtype == SIGMA_F32 ? 4 : 8;   // elements per 16 bytes
+  SIGMA_CHECK_ARG(x && w && dy && dx && dw, "%s: null pointer", fn);
+  SIGMA_CHECK_ARG((bias == nullptr) == (dbias == nullptr), "%s: bias and dbias must be given together (or both NULL)", fn);
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % q == 0, "%s: bad sizes batch=%d H=%d W=%d D=%d (D %% %d == 0)", fn, batch,
+                  H, W, D, q);
+  SIGMA_CHECK_ARG(al16(x) && al16(dy) && al16(dx) && x_row_stride % q == 0 && x_batch_stride % q == 0 && dy_batch_stride % q == 0 &&
+                      dx_batch_stride % q == 0,
+                  "%s: x, dy, dx must be 16-byte aligned with strides multiples of %d elements (TMA)", fn, q);
+  const size_t need = dwconv3x3_silu_bwd_workspace_bytes(batch, H, W, D);
+  SIGMA_CHECK_ARG(workspace != nullptr && al16(workspace) && workspace_bytes >= need,
+                  "%s: needs %zu 16-byte aligned workspace bytes, got %zu", fn, need, workspace_bytes);
+  return dwconv3x3_silu_bwd_launch(dtype, x, x_row_stride, x_batch_stride, w, bias, dy, dy_batch_stride, dx, dx_batch_stride, dw, dbias,
+                                   batch, H, W, D, workspace, (cudaStream_t)stream);
+}
+
+int sigma_dwconv3x3_silu_bwd(const float *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
+                             const float *dy, int64_t dy_batch_stride, float *dx, int64_t dx_batch_stride, float *dw, float *dbias,
+                             int batch, int H, int W, int D, void *workspace, size_t workspace_bytes, void *stream) {
+  return dwconv3x3_silu_bwd_any("sigma_dwconv3x3_silu_bwd", SIGMA_F32, x, x_row_stride, x_batch_stride, w, bias, dy, dy_batch_stride, dx,
+                                dx_batch_stride, dw, dbias, batch, H, W, D, workspace, workspace_bytes, stream);
+}
+
+int sigma_dwconv3x3_silu_bwd_bf16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
+                                  const void *dy, int64_t dy_batch_stride, void *dx, int64_t dx_batch_stride, float *dw, float *dbias,
+                                  int batch, int H, int W, int D, void *workspace, size_t workspace_bytes, void *stream) {
+  return dwconv3x3_silu_bwd_any("sigma_dwconv3x3_silu_bwd_bf16", SIGMA_BF16, x, x_row_stride, x_batch_stride, w, bias, dy, dy_batch_stride,
+                                dx, dx_batch_stride, dw, dbias, batch, H, W, D, workspace, workspace_bytes, stream);
+}
+
+int sigma_dwconv3x3_silu_bwd_fp16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
+                                  const void *dy, int64_t dy_batch_stride, void *dx, int64_t dx_batch_stride, float *dw, float *dbias,
+                                  int batch, int H, int W, int D, void *workspace, size_t workspace_bytes, void *stream) {
+  return dwconv3x3_silu_bwd_any("sigma_dwconv3x3_silu_bwd_fp16", SIGMA_F16, x, x_row_stride, x_batch_stride, w, bias, dy, dy_batch_stride,
+                                dx, dx_batch_stride, dw, dbias, batch, H, W, D, workspace, workspace_bytes, stream);
+}
+
 int sigma_ss2d_padded_cp(int N, int R) {
   const int rp = pad_rp(R);
   return rp < 0 ? -1 : 2 * N + rp;

@@ -187,4 +187,285 @@ int dwconv3x3_silu_16bit_launch(int dtype, const void *x, long long x_row_stride
                                           y_batch_stride, batch, H, W, D, stream);
 }
 
+// ---- backward (training): y = SiLU(pre), pre = conv3x3(x) + b; dy -> dx, dw, db ----
+// The pre-activation is recomputed from x, so the forward saves nothing but x.  Per 8 x 16 output tile and 32-channel block, two
+// TMA boxes land in one ring slot: x with a 2-pixel halo (12 x 20) and dy with a 1-pixel halo (10 x 18).  Zero fill gives the
+// padding, and dy = 0 outside the image makes g = 0 there.  Then:
+//   phase 1: g = dy·s·(1 + pre·(1 − s)), s = sigmoid(pre), on the 10 x 18 one-halo region, fp32 in shared memory (in place of the dy
+//            box for fp32, whose size it has; a separate buffer for 16-bit dy);
+//   phase 2: dx = the transposed (flipped) stencil of g on the tile; dw[c, tap] += g·(x at the tap's shift) and db += g over the
+//            tile's own pixels, in registers.
+// x and dy are read once and dx written once (12 B per element in fp32, 6 B in 16-bit; halo re-reads hit L2).  Deterministic by
+// construction: each persistent CTA walks its tiles in a fixed order, sums its threads' dw / db in a fixed order into one partial
+// row of the workspace, and sum_parts_det_kernel adds the rows in order.  No float atomics.
+constexpr int DB_NSLOT = 2;                                     // two slots keep two CTAs per SM in fp32 (105 KB of ring each)
+constexpr int DB_XW = DC_TW + 4, DB_GW = DC_TW + 2;             // x box / g region widths
+constexpr int DB_XTILE = DC_CB * DB_XW * (DC_TH + 4);
+constexpr int DB_GTILE = DC_CB * DB_GW * (DC_TH + 2);           // = DC_TILE_FL
+constexpr int DB_UNITS = DC_THREADS / 8;                        // 16 pixel units per channel quad
+
+struct DwBwdParams {
+  CUtensorMap xmap, dymap;
+  const float *w, *bias;
+  void *dx;
+  float *part_w, *part_b;                                       // (gridDim.y, 9·D) and (gridDim.y, D) partial rows
+  long long dx_batch_stride;
+  int H, W, D, tiles_w, tiles_h;
+  long long ntiles;
+};
+
+__device__ __forceinline__ void fma4(float4 &a, float4 v, float4 k) {
+  const f2 lo = fma2(f2{v.x, v.y}, f2{k.x, k.y}, f2{a.x, a.y});
+  const f2 hi = fma2(f2{v.z, v.w}, f2{k.z, k.w}, f2{a.z, a.w});
+  a = make_float4(lo.x, lo.y, hi.x, hi.y);
+}
+
+__device__ __forceinline__ float silu_grad(float pre, float d) {
+  const float s = __fdividef(1.f, 1.f + ex2(-pre * kLog2e));
+  return d * s * fmaf(pre, 1.f - s, 1.f);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(DC_THREADS, 2) dwconv3x3_silu_bwd_tma_kernel(const __grid_constant__ DwBwdParams p) {
+  constexpr bool kGInPlace = sizeof(T) == sizeof(float);
+  constexpr int XB = DB_XTILE * (int)sizeof(T), SLOT = XB + DB_GTILE * (int)sizeof(T);
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  float *gsep = reinterpret_cast<float *>(smem_raw + DB_NSLOT * SLOT);
+  uint64_t *full = reinterpret_cast<uint64_t *>(smem_raw + DB_NSLOT * SLOT + (kGInPlace ? 0 : DB_GTILE * 4));
+  __shared__ __align__(16) float sw[9][DC_CB];
+  __shared__ __align__(16) float sb[DC_CB];
+
+  const int tid = threadIdx.x;
+  const int c0 = blockIdx.x * DC_CB;
+  for (int i = tid; i < 9 * DC_CB; i += blockDim.x) {
+    const int c = i / 9, tap = i - c * 9;
+    sw[tap][c] = (c0 + c < p.D) ? p.w[(long long)(c0 + c) * 9 + tap] : 0.f;
+  }
+  for (int i = tid; i < DC_CB; i += blockDim.x) sb[i] = (p.bias && c0 + i < p.D) ? p.bias[c0 + i] : 0.f;
+  if (tid == 0) {
+    for (int i = 0; i < DB_NSLOT; ++i) mbar_init(&full[i], 1);
+    fence_mbar_init();
+    tma_prefetch_desc(&p.xmap);
+    tma_prefetch_desc(&p.dymap);
+  }
+  __syncthreads();
+
+  const int cq = tid & 7, unit = tid >> 3;
+  const int wg = unit % (DC_TW / 4), hp = unit / (DC_TW / 4);   // phase 2: column group (4 pixels), row pair of the tile
+  const int gv = unit % 3, gu = unit / 3;                         // phase 1: column sextet, row pair of the g region (unit 15 idles)
+  float4 wt[9];
+#pragma unroll
+  for (int tap = 0; tap < 9; ++tap) wt[tap] = *reinterpret_cast<const float4 *>(&sw[tap][4 * cq]);
+  const float4 bv = *reinterpret_cast<const float4 *>(&sb[4 * cq]);
+  const int c = c0 + 4 * cq;
+  const long long tiles_per_img = (long long)p.tiles_w * p.tiles_h;
+  float4 dwa[9], dba = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int k = 0; k < 9; ++k) dwa[k] = dba;
+
+  auto issue = [&](long long t, int st) {
+    const int b = (int)(t / tiles_per_img);
+    const int r = (int)(t - (long long)b * tiles_per_img);
+    const int th = r / p.tiles_w, tw = r - th * p.tiles_w;
+    unsigned char *slot = smem_raw + st * SLOT;
+    mbar_arrive_expect_tx(&full[st], SLOT);
+    tma_load_4d(slot, &p.xmap, &full[st], c0, tw * DC_TW - 2, th * DC_TH - 2, b);
+    tma_load_4d(slot + XB, &p.dymap, &full[st], c0, tw * DC_TW - 1, th * DC_TH - 1, b);
+  };
+
+  long long t = blockIdx.y;
+  if (tid == 0)
+    for (int k = 0; k < DB_NSLOT - 1; ++k)
+      if (t + (long long)k * gridDim.y < p.ntiles) issue(t + (long long)k * gridDim.y, k);
+  int st = 0, ph = 0;
+  for (; t < p.ntiles; t += gridDim.y) {
+    const long long tn = t + (long long)(DB_NSLOT - 1) * gridDim.y;
+    // the slot of the previous tile was released by the barrier that ended its iteration
+    if (tid == 0 && tn < p.ntiles) issue(tn, st == 0 ? DB_NSLOT - 1 : st - 1);
+    mbar_wait(&full[st], (uint32_t)ph);
+
+    const T *xs = reinterpret_cast<const T *>(smem_raw + st * SLOT);
+    const T *dys = reinterpret_cast<const T *>(smem_raw + st * SLOT + XB);
+    float *g = kGInPlace ? reinterpret_cast<float *>(smem_raw + st * SLOT + XB) : gsep;
+
+    // phase 1: 2 rows x 6 columns of g per thread from a 4 x 8 window of x (each g element is read as dy and written as g by the
+    // same thread, so the in-place fp32 buffer has no hazard)
+    if (gu < (DC_TH + 2) / 2) {
+      float4 acc[2][6];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+        for (int j = 0; j < 6; ++j) acc[rr][j] = bv;
+      const T *xb = xs + ((2 * gu) * DB_XW + 6 * gv) * DC_CB + 4 * cq;
+#pragma unroll
+      for (int xr = 0; xr < 4; ++xr) {
+        float4 win[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) win[j] = ld4(xb + (xr * DB_XW + j) * DC_CB);
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int tr = xr - rr;
+          if (tr < 0 || tr > 2) continue;
+#pragma unroll
+          for (int j = 0; j < 6; ++j)
+#pragma unroll
+            for (int dxx = 0; dxx < 3; ++dxx) fma4(acc[rr][j], win[j + dxx], wt[tr * 3 + dxx]);
+        }
+      }
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+        for (int j = 0; j < 6; ++j) {
+          const int off = ((2 * gu + rr) * DB_GW + 6 * gv + j) * DC_CB + 4 * cq;
+          const float4 d = ld4(dys + off), a = acc[rr][j];
+          *reinterpret_cast<float4 *>(g + off) =
+              make_float4(silu_grad(a.x, d.x), silu_grad(a.y, d.y), silu_grad(a.z, d.z), silu_grad(a.w, d.w));
+        }
+      if (kGInPlace) fence_proxy_async();   // g overwrote the dy box by the generic proxy: order it before the slot's next TMA write
+    }
+    __syncthreads();
+
+    // phase 2: dx of 2 rows x 4 columns from a 4 x 6 window of g (flipped taps), keeping g of the thread's own pixels ...
+    const int b = (int)(t / tiles_per_img);
+    const int r = (int)(t - (long long)b * tiles_per_img);
+    const int th = r / p.tiles_w, tw = r - th * p.tiles_w;
+    float4 own[2][4], acc[2][4];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) acc[rr][j] = make_float4(0.f, 0.f, 0.f, 0.f);
+    const float *gb = g + ((2 * hp) * DB_GW + 4 * wg) * DC_CB + 4 * cq;
+#pragma unroll
+    for (int wr = 0; wr < 4; ++wr) {       // g row wr feeds output row rr with tap row 2 - (wr - rr)
+      float4 win[6];
+#pragma unroll
+      for (int j = 0; j < 6; ++j) win[j] = *reinterpret_cast<const float4 *>(gb + (wr * DB_GW + j) * DC_CB);
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        if (wr == rr + 1)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) own[rr][j] = win[j + 1];
+        const int rel = wr - rr;
+        if (rel < 0 || rel > 2) continue;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int dxx = 0; dxx < 3; ++dxx) fma4(acc[rr][j], win[j + dxx], wt[(2 - rel) * 3 + 2 - dxx]);
+      }
+    }
+    if (c < p.D) {
+      const int h0 = th * DC_TH + 2 * hp, w0 = tw * DC_TW + 4 * wg;
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int h = h0 + rr;
+        if (h >= p.H) continue;
+        T *dxb = reinterpret_cast<T *>(p.dx) + (long long)b * p.dx_batch_stride + ((long long)h * p.W + w0) * p.D + c;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (w0 + j < p.W) st4(dxb + (long long)j * p.D, acc[rr][j]);
+      }
+    }
+    // ... and dw / db of those pixels from a 4 x 6 window of x (x box row 2·hp + 1 + xr is tap row xr - rr of output row rr)
+    const T *xb = xs + ((2 * hp + 1) * DB_XW + 4 * wg + 1) * DC_CB + 4 * cq;
+#pragma unroll
+    for (int xr = 0; xr < 4; ++xr) {
+      float4 win[6];
+#pragma unroll
+      for (int j = 0; j < 6; ++j) win[j] = ld4(xb + (xr * DB_XW + j) * DC_CB);
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int tr = xr - rr;
+        if (tr < 0 || tr > 2) continue;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int dxx = 0; dxx < 3; ++dxx) fma4(dwa[tr * 3 + dxx], own[rr][j], win[j + dxx]);
+      }
+    }
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) dba = make_float4(dba.x + own[rr][j].x, dba.y + own[rr][j].y, dba.z + own[rr][j].z, dba.w + own[rr][j].w);
+    __syncthreads();   // every thread is done with slot st (and g) before either is written again
+    if (++st == DB_NSLOT) { st = 0; ph ^= 1; }
+  }
+
+  // the CTA's partial row: the 16 units' sums of each channel added in unit order, in the idle ring (every box issued was waited for)
+  float *red = reinterpret_cast<float *>(smem_raw);             // [unit][10][DC_CB]: taps 0..8, then db
+#pragma unroll
+  for (int k = 0; k < 9; ++k) *reinterpret_cast<float4 *>(&red[(unit * 10 + k) * DC_CB + 4 * cq]) = dwa[k];
+  *reinterpret_cast<float4 *>(&red[(unit * 10 + 9) * DC_CB + 4 * cq]) = dba;
+  __syncthreads();
+  for (int i = tid; i < 10 * DC_CB; i += blockDim.x) {
+    const int k = i / DC_CB, cc = i - k * DC_CB, ch = c0 + cc;
+    float s = 0.f;
+    for (int u = 0; u < DB_UNITS; ++u) s += red[(u * 10 + k) * DC_CB + cc];
+    if (ch < p.D) {
+      if (k < 9) p.part_w[(long long)blockIdx.y * 9 * p.D + (long long)ch * 9 + k] = s;
+      else if (p.part_b) p.part_b[(long long)blockIdx.y * p.D + ch] = s;
+    }
+  }
+}
+
+// the launch plan of the backward: persistent CTAs per channel block (gridDim.y), which is also the number of partial rows.  A
+// function of the shape alone, so the order of every sum is too.
+static int dwconv_bwd_parts(int batch, int H, int W, int D) {
+  const long long ntiles = (long long)batch * ((W + DC_TW - 1) / DC_TW) * ((H + DC_TH - 1) / DC_TH);
+  const int cblocks = (D + DC_CB - 1) / DC_CB;
+  return (int)std::max<long long>(1, std::min<long long>(ntiles, (long long)kNumSMs * 2 / cblocks));
+}
+
+size_t dwconv3x3_silu_bwd_workspace_bytes(int batch, int H, int W, int D) {
+  const size_t ny = (size_t)dwconv_bwd_parts(batch, H, W, D);
+  return align256(ny * 9 * D * sizeof(float)) + align256(ny * D * sizeof(float));
+}
+
+template <typename T>
+static int dwconv_bwd_tma_launch(const T *x, long long x_row_stride, long long x_batch_stride, const float *w, const float *bias,
+                                 const T *dy, long long dy_batch_stride, T *dx, long long dx_batch_stride, float *dw, float *db,
+                                 int batch, int H, int W, int D, void *ws, cudaStream_t stream) {
+  constexpr int es = (int)sizeof(T);
+  const CUtensorMapDataType dt = es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  // a runtime call before the tensor maps are encoded: it binds the device's context to the calling thread, which autograd's worker
+  // thread (a backward that starts at this node) does not have yet, and cuTensorMapEncodeTiled would fail there
+  const size_t smem = (size_t)DB_NSLOT * (DB_XTILE + DB_GTILE) * es + (es == 4 ? 0 : DB_GTILE * sizeof(float)) + 64;
+  SIGMA_CHECK_CUDA(cudaFuncSetAttribute(dwconv3x3_silu_bwd_tma_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  DwBwdParams p;
+  const uint64_t dims[4] = {(uint64_t)D, (uint64_t)W, (uint64_t)H, (uint64_t)batch};
+  const uint64_t xstr[3] = {(uint64_t)x_row_stride * es, (uint64_t)W * x_row_stride * es, (uint64_t)x_batch_stride * es};
+  const uint32_t xbox[4] = {DC_CB, DB_XW, DC_TH + 4, 1};
+  int rc = make_tmap(&p.xmap, dt, 4, x, dims, xstr, xbox, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+  if (rc) return rc;
+  const uint64_t ystr[3] = {(uint64_t)D * es, (uint64_t)W * D * es, (uint64_t)dy_batch_stride * es};
+  const uint32_t ybox[4] = {DC_CB, DB_GW, DC_TH + 2, 1};
+  if ((rc = make_tmap(&p.dymap, dt, 4, dy, dims, ystr, ybox, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
+  const int ny = dwconv_bwd_parts(batch, H, W, D);
+  p.w = w; p.bias = bias; p.dx = dx; p.dx_batch_stride = dx_batch_stride;
+  p.part_w = (float *)ws;
+  p.part_b = bias ? (float *)((char *)ws + align256((size_t)ny * 9 * D * sizeof(float))) : nullptr;
+  p.H = H; p.W = W; p.D = D;
+  p.tiles_w = (W + DC_TW - 1) / DC_TW;
+  p.tiles_h = (H + DC_TH - 1) / DC_TH;
+  p.ntiles = (long long)batch * p.tiles_w * p.tiles_h;
+  dwconv3x3_silu_bwd_tma_kernel<T><<<dim3((D + DC_CB - 1) / DC_CB, ny), DC_THREADS, smem, stream>>>(p);
+  SIGMA_CHECK_LAUNCH();
+  if ((rc = sum_parts_det_launch(p.part_w, ny, 9LL * D, 9LL * D, 0, dw, stream))) return rc;
+  return bias ? sum_parts_det_launch(p.part_b, ny, D, D, 0, db, stream) : SIGMA_OK;
+}
+
+int dwconv3x3_silu_bwd_launch(int dtype, const void *x, long long x_row_stride, long long x_batch_stride, const float *w,
+                              const float *bias, const void *dy, long long dy_batch_stride, void *dx, long long dx_batch_stride, float *dw,
+                              float *db, int batch, int H, int W, int D, void *ws, cudaStream_t stream) {
+  if (dtype == SIGMA_F32)
+    return dwconv_bwd_tma_launch<float>((const float *)x, x_row_stride, x_batch_stride, w, bias, (const float *)dy, dy_batch_stride,
+                                        (float *)dx, dx_batch_stride, dw, db, batch, H, W, D, ws, stream);
+  if (dtype == SIGMA_F16)
+    return dwconv_bwd_tma_launch<__half>((const __half *)x, x_row_stride, x_batch_stride, w, bias, (const __half *)dy, dy_batch_stride,
+                                         (__half *)dx, dx_batch_stride, dw, db, batch, H, W, D, ws, stream);
+  return dwconv_bwd_tma_launch<__nv_bfloat16>((const __nv_bfloat16 *)x, x_row_stride, x_batch_stride, w, bias,
+                                              (const __nv_bfloat16 *)dy, dy_batch_stride, (__nv_bfloat16 *)dx, dx_batch_stride, dw, db,
+                                              batch, H, W, D, ws, stream);
+}
+
 }  // namespace sigma

@@ -176,6 +176,11 @@ int dwconv3x3_silu_tma_launch(const float *x, long long x_row_stride, long long 
 // dtype: SIGMA_BF16 or SIGMA_F16 x and y
 int dwconv3x3_silu_16bit_launch(int dtype, const void *x, long long x_row_stride, long long x_batch_stride, const float *w,
                                 const float *bias, void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream);
+// backward: dtype SIGMA_F32, SIGMA_BF16 or SIGMA_F16 x, dy and dx; ws holds dwconv3x3_silu_bwd_workspace_bytes (16-byte aligned)
+size_t dwconv3x3_silu_bwd_workspace_bytes(int batch, int H, int W, int D);
+int dwconv3x3_silu_bwd_launch(int dtype, const void *x, long long x_row_stride, long long x_batch_stride, const float *w,
+                              const float *bias, const void *dy, long long dy_batch_stride, void *dx, long long dx_batch_stride, float *dw,
+                              float *db, int batch, int H, int W, int D, void *ws, cudaStream_t stream);
 
 // ---- gemm_tf32.cu ----
 // tf32x3 (W_lo != nullptr) stores its output tiles with TMA; reg_epilogue = true stores them from registers instead (the

@@ -209,8 +209,7 @@ class SS2D(nn.Module):
             # training through the fused core (f1): conv on the channels_last view, then x_proj + 4-direction scan + CrossMerge as
             # ONE autograd node over channels-last tensors (no CrossScan / delta / CrossMerge copies in either direction)
             B, H, W, _ = x.shape
-            xi = self.act(self.conv2d(xi.permute(0, 3, 1, 2)))                       # (B,D,H,W), channels_last memory
-            xc = xi.permute(0, 2, 3, 1).reshape(B, H * W, self.d_inner)
+            xc = ops.DwConvSiLUFn.apply(xi, self.conv2d.weight, self.conv2d.bias)   # (B, H·W, D), xi read in place
             y = ops.FusedSS2DCore.apply(xc, self.x_proj_weight, self.dt_projs_weight, self.dt_projs_bias, self.A_logs, self.Ds,
                                         _lib_kinds()[0], H, W)
             y = ops.layer_norm(self.out_norm, y.view(B, H, W, self.d_inner)).to(x.dtype) * F.silu(z)
@@ -272,22 +271,26 @@ class ConMB_SS2D(nn.Module):
         if _fused_block_ok(self, x_rgb, x_e) and isinstance(self.dropout, nn.Identity):
             from . import fused
             return fused.conmb_ss2d(self, x_rgb, x_e, residual=residual)
-        t_r = self.in_proj(x_rgb).permute(0, 3, 1, 2).contiguous()
-        t_e = self.in_proj_modalx(x_e).permute(0, 3, 1, 2).contiguous()
         if ops.fused_core_ok(x_rgb, self.d_inner, self.d_state):
-            # training through the fused core (f1), kind SEQ2: [rgb ‖ x] along L, forward + reversed scan, merged
+            # training through the fused core (f1), kind SEQ2: [rgb ‖ x] along L, forward + reversed scan, merged; channels-last
+            # throughout (the conv + SiLU nodes read the in_proj outputs in place)
             B, H, W, _ = x_rgb.shape
             D, L = self.d_inner, H * W
-            c_r = self.act(self.conv2d(t_r)).permute(0, 2, 3, 1).reshape(B, L, D)
-            c_e = self.act(self.conv2d_modalx(t_e)).permute(0, 2, 3, 1).reshape(B, L, D)
+            t_r, t_e = self.in_proj(x_rgb), self.in_proj_modalx(x_e)                                            # (B, H, W, D)
+            c_r = ops.DwConvSiLUFn.apply(t_r, self.conv2d.weight, self.conv2d.bias)
+            c_e = ops.DwConvSiLUFn.apply(t_e, self.conv2d_modalx.weight, self.conv2d_modalx.bias)
             ys = ops.FusedSS2DCore.apply(torch.cat([c_r, c_e], dim=1), self.x_proj_weight, self.dt_projs_weight, self.dt_projs_bias,
                                          self.A_logs, self.Ds, _lib_kinds()[1], H, W)                          # (B, 2L, D)
             y_r = ops.layer_norm(self.out_norm1, ys[:, :L].reshape(B, H, W, D)).to(x_rgb.dtype)
             y_e = ops.layer_norm(self.out_norm2, ys[:, L:].reshape(B, H, W, D)).to(x_e.dtype)
+            hw = (1, 2)
         else:
+            t_r = self.in_proj(x_rgb).permute(0, 3, 1, 2).contiguous()
+            t_e = self.in_proj_modalx(x_e).permute(0, 3, 1, 2).contiguous()
             y_r, y_e = self.forward_corev2_multimodal(self.act(self.conv2d(t_r)), self.act(self.conv2d_modalx(t_e)))
-        g_r = self.fc1(t_r.mean(dim=(2, 3)))          # gates come from the PRE-conv projections (vmamba.py:1276-1279)
-        g_e = self.fc2(t_e.mean(dim=(2, 3)))
+            hw = (2, 3)
+        g_r = self.fc1(t_r.mean(dim=hw))             # gates come from the PRE-conv projections (vmamba.py:1276-1279)
+        g_e = self.fc2(t_e.mean(dim=hw))
         y = torch.cat([y_r * g_e[:, None, None, :], y_e * g_r[:, None, None, :]], dim=-1)  # cross-applied (:1280-1281)
         out = self.dropout(self.out_proj(y))
         return out if residual is None else residual + out
@@ -374,7 +377,7 @@ class CrossMambaFusion_SS2D_SSM(nn.Module):
             from . import _lib
             D, cm = self.d_inner, self.CMA_ssm
             t = torch.cat([self.in_proj(x_rgb), self.in_proj_modalx(x_e)], dim=0)             # (2B, H, W, D)
-            xc = self.act(self.conv2d(t.permute(0, 3, 1, 2))).permute(0, 2, 3, 1).reshape(2 * B, H * W, D)   # one shared conv
+            xc = ops.DwConvSiLUFn.apply(t, self.conv2d.weight, self.conv2d.bias)                # one shared conv over 2B images
             y = ops.FusedSS2DCore.apply(xc, torch.stack([cm.x_proj_1.weight, cm.x_proj_2.weight]),
                                         torch.stack([cm.dt_proj_1.weight, cm.dt_proj_2.weight]),
                                         torch.stack([cm.dt_proj_1.bias, cm.dt_proj_2.bias]), torch.cat([cm.A_log_1, cm.A_log_2]),

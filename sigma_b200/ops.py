@@ -472,6 +472,65 @@ def layer_norm(norm, x):
     return norm(x)
 
 
+_DWCONV_FWD = {torch.float32: "sigma_dwconv3x3_silu_fwd", torch.bfloat16: "sigma_dwconv3x3_silu_fwd_bf16",
+               torch.float16: "sigma_dwconv3x3_silu_fwd_fp16"}
+_DWCONV_BWD = {torch.float32: "sigma_dwconv3x3_silu_bwd", torch.bfloat16: "sigma_dwconv3x3_silu_bwd_bf16",
+               torch.float16: "sigma_dwconv3x3_silu_bwd_fp16"}
+
+
+def _rows_ok(t, row_stride):
+    """t (B, ..., D) can be passed as rows `row_stride` elements apart with a batch stride: unit channel stride and 16-byte aligned
+    pointer and strides, as the library's TMA maps need"""
+    q = 16 // t.element_size()
+    return t.stride(-1) == 1 and t.data_ptr() % 16 == 0 and row_stride % q == 0 and t.stride(0) % q == 0
+
+
+class DwConvSiLUFn(torch.autograd.Function):
+    """SiLU(nn.Conv2d(D, D, 3, padding=1, groups=D)(x)) of a channels-last activation under autograd: x (B, H, W, D), whose pixel rows
+    may be a strided view (the x half of in_proj's [x | z] output) -> xc (B, H·W, D) in x's dtype (fp32, bf16 or fp16).  Forward =
+    sigma_dwconv3x3_silu_fwd[_bf16|_fp16] with the fp32 weights as given (autocast is off inside, so it does not cast them); backward
+    = sigma_dwconv3x3_silu_bwd[_bf16|_fp16], which recomputes the pre-activation from x, so the node saves nothing but x.  dweight and
+    dbias are fp32 in the parameters' shapes.  The backward is deterministic by construction: one kernel with or without
+    torch.use_deterministic_algorithms(True)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        B, H, W, D = x.shape
+        if x.dtype not in _DWCONV_FWD or weight.shape != (D, 1, 3, 3) or weight.dtype != torch.float32 or \
+                (bias is not None and bias.dtype != torch.float32):
+            raise RuntimeError(f"DwConvSiLUFn: a 3x3 depthwise conv with fp32 weights over fp32 / bf16 / fp16 x, got x {x.dtype}, "
+                               f"weight {tuple(weight.shape)} {weight.dtype}")
+        if not (_rows_ok(x, x.stride(2)) and x.stride(1) == W * x.stride(2)):
+            x = x.contiguous()
+        w = weight.contiguous()
+        b = bias.contiguous() if bias is not None else None
+        y = torch.empty((B, H * W, D), dtype=x.dtype, device=x.device)
+        fn = _DWCONV_FWD[x.dtype]
+        with torch.autocast("cuda", enabled=False):
+            _lib.check(getattr(_lib.lib(), fn)(ptr(x), x.stride(2), x.stride(0), ptr(w), ptr(b), ptr(y), H * W * D, B, H, W, D, stream()),
+                       fn)
+        ctx.save_for_backward(x, w, b)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, b = ctx.saved_tensors
+        B, H, W, D = x.shape
+        dy = dy.to(x.dtype)
+        if not (_rows_ok(dy, D) and dy.stride(1) == D):
+            dy = dy.contiguous()                 # a slice of the (B, 2L, D) core gradient (ConMB) passes as it is
+        dx = torch.empty((B, H, W, D), dtype=x.dtype, device=x.device)
+        dw = torch.empty_like(w)
+        db = torch.empty_like(b) if b is not None else None
+        L_ = _lib.lib()
+        wsb = L_.sigma_dwconv3x3_silu_bwd_workspace_bytes(B, H, W, D)
+        ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+        fn = _DWCONV_BWD[x.dtype]
+        _lib.check(getattr(L_, fn)(ptr(x), x.stride(2), x.stride(0), ptr(w), ptr(b), ptr(dy), dy.stride(0), ptr(dx), H * W * D, ptr(dw),
+                                   ptr(db), B, H, W, D, ptr(ws), wsb, stream()), fn)
+        return dx, dw, db
+
+
 _SAVED_BF16 = 2               # `saved` of _call_ss2d_bwd: the arguments are those of sigma_ss2d_scan_bwd_saved_bf16
 _SAVED_FP16 = 3               # ... of sigma_ss2d_scan_bwd_saved_fp16 (the same layout)
 
