@@ -10,7 +10,7 @@ Operations (x a row of D channels; every kernel normalises with a divisor of D):
   head_ref64          the (NCLS, C) 1x1 projection of upsample2x_norm_ref64, NCHW
   pool_avgmax_ref64, pool_partial_ref64, scale_add_ref64, layernorm_bwd_ref64 (dx, dgamma, dbeta)
 
-Lane layouts (*_plan, mirroring rowwise.cu's dispatch; tests/test_rowwise_ref64_cpu.py checks the tables against the source):
+Lane layouts (*_plan, mirroring rowwise.cu's dispatch; tests/test_rowwise_ref64_cpu.py checks the tables against the built library):
 a row is held by LPR lanes with V float4 each (fast kernels, D = 4·LPR·V) or by the 32 lanes of a warp with MAXV float4 slots
 (generic kernels).  Lane l holds float4 number l + LPR·v.
 
@@ -46,7 +46,7 @@ rounded once, and a compiler-contracted FMA rounds less often than the separate 
 Every first-order bound is multiplied by SAFETY = 1.25 for the second-order products of the itemised errors (each below 1e-4 of
 the first-order total on these inputs).  Every bound is per element; none is a fraction of a tensor's maximum.
 
-bf16 instances (RowNormParams::io = 1: fp32 in, bf16 out; io = 2: bf16 y / z in, bf16 out; layernorm_bwd with bf16 x, dy, dx;
+bf16 instances (element pairs (f32, bf16): fp32 in, bf16 out; (bf16, bf16): bf16 y / z in, bf16 out; layernorm_bwd with bf16 x, dy, dx;
 dwconv3x3_silu_tma_kernel<__nv_bfloat16>).  Every bf16 operand is widened exactly and all arithmetic is the fp32 kernel's, so the
 inputs are rounded to bf16 first and the reference and its fp32 bound e are computed from those exact values: operand rounding
 never enters the comparison.  A bf16 store rounds the kernel's fp32 value v, |v - ref| <= e, to nearest even, which moves it by at
@@ -70,13 +70,26 @@ NUM_SMS = 132             # kNumSMs of common.cuh: the grid caps of layernorm_bw
 # rowwise.cu's instantiation tables: (lanes per row, float4 per lane)
 ROW_FAST = [(8, 2), (8, 3), (8, 4), (16, 3), (16, 4), (32, 3), (32, 4), (32, 6), (32, 8), (32, 12), (32, 16)]
 ROW_FAST_K = (1, 2, 4)
-# row_norm_fast_k's dispatch per io (0: fp32, 1: fp32 in / bf16 out, 2: bf16 in and out): mode -> the K with a fast instance
-ROW_FAST_IO = {0: {0: ROW_FAST_K, 1: (1,), 2: (1,)}, 1: {0: (1,), 1: (1,)}, 2: {0: ROW_FAST_K}}
+MAXV_GENERIC = (1, 2, 4, 8, 16, 32)
+# row_norm_launch's dispatch per element pair (y / z, out): mode -> the K with a fast instance, and the generic kernel's float4
+# slots per lane (plain rows only, D <= 128·MAXV; e4m3 output holds the whole row in registers and stops at MAXV 8)
+ROW_FAST_PAIRS = {
+    ("f32", "f32"): {0: ROW_FAST_K, 1: (1,), 2: (1,)},
+    ("f32", "bf16"): {0: (1,), 1: (1,)},
+    ("f32", "f16"): {0: (1,), 1: (1,)},
+    ("f32", "e4m3"): {0: (1,), 1: (1,)},
+    ("bf16", "bf16"): {0: ROW_FAST_K},
+    ("f16", "f16"): {0: ROW_FAST_K},
+    ("bf16", "e4m3"): {0: (1, 4)},
+}
+ROW_GENERIC_MAXV = {pair: MAXV_GENERIC[:4] if pair[1] == "e4m3" else MAXV_GENERIC for pair in ROW_FAST_PAIRS}
+ROW_E4M3_K = (1, 4)        # the only K of e4m3 output, fast or generic
+# the integer element labels of tests/test_rowwise_fp64_gpu.py
+IO_PAIRS = {0: ("f32", "f32"), 1: ("f32", "bf16"), 2: ("bf16", "bf16")}
 HEAD_FAST = [(8, 2), (8, 3), (8, 4), (16, 3), (16, 4)]
 HEAD_FAST_MAX_NCLS = 24
 HEAD_NCLS = [2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 16, 19, 20, 21, 37, 40, 41]
 BWD_FAST = [(8, 1), (8, 2), (8, 3), (8, 4), (16, 3), (16, 4), (32, 3), (32, 4), (32, 6), (32, 8), (32, 12)]
-MAXV_GENERIC = (1, 2, 4, 8, 16, 32)
 
 
 # ---------------------------------------------------------------- launch plans (lane layouts)
@@ -89,14 +102,17 @@ def _maxv(nvec, cap=32):
 
 def row_plan(D, K=1, mode=0, io=0):
     """(lanes, float4 per lane, fast) of row_norm_launch for D channels, K directions, mode 0 / 1 (gather) / 2 (pixel shuffle) and
-    element types io (ROW_FAST_IO)"""
+    element pair io (a key of ROW_FAST_PAIRS, or an IO_PAIRS label)"""
+    pair = IO_PAIRS.get(io, io)
+    if pair[1] == "e4m3" and K not in ROW_E4M3_K:
+        raise ValueError(f"e4m3 output: K={K} has no instantiation")
     nvec = D // 4
     for lpr, v in ROW_FAST:
-        if nvec == lpr * v and K in ROW_FAST_IO[io].get(mode, ()):
+        if nvec == lpr * v and K in ROW_FAST_PAIRS[pair].get(mode, ()):
             return lpr, v, True
     if mode != 0:
         raise ValueError(f"mode {mode}: D={D} has no fast instantiation")
-    return 32, _maxv(nvec), False
+    return 32, _maxv(nvec, cap=ROW_GENERIC_MAXV[pair][-1]), False
 
 
 def head_plan(C, ncls):

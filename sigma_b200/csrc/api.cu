@@ -316,69 +316,91 @@ int sigma_test_scan_plan(int sweep, int batch, int dim, int seqlen, int dstate, 
 namespace sigma {
 static bool al16(const void *p) { return ((uintptr_t)p & 15) == 0; }
 static bool al8(const void *p) { return ((uintptr_t)p & 7) == 0; }
+// The row norms and the depthwise conv's output move 4 elements at a time: a pointer to elements of type t (SIGMA_F32,
+// SIGMA_BF16, SIGMA_F16 or SIGMA_E4M3_ROWS) is aligned to 4 of them, 16 bytes for fp32, 8 for 16-bit and 4 for e4m3.  NULL passes.
+static bool al4(const void *p, int t) {
+  const uintptr_t bytes = t == SIGMA_F32 ? 16 : t == SIGMA_E4M3_ROWS ? 4 : 8;
+  return ((uintptr_t)p & (bytes - 1)) == 0;
+}
+
+// The row-norm entry points share one checked body per operation shape.  fn names the entry point in every message; ti / to are
+// the element types of the input rows (and z) and of the output.  e4m3 output (to = SIGMA_E4M3_ROWS) also writes each row's fp32
+// scale to `scale`.  gamma, beta and gate are fp32.  Every check runs before the first CUDA call.
+
+// LayerNorm of (rows, C) rows
+static int layernorm_rows(const char *fn, int ti, int to, const void *x, const float *w, const float *b, void *y, float *scale,
+                          int64_t rows, int C, float eps, void *stream) {
+  SIGMA_CHECK_ARG(x && w && b && y && (to != SIGMA_E4M3_ROWS || scale), "%s: null pointer", fn);
+  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "%s: C=%d must be a positive multiple of 4", fn, C);
+  SIGMA_CHECK_ARG(al4(x, ti) && al16(w) && al16(b) && al4(y, to), "%s: x, y must be aligned to 4 elements and w, b to 16 bytes", fn);
+  RowNormParams p{(const float *)x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
+  p.qscale = scale;
+  return row_norm_launch(ti, to, p, (cudaStream_t)stream);
+}
+
+// LayerNorm of an fp32 (batch, H, W, C) image's rows gathered by mode: 1 = PatchMerging2D's 2x2 blocks, rows of 4C; 2 = PatchExpand's
+// pixel shuffle, each pixel's 4C channels as 4 rows of C stored at (batch, 2H, 2W, C)
+static int layernorm_image(const char *fn, int mode, int to, const float *x, const float *w, const float *b, void *y, float *scale,
+                           int batch, int H, int W, int C, float eps, void *stream) {
+  SIGMA_CHECK_ARG(x && w && b && y && (to != SIGMA_E4M3_ROWS || scale), "%s: null pointer", fn);
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "%s: bad sizes", fn);
+  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al4(y, to), "%s: x, w, b must be 16-byte and y 4-element aligned", fn);
+  const int64_t rows = mode == 1 ? (int64_t)batch * ((H + 1) / 2) * ((W + 1) / 2) : (int64_t)batch * H * W * 4;
+  const int D = mode == 1 ? 4 * C : C;
+  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows, 0, 0, D, D, eps};
+  p.mode = mode; p.gH = H; p.gW = W; p.qscale = scale;
+  return row_norm_launch(SIGMA_F32, to, p, (cudaStream_t)stream);
+}
+
+// sum of K direction slabs -> LayerNorm [· SiLU(z)] [· gate]; e4m3 output merges K = 1 or 4 slabs
+static int merge_norm_gate(const char *fn, int ti, int to, const void *y, int K, int64_t k_stride, int64_t in_batch_stride,
+                           const float *gamma, const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *out,
+                           float *scale, int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch, int D,
+                           float eps, void *stream) {
+  const bool e4m3 = to == SIGMA_E4M3_ROWS;
+  SIGMA_CHECK_ARG(y && gamma && beta && out && (!e4m3 || scale), "%s: null pointer", fn);
+  SIGMA_CHECK_ARG((e4m3 ? K == 1 || K == 4 : K >= 1 && K <= 8) && D > 0 && D % 4 == 0 && rows >= 0 && rows_per_batch > 0,
+                  "%s: bad sizes K=%d (%s) D=%d rows=%lld rows_per_batch=%lld", fn, K, e4m3 ? "1 or 4" : "1 to 8", D, (long long)rows,
+                  (long long)rows_per_batch);
+  SIGMA_CHECK_ARG(al4(y, ti) && al4(z, ti) && al4(out, to) && al16(gamma) && al16(beta) && al16(gate) && k_stride % 4 == 0 &&
+                      in_batch_stride % 4 == 0 && out_batch_stride % 4 == 0 && out_row_stride % 4 == 0 && z_row_stride % 4 == 0,
+                  "%s: y / z / out must be 4-element and gamma / beta / gate 16-byte aligned, strides multiples of 4", fn);
+  RowNormParams p{(const float *)y, k_stride, K, gamma, beta, (const float *)z, z_row_stride, gate, (float *)out, rows, rows_per_batch,
+                  in_batch_stride, out_batch_stride, out_row_stride, D, eps};
+  p.qscale = scale;
+  return row_norm_launch(ti, to, p, (cudaStream_t)stream);
+}
+
+// LayerNorm backward, x / dy / dx of element type dtype; det: the deterministic build in `workspace`
+static int layernorm_bwd_checked(const char *fn, int dtype, const void *x, const void *dy, const float *w, void *dx, float *dw, float *db,
+                                 int64_t rows, int C, float eps, void *stream, bool det = false, void *workspace = nullptr,
+                                 size_t workspace_bytes = 0) {
+  SIGMA_CHECK_ARG(x && dy && w && dx && dw && db, "%s: null pointer", fn);
+  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "%s: C=%d must be a positive multiple of 4", fn, C);
+  SIGMA_CHECK_ARG(al4(x, dtype) && al4(dy, dtype) && al4(dx, dtype) && al16(w), "%s: x, dy, dx must be 4-element and w 16-byte aligned",
+                  fn);
+  if (det) {
+    const size_t need = layernorm_bwd_det_workspace_bytes(rows, C);
+    SIGMA_CHECK_ARG(workspace != nullptr && al16(workspace) && workspace_bytes >= need,
+                    "%s: needs %zu 16-byte aligned workspace bytes, got %zu", fn, need, workspace_bytes);
+  }
+  return layernorm_bwd_launch(dtype, x, dy, w, dx, dw, db, rows, C, eps, (cudaStream_t)stream, det ? (float *)workspace : nullptr);
+}
+
+static int dwconv3x3_silu_fwd_any(const char *fn, int dtype, const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w,
+                                  const float *bias, void *y, int64_t y_batch_stride, int batch, int H, int W, int D, void *stream) {
+  const int q = dtype == SIGMA_F32 ? 4 : 8;   // elements per 16 bytes
+  SIGMA_CHECK_ARG(x && w && y, "%s: null pointer", fn);
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % 4 == 0, "%s: bad sizes", fn);
+  SIGMA_CHECK_ARG(al16(x) && al4(y, dtype) && x_row_stride % q == 0 && x_batch_stride % q == 0 && y_batch_stride % 4 == 0,
+                  "%s: x must be 16-byte aligned with strides multiples of %d elements (TMA), y 4-element aligned", fn, q);
+  return dwconv3x3_silu_fwd_launch(dtype, x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D,
+                                   (cudaStream_t)stream);
+}
 }  // namespace sigma
 
 extern "C" {
 #pragma GCC visibility push(default)
-
-int sigma_layernorm_fwd(const float *x, const float *w, const float *b, float *y, int64_t rows, int C, float eps,
-                        void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && y, "sigma_layernorm_fwd: null pointer");
-  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd: C=%d must be a positive multiple of 4", C);
-  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al16(y), "sigma_layernorm_fwd: pointers must be 16-byte aligned");
-  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
-  return row_norm_launch(p, (cudaStream_t)stream);
-}
-
-// The bf16 and fp16 twins of one entry point share a body: `fn` names the entry point in its error strings, dtype (SIGMA_BF16 or
-// SIGMA_F16) is the 16-bit element type.
-static int layernorm_fwd_16bit(const char *fn, int dtype, const float *x, const float *w, const float *b, void *y, int64_t rows, int C,
-                               float eps, void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && y, "%s: null pointer", fn);
-  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "%s: C=%d must be a positive multiple of 4", fn, C);
-  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al8(y), "%s: x, w, b must be 16-byte and y 8-byte aligned", fn);
-  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
-  p.io = dtype == SIGMA_F16 ? 5 : 1;
-  return row_norm_launch(p, (cudaStream_t)stream);
-}
-
-static int patch_merge_norm_fwd_16bit(const char *fn, int dtype, const float *x, const float *w, const float *b, void *y, int batch, int H,
-                                      int W, int C, float eps, void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && y, "%s: null pointer", fn);
-  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "%s: bad sizes", fn);
-  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al8(y), "%s: x, w, b must be 16-byte and y 8-byte aligned", fn);
-  const int64_t rows = (int64_t)batch * ((H + 1) / 2) * ((W + 1) / 2);
-  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows, 0, 0, 4 * C, 4 * C, eps};
-  p.mode = 1; p.gH = H; p.gW = W; p.io = dtype == SIGMA_F16 ? 5 : 1;
-  return row_norm_launch(p, (cudaStream_t)stream);
-}
-
-static int merge_norm_gate_fwd_16bit(const char *fn, int dtype, const void *y, int K, int64_t k_stride, int64_t in_batch_stride,
-                                     const float *gamma, const float *beta, const void *z, int64_t z_row_stride, const float *gate,
-                                     void *out, int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
-                                     int D, float eps, void *stream) {
-  SIGMA_CHECK_ARG(y && gamma && beta && out, "%s: null pointer", fn);
-  SIGMA_CHECK_ARG(K >= 1 && K <= 8 && D > 0 && D % 4 == 0 && rows >= 0 && rows_per_batch > 0,
-                  "%s: bad sizes K=%d D=%d rows=%lld rows_per_batch=%lld", fn, K, D, (long long)rows, (long long)rows_per_batch);
-  SIGMA_CHECK_ARG(al8(y) && al16(gamma) && al16(beta) && al8(out) && al8(z) && al16(gate) && k_stride % 4 == 0 &&
-                      in_batch_stride % 4 == 0 && out_batch_stride % 4 == 0 && out_row_stride % 4 == 0 && z_row_stride % 4 == 0,
-                  "%s: y / z / out must be 8-byte and gamma / beta / gate 16-byte aligned, strides multiples of 4", fn);
-  RowNormParams p{(const float *)y, k_stride, K, gamma, beta, (const float *)z, z_row_stride, gate, (float *)out, rows, rows_per_batch,
-                  in_batch_stride, out_batch_stride, out_row_stride, D, eps};
-  p.io = dtype == SIGMA_F16 ? 6 : 2;
-  return row_norm_launch(p, (cudaStream_t)stream);
-}
-
-static int dwconv3x3_silu_fwd_16bit(const char *fn, int dtype, const void *x, int64_t x_row_stride, int64_t x_batch_stride,
-                                    const float *w, const float *bias, void *y, int64_t y_batch_stride, int batch, int H, int W, int D,
-                                    void *stream) {
-  SIGMA_CHECK_ARG(x && w && y, "%s: null pointer", fn);
-  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % 4 == 0, "%s: bad sizes", fn);
-  SIGMA_CHECK_ARG(al16(x) && al8(y) && x_row_stride % 8 == 0 && x_batch_stride % 8 == 0 && y_batch_stride % 4 == 0,
-                  "%s: x must be 16-byte aligned with strides multiples of 8 elements (TMA), y 8-byte aligned", fn);
-  return dwconv3x3_silu_16bit_launch(dtype, x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D,
-                                     (cudaStream_t)stream);
-}
 
 static int linear_16bit(const char *fn, int dtype, const void *A, int64_t lda, const void *W, const float *bias, const float *residual,
                         int64_t ldr, const float *rscale, void *C, int64_t ldc, int c_dtype, int64_t M, int N, int K, void *stream) {
@@ -393,65 +415,46 @@ static int linear_16bit(const char *fn, int dtype, const void *A, int64_t lda, c
   return gemm_16bit_launch(dtype, A, lda, W, bias, residual, ldr, rscale, C, ldc, c_dtype == dtype, M, N, K, (cudaStream_t)stream);
 }
 
+int sigma_layernorm_fwd(const float *x, const float *w, const float *b, float *y, int64_t rows, int C, float eps,
+                        void *stream) {
+  return layernorm_rows("sigma_layernorm_fwd", SIGMA_F32, SIGMA_F32, x, w, b, y, nullptr, rows, C, eps, stream);
+}
+
 int sigma_layernorm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
-  return layernorm_fwd_16bit("sigma_layernorm_fwd_bf16", SIGMA_BF16, x, w, b, y, rows, C, eps, stream);
+  return layernorm_rows("sigma_layernorm_fwd_bf16", SIGMA_F32, SIGMA_BF16, x, w, b, y, nullptr, rows, C, eps, stream);
 }
 
 int sigma_layernorm_fwd_fp16(const float *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
-  return layernorm_fwd_16bit("sigma_layernorm_fwd_fp16", SIGMA_F16, x, w, b, y, rows, C, eps, stream);
+  return layernorm_rows("sigma_layernorm_fwd_fp16", SIGMA_F32, SIGMA_F16, x, w, b, y, nullptr, rows, C, eps, stream);
 }
 
 int sigma_layernorm_fwd_fp8(const float *x, const float *w, const float *b, void *q, float *scale, int64_t rows, int C, float eps,
                             void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && q && scale, "sigma_layernorm_fwd_fp8: null pointer");
-  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd_fp8: C=%d must be a positive multiple of 4", C);
-  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && ((uintptr_t)q & 3) == 0, "sigma_layernorm_fwd_fp8: x, w, b must be 16-byte and q 4-byte aligned");
-  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)q, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
-  p.io = 3; p.qscale = scale;
-  return row_norm_launch(p, (cudaStream_t)stream);
+  return layernorm_rows("sigma_layernorm_fwd_fp8", SIGMA_F32, SIGMA_E4M3_ROWS, x, w, b, q, scale, rows, C, eps, stream);
 }
 
 int sigma_layernorm_fwd_bf16io(const void *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && y, "sigma_layernorm_fwd_bf16io: null pointer");
-  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd_bf16io: C=%d must be a positive multiple of 4", C);
-  SIGMA_CHECK_ARG(al8(x) && al16(w) && al16(b) && al8(y), "sigma_layernorm_fwd_bf16io: w, b must be 16-byte and x, y 8-byte aligned");
-  RowNormParams p{(const float *)x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
-  p.io = 2;
-  return row_norm_launch(p, (cudaStream_t)stream);
-}
-
-int sigma_layernorm_bwd_bf16(const void *x, const void *dy, const float *w, void *dx, float *dw, float *db, int64_t rows, int C, float eps,
-                             void *stream) {
-  SIGMA_CHECK_ARG(x && dy && w && dx && dw && db, "sigma_layernorm_bwd_bf16: null pointer");
-  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_bwd_bf16: C=%d must be a positive multiple of 4", C);
-  SIGMA_CHECK_ARG(al8(x) && al8(dy) && al16(w) && al8(dx), "sigma_layernorm_bwd_bf16: w must be 16-byte and x, dy, dx 8-byte aligned");
-  return layernorm_bwd_launch((const float *)x, (const float *)dy, w, (float *)dx, dw, db, rows, C, eps, (cudaStream_t)stream, nullptr, SIGMA_BF16);
+  return layernorm_rows("sigma_layernorm_fwd_bf16io", SIGMA_BF16, SIGMA_BF16, x, w, b, y, nullptr, rows, C, eps, stream);
 }
 
 // the fp16 training mode: x and y fp16 (merge + norm + gate's fp16 in / out instance with one input and no gate)
 int sigma_layernorm_fwd_fp16io(const void *x, const float *w, const float *b, void *y, int64_t rows, int C, float eps, void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && y, "sigma_layernorm_fwd_fp16io: null pointer");
-  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_fwd_fp16io: C=%d must be a positive multiple of 4", C);
-  SIGMA_CHECK_ARG(al8(x) && al16(w) && al16(b) && al8(y), "sigma_layernorm_fwd_fp16io: w, b must be 16-byte and x, y 8-byte aligned");
-  RowNormParams p{(const float *)x, 0, 1, w, b, nullptr, 0, nullptr, (float *)y, rows, rows > 0 ? rows : 1, 0, 0, C, C, eps};
-  p.io = 6;
-  return row_norm_launch(p, (cudaStream_t)stream);
-}
-
-int sigma_layernorm_bwd_fp16(const void *x, const void *dy, const float *w, void *dx, float *dw, float *db, int64_t rows, int C, float eps,
-                             void *stream) {
-  SIGMA_CHECK_ARG(x && dy && w && dx && dw && db, "sigma_layernorm_bwd_fp16: null pointer");
-  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_bwd_fp16: C=%d must be a positive multiple of 4", C);
-  SIGMA_CHECK_ARG(al8(x) && al8(dy) && al16(w) && al8(dx), "sigma_layernorm_bwd_fp16: w must be 16-byte and x, dy, dx 8-byte aligned");
-  return layernorm_bwd_launch((const float *)x, (const float *)dy, w, (float *)dx, dw, db, rows, C, eps, (cudaStream_t)stream, nullptr, SIGMA_F16);
+  return layernorm_rows("sigma_layernorm_fwd_fp16io", SIGMA_F16, SIGMA_F16, x, w, b, y, nullptr, rows, C, eps, stream);
 }
 
 int sigma_layernorm_bwd(const float *x, const float *dy, const float *w, float *dx, float *dw, float *db, int64_t rows, int C, float eps,
                         void *stream) {
-  SIGMA_CHECK_ARG(x && dy && w && dx && dw && db, "sigma_layernorm_bwd: null pointer");
-  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_bwd: C=%d must be a positive multiple of 4", C);
-  SIGMA_CHECK_ARG(al16(x) && al16(dy) && al16(w) && al16(dx), "sigma_layernorm_bwd: pointers must be 16-byte aligned");
-  return layernorm_bwd_launch(x, dy, w, dx, dw, db, rows, C, eps, (cudaStream_t)stream);
+  return layernorm_bwd_checked("sigma_layernorm_bwd", SIGMA_F32, x, dy, w, dx, dw, db, rows, C, eps, stream);
+}
+
+int sigma_layernorm_bwd_bf16(const void *x, const void *dy, const float *w, void *dx, float *dw, float *db, int64_t rows, int C, float eps,
+                             void *stream) {
+  return layernorm_bwd_checked("sigma_layernorm_bwd_bf16", SIGMA_BF16, x, dy, w, dx, dw, db, rows, C, eps, stream);
+}
+
+int sigma_layernorm_bwd_fp16(const void *x, const void *dy, const float *w, void *dx, float *dw, float *db, int64_t rows, int C, float eps,
+                             void *stream) {
+  return layernorm_bwd_checked("sigma_layernorm_bwd_fp16", SIGMA_F16, x, dy, w, dx, dw, db, rows, C, eps, stream);
 }
 
 size_t sigma_layernorm_bwd_det_workspace_bytes(int64_t rows, int C) {
@@ -461,13 +464,8 @@ size_t sigma_layernorm_bwd_det_workspace_bytes(int64_t rows, int C) {
 
 int sigma_layernorm_bwd_det(const float *x, const float *dy, const float *w, float *dx, float *dw, float *db, int64_t rows, int C, float eps,
                             void *workspace, size_t workspace_bytes, void *stream) {
-  SIGMA_CHECK_ARG(x && dy && w && dx && dw && db, "sigma_layernorm_bwd_det: null pointer");
-  SIGMA_CHECK_ARG(C > 0 && C % 4 == 0 && rows >= 0, "sigma_layernorm_bwd_det: C=%d must be a positive multiple of 4", C);
-  SIGMA_CHECK_ARG(al16(x) && al16(dy) && al16(w) && al16(dx), "sigma_layernorm_bwd_det: pointers must be 16-byte aligned");
-  const size_t need = layernorm_bwd_det_workspace_bytes(rows, C);
-  SIGMA_CHECK_ARG(workspace != nullptr && al16(workspace) && workspace_bytes >= need,
-                  "sigma_layernorm_bwd_det: needs %zu 16-byte aligned workspace bytes, got %zu", need, workspace_bytes);
-  return layernorm_bwd_launch(x, dy, w, dx, dw, db, rows, C, eps, (cudaStream_t)stream, (float *)workspace);
+  return layernorm_bwd_checked("sigma_layernorm_bwd_det", SIGMA_F32, x, dy, w, dx, dw, db, rows, C, eps, stream, true, workspace,
+                               workspace_bytes);
 }
 
 int sigma_upsample_bilinear_bwd(const float *dy, float *dx, int batch, int C, int Hin, int Win, int Hout, int Wout, float ratio_h,
@@ -480,119 +478,78 @@ int sigma_upsample_bilinear_bwd(const float *dy, float *dx, int batch, int C, in
 
 int sigma_patch_merge_norm_fwd(const float *x, const float *w, const float *b, float *y, int batch, int H, int W, int C,
                                float eps, void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && y, "sigma_patch_merge_norm_fwd: null pointer");
-  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "sigma_patch_merge_norm_fwd: bad sizes");
-  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al16(y), "sigma_patch_merge_norm_fwd: pointers must be 16-byte aligned");
-  const int64_t rows = (int64_t)batch * ((H + 1) / 2) * ((W + 1) / 2);
-  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, y, rows, rows, 0, 0, 4 * C, 4 * C, eps};
-  p.mode = 1; p.gH = H; p.gW = W;
-  return row_norm_launch(p, (cudaStream_t)stream);
+  return layernorm_image("sigma_patch_merge_norm_fwd", 1, SIGMA_F32, x, w, b, y, nullptr, batch, H, W, C, eps, stream);
 }
 
 int sigma_patch_merge_norm_fwd_bf16(const float *x, const float *w, const float *b, void *y, int batch, int H, int W, int C,
                                     float eps, void *stream) {
-  return patch_merge_norm_fwd_16bit("sigma_patch_merge_norm_fwd_bf16", SIGMA_BF16, x, w, b, y, batch, H, W, C, eps, stream);
+  return layernorm_image("sigma_patch_merge_norm_fwd_bf16", 1, SIGMA_BF16, x, w, b, y, nullptr, batch, H, W, C, eps, stream);
 }
 
 int sigma_patch_merge_norm_fwd_fp16(const float *x, const float *w, const float *b, void *y, int batch, int H, int W, int C,
                                     float eps, void *stream) {
-  return patch_merge_norm_fwd_16bit("sigma_patch_merge_norm_fwd_fp16", SIGMA_F16, x, w, b, y, batch, H, W, C, eps, stream);
+  return layernorm_image("sigma_patch_merge_norm_fwd_fp16", 1, SIGMA_F16, x, w, b, y, nullptr, batch, H, W, C, eps, stream);
 }
 
 int sigma_patch_merge_norm_fwd_fp8(const float *x, const float *w, const float *b, void *q, float *scale, int batch, int H, int W, int C,
                                    float eps, void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && q && scale, "sigma_patch_merge_norm_fwd_fp8: null pointer");
-  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "sigma_patch_merge_norm_fwd_fp8: bad sizes");
-  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && ((uintptr_t)q & 3) == 0,
-                  "sigma_patch_merge_norm_fwd_fp8: x, w, b must be 16-byte and q 4-byte aligned");
-  const int64_t rows = (int64_t)batch * ((H + 1) / 2) * ((W + 1) / 2);
-  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, (float *)q, rows, rows, 0, 0, 4 * C, 4 * C, eps};
-  p.mode = 1; p.gH = H; p.gW = W; p.io = 3; p.qscale = scale;
-  return row_norm_launch(p, (cudaStream_t)stream);
+  return layernorm_image("sigma_patch_merge_norm_fwd_fp8", 1, SIGMA_E4M3_ROWS, x, w, b, q, scale, batch, H, W, C, eps, stream);
 }
 
 int sigma_pixel_shuffle_norm_fwd(const float *x, const float *w, const float *b, float *y, int batch, int H, int W, int C,
                                  float eps, void *stream) {
-  SIGMA_CHECK_ARG(x && w && b && y, "sigma_pixel_shuffle_norm_fwd: null pointer");
-  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "sigma_pixel_shuffle_norm_fwd: bad sizes");
-  SIGMA_CHECK_ARG(al16(x) && al16(w) && al16(b) && al16(y), "sigma_pixel_shuffle_norm_fwd: pointers must be 16-byte aligned");
-  const int64_t rows = (int64_t)batch * H * W * 4;
-  RowNormParams p{x, 0, 1, w, b, nullptr, 0, nullptr, y, rows, rows, 0, 0, C, C, eps};
-  p.mode = 2; p.gH = H; p.gW = W;
-  return row_norm_launch(p, (cudaStream_t)stream);
+  return layernorm_image("sigma_pixel_shuffle_norm_fwd", 2, SIGMA_F32, x, w, b, y, nullptr, batch, H, W, C, eps, stream);
 }
 
 int sigma_merge_norm_gate_fwd(const float *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
                               const float *beta, const float *z, int64_t z_row_stride, const float *gate, float *out,
                               int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
                               int D, float eps, void *stream) {
-  SIGMA_CHECK_ARG(y && gamma && beta && out, "sigma_merge_norm_gate_fwd: null pointer");
-  SIGMA_CHECK_ARG(K >= 1 && K <= 8 && D > 0 && D % 4 == 0 && rows >= 0 && rows_per_batch > 0,
-                  "sigma_merge_norm_gate_fwd: bad sizes K=%d D=%d rows=%lld rows_per_batch=%lld", K, D, (long long)rows,
-                  (long long)rows_per_batch);
-  SIGMA_CHECK_ARG(al16(y) && al16(gamma) && al16(beta) && al16(out) && al16(z) && al16(gate) && k_stride % 4 == 0 &&
-                      in_batch_stride % 4 == 0 && out_batch_stride % 4 == 0 && out_row_stride % 4 == 0 &&
-                      z_row_stride % 4 == 0,
-                  "sigma_merge_norm_gate_fwd: pointers / strides must be 16-byte aligned");
-  RowNormParams p{y, k_stride, K, gamma, beta, z, z_row_stride, gate, out, rows, rows_per_batch, in_batch_stride,
-                  out_batch_stride, out_row_stride, D, eps};
-  return row_norm_launch(p, (cudaStream_t)stream);
+  return merge_norm_gate("sigma_merge_norm_gate_fwd", SIGMA_F32, SIGMA_F32, y, K, k_stride, in_batch_stride, gamma, beta, z, z_row_stride,
+                         gate, out, nullptr, out_batch_stride, out_row_stride, rows, rows_per_batch, D, eps, stream);
 }
 
 int sigma_merge_norm_gate_fwd_fp8(const void *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
                                   const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *q, float *scale,
                                   int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
                                   int D, float eps, void *stream) {
-  SIGMA_CHECK_ARG(y && gamma && beta && q && scale, "sigma_merge_norm_gate_fwd_fp8: null pointer");
-  SIGMA_CHECK_ARG((K == 1 || K == 4) && D > 0 && D % 4 == 0 && rows >= 0 && rows_per_batch > 0,
-                  "sigma_merge_norm_gate_fwd_fp8: bad sizes K=%d (1 or 4) D=%d rows=%lld rows_per_batch=%lld", K, D, (long long)rows,
-                  (long long)rows_per_batch);
-  SIGMA_CHECK_ARG(al8(y) && al16(gamma) && al16(beta) && ((uintptr_t)q & 3) == 0 && al8(z) && al16(gate) && k_stride % 4 == 0 &&
-                      in_batch_stride % 4 == 0 && out_batch_stride % 4 == 0 && out_row_stride % 4 == 0 && z_row_stride % 4 == 0,
-                  "sigma_merge_norm_gate_fwd_fp8: y / z must be 8-byte, q 4-byte and gamma / beta / gate 16-byte aligned, strides multiples of 4");
-  RowNormParams p{(const float *)y, k_stride, K, gamma, beta, (const float *)z, z_row_stride, gate, (float *)q, rows, rows_per_batch,
-                  in_batch_stride, out_batch_stride, out_row_stride, D, eps};
-  p.io = 4; p.qscale = scale;
-  return row_norm_launch(p, (cudaStream_t)stream);
+  return merge_norm_gate("sigma_merge_norm_gate_fwd_fp8", SIGMA_BF16, SIGMA_E4M3_ROWS, y, K, k_stride, in_batch_stride, gamma, beta, z,
+                         z_row_stride, gate, q, scale, out_batch_stride, out_row_stride, rows, rows_per_batch, D, eps, stream);
 }
 
 int sigma_merge_norm_gate_fwd_bf16(const void *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
                                    const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *out,
                                    int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
                                    int D, float eps, void *stream) {
-  return merge_norm_gate_fwd_16bit("sigma_merge_norm_gate_fwd_bf16", SIGMA_BF16, y, K, k_stride, in_batch_stride, gamma, beta, z,
-                                   z_row_stride, gate, out, out_batch_stride, out_row_stride, rows, rows_per_batch, D, eps, stream);
+  return merge_norm_gate("sigma_merge_norm_gate_fwd_bf16", SIGMA_BF16, SIGMA_BF16, y, K, k_stride, in_batch_stride, gamma, beta, z,
+                         z_row_stride, gate, out, nullptr, out_batch_stride, out_row_stride, rows, rows_per_batch, D, eps, stream);
 }
 
 int sigma_merge_norm_gate_fwd_fp16(const void *y, int K, int64_t k_stride, int64_t in_batch_stride, const float *gamma,
                                    const float *beta, const void *z, int64_t z_row_stride, const float *gate, void *out,
                                    int64_t out_batch_stride, int64_t out_row_stride, int64_t rows, int64_t rows_per_batch,
                                    int D, float eps, void *stream) {
-  return merge_norm_gate_fwd_16bit("sigma_merge_norm_gate_fwd_fp16", SIGMA_F16, y, K, k_stride, in_batch_stride, gamma, beta, z,
-                                   z_row_stride, gate, out, out_batch_stride, out_row_stride, rows, rows_per_batch, D, eps, stream);
+  return merge_norm_gate("sigma_merge_norm_gate_fwd_fp16", SIGMA_F16, SIGMA_F16, y, K, k_stride, in_batch_stride, gamma, beta, z,
+                         z_row_stride, gate, out, nullptr, out_batch_stride, out_row_stride, rows, rows_per_batch, D, eps, stream);
 }
 
 int sigma_dwconv3x3_silu_fwd(const float *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w,
                              const float *bias, float *y, int64_t y_batch_stride, int batch, int H, int W, int D,
                              void *stream) {
-  SIGMA_CHECK_ARG(x && w && y, "sigma_dwconv3x3_silu_fwd: null pointer");
-  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && D > 0 && D % 4 == 0, "sigma_dwconv3x3_silu_fwd: bad sizes");
-  SIGMA_CHECK_ARG(al16(x) && al16(y) && x_row_stride % 4 == 0 && x_batch_stride % 4 == 0 && y_batch_stride % 4 == 0,
-                  "sigma_dwconv3x3_silu_fwd: pointers / strides must be 16-byte aligned");
-  return dwconv3x3_silu_launch(x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D,
-                               (cudaStream_t)stream);
+  return dwconv3x3_silu_fwd_any("sigma_dwconv3x3_silu_fwd", SIGMA_F32, x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch,
+                                H, W, D, stream);
 }
 
 int sigma_dwconv3x3_silu_fwd_bf16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
                                   void *y, int64_t y_batch_stride, int batch, int H, int W, int D, void *stream) {
-  return dwconv3x3_silu_fwd_16bit("sigma_dwconv3x3_silu_fwd_bf16", SIGMA_BF16, x, x_row_stride, x_batch_stride, w, bias, y,
-                                  y_batch_stride, batch, H, W, D, stream);
+  return dwconv3x3_silu_fwd_any("sigma_dwconv3x3_silu_fwd_bf16", SIGMA_BF16, x, x_row_stride, x_batch_stride, w, bias, y,
+                                y_batch_stride, batch, H, W, D, stream);
 }
 
 int sigma_dwconv3x3_silu_fwd_fp16(const void *x, int64_t x_row_stride, int64_t x_batch_stride, const float *w, const float *bias,
                                   void *y, int64_t y_batch_stride, int batch, int H, int W, int D, void *stream) {
-  return dwconv3x3_silu_fwd_16bit("sigma_dwconv3x3_silu_fwd_fp16", SIGMA_F16, x, x_row_stride, x_batch_stride, w, bias, y,
-                                  y_batch_stride, batch, H, W, D, stream);
+  return dwconv3x3_silu_fwd_any("sigma_dwconv3x3_silu_fwd_fp16", SIGMA_F16, x, x_row_stride, x_batch_stride, w, bias, y,
+                                y_batch_stride, batch, H, W, D, stream);
 }
 
 size_t sigma_dwconv3x3_silu_bwd_workspace_bytes(int batch, int H, int W, int D) {

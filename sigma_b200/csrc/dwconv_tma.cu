@@ -168,18 +168,11 @@ static int dwconv_tma_launch(const T *x, long long x_row_stride, long long x_bat
   return SIGMA_OK;
 }
 
-// returns SIGMA_OK, an error, or 1 when the shape cannot use the TMA path (caller falls back to the direct kernel)
-int dwconv3x3_silu_tma_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
-                              const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
-                              cudaStream_t stream) {
-  if ((x_row_stride & 3) || (x_batch_stride & 3) || ((uintptr_t)x & 15) || (D & 3)) return 1;
-  return dwconv_tma_launch<float>(x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D, stream);
-}
-
-// 16-bit x and y, dtype SIGMA_BF16 or SIGMA_F16 (the caller checks the 16-byte stride / alignment TMA needs: there is no direct
-// 16-bit kernel to fall back to)
-int dwconv3x3_silu_16bit_launch(int dtype, const void *x, long long x_row_stride, long long x_batch_stride, const float *w,
-                                const float *bias, void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream) {
+int dwconv3x3_silu_fwd_launch(int dtype, const void *x, long long x_row_stride, long long x_batch_stride, const float *w,
+                              const float *bias, void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream) {
+  if (dtype == SIGMA_F32)
+    return dwconv_tma_launch<float>((const float *)x, x_row_stride, x_batch_stride, w, bias, (float *)y, y_batch_stride, batch, H, W,
+                                    D, stream);
   if (dtype == SIGMA_F16)
     return dwconv_tma_launch<__half>((const __half *)x, x_row_stride, x_batch_stride, w, bias, (__half *)y, y_batch_stride, batch, H,
                                      W, D, stream);

@@ -21,9 +21,15 @@ struct ScanOpPlan {
   int nst;               // ring / pipeline stages
 };
 
+// Element code of e4m3 rows with one fp32 scale per row (the FP8 inference mode's row-norm output, E4M3Rows in common.cuh).
+// Internal to the library: no entry point takes it, so it is not one of the public SIGMA_F32 / SIGMA_F16 / SIGMA_BF16 codes.
+constexpr int SIGMA_E4M3_ROWS = 3;
+
+// One row-norm launch.  The element types of y / z (input) and out are passed to row_norm_launch beside this block: the
+// pointers are typed fp32 but hold elements of those types, and strides count them.  gamma, beta and gate are fp32.
 struct RowNormParams {
   const float *y;          // K slabs
-  long long k_stride;      // floats between slabs
+  long long k_stride;      // elements between slabs
   int K;
   const float *gamma, *beta;
   const float *z; long long z_row_stride;       // nullable
@@ -39,13 +45,7 @@ struct RowNormParams {
   // 2 = PatchExpand pixel shuffle (MambaDecoder.py:24-28): input rows are (b, h, w, p1, p2) sub-rows of D channels,
   //     row lands at out (b, 2h+p1, 2w+p2)
   int mode = 0, gH = 0, gW = 0;
-  // element types (the bf16 inference mode): 0 = y, z, out fp32; 1 = y fp32, out bf16 (LayerNorm / patch-merge LN feeding a
-  // bf16 GEMM); 2 = y, z, out bf16 (merge + out_norm + gate of the bf16 scan output).  Pointers and strides count elements.
-  // The FP8 inference mode: 3 = y fp32, out e4m3 (LayerNorm / patch-merge LN feeding sigma_linear_fp8); 4 = y, z bf16, out e4m3
-  // (merge + out_norm + gate).  Both write row r's scale to qscale[r].
-  // The fp16 inference mode: 5 = y fp32, out fp16 (as 1); 6 = y, z, out fp16 (as 2).
-  int io = 0;
-  float *qscale = nullptr;
+  float *qscale = nullptr;   // e4m3 output: row r's scale
 };
 
 struct ImagePreParams {
@@ -152,17 +152,16 @@ int upsample_bilinear_bwd_launch(const float *dy, float *dx, int batch, int C, i
                                  int channels_last, cudaStream_t stream);
 
 // ---- rowwise.cu ----
-int row_norm_launch(const RowNormParams &p, cudaStream_t stream);
+// ti: element type of y and z, to: of out.  The pairs with instances: (SIGMA_F32, SIGMA_F32 / SIGMA_BF16 / SIGMA_F16 /
+// SIGMA_E4M3_ROWS), (SIGMA_BF16, SIGMA_BF16 / SIGMA_E4M3_ROWS) and (SIGMA_F16, SIGMA_F16); any other is SIGMA_EUNSUPPORTED.
+int row_norm_launch(int ti, int to, const RowNormParams &p, cudaStream_t stream);
 int quantize_e4m3_rows_launch(const void *x, bool bf16, long long ldx, void *q, long long ldq, float *scale, long long rows, int C,
                               cudaStream_t stream);
-// part != nullptr: the deterministic build (layernorm_bwd_det_workspace_bytes of scratch); xdtype SIGMA_BF16 / SIGMA_F16 (excludes
-// part): x, dy and dx are bf16 / fp16 behind the float pointers
-int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                         int D, float eps, cudaStream_t stream, float *part = nullptr, int xdtype = SIGMA_F32);
+// dtype: element type of x, dy and dx, SIGMA_F32, SIGMA_BF16 or SIGMA_F16; part != nullptr (SIGMA_F32 only): the deterministic
+// build (layernorm_bwd_det_workspace_bytes of scratch)
+int layernorm_bwd_launch(int dtype, const void *x, const void *dy, const float *gamma, void *dx, float *dgamma, float *dbeta,
+                         long long rows, int D, float eps, cudaStream_t stream, float *part = nullptr);
 size_t layernorm_bwd_det_workspace_bytes(long long rows, int D);
-int dwconv3x3_silu_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
-                          const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
-                          cudaStream_t stream);
 int upsample2x_norm_launch(const float *in, const float *gamma, const float *beta, const float *wcls, int ncls, float *out,
                            int B, int Hin, int Win, int C, float eps, cudaStream_t stream);
 int pool_avgmax_partial_launch(const float *x, float *partial, int B, long long L, int C, int nslice, cudaStream_t stream);
@@ -170,12 +169,9 @@ int scale_add_launch(const float *a, const float *sa, const float *b, const floa
                      long long rows_per_batch, int C, cudaStream_t stream);
 
 // ---- dwconv_tma.cu ----
-int dwconv3x3_silu_tma_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
-                              const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
-                              cudaStream_t stream);
-// dtype: SIGMA_BF16 or SIGMA_F16 x and y
-int dwconv3x3_silu_16bit_launch(int dtype, const void *x, long long x_row_stride, long long x_batch_stride, const float *w,
-                                const float *bias, void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream);
+// dtype SIGMA_F32, SIGMA_BF16 or SIGMA_F16 x and y; x 16-byte aligned with strides multiples of 16 bytes (TMA: the caller checks)
+int dwconv3x3_silu_fwd_launch(int dtype, const void *x, long long x_row_stride, long long x_batch_stride, const float *w,
+                              const float *bias, void *y, long long y_batch_stride, int batch, int H, int W, int D, cudaStream_t stream);
 // backward: dtype SIGMA_F32, SIGMA_BF16 or SIGMA_F16 x, dy and dx; ws holds dwconv3x3_silu_bwd_workspace_bytes (16-byte aligned)
 size_t dwconv3x3_silu_bwd_workspace_bytes(int batch, int H, int W, int D);
 int dwconv3x3_silu_bwd_launch(int dtype, const void *x, long long x_row_stride, long long x_batch_stride, const float *w,

@@ -1,11 +1,13 @@
-// Row-wise / stencil kernels of the channels-last pipeline (fp32):
+// Row-wise kernels of the channels-last pipeline:
 //   row_norm_kernel  : [sum over K direction outputs] -> LayerNorm -> [· SiLU(z)] -> [· gate]   (one warp per row)
 //                      = nn.LayerNorm (vmamba.py:1693,2173,...) when K=1, z=gate=NULL, and
-//                      = CrossMerge sum + out_norm + y·SiLU(z) (vmamba.py:217-224,1077) otherwise
-//   dwconv3x3_silu   : depthwise 3x3 (pad 1) + bias + SiLU on NHWC (vmamba.py:683-692,1072)
-// All are HBM-bound; loads/stores are 16-byte, rows are contiguous in the channel dimension.
+//                      = CrossMerge sum + out_norm + y·SiLU(z) (vmamba.py:217-224,1077) otherwise;
+//                      y / z fp32, bf16 or fp16, out fp32, bf16, fp16 or e4m3 rows (row_norm_launch lists the pairs)
+//   layernorm_bwd    : dx, dgamma, dbeta of the LayerNorm, x / dy / dx fp32, bf16 or fp16
+//   the e4m3 row quantizer and the decoder tail (bilinear x2 + LayerNorm [+ head], pooling, scale-add), fp32
+// All are HBM-bound; loads/stores are 16-byte (8 for 16-bit, 4 for e4m3 elements), rows are contiguous in the channel dimension.
+// gamma, beta, gate and all arithmetic are fp32.
 #include <algorithm>
-#include <cstdlib>
 #include <type_traits>
 
 #include "common.cuh"
@@ -38,8 +40,8 @@ __device__ __forceinline__ float4 norm_gate4(float4 x, float mean, float rstd, c
   return o;
 }
 
-// TI: element type of y and z, TO: of out (RowNormParams::io; E4M3Rows: e4m3 bytes + p.qscale); gamma, beta, gate and all
-// arithmetic are fp32
+// TI: element type of y and z, TO: of out (row_norm_launch's ti / to; E4M3Rows: e4m3 bytes + p.qscale); gamma, beta, gate and
+// all arithmetic are fp32
 template <int MAXV, typename TI, typename TO>
 __global__ void __launch_bounds__(256) row_norm_kernel(const RowNormParams p) {
   const int lane = threadIdx.x & 31;
@@ -229,44 +231,53 @@ __global__ void __launch_bounds__(256) row_norm_fast_kernel(const RowNormParams 
   }
 }
 
-template <int LPR, int V>
-static bool row_norm_fast_k(const RowNormParams &p, cudaStream_t stream) {
-  using bf16 = __nv_bfloat16;
-  const int warps = 8, rows_per_cta = warps * (32 / LPR);
-  const unsigned grid = (unsigned)((p.rows + rows_per_cta - 1) / rows_per_cta);
-  if (p.io == 1) {   // LayerNorm / patch-merge LayerNorm with bf16 output
-    if (p.K != 1) return false;
-    if (p.mode == 0) { row_norm_fast_kernel<LPR, V, 1, 0, float, bf16><<<grid, warps * 32, 0, stream>>>(p); return true; }
-    if (p.mode == 1) { row_norm_fast_kernel<LPR, V, 1, 1, float, bf16><<<grid, warps * 32, 0, stream>>>(p); return true; }
-    return false;
+// ---- row_norm_launch: one dispatcher over the element pairs (TI, TO) ----
+// What each pair has instances for:
+//  * fast kernel, plain rows (mode 0): K = 1 for every pair; K = 2 and 4 (the direction merge of a scan output) where the input
+//    is 16-bit or both types are fp32.  Patch-merge gather (mode 1): fp32 input, K = 1.  Pixel shuffle (mode 2): fp32 only, K = 1.
+//  * generic kernel, plain rows only: D <= 4096, or D <= 1024 for e4m3 output, which holds the whole row in registers before it
+//    stores it (a wider row would spill).
+//  * e4m3 output: K = 1 or 4 only.
+template <typename TI, typename TO>
+struct RowNormPair {
+  static constexpr bool E4M3 = std::is_same<TO, E4M3Rows>::value;
+  static constexpr bool F32_IN = std::is_same<TI, float>::value, F32_OUT = std::is_same<TO, float>::value;
+  static constexpr int GENERIC_MAXV = E4M3 ? 8 : 32;
+  static constexpr bool k_ok(int K) { return !E4M3 || K == 1 || K == 4; }
+  static constexpr bool fast(int mode, int K) {
+    if (mode == 0) return K == 1 || ((!F32_IN || F32_OUT) && (K == 2 || K == 4) && k_ok(K));
+    return K == 1 && F32_IN && (mode == 1 || (mode == 2 && F32_OUT));
   }
-  if (p.io == 2) {   // merge + norm + gate, bf16 in and out
-    if (p.mode != 0) return false;
-    switch (p.K) {
-      case 1: row_norm_fast_kernel<LPR, V, 1, 0, bf16, bf16><<<grid, warps * 32, 0, stream>>>(p); return true;
-      case 2: row_norm_fast_kernel<LPR, V, 2, 0, bf16, bf16><<<grid, warps * 32, 0, stream>>>(p); return true;
-      case 4: row_norm_fast_kernel<LPR, V, 4, 0, bf16, bf16><<<grid, warps * 32, 0, stream>>>(p); return true;
+};
+
+template <int LPR, int V, int K, int MODE, typename TI, typename TO>
+static bool row_norm_fast_if(const RowNormParams &p, unsigned grid, cudaStream_t stream) {
+  if constexpr (RowNormPair<TI, TO>::fast(MODE, K)) {
+    if (p.mode == MODE && p.K == K) {
+      row_norm_fast_kernel<LPR, V, K, MODE, TI, TO><<<grid, 256, 0, stream>>>(p);
+      return true;
     }
-    return false;
-  }
-  if (p.mode == 1 && p.K == 1) { row_norm_fast_kernel<LPR, V, 1, 1, float, float><<<grid, warps * 32, 0, stream>>>(p); return true; }
-  if (p.mode == 2 && p.K == 1) { row_norm_fast_kernel<LPR, V, 1, 2, float, float><<<grid, warps * 32, 0, stream>>>(p); return true; }
-  if (p.mode != 0) return false;
-  switch (p.K) {
-    case 1: row_norm_fast_kernel<LPR, V, 1, 0, float, float><<<grid, warps * 32, 0, stream>>>(p); return true;
-    case 2: row_norm_fast_kernel<LPR, V, 2, 0, float, float><<<grid, warps * 32, 0, stream>>>(p); return true;
-    case 4: row_norm_fast_kernel<LPR, V, 4, 0, float, float><<<grid, warps * 32, 0, stream>>>(p); return true;
   }
   return false;
 }
 
-// picks (lanes per row, float4 per lane) for D; false if D has no fast instantiation
+template <typename TI, typename TO, int LPR, int V>
+static bool row_norm_fast_k(const RowNormParams &p, cudaStream_t stream) {
+  const int rows_per_cta = 8 * (32 / LPR);   // 8 warps
+  const unsigned grid = (unsigned)((p.rows + rows_per_cta - 1) / rows_per_cta);
+  return row_norm_fast_if<LPR, V, 1, 0, TI, TO>(p, grid, stream) || row_norm_fast_if<LPR, V, 2, 0, TI, TO>(p, grid, stream) ||
+         row_norm_fast_if<LPR, V, 4, 0, TI, TO>(p, grid, stream) || row_norm_fast_if<LPR, V, 1, 1, TI, TO>(p, grid, stream) ||
+         row_norm_fast_if<LPR, V, 1, 2, TI, TO>(p, grid, stream);
+}
+
+// picks (lanes per row, float4 per lane) for D; false if D, a stride or (mode, K) has no fast instance
+template <typename TI, typename TO>
 static bool row_norm_fast(const RowNormParams &p, cudaStream_t stream) {
   if ((p.D & 3) || (p.k_stride & 3) || (p.in_batch_stride & 3) || (p.out_row_stride & 3) || (p.out_batch_stride & 3) ||
       (p.z_row_stride & 3))
     return false;
   const int nvec = p.D >> 2;
-#define TRY(LPR, V) if (nvec == (LPR) * (V)) return row_norm_fast_k<LPR, V>(p, stream)
+#define TRY(LPR, V) if (nvec == (LPR) * (V)) return row_norm_fast_k<TI, TO, LPR, V>(p, stream)
   TRY(8, 2); TRY(8, 3); TRY(8, 4);
   TRY(16, 3); TRY(16, 4);
   TRY(32, 3); TRY(32, 4); TRY(32, 6); TRY(32, 8); TRY(32, 12); TRY(32, 16);
@@ -274,139 +285,43 @@ static bool row_norm_fast(const RowNormParams &p, cudaStream_t stream) {
   return false;
 }
 
-// The e4m3-output instances (io 3, 4: the FP8 inference mode), at the fast widths of row_norm_fast and, for other widths up to
-// 1024 channels, the generic kernel (a wider row held in registers would spill).
-template <int LPR, int V>
-static bool row_norm_e4m3_fast_k(const RowNormParams &p, cudaStream_t stream) {
-  using bf16 = __nv_bfloat16;
-  const int warps = 8, rows_per_cta = warps * (32 / LPR);
-  const unsigned grid = (unsigned)((p.rows + rows_per_cta - 1) / rows_per_cta);
-  if (p.io == 3) {   // LayerNorm / patch-merge LayerNorm
-    if (p.K != 1) return false;
-    if (p.mode == 0) { row_norm_fast_kernel<LPR, V, 1, 0, float, E4M3Rows><<<grid, warps * 32, 0, stream>>>(p); return true; }
-    if (p.mode == 1) { row_norm_fast_kernel<LPR, V, 1, 1, float, E4M3Rows><<<grid, warps * 32, 0, stream>>>(p); return true; }
-    return false;
+// the generic kernel with the fewest float4 slots (1, 2, 4, ... GENERIC_MAXV) that hold nvec
+template <typename TI, typename TO, int MAXV = 1>
+static void row_norm_generic(const RowNormParams &p, int nvec, cudaStream_t stream) {
+  if constexpr (MAXV < RowNormPair<TI, TO>::GENERIC_MAXV) {
+    if (nvec > 32 * MAXV) return row_norm_generic<TI, TO, 2 * MAXV>(p, nvec, stream);
   }
-  if (p.mode != 0) return false;   // io 4: merge + norm + gate, bf16 in
-  if (p.K == 1) { row_norm_fast_kernel<LPR, V, 1, 0, bf16, E4M3Rows><<<grid, warps * 32, 0, stream>>>(p); return true; }
-  if (p.K == 4) { row_norm_fast_kernel<LPR, V, 4, 0, bf16, E4M3Rows><<<grid, warps * 32, 0, stream>>>(p); return true; }
-  return false;
+  row_norm_kernel<MAXV, TI, TO><<<(unsigned)((p.rows + 7) / 8), 256, 0, stream>>>(p);
 }
 
-static int row_norm_e4m3_launch(const RowNormParams &p, cudaStream_t stream) {
-  const int nvec = p.D >> 2;
-  bool ok = false;
-  if (!((p.D & 3) || (p.k_stride & 3) || (p.in_batch_stride & 3) || (p.out_row_stride & 3) || (p.out_batch_stride & 3) ||
-        (p.z_row_stride & 3))) {
-#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) ok = row_norm_e4m3_fast_k<LPR, V>(p, stream)
-    TRY(8, 2); TRY(8, 3); TRY(8, 4);
-    TRY(16, 3); TRY(16, 4);
-    TRY(32, 3); TRY(32, 4); TRY(32, 6); TRY(32, 8); TRY(32, 12); TRY(32, 16);
-#undef TRY
-  }
-  if (!ok) {
-    if (p.mode != 0 || nvec > 256 || (p.io == 4 && p.K != 1 && p.K != 4)) {
-      set_error("row_norm: no e4m3-output instance for D=%d, mode %d, K=%d (fast widths, or D <= 1024 plain rows)", p.D, p.mode, p.K);
+template <typename TI, typename TO>
+static int row_norm_dispatch(const RowNormParams &p, cudaStream_t stream) {
+  using Pair = RowNormPair<TI, TO>;
+  if (p.rows == 0) return SIGMA_OK;
+  if (!row_norm_fast<TI, TO>(p, stream)) {
+    const int nvec = p.D >> 2;
+    if (p.mode != 0 || !Pair::k_ok(p.K) || nvec > 32 * Pair::GENERIC_MAXV) {
+      set_error("row_norm: no instance for D=%d, mode %d, K=%d (gather / pixel-shuffle modes need D = 4·LPR·V; plain rows reach "
+                "D <= %d%s)", p.D, p.mode, p.K, 128 * Pair::GENERIC_MAXV, Pair::E4M3 ? ", K = 1 or 4 for e4m3 output" : "");
       return SIGMA_EUNSUPPORTED;
     }
-    const unsigned grid = (unsigned)((p.rows + 7) / 8);
-#define LAUNCH_E4M3(MV)                                                                                                  \
-    do {                                                                                                                 \
-      if (p.io == 3) row_norm_kernel<MV, float, E4M3Rows><<<grid, 256, 0, stream>>>(p);                                  \
-      else row_norm_kernel<MV, __nv_bfloat16, E4M3Rows><<<grid, 256, 0, stream>>>(p);                                    \
-    } while (0)
-    if (nvec <= 32) LAUNCH_E4M3(1);
-    else if (nvec <= 64) LAUNCH_E4M3(2);
-    else if (nvec <= 128) LAUNCH_E4M3(4);
-    else LAUNCH_E4M3(8);
-#undef LAUNCH_E4M3
+    row_norm_generic<TI, TO>(p, nvec, stream);
   }
   SIGMA_CHECK_LAUNCH();
   return SIGMA_OK;
 }
 
-// The fp16 instances (io 5, 6: the fp16 inference mode): io 1 / 2's kernels with __half for bf16, at the same fast widths and, for
-// other widths, the generic kernel.
-template <int LPR, int V>
-static bool row_norm_fp16_fast_k(const RowNormParams &p, cudaStream_t stream) {
-  using f16 = __half;
-  const int warps = 8, rows_per_cta = warps * (32 / LPR);
-  const unsigned grid = (unsigned)((p.rows + rows_per_cta - 1) / rows_per_cta);
-  if (p.io == 5) {   // LayerNorm / patch-merge LayerNorm with fp16 output
-    if (p.K != 1) return false;
-    if (p.mode == 0) { row_norm_fast_kernel<LPR, V, 1, 0, float, f16><<<grid, warps * 32, 0, stream>>>(p); return true; }
-    if (p.mode == 1) { row_norm_fast_kernel<LPR, V, 1, 1, float, f16><<<grid, warps * 32, 0, stream>>>(p); return true; }
-    return false;
-  }
-  if (p.mode != 0) return false;   // io 6: merge + norm + gate, fp16 in and out
-  switch (p.K) {
-    case 1: row_norm_fast_kernel<LPR, V, 1, 0, f16, f16><<<grid, warps * 32, 0, stream>>>(p); return true;
-    case 2: row_norm_fast_kernel<LPR, V, 2, 0, f16, f16><<<grid, warps * 32, 0, stream>>>(p); return true;
-    case 4: row_norm_fast_kernel<LPR, V, 4, 0, f16, f16><<<grid, warps * 32, 0, stream>>>(p); return true;
-  }
-  return false;
-}
-
-static int row_norm_fp16_launch(const RowNormParams &p, cudaStream_t stream) {
-  const int nvec = p.D >> 2;
-  bool ok = false;
-  if (!((p.D & 3) || (p.k_stride & 3) || (p.in_batch_stride & 3) || (p.out_row_stride & 3) || (p.out_batch_stride & 3) ||
-        (p.z_row_stride & 3))) {
-#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) ok = row_norm_fp16_fast_k<LPR, V>(p, stream)
-    TRY(8, 2); TRY(8, 3); TRY(8, 4);
-    TRY(16, 3); TRY(16, 4);
-    TRY(32, 3); TRY(32, 4); TRY(32, 6); TRY(32, 8); TRY(32, 12); TRY(32, 16);
-#undef TRY
-  }
-  if (!ok) {
-    if (p.mode != 0) { set_error("row_norm: gather / pixel-shuffle modes need D = 4·LPR·V (D=%d has no fast instantiation)", p.D); return SIGMA_EUNSUPPORTED; }
-    const unsigned grid = (unsigned)((p.rows + 7) / 8);
-#define LAUNCH_F16(MV)                                                                                                   \
-    do {                                                                                                                 \
-      if (p.io == 5) row_norm_kernel<MV, float, __half><<<grid, 256, 0, stream>>>(p);                                    \
-      else row_norm_kernel<MV, __half, __half><<<grid, 256, 0, stream>>>(p);                                             \
-    } while (0)
-    if (nvec <= 32) LAUNCH_F16(1);
-    else if (nvec <= 64) LAUNCH_F16(2);
-    else if (nvec <= 128) LAUNCH_F16(4);
-    else if (nvec <= 256) LAUNCH_F16(8);
-    else if (nvec <= 512) LAUNCH_F16(16);
-    else if (nvec <= 1024) LAUNCH_F16(32);
-    else { set_error("row_norm: D=%d > 4096 unsupported", p.D); return SIGMA_EUNSUPPORTED; }
-#undef LAUNCH_F16
-  }
-  SIGMA_CHECK_LAUNCH();
-  return SIGMA_OK;
-}
-
-int row_norm_launch(const RowNormParams &p, cudaStream_t stream) {
-  if (p.rows == 0) return SIGMA_OK;
-  if (p.io == 5 || p.io == 6) return row_norm_fp16_launch(p, stream);
-  if (p.io >= 3) return row_norm_e4m3_launch(p, stream);
-  if (row_norm_fast(p, stream)) {
-    SIGMA_CHECK_LAUNCH();
-    return SIGMA_OK;
-  }
-  if (p.mode != 0) { set_error("row_norm: gather / pixel-shuffle modes need D = 4·LPR·V (D=%d has no fast instantiation)", p.D); return SIGMA_EUNSUPPORTED; }
-  const int nvec = p.D >> 2;
-  const int warps = 8;
-  const unsigned grid = (unsigned)((p.rows + warps - 1) / warps);
-#define LAUNCH(MV)                                                                                                     \
-  do {                                                                                                                 \
-    if (p.io == 1) row_norm_kernel<MV, float, __nv_bfloat16><<<grid, warps * 32, 0, stream>>>(p);                      \
-    else if (p.io == 2) row_norm_kernel<MV, __nv_bfloat16, __nv_bfloat16><<<grid, warps * 32, 0, stream>>>(p);         \
-    else row_norm_kernel<MV, float, float><<<grid, warps * 32, 0, stream>>>(p);                                        \
-  } while (0)
-  if (nvec <= 32) LAUNCH(1);
-  else if (nvec <= 64) LAUNCH(2);
-  else if (nvec <= 128) LAUNCH(4);
-  else if (nvec <= 256) LAUNCH(8);
-  else if (nvec <= 512) LAUNCH(16);
-  else if (nvec <= 1024) LAUNCH(32);
-  else { set_error("row_norm: D=%d > 4096 unsupported", p.D); return SIGMA_EUNSUPPORTED; }
-#undef LAUNCH
-  SIGMA_CHECK_LAUNCH();
-  return SIGMA_OK;
+int row_norm_launch(int ti, int to, const RowNormParams &p, cudaStream_t stream) {
+  using bf16 = __nv_bfloat16;
+  if (ti == SIGMA_F32 && to == SIGMA_F32) return row_norm_dispatch<float, float>(p, stream);
+  if (ti == SIGMA_F32 && to == SIGMA_BF16) return row_norm_dispatch<float, bf16>(p, stream);
+  if (ti == SIGMA_F32 && to == SIGMA_F16) return row_norm_dispatch<float, __half>(p, stream);
+  if (ti == SIGMA_F32 && to == SIGMA_E4M3_ROWS) return row_norm_dispatch<float, E4M3Rows>(p, stream);
+  if (ti == SIGMA_BF16 && to == SIGMA_BF16) return row_norm_dispatch<bf16, bf16>(p, stream);
+  if (ti == SIGMA_BF16 && to == SIGMA_E4M3_ROWS) return row_norm_dispatch<bf16, E4M3Rows>(p, stream);
+  if (ti == SIGMA_F16 && to == SIGMA_F16) return row_norm_dispatch<__half, __half>(p, stream);
+  set_error("row_norm: no instances for element types (%d, %d)", ti, to);
+  return SIGMA_EUNSUPPORTED;
 }
 
 // ---- standalone e4m3 row quantizer (the FP8 inference mode: weights per output channel, and activations no producer holds a
@@ -601,15 +516,15 @@ static unsigned layernorm_bwd_grid(long long rows, int D) {
 }
 
 template <int LPR, int V>
-static void layernorm_bwd_k(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                            int D, float eps, float *part, cudaStream_t stream, int xdtype) {
+static void layernorm_bwd_k(int dtype, const void *x, const void *dy, const float *gamma, void *dx, float *dgamma, float *dbeta,
+                            long long rows, int D, float eps, float *part, cudaStream_t stream) {
   using bf = __nv_bfloat16;
   const int warps = 8;
   const unsigned grid = layernorm_bwd_grid(rows, D);
-  if (xdtype == SIGMA_F16) layernorm_bwd_fp16_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>((const __half *)x, (const __half *)dy, gamma, (__half *)dx, dgamma, dbeta, rows, D, eps);
-  else if (xdtype == SIGMA_BF16) layernorm_bwd_bf16_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>((const bf *)x, (const bf *)dy, gamma, (bf *)dx, dgamma, dbeta, rows, D, eps);
-  else if (part) layernorm_bwd_det_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>(x, dy, gamma, dx, rows, D, eps, part);
-  else layernorm_bwd_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps);
+  if (dtype == SIGMA_F16) layernorm_bwd_fp16_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>((const __half *)x, (const __half *)dy, gamma, (__half *)dx, dgamma, dbeta, rows, D, eps);
+  else if (dtype == SIGMA_BF16) layernorm_bwd_bf16_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>((const bf *)x, (const bf *)dy, gamma, (bf *)dx, dgamma, dbeta, rows, D, eps);
+  else if (part) layernorm_bwd_det_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>((const float *)x, (const float *)dy, gamma, (float *)dx, rows, D, eps, part);
+  else layernorm_bwd_kernel<LPR, V><<<grid, warps * 32, 0, stream>>>((const float *)x, (const float *)dy, gamma, (float *)dx, dgamma, dbeta, rows, D, eps);
 }
 
 // deterministic build: one dgamma and one dbeta row of D floats per warp of the grid
@@ -619,10 +534,9 @@ size_t layernorm_bwd_det_workspace_bytes(long long rows, int D) {
 
 // dgamma / dbeta are zeroed here and accumulated into; false if D has no instantiation (the fast forward's D set).
 // part != nullptr: the deterministic build (layernorm_bwd_det_workspace_bytes of scratch), dgamma / dbeta written by the
-// fixed-order sum over the grid's warps.  xdtype SIGMA_BF16 / SIGMA_F16 (never with part): x, dy and dx are bf16 / fp16 behind the
-// float pointers
-int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, float *dx, float *dgamma, float *dbeta, long long rows,
-                         int D, float eps, cudaStream_t stream, float *part, int xdtype) {
+// fixed-order sum over the grid's warps.  dtype: element type of x, dy and dx (SIGMA_BF16 / SIGMA_F16 never with part)
+int layernorm_bwd_launch(int dtype, const void *x, const void *dy, const float *gamma, void *dx, float *dgamma, float *dbeta,
+                         long long rows, int D, float eps, cudaStream_t stream, float *part) {
   if (D & 3) { set_error("layernorm_bwd: D=%d must be a multiple of 4", D); return SIGMA_EUNSUPPORTED; }
   if (rows == 0 && !part) return SIGMA_OK;
   if (rows == 0) {
@@ -636,7 +550,7 @@ int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, fl
   }
   const int nvec = D >> 2;
   bool ok = false;
-#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) { layernorm_bwd_k<LPR, V>(x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, part, stream, xdtype); SIGMA_CHECK_LAUNCH(); ok = true; }
+#define TRY(LPR, V) if (!ok && nvec == (LPR) * (V)) { layernorm_bwd_k<LPR, V>(dtype, x, dy, gamma, dx, dgamma, dbeta, rows, D, eps, part, stream); SIGMA_CHECK_LAUNCH(); ok = true; }
   TRY(8, 1) TRY(8, 2) TRY(8, 3) TRY(8, 4)
   TRY(16, 3) TRY(16, 4)
   TRY(32, 3) TRY(32, 4) TRY(32, 6) TRY(32, 8) TRY(32, 12)
@@ -649,94 +563,6 @@ int layernorm_bwd_launch(const float *x, const float *dy, const float *gamma, fl
   const int nw = (int)layernorm_bwd_grid(rows, D) * 8;
   const int rc = sum_parts_det_launch(part, nw, D, D, 0, dgamma, stream);
   return rc ? rc : sum_parts_det_launch(part + (size_t)nw * D, nw, D, D, 0, dbeta, stream);
-}
-
-// ---- depthwise 3x3 + bias + SiLU, NHWC ----
-// CTA: 64 channels (16 float4 lanes) x 16 position-threads.  A thread produces DW_WB = 4 horizontally adjacent
-// outputs of its 4 channels from a 3 x 6 window held in registers (18 loads for 4 outputs instead of 36), the
-// 9 taps of its channels live in registers (loaded once through shared memory from the (D,1,3,3) weight).
-constexpr int DW_CH = 64, DW_PT = 16, DW_WB = 4, DW_GROUPS_PER_CTA = 64;
-
-__global__ void __launch_bounds__(256) dwconv3x3_silu_kernel(const float *__restrict__ x, long long x_row_stride,
-                                                            long long x_batch_stride, const float *__restrict__ w,
-                                                            const float *__restrict__ bias, float *__restrict__ y,
-                                                            long long y_batch_stride, int batch, int H, int W, int D) {
-  __shared__ __align__(16) float sw[9][DW_CH];
-  __shared__ __align__(16) float sb[DW_CH];
-  const int c0 = blockIdx.x * DW_CH;
-  for (int i = threadIdx.x; i < 9 * DW_CH; i += blockDim.x) {
-    const int c = i / 9, tap = i - c * 9;
-    sw[tap][c] = (c0 + c < D) ? w[(long long)(c0 + c) * 9 + tap] : 0.f;
-  }
-  for (int i = threadIdx.x; i < DW_CH; i += blockDim.x) sb[i] = (bias && c0 + i < D) ? bias[c0 + i] : 0.f;
-  __syncthreads();
-  const int cq = threadIdx.x & 15, pr = threadIdx.x >> 4;
-  const int c = c0 + 4 * cq;
-  if (c >= D) return;
-  float4 wt[9];
-#pragma unroll
-  for (int tap = 0; tap < 9; ++tap) wt[tap] = *reinterpret_cast<const float4 *>(&sw[tap][4 * cq]);
-  const float4 bv = *reinterpret_cast<const float4 *>(&sb[4 * cq]);
-  const int gpr = (W + DW_WB - 1) / DW_WB;                          // groups per image row
-  const long long total = (long long)batch * H * gpr;
-  const long long g0 = (long long)blockIdx.y * DW_GROUPS_PER_CTA;
-  for (long long g = g0 + pr; g < min(total, g0 + DW_GROUPS_PER_CTA); g += DW_PT) {
-    const int gw = (int)(g % gpr);
-    const long long bh = g / gpr;
-    const int h = (int)(bh % H), b = (int)(bh / H);
-    const int w0 = gw * DW_WB;
-    const float *xb = x + (long long)b * x_batch_stride + c;
-    float4 acc[DW_WB];
-#pragma unroll
-    for (int j = 0; j < DW_WB; ++j) acc[j] = bv;
-#pragma unroll
-    for (int dy = -1; dy <= 1; ++dy) {
-      const int hh = h + dy;
-      if (hh < 0 || hh >= H) continue;
-      float4 win[DW_WB + 2];
-#pragma unroll
-      for (int j = 0; j < DW_WB + 2; ++j) {
-        const int ww = w0 - 1 + j;
-        win[j] = (ww >= 0 && ww < W) ? __ldg(reinterpret_cast<const float4 *>(xb + ((long long)hh * W + ww) * x_row_stride))
-                                     : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int j = 0; j < DW_WB; ++j) {
-#pragma unroll
-        for (int dx = 0; dx < 3; ++dx) {
-          const float4 v = win[j + dx];
-          const float4 k = wt[(dy + 1) * 3 + dx];
-          acc[j].x = fmaf(v.x, k.x, acc[j].x); acc[j].y = fmaf(v.y, k.y, acc[j].y);
-          acc[j].z = fmaf(v.z, k.z, acc[j].z); acc[j].w = fmaf(v.w, k.w, acc[j].w);
-        }
-      }
-    }
-    float *yb = y + (long long)b * y_batch_stride + ((long long)h * W + w0) * D + c;
-#pragma unroll
-    for (int j = 0; j < DW_WB; ++j) {
-      if (w0 + j < W) {
-        float4 o;
-        o.x = silu(acc[j].x); o.y = silu(acc[j].y); o.z = silu(acc[j].z); o.w = silu(acc[j].w);
-        *reinterpret_cast<float4 *>(yb + (long long)j * D) = o;
-      }
-    }
-  }
-}
-
-int dwconv3x3_silu_launch(const float *x, long long x_row_stride, long long x_batch_stride, const float *w,
-                          const float *bias, float *y, long long y_batch_stride, int batch, int H, int W, int D,
-                          cudaStream_t stream) {
-  static const bool direct = getenv("SIGMA_DWCONV_DIRECT") != nullptr;   // A/B switch: the first (L1-windowed) kernel
-  if (!direct) {
-    const int rc = dwconv3x3_silu_tma_launch(x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D, stream);
-    if (rc != 1) return rc;
-  }
-  const long long total = (long long)batch * H * ((W + DW_WB - 1) / DW_WB);
-  if (total == 0) return SIGMA_OK;
-  dim3 grid((D + DW_CH - 1) / DW_CH, (unsigned)((total + DW_GROUPS_PER_CTA - 1) / DW_GROUPS_PER_CTA));
-  dwconv3x3_silu_kernel<<<grid, 256, 0, stream>>>(x, x_row_stride, x_batch_stride, w, bias, y, y_batch_stride, batch, H, W, D);
-  SIGMA_CHECK_LAUNCH();
-  return SIGMA_OK;
 }
 
 }  // namespace sigma

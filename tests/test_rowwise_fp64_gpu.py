@@ -40,7 +40,7 @@ LN_GENERIC_D = [32, 200, 400, 1000, 2000, 4000, 4096]
 MERGE_K = [1, 2, 3, 4, 5, 6, 7, 8]
 MERGE_D = [96, 192, 384, 768, 1536, 256, 512, 1024, 2048, 64, 128]
 PATCH_MERGE_C = [96, 192, 384, 128, 256, 512, 16, 24, 32, 48, 64]
-# element types (RowNormParams::io) each test runs: 0 fp32, 1 fp32 in / bf16 out, 2 bf16 in and out
+# element pairs each test runs (oracle/rowwise_ref64.IO_PAIRS): 0 fp32, 1 fp32 in / bf16 out, 2 bf16 in and out
 LN_IO = [0, 1, 2]
 MERGE_IO = [0, 2]
 PATCH_MERGE_IO = [0, 1]

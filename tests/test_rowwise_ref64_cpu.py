@@ -5,11 +5,11 @@ tests/test_rowwise_fp64_gpu.py compares the kernels with.
 * soundness: an fp32 emulation of each kernel's operation order (its lane layout, float4 sums, butterflies, fmaf epilogues; rsqrtf,
   ex2 and __fdividef perturbed by their documented error) stays inside the bound on every input family;
 * sharpness: each plausible kernel mistake, emulated in fp32 the same way, lands outside the bound on the designed inputs;
-* coverage: the instantiation tables of rowwise.cu, the oracle's copies of them and the GPU test's parameter lists agree, so a new
-  instantiation fails here until the GPU test has a case for it."""
+* coverage: the kernel instances of the built library, the oracle's tables of them and the GPU test's parameter lists agree, so a
+  new instantiation fails here until the oracle lists it and the GPU test has a case for it."""
 import math
-import os
 import re
+import subprocess
 
 import pytest
 import torch
@@ -23,7 +23,6 @@ F32 = torch.float32
 BF = torch.bfloat16
 LOG2E_F32 = torch.tensor(1.4426950408889634, dtype=F32)
 EPS = 1e-5
-SRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "sigma_b200", "csrc", "rowwise.cu")
 
 
 # ---------------------------------------------------------------- fp32 emulation of the kernels
@@ -528,33 +527,39 @@ def test_shuffle_and_gather_mistakes_are_rejected():
     _outside(emu_norm(swapped[None], g4, b4, EPS, plan4), ref, bound, "patch-merge quadrants swapped")
 
 
-# ---------------------------------------------------------------- coverage cross-check
-def _block(src, start):
-    i = src.index(start)
-    return src[i:src.index("#undef TRY", i)]
+# ---------------------------------------------------------------- coverage cross-check, against the built library
+_ELEM = {"float": "f32", "__nv_bfloat16": "bf16", "__half": "f16", "sigma::E4M3Rows": "e4m3"}
+_BWD = ("layernorm_bwd_kernel", "layernorm_bwd_det_kernel", "layernorm_bwd_bf16_kernel", "layernorm_bwd_fp16_kernel")
 
 
-def _pairs(text):
-    return [(int(a), int(b)) for a, b in re.findall(r"TRY\((\d+),\s*(\d+)\)", text)]
+@pytest.fixture(scope="module")
+def instances():
+    """{kernel: set of template-argument tuples} of the row-wise kernels in libsigma_b200.so (`cuobjdump -sass`, demangled by
+    cu++filt); integer arguments as ints, element types by the oracle's names"""
+    from sigma_b200 import _lib
+    out = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    names = subprocess.run(["cu++filt"], input="\n".join(re.findall(r"Function : (\S+)", out)), capture_output=True, text=True,
+                           check=True).stdout
+    inst = {}
+    for kernel, args in re.findall(r"sigma::(row_norm\w*|layernorm_bwd\w*|upsample2x_norm\w*)<([^<>]*)>\(", names):
+        inst.setdefault(kernel, set()).add(tuple(int(a[5:]) if a.startswith("(int)") else _ELEM[a] for a in args.split(", ")))
+    return inst
 
 
-def test_instantiation_tables_are_covered():
-    src = open(SRC).read()
-    row = _pairs(_block(src, "static bool row_norm_fast("))
-    head = _pairs(_block(src, "static bool upsample2x_norm_head_fast("))
-    bwd = _pairs(_block(src, "int layernorm_bwd_launch("))
-    i = src.index("int upsample2x_norm_launch(")
-    cases = [int(n) for n in re.findall(r"CASE\((\d+)\)", src[i:src.index("set_error", i)])]
-    mh = re.search(r"NCLS > (\d+)\) return false", src)
-    assert row and head and bwd and cases and mh
-    assert row == R.ROW_FAST and head == R.HEAD_FAST and bwd == R.BWD_FAST and cases == R.HEAD_NCLS
-    assert int(mh.group(1)) == R.HEAD_FAST_MAX_NCLS
+def test_instantiation_tables_are_covered(instances):
+    row = {(l, v) for l, v, *_ in instances["row_norm_fast_kernel"]}
+    head = instances["upsample2x_norm_head_fast_kernel"]
+    cases = sorted({n for _, n in instances["upsample2x_norm_kernel"]} - {0})
+    fast_ncls = {n for n in cases if n <= R.HEAD_FAST_MAX_NCLS}
+    assert row == set(R.ROW_FAST) and cases == R.HEAD_NCLS
+    assert all(instances[k] == set(R.BWD_FAST) for k in _BWD)
+    # the fast head at every class count up to HEAD_FAST_MAX_NCLS (NCLS 1: the placeholder the larger class counts compile)
+    assert head == {(l, v, n) for l, v in R.HEAD_FAST for n in fast_ncls | {1}}
     # the GPU test reaches every instantiation
     assert {4 * l * v for l, v in row} <= set(G.LN_FAST_D)
     assert {R.row_plan(D)[1] for D in G.LN_GENERIC_D if not R.row_plan(D)[2]} == set(R.MAXV_GENERIC)
     assert all(R.row_plan(D)[2] for D in G.MERGE_D) and set(G.MERGE_K) == set(range(1, 9))
-    assert {4 * l * v for l, v in head} <= set(G.HEAD_FAST_C)
-    fast_ncls = {n for n in cases if n <= R.HEAD_FAST_MAX_NCLS}
+    assert {4 * l * v for l, v in R.HEAD_FAST} <= set(G.HEAD_FAST_C)
     assert fast_ncls <= set(G.HEAD_FAST_NCLS) and set(cases) - fast_ncls <= set(G.HEAD_GENERIC_NCLS)
     assert all(not R.head_plan(C, 9)[2] for C in G.HEAD_GENERIC_C)
     assert {R.head_plan(C, 0)[1] for C in G.UPSAMPLE_C} == {1, 2, 4, 8}
@@ -562,28 +567,16 @@ def test_instantiation_tables_are_covered():
     assert {4 * l * v for l, v in row} <= set(G.SHUFFLE_D)
 
 
-_IO = {("float", "float"): 0, ("float", "bf16"): 1, ("bf16", "bf16"): 2}
-
-
-def _io(ti, to):
-    return _IO[tuple("bf16" if t == "__nv_bfloat16" else t for t in (ti, to))]
-
-
-def test_io_dispatch_is_the_oracles_and_covered():
-    """row_norm_fast_k's (io, mode, K) instances and row_norm_launch's generic (io, MAXV) ones, parsed from rowwise.cu, are the
-    oracle's (ROW_FAST_IO, MAXV_GENERIC), and the GPU test's parameter lists reach every one of them at every fast width; the bf16
-    LayerNorm backward exists and its GPU test runs every BWD_FAST width"""
-    src = open(SRC).read()
-    i = src.index("static bool row_norm_fast_k(")
-    fast = {(_io(ti, to), int(mode), int(k))
-            for k, mode, ti, to in re.findall(r"row_norm_fast_kernel<LPR, V, (\d), (\d), (\w+), (\w+)>", src[i:src.index("\n}\n", i)])}
-    assert fast == {(io, mode, k) for io, modes in R.ROW_FAST_IO.items() for mode, ks in modes.items() for k in ks}
-    i = src.index("int row_norm_launch(")
-    body = src[i:src.index("\n}\n", i)]
-    gen_io = {_io(ti, to) for ti, to in re.findall(r"row_norm_kernel<MV, (\w+), (\w+)>", body)}
-    maxv = [int(m) for m in re.findall(r"LAUNCH\((\d+)\);", body)]
-    assert gen_io == {0, 1, 2} and tuple(maxv) == R.MAXV_GENERIC
-    # what the GPU cases reach: fast (io, mode, K, lanes, vecs) and generic (io, MAXV)
+def test_row_norm_instances_are_the_oracles_and_covered(instances):
+    """The built row_norm_fast_kernel and row_norm_kernel instances are exactly the oracle's: every fast width at each (mode, K) of
+    ROW_FAST_PAIRS, and the generic kernel at each MAXV of ROW_GENERIC_MAXV, for all seven element pairs.  The GPU test's parameter
+    lists reach every fp32 / bf16 instance of them at every fast width, and its bf16 LayerNorm backward runs every BWD_FAST width."""
+    fast, generic = instances["row_norm_fast_kernel"], instances["row_norm_kernel"]
+    assert fast == {(l, v, k, mode, *pair) for pair, modes in R.ROW_FAST_PAIRS.items() for mode, ks in modes.items() for k in ks
+                    for l, v in R.ROW_FAST}
+    assert generic == {(mv, *pair) for pair, mvs in R.ROW_GENERIC_MAXV.items() for mv in mvs}
+    assert len(fast) == 209 and len(generic) == 38
+    # what the GPU cases reach: fast (lanes, vecs, K, mode, pair) and generic (MAXV, pair)
     cases = [(D, 1, 0, io) for D in G.LN_FAST_D + G.LN_GENERIC_D for io in G.LN_IO]
     cases += [(D, K, 0, io) for K in G.MERGE_K for D in G.MERGE_D for io in G.MERGE_IO]
     cases += [(4 * C, 1, 1, io) for C in G.PATCH_MERGE_C for io in G.PATCH_MERGE_IO]
@@ -591,9 +584,7 @@ def test_io_dispatch_is_the_oracles_and_covered():
     reached = set()
     for D, K, mode, io in cases:
         lanes, vecs, is_fast = R.row_plan(D, K, mode, io)
-        reached.add((io, mode, K, lanes, vecs) if is_fast else (io, vecs))
-    want = {(io, mode, k, l, v) for io, mode, k in fast for l, v in R.ROW_FAST} | {(io, mv) for io in gen_io for mv in maxv}
+        reached.add((lanes, vecs, K, mode, *R.IO_PAIRS[io]) if is_fast else (vecs, *R.IO_PAIRS[io]))
+    want = {i for i in fast | generic if i[-2:] in set(R.IO_PAIRS.values())}
     assert want <= reached, sorted(want - reached)
-    i = src.index("static void layernorm_bwd_k(")
-    assert "layernorm_bwd_bf16_kernel<LPR, V>" in src[i:src.index("\n}\n", i)]
     assert set(G.BWD_BF16_D) == {4 * l * v for l, v in R.BWD_FAST}
