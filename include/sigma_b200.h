@@ -429,6 +429,29 @@ int sigma_merge_norm_gate_fwd_fp8(const void *y, int K, int64_t k_stride, int64_
 int sigma_conv3x3_tf32(const float *x, const float *w9, const float *w9_lo, const float *bias, int act, float *y, int batch, int H, int W,
                        int Cin, int Cout, void *stream);
 
+/* Training of conv3x3 + GELU (the ChannelAttentionBlock's first conv and its activation; ops.CabConvFn).  Same layouts, precision
+ * rule (w9_lo) and checks as sigma_conv3x3_tf32.  Forward that keeps the pre-activation: pre = conv(x, w9) + bias and
+ * y = GELU(pre) (exact, erf), both (batch, H, W, Cout).  bias may be NULL.                                                   */
+int sigma_conv3x3_gelu_save_tf32(const float *x, const float *w9, const float *w9_lo, const float *bias, float *y, float *pre, int batch,
+                                 int H, int W, int Cin, int Cout, void *stream);
+/* Data gradient of a 3x3 conv (pad 1) with Cin inputs and Cout outputs: dx (batch, H, W, Cin) = the 3x3 conv of dy (batch, H, W, Cout)
+ * with w9t (3·3, Cin, Cout), the weight flipped in the taps and transposed: w9t[tap][ci][co] = w[co][ci][8 − tap] of the nn.Conv2d
+ * weight w (Cout, Cin, 3, 3) (w9t_lo: its tf32x3 split, or NULL for TF32).  gelu_pre != NULL (batch, H, W, Cin): dx is multiplied
+ * by GELU'(gelu_pre) = Φ(u) + u·φ(u), the gradient at the pre-activation of a GELU that fed the conv.  Cin, Cout % 4 == 0.     */
+int sigma_conv3x3_dgrad_tf32(const float *dy, const float *w9t, const float *w9t_lo, const float *gelu_pre, float *dx, int batch, int H,
+                             int W, int Cin, int Cout, void *stream);
+/* Weight gradient of the same conv: dw (Cout, Cin, 3, 3) = Σ over pixels of dy[p, co]·x[p + s(tap), ci] (nn.Conv2d's layout) and
+ * dbias (Cout) = Σ dy (NULL: not computed); x (batch, H, W, Cin) or, gelu_x = 1, the pre-activation whose GELU was the conv's input.
+ * x3 = 0: one TF32 MMA per k-step; 1: tf32x3 (fp32 grade).  Deterministic by construction: each CTA sums a fixed pixel range into one
+ * partial row of the caller's workspace (sigma_conv3x3_wgrad_workspace_bytes, 16-byte aligned), and the rows are added in order, so
+ * the same inputs give the same bits with or without a deterministic mode.  Cin, Cout % 4 == 0; x, dy 16-byte aligned.            */
+size_t sigma_conv3x3_wgrad_workspace_bytes(int batch, int H, int W, int Cin, int Cout);
+int sigma_conv3x3_wgrad_tf32(const float *x, int gelu_x, const float *dy, float *dw, float *dbias, int batch, int H, int W, int Cin,
+                             int Cout, int x3, void *workspace, size_t workspace_bytes, void *stream);
+/* Launch plan of sigma_conv3x3_wgrad_tf32, host only (no CUDA call): out4_host = {output channels per tile, output tiles, partial
+ * rows (pixel ranges), CTAs}.  A function of the shape alone.                                                                  */
+int sigma_test_conv3x3_wgrad_plan(int batch, int H, int W, int Cin, int Cout, int64_t *out4_host);
+
 /* Launch plan of the two calls above, host only (no CUDA call, works without a GPU): what sigma_linear_tf32{,x3} (conv_B = 0; M rows,
  * N outputs, K inputs) or sigma_conv3x3_tf32 (conv_B > 0: input (conv_B, conv_H, conv_W, K), N = Cout; M unused) would launch under
  * the current environment.  out6_host = {tile width, ring stages, persistent grid, output tiles, dynamic shared memory bytes, CTAs

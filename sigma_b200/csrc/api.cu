@@ -1057,6 +1057,57 @@ int sigma_conv3x3_tf32(const float *x, const float *w9, const float *w9_lo, cons
   return conv3x3_tf32_launch(x, w9, w9_lo, bias, act, y, batch, H, W, Cin, Cout, (cudaStream_t)stream);
 }
 
+int sigma_conv3x3_gelu_save_tf32(const float *x, const float *w9, const float *w9_lo, const float *bias, float *y, float *pre, int batch,
+                                 int H, int W, int Cin, int Cout, void *stream) {
+  SIGMA_CHECK_ARG(x && w9 && y && pre, "sigma_conv3x3_gelu_save_tf32: null pointer");
+  SIGMA_CHECK_ARG(batch >= 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && Cin % 4 == 0 && Cout % 4 == 0,
+                  "sigma_conv3x3_gelu_save_tf32: bad sizes (Cin=%d, Cout=%d must be multiples of 4)", Cin, Cout);
+  SIGMA_CHECK_ARG(al16(x) && al16(w9) && al16(w9_lo) && al16(bias) && al16(y) && al16(pre),
+                  "sigma_conv3x3_gelu_save_tf32: pointers must be 16-byte aligned");
+  return conv3x3_tf32_launch(x, w9, w9_lo, bias, 1, y, batch, H, W, Cin, Cout, (cudaStream_t)stream, 1, pre);
+}
+
+int sigma_conv3x3_dgrad_tf32(const float *dy, const float *w9t, const float *w9t_lo, const float *gelu_pre, float *dx, int batch, int H,
+                             int W, int Cin, int Cout, void *stream) {
+  SIGMA_CHECK_ARG(dy && w9t && dx, "sigma_conv3x3_dgrad_tf32: null pointer");
+  SIGMA_CHECK_ARG(batch >= 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && Cin % 4 == 0 && Cout % 4 == 0,
+                  "sigma_conv3x3_dgrad_tf32: bad sizes (Cin=%d, Cout=%d must be multiples of 4)", Cin, Cout);
+  SIGMA_CHECK_ARG(al16(dy) && al16(w9t) && al16(w9t_lo) && al16(gelu_pre) && al16(dx),
+                  "sigma_conv3x3_dgrad_tf32: pointers must be 16-byte aligned");
+  // the conv of dy (Cout channels in) to dx (Cin channels out)
+  return conv3x3_tf32_launch(dy, w9t, w9t_lo, nullptr, 0, dx, batch, H, W, Cout, Cin, (cudaStream_t)stream, gelu_pre ? 2 : 0,
+                             (float *)gelu_pre);
+}
+
+size_t sigma_conv3x3_wgrad_workspace_bytes(int batch, int H, int W, int Cin, int Cout) {
+  if (batch <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0) return 0;
+  return conv3x3_wgrad_workspace_bytes(batch, H, W, Cin, Cout);
+}
+
+int sigma_conv3x3_wgrad_tf32(const float *x, int gelu_x, const float *dy, float *dw, float *dbias, int batch, int H, int W, int Cin,
+                             int Cout, int x3, void *workspace, size_t workspace_bytes, void *stream) {
+  SIGMA_CHECK_ARG(x && dy && dw, "sigma_conv3x3_wgrad_tf32: null pointer");
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && Cin % 4 == 0 && Cout % 4 == 0,
+                  "sigma_conv3x3_wgrad_tf32: bad sizes batch=%d H=%d W=%d Cin=%d Cout=%d (Cin, Cout must be multiples of 4)", batch, H,
+                  W, Cin, Cout);
+  SIGMA_CHECK_ARG((gelu_x == 0 || gelu_x == 1) && (x3 == 0 || x3 == 1), "sigma_conv3x3_wgrad_tf32: gelu_x and x3 must be 0 or 1");
+  SIGMA_CHECK_ARG(al16(x) && al16(dy), "sigma_conv3x3_wgrad_tf32: x and dy must be 16-byte aligned");
+  const size_t need = conv3x3_wgrad_workspace_bytes(batch, H, W, Cin, Cout);
+  if (workspace == nullptr || !al16(workspace) || workspace_bytes < need) {
+    set_error("sigma_conv3x3_wgrad_tf32: needs %zu 16-byte aligned workspace bytes, got %zu", need, workspace ? workspace_bytes : 0);
+    return SIGMA_EWORKSPACE;
+  }
+  return conv3x3_wgrad_launch(x, gelu_x, dy, dw, dbias, batch, H, W, Cin, Cout, x3, workspace, (cudaStream_t)stream);
+}
+
+int sigma_test_conv3x3_wgrad_plan(int batch, int H, int W, int Cin, int Cout, int64_t *out4_host) {
+  SIGMA_CHECK_ARG(out4_host && batch > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0, "sigma_test_conv3x3_wgrad_plan: bad arguments");
+  long long out[4];
+  conv3x3_wgrad_plan(batch, H, W, Cin, Cout, out);
+  for (int i = 0; i < 4; ++i) out4_host[i] = out[i];
+  return SIGMA_OK;
+}
+
 int sigma_split_tf32_fwd(const float *x, float *hi, float *lo, int64_t n, void *stream) {
   SIGMA_CHECK_ARG(x && hi && lo && n >= 0, "sigma_split_tf32_fwd: bad arguments");
   return split_tf32_launch(x, hi, lo, n, (cudaStream_t)stream);

@@ -49,6 +49,7 @@ struct alignas(64) GemmParams {
   int cH, cW, tiles_w, tiles_hw, kbc, act;   // CONV: image size, 8x16 patches per row / per image, Cin blocks per tap, activation
   const float *sa, *sw;   // FP8: per-row scales of A, per-output-channel scales of W
   CUtensorMap m_c, m_r;   // TMA_C: C and (if any) the residual, GM_CHUNK x 64 boxes
+  float *aux;             // conv3x3_epi_kernel: EPI 1 stores the pre-activation here, EPI 2 reads GELU's input from it (C's layout)
 };
 
 // One ring stage holds a k-block's K-major, 128-byte-swizzled operand tiles, each 1024-aligned: [A | W].  tf32x3 adds W_lo:
@@ -812,6 +813,11 @@ __device__ __forceinline__ void load_residual_chunk(const GemmParams &p, unsigne
   tma_load_2d(stg + (e & 1) * GM_CHUNK_BYTES, &p.m_r, &rfull[e & 1], col, row);
 }
 
+// d/du of nn.GELU()'s exact form u·Φ(u): Φ(u) + u·φ(u)
+__device__ __forceinline__ float gelu_grad(float u) {
+  return 0.5f * (1.f + erff(u * 0.70710678118654752f)) + u * 0.39894228040143268f * expf(-0.5f * u * u);
+}
+
 // The body of every instance.  FP8 (gemm_fp8_kernel): e4m3 operands, 128 per k-block; each k-block's four k32 MMAs accumulate
 // into a zeroed fragment that is then added to the fp32 accumulators in registers (the tensor core's e4m3 accumulation keeps
 // fewer bits than fp32, DESIGN §5.4), and the epilogue scales acc[row, col] by sa[row]·sw[col] before the bias / residual.
@@ -819,8 +825,11 @@ __device__ __forceinline__ void load_residual_chunk(const GemmParams &p, unsigne
 // stores them with TMA, asynchronously, so the consumers go on to the next tile's MMAs while the stores drain; the residual
 // chunks arrive by TMA as well, the first two during the tile's k-loop.
 // F16 (gemm_fp16_kernel): the BF16 instance on fp16 operands, C fp32 or (p.c_bf16) fp16.
-template <int BN, bool X3, bool CONV, bool BF16, bool FP8, bool TMA_C = false, bool F16 = false>
+// EPI (conv3x3_epi_kernel, the CAB convs' training instances): 1 = also store pre = conv + bias to p.aux before the GELU;
+// 2 = multiply the result by GELU'(p.aux) (the data gradient of the second conv, emitted at the first conv's pre-activation).
+template <int BN, bool X3, bool CONV, bool BF16, bool FP8, bool TMA_C = false, bool F16 = false, int EPI = 0>
 __device__ __forceinline__ void gemm_body(const GemmParams &p) {
+  static_assert(EPI == 0 || (CONV && !BF16 && !FP8 && !TMA_C && !F16), "the training epilogues are the fp32 conv's");
   static_assert(!BF16 || (!X3 && !CONV), "the bf16 instance is a plain GEMM");
   static_assert(!FP8 || (!X3 && !CONV && !BF16), "the e4m3 instance is a plain GEMM");
   static_assert(!F16 || (!X3 && !CONV && !BF16 && !FP8), "the fp16 instance is a plain GEMM");
@@ -1088,6 +1097,11 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
             o.x += rv.x; o.y += rv.y;
           }
         }
+        if constexpr (EPI == 1) *reinterpret_cast<float2 *>(p.aux + coff + n) = o;
+        if constexpr (EPI == 2) {
+          const float2 u = *reinterpret_cast<const float2 *>(p.aux + coff + n);
+          o.x *= gelu_grad(u.x); o.y *= gelu_grad(u.y);
+        }
         if (CONV && p.act == 1) {   // nn.GELU() (exact, erf)
           o.x = 0.5f * o.x * (1.f + erff(o.x * 0.70710678118654752f));
           o.y = 0.5f * o.y * (1.f + erff(o.y * 0.70710678118654752f));
@@ -1107,6 +1121,13 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
 template <int BN, bool X3, bool CONV, bool BF16 = false>
 __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_tf32_kernel(const __grid_constant__ GemmParams p) {
   gemm_body<BN, X3, CONV, BF16, false>(p);
+}
+
+// The conv's training instances (CabConvFn): EPI 1 = the forward that keeps the pre-activation, EPI 2 = the data gradient with the
+// GELU' factor.  A separate kernel, so that gemm_tf32_kernel keeps its code; widths up to kEpiMaxBn.
+template <int BN, bool X3, int EPI>
+__global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) conv3x3_epi_kernel(const __grid_constant__ GemmParams p) {
+  gemm_body<BN, X3, true, false, false, false, false, EPI>(p);
 }
 
 // The tf32x3 linear instance with the TMA-stored epilogue: fp32 C (and residual) whose rows a tensor map can describe.
@@ -1219,13 +1240,14 @@ constexpr int kFp8MaxBn = 64;
 // conv_B > 0: the implicit-GEMM 3x3 convolution of a (conv_B, conv_H, conv_W, K) input with N output channels (M unused).
 // fp8: the e4m3 instance (widths up to kFp8MaxBn, two CTAs per SM).  tma_c: the tf32x3 linear instance with the TMA-stored
 // epilogue, whose staging buffers come out of the budget before the ring.
+// max_bn: the widest instance of the kernel that will run (conv3x3_epi_kernel: kEpiMaxBn).
 static int plan_gemm(long long M, int N, int K, bool x3, int conv_B, int conv_H, int conv_W, GemmPlan *pl, bool fp8 = false,
-                     bool tma_c = false) {
+                     bool tma_c = false, int max_bn = 256) {
   (void)K;   // the K loop does not enter the plan
   const bool conv = conv_B > 0;
   const long long m_tiles = conv ? (long long)conv_B * ((conv_W + CV_TW - 1) / CV_TW) * ((conv_H + CV_TH - 1) / CV_TH)
                                  : (M + GM_BM - 1) / GM_BM;
-  int bn = conv ? pick_bn(N) : pick_bn(N, m_tiles, fp8 ? kFp8MaxBn : 256);
+  int bn = conv ? pick_bn(N, 1 << 30, max_bn) : pick_bn(N, m_tiles, fp8 ? kFp8MaxBn : 256);
   if (!conv && !fp8) {
     if (const char *e = getenv("SIGMA_GEMM_BN_RULE")) { if (e[0] == 'o') bn = pick_bn(N); }   // "old": ignore the row-tile count
   }
@@ -1233,6 +1255,10 @@ static int plan_gemm(long long M, int N, int K, bool x3, int conv_B, int conv_H,
   if (fbn < 0) return fbn;
   if (fbn > 0 && fp8 && fbn > kFp8MaxBn) {
     set_error("SIGMA_GEMM_BN=%d: the e4m3 GEMM's tiles are at most %d wide", fbn, kFp8MaxBn);
+    return SIGMA_EINVAL;
+  }
+  if (fbn > max_bn) {
+    set_error("SIGMA_GEMM_BN=%d: this conv's tiles are at most %d wide", fbn, max_bn);
     return SIGMA_EINVAL;
   }
   if (fbn > 0) bn = fbn;
@@ -1372,18 +1398,23 @@ int gemm_fp8_launch(const void *A, long long lda, const float *sa, const void *W
   return SIGMA_OK;
 }
 
+// The widest tile of conv3x3_epi_kernel: the CAB's C/3 (32 / 64 / 128 in Sigma-tiny and -small) fits one tile; wider outputs
+// take several.
+constexpr int kEpiMaxBn = 128;
+
 // 3x3 convolution, pad 1, stride 1, channels-last: y (B,H,W,Cout) = conv(x (B,H,W,Cin), W9 (9, Cout, Cin)) + bias, optional GELU.
-// W9_lo == nullptr: plain TF32; else tf32x3 with W9 = W9_hi.
+// W9_lo == nullptr: plain TF32; else tf32x3 with W9 = W9_hi.  epi 1 (act 1): pre = conv + bias also stored to aux; epi 2 (act 0):
+// the result times GELU'(aux); both run conv3x3_epi_kernel.
 int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, const float *bias, int act, float *y, int B, int H, int W,
-                        int Cin, int Cout, cudaStream_t stream) {
+                        int Cin, int Cout, cudaStream_t stream, int epi, float *aux) {
   if (B == 0) return SIGMA_OK;
   const bool x3 = W9_lo != nullptr;
   GemmPlan pl;
   int rc;
-  if ((rc = plan_gemm(0, Cout, Cin, x3, B, H, W, &pl))) return rc;
+  if ((rc = plan_gemm(0, Cout, Cin, x3, B, H, W, &pl, false, false, epi ? kEpiMaxBn : 256))) return rc;
   GemmParams p;
   memset(&p, 0, sizeof(p));
-  p.bias = bias; p.C = y;
+  p.bias = bias; p.C = y; p.aux = aux;
   p.N = Cout; p.K = Cin;
   p.cH = H; p.cW = W; p.act = act;
   p.tiles_w = (W + CV_TW - 1) / CV_TW;
@@ -1400,7 +1431,24 @@ int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, con
   }
   if ((rc = make_tmap_2d_sw128(&p.m_w, W9, 9LL * Cout, Cin, Cin, p.BN))) return rc;
   if (x3 && (rc = make_tmap_2d_sw128(&p.m_wlo, W9_lo, 9LL * Cout, Cin, Cin, p.BN))) return rc;
-  return x3 ? launch_gemm<true, true>(p, pl, stream) : launch_gemm<false, true>(p, pl, stream);
+  if (epi == 0) return x3 ? launch_gemm<true, true>(p, pl, stream) : launch_gemm<false, true>(p, pl, stream);
+  p.stages = pl.stages;
+  const void *kern = nullptr;
+  switch (p.BN) {
+#define SIGMA_EPI_BN(bn)                                                                                                         \
+  case bn:                                                                                                                       \
+    kern = epi == 1 ? (x3 ? (const void *)conv3x3_epi_kernel<bn, true, 1> : (const void *)conv3x3_epi_kernel<bn, false, 1>)      \
+                    : (x3 ? (const void *)conv3x3_epi_kernel<bn, true, 2> : (const void *)conv3x3_epi_kernel<bn, false, 2>);     \
+    break;
+    SIGMA_EPI_BN(32) SIGMA_EPI_BN(64) SIGMA_EPI_BN(96) SIGMA_EPI_BN(128)
+#undef SIGMA_EPI_BN
+    default: set_error("conv3x3: the training epilogues have tiles of at most %d columns, not %d", kEpiMaxBn, p.BN); return SIGMA_EINVAL;
+  }
+  SIGMA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
+  void *args[] = {&p};
+  SIGMA_CHECK_CUDA(cudaLaunchKernel(kern, dim3(pl.grid), dim3(GM_THREADS), args, pl.smem, stream));
+  count_launch();
+  return SIGMA_OK;
 }
 
 }  // namespace sigma

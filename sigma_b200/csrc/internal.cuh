@@ -191,11 +191,19 @@ int gemm_16bit_launch(int dtype, const void *A, long long lda, const void *W, co
 int gemm_fp8_launch(const void *A, long long lda, const float *sa, const void *W, const float *sw, const float *bias,
                     const float *residual, long long ldr, const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N,
                     int K, cudaStream_t stream);
+// epi 1 (with act 1): also store pre = conv + bias to aux; epi 2 (act 0): multiply the result by GELU'(aux) (aux in y's layout)
 int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, const float *bias, int act, float *y, int B, int H, int W,
-                        int Cin, int Cout, cudaStream_t stream);
+                        int Cin, int Cout, cudaStream_t stream, int epi = 0, float *aux = nullptr);
 int split_tf32_launch(const float *x, float *hi, float *lo, long long n, cudaStream_t stream);
 int gemm_pick_bn_hook(int N, long long m_tiles);
 int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out);
+
+// ---- conv3x3_wgrad.cu ----
+// Launch plan of the weight gradient: {output channels per tile, output tiles, partial rows, CTAs}
+void conv3x3_wgrad_plan(int batch, int H, int W, int Cin, int Cout, long long *out4);
+size_t conv3x3_wgrad_workspace_bytes(int batch, int H, int W, int Cin, int Cout);
+int conv3x3_wgrad_launch(const float *x, int gelu_x, const float *dy, float *dw, float *db, int batch, int H, int W, int Cin, int Cout,
+                         int x3, void *ws, cudaStream_t stream);
 
 // ---- evaluator.cu ----
 int argmax_hist_launch(const float *logits, const void *labels, int label_bytes, unsigned long long *hist,

@@ -531,6 +531,102 @@ class DwConvSiLUFn(torch.autograd.Function):
         return dx, dw, db
 
 
+# ---- the ChannelAttentionBlock's dense convs under autograd ----
+# On, CVSSDecoderBlock's training forward runs cab[0] -> GELU -> cab[2] as one CabConvFn on channels-last tensors (library kernels
+# forward and backward); off, it runs nn.Conv2d (cuDNN) on an NCHW copy.  Applies to fp32 without autocast (cab_conv_ok).
+FUSED_CAB_TRAINING = True
+
+
+def _conv3x3_ok(conv):
+    return (isinstance(conv, torch.nn.Conv2d) and conv.kernel_size == (3, 3) and conv.stride == (1, 1) and conv.padding == (1, 1)
+            and conv.dilation == (1, 1) and conv.groups == 1 and conv.in_channels % 4 == 0 and conv.out_channels % 4 == 0
+            and conv.bias is not None and conv.padding_mode == "zeros")
+
+
+def cab_conv_ok(cab, x):
+    """CabConvFn takes `cab` (the nn.Sequential of ChannelAttentionBlock) on x: autograd recording, both switches on, fp32 CUDA x with
+    autocast off, an exact nn.GELU between two 3x3 / pad 1 / stride 1 convs whose channel counts are multiples of 4"""
+    return (FUSED_TRAINING and FUSED_CAB_TRAINING and torch.is_grad_enabled() and x.is_cuda and x.dtype == torch.float32
+            and not torch.is_autocast_enabled("cuda") and isinstance(cab[1], torch.nn.GELU) and cab[1].approximate == "none"
+            and _conv3x3_ok(cab[0]) and _conv3x3_ok(cab[2]) and cab[0].out_channels == cab[2].in_channels)
+
+
+def _tf32_split(w):
+    """(hi, lo) of sigma_split_tf32_fwd, computed per call (inside a captured graph, so a replayed optimizer step is seen)"""
+    hi, lo = torch.empty_like(w), torch.empty_like(w)
+    _lib.check(_lib.lib().sigma_split_tf32_fwd(ptr(w), ptr(hi), ptr(lo), w.numel(), stream()), "sigma_split_tf32_fwd")
+    return hi, lo
+
+
+def _w9(w, x3, grad=False):
+    """the nn.Conv2d weight (Cout, Cin, 3, 3) as the conv kernel's (9, Cout, Cin) or, grad, the data gradient's flipped and transposed
+    (9, Cin, Cout), with its tf32x3 split when x3 (else lo = None)"""
+    w = w.detach()
+    w9 = (w.flip(2, 3).permute(2, 3, 1, 0) if grad else w.permute(2, 3, 0, 1)).reshape(-1, w.shape[0] if grad else w.shape[1]).contiguous()
+    return _tf32_split(w9) if x3 else (w9, None)
+
+
+class CabConvFn(torch.autograd.Function):
+    """cab[2](GELU(cab[0](x))) of ChannelAttentionBlock on a channels-last fp32 x (B, H, W, C) -> (B, H, W, C) under autograd, both
+    convs 3x3 / pad 1 with bias.  Forward = sigma_conv3x3_gelu_save_tf32 (conv 1 + bias, keeping the pre-activation, and its GELU)
+    + sigma_conv3x3_tf32 (conv 2 + bias); backward = sigma_conv3x3_wgrad_tf32 of conv 2 (GELU applied to the saved pre-activation as
+    it is staged), sigma_conv3x3_dgrad_tf32 of conv 2 times GELU', then the wgrad and dgrad of conv 1.  It saves x and the
+    pre-activation, not the GELU output.  Precision follows torch.backends.cudnn.allow_tf32 at the forward, as nn.Conv2d's does (True:
+    one TF32 MMA per k-step; False: tf32x3).  The weights are re-ordered (and split) per call, never from an inference cache, so a
+    graph-replayed step sees the optimizer's updates.  The weight gradients are deterministic by construction (fixed-order partial
+    sums), with or without torch.use_deterministic_algorithms(True)."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2):
+        x = x.contiguous()
+        B, H, W, C = x.shape
+        C1 = w1.shape[0]
+        x3 = not torch.backends.cudnn.allow_tf32
+        L_ = _lib.lib()
+        pre = torch.empty((B, H, W, C1), dtype=torch.float32, device=x.device)
+        h = torch.empty_like(pre)
+        hi, lo = _w9(w1, x3)
+        _lib.check(L_.sigma_conv3x3_gelu_save_tf32(ptr(x), ptr(hi), ptr(lo), ptr(b1), ptr(h), ptr(pre), B, H, W, C, C1, stream()),
+                   "sigma_conv3x3_gelu_save_tf32")
+        y = torch.empty((B, H, W, w2.shape[0]), dtype=torch.float32, device=x.device)
+        hi, lo = _w9(w2, x3)
+        _lib.check(L_.sigma_conv3x3_tf32(ptr(h), ptr(hi), ptr(lo), ptr(b2), 0, ptr(y), B, H, W, C1, w2.shape[0], stream()),
+                   "sigma_conv3x3_tf32")
+        ctx.save_for_backward(x, pre, w1, w2)
+        ctx.x3 = x3
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, pre, w1, w2 = ctx.saved_tensors
+        dy = dy.contiguous()
+        B, H, W, C = x.shape
+        C1, C2 = w1.shape[0], w2.shape[0]
+        L_ = _lib.lib()
+
+        def wgrad(xin, gelu_x, g, cin, cout):
+            dw = torch.empty((cout, cin, 3, 3), dtype=torch.float32, device=x.device)
+            db = torch.empty(cout, dtype=torch.float32, device=x.device)
+            wsb = L_.sigma_conv3x3_wgrad_workspace_bytes(B, H, W, cin, cout)
+            ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+            _lib.check(L_.sigma_conv3x3_wgrad_tf32(ptr(xin), gelu_x, ptr(g), ptr(dw), ptr(db), B, H, W, cin, cout, int(ctx.x3), ptr(ws),
+                                                   wsb, stream()), "sigma_conv3x3_wgrad_tf32")
+            return dw, db
+
+        def dgrad(g, w, gelu_pre, cin, cout):
+            dx = torch.empty((B, H, W, cin), dtype=torch.float32, device=x.device)
+            hi, lo = _w9(w, ctx.x3, grad=True)
+            _lib.check(L_.sigma_conv3x3_dgrad_tf32(ptr(g), ptr(hi), ptr(lo), ptr(gelu_pre), ptr(dx), B, H, W, cin, cout, stream()),
+                       "sigma_conv3x3_dgrad_tf32")
+            return dx
+
+        dw2, db2 = wgrad(pre, 1, dy, C1, C2)
+        dpre = dgrad(dy, w2, pre, C1, C2)          # the gradient at conv 1's pre-activation
+        dw1, db1 = wgrad(x, 0, dpre, C, C1)
+        dx = dgrad(dpre, w1, None, C, C1)
+        return dx, dw1, db1, dw2, db2
+
+
 _SAVED_BF16 = 2               # `saved` of _call_ss2d_bwd: the arguments are those of sigma_ss2d_scan_bwd_saved_bf16
 _SAVED_FP16 = 3               # ... of sigma_ss2d_scan_bwd_saved_fp16 (the same layout)
 
