@@ -452,6 +452,26 @@ int sigma_conv3x3_wgrad_tf32(const float *x, int gelu_x, const float *dy, float 
  * rows (pixel ranges), CTAs}.  A function of the shape alone.                                                                  */
 int sigma_test_conv3x3_wgrad_plan(int batch, int H, int W, int Cin, int Cout, int64_t *out4_host);
 
+/* The four calls above on pitched rows, for channel counts that are not multiples of 4 (the CAB convs of Sigma-base, whose C/3 is
+ * 42 / 85 / 170; ops.CabConvPitchedFn, fused.cvss_decoder_block).  Each activation and weight is given with its row pitch in
+ * elements: a multiple of 4, at least its channel count.  Channels between the count and the pitch are pad: never read into a kept
+ * output (the conv's tensor maps end at the count, so TMA fills zeros past it) and never written.  Weights are the layouts above
+ * with rows at the pitch: w9 (9·Cout rows of Cin at w9_pitch), w9t (9·Cin rows of Cout at w9t_pitch), w9_lo / w9t_lo (or NULL) at
+ * the same pitch.  dw and dbias keep nn.Conv2d's unpadded layout, and the weight gradient's workspace is
+ * sigma_conv3x3_wgrad_workspace_bytes (the same plan).  x, y, pre (at y_pitch), dy, dx and gelu_pre (at dx_pitch) 16-byte
+ * aligned.  With every pitch equal to its count (a multiple of 4), each call computes what its unpitched twin does.           */
+int sigma_conv3x3_pitched_tf32(const float *x, int x_pitch, const float *w9, int w9_pitch, const float *w9_lo, const float *bias, int act,
+                               float *y, int y_pitch, int batch, int H, int W, int Cin, int Cout, void *stream);
+int sigma_conv3x3_gelu_save_pitched_tf32(const float *x, int x_pitch, const float *w9, int w9_pitch, const float *w9_lo,
+                                         const float *bias, float *y, float *pre, int y_pitch, int batch, int H, int W, int Cin, int Cout,
+                                         void *stream);
+int sigma_conv3x3_dgrad_pitched_tf32(const float *dy, int dy_pitch, const float *w9t, int w9t_pitch, const float *w9t_lo,
+                                     const float *gelu_pre, float *dx, int dx_pitch, int batch, int H, int W, int Cin, int Cout,
+                                     void *stream);
+int sigma_conv3x3_wgrad_pitched_tf32(const float *x, int x_pitch, int gelu_x, const float *dy, int dy_pitch, float *dw, float *dbias,
+                                     int batch, int H, int W, int Cin, int Cout, int x3, void *workspace, size_t workspace_bytes,
+                                     void *stream);
+
 /* Launch plan of the two calls above, host only (no CUDA call, works without a GPU): what sigma_linear_tf32{,x3} (conv_B = 0; M rows,
  * N outputs, K inputs) or sigma_conv3x3_tf32 (conv_B > 0: input (conv_B, conv_H, conv_W, K), N = Cout; M unused) would launch under
  * the current environment.  out6_host = {tile width, ring stages, persistent grid, output tiles, dynamic shared memory bytes, CTAs

@@ -1,17 +1,19 @@
 """Time the ChannelAttentionBlock's dense convs in training: ops.CabConvFn (sigma_conv3x3_gelu_save_tf32 + sigma_conv3x3_tf32 forward,
-sigma_conv3x3_wgrad_tf32 / sigma_conv3x3_dgrad_tf32 backward) against the route it replaces in CVSSDecoderBlock (an NCHW copy of the
+sigma_conv3x3_wgrad_tf32 / sigma_conv3x3_dgrad_tf32 backward), or ops.CabConvPitchedFn (the same on the pitched entry points) where
+C/3 is not a multiple of 4, against the route it replaces in CVSSDecoderBlock (an NCHW copy of the
 LayerNorm output, nn.Conv2d -> nn.GELU -> nn.Conv2d on cuDNN, and the copy back to channels-last), and the whole training step with
 each (ops.FUSED_CAB_TRAINING on / off).
 
     python scripts/bench_cab_train.py [--out DIR (default: a temporary directory)] [--rounds 5] [--iters 20] [--steps 10] [--models sigma_tiny,sigma_small]
-                                      [--skip-step] [--skip-profile]
+                                      [--stages tiny|base] [--skip-step] [--skip-profile]
 
-Op arm: the Sigma-tiny / Sigma-small decoder stages at 480 x 640, batch 2, fp32 with torch's default precision for convolutions
+Op arm: the Sigma-tiny / Sigma-small (--stages tiny: C = 96 / 192 / 384) or Sigma-base (--stages base: C = 128 / 256 / 512, C/3 =
+42 / 85 / 170) decoder stages at 480 x 640, batch 2, fp32 with torch's default precision for convolutions
 (cudnn.allow_tf32 = True: TF32 on both routes), forward + backward.  CUDA events around --iters back-to-back calls, median [min, max]
 of --rounds rounds, the two routes alternating.  Algorithmic FLOPs, counted from the shapes: 2·(B·H·W)·9·C·C1 per conv pass, three
 passes per conv (forward, data and weight gradient); FLOP/s over the measured time, next to the H100 SXM's dense TF32 rate (495
 TFLOP/s).  A torch.profiler run of each route (separate from the timed rounds) gives the per-kernel device time.
-Whole-step arm: Sigma-tiny and Sigma-small at 480 x 640, batch 2, fp32 (TF32 dense layers), AdamW through GraphedTrainStep, the
+Whole-step arm: each of --models (Sigma-base takes CabConvPitchedFn) at 480 x 640, batch 2, fp32 (TF32 dense layers), AdamW through GraphedTrainStep, the
 switch on and off captured as two graphs in one process and replayed alternately, --rounds x --steps; eager peak memory
 (max_memory_allocated over two eager steps) of both.  Profile arm: torch.profiler over one eager Sigma-tiny step per setting; the
 device time of the kernels that belong to the CAB convs (by name) against the step's total.  The card's name and power limit are read
@@ -30,13 +32,13 @@ import types
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-SHAPES = [(2, 120, 160, 96), (2, 60, 80, 192), (2, 30, 40, 384)]
+SHAPES = {"tiny": [(2, 120, 160, 96), (2, 60, 80, 192), (2, 30, 40, 384)], "base": [(2, 120, 160, 128), (2, 60, 80, 256), (2, 30, 40, 512)]}
 TF32_PEAK = 495e12
 # kernel names of the dense convs on either route: ours (the conv instances of gemm_tf32_kernel, the epilogue variants, the weight
-# gradient), cuDNN's convolution, gradient and layout kernels, torch's GELU and its backward.  The patch-embed conv's cuDNN kernels
+# gradient, and their pitched twins), cuDNN's convolution, gradient and layout kernels, torch's GELU and its backward.  The patch-embed conv's cuDNN kernels
 # match too, in both settings alike; the partial sums (sum_parts_det, shared with the depthwise conv's backward) and torch's permute
 # copies are not counted.
-CAB_KERNELS = ("conv3x3_epi", "conv3x3_wgrad", ", true, false>(sigma::GemmParams)", "ImplicitGemmConvolution", "implicit_gemm",
+CAB_KERNELS = ("conv3x3_epi", "conv3x3_wgrad", "cab_conv_pitched", "cab_wgrad_pitched", ", true, false>(sigma::GemmParams)", "ImplicitGemmConvolution", "implicit_gemm",
                "s1688wgrad", "nchwToNhwc", "nhwcToNchw", "GeluCUDAKernelImpl", "GeluBackwardCUDAKernelImpl")
 
 
@@ -69,12 +71,13 @@ def op_arm(a):
     import torch
     from sigma_b200 import ops
     out = []
-    for B, H, W, C in SHAPES:
+    for B, H, W, C in SHAPES[a.stages]:
         g = torch.Generator(device="cuda").manual_seed(0)
         xn = torch.randn(B, H, W, C, device="cuda", generator=g).requires_grad_(True)
         dy = torch.randn(B, H, W, C, device="cuda", generator=g)
         cab = torch.nn.Sequential(torch.nn.Conv2d(C, C // 3, 3, 1, 1), torch.nn.GELU(), torch.nn.Conv2d(C // 3, C, 3, 1, 1)).cuda()
-        arms = {"ours": lambda: ops.CabConvFn.apply(xn, cab[0].weight, cab[0].bias, cab[2].weight, cab[2].bias),
+        node = ops.CabConvFn if (C // 3) % 4 == 0 else ops.CabConvPitchedFn
+        arms = {"ours": lambda: node.apply(xn, cab[0].weight, cab[0].bias, cab[2].weight, cab[2].bias),
                 "cudnn": lambda: cudnn_route(xn, cab)}
 
         def run(fn):
@@ -216,6 +219,7 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--models", default="sigma_tiny,sigma_small")
+    ap.add_argument("--stages", choices=sorted(SHAPES), default="tiny")
     ap.add_argument("--skip-step", action="store_true")
     ap.add_argument("--skip-profile", action="store_true")
     a = ap.parse_args()

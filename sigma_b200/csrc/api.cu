@@ -1108,6 +1108,74 @@ int sigma_test_conv3x3_wgrad_plan(int batch, int H, int W, int Cin, int Cout, in
   return SIGMA_OK;
 }
 
+// a pitch is a multiple of 4 elements (16 bytes: TMA strides, cp.async chunks) and holds the row's channels
+static bool pitch_ok(int pitch, int count) { return pitch >= count && pitch % 4 == 0; }
+
+int sigma_conv3x3_pitched_tf32(const float *x, int x_pitch, const float *w9, int w9_pitch, const float *w9_lo, const float *bias, int act,
+                               float *y, int y_pitch, int batch, int H, int W, int Cin, int Cout, void *stream) {
+  SIGMA_CHECK_ARG(x && w9 && y, "sigma_conv3x3_pitched_tf32: null pointer");
+  SIGMA_CHECK_ARG(batch >= 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && (act == 0 || act == 1),
+                  "sigma_conv3x3_pitched_tf32: bad sizes batch=%d H=%d W=%d Cin=%d Cout=%d or act=%d", batch, H, W, Cin, Cout, act);
+  SIGMA_CHECK_ARG(pitch_ok(x_pitch, Cin) && pitch_ok(w9_pitch, Cin) && pitch_ok(y_pitch, Cout),
+                  "sigma_conv3x3_pitched_tf32: pitches (x %d, w9 %d, y %d) must be multiples of 4 and at least Cin=%d / Cout=%d", x_pitch,
+                  w9_pitch, y_pitch, Cin, Cout);
+  SIGMA_CHECK_ARG(al16(x) && al16(w9) && al16(w9_lo) && al16(bias) && al16(y),
+                  "sigma_conv3x3_pitched_tf32: pointers must be 16-byte aligned");
+  return conv3x3_pitched_launch(x, x_pitch, w9, w9_lo, w9_pitch, bias, act, y, y_pitch, batch, H, W, Cin, Cout, (cudaStream_t)stream);
+}
+
+int sigma_conv3x3_gelu_save_pitched_tf32(const float *x, int x_pitch, const float *w9, int w9_pitch, const float *w9_lo,
+                                         const float *bias, float *y, float *pre, int y_pitch, int batch, int H, int W, int Cin, int Cout,
+                                         void *stream) {
+  SIGMA_CHECK_ARG(x && w9 && y && pre, "sigma_conv3x3_gelu_save_pitched_tf32: null pointer");
+  SIGMA_CHECK_ARG(batch >= 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0,
+                  "sigma_conv3x3_gelu_save_pitched_tf32: bad sizes batch=%d H=%d W=%d Cin=%d Cout=%d", batch, H, W, Cin, Cout);
+  SIGMA_CHECK_ARG(pitch_ok(x_pitch, Cin) && pitch_ok(w9_pitch, Cin) && pitch_ok(y_pitch, Cout),
+                  "sigma_conv3x3_gelu_save_pitched_tf32: pitches (x %d, w9 %d, y %d) must be multiples of 4 and at least Cin=%d / "
+                  "Cout=%d", x_pitch, w9_pitch, y_pitch, Cin, Cout);
+  SIGMA_CHECK_ARG(al16(x) && al16(w9) && al16(w9_lo) && al16(bias) && al16(y) && al16(pre),
+                  "sigma_conv3x3_gelu_save_pitched_tf32: pointers must be 16-byte aligned");
+  return conv3x3_pitched_launch(x, x_pitch, w9, w9_lo, w9_pitch, bias, 1, y, y_pitch, batch, H, W, Cin, Cout, (cudaStream_t)stream, 1,
+                                pre);
+}
+
+int sigma_conv3x3_dgrad_pitched_tf32(const float *dy, int dy_pitch, const float *w9t, int w9t_pitch, const float *w9t_lo,
+                                     const float *gelu_pre, float *dx, int dx_pitch, int batch, int H, int W, int Cin, int Cout,
+                                     void *stream) {
+  SIGMA_CHECK_ARG(dy && w9t && dx, "sigma_conv3x3_dgrad_pitched_tf32: null pointer");
+  SIGMA_CHECK_ARG(batch >= 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0,
+                  "sigma_conv3x3_dgrad_pitched_tf32: bad sizes batch=%d H=%d W=%d Cin=%d Cout=%d", batch, H, W, Cin, Cout);
+  SIGMA_CHECK_ARG(pitch_ok(dy_pitch, Cout) && pitch_ok(w9t_pitch, Cout) && pitch_ok(dx_pitch, Cin),
+                  "sigma_conv3x3_dgrad_pitched_tf32: pitches (dy %d, w9t %d, dx %d) must be multiples of 4 and at least Cout=%d / "
+                  "Cin=%d", dy_pitch, w9t_pitch, dx_pitch, Cout, Cin);
+  SIGMA_CHECK_ARG(al16(dy) && al16(w9t) && al16(w9t_lo) && al16(gelu_pre) && al16(dx),
+                  "sigma_conv3x3_dgrad_pitched_tf32: pointers must be 16-byte aligned");
+  // the conv of dy (Cout channels in) to dx (Cin channels out)
+  return conv3x3_pitched_launch(dy, dy_pitch, w9t, w9t_lo, w9t_pitch, nullptr, 0, dx, dx_pitch, batch, H, W, Cout, Cin,
+                                (cudaStream_t)stream, gelu_pre ? 2 : 0, (float *)gelu_pre);
+}
+
+int sigma_conv3x3_wgrad_pitched_tf32(const float *x, int x_pitch, int gelu_x, const float *dy, int dy_pitch, float *dw, float *dbias,
+                                     int batch, int H, int W, int Cin, int Cout, int x3, void *workspace, size_t workspace_bytes,
+                                     void *stream) {
+  SIGMA_CHECK_ARG(x && dy && dw, "sigma_conv3x3_wgrad_pitched_tf32: null pointer");
+  SIGMA_CHECK_ARG(batch > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0,
+                  "sigma_conv3x3_wgrad_pitched_tf32: bad sizes batch=%d H=%d W=%d Cin=%d Cout=%d", batch, H, W, Cin, Cout);
+  SIGMA_CHECK_ARG(pitch_ok(x_pitch, Cin) && pitch_ok(dy_pitch, Cout),
+                  "sigma_conv3x3_wgrad_pitched_tf32: pitches (x %d, dy %d) must be multiples of 4 and at least Cin=%d / Cout=%d",
+                  x_pitch, dy_pitch, Cin, Cout);
+  SIGMA_CHECK_ARG((gelu_x == 0 || gelu_x == 1) && (x3 == 0 || x3 == 1),
+                  "sigma_conv3x3_wgrad_pitched_tf32: gelu_x and x3 must be 0 or 1");
+  SIGMA_CHECK_ARG(al16(x) && al16(dy), "sigma_conv3x3_wgrad_pitched_tf32: x and dy must be 16-byte aligned");
+  const size_t need = conv3x3_wgrad_workspace_bytes(batch, H, W, Cin, Cout);
+  if (workspace == nullptr || !al16(workspace) || workspace_bytes < need) {
+    set_error("sigma_conv3x3_wgrad_pitched_tf32: needs %zu 16-byte aligned workspace bytes, got %zu", need,
+              workspace ? workspace_bytes : 0);
+    return SIGMA_EWORKSPACE;
+  }
+  return conv3x3_wgrad_launch(x, gelu_x, dy, dw, dbias, batch, H, W, Cin, Cout, x3, workspace, (cudaStream_t)stream, x_pitch, dy_pitch);
+}
+
 int sigma_split_tf32_fwd(const float *x, float *hi, float *lo, int64_t n, void *stream) {
   SIGMA_CHECK_ARG(x && hi && lo && n >= 0, "sigma_split_tf32_fwd: bad arguments");
   return split_tf32_launch(x, hi, lo, n, (cudaStream_t)stream);

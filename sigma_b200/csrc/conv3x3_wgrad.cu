@@ -45,6 +45,7 @@ struct WgradParams {
   float *part_w, *part_b;   // (nsplit, Cout·Cin·9) in nn.Conv2d's (Cout, Cin, 3, 3) order; (nsplit, Cout), or nullptr
   int H, W, Cin, Cout, tiles_w, tiles_hw, co_tiles, nsplit, gelu_x;
   long long npatch;
+  int x_ld, dy_ld;          // cab_wgrad_pitched_kernel: the row pitches of x and dy in elements (multiples of 4, >= Cin / Cout)
 };
 
 // D[16 x 8] += A[16 x 8] · B[8 x 8]: a = rows g, g + 8, g, g + 8 / columns t, t, t + 4, t + 4; b = rows t, t + 4 / column g;
@@ -58,131 +59,26 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
 __device__ __forceinline__ uint32_t tf32_hi(uint32_t v) { return v & 0xFFFFE000u; }
 __device__ __forceinline__ uint32_t tf32_lo(uint32_t v) { return __float_as_uint(__uint_as_float(v) - __uint_as_float(v & 0xFFFFE000u)); }
 
-template <int CO, bool X3>
-__global__ void __launch_bounds__(WG_THREADS, 1) conv3x3_wgrad_kernel(const __grid_constant__ WgradParams p) {
-  using T = WgradTile<CO>;
-  constexpr int NT = CO / 8;   // n8 fragments per warp
-  extern __shared__ __align__(16) float smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
-  const int tile = blockIdx.x, split = blockIdx.y;
-  const int ci0 = (tile / p.co_tiles) * WG_CI, co0 = (tile % p.co_tiles) * CO;
-  const long long pbeg = p.npatch * split / p.nsplit, pend = p.npatch * (split + 1) / p.nsplit;
-  const bool do_db = p.part_b != nullptr && ci0 == 0;
+#define SIGMA_WGRAD_KERNEL conv3x3_wgrad_kernel
+#define SIGMA_WGRAD_X_LD p.Cin
+#define SIGMA_WGRAD_DY_LD p.Cout
+#include "conv3x3_wgrad_kernel.inc"
+#undef SIGMA_WGRAD_KERNEL
+#undef SIGMA_WGRAD_X_LD
+#undef SIGMA_WGRAD_DY_LD
 
-  // stage patch `pt` into buffer `buf`: x box (10 x 18 pixels x 32 channels from ci0) and dy patch (128 pixels x CO from co0), as
-  // 16-byte cp.async chunks whose source-size 0 outside the image or the channel range writes zeros
-  auto issue = [&](long long pt, int buf) {
-    const int b = (int)(pt / p.tiles_hw), r = (int)(pt - (long long)b * p.tiles_hw);
-    const int y0 = (r / p.tiles_w) * WG_TH, x0 = (r % p.tiles_w) * WG_TW;
-    float *xs = smem + buf * T::buf_floats, *dys = xs + T::x_floats;
-    for (int i = tid; i < WG_XH * WG_XW * (WG_CI / 4); i += WG_THREADS) {
-      const int pix = i / (WG_CI / 4), c = ci0 + 4 * (i % (WG_CI / 4));
-      const int yy = y0 - 1 + pix / WG_XW, xx = x0 - 1 + pix % WG_XW;
-      const bool ok = yy >= 0 && yy < p.H && xx >= 0 && xx < p.W && c < p.Cin;
-      const float *src = ok ? p.x + (((long long)b * p.H + yy) * p.W + xx) * p.Cin + c : p.x;
-      cp_async16(xs + pix * WG_XLD + 4 * (i % (WG_CI / 4)), src, ok ? 16 : 0);
-    }
-    for (int i = tid; i < WG_PIX * (CO / 4); i += WG_THREADS) {
-      const int pix = i / (CO / 4), c = co0 + 4 * (i % (CO / 4));
-      const int yy = y0 + pix / WG_TW, xx = x0 + pix % WG_TW;
-      const bool ok = yy < p.H && xx < p.W && c < p.Cout;
-      const float *src = ok ? p.dy + (((long long)b * p.H + yy) * p.W + xx) * p.Cout + c : p.dy;
-      cp_async16(dys + pix * T::dy_ld + 4 * (i % (CO / 4)), src, ok ? 16 : 0);
-    }
-    cp_async_commit();
-  };
-
-  float acc[2][NT][4];
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int n = 0; n < NT; ++n)
-#pragma unroll
-      for (int i = 0; i < 4; ++i) acc[h][n][i] = 0.f;
-  float dbacc = 0.f;
-  const int tdy = warp / 3, tdx = warp % 3;
-
-  if (pbeg < pend) issue(pbeg, 0);
-  int buf = 0;
-  for (long long pt = pbeg; pt < pend; ++pt, buf ^= 1) {
-    if (pt + 1 < pend) { issue(pt + 1, buf ^ 1); cp_async_wait<1>(); }
-    else cp_async_wait<0>();
-    asm volatile("" ::: "memory");   // no shared-memory access moves above the wait
-    float *xs = smem + buf * T::buf_floats;
-    const float *dys = xs + T::x_floats;
-    if (p.gelu_x) {   // the chunks this thread copied, which its own wait made visible to it; GELU(0) = 0 keeps the padding
-      for (int i = tid; i < WG_XH * WG_XW * (WG_CI / 4); i += WG_THREADS) {
-        float4 *q = reinterpret_cast<float4 *>(xs + (i / (WG_CI / 4)) * WG_XLD + 4 * (i % (WG_CI / 4)));
-        float4 v = *q;
-        v.x = 0.5f * v.x * (1.f + erff(v.x * 0.70710678118654752f));
-        v.y = 0.5f * v.y * (1.f + erff(v.y * 0.70710678118654752f));
-        v.z = 0.5f * v.z * (1.f + erff(v.z * 0.70710678118654752f));
-        v.w = 0.5f * v.w * (1.f + erff(v.w * 0.70710678118654752f));
-        *q = v;
-      }
-    }
-    __syncthreads();
-
-    // k8 step kk covers pixels 8kk .. 8kk + 7: patch row kk / 2, columns 8·(kk % 2) ..; x box pixel of tap (tdy, tdx) = (row + tdy,
-    // column + tdx)
-    const uint32_t *xw = reinterpret_cast<const uint32_t *>(xs), *dw = reinterpret_cast<const uint32_t *>(dys);
-#pragma unroll 2
-    for (int kk = 0; kk < WG_PIX / 8; ++kk) {
-      const int xp = ((kk >> 1) + tdy) * WG_XW + 8 * (kk & 1) + tdx + t;
-      uint32_t a[2][4], bf[NT][2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        a[h][0] = xw[xp * WG_XLD + 16 * h + g];
-        a[h][1] = xw[xp * WG_XLD + 16 * h + g + 8];
-        a[h][2] = xw[(xp + 4) * WG_XLD + 16 * h + g];
-        a[h][3] = xw[(xp + 4) * WG_XLD + 16 * h + g + 8];
-      }
-#pragma unroll
-      for (int n = 0; n < NT; ++n) {
-        bf[n][0] = dw[(8 * kk + t) * T::dy_ld + 8 * n + g];
-        bf[n][1] = dw[(8 * kk + t + 4) * T::dy_ld + 8 * n + g];
-      }
-      if constexpr (X3) {
-        uint32_t ah[2][4], al[2][4];
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int i = 0; i < 4; ++i) { ah[h][i] = tf32_hi(a[h][i]); al[h][i] = tf32_lo(a[h][i]); }
-#pragma unroll
-        for (int n = 0; n < NT; ++n) {
-          const uint32_t bh[2] = {tf32_hi(bf[n][0]), tf32_hi(bf[n][1])}, bl[2] = {tf32_lo(bf[n][0]), tf32_lo(bf[n][1])};
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            mma_tf32(acc[h][n], al[h], bh);
-            mma_tf32(acc[h][n], ah[h], bl);
-            mma_tf32(acc[h][n], ah[h], bh);
-          }
-        }
-      } else {
-#pragma unroll
-        for (int n = 0; n < NT; ++n)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) mma_tf32(acc[h][n], a[h], bf[n]);
-      }
-    }
-    if (do_db && tid < CO)
-      for (int q = 0; q < WG_PIX; ++q) dbacc += dys[q * T::dy_ld + tid];
-    __syncthreads();   // every warp is done with this buffer before the next iteration's issue overwrites it
-  }
-
-  // the CTA's partial row: (co, ci, tap) at (co·Cin + ci)·9 + tap
-  float *pw = p.part_w + (long long)split * p.Cout * p.Cin * 9;
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int n = 0; n < NT; ++n)
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int ci = ci0 + 16 * h + g + 8 * (i >> 1), co = co0 + 8 * n + 2 * t + (i & 1);
-        if (ci < p.Cin && co < p.Cout) pw[((long long)co * p.Cin + ci) * 9 + warp] = acc[h][n][i];
-      }
-  if (do_db && tid < CO && co0 + tid < p.Cout) p.part_b[(long long)split * p.Cout + co0 + tid] = dbacc;
-}
+// The same on pitched rows (the CAB convs of Sigma-base): x and dy rows are p.x_ld / p.dy_ld elements apart, and Cin, Cout need not
+// be multiples of 4.  A chunk is staged when it starts below the count, and the pitch (a multiple of 4) keeps it inside the row, so a
+// chunk that straddles the count also stages pad elements.  Those are input channels ci >= Cin (A rows, reaching only dW[., ci])
+// and output channels co >= Cout (B columns, reaching only dW[co, .] and db[co]), none of which is stored: whatever the pads hold,
+// no kept output sees it.
+#define SIGMA_WGRAD_KERNEL cab_wgrad_pitched_kernel
+#define SIGMA_WGRAD_X_LD p.x_ld
+#define SIGMA_WGRAD_DY_LD p.dy_ld
+#include "conv3x3_wgrad_kernel.inc"
+#undef SIGMA_WGRAD_KERNEL
+#undef SIGMA_WGRAD_X_LD
+#undef SIGMA_WGRAD_DY_LD
 
 // output channels per tile: 64 when Cout is a multiple of 64 (Sigma's 64 / 128 / 192 / 384), else 32 (32, 96, ragged counts)
 static int wgrad_co(int Cout) { return Cout % 64 == 0 ? 64 : 32; }
@@ -204,7 +100,8 @@ size_t conv3x3_wgrad_workspace_bytes(int batch, int H, int W, int Cin, int Cout)
 }
 
 int conv3x3_wgrad_launch(const float *x, int gelu_x, const float *dy, float *dw, float *db, int batch, int H, int W, int Cin, int Cout,
-                         int x3, void *ws, cudaStream_t stream) {
+                         int x3, void *ws, cudaStream_t stream, int x_ld, int dy_ld) {
+  const bool pitched = x_ld > 0;
   long long pl[4];
   conv3x3_wgrad_plan(batch, H, W, Cin, Cout, pl);
   WgradParams p;
@@ -218,8 +115,14 @@ int conv3x3_wgrad_launch(const float *x, int gelu_x, const float *dy, float *dw,
   p.nsplit = (int)pl[2];
   p.gelu_x = gelu_x;
   p.npatch = (long long)batch * p.tiles_hw;
-  const void *kern = pl[0] == 64 ? (x3 ? (const void *)conv3x3_wgrad_kernel<64, true> : (const void *)conv3x3_wgrad_kernel<64, false>)
-                                 : (x3 ? (const void *)conv3x3_wgrad_kernel<32, true> : (const void *)conv3x3_wgrad_kernel<32, false>);
+  p.x_ld = pitched ? x_ld : Cin; p.dy_ld = pitched ? dy_ld : Cout;
+  const void *kern;
+  if (pitched)
+    kern = pl[0] == 64 ? (x3 ? (const void *)cab_wgrad_pitched_kernel<64, true> : (const void *)cab_wgrad_pitched_kernel<64, false>)
+                       : (x3 ? (const void *)cab_wgrad_pitched_kernel<32, true> : (const void *)cab_wgrad_pitched_kernel<32, false>);
+  else
+    kern = pl[0] == 64 ? (x3 ? (const void *)conv3x3_wgrad_kernel<64, true> : (const void *)conv3x3_wgrad_kernel<64, false>)
+                       : (x3 ? (const void *)conv3x3_wgrad_kernel<32, true> : (const void *)conv3x3_wgrad_kernel<32, false>);
   const size_t smem = pl[0] == 64 ? WgradTile<64>::smem : WgradTile<32>::smem;
   SIGMA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   void *args[] = {&p};

@@ -827,9 +827,12 @@ __device__ __forceinline__ float gelu_grad(float u) {
 // F16 (gemm_fp16_kernel): the BF16 instance on fp16 operands, C fp32 or (p.c_bf16) fp16.
 // EPI (conv3x3_epi_kernel, the CAB convs' training instances): 1 = also store pre = conv + bias to p.aux before the GELU;
 // 2 = multiply the result by GELU'(p.aux) (the data gradient of the second conv, emitted at the first conv's pre-activation).
-template <int BN, bool X3, bool CONV, bool BF16, bool FP8, bool TMA_C = false, bool F16 = false, int EPI = 0>
+// PITCHED (cab_conv_pitched_kernel): the conv's output rows (C and aux) are p.ldc elements apart instead of p.N, and N may be odd:
+// an odd N's last column is loaded and stored alone.  The input's pitch is in its tensor map.
+template <int BN, bool X3, bool CONV, bool BF16, bool FP8, bool TMA_C = false, bool F16 = false, int EPI = 0, bool PITCHED = false>
 __device__ __forceinline__ void gemm_body(const GemmParams &p) {
   static_assert(EPI == 0 || (CONV && !BF16 && !FP8 && !TMA_C && !F16), "the training epilogues are the fp32 conv's");
+  static_assert(!PITCHED || (CONV && !BF16 && !FP8 && !TMA_C && !F16), "the pitched instances are the fp32 conv's");
   static_assert(!BF16 || (!X3 && !CONV), "the bf16 instance is a plain GEMM");
   static_assert(!FP8 || (!X3 && !CONV && !BF16), "the e4m3 instance is a plain GEMM");
   static_assert(!F16 || (!X3 && !CONV && !BF16 && !FP8), "the fp16 instance is a plain GEMM");
@@ -1067,7 +1070,8 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
       if (CONV) {   // row r = pixel (r / 16, r % 16) of the 8 x 16 patch
         const int y = cy0 + r / CV_TW, x = cx0 + (r % CV_TW);
         if (y >= p.cH || x >= p.cW) continue;
-        coff = (((long long)cb * p.cH + y) * p.cW + x) * p.N;
+        if constexpr (PITCHED) coff = (((long long)cb * p.cH + y) * p.cW + x) * p.ldc;
+        else coff = (((long long)cb * p.cH + y) * p.cW + x) * p.N;
       } else {
         const int row = mt * GM_BM + r;
         if (row >= p.M) continue;
@@ -1083,6 +1087,17 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
         if constexpr (FP8) {
           const float2 sw = __ldg(reinterpret_cast<const float2 *>(p.sw + n));
           o.x = o.x * srow * sw.x; o.y = o.y * srow * sw.y;
+        }
+        if constexpr (PITCHED) {   // PITCHED: N may be odd, and column N - 1 of an odd N is the pair's only column
+          if (n + 1 == p.N) {
+            float v = o.x;
+            if (p.bias) v += __ldg(p.bias + n);
+            if constexpr (EPI == 1) p.aux[coff + n] = v;
+            if constexpr (EPI == 2) v *= gelu_grad(p.aux[coff + n]);
+            if (p.act == 1) v = 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
+            p.C[coff + n] = v;
+            continue;
+          }
         }
         if (p.bias) {
           const float2 b = __ldg(reinterpret_cast<const float2 *>(p.bias + n));
@@ -1128,6 +1143,15 @@ __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_tf32_kerne
 template <int BN, bool X3, int EPI>
 __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) conv3x3_epi_kernel(const __grid_constant__ GemmParams p) {
   gemm_body<BN, X3, true, false, false, false, false, EPI>(p);
+}
+
+// The pitched conv (the CAB convs of Sigma-base, whose C/3 is not a multiple of 4): x, y and the weights have row pitches that are
+// multiples of 4 elements while the channel counts need not be.  The tensor maps' widths are the logical counts, so TMA fills
+// channels past them with zeros whatever the pad bytes hold; the epilogue addresses rows at p.ldc and never stores a column
+// >= N.  EPI as conv3x3_epi_kernel's, and 0 = plain or (p.act) GELU.  Widths up to 256 for EPI 0, kEpiMaxBn for EPI 1 and 2.
+template <int BN, bool X3, int EPI>
+__global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) cab_conv_pitched_kernel(const __grid_constant__ GemmParams p) {
+  gemm_body<BN, X3, true, false, false, false, false, EPI, true>(p);
 }
 
 // The tf32x3 linear instance with the TMA-stored epilogue: fp32 C (and residual) whose rows a tensor map can describe.
@@ -1398,9 +1422,47 @@ int gemm_fp8_launch(const void *A, long long lda, const float *sa, const void *W
   return SIGMA_OK;
 }
 
-// The widest tile of conv3x3_epi_kernel: the CAB's C/3 (32 / 64 / 128 in Sigma-tiny and -small) fits one tile; wider outputs
-// take several.
+// The widest tile of conv3x3_epi_kernel and of cab_conv_pitched_kernel's EPI 1 / 2: the CAB's C/3 (32 / 64 / 128 in Sigma-tiny and
+// -small) fits one tile; wider outputs (Sigma-base's 170) take several.  The training epilogues keep two CTAs per SM, whose register
+// budget ends at 128-column tiles (plan_gemm).
 constexpr int kEpiMaxBn = 128;
+
+// The plan and parameters of a 3x3 conv (pad 1, stride 1, channels-last) whose x, W9 and y (and aux) rows are x_ld, w_ld and y_ld
+// elements apart: the tensor maps' widths are Cin, so channels past Cin arrive as zeros; the epilogue never stores a column >= Cout.
+static int conv3x3_setup(GemmParams &p, GemmPlan &pl, const float *x, long long x_ld, const float *W9, const float *W9_lo, long long w_ld,
+                         const float *bias, int act, float *y, long long y_ld, int B, int H, int W, int Cin, int Cout, float *aux,
+                         int max_bn) {
+  int rc;
+  if ((rc = plan_gemm(0, Cout, Cin, W9_lo != nullptr, B, H, W, &pl, false, false, max_bn))) return rc;
+  memset(&p, 0, sizeof(p));
+  p.bias = bias; p.C = y; p.aux = aux; p.ldc = y_ld;
+  p.N = Cout; p.K = Cin;
+  p.cH = H; p.cW = W; p.act = act;
+  p.tiles_w = (W + CV_TW - 1) / CV_TW;
+  p.tiles_hw = p.tiles_w * ((H + CV_TH - 1) / CV_TH);
+  p.M = B * p.tiles_hw;
+  p.kbc = (Cin + GM_BK - 1) / GM_BK;
+  p.BN = pl.BN;
+  p.stages = pl.stages;
+  {
+    uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
+    uint64_t str[3] = {(uint64_t)x_ld * 4, (uint64_t)W * x_ld * 4, (uint64_t)H * W * x_ld * 4};
+    uint32_t box[4] = {(uint32_t)GM_BK, (uint32_t)CV_TW, (uint32_t)CV_TH, 1};
+    if ((rc = make_tmap(&p.m_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                        CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
+  }
+  if ((rc = make_tmap_2d_sw128(&p.m_w, W9, 9LL * Cout, Cin, w_ld, p.BN))) return rc;
+  if (W9_lo && (rc = make_tmap_2d_sw128(&p.m_wlo, W9_lo, 9LL * Cout, Cin, w_ld, p.BN))) return rc;
+  return SIGMA_OK;
+}
+
+static int launch_conv(const void *kern, const GemmParams &p, const GemmPlan &pl, cudaStream_t stream) {
+  SIGMA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
+  void *args[] = {(void *)&p};
+  SIGMA_CHECK_CUDA(cudaLaunchKernel(kern, dim3(pl.grid), dim3(GM_THREADS), args, pl.smem, stream));
+  count_launch();
+  return SIGMA_OK;
+}
 
 // 3x3 convolution, pad 1, stride 1, channels-last: y (B,H,W,Cout) = conv(x (B,H,W,Cin), W9 (9, Cout, Cin)) + bias, optional GELU.
 // W9_lo == nullptr: plain TF32; else tf32x3 with W9 = W9_hi.  epi 1 (act 1): pre = conv + bias also stored to aux; epi 2 (act 0):
@@ -1410,29 +1472,11 @@ int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, con
   if (B == 0) return SIGMA_OK;
   const bool x3 = W9_lo != nullptr;
   GemmPlan pl;
-  int rc;
-  if ((rc = plan_gemm(0, Cout, Cin, x3, B, H, W, &pl, false, false, epi ? kEpiMaxBn : 256))) return rc;
   GemmParams p;
-  memset(&p, 0, sizeof(p));
-  p.bias = bias; p.C = y; p.aux = aux;
-  p.N = Cout; p.K = Cin;
-  p.cH = H; p.cW = W; p.act = act;
-  p.tiles_w = (W + CV_TW - 1) / CV_TW;
-  p.tiles_hw = p.tiles_w * ((H + CV_TH - 1) / CV_TH);
-  p.M = B * p.tiles_hw;
-  p.kbc = (Cin + GM_BK - 1) / GM_BK;
-  p.BN = pl.BN;
-  {
-    uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
-    uint64_t str[3] = {(uint64_t)Cin * 4, (uint64_t)W * Cin * 4, (uint64_t)H * W * Cin * 4};
-    uint32_t box[4] = {(uint32_t)GM_BK, (uint32_t)CV_TW, (uint32_t)CV_TH, 1};
-    if ((rc = make_tmap(&p.m_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B,
-                        CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
-  }
-  if ((rc = make_tmap_2d_sw128(&p.m_w, W9, 9LL * Cout, Cin, Cin, p.BN))) return rc;
-  if (x3 && (rc = make_tmap_2d_sw128(&p.m_wlo, W9_lo, 9LL * Cout, Cin, Cin, p.BN))) return rc;
+  int rc;
+  if ((rc = conv3x3_setup(p, pl, x, Cin, W9, W9_lo, Cin, bias, act, y, Cout, B, H, W, Cin, Cout, aux, epi ? kEpiMaxBn : 256)))
+    return rc;
   if (epi == 0) return x3 ? launch_gemm<true, true>(p, pl, stream) : launch_gemm<false, true>(p, pl, stream);
-  p.stages = pl.stages;
   const void *kern = nullptr;
   switch (p.BN) {
 #define SIGMA_EPI_BN(bn)                                                                                                         \
@@ -1444,11 +1488,45 @@ int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, con
 #undef SIGMA_EPI_BN
     default: set_error("conv3x3: the training epilogues have tiles of at most %d columns, not %d", kEpiMaxBn, p.BN); return SIGMA_EINVAL;
   }
-  SIGMA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
-  void *args[] = {&p};
-  SIGMA_CHECK_CUDA(cudaLaunchKernel(kern, dim3(pl.grid), dim3(GM_THREADS), args, pl.smem, stream));
-  count_launch();
-  return SIGMA_OK;
+  return launch_conv(kern, p, pl, stream);
+}
+
+// The same conv on pitched rows (cab_conv_pitched_kernel): x (B,H,W,x_ld) holds Cin channels, W9 (9·Cout, w_ld) Cin, y and aux
+// (B,H,W,y_ld) Cout; the pitches are multiples of 4 and at least the counts, which need not be.  The plan is conv3x3_tf32_launch's.
+int conv3x3_pitched_launch(const float *x, long long x_ld, const float *W9, const float *W9_lo, long long w_ld, const float *bias, int act,
+                           float *y, long long y_ld, int B, int H, int W, int Cin, int Cout, cudaStream_t stream, int epi, float *aux) {
+  if (B == 0) return SIGMA_OK;
+  const bool x3 = W9_lo != nullptr;
+  GemmPlan pl;
+  GemmParams p;
+  int rc;
+  if ((rc = conv3x3_setup(p, pl, x, x_ld, W9, W9_lo, w_ld, bias, act, y, y_ld, B, H, W, Cin, Cout, aux, epi ? kEpiMaxBn : 256)))
+    return rc;
+  const void *kern = nullptr;
+#define SIGMA_PITCHED_BN(bn, E)                                                                                                  \
+  case bn:                                                                                                                       \
+    kern = x3 ? (const void *)cab_conv_pitched_kernel<bn, true, E> : (const void *)cab_conv_pitched_kernel<bn, false, E>;        \
+    break;
+#define SIGMA_PITCHED_EPI(E) \
+    SIGMA_PITCHED_BN(32, E) SIGMA_PITCHED_BN(64, E) SIGMA_PITCHED_BN(96, E) SIGMA_PITCHED_BN(128, E)
+  if (epi == 0) {
+    switch (p.BN) {
+      SIGMA_PITCHED_EPI(0)
+      SIGMA_PITCHED_BN(160, 0) SIGMA_PITCHED_BN(192, 0) SIGMA_PITCHED_BN(224, 0) SIGMA_PITCHED_BN(256, 0)
+      default: break;
+    }
+  } else if (epi == 1) {
+    switch (p.BN) { SIGMA_PITCHED_EPI(1) default: break; }
+  } else {
+    switch (p.BN) { SIGMA_PITCHED_EPI(2) default: break; }
+  }
+#undef SIGMA_PITCHED_EPI
+#undef SIGMA_PITCHED_BN
+  if (kern == nullptr) {
+    set_error("conv3x3 (pitched): no instance of width %d for epilogue %d", p.BN, epi);
+    return SIGMA_EINVAL;
+  }
+  return launch_conv(kern, p, pl, stream);
 }
 
 }  // namespace sigma

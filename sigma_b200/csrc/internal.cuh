@@ -194,6 +194,9 @@ int gemm_fp8_launch(const void *A, long long lda, const float *sa, const void *W
 // epi 1 (with act 1): also store pre = conv + bias to aux; epi 2 (act 0): multiply the result by GELU'(aux) (aux in y's layout)
 int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, const float *bias, int act, float *y, int B, int H, int W,
                         int Cin, int Cout, cudaStream_t stream, int epi = 0, float *aux = nullptr);
+int conv3x3_pitched_launch(const float *x, long long x_ld, const float *W9, const float *W9_lo, long long w_ld, const float *bias, int act,
+                           float *y, long long y_ld, int B, int H, int W, int Cin, int Cout, cudaStream_t stream, int epi = 0,
+                           float *aux = nullptr);
 int split_tf32_launch(const float *x, float *hi, float *lo, long long n, cudaStream_t stream);
 int gemm_pick_bn_hook(int N, long long m_tiles);
 int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out);
@@ -202,8 +205,9 @@ int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, in
 // Launch plan of the weight gradient: {output channels per tile, output tiles, partial rows, CTAs}
 void conv3x3_wgrad_plan(int batch, int H, int W, int Cin, int Cout, long long *out4);
 size_t conv3x3_wgrad_workspace_bytes(int batch, int H, int W, int Cin, int Cout);
+// x_ld > 0: x and dy rows are x_ld / dy_ld elements apart (cab_wgrad_pitched_kernel); 0: Cin / Cout (conv3x3_wgrad_kernel)
 int conv3x3_wgrad_launch(const float *x, int gelu_x, const float *dy, float *dw, float *db, int batch, int H, int W, int Cin, int Cout,
-                         int x3, void *ws, cudaStream_t stream);
+                         int x3, void *ws, cudaStream_t stream, int x_ld = 0, int dy_ld = 0);
 
 // ---- evaluator.cu ----
 int argmax_hist_launch(const float *logits, const void *labels, int label_bytes, unsigned long long *hist,

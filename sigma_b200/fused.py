@@ -367,6 +367,50 @@ def conv3x3(x, conv, gelu=False):
     return y
 
 
+_W9P = {}   # id(conv.weight) -> (weakref, version, w9): the (9, Cout, Cin) re-ordering with rows padded to a multiple of 4
+
+
+def _conv3x3_form(conv):
+    return (conv.kernel_size == (3, 3) and conv.stride == (1, 1) and conv.padding == (1, 1) and conv.dilation == (1, 1)
+            and conv.groups == 1 and conv.padding_mode == "zeros")
+
+
+def cab_convs_pitched(x, cab):
+    """cab[2](GELU(cab[0](x))) of ChannelAttentionBlock on a channels-last fp32 x (B, H, W, C) when C1 = cab[0].out_channels is not a
+    multiple of 4 (Sigma-base's 42 / 85 / 170), which conv3x3 cannot take: conv 1 + bias + GELU into h (B, H, W, round4(C1)), whose
+    pad channels the second conv never reads (sigma_conv3x3_pitched_tf32), then conv 2 + bias from h at that pitch.  The second
+    conv's weight is cached re-ordered with its rows padded to round4(C1), on the weight's _version as _W9 is.  Precision as
+    conv3x3's.  Returns (B, H, W, C), or None when C is not a multiple of 4 or the convs are not of that form (cuDNN fallback)."""
+    import weakref
+    c1, c2 = cab[0], cab[2]
+    if not (USE_OWN_GEMM and _conv3x3_form(c1) and _conv3x3_form(c2)) or c1.in_channels % 4 or c2.out_channels % 4 \
+            or c1.out_channels != c2.in_channels:
+        return None
+    x = x.contiguous()
+    B, H, W, C = x.shape
+    C1, C2 = c1.out_channels, c2.out_channels
+    k1 = (C1 + 3) // 4 * 4
+    ws = []
+    for conv, cin in ((c1, C), (c2, C1)):
+        w, kp = conv.weight, (cin + 3) // 4 * 4
+        ent = _W9P.get(id(w))
+        if ent is None or ent[0]() is not w or ent[1] != w._version:
+            key = id(w)
+            w9 = F.pad(w.detach().permute(2, 3, 0, 1).reshape(9 * conv.out_channels, cin), (0, kp - cin)).contiguous()
+            ent = (weakref.ref(w, lambda _r, k=key: _W9P.pop(k, None)), w._version, w9)
+            _W9P[key] = ent
+        ws.append((ent[2], None) if torch.backends.cudnn.allow_tf32 else _split_weight(ent[2]))
+    L_ = _lib.lib()
+    h = torch.empty((B, H, W, k1), dtype=torch.float32, device=x.device)
+    (hi, lo), (hi2, lo2) = ws
+    _lib.check(L_.sigma_conv3x3_pitched_tf32(ptr(x), C, ptr(hi), C, ptr(lo), ptr(c1.bias), 1, ptr(h), k1, B, H, W, C, C1, stream()),
+               "sigma_conv3x3_pitched_tf32")
+    y = torch.empty((B, H, W, C2), dtype=torch.float32, device=x.device)
+    _lib.check(L_.sigma_conv3x3_pitched_tf32(ptr(h), k1, ptr(hi2), k1, ptr(lo2), ptr(c2.bias), 0, ptr(y), C2, B, H, W, C1, C2, stream()),
+               "sigma_conv3x3_pitched_tf32")
+    return y
+
+
 def dwconv3x3_silu(x, x_row_stride, x_batch_stride, conv, out, out_batch_stride, batch, H, W, D):
     """x and out both fp32, both bf16 (sigma_dwconv3x3_silu_fwd_bf16) or both fp16 (sigma_dwconv3x3_silu_fwd_fp16)."""
     fn = _entry("sigma_dwconv3x3_silu_fwd", x.dtype)
@@ -690,6 +734,8 @@ def cvss_decoder_block(blk, x):
     if isinstance(cab[1], torch.nn.GELU) and getattr(cab[1], "approximate", "none") == "none":
         h1 = conv3x3(xn2, cab[0], gelu=True)                         # conv3x3 + bias + GELU: implicit GEMM on the wgmma kernel
         t = conv3x3(h1, cab[2]) if h1 is not None else None
+        if h1 is None:                                               # C/3 not a multiple of 4 (Sigma-base): pitched rows
+            t = cab_convs_pitched(xn2, cab)
     with _no_autocast():                                             # CAB stays in the dense mode under autocast
         if t is None:                                                # other conv forms: cuDNN on a channels_last view
             t = cab[2](cab[1](cab[0](xn2.permute(0, 3, 1, 2)))).permute(0, 2, 3, 1).contiguous()

@@ -508,9 +508,11 @@ class CVSSDecoderBlock(nn.Module):
             return fused.cvss_decoder_block(self, input)
         x = input * self.scale1 + self.drop_path(self.op(ops.layer_norm(self.norm1, input)))
         cab = self.conv_blk.cab
-        if not _FORCE_COMPOSED and ops.cab_conv_ok(cab, x):
-            # channels-last throughout: the convs as one CabConvFn, then ChannelAttention.forward's arithmetic over (H, W)
-            t = ops.CabConvFn.apply(ops.layer_norm(self.norm2, x), cab[0].weight, cab[0].bias, cab[2].weight, cab[2].bias)
+        fn = None if _FORCE_COMPOSED else ops.cab_conv_fn(cab, x)
+        if fn is not None:
+            # channels-last throughout: the convs as one CabConvFn / CabConvPitchedFn, then ChannelAttention.forward's arithmetic
+            # over (H, W)
+            t = fn.apply(ops.layer_norm(self.norm2, x), cab[0].weight, cab[0].bias, cab[2].weight, cab[2].bias)
             ca = cab[3]
             avg, mx = t.mean(dim=(1, 2), keepdim=True), t.amax(dim=(1, 2), keepdim=True)
             attn = ca.sigmoid(ca.fc(avg.permute(0, 3, 1, 2)) + ca.fc(mx.permute(0, 3, 1, 2)))

@@ -532,23 +532,43 @@ class DwConvSiLUFn(torch.autograd.Function):
 
 
 # ---- the ChannelAttentionBlock's dense convs under autograd ----
-# On, CVSSDecoderBlock's training forward runs cab[0] -> GELU -> cab[2] as one CabConvFn on channels-last tensors (library kernels
-# forward and backward); off, it runs nn.Conv2d (cuDNN) on an NCHW copy.  Applies to fp32 without autocast (cab_conv_ok).
+# On, CVSSDecoderBlock's training forward runs cab[0] -> GELU -> cab[2] as one CabConvFn (or, where C/3 is not a multiple of 4,
+# CabConvPitchedFn) on channels-last tensors (library kernels forward and backward); off, it runs nn.Conv2d (cuDNN) on an NCHW copy.
+# Applies to fp32 without autocast (cab_conv_fn).
 FUSED_CAB_TRAINING = True
 
 
-def _conv3x3_ok(conv):
+def _conv3x3_ok(conv, pitched=False):
+    """a 3x3 / pad 1 / stride 1 conv with bias whose channel counts are multiples of 4 (pitched: any counts)"""
     return (isinstance(conv, torch.nn.Conv2d) and conv.kernel_size == (3, 3) and conv.stride == (1, 1) and conv.padding == (1, 1)
-            and conv.dilation == (1, 1) and conv.groups == 1 and conv.in_channels % 4 == 0 and conv.out_channels % 4 == 0
+            and conv.dilation == (1, 1) and conv.groups == 1 and (pitched or (conv.in_channels % 4 == 0 and conv.out_channels % 4 == 0))
             and conv.bias is not None and conv.padding_mode == "zeros")
+
+
+def _cab_ok(cab, x, pitched):
+    return (FUSED_TRAINING and FUSED_CAB_TRAINING and torch.is_grad_enabled() and x.is_cuda and x.dtype == torch.float32
+            and not torch.is_autocast_enabled("cuda") and isinstance(cab[1], torch.nn.GELU) and cab[1].approximate == "none"
+            and _conv3x3_ok(cab[0], pitched) and _conv3x3_ok(cab[2], pitched) and cab[0].out_channels == cab[2].in_channels)
 
 
 def cab_conv_ok(cab, x):
     """CabConvFn takes `cab` (the nn.Sequential of ChannelAttentionBlock) on x: autograd recording, both switches on, fp32 CUDA x with
     autocast off, an exact nn.GELU between two 3x3 / pad 1 / stride 1 convs whose channel counts are multiples of 4"""
-    return (FUSED_TRAINING and FUSED_CAB_TRAINING and torch.is_grad_enabled() and x.is_cuda and x.dtype == torch.float32
-            and not torch.is_autocast_enabled("cuda") and isinstance(cab[1], torch.nn.GELU) and cab[1].approximate == "none"
-            and _conv3x3_ok(cab[0]) and _conv3x3_ok(cab[2]) and cab[0].out_channels == cab[2].in_channels)
+    return _cab_ok(cab, x, False)
+
+
+def cab_conv_fn(cab, x):
+    """the autograd node that runs `cab` on x in training: CabConvFn where cab_conv_ok; CabConvPitchedFn where only C/3 (cab[0]'s
+    output channels) is not a multiple of 4 (Sigma-base's 42 / 85 / 170, hidden 32's 10); None: the cuDNN route"""
+    if cab_conv_ok(cab, x):
+        return CabConvFn
+    if _cab_ok(cab, x, True) and cab[0].in_channels % 4 == 0 and cab[2].out_channels % 4 == 0:
+        return CabConvPitchedFn
+    return None
+
+
+def _round4(n):
+    return (n + 3) // 4 * 4
 
 
 def _tf32_split(w):
@@ -558,12 +578,80 @@ def _tf32_split(w):
     return hi, lo
 
 
-def _w9(w, x3, grad=False):
+def _w9(w, x3, grad=False, pitch=None):
     """the nn.Conv2d weight (Cout, Cin, 3, 3) as the conv kernel's (9, Cout, Cin) or, grad, the data gradient's flipped and transposed
-    (9, Cin, Cout), with its tf32x3 split when x3 (else lo = None)"""
+    (9, Cin, Cout), with its tf32x3 split when x3 (else lo = None); pitch: rows zero-padded to that many elements"""
     w = w.detach()
-    w9 = (w.flip(2, 3).permute(2, 3, 1, 0) if grad else w.permute(2, 3, 0, 1)).reshape(-1, w.shape[0] if grad else w.shape[1]).contiguous()
+    w9 = (w.flip(2, 3).permute(2, 3, 1, 0) if grad else w.permute(2, 3, 0, 1)).reshape(-1, w.shape[0] if grad else w.shape[1])
+    if pitch is not None and pitch > w9.shape[1]:
+        w9 = F.pad(w9, (0, pitch - w9.shape[1]))
+    w9 = w9.contiguous()
     return _tf32_split(w9) if x3 else (w9, None)
+
+
+def _cab_forward(x, w1, b1, w2, b2, x3, pitched):
+    """(y, pre) of the CAB node's forward.  pitched: h and pre are (B, H, W, round4(C1)) and the pitched entry points run"""
+    B, H, W, C = x.shape
+    C1, C2 = w1.shape[0], w2.shape[0]
+    k1 = _round4(C1) if pitched else C1
+    L_ = _lib.lib()
+    pre = torch.empty((B, H, W, k1), dtype=torch.float32, device=x.device)
+    h = torch.empty_like(pre)
+    y = torch.empty((B, H, W, C2), dtype=torch.float32, device=x.device)
+    hi, lo = _w9(w1, x3)
+    if pitched:
+        _lib.check(L_.sigma_conv3x3_gelu_save_pitched_tf32(ptr(x), C, ptr(hi), C, ptr(lo), ptr(b1), ptr(h), ptr(pre), k1, B, H, W, C, C1,
+                                                           stream()), "sigma_conv3x3_gelu_save_pitched_tf32")
+        hi, lo = _w9(w2, x3, pitch=k1)
+        _lib.check(L_.sigma_conv3x3_pitched_tf32(ptr(h), k1, ptr(hi), k1, ptr(lo), ptr(b2), 0, ptr(y), C2, B, H, W, C1, C2, stream()),
+                   "sigma_conv3x3_pitched_tf32")
+    else:
+        _lib.check(L_.sigma_conv3x3_gelu_save_tf32(ptr(x), ptr(hi), ptr(lo), ptr(b1), ptr(h), ptr(pre), B, H, W, C, C1, stream()),
+                   "sigma_conv3x3_gelu_save_tf32")
+        hi, lo = _w9(w2, x3)
+        _lib.check(L_.sigma_conv3x3_tf32(ptr(h), ptr(hi), ptr(lo), ptr(b2), 0, ptr(y), B, H, W, C1, C2, stream()), "sigma_conv3x3_tf32")
+    return y, pre
+
+
+def _cab_backward(x, pre, w1, w2, dy, x3, pitched):
+    """(dx, dw1, db1, dw2, db2) of the CAB node from the saved x and pre-activation.  Every activation's row pitch is its last
+    dimension (pitched: pre and dpre at round4(C1))."""
+    B, H, W, C = x.shape
+    C1, C2 = w1.shape[0], w2.shape[0]
+    L_ = _lib.lib()
+
+    def wgrad(xin, gelu_x, g, cin, cout):
+        dw = torch.empty((cout, cin, 3, 3), dtype=torch.float32, device=x.device)
+        db = torch.empty(cout, dtype=torch.float32, device=x.device)
+        wsb = L_.sigma_conv3x3_wgrad_workspace_bytes(B, H, W, cin, cout)
+        ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+        if pitched:
+            _lib.check(L_.sigma_conv3x3_wgrad_pitched_tf32(ptr(xin), xin.shape[-1], gelu_x, ptr(g), g.shape[-1], ptr(dw), ptr(db), B, H,
+                                                           W, cin, cout, int(x3), ptr(ws), wsb, stream()),
+                       "sigma_conv3x3_wgrad_pitched_tf32")
+        else:
+            _lib.check(L_.sigma_conv3x3_wgrad_tf32(ptr(xin), gelu_x, ptr(g), ptr(dw), ptr(db), B, H, W, cin, cout, int(x3), ptr(ws), wsb,
+                                                   stream()), "sigma_conv3x3_wgrad_tf32")
+        return dw, db
+
+    def dgrad(g, w, gelu_pre, cin, cout):
+        ld = _round4(cin) if pitched else cin
+        dx = torch.empty((B, H, W, ld), dtype=torch.float32, device=x.device)
+        if pitched:
+            hi, lo = _w9(w, x3, grad=True, pitch=g.shape[-1])
+            _lib.check(L_.sigma_conv3x3_dgrad_pitched_tf32(ptr(g), g.shape[-1], ptr(hi), g.shape[-1], ptr(lo), ptr(gelu_pre), ptr(dx), ld,
+                                                           B, H, W, cin, cout, stream()), "sigma_conv3x3_dgrad_pitched_tf32")
+        else:
+            hi, lo = _w9(w, x3, grad=True)
+            _lib.check(L_.sigma_conv3x3_dgrad_tf32(ptr(g), ptr(hi), ptr(lo), ptr(gelu_pre), ptr(dx), B, H, W, cin, cout, stream()),
+                       "sigma_conv3x3_dgrad_tf32")
+        return dx
+
+    dw2, db2 = wgrad(pre, 1, dy, C1, C2)
+    dpre = dgrad(dy, w2, pre, C1, C2)          # the gradient at conv 1's pre-activation
+    dw1, db1 = wgrad(x, 0, dpre, C, C1)
+    dx = dgrad(dpre, w1, None, C, C1)
+    return dx, dw1, db1, dw2, db2
 
 
 class CabConvFn(torch.autograd.Function):
@@ -579,52 +667,36 @@ class CabConvFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w1, b1, w2, b2):
         x = x.contiguous()
-        B, H, W, C = x.shape
-        C1 = w1.shape[0]
-        x3 = not torch.backends.cudnn.allow_tf32
-        L_ = _lib.lib()
-        pre = torch.empty((B, H, W, C1), dtype=torch.float32, device=x.device)
-        h = torch.empty_like(pre)
-        hi, lo = _w9(w1, x3)
-        _lib.check(L_.sigma_conv3x3_gelu_save_tf32(ptr(x), ptr(hi), ptr(lo), ptr(b1), ptr(h), ptr(pre), B, H, W, C, C1, stream()),
-                   "sigma_conv3x3_gelu_save_tf32")
-        y = torch.empty((B, H, W, w2.shape[0]), dtype=torch.float32, device=x.device)
-        hi, lo = _w9(w2, x3)
-        _lib.check(L_.sigma_conv3x3_tf32(ptr(h), ptr(hi), ptr(lo), ptr(b2), 0, ptr(y), B, H, W, C1, w2.shape[0], stream()),
-                   "sigma_conv3x3_tf32")
+        ctx.x3 = not torch.backends.cudnn.allow_tf32
+        y, pre = _cab_forward(x, w1, b1, w2, b2, ctx.x3, False)
         ctx.save_for_backward(x, pre, w1, w2)
-        ctx.x3 = x3
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, pre, w1, w2 = ctx.saved_tensors
-        dy = dy.contiguous()
-        B, H, W, C = x.shape
-        C1, C2 = w1.shape[0], w2.shape[0]
-        L_ = _lib.lib()
+        return _cab_backward(x, pre, w1, w2, dy.contiguous(), ctx.x3, False)
 
-        def wgrad(xin, gelu_x, g, cin, cout):
-            dw = torch.empty((cout, cin, 3, 3), dtype=torch.float32, device=x.device)
-            db = torch.empty(cout, dtype=torch.float32, device=x.device)
-            wsb = L_.sigma_conv3x3_wgrad_workspace_bytes(B, H, W, cin, cout)
-            ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
-            _lib.check(L_.sigma_conv3x3_wgrad_tf32(ptr(xin), gelu_x, ptr(g), ptr(dw), ptr(db), B, H, W, cin, cout, int(ctx.x3), ptr(ws),
-                                                   wsb, stream()), "sigma_conv3x3_wgrad_tf32")
-            return dw, db
 
-        def dgrad(g, w, gelu_pre, cin, cout):
-            dx = torch.empty((B, H, W, cin), dtype=torch.float32, device=x.device)
-            hi, lo = _w9(w, ctx.x3, grad=True)
-            _lib.check(L_.sigma_conv3x3_dgrad_tf32(ptr(g), ptr(hi), ptr(lo), ptr(gelu_pre), ptr(dx), B, H, W, cin, cout, stream()),
-                       "sigma_conv3x3_dgrad_tf32")
-            return dx
+class CabConvPitchedFn(torch.autograd.Function):
+    """CabConvFn for C1 = cab[0].out_channels that is not a multiple of 4 (C still is): the same calls, order, precision rule and
+    determinism on the pitched entry points (sigma_conv3x3_*_pitched_tf32).  The GELU output and the saved pre-activation are
+    (B, H, W, round4(C1)), as is the gradient at the pre-activation; their pad channels are never written and never reach an output.
+    The weights that are read along C1 (conv 2's, and conv 1's transposed for its data gradient) are re-ordered per call with their
+    rows zero-padded to round4(C1)."""
 
-        dw2, db2 = wgrad(pre, 1, dy, C1, C2)
-        dpre = dgrad(dy, w2, pre, C1, C2)          # the gradient at conv 1's pre-activation
-        dw1, db1 = wgrad(x, 0, dpre, C, C1)
-        dx = dgrad(dpre, w1, None, C, C1)
-        return dx, dw1, db1, dw2, db2
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2):
+        x = x.contiguous()
+        ctx.x3 = not torch.backends.cudnn.allow_tf32
+        y, pre = _cab_forward(x, w1, b1, w2, b2, ctx.x3, True)
+        ctx.save_for_backward(x, pre, w1, w2)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, pre, w1, w2 = ctx.saved_tensors
+        return _cab_backward(x, pre, w1, w2, dy.contiguous(), ctx.x3, True)
 
 
 _SAVED_BF16 = 2               # `saved` of _call_ss2d_bwd: the arguments are those of sigma_ss2d_scan_bwd_saved_bf16
