@@ -412,7 +412,8 @@ static int linear_16bit(const char *fn, int dtype, const void *A, int64_t lda, c
                   "%s: K and lda must be multiples of 8 (16-byte %s TMA rows); N, ldc, ldr multiples of 4", fn, f16 ? "fp16" : "bf16");
   SIGMA_CHECK_ARG(al16(A) && al16(W) && al16(C) && al16(bias) && al16(residual) && al16(rscale), "%s: pointers must be 16-byte aligned", fn);
   SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "%s: rscale without residual", fn);
-  return gemm_16bit_launch(dtype, A, lda, W, bias, residual, ldr, rscale, C, ldc, c_dtype == dtype, M, N, K, (cudaStream_t)stream);
+  return gemm_launch(f16 ? GemmOp::F16 : GemmOp::BF16, A, lda, W, nullptr, nullptr, nullptr, bias, residual, ldr, rscale, C, ldc,
+                     c_dtype == dtype, M, N, K, (cudaStream_t)stream);
 }
 
 int sigma_layernorm_fwd(const float *x, const float *w, const float *b, float *y, int64_t rows, int C, float eps,
@@ -988,7 +989,8 @@ int sigma_linear_tf32(const float *A, int64_t lda, const float *W, const float *
   SIGMA_CHECK_ARG(al16(A) && al16(W) && al16(C) && al16(bias) && al16(residual) && al16(rscale),
                   "sigma_linear_tf32: pointers must be 16-byte aligned");
   SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "sigma_linear_tf32: rscale without residual");
-  return gemm_tf32_launch(A, lda, W, nullptr, bias, residual, ldr, rscale, C, ldc, M, N, K, (cudaStream_t)stream);
+  return gemm_launch(GemmOp::TF32, A, lda, W, nullptr, nullptr, nullptr, bias, residual, ldr, rscale, C, ldc, 0, M, N, K,
+                     (cudaStream_t)stream);
 }
 
 int sigma_linear_bf16(const void *A, int64_t lda, const void *W, const float *bias, const float *residual, int64_t ldr,
@@ -1011,7 +1013,8 @@ int sigma_linear_fp8(const void *A, int64_t lda, const float *sa, const void *Wq
   SIGMA_CHECK_ARG(al16(A) && al16(Wq) && al16(C) && al16(bias) && al16(residual) && al16(rscale) && al8(sw),
                   "sigma_linear_fp8: A, Wq, C, bias, residual, rscale must be 16-byte and sw 8-byte aligned");
   SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "sigma_linear_fp8: rscale without residual");
-  return gemm_fp8_launch(A, lda, sa, Wq, sw, bias, residual, ldr, rscale, C, ldc, c_dtype == SIGMA_BF16, M, N, K, (cudaStream_t)stream);
+  return gemm_launch(GemmOp::E4M3, A, lda, Wq, nullptr, sa, sw, bias, residual, ldr, rscale, C, ldc, c_dtype == SIGMA_BF16, M, N, K,
+                     (cudaStream_t)stream);
 }
 
 int sigma_quantize_e4m3_rows(const void *x, int x_dtype, int64_t ldx, void *q, int64_t ldq, float *scale, int64_t rows, int C, void *stream) {
@@ -1033,7 +1036,8 @@ static int linear_tf32x3(const float *A, int64_t lda, const float *W_hi, const f
   SIGMA_CHECK_ARG(al16(A) && al16(W_hi) && al16(W_lo) && al16(C) && al16(bias) && al16(residual) && al16(rscale),
                   "sigma_linear_tf32x3: pointers must be 16-byte aligned");
   SIGMA_CHECK_ARG(rscale == nullptr || residual != nullptr, "sigma_linear_tf32x3: rscale without residual");
-  return gemm_tf32_launch(A, lda, W_hi, W_lo, bias, residual, ldr, rscale, C, ldc, M, N, K, (cudaStream_t)stream, reg_epilogue);
+  return gemm_launch(GemmOp::TF32X3, A, lda, W_hi, W_lo, nullptr, nullptr, bias, residual, ldr, rscale, C, ldc, 0, M, N, K,
+                     (cudaStream_t)stream, reg_epilogue);
 }
 
 int sigma_linear_tf32x3(const float *A, int64_t lda, const float *W_hi, const float *W_lo, const float *bias, const float *residual,

@@ -10,12 +10,12 @@
 // 128 x BN output tiles (BN a multiple of 32 up to 256, one template instance per width, chosen per call); the producer
 // runs ahead across tile boundaries, so the loads of the next tile overlap the epilogue of the current one.  The epilogue
 // adds bias / residual·rscale to the register accumulators and stores them directly (each warp store covers 8 rows x 32 B);
-// the tf32x3 linear instance (gemm_x3_tma_kernel) stages them in shared memory and stores them with TMA instead (TMA_C).
+// the tf32x3 linear instance (gemm_x3_tma_kernel) stages them in shared memory and stores them with TMA instead (GemmEpi::TMA).
 // These GEMMs are HBM-bound at the Sigma shapes (K = 96..1536): what matters is one pass over A and one over C.
 //
-// X3 = true ("tf32x3", sigma_linear_tf32x3): fp32-grade products on the TF32 tensor pipe by error compensation,
+// GemmOp::TF32X3 (sigma_linear_tf32x3): fp32-grade products on the TF32 tensor pipe by error compensation,
 //     A·W = A_hi·W_hi + A_lo·W_hi + A_hi·W_lo  (+ A_lo·W_lo ~ 2^-22, dropped),   x_hi = x with the low 13 mantissa bits cleared.
-// CONV = true (sigma_conv3x3_tf32): the SAME kernel as an implicit-GEMM 3x3 convolution (pad 1, stride 1) over a channels-last
+// GemmSrc::CONV (sigma_conv3x3_tf32): the SAME kernel as an implicit-GEMM 3x3 convolution (pad 1, stride 1) over a channels-last
 // (B, H, W, Cin) tensor: an M tile is an 8 x 16 pixel patch, the K loop runs over 9 taps x Cin blocks, and the A tile of tap
 // (dy, dx) is ONE 4-D TMA box of the input shifted by (dy-1, dx-1) whose out-of-bounds fill is the zero padding (no im2col
 // tensor); weights are (9, Cout, Cin); bias and an optional exact GELU are fused in the epilogue.  Replaces the
@@ -28,6 +28,7 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "tma.cuh"
@@ -39,17 +40,59 @@ constexpr int GM_BK = 32;        // fp32 elements per k-block = one 128-byte swi
 constexpr int GM_UK = 8;         // wgmma K for tf32 (32 bytes)
 constexpr int GM_THREADS = 288;  // two consumer warpgroups + one producer warp
 
+// The FP8 instance's widest tile.  acc and the k-block fragment take BN registers per thread, so only BN <= 64 fits two CTAs
+// per SM (96 registers at 64; 96 and 128 wide tiles take 114 / 146 and run one CTA per SM, 160 spills).  On an H100 the
+// 64-wide tiles at two CTAs per SM ran Sigma-tiny's quantized GEMMs 1.1-2.1x faster than 128-wide ones at one, whose
+// epilogue stores nothing overlaps (DESIGN §5.4), so the instance has the widths 32 and 64 only.
+constexpr int kFp8MaxBn = 64;
+// The widest tile of the conv's training epilogues (conv3x3_epi_kernel, cab_conv_pitched_kernel's EPI 1 / 2): the CAB's C/3
+// (32 / 64 / 128 in Sigma-tiny and -small) fits one tile; wider outputs (Sigma-base's 170) take several.  The training
+// epilogues keep two CTAs per SM, whose register budget ends at 128-column tiles (plan_gemm).
+constexpr int kEpiMaxBn = 128;
+
+// What the body and the host take from the operand kind; the wgmma form is wgmma_ss<OP, BN> (tf32x3: wgmma_tf32_rs) and the
+// 16-bit type of C is GemmC16<OP>
+struct GemmOpTraits {
+  int bytes;                 // per operand element: a k-block is one 128-byte swizzle row, GM_BK·4 / bytes elements
+  int max_bn;                // the widest tile instance
+  CUtensorMapDataType tma;   // the operand tensor maps' element type
+};
+__host__ __device__ constexpr GemmOpTraits gemm_op_traits(GemmOp op) {
+  return op == GemmOp::E4M3   ? GemmOpTraits{1, kFp8MaxBn, CU_TENSOR_MAP_DATA_TYPE_UINT8}
+         : op == GemmOp::BF16 ? GemmOpTraits{2, 256, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16}
+         : op == GemmOp::F16  ? GemmOpTraits{2, 256, CU_TENSOR_MAP_DATA_TYPE_FLOAT16}
+                              : GemmOpTraits{4, 256, CU_TENSOR_MAP_DATA_TYPE_FLOAT32};
+}
+// The type C is stored in when p.c_bf16 is set; float: the fp32 kinds store fp32 C only
+template <GemmOp OP>
+using GemmC16 = std::conditional_t<OP == GemmOp::F16, __half,
+                                   std::conditional_t<OP == GemmOp::BF16 || OP == GemmOp::E4M3, __nv_bfloat16, float>>;
+
+// Where the A tiles come from: rows of a matrix, or the taps of a 3x3 conv over a channels-last tensor whose rows are Cin
+// (CONV) or a pitch (PITCHED) elements apart
+enum class GemmSrc { ROWS, CONV, PITCHED };
+// What the epilogue does with the accumulators: store C from registers (REGS; the conv's plain or GELU output), or through
+// shared memory with TMA (TMA); the conv's training epilogues also store pre = conv + bias to p.aux (PRE), or multiply the
+// result by GELU'(p.aux) (DGELU)
+enum class GemmEpi { REGS, TMA, PRE, DGELU };
+// The instances there are: every kind on rows with C stored from registers, tf32x3 on rows with the TMA-stored epilogue, and
+// the fp32 kinds' convs with the conv epilogues
+constexpr bool gemm_instance_ok(GemmOp op, GemmSrc src, GemmEpi epi) {
+  return src == GemmSrc::ROWS ? epi == GemmEpi::REGS || (epi == GemmEpi::TMA && op == GemmOp::TF32X3)
+                              : (op == GemmOp::TF32 || op == GemmOp::TF32X3) && epi != GemmEpi::TMA;
+}
+
 struct alignas(64) GemmParams {
   CUtensorMap m_a, m_w, m_wlo;
   const float *bias, *residual, *rscale;
   float *C;
   long long ldr, ldc;
   int M, N, K, BN, stages;   // BN: host-side choice of the template instance
-  int c_bf16;       // BF16, FP8: 1 = C is stored as bf16; F16: as fp16 (bias / residual / rscale stay fp32)
+  int c_bf16;       // 1 = C is stored as GemmC16 (bf16 or fp16; bias / residual / rscale stay fp32)
   int cH, cW, tiles_w, tiles_hw, kbc, act;   // CONV: image size, 8x16 patches per row / per image, Cin blocks per tap, activation
-  const float *sa, *sw;   // FP8: per-row scales of A, per-output-channel scales of W
-  CUtensorMap m_c, m_r;   // TMA_C: C and (if any) the residual, GM_CHUNK x 64 boxes
-  float *aux;             // conv3x3_epi_kernel: EPI 1 stores the pre-activation here, EPI 2 reads GELU's input from it (C's layout)
+  const float *sa, *sw;   // E4M3: per-row scales of A, per-output-channel scales of W
+  CUtensorMap m_c, m_r;   // GemmEpi::TMA: C and (if any) the residual, GM_CHUNK x 64 boxes
+  float *aux;             // GemmEpi::PRE stores the pre-activation here, DGELU reads GELU's input from it (C's layout)
 };
 
 // One ring stage holds a k-block's K-major, 128-byte-swizzled operand tiles, each 1024-aligned: [A | W].  tf32x3 adds W_lo:
@@ -96,708 +139,93 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t addr) {
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
 }
 
-// D[64 x N] (+)= A[64 x 8] · B[N x 8]^T, both operands K-major in shared memory; scale_d = 0 overwrites D
-template <int N>
-__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
-template <> __device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "%16, %17, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "%32, %33, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32<96>(float (&d)[48], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
-      "%48, %49, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32<160>(float (&d)[80], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %82, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n160k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
-      "%80, %81, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32<192>(float (&d)[96], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %98, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n192k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
-      "%96, %97, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32<224>(float (&d)[112], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %114, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n224k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111}, "
-      "%112, %113, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32<256>(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-      "%128, %129, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
+// The wgmma forms, one explicit specialisation per tile width N = 32 .. 256: D[64 x N] (+)= A[64 x k] · B[N x k]^T into N / 2
+// fp32 accumulators per thread.  WG_ACC_<N> / WG_CON_<N> are the accumulators' asm placeholders and "+f" constraints, built
+// from chunks of 8; WG_WIDTHS lists each width with the numbers of the six operands that can follow them (nvcc takes no named
+// asm operands, so these are spelled out).  The host's kernel selection iterates the same table.
+#define WG_P0 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define WG_P1 "%8, %9, %10, %11, %12, %13, %14, %15"
+#define WG_P2 "%16, %17, %18, %19, %20, %21, %22, %23"
+#define WG_P3 "%24, %25, %26, %27, %28, %29, %30, %31"
+#define WG_P4 "%32, %33, %34, %35, %36, %37, %38, %39"
+#define WG_P5 "%40, %41, %42, %43, %44, %45, %46, %47"
+#define WG_P6 "%48, %49, %50, %51, %52, %53, %54, %55"
+#define WG_P7 "%56, %57, %58, %59, %60, %61, %62, %63"
+#define WG_P8 "%64, %65, %66, %67, %68, %69, %70, %71"
+#define WG_P9 "%72, %73, %74, %75, %76, %77, %78, %79"
+#define WG_P10 "%80, %81, %82, %83, %84, %85, %86, %87"
+#define WG_P11 "%88, %89, %90, %91, %92, %93, %94, %95"
+#define WG_P12 "%96, %97, %98, %99, %100, %101, %102, %103"
+#define WG_P13 "%104, %105, %106, %107, %108, %109, %110, %111"
+#define WG_P14 "%112, %113, %114, %115, %116, %117, %118, %119"
+#define WG_P15 "%120, %121, %122, %123, %124, %125, %126, %127"
+#define WG_ACC_32 WG_P0 ", " WG_P1
+#define WG_ACC_64 WG_ACC_32 ", " WG_P2 ", " WG_P3
+#define WG_ACC_96 WG_ACC_64 ", " WG_P4 ", " WG_P5
+#define WG_ACC_128 WG_ACC_96 ", " WG_P6 ", " WG_P7
+#define WG_ACC_160 WG_ACC_128 ", " WG_P8 ", " WG_P9
+#define WG_ACC_192 WG_ACC_160 ", " WG_P10 ", " WG_P11
+#define WG_ACC_224 WG_ACC_192 ", " WG_P12 ", " WG_P13
+#define WG_ACC_256 WG_ACC_224 ", " WG_P14 ", " WG_P15
+#define WG_D(c)                                                                                                                  \
+  "+f"(d[8 * c]), "+f"(d[8 * c + 1]), "+f"(d[8 * c + 2]), "+f"(d[8 * c + 3]), "+f"(d[8 * c + 4]), "+f"(d[8 * c + 5]),            \
+      "+f"(d[8 * c + 6]), "+f"(d[8 * c + 7])
+#define WG_CON_32 WG_D(0), WG_D(1)
+#define WG_CON_64 WG_CON_32, WG_D(2), WG_D(3)
+#define WG_CON_96 WG_CON_64, WG_D(4), WG_D(5)
+#define WG_CON_128 WG_CON_96, WG_D(6), WG_D(7)
+#define WG_CON_160 WG_CON_128, WG_D(8), WG_D(9)
+#define WG_CON_192 WG_CON_160, WG_D(10), WG_D(11)
+#define WG_CON_224 WG_CON_192, WG_D(12), WG_D(13)
+#define WG_CON_256 WG_CON_224, WG_D(14), WG_D(15)
+// X(N, o0, .. o5): %o0 .. %o5 are the operands after the N / 2 accumulators
+#define WG_WIDTHS(X)                 \
+  X(32, 16, 17, 18, 19, 20, 21)      \
+  X(64, 32, 33, 34, 35, 36, 37)      \
+  X(96, 48, 49, 50, 51, 52, 53)      \
+  X(128, 64, 65, 66, 67, 68, 69)     \
+  X(160, 80, 81, 82, 83, 84, 85)     \
+  X(192, 96, 97, 98, 99, 100, 101)   \
+  X(224, 112, 113, 114, 115, 116, 117) \
+  X(256, 128, 129, 130, 131, 132, 133)
+
+// Both operands K-major in shared memory (descriptors da, db), every operand kind but tf32x3; scale_d = 0 overwrites D.  Each
+// kind's k step (k8 tf32, k16 bf16 / fp16, k32 e4m3) is 32 bytes, so the swizzled stage layout and the +32 B descriptor advance
+// are shared.  The 16-bit forms take the transpose flags (0: K-major); tf32 and e4m3 are K-major only.
+template <GemmOp OP, int N>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+#define WG_SS(OP, SHAPE, TAIL, N, a, b, s)                                                                                       \
+  template <>                                                                                                                    \
+  __device__ __forceinline__ void wgmma_ss<GemmOp::OP, N>(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {      \
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #s ", 0;\n"                                                               \
+                 "wgmma.mma_async.sync.aligned.m64n" #N SHAPE " {" WG_ACC_##N "}, %" #a ", %" #b ", p, 1, 1" TAIL ";\n}\n"       \
+                 : WG_CON_##N                                                                                                    \
+                 : "l"(da), "l"(db), "r"(scale_d));                                                                              \
+  }
+#define WG_SS_TF32(N, o0, o1, o2, ...) WG_SS(TF32, "k8.f32.tf32.tf32", "", N, o0, o1, o2)
+#define WG_SS_BF16(N, o0, o1, o2, ...) WG_SS(BF16, "k16.f32.bf16.bf16", ", 0, 0", N, o0, o1, o2)
+#define WG_SS_F16(N, o0, o1, o2, ...) WG_SS(F16, "k16.f32.f16.f16", ", 0, 0", N, o0, o1, o2)
+#define WG_SS_E4M3(N, o0, o1, o2, ...) WG_SS(E4M3, "k32.f32.e4m3.e4m3", "", N, o0, o1, o2)
+WG_WIDTHS(WG_SS_TF32)
+WG_WIDTHS(WG_SS_BF16)
+WG_WIDTHS(WG_SS_F16)
+WG_WIDTHS(WG_SS_E4M3)
 
 // D[64 x N] (+)= A[64 x 8] · B[N x 8]^T with A from registers (the .tf32 A fragment: a[0..3] = rows g, g + 8, g, g + 8 and
 // columns t, t, t + 4, t + 4 of this warp's 16 rows, g = lane / 4, t = lane % 4) and B K-major in shared memory.  The a
 // registers must not change until a wgmma.wait_group has retired the MMA that reads them.
 template <int N>
 __device__ __forceinline__ void wgmma_tf32_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d);
-template <> __device__ __forceinline__ void wgmma_tf32_rs<32>(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "{%16, %17, %18, %19}, %20, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32_rs<64>(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "{%32, %33, %34, %35}, %36, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32_rs<96>(float (&d)[48], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %53, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
-      "{%48, %49, %50, %51}, %52, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32_rs<128>(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "{%64, %65, %66, %67}, %68, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32_rs<160>(float (&d)[80], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %85, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n160k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
-      "{%80, %81, %82, %83}, %84, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32_rs<192>(float (&d)[96], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %101, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n192k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
-      "{%96, %97, %98, %99}, %100, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32_rs<224>(float (&d)[112], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %117, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n224k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111}, "
-      "{%112, %113, %114, %115}, %116, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_tf32_rs<256>(float (&d)[128], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %133, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-      "{%128, %129, %130, %131}, %132, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
-}
-
-// D[64 x N] (+)= A[64 x 16] · B[N x 16]^T in bf16 (BF16 instance): a k16 bf16 step is 32 bytes, like a k8 tf32 step, so the
-// swizzled stage layout and the +32 B descriptor advance are shared; both operands K-major (transpose flags 0)
-template <int N>
-__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
-template <> __device__ __forceinline__ void wgmma_bf16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "%16, %17, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "%32, %33, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<96>(float (&d)[48], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
-      "%48, %49, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<160>(float (&d)[80], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %82, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n160k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
-      "%80, %81, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<192>(float (&d)[96], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %98, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
-      "%96, %97, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<224>(float (&d)[112], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %114, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n224k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111}, "
-      "%112, %113, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<256>(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-      "%128, %129, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-
-// the same in fp16 (F16 instance, gemm_fp16_kernel): `k16.f32.f16.f16`, the same stage layout and descriptor advance
-template <int N>
-__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
-template <> __device__ __forceinline__ void wgmma_f16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "%16, %17, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_f16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "%32, %33, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_f16<96>(float (&d)[48], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
-      "%48, %49, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_f16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_f16<160>(float (&d)[80], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %82, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n160k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
-      "%80, %81, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_f16<192>(float (&d)[96], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %98, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n192k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
-      "%96, %97, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_f16<224>(float (&d)[112], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %114, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n224k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111}, "
-      "%112, %113, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_f16<256>(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-      "%128, %129, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-
-// D[64 x N] (+)= A[64 x 32] · B[N x 32]^T in e4m3 (FP8 instance): a k32 e4m3 step is 32 bytes, like a k8 tf32 step, so the
-// swizzled stage layout and the +32 B descriptor advance are shared; both operands K-major (the only layout e4m3 wgmma takes)
-template <int N>
-__device__ __forceinline__ void wgmma_e4m3(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
-template <> __device__ __forceinline__ void wgmma_e4m3<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "%16, %17, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_e4m3<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "%32, %33, p, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
+#define WG_RS(N, a0, a1, a2, a3, b, s)                                                                                           \
+  template <>                                                                                                                    \
+  __device__ __forceinline__ void wgmma_tf32_rs<N>(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {  \
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #s ", 0;\n"                                                               \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k8.f32.tf32.tf32 {" WG_ACC_##N "}, {%" #a0 ", %" #a1 ", %" #a2      \
+                 ", %" #a3 "}, %" #b ", p, 1, 1;\n}\n"                                                                          \
+                 : WG_CON_##N                                                                                                    \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));                                          \
+  }
+WG_WIDTHS(WG_RS)
 
 // shared -> global, 2-D tile, bulk-group completion (SASS: UTMASTG); out-of-bounds elements are not written
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void *smem_src, int c0, int c1) {
@@ -818,26 +246,23 @@ __device__ __forceinline__ float gelu_grad(float u) {
   return 0.5f * (1.f + erff(u * 0.70710678118654752f)) + u * 0.39894228040143268f * expf(-0.5f * u * u);
 }
 
-// The body of every instance.  FP8 (gemm_fp8_kernel): e4m3 operands, 128 per k-block; each k-block's four k32 MMAs accumulate
-// into a zeroed fragment that is then added to the fp32 accumulators in registers (the tensor core's e4m3 accumulation keeps
-// fewer bits than fp32, DESIGN §5.4), and the epilogue scales acc[row, col] by sa[row]·sw[col] before the bias / residual.
-// TMA_C (gemm_x3_tma_kernel): the epilogue stages each warpgroup's output in GM_CHUNK-column chunks in shared memory and
+// The body of every instance, for the operand kind OP, the A source SRC and the epilogue EPI (gemm_instance_ok).
+// E4M3 (gemm_fp8_kernel): 128 operands per k-block; each k-block's four k32 MMAs accumulate into a zeroed fragment that is
+// then added to the fp32 accumulators in registers (the tensor core's e4m3 accumulation keeps fewer bits than fp32, DESIGN
+// §5.4), and the epilogue scales acc[row, col] by sa[row]·sw[col] before the bias / residual.
+// GemmEpi::TMA (gemm_x3_tma_kernel): the epilogue stages each warpgroup's output in GM_CHUNK-column chunks in shared memory and
 // stores them with TMA, asynchronously, so the consumers go on to the next tile's MMAs while the stores drain; the residual
 // chunks arrive by TMA as well, the first two during the tile's k-loop.
-// F16 (gemm_fp16_kernel): the BF16 instance on fp16 operands, C fp32 or (p.c_bf16) fp16.
-// EPI (conv3x3_epi_kernel, the CAB convs' training instances): 1 = also store pre = conv + bias to p.aux before the GELU;
-// 2 = multiply the result by GELU'(p.aux) (the data gradient of the second conv, emitted at the first conv's pre-activation).
+// PRE / DGELU (conv3x3_epi_kernel, the CAB convs' training instances): also store pre = conv + bias to p.aux before the GELU;
+// multiply the result by GELU'(p.aux) (the data gradient of the second conv, emitted at the first conv's pre-activation).
 // PITCHED (cab_conv_pitched_kernel): the conv's output rows (C and aux) are p.ldc elements apart instead of p.N, and N may be odd:
 // an odd N's last column is loaded and stored alone.  The input's pitch is in its tensor map.
-template <int BN, bool X3, bool CONV, bool BF16, bool FP8, bool TMA_C = false, bool F16 = false, int EPI = 0, bool PITCHED = false>
+template <int BN, GemmOp OP, GemmSrc SRC = GemmSrc::ROWS, GemmEpi EPI = GemmEpi::REGS>
 __device__ __forceinline__ void gemm_body(const GemmParams &p) {
-  static_assert(EPI == 0 || (CONV && !BF16 && !FP8 && !TMA_C && !F16), "the training epilogues are the fp32 conv's");
-  static_assert(!PITCHED || (CONV && !BF16 && !FP8 && !TMA_C && !F16), "the pitched instances are the fp32 conv's");
-  static_assert(!BF16 || (!X3 && !CONV), "the bf16 instance is a plain GEMM");
-  static_assert(!FP8 || (!X3 && !CONV && !BF16), "the e4m3 instance is a plain GEMM");
-  static_assert(!F16 || (!X3 && !CONV && !BF16 && !FP8), "the fp16 instance is a plain GEMM");
-  static_assert(!TMA_C || (X3 && !CONV), "the TMA-stored epilogue is the tf32x3 linear instance's");
-  constexpr int KB = FP8 ? 4 * GM_BK : (BF16 || F16) ? 2 * GM_BK : GM_BK;   // elements per k-block: one 128-byte swizzle row in every case
+  static_assert(gemm_instance_ok(OP, SRC, EPI), "no such instance");
+  constexpr bool X3 = OP == GemmOp::TF32X3, FP8 = OP == GemmOp::E4M3;
+  constexpr bool CONV = SRC != GemmSrc::ROWS, PITCHED = SRC == GemmSrc::PITCHED, TMA_C = EPI == GemmEpi::TMA;
+  constexpr int KB = GM_BK * 4 / gemm_op_traits(OP).bytes;   // elements per k-block: one 128-byte swizzle row in every case
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const int S = p.stages;
   constexpr int a_bytes = GM_BM * GM_BK * 4, b_bytes = BN * GM_BK * 4;
@@ -929,7 +354,7 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
       const int st = (int)(it % S);
       mbar_wait(&full[st], (uint32_t)((it / S) & 1));
       unsigned char *sa = smem_raw + (size_t)st * stage_bytes;
-      if (X3) {
+      if constexpr (X3) {
         // A from registers, W_hi / W_lo from shared memory.  Per k8 step, two commit groups, small terms first: {A_lo·W_hi}
         // and {A_hi·W_lo, A_hi·W_hi}.  Each group's fragment is loaded from the stage and split just before it is issued, after
         // a wait_group 1 has retired the group before the previous one, so at most 8 fragment registers are live (the
@@ -971,7 +396,7 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < GM_BK / GM_UK; ++k)     // four k32 steps, +32 B each; the first one overwrites the fragment
-          wgmma_e4m3<BN>(part, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), k ? 1u : 0u);
+          wgmma_ss<OP, BN>(part, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), k ? 1u : 0u);
         wgmma_commit();
         acc_fence(part);
         wgmma_wait<0>();                            // the k-block's MMAs are done: the stage is free, the fragment final
@@ -986,9 +411,7 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < GM_BK / GM_UK; ++k) {   // +32 B along K inside the swizzle row = +2 in 16-byte units
-          if constexpr (F16) wgmma_f16<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
-          else if (BF16) wgmma_bf16<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
-          else wgmma_tf32<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
+          wgmma_ss<OP, BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
         }
         wgmma_commit();
         acc_fence(acc);
@@ -1064,9 +487,9 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;   // row inside the 128-row tile
-      long long coff;   // element offset of the row in C (fp32 or, (BF16 || FP8 || F16) && p.c_bf16, bf16 / fp16)
+      long long coff;   // element offset of the row in C (fp32 or, p.c_bf16, GemmC16)
       const float *rrow = nullptr;
-      float srow = 1.f;   // FP8: the activation row's scale
+      float srow = 1.f;   // E4M3: the activation row's scale
       if (CONV) {   // row r = pixel (r / 16, r % 16) of the 8 x 16 patch
         const int y = cy0 + r / CV_TW, x = cx0 + (r % CV_TW);
         if (y >= p.cH || x >= p.cW) continue;
@@ -1092,8 +515,8 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
           if (n + 1 == p.N) {
             float v = o.x;
             if (p.bias) v += __ldg(p.bias + n);
-            if constexpr (EPI == 1) p.aux[coff + n] = v;
-            if constexpr (EPI == 2) v *= gelu_grad(p.aux[coff + n]);
+            if constexpr (EPI == GemmEpi::PRE) p.aux[coff + n] = v;
+            if constexpr (EPI == GemmEpi::DGELU) v *= gelu_grad(p.aux[coff + n]);
             if (p.act == 1) v = 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
             p.C[coff + n] = v;
             continue;
@@ -1112,8 +535,8 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
             o.x += rv.x; o.y += rv.y;
           }
         }
-        if constexpr (EPI == 1) *reinterpret_cast<float2 *>(p.aux + coff + n) = o;
-        if constexpr (EPI == 2) {
+        if constexpr (EPI == GemmEpi::PRE) *reinterpret_cast<float2 *>(p.aux + coff + n) = o;
+        if constexpr (EPI == GemmEpi::DGELU) {
           const float2 u = *reinterpret_cast<const float2 *>(p.aux + coff + n);
           o.x *= gelu_grad(u.x); o.y *= gelu_grad(u.y);
         }
@@ -1121,9 +544,9 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
           o.x = 0.5f * o.x * (1.f + erff(o.x * 0.70710678118654752f));
           o.y = 0.5f * o.y * (1.f + erff(o.y * 0.70710678118654752f));
         }
-        if (F16 && p.c_bf16)
+        if (std::is_same<GemmC16<OP>, __half>::value && p.c_bf16)
           *reinterpret_cast<__half2 *>(reinterpret_cast<__half *>(p.C) + coff + n) = __floats2half2_rn(o.x, o.y);
-        else if ((BF16 || FP8) && p.c_bf16)
+        else if (std::is_same<GemmC16<OP>, __nv_bfloat16>::value && p.c_bf16)
           *reinterpret_cast<__nv_bfloat162 *>(reinterpret_cast<__nv_bfloat16 *>(p.C) + coff + n) = __floats2bfloat162_rn(o.x, o.y);
         else
           *reinterpret_cast<float2 *>(p.C + coff + n) = o;
@@ -1135,14 +558,17 @@ __device__ __forceinline__ void gemm_body(const GemmParams &p) {
 
 template <int BN, bool X3, bool CONV, bool BF16 = false>
 __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_tf32_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<BN, X3, CONV, BF16, false>(p);
+  gemm_body<BN, BF16 ? GemmOp::BF16 : X3 ? GemmOp::TF32X3 : GemmOp::TF32, CONV ? GemmSrc::CONV : GemmSrc::ROWS>(p);
 }
+
+// the conv wrappers' EPI: 0 = plain or (p.act) GELU, 1 = PRE, 2 = DGELU
+constexpr GemmEpi conv_epi(int epi) { return epi == 1 ? GemmEpi::PRE : epi == 2 ? GemmEpi::DGELU : GemmEpi::REGS; }
 
 // The conv's training instances (CabConvFn): EPI 1 = the forward that keeps the pre-activation, EPI 2 = the data gradient with the
 // GELU' factor.  A separate kernel, so that gemm_tf32_kernel keeps its code; widths up to kEpiMaxBn.
 template <int BN, bool X3, int EPI>
 __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) conv3x3_epi_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<BN, X3, true, false, false, false, false, EPI>(p);
+  gemm_body<BN, X3 ? GemmOp::TF32X3 : GemmOp::TF32, GemmSrc::CONV, conv_epi(EPI)>(p);
 }
 
 // The pitched conv (the CAB convs of Sigma-base, whose C/3 is not a multiple of 4): x, y and the weights have row pitches that are
@@ -1151,48 +577,38 @@ __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) conv3x3_epi_ker
 // >= N.  EPI as conv3x3_epi_kernel's, and 0 = plain or (p.act) GELU.  Widths up to 256 for EPI 0, kEpiMaxBn for EPI 1 and 2.
 template <int BN, bool X3, int EPI>
 __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) cab_conv_pitched_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<BN, X3, true, false, false, false, false, EPI, true>(p);
+  gemm_body<BN, X3 ? GemmOp::TF32X3 : GemmOp::TF32, GemmSrc::PITCHED, conv_epi(EPI)>(p);
 }
 
 // The tf32x3 linear instance with the TMA-stored epilogue: fp32 C (and residual) whose rows a tensor map can describe.
 // Widths up to 96 run two CTAs per SM; from 128 on, the staging buffers leave room for one (plan_gemm) and its registers.
 template <int BN>
 __global__ void __launch_bounds__(GM_THREADS, BN < 128 ? 2 : 1) gemm_x3_tma_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<BN, true, false, false, false, true>(p);
+  gemm_body<BN, GemmOp::TF32X3, GemmSrc::ROWS, GemmEpi::TMA>(p);
 }
 
 // The FP8 instance.  Its two accumulator sets (acc and the k-block fragment) need BN registers per thread; at BN <= kFp8MaxBn
 // two CTAs per SM (<= 112 registers each) hold them without spilling.
 template <int BN>
 __global__ void __launch_bounds__(GM_THREADS, 2) gemm_fp8_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<BN, false, false, false, true>(p);
+  gemm_body<BN, GemmOp::E4M3>(p);
 }
 
 // The fp16 instance: the bf16 instance's widths, ring and occupancy with `k16.f32.f16.f16` MMAs (a separate kernel, so that
 // gemm_tf32_kernel<..., BF16> stays as it was)
 template <int BN>
 __global__ void __launch_bounds__(GM_THREADS, BN <= 128 ? 2 : 1) gemm_fp16_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<BN, false, false, false, false, false, true>(p);
+  gemm_body<BN, GemmOp::F16>(p);
 }
 
 // ---- host ----
-// K-major operand map: 128-byte box rows (GM_BK fp32 or, dtype SIGMA_BF16 / SIGMA_F16, 2·GM_BK 16-bit elements) with the
-// 128-byte swizzle
-static int make_tmap_2d_sw128(CUtensorMap *map, const void *base, long long rows, long long cols, long long ld, int box_rows,
-                              int dtype = SIGMA_F32) {
-  const bool h = dtype != SIGMA_F32;
-  const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows}, str[1] = {(uint64_t)ld * (h ? 2 : 4)};
-  const uint32_t box[2] = {(uint32_t)(h ? 2 * GM_BK : GM_BK), (uint32_t)box_rows};
-  const CUtensorMapDataType dt = dtype == SIGMA_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                 : dtype == SIGMA_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  return make_tmap(map, dt, 2, base, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
-}
-// the same for e4m3 operands: 128 one-byte elements per box row
-static int make_tmap_2d_sw128_u8(CUtensorMap *map, const void *base, long long rows, long long cols, long long ld, int box_rows) {
-  const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows}, str[1] = {(uint64_t)ld};
-  const uint32_t box[2] = {(uint32_t)(4 * GM_BK), (uint32_t)box_rows};
-  return make_tmap(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, base, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+// K-major operand map of kind op: 128-byte box rows (GM_BK·4 / bytes elements) with the 128-byte swizzle
+static int make_tmap_2d_sw128(CUtensorMap *map, GemmOp op, const void *base, long long rows, long long cols, long long ld,
+                              int box_rows) {
+  const GemmOpTraits t = gemm_op_traits(op);
+  const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows}, str[1] = {(uint64_t)ld * t.bytes};
+  const uint32_t box[2] = {(uint32_t)(GM_BK * 4 / t.bytes), (uint32_t)box_rows};
+  return make_tmap(map, t.tma, 2, base, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 
 // BN is a multiple of 32 (one wgmma width per template instance); a last column tile that overhangs N is zero-filled by
@@ -1231,8 +647,8 @@ int split_tf32_launch(const float *x, float *hi, float *lo, long long n, cudaStr
   return SIGMA_OK;
 }
 
-// The launch plan of one call: tile width, ring depth, shared memory and persistent grid.  gemm_tf32_launch,
-// conv3x3_tf32_launch and the sigma_test_gemm_plan hook all take it from plan_gemm, so a test that asserts a property of
+// The launch plan of one call: tile width, ring depth, shared memory and persistent grid.  gemm_launch,
+// conv3x3_launch and the sigma_test_gemm_plan hook all take it from plan_gemm, so a test that asserts a property of
 // the plan (e.g. "every CTA walks >= 3 tiles") asserts it of the launch.
 struct GemmPlan {
   int BN, stages, ctas_per_sm;
@@ -1255,40 +671,25 @@ static int forced_bn() {
   return (int)v;
 }
 
-// The FP8 instance's widest tile.  acc and the k-block fragment take BN registers per thread, so only BN <= 64 fits two CTAs
-// per SM (96 registers at 64; 96 and 128 wide tiles take 114 / 146 and run one CTA per SM, 160 spills).  On an H100 the
-// 64-wide tiles at two CTAs per SM ran Sigma-tiny's quantized GEMMs 1.1-2.1x faster than 128-wide ones at one, whose
-// epilogue stores nothing overlaps (DESIGN §5.4), so the instance has the widths 32 and 64 only.
-constexpr int kFp8MaxBn = 64;
-
 // conv_B > 0: the implicit-GEMM 3x3 convolution of a (conv_B, conv_H, conv_W, K) input with N output channels (M unused).
-// fp8: the e4m3 instance (widths up to kFp8MaxBn, two CTAs per SM).  tma_c: the tf32x3 linear instance with the TMA-stored
-// epilogue, whose staging buffers come out of the budget before the ring.
-// max_bn: the widest instance of the kernel that will run (conv3x3_epi_kernel: kEpiMaxBn).
-static int plan_gemm(long long M, int N, int K, bool x3, int conv_B, int conv_H, int conv_W, GemmPlan *pl, bool fp8 = false,
-                     bool tma_c = false, int max_bn = 256) {
-  (void)K;   // the K loop does not enter the plan
-  const bool conv = conv_B > 0;
+// The widest tile is the kind's (E4M3: kFp8MaxBn, two CTAs per SM), and kEpiMaxBn for the conv's training epilogues.
+// GemmEpi::TMA (the tf32x3 linear instance): the staging buffers come out of the budget before the ring.
+static int plan_gemm(GemmOp op, GemmEpi epi, long long M, int N, int conv_B, int conv_H, int conv_W, GemmPlan *pl) {
+  const bool conv = conv_B > 0, fp8 = op == GemmOp::E4M3, tma_c = epi == GemmEpi::TMA;
+  const int max_bn = epi == GemmEpi::PRE || epi == GemmEpi::DGELU ? kEpiMaxBn : gemm_op_traits(op).max_bn;
   const long long m_tiles = conv ? (long long)conv_B * ((conv_W + CV_TW - 1) / CV_TW) * ((conv_H + CV_TH - 1) / CV_TH)
                                  : (M + GM_BM - 1) / GM_BM;
-  int bn = conv ? pick_bn(N, 1 << 30, max_bn) : pick_bn(N, m_tiles, fp8 ? kFp8MaxBn : 256);
-  if (!conv && !fp8) {
-    if (const char *e = getenv("SIGMA_GEMM_BN_RULE")) { if (e[0] == 'o') bn = pick_bn(N); }   // "old": ignore the row-tile count
-  }
+  int bn = pick_bn(N, conv ? 1 << 30 : m_tiles, max_bn);
   const int fbn = forced_bn();
   if (fbn < 0) return fbn;
-  if (fbn > 0 && fp8 && fbn > kFp8MaxBn) {
-    set_error("SIGMA_GEMM_BN=%d: the e4m3 GEMM's tiles are at most %d wide", fbn, kFp8MaxBn);
-    return SIGMA_EINVAL;
-  }
   if (fbn > max_bn) {
-    set_error("SIGMA_GEMM_BN=%d: this conv's tiles are at most %d wide", fbn, max_bn);
+    set_error("SIGMA_GEMM_BN=%d: %s tiles are at most %d wide", fbn, fp8 ? "the e4m3 GEMM's" : "this conv's", max_bn);
     return SIGMA_EINVAL;
   }
   if (fbn > 0) bn = fbn;
   pl->BN = bn;
   pl->tiles = m_tiles * ((N + bn - 1) / bn);
-  const int stage_bytes = gemm_stage_bytes(bn, x3, tma_c), staging = tma_c ? GM_STAGING_BYTES : 0;
+  const int stage_bytes = gemm_stage_bytes(bn, op == GemmOp::TF32X3, tma_c), staging = tma_c ? GM_STAGING_BYTES : 0;
   // up to 227 KB per block; tiles of <= 128 columns keep the ring small enough for two CTAs per SM (their register budget)
   int regs_ctas = bn <= (fp8 ? 64 : 128) ? 2 : 1;
   const auto ring = [&](int ctas) { return ((ctas == 2 ? 112 * 1024 : 226 * 1024) - 1024 - staging) / stage_bytes; };
@@ -1301,38 +702,73 @@ static int plan_gemm(long long M, int N, int K, bool x3, int conv_B, int conv_H,
   return SIGMA_OK;
 }
 
-// api.cu test hook: out = {BN, stages, grid, tiles, smem bytes, CTAs per SM}.  x3: 0 = tf32, 1 = tf32x3 with the register-stored
-// epilogue (the conv, and sigma_test_linear_tf32x3_regs), 2 = bf16 (the bf16 instance stages the
-// same bytes per k-block as tf32 — 128-byte rows — so its plan is the tf32 plan), 4 = e4m3 (the same stage bytes too, narrower
-// widths), 5 = tf32x3 with the TMA-stored epilogue (linear only), 7 = fp16 (the bf16 plan); 3 and 6 are not modes
-int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out) {
-  GemmPlan pl;
-  if (x3 < 0 || x3 > 7 || x3 == 3 || x3 == 6 || (x3 >= 2 && conv_B > 0)) {
-    set_error("gemm plan: mode %d (0 tf32, 1 tf32x3, 2 bf16, 4 e4m3, 5 tf32x3 TMA-stored, 7 fp16; only 0 and 1 have a conv)", x3);
+// api.cu test hook: out = {BN, stages, grid, tiles, smem bytes, CTAs per SM}.  mode: 0 = tf32, 1 = tf32x3 with the
+// register-stored epilogue (the conv, and sigma_test_linear_tf32x3_regs), 2 = bf16 (the bf16 instance stages the same bytes per
+// k-block as tf32 — 128-byte rows — so its plan is the tf32 plan), 4 = e4m3 (the same stage bytes too, narrower widths),
+// 5 = tf32x3 with the TMA-stored epilogue (linear only), 7 = fp16 (the bf16 plan); 3 and 6 are not modes.  The K loop does not
+// enter the plan.
+int gemm_plan_hook(long long M, int N, int K, int mode, int conv_B, int conv_H, int conv_W, long long *out) {
+  (void)K;
+  static const GemmOp ops[8] = {GemmOp::TF32, GemmOp::TF32X3, GemmOp::BF16, GemmOp::TF32,
+                                GemmOp::E4M3, GemmOp::TF32X3, GemmOp::TF32, GemmOp::F16};
+  if (mode < 0 || mode > 7 || mode == 3 || mode == 6 || (mode >= 2 && conv_B > 0)) {
+    set_error("gemm plan: mode %d (0 tf32, 1 tf32x3, 2 bf16, 4 e4m3, 5 tf32x3 TMA-stored, 7 fp16; only 0 and 1 have a conv)", mode);
     return SIGMA_EINVAL;
   }
-  const int rc = plan_gemm(M, N, K, x3 == 1 || x3 == 5, conv_B, conv_H, conv_W, &pl, x3 == 4, x3 == 5);
+  GemmPlan pl;
+  const int rc = plan_gemm(ops[mode], mode == 5 ? GemmEpi::TMA : GemmEpi::REGS, M, N, conv_B, conv_H, conv_W, &pl);
   if (rc) return rc;
   out[0] = pl.BN; out[1] = pl.stages; out[2] = pl.grid; out[3] = pl.tiles; out[4] = (long long)pl.smem; out[5] = pl.ctas_per_sm;
   return SIGMA_OK;
 }
 
-// The launch of the instance for pl.BN (F16: gemm_fp16_kernel).
-template <bool X3, bool CONV, bool BF16 = false, bool TMA_C = false, bool F16 = false>
-static int launch_gemm(GemmParams &p, const GemmPlan &pl, cudaStream_t stream) {
-  p.stages = pl.stages;
-  const void *kern = nullptr;
-  switch (p.BN) {
-#define SIGMA_GEMM_BN(bn)                                                                                                        \
-  case bn:                                                                                                                       \
-    kern = F16 ? (const void *)gemm_fp16_kernel<bn>                                                                              \
-               : TMA_C ? (const void *)gemm_x3_tma_kernel<bn> : (const void *)gemm_tf32_kernel<bn, X3, CONV, BF16>;             \
-    break;
-    SIGMA_GEMM_BN(32) SIGMA_GEMM_BN(64) SIGMA_GEMM_BN(96) SIGMA_GEMM_BN(128)
-    SIGMA_GEMM_BN(160) SIGMA_GEMM_BN(192) SIGMA_GEMM_BN(224) SIGMA_GEMM_BN(256)
-#undef SIGMA_GEMM_BN
-    default: set_error("gemm: unsupported tile width %d", p.BN); return SIGMA_EINVAL;
+// The instance of width BN for (op, src, epi), one of gemm_instance_ok's; nullptr past the widest tile of E4M3 or of the conv's
+// training epilogues
+template <int BN>
+static const void *gemm_kernel(GemmOp op, GemmSrc src, GemmEpi epi) {
+  const bool x3 = op == GemmOp::TF32X3;
+  if (src == GemmSrc::ROWS) {
+    switch (op) {
+      case GemmOp::TF32: return (const void *)gemm_tf32_kernel<BN, false, false>;
+      case GemmOp::TF32X3:
+        return epi == GemmEpi::TMA ? (const void *)gemm_x3_tma_kernel<BN> : (const void *)gemm_tf32_kernel<BN, true, false>;
+      case GemmOp::BF16: return (const void *)gemm_tf32_kernel<BN, false, false, true>;
+      case GemmOp::F16: return (const void *)gemm_fp16_kernel<BN>;
+      case GemmOp::E4M3:
+        if constexpr (BN <= kFp8MaxBn) return (const void *)gemm_fp8_kernel<BN>;
+        break;
+    }
+    return nullptr;
   }
+  if (epi == GemmEpi::REGS) {
+    if (src == GemmSrc::CONV) return x3 ? (const void *)gemm_tf32_kernel<BN, true, true> : (const void *)gemm_tf32_kernel<BN, false, true>;
+    return x3 ? (const void *)cab_conv_pitched_kernel<BN, true, 0> : (const void *)cab_conv_pitched_kernel<BN, false, 0>;
+  }
+  if constexpr (BN <= kEpiMaxBn) {
+    const bool pre = epi == GemmEpi::PRE;
+    if (src == GemmSrc::CONV)
+      return x3 ? (pre ? (const void *)conv3x3_epi_kernel<BN, true, 1> : (const void *)conv3x3_epi_kernel<BN, true, 2>)
+                : (pre ? (const void *)conv3x3_epi_kernel<BN, false, 1> : (const void *)conv3x3_epi_kernel<BN, false, 2>);
+    return x3 ? (pre ? (const void *)cab_conv_pitched_kernel<BN, true, 1> : (const void *)cab_conv_pitched_kernel<BN, true, 2>)
+              : (pre ? (const void *)cab_conv_pitched_kernel<BN, false, 1> : (const void *)cab_conv_pitched_kernel<BN, false, 2>);
+  }
+  return nullptr;
+}
+
+// Launches the instance for (op, src, epi) at the plan's width on its persistent grid
+static int gemm_run(GemmOp op, GemmSrc src, GemmEpi epi, GemmParams &p, const GemmPlan &pl, cudaStream_t stream) {
+  const void *kern = nullptr;
+  switch (pl.BN) {
+#define GEMM_KERNEL_AT(N, ...) case N: kern = gemm_kernel<N>(op, src, epi); break;
+    WG_WIDTHS(GEMM_KERNEL_AT)
+#undef GEMM_KERNEL_AT
+  }
+  if (kern == nullptr) {
+    set_error("gemm: no instance of width %d for this operand kind and epilogue", pl.BN);
+    return SIGMA_EINVAL;
+  }
+  p.BN = pl.BN;
+  p.stages = pl.stages;
   SIGMA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
   void *args[] = {&p};
   SIGMA_CHECK_CUDA(cudaLaunchKernel(kern, dim3(pl.grid), dim3(GM_THREADS), args, pl.smem, stream));
@@ -1340,100 +776,47 @@ static int launch_gemm(GemmParams &p, const GemmPlan &pl, cudaStream_t stream) {
   return SIGMA_OK;
 }
 
-// W_lo == nullptr: plain TF32 (one MMA per k-step); else tf32x3 with W = W_hi, whose output tiles go out through TMA
-// (gemm_x3_tma_kernel) unless reg_epilogue
-int gemm_tf32_launch(const float *A, long long lda, const float *W, const float *W_lo, const float *bias, const float *residual,
-                     long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream,
-                     bool reg_epilogue) {
+int gemm_launch(GemmOp op, const void *A, long long lda, const void *W, const void *W_lo, const float *sa, const float *sw,
+                const float *bias, const float *residual, long long ldr, const float *rscale, void *C, long long ldc, int c_16,
+                long long M, int N, int K, cudaStream_t stream, bool reg_epilogue) {
   if (M == 0) return SIGMA_OK;
-  const bool x3 = W_lo != nullptr;
-  const bool tma_c = x3 && !reg_epilogue;
+  const bool x3 = op == GemmOp::TF32X3;
+  const GemmEpi epi = x3 && !reg_epilogue ? GemmEpi::TMA : GemmEpi::REGS;
   GemmPlan pl;
   int rc;
-  if ((rc = plan_gemm(M, N, K, x3, 0, 0, 0, &pl, false, tma_c))) return rc;
+  if ((rc = plan_gemm(op, epi, M, N, 0, 0, 0, &pl))) return rc;
   GemmParams p;
   memset(&p, 0, sizeof(p));
-  p.bias = bias; p.residual = residual; p.rscale = rscale; p.C = C; p.ldr = ldr; p.ldc = ldc;
+  p.bias = bias; p.residual = residual; p.rscale = rscale; p.C = (float *)C; p.ldr = ldr; p.ldc = ldc; p.c_bf16 = c_16;
+  p.sa = sa; p.sw = sw;
   p.M = (int)M; p.N = N; p.K = K;
-  p.BN = pl.BN;
-  if ((rc = make_tmap_2d_sw128(&p.m_a, A, M, K, lda, GM_BM))) return rc;
-  if ((rc = make_tmap_2d_sw128(&p.m_w, W, N, K, K, p.BN))) return rc;
-  if (x3 && (rc = make_tmap_2d_sw128(&p.m_wlo, W_lo, N, K, K, p.BN))) return rc;
-  if (tma_c) {
+  if ((rc = make_tmap_2d_sw128(&p.m_a, op, A, M, K, lda, GM_BM))) return rc;
+  if ((rc = make_tmap_2d_sw128(&p.m_w, op, W, N, K, K, pl.BN))) return rc;
+  if (x3 && (rc = make_tmap_2d_sw128(&p.m_wlo, op, W_lo, N, K, K, pl.BN))) return rc;
+  if (epi == GemmEpi::TMA) {
     const uint64_t dims[2] = {(uint64_t)N, (uint64_t)M}, str_c[1] = {(uint64_t)ldc * 4}, str_r[1] = {(uint64_t)ldr * 4};
     const uint32_t box[2] = {GM_CHUNK, 64};
     if ((rc = make_tmap(&p.m_c, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, C, dims, str_c, box, CU_TENSOR_MAP_SWIZZLE_128B,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
     if (residual && (rc = make_tmap(&p.m_r, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, residual, dims, str_r, box,
                                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
-    return launch_gemm<true, false, false, true>(p, pl, stream);
   }
-  return x3 ? launch_gemm<true, false>(p, pl, stream) : launch_gemm<false, false>(p, pl, stream);
+  return gemm_run(op, GemmSrc::ROWS, epi, p, pl, stream);
 }
 
-// bf16 (dtype SIGMA_BF16) or fp16 (SIGMA_F16) operands (A (M, K) row stride lda, W (N, K)), fp32 accumulation, C fp32 or (c_16)
-// the operands' type; bias / residual / rscale fp32.  Both instances stage the same bytes, so both run the tf32 plan.
-int gemm_16bit_launch(int dtype, const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
-                      const float *rscale, void *C, long long ldc, int c_16, long long M, int N, int K, cudaStream_t stream) {
-  if (M == 0) return SIGMA_OK;
+// 3x3 convolution, pad 1, stride 1, channels-last: y (B,H,W,Cout) = conv(x (B,H,W,Cin), W9 (9, Cout, Cin)) + bias, optional GELU,
+// with x, W9 and y (and aux) rows x_ld, w_ld and y_ld elements apart: the tensor maps' widths are Cin, so channels past Cin arrive
+// as zeros; the epilogue never stores a column >= Cout.  W9_lo == nullptr: plain TF32; else tf32x3 with W9 = W9_hi.  epi 1
+// (act 1): pre = conv + bias also stored to aux; epi 2 (act 0): the result times GELU'(aux).
+static int conv3x3_launch(GemmSrc src, const float *x, long long x_ld, const float *W9, const float *W9_lo, long long w_ld,
+                          const float *bias, int act, float *y, long long y_ld, int B, int H, int W, int Cin, int Cout,
+                          cudaStream_t stream, int epi, float *aux) {
+  if (B == 0) return SIGMA_OK;
+  const GemmOp op = W9_lo ? GemmOp::TF32X3 : GemmOp::TF32;
   GemmPlan pl;
   int rc;
-  if ((rc = plan_gemm(M, N, K, false, 0, 0, 0, &pl))) return rc;
+  if ((rc = plan_gemm(op, conv_epi(epi), 0, Cout, B, H, W, &pl))) return rc;
   GemmParams p;
-  memset(&p, 0, sizeof(p));
-  p.bias = bias; p.residual = residual; p.rscale = rscale; p.C = (float *)C; p.ldr = ldr; p.ldc = ldc; p.c_bf16 = c_16;
-  p.M = (int)M; p.N = N; p.K = K;
-  p.BN = pl.BN;
-  if ((rc = make_tmap_2d_sw128(&p.m_a, A, M, K, lda, GM_BM, dtype))) return rc;
-  if ((rc = make_tmap_2d_sw128(&p.m_w, W, N, K, K, p.BN, dtype))) return rc;
-  if (dtype == SIGMA_F16) return launch_gemm<false, false, false, false, true>(p, pl, stream);
-  return launch_gemm<false, false, true>(p, pl, stream);
-}
-
-// e4m3 operands (A (M, K) row stride lda bytes, W (N, K) contiguous) with fp32 scales sa (M) and sw (N): C = (A·W^T)·sa·sw
-// (+ bias) (+ residual · rscale), C fp32 or (c_bf16) bf16
-int gemm_fp8_launch(const void *A, long long lda, const float *sa, const void *W, const float *sw, const float *bias,
-                    const float *residual, long long ldr, const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N,
-                    int K, cudaStream_t stream) {
-  if (M == 0) return SIGMA_OK;
-  GemmPlan pl;
-  int rc;
-  if ((rc = plan_gemm(M, N, K, false, 0, 0, 0, &pl, true))) return rc;
-  GemmParams p;
-  memset(&p, 0, sizeof(p));
-  p.bias = bias; p.residual = residual; p.rscale = rscale; p.C = (float *)C; p.ldr = ldr; p.ldc = ldc; p.c_bf16 = c_bf16;
-  p.sa = sa; p.sw = sw;
-  p.M = (int)M; p.N = N; p.K = K;
-  p.BN = pl.BN;
-  if ((rc = make_tmap_2d_sw128_u8(&p.m_a, A, M, K, lda, GM_BM))) return rc;
-  if ((rc = make_tmap_2d_sw128_u8(&p.m_w, W, N, K, K, p.BN))) return rc;
-  p.stages = pl.stages;
-  const void *kern = nullptr;
-  switch (p.BN) {
-#define SIGMA_GEMM_BN(bn) case bn: kern = (const void *)gemm_fp8_kernel<bn>; break;
-    SIGMA_GEMM_BN(32) SIGMA_GEMM_BN(64)
-#undef SIGMA_GEMM_BN
-    default: set_error("gemm e4m3: unsupported tile width %d", p.BN); return SIGMA_EINVAL;
-  }
-  SIGMA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
-  void *args[] = {&p};
-  SIGMA_CHECK_CUDA(cudaLaunchKernel(kern, dim3(pl.grid), dim3(GM_THREADS), args, pl.smem, stream));
-  count_launch();
-  return SIGMA_OK;
-}
-
-// The widest tile of conv3x3_epi_kernel and of cab_conv_pitched_kernel's EPI 1 / 2: the CAB's C/3 (32 / 64 / 128 in Sigma-tiny and
-// -small) fits one tile; wider outputs (Sigma-base's 170) take several.  The training epilogues keep two CTAs per SM, whose register
-// budget ends at 128-column tiles (plan_gemm).
-constexpr int kEpiMaxBn = 128;
-
-// The plan and parameters of a 3x3 conv (pad 1, stride 1, channels-last) whose x, W9 and y (and aux) rows are x_ld, w_ld and y_ld
-// elements apart: the tensor maps' widths are Cin, so channels past Cin arrive as zeros; the epilogue never stores a column >= Cout.
-static int conv3x3_setup(GemmParams &p, GemmPlan &pl, const float *x, long long x_ld, const float *W9, const float *W9_lo, long long w_ld,
-                         const float *bias, int act, float *y, long long y_ld, int B, int H, int W, int Cin, int Cout, float *aux,
-                         int max_bn) {
-  int rc;
-  if ((rc = plan_gemm(0, Cout, Cin, W9_lo != nullptr, B, H, W, &pl, false, false, max_bn))) return rc;
   memset(&p, 0, sizeof(p));
   p.bias = bias; p.C = y; p.aux = aux; p.ldc = y_ld;
   p.N = Cout; p.K = Cin;
@@ -1442,8 +825,6 @@ static int conv3x3_setup(GemmParams &p, GemmPlan &pl, const float *x, long long 
   p.tiles_hw = p.tiles_w * ((H + CV_TH - 1) / CV_TH);
   p.M = B * p.tiles_hw;
   p.kbc = (Cin + GM_BK - 1) / GM_BK;
-  p.BN = pl.BN;
-  p.stages = pl.stages;
   {
     uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
     uint64_t str[3] = {(uint64_t)x_ld * 4, (uint64_t)W * x_ld * 4, (uint64_t)H * W * x_ld * 4};
@@ -1451,82 +832,22 @@ static int conv3x3_setup(GemmParams &p, GemmPlan &pl, const float *x, long long 
     if ((rc = make_tmap(&p.m_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B))) return rc;
   }
-  if ((rc = make_tmap_2d_sw128(&p.m_w, W9, 9LL * Cout, Cin, w_ld, p.BN))) return rc;
-  if (W9_lo && (rc = make_tmap_2d_sw128(&p.m_wlo, W9_lo, 9LL * Cout, Cin, w_ld, p.BN))) return rc;
-  return SIGMA_OK;
+  if ((rc = make_tmap_2d_sw128(&p.m_w, op, W9, 9LL * Cout, Cin, w_ld, pl.BN))) return rc;
+  if (W9_lo && (rc = make_tmap_2d_sw128(&p.m_wlo, op, W9_lo, 9LL * Cout, Cin, w_ld, pl.BN))) return rc;
+  return gemm_run(op, src, conv_epi(epi), p, pl, stream);
 }
 
-static int launch_conv(const void *kern, const GemmParams &p, const GemmPlan &pl, cudaStream_t stream) {
-  SIGMA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
-  void *args[] = {(void *)&p};
-  SIGMA_CHECK_CUDA(cudaLaunchKernel(kern, dim3(pl.grid), dim3(GM_THREADS), args, pl.smem, stream));
-  count_launch();
-  return SIGMA_OK;
-}
-
-// 3x3 convolution, pad 1, stride 1, channels-last: y (B,H,W,Cout) = conv(x (B,H,W,Cin), W9 (9, Cout, Cin)) + bias, optional GELU.
-// W9_lo == nullptr: plain TF32; else tf32x3 with W9 = W9_hi.  epi 1 (act 1): pre = conv + bias also stored to aux; epi 2 (act 0):
-// the result times GELU'(aux); both run conv3x3_epi_kernel.
+// the unpitched conv: rows Cin (x, W9) and Cout (y, aux) elements apart
 int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, const float *bias, int act, float *y, int B, int H, int W,
                         int Cin, int Cout, cudaStream_t stream, int epi, float *aux) {
-  if (B == 0) return SIGMA_OK;
-  const bool x3 = W9_lo != nullptr;
-  GemmPlan pl;
-  GemmParams p;
-  int rc;
-  if ((rc = conv3x3_setup(p, pl, x, Cin, W9, W9_lo, Cin, bias, act, y, Cout, B, H, W, Cin, Cout, aux, epi ? kEpiMaxBn : 256)))
-    return rc;
-  if (epi == 0) return x3 ? launch_gemm<true, true>(p, pl, stream) : launch_gemm<false, true>(p, pl, stream);
-  const void *kern = nullptr;
-  switch (p.BN) {
-#define SIGMA_EPI_BN(bn)                                                                                                         \
-  case bn:                                                                                                                       \
-    kern = epi == 1 ? (x3 ? (const void *)conv3x3_epi_kernel<bn, true, 1> : (const void *)conv3x3_epi_kernel<bn, false, 1>)      \
-                    : (x3 ? (const void *)conv3x3_epi_kernel<bn, true, 2> : (const void *)conv3x3_epi_kernel<bn, false, 2>);     \
-    break;
-    SIGMA_EPI_BN(32) SIGMA_EPI_BN(64) SIGMA_EPI_BN(96) SIGMA_EPI_BN(128)
-#undef SIGMA_EPI_BN
-    default: set_error("conv3x3: the training epilogues have tiles of at most %d columns, not %d", kEpiMaxBn, p.BN); return SIGMA_EINVAL;
-  }
-  return launch_conv(kern, p, pl, stream);
+  return conv3x3_launch(GemmSrc::CONV, x, Cin, W9, W9_lo, Cin, bias, act, y, Cout, B, H, W, Cin, Cout, stream, epi, aux);
 }
 
 // The same conv on pitched rows (cab_conv_pitched_kernel): x (B,H,W,x_ld) holds Cin channels, W9 (9·Cout, w_ld) Cin, y and aux
-// (B,H,W,y_ld) Cout; the pitches are multiples of 4 and at least the counts, which need not be.  The plan is conv3x3_tf32_launch's.
+// (B,H,W,y_ld) Cout; the pitches are multiples of 4 and at least the counts, which need not be.  The plan is the unpitched conv's.
 int conv3x3_pitched_launch(const float *x, long long x_ld, const float *W9, const float *W9_lo, long long w_ld, const float *bias, int act,
                            float *y, long long y_ld, int B, int H, int W, int Cin, int Cout, cudaStream_t stream, int epi, float *aux) {
-  if (B == 0) return SIGMA_OK;
-  const bool x3 = W9_lo != nullptr;
-  GemmPlan pl;
-  GemmParams p;
-  int rc;
-  if ((rc = conv3x3_setup(p, pl, x, x_ld, W9, W9_lo, w_ld, bias, act, y, y_ld, B, H, W, Cin, Cout, aux, epi ? kEpiMaxBn : 256)))
-    return rc;
-  const void *kern = nullptr;
-#define SIGMA_PITCHED_BN(bn, E)                                                                                                  \
-  case bn:                                                                                                                       \
-    kern = x3 ? (const void *)cab_conv_pitched_kernel<bn, true, E> : (const void *)cab_conv_pitched_kernel<bn, false, E>;        \
-    break;
-#define SIGMA_PITCHED_EPI(E) \
-    SIGMA_PITCHED_BN(32, E) SIGMA_PITCHED_BN(64, E) SIGMA_PITCHED_BN(96, E) SIGMA_PITCHED_BN(128, E)
-  if (epi == 0) {
-    switch (p.BN) {
-      SIGMA_PITCHED_EPI(0)
-      SIGMA_PITCHED_BN(160, 0) SIGMA_PITCHED_BN(192, 0) SIGMA_PITCHED_BN(224, 0) SIGMA_PITCHED_BN(256, 0)
-      default: break;
-    }
-  } else if (epi == 1) {
-    switch (p.BN) { SIGMA_PITCHED_EPI(1) default: break; }
-  } else {
-    switch (p.BN) { SIGMA_PITCHED_EPI(2) default: break; }
-  }
-#undef SIGMA_PITCHED_EPI
-#undef SIGMA_PITCHED_BN
-  if (kern == nullptr) {
-    set_error("conv3x3 (pitched): no instance of width %d for epilogue %d", p.BN, epi);
-    return SIGMA_EINVAL;
-  }
-  return launch_conv(kern, p, pl, stream);
+  return conv3x3_launch(GemmSrc::PITCHED, x, x_ld, W9, W9_lo, w_ld, bias, act, y, y_ld, B, H, W, Cin, Cout, stream, epi, aux);
 }
 
 }  // namespace sigma

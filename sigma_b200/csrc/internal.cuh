@@ -179,18 +179,17 @@ int dwconv3x3_silu_bwd_launch(int dtype, const void *x, long long x_row_stride, 
                               float *db, int batch, int H, int W, int D, void *ws, cudaStream_t stream);
 
 // ---- gemm_tf32.cu ----
-// tf32x3 (W_lo != nullptr) stores its output tiles with TMA; reg_epilogue = true stores them from registers instead (the
-// TMA-stored epilogue's reference in the tests, sigma_test_linear_tf32x3_regs).  C and the residual: 16-byte-aligned base and
-// row stride (sigma_linear_tf32{,x3} check it).
-int gemm_tf32_launch(const float *A, long long lda, const float *W, const float *W_lo, const float *bias, const float *residual,
-                     long long ldr, const float *rscale, float *C, long long ldc, long long M, int N, int K, cudaStream_t stream,
-                     bool reg_epilogue = false);
-// dtype: SIGMA_BF16 or SIGMA_F16 operands; c_16 = 1: C stored in that type (else fp32)
-int gemm_16bit_launch(int dtype, const void *A, long long lda, const void *W, const float *bias, const float *residual, long long ldr,
-                      const float *rscale, void *C, long long ldc, int c_16, long long M, int N, int K, cudaStream_t stream);
-int gemm_fp8_launch(const void *A, long long lda, const float *sa, const void *W, const float *sw, const float *bias,
-                    const float *residual, long long ldr, const float *rscale, void *C, long long ldc, int c_bf16, long long M, int N,
-                    int K, cudaStream_t stream);
+// The operand kind of the wgmma GEMM: fp32 operands read as TF32 or split into tf32x3 (A·W = A_hi·W_hi + A_lo·W_hi + A_hi·W_lo),
+// bf16, fp16 or e4m3 operands; fp32 accumulation in every case
+enum class GemmOp { TF32, TF32X3, BF16, F16, E4M3 };
+// C = A (M, K) · W (N, K)^T (+ bias) (+ residual · rscale), lda / ldc / ldr in elements.  TF32X3: W = W_hi and W_lo, output tiles
+// stored with TMA unless reg_epilogue (the TMA-stored epilogue's reference in the tests, sigma_test_linear_tf32x3_regs); C and
+// the residual then need 16-byte-aligned bases and row strides (sigma_linear_tf32x3 checks it).  E4M3: A and W scaled by the fp32
+// sa (M) and sw (N) before the bias.  c_16 = 1: C stored as fp16 (F16) or bf16 (BF16, E4M3), else fp32; bias / residual / rscale
+// are fp32 for every kind.
+int gemm_launch(GemmOp op, const void *A, long long lda, const void *W, const void *W_lo, const float *sa, const float *sw,
+                const float *bias, const float *residual, long long ldr, const float *rscale, void *C, long long ldc, int c_16,
+                long long M, int N, int K, cudaStream_t stream, bool reg_epilogue = false);
 // epi 1 (with act 1): also store pre = conv + bias to aux; epi 2 (act 0): multiply the result by GELU'(aux) (aux in y's layout)
 int conv3x3_tf32_launch(const float *x, const float *W9, const float *W9_lo, const float *bias, int act, float *y, int B, int H, int W,
                         int Cin, int Cout, cudaStream_t stream, int epi = 0, float *aux = nullptr);
@@ -199,7 +198,7 @@ int conv3x3_pitched_launch(const float *x, long long x_ld, const float *W9, cons
                            float *aux = nullptr);
 int split_tf32_launch(const float *x, float *hi, float *lo, long long n, cudaStream_t stream);
 int gemm_pick_bn_hook(int N, long long m_tiles);
-int gemm_plan_hook(long long M, int N, int K, int x3, int conv_B, int conv_H, int conv_W, long long *out);
+int gemm_plan_hook(long long M, int N, int K, int mode, int conv_B, int conv_H, int conv_W, long long *out);
 
 // ---- conv3x3_wgrad.cu ----
 // Launch plan of the weight gradient: {output channels per tile, output tiles, partial rows, CTAs}
